@@ -210,7 +210,8 @@ int b200mdm_test_qkv_attention(const void* h16_dev, int32_t ld, const void* wqkv
                                void* out16_dev, const int32_t* kvlen_dev, int32_t n_samples, int32_t S, void* stream);
 /* h[M,512] <- LayerNorm(h + A16[M,K] @ W16[512,K]^T + bias; gamma, beta, 1e-5) in place (the fused out-projection /
  * FFN-down kernel of the transformer layer).  h is the engine's residual-stream format: fp16 [M, 1024] = [hi | lo],
- * value = hi + lo.  K % 8 == 0. */
+ * value = hi + lo, read and written only with TMA (rows past M are never touched).  K % 8 == 0; a16, w16 and hres16
+ * 16-byte aligned. */
 int b200mdm_test_gemm_resid_ln(const void* a16_dev, const void* w16_dev, const float* bias_dev, const float* gamma_dev,
                                const float* beta_dev, void* hres16_dev, int32_t M, int32_t K, void* stream);
 

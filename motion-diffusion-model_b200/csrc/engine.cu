@@ -96,6 +96,11 @@ static int make_map_3d(CUtensorMap* m, const void* ptr, uint64_t n, uint64_t row
   return B200MDM_OK;
 }
 
+// Residual stream [M, 2 x 512] fp16 as the residual + LayerNorm GEMM moves it: box 64 columns x GLN_RES_BOX_ROWS rows.
+static int make_hres_map(CUtensorMap* m, const void* hres, uint64_t rows) {
+  return make_map(m, hres, rows, 2 * GLN_D, 2 * GLN_D, GLN_RES_BOX_ROWS);
+}
+
 // Residual stream fp16 [rows, 2d] = [hi | lo]: box {32 cols, 32 rows} with 64-byte rows and the 64-byte swizzle; an
 // epilogue chunk of 32 columns moves one such box from the hi half and one from the lo half.
 static int make_map_res(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t d) {
@@ -152,6 +157,7 @@ struct Workspace {
   CUtensorMap m_qkv_st, m_ffn_st;                      // epilogue slabs (box 32 rows x 128 bytes)
   CUtensorMap m_qkv_kv;                                // attention core: per-sample K / V tiles of qkv16 (box all keys)
   CUtensorMap m_res_c, m_res_u;                        // per-CFG-half views of the residual stream (embedding epilogue)
+  CUtensorMap m_hres;                                  // the whole residual stream [M, 2d], box 64 x 64 (residual + LayerNorm)
   float* pe_bias = nullptr;
   bool cond_set = false;
   // trans_dec (DiP): prefix frames + text-token memory
@@ -323,8 +329,9 @@ static int launch_gemm_bias(const CUtensorMap& a, const CUtensorMap& b, const CU
 }
 
 // h <- LayerNorm(h + A W^T + bias), 2-CTA cluster splitting the 512 columns, LayerNorm statistics exchanged through
-// distributed shared memory (w256: W map with box 256 rows; hres: the residual stream [M, 2 x 512] fp16)
-static int launch_gemm_resid_ln(const CUtensorMap& a, const CUtensorMap& w256, __half* hres, int M, int K,
+// distributed shared memory (w256: W map with box 256 rows; hres: map of the residual stream [M, 2 x 512] fp16 with
+// box GLN_RES_BOX_ROWS rows x 64 columns, make_hres_map)
+static int launch_gemm_resid_ln(const CUtensorMap& a, const CUtensorMap& w256, const CUtensorMap& hres, int M, int K,
                                 const float* bias, const float* gamma, const float* beta, cudaStream_t s, int num_sms) {
   const int tiles = (M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M;
   const int max_clusters = num_sms / 2;
@@ -700,6 +707,7 @@ static int build_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStre
   TRY(make_map_t(&e->m_ffn_st, e->ffn16, 2, M, kw * e->ff, kw * e->ff, 32));
   TRY(make_map_res(&e->m_res_c, e->hres, MB, d));
   TRY(make_map_res(&e->m_res_u, e->hres + (halves == 2 ? MB * d * 2 : 0), MB, d));
+  TRY(make_hres_map(&e->m_hres, e->hres, M));
   TRY(dalloc(&e->pe_bias, static_cast<size_t>(S) * d));
   pe_bias_kernel<<<S, 128, 0, s>>>(e->pe_bias, e->pe, e->b_in, S, d);   // on the caller's stream: ordered before any forward
   CUDA_TRY(cudaGetLastError());
@@ -974,7 +982,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
       }
       TRY(launch_attention_tc(e->m_qkv_kv, e->qkv16, e->att16, e->kvlen, e->Bp, S, d, e->H, s, wide));
     }
-    if (!B200_SKIP(2)) TRY(launch_gemm_resid_ln(e->m_att, w.m_wo_256, e->hres, e->M, kw * d, w.bo, w.g1, w.be1, s, e->num_sms));
+    if (!B200_SKIP(2)) TRY(launch_gemm_resid_ln(e->m_att, w.m_wo_256, e->m_hres, e->M, kw * d, w.bo, w.g1, w.be1, s, e->num_sms));
     if (e->dec) {
       // cross-attention block of nn.TransformerDecoderLayer: q from the sequence, k/v from the text memory
       TRY((launch_gemm_bias<false>(e->m_h16, w.m_wq_c, e->m_qc_st, e->M, d, d, w.bq_c, s, e->num_sms)));
@@ -990,7 +998,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
         else
           CUDA_TRY(launch_k(cross_attention_kernel<8>, cg, cb, 0, s, e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
       }
-      TRY(launch_gemm_resid_ln(e->m_att, w.m_wo_c_256, e->hres, e->M, d, w.bo_c, w.g2, w.be2, s, e->num_sms));   // cross-attention output: hi half
+      TRY(launch_gemm_resid_ln(e->m_att, w.m_wo_c_256, e->m_hres, e->M, d, w.bo_c, w.g2, w.be2, s, e->num_sms));   // cross-attention output: hi half
       nk += 3;
     }
     if (wide) {
@@ -999,7 +1007,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     } else if (!B200_SKIP(4)) {
       TRY((launch_gemm_bias<true>(e->m_h16, w.m_w1, e->m_ffn_st, e->M, ff, d, w.b1, s, e->num_sms)));
     }
-    if (!B200_SKIP(8)) TRY(launch_gemm_resid_ln(e->m_ffn, w.m_w2_256, e->hres, e->M, kw * ff, w.b2, e->dec ? w.g3 : w.g2,
+    if (!B200_SKIP(8)) TRY(launch_gemm_resid_ln(e->m_ffn, w.m_w2_256, e->m_hres, e->M, kw * ff, w.b2, e->dec ? w.g3 : w.g2,
                              e->dec ? w.be3 : w.be2, s, e->num_sms));
     nk += 5;
   }
@@ -1315,10 +1323,11 @@ extern "C" int b200mdm_test_gemm_resid_ln(const void* a16_dev, const void* w16_d
   int dev = 0, sms = 132;
   CUDA_TRY(cudaGetDevice(&dev));
   CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CUtensorMap ma, mb;
+  CUtensorMap ma, mb, mh;
   TRY(make_map(&ma, a16_dev, M, K, K, GEMM_BLOCK_M));
   TRY(make_map(&mb, w16_dev, GLN_D, K, K, 256));
-  return launch_gemm_resid_ln(ma, mb, static_cast<__half*>(hres16_dev), M, K, bias_dev, gamma_dev, beta_dev, static_cast<cudaStream_t>(stream), sms);
+  TRY(make_hres_map(&mh, hres16_dev, M));
+  return launch_gemm_resid_ln(ma, mb, mh, M, K, bias_dev, gamma_dev, beta_dev, static_cast<cudaStream_t>(stream), sms);
 }
 
 // ------------------------------------------------------------------------------------------------ post-processing

@@ -5,14 +5,20 @@
 //
 // Both CTAs of a cluster work on the SAME 128 rows; CTA r owns columns [256 r, 256 r + 256) (its own 256 rows of W).
 // Warpgroup 0 is the TMA producer; consumer warpgroup g (1, 2) issues wgmma m64n256k16 for rows [64 (g-1), +64) and
-// keeps its 64 x 256 fp32 accumulator in registers (128 per thread) for the whole epilogue:
-//   pass 1    v = acc + bias + residual (read in the accumulator's fragment layout), kept in the accumulator registers;
+// keeps its 64 x 256 fp32 accumulator in registers (128 per thread) for the whole epilogue.
+//
+// The residual moves only as bulk TMA traffic.  After a tile's last k-block the producer loads the CTA's 256 residual
+// columns as four 64-column groups, each a 128-row hi box + the matching lo box (2 x 16 KB, 128-byte swizzle), into the
+// next four stages of the operand ring, so the loads overlap the tail of the mainloop.  Epilogue:
+//   pass 1    v = acc + bias + residual (read from the swizzled slab in the accumulator's fragment layout: the 8 rows of a
+//             quad group land on distinct 16-byte chunks, no bank conflicts), kept in the accumulator registers;
 //             per-row partial sum / sum of squares over the CTA's 256 columns (quad shuffles)
 //   exchange  one lane per row pushes the CTA's partial into the PEER CTA's shared memory with st.async (data + mbarrier
 //             complete_tx in one message, no release fence); both CTAs now own the statistics of the 512-wide rows
-//   pass 2    y = (v - mean) rstd gamma + beta -> [hi | lo] fp16, stored in place
-// The residual is read and written only by the thread that owns the element, so in-place update needs no ordering
-// beyond program order.  The producer streams the next tile's operands while the consumers run this epilogue.
+//   pass 2    y = (v - mean) rstd gamma + beta -> [hi | lo] fp16, written back over the slab element by element (only the
+//             owning thread touches each one); group by group, each warpgroup ships its 64 rows with TMA stores and hands
+//             the ring stage back once the store has read it, so the next tile's first k-blocks load under the epilogue.
+// Tail rows: loads zero-fill past row M (a box that lies wholly past M is not loaded), stores clip at M.
 #pragma once
 #include "epilogues.cuh"
 #include "gemm.cuh"
@@ -24,6 +30,13 @@ constexpr int GLN_D = 512;
 constexpr int GLN_BN = 256;                       // columns per CTA
 constexpr int GLN_STAGE_BYTES = (128 + GLN_BN) * GEMM_BLOCK_K * 2;   // 48 KB
 constexpr int GLN_STAGES = 4;
+// residual groups: 64 columns of the CTA's 256, hi slab [128 rows x 128 B] then lo slab, in one ring stage
+constexpr int GLN_GROUPS = GLN_BN / 64;
+constexpr int GLN_RES_BOX_ROWS = 64;                            // box of the residual map: one consumer warpgroup's rows
+constexpr int GLN_RES_BOX_BYTES = GLN_RES_BOX_ROWS * 128;       // 8 KB
+constexpr int GLN_RES_HALF = GEMM_BLOCK_M * 128;                // 16 KB: the hi (or lo) slab of a group
+static_assert(2 * GLN_RES_HALF <= GLN_STAGE_BYTES, "a residual group fits in one ring stage");
+static_assert(GLN_GROUPS <= GLN_STAGES, "a tile's residual groups occupy distinct ring stages");
 // setmaxnreg: the producer warpgroup hands its registers to the consumers, whose 128 accumulators stay live through
 // the epilogue (40 + 2 x 232 = 504 <= 3 x 168, the pool a 384-thread CTA gets at launch)
 constexpr int GLN_REGS_PRODUCER = 40, GLN_REGS_CONSUMER = 232;
@@ -42,19 +55,22 @@ struct GemmLnParams {
 };
 
 // map_a: A [M, K] fp16, box 128 rows; map_b: W [512, K] fp16, box 256 rows;
-// hres: the residual stream h, fp16 [M, 1024] = [hi | lo] (hi + lo carries ~22 bits), updated in place.
+// map_h: the residual stream h, fp16 [M, 1024] = [hi | lo] (hi + lo carries ~22 bits), box 64 rows x 64 columns,
+// 128-byte swizzle; updated in place.
 // The hi half doubles as the fp16 A operand of the next GEMM (the trans_dec engine feeds both halves, K = 1024).
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GLN_THREADS, 1)
 gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                      __half* __restrict__ hres, int M, int K, const GemmLnParams lp) {
+                      const __grid_constant__ CUtensorMap map_h, int M, int K, const GemmLnParams lp) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // 1024-byte alignment as an offset from smem_raw, so that the compiler still sees shared-memory pointers (LDS / STS)
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* tiles = smem;
   float* prm = reinterpret_cast<float*>(smem + GLN_STAGES * GLN_STAGE_BYTES);   // bias | gamma | beta  (this CTA's 256 cols)
   float2* st_remote = reinterpret_cast<float2*>(prm + 3 * GLN_BN);             // [2 stages][128 rows], written by the PEER
   uint64_t* bars = reinterpret_cast<uint64_t*>(st_remote + 256);
   uint64_t* full_bar = bars;                       // [STAGES]
-  uint64_t* empty_bar = bars + GLN_STAGES;         // [STAGES]  one arrival per consumer warp
+  uint64_t* empty_bar = bars + GLN_STAGES;         // [STAGES]  8 arrivals: one per consumer warp (k-block), or 4 from
+                                                   //           each warpgroup's store thread (residual group)
   uint64_t* xbar = bars + 2 * GLN_STAGES;          // [2 stages][8 consumer warps]  peer's statistics have landed
 
   const int warp = threadIdx.x >> 5;
@@ -75,6 +91,7 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
+    tma_prefetch_desc(&map_h);
     for (int s = 0; s < GLN_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);
@@ -101,6 +118,22 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
           tma_load_2d(sa + 16384, &map_b, &full_bar[stage], kb * GEMM_BLOCK_K, col_cta);
           if (++stage == GLN_STAGES) { stage = 0; phase ^= 1; }
         }
+        // the tile's residual, group by group, into the next ring stages (hi slab | lo slab)
+        const int r0 = tile * GEMM_BLOCK_M;
+        const bool two = r0 + GLN_RES_BOX_ROWS < M;   // the second warpgroup's rows exist
+        for (int grp = 0; grp < GLN_GROUPS; ++grp) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sr = tiles + stage * GLN_STAGE_BYTES;
+          const int c = col_cta + 64 * grp;
+          mbar_expect_tx(&full_bar[stage], (two ? 4 : 2) * GLN_RES_BOX_BYTES);
+          tma_load_2d(sr, &map_h, &full_bar[stage], c, r0);
+          tma_load_2d(sr + GLN_RES_HALF, &map_h, &full_bar[stage], GLN_D + c, r0);
+          if (two) {
+            tma_load_2d(sr + GLN_RES_BOX_BYTES, &map_h, &full_bar[stage], c, r0 + GLN_RES_BOX_ROWS);
+            tma_load_2d(sr + GLN_RES_HALF + GLN_RES_BOX_BYTES, &map_h, &full_bar[stage], GLN_D + c, r0 + GLN_RES_BOX_ROWS);
+          }
+          if (++stage == GLN_STAGES) { stage = 0; phase ^= 1; }
+        }
       }
     }
   } else {
@@ -111,6 +144,10 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
     const int cw = warp - 4;                          // consumer warp 0..7
     const int g = lane >> 2, t = lane & 3;
     const int lrow = 64 * wg + 16 * wq + g;           // first of this thread's two rows inside the tile (+8 for the second)
+    const bool store_thread = wq == 0 && lane == 0;   // issues the warpgroup's residual stores
+    // byte offset of this thread's column pair in row lrow of a 128-byte-swizzled slab, before the chunk index: column
+    // 8 jj + 2 t of a group sits in 16-byte chunk jj ^ (row & 7) = jj ^ g (row lrow + 8 is 1024 bytes further, same chunk)
+    const int toff = lrow * 128 + 4 * t;
     const float* bias_s = prm;
     const float* gamma_s = prm + GLN_BN;
     const float* beta_s = prm + 2 * GLN_BN;
@@ -142,24 +179,29 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      // the residual groups sit in the next GLN_GROUPS ring stages: group grp in stage (rs0 + grp) % GLN_STAGES
+      const int rs0 = stage;
+      const uint32_t rph0 = phase;
 
       // ---- pass 1: v = residual + (acc + bias) in place, partial statistics of the two rows
-      const int row_a = tile * GEMM_BLOCK_M + lrow, row_b = row_a + 8;
-      const bool live_a = row_a < M, live_b = row_b < M;
-      __half2* ha = reinterpret_cast<__half2*>(hres + static_cast<size_t>(live_a ? row_a : 0) * (2 * GLN_D) + col_cta);
-      __half2* hb = reinterpret_cast<__half2*>(hres + static_cast<size_t>(live_b ? row_b : 0) * (2 * GLN_D) + col_cta);
       float sa = 0.f, qa = 0.f, sb = 0.f, qb = 0.f;
 #pragma unroll
       for (int j = 0; j < GLN_BN / 8; ++j) {
+        const int grp = j >> 3, jj = j & 7;
+        const int rs = (rs0 + grp) % GLN_STAGES;
+        if (jj == 0) mbar_wait(&full_bar[rs], rph0 ^ (rs0 + grp >= GLN_STAGES ? 1u : 0u));
+        const uint8_t* slab = tiles + rs * GLN_STAGE_BYTES + toff + ((jj ^ g) << 4);
         const int c = 8 * j + 2 * t;                   // local column of acc[4j], acc[4j+1] (and of acc[4j+2..3], row b)
         const float2 bb = *reinterpret_cast<const float2*>(bias_s + c);
-        float2 ra = make_float2(0.f, 0.f), rb = make_float2(0.f, 0.f);
-        if (live_a) {
-          const float2 h = __half22float2(ha[c >> 1]), l = __half22float2(ha[(GLN_D + c) >> 1]);
+        float2 ra, rb;
+        {
+          const float2 h = __half22float2(*reinterpret_cast<const __half2*>(slab));
+          const float2 l = __half22float2(*reinterpret_cast<const __half2*>(slab + GLN_RES_HALF));
           ra = make_float2(h.x + l.x, h.y + l.y);
         }
-        if (live_b) {
-          const float2 h = __half22float2(hb[c >> 1]), l = __half22float2(hb[(GLN_D + c) >> 1]);
+        {
+          const float2 h = __half22float2(*reinterpret_cast<const __half2*>(slab + 1024));
+          const float2 l = __half22float2(*reinterpret_cast<const __half2*>(slab + GLN_RES_HALF + 1024));
           rb = make_float2(h.x + l.x, h.y + l.y);
         }
         acc[4 * j] = ra.x + (acc[4 * j] + bb.x);
@@ -191,28 +233,50 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
       const float mean_a = (sa + pa.x) * (1.f / GLN_D), mean_b = (sb + pb.x) * (1.f / GLN_D);
       const float rstd_a = rsqrtf(fmaxf((qa + pa.y) * (1.f / GLN_D) - mean_a * mean_a, 0.f) + lp.eps);
       const float rstd_b = rsqrtf(fmaxf((qb + pb.y) * (1.f / GLN_D) - mean_b * mean_b, 0.f) + lp.eps);
-      // ---- pass 2: y -> [hi | lo] in place
+      // ---- pass 2: y -> [hi | lo] over the slab, then out by TMA store, one group at a time
+      const int row_wg = tile * GEMM_BLOCK_M + 64 * wg;   // first row of this warpgroup's half of the tile
 #pragma unroll
       for (int j = 0; j < GLN_BN / 8; ++j) {
+        const int grp = j >> 3, jj = j & 7;
+        const int rs = (rs0 + grp) % GLN_STAGES;
+        uint8_t* slab = tiles + rs * GLN_STAGE_BYTES + toff + ((jj ^ g) << 4);
         const int c = 8 * j + 2 * t;
         const float2 gg = *reinterpret_cast<const float2*>(gamma_s + c);
         const float2 ee = *reinterpret_cast<const float2*>(beta_s + c);
-        if (live_a) {
+        {
           const float y0 = (acc[4 * j] - mean_a) * rstd_a * gg.x + ee.x, y1 = (acc[4 * j + 1] - mean_a) * rstd_a * gg.y + ee.y;
           const __half2 h = __floats2half2_rn(y0, y1);
           const float2 f = __half22float2(h);
-          ha[c >> 1] = h;
-          ha[(GLN_D + c) >> 1] = __floats2half2_rn(y0 - f.x, y1 - f.y);
+          *reinterpret_cast<__half2*>(slab) = h;
+          *reinterpret_cast<__half2*>(slab + GLN_RES_HALF) = __floats2half2_rn(y0 - f.x, y1 - f.y);
         }
-        if (live_b) {
+        {
           const float y0 = (acc[4 * j + 2] - mean_b) * rstd_b * gg.x + ee.x, y1 = (acc[4 * j + 3] - mean_b) * rstd_b * gg.y + ee.y;
           const __half2 h = __floats2half2_rn(y0, y1);
           const float2 f = __half22float2(h);
-          hb[c >> 1] = h;
-          hb[(GLN_D + c) >> 1] = __floats2half2_rn(y0 - f.x, y1 - f.y);
+          *reinterpret_cast<__half2*>(slab + 1024) = h;
+          *reinterpret_cast<__half2*>(slab + GLN_RES_HALF + 1024) = __floats2half2_rn(y0 - f.x, y1 - f.y);
+        }
+        if (jj == 7) {   // the warpgroup's 64 rows of this group are complete
+          fence_proxy_async_smem();
+          named_bar_sync(1 + wg, 128);
+          if (store_thread) {
+            uint8_t* sg = tiles + rs * GLN_STAGE_BYTES + wg * GLN_RES_BOX_BYTES;
+            if (row_wg < M) {
+              const int cg = col_cta + 64 * grp;
+              tma_store_2d(&map_h, sg, cg, row_wg);
+              tma_store_2d(&map_h, sg + GLN_RES_HALF, GLN_D + cg, row_wg);
+              bulk_commit_group();
+            }
+            bulk_wait_group_read<0>();                   // the store has read the slab: the stage may be refilled
+            mbar_arrive_cnt(&empty_bar[rs], 4);
+          }
         }
       }
+      for (int grp = 0; grp < GLN_GROUPS; ++grp)
+        if (++stage == GLN_STAGES) { stage = 0; phase ^= 1; }
     }
+    if (store_thread) bulk_wait_group<0>();   // the last stores have landed before the CTA exits
   }
 
   // the peer may still be writing into this CTA's shared memory / signalling its barriers
