@@ -191,8 +191,37 @@ int b200mdm_recover_from_ric(const float* data_dev, int64_t stride_b, int64_t st
  * and N <= 64 x the number of SMs, B200MDM_ENOTIMPL otherwise). */
 int b200mdm_test_gemm_f16(const void* a16_dev, const void* w16_dev, const float* bias_dev, void* out16_dev, int32_t M,
                           int32_t N, int32_t K, int32_t act, int32_t block_n, void* stream);
-/* out16[n*S, d] = softmax(q k^T / sqrt(128) + mask) v per (sample, head); qkv16 [n*S, 3d]; kvlen int32 [n] device.
- * impl must be 0 (tensor-core kernel, S <= 256). */
+/* The two projection-GEMM epilogues b200mdm_test_gemm_f16 does not reach, on 128 x 128 tiles; a16 [M,K], w16 [N,K] fp16,
+ * bias fp32 [N], K % 8 == 0:
+ *   epi 0: EpiBiasF16Wide<GELU> (the DiP FFN up-projection): out16 fp16 [M, 2N], columns [0, N) = hi, [N, 2N) = lo with
+ *          hi + lo = gelu(A W^T + bias) to ~22 bits.  N % 64 == 0, N <= 2048.
+ *   epi 1: EpiBiasF16Global (the DiP K/V projection of all layers): out16 fp16 [M, N] = fp16(A W^T + bias), bias read
+ *          from global memory per chunk, so N is not limited by the staged-vector size.  N % 32 == 0. */
+int b200mdm_test_gemm_epi(const void* a16_dev, const void* w16_dev, const float* bias_dev, void* out16_dev, int32_t M,
+                          int32_t N, int32_t K, int32_t epi, void* stream);
+/* The embedding launches of the step (InputProcess + positional encoding, model/mdm.py:238,252,343-349) through scratch
+ * buffers allocated on `stream`: pack_input (frame t -> row s = s_off + t), split_weight of w_in, pe_bias, then the
+ * split-precision EpiEmbed GEMM.  x fp32 [B, JF, T]; w_in fp32 [d, JF]; b_in fp32 [d]; pe fp32 [>= T + s_off, d].
+ * hres16 fp16 [halves*B*S, 2d] (S = T + s_off) receives [hi | lo] of x W^T + b_in + pe[s] in rows (b, s) of each CFG
+ * half (rows s < s_off: b_in + pe[s]).  d % 64 == 0, d <= 2048, halves 1 or 2. */
+int b200mdm_test_embed(const float* x_dev, const float* w_in_dev, const float* b_in_dev, const float* pe_dev, void* hres16_dev,
+                       int32_t B, int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream);
+/* The output launches of the step through scratch buffers allocated on `stream`: blend_split of the residual stream, then
+ * the split-weight EpiOutStep GEMM (BLOCK_N 96) with the sampler update, schedule row `sched_row` (8 floats, device; see
+ * b200mdm_set_schedule) as a one-row table at index 0.
+ * hres16 fp16 [halves*B*S, 2d] = [hi | lo] (S = T + s_off; rows s >= s_off are frames); scale fp32 [B] (NULL when
+ * halves == 1); w_out fp32 [JF, d]; b_out fp32 [JF]; x_t, noise, x_out, pred_xstart fp32 [B, JF, T] (x_out may alias
+ * x_t; noise may be NULL for mode B200MDM_MODE_X0); mode B200MDM_MODE_*; flags B200MDM_FLAG_CONST_NOISE (noise [JF, T]
+ * for every sample) | B200MDM_FLAG_CLIP_DENOISED; inpaint_mask uint8 / inpaint_motion fp32 [B, JF, T] or both NULL. */
+int b200mdm_test_out_step(const void* hres16_dev, const float* scale_dev, const float* w_out_dev, const float* b_out_dev,
+                          const float* x_t_dev, const float* noise_dev, const float* sched_row_dev, int32_t mode, int32_t flags,
+                          const uint8_t* inpaint_mask_dev, const float* inpaint_motion_dev, float* x_out_dev,
+                          float* pred_xstart_dev, int32_t B, int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves,
+                          void* stream);
+/* Self-attention core (tensor-core kernel, S <= 256): softmax(q k^T / sqrt(128) + mask) v per (sample, head);
+ * qkv16 [n*S, 3d]; kvlen int32 [n] device (valid keys per sample, a prefix).
+ * impl 0: out16 fp16 [n*S, d] (the encoder); impl 1: out16 fp16 [n*S, 2d] = [hi | lo] with hi + lo = the fp32 result
+ * to ~22 bits (the DiP decoder). */
 int b200mdm_test_attention(const void* qkv16_dev, void* out16_dev, const int32_t* kvlen_dev, int32_t n_samples,
                            int32_t S, int32_t d, int32_t impl, void* stream);
 /* Cross-attention core of the trans_dec (DiP) layers, nn.MultiheadAttention(query = sequence, key = value = text memory)

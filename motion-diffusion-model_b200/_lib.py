@@ -23,7 +23,7 @@ SYMBOLS = [
     "b200mdm_denoise", "b200mdm_sample_step", "b200mdm_sample_loop", "b200mdm_q_sample", "b200mdm_launch_count",
     "b200mdm_sample_loop_range", "b200mdm_set_noise_stream", "b200mdm_philox_normal",
     "b200mdm_recover_from_ric", "b200mdm_test_gemm_f16", "b200mdm_test_attention", "b200mdm_test_cross_attention", "b200mdm_test_qkv_attention",
-    "b200mdm_test_gemm_resid_ln",
+    "b200mdm_test_gemm_resid_ln", "b200mdm_test_gemm_epi", "b200mdm_test_embed", "b200mdm_test_out_step",
 ]
 
 
@@ -82,6 +82,12 @@ def load():
         lib.b200mdm_test_cross_attention.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b200mdm_test_qkv_attention.argtypes = [vp, i32, vp, vp, vp, vp, i32, i32, vp]
     lib.b200mdm_test_gemm_resid_ln.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, vp]
+    for name, args in (("b200mdm_test_gemm_epi", [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+                       ("b200mdm_test_embed", [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
+                       ("b200mdm_test_out_step", [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp,
+                                                  i32, i32, i32, i32, i32, i32, vp])):
+        if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
+            getattr(lib, name).argtypes = args
     for name in SYMBOLS:
         if not hasattr(lib, name) and os.environ.get("B200MDM_LIB"):
             continue                                  # an older A/B build of the same ABI may lack the newest test hooks

@@ -1255,17 +1255,151 @@ extern "C" int b200mdm_test_gemm_f16(const void* a16_dev, const void* w16_dev, c
   return fail(B200MDM_EINVAL, "block_n must be 128 (128 x 128 tiles), 512 (128 x 256 tiles) or 513 (W-resident, 128 x 64 tiles)");
 }
 
+// Scratch device memory of a kernel-test entry point, allocated and freed in the order of `s`.
+struct StreamScratch {
+  cudaStream_t s;
+  std::vector<void*> ptrs;
+  explicit StreamScratch(cudaStream_t st) : s(st) {}
+  ~StreamScratch() {
+    for (void* p : ptrs) cudaFreeAsync(p, s);
+  }
+  template <class T>
+  int alloc(T** p, size_t n, bool zero = false) {
+    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(p), n * sizeof(T), s));
+    ptrs.push_back(*p);
+    if (zero) CUDA_TRY(cudaMemsetAsync(*p, 0, n * sizeof(T), s));
+    return B200MDM_OK;
+  }
+};
+
+static int device_sms(int* sms) {
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  CUDA_TRY(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_test_gemm_epi(const void* a16_dev, const void* w16_dev, const float* bias_dev, void* out16_dev,
+                                     int32_t M, int32_t N, int32_t K, int32_t epi, void* stream) {
+  if (!a16_dev || !w16_dev || !bias_dev || !out16_dev || M <= 0 || N <= 0 || K <= 0 || K % 8)
+    return fail(B200MDM_EINVAL, "bad argument (K %% 8 == 0 required)");
+  TRY(init_kernel_attrs());
+  int sms = 132;
+  TRY(device_sms(&sms));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUtensorMap ma, mb, mc;
+  TRY(make_map(&ma, a16_dev, M, K, K, GEMM_BLOCK_M));
+  TRY(make_map(&mb, w16_dev, N, K, K, 128));
+  if (epi == 0) {
+    // the hi slab of the last 64-column block must not reach into the lo half: N % 64 == 0
+    if (N % 64) return fail(B200MDM_EINVAL, "EpiBiasF16Wide needs N %% 64 == 0");
+    TRY(make_map_t(&mc, out16_dev, 2, M, 2 * static_cast<uint64_t>(N), 2 * static_cast<uint64_t>(N), 32));
+    EpiBiasF16Wide<true>::Params p{bias_dev, N};
+    return launch_gemm<128, EpiBiasF16Wide<true>>(ma, mb, mc, M, N, K, p, s, sms);
+  }
+  if (epi == 1) {
+    if (N % 32) return fail(B200MDM_EINVAL, "EpiBiasF16Global needs N %% 32 == 0");
+    TRY(make_map_t(&mc, out16_dev, 2, M, N, N, 32));
+    EpiBiasF16Global::Params p{bias_dev};
+    return launch_gemm<128, EpiBiasF16Global>(ma, mb, mc, M, N, K, p, s, sms);
+  }
+  return fail(B200MDM_EINVAL, "epi must be 0 (EpiBiasF16Wide<GELU>) or 1 (EpiBiasF16Global)");
+}
+
+extern "C" int b200mdm_test_embed(const float* x_dev, const float* w_in_dev, const float* b_in_dev, const float* pe_dev,
+                                  void* hres16_dev, int32_t B, int32_t JF, int32_t T, int32_t d, int32_t s_off,
+                                  int32_t halves, void* stream) {
+  if (!x_dev || !w_in_dev || !b_in_dev || !pe_dev || !hres16_dev || B <= 0 || JF <= 0 || T <= 0 || s_off < 0 ||
+      d <= 0 || d % 64 || d * 4 > GEMM_BIAS_BYTES || (halves != 1 && halves != 2))
+    return fail(B200MDM_EINVAL, "bad argument (d %% 64 == 0, d <= %d, halves 1 or 2)", GEMM_BIAS_BYTES / 4);
+  TRY(init_kernel_attrs());
+  int sms = 132;
+  TRY(device_sms(&sms));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int S = T + s_off, Kp = (JF + 7) & ~7, MB = B * S;
+  StreamScratch scr(s);
+  __half *xin16 = nullptr, *w_in3 = nullptr;
+  float* pe_bias = nullptr;
+  TRY(scr.alloc(&xin16, static_cast<size_t>(MB) * 3 * Kp, true));   // rows s < s_off and the pad columns stay zero
+  TRY(scr.alloc(&w_in3, static_cast<size_t>(d) * 3 * Kp, true));
+  TRY(scr.alloc(&pe_bias, static_cast<size_t>(S) * d));
+  {
+    dim3 grid((T + 31) / 32, (JF + 31) / 32, B), block(32, 8);
+    pack_input_kernel<<<grid, block, 0, s>>>(x_dev, xin16, B, JF, T, S, Kp, 3 * Kp, s_off);
+    CUDA_TRY(cudaGetLastError());
+  }
+  split_weight_kernel<<<d, 128, 0, s>>>(w_in_dev, w_in3, d, JF, Kp);
+  CUDA_TRY(cudaGetLastError());
+  pe_bias_kernel<<<S, 128, 0, s>>>(pe_bias, pe_dev, b_in_dev, S, d);
+  CUDA_TRY(cudaGetLastError());
+  CUtensorMap m_xin, m_win;
+  TRY(make_map(&m_xin, xin16, MB, 3 * Kp, 3 * Kp, GEMM_BLOCK_M));
+  TRY(make_map(&m_win, w_in3, d, 3 * Kp, 3 * Kp, 128));
+  EpiEmbed::Params p;
+  TRY(make_map_res(&p.res_c, hres16_dev, MB, d));
+  TRY(make_map_res(&p.res_u, static_cast<__half*>(hres16_dev) + (halves == 2 ? static_cast<size_t>(MB) * d * 2 : 0), MB, d));
+  p.pe_bias = pe_bias;
+  p.S = S; p.d = d; p.halves = halves;
+  return launch_gemm<128, EpiEmbed>(m_xin, m_win, m_xin, MB, d, 3 * Kp, p, s, sms);
+}
+
+extern "C" int b200mdm_test_out_step(const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
+                                     const float* b_out_dev, const float* x_t_dev, const float* noise_dev,
+                                     const float* sched_row_dev, int32_t mode, int32_t flags, const uint8_t* inpaint_mask_dev,
+                                     const float* inpaint_motion_dev, float* x_out_dev, float* pred_xstart_dev, int32_t B,
+                                     int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream) {
+  if (!hres16_dev || !w_out_dev || !b_out_dev || !x_t_dev || !x_out_dev || !pred_xstart_dev || B <= 0 || JF <= 0 ||
+      T <= 0 || s_off < 0 || d <= 0 || d % 64 || (halves != 1 && halves != 2) || (halves == 2 && !scale_dev) ||
+      mode < B200MDM_MODE_X0 || mode > B200MDM_MODE_DDIM || (mode != B200MDM_MODE_X0 && (!noise_dev || !sched_row_dev)) ||
+      (inpaint_mask_dev == nullptr) != (inpaint_motion_dev == nullptr))
+    return fail(B200MDM_EINVAL, "bad argument");
+  TRY(init_kernel_attrs());
+  int sms = 132;
+  TRY(device_sms(&sms));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int S = T + s_off, N_out_pad = ((JF + 95) / 96) * 96;
+  StreamScratch scr(s);
+  __half *g16 = nullptr, *w_out3 = nullptr;
+  StepState* st = nullptr;
+  TRY(scr.alloc(&g16, static_cast<size_t>(B) * T * 3 * d));
+  TRY(scr.alloc(&w_out3, static_cast<size_t>(N_out_pad) * 3 * d, true));
+  TRY(scr.alloc(&st, 1, true));   // cur = 0: the one-row schedule table
+  split_weight_kernel<<<JF, 128, 0, s>>>(w_out_dev, w_out3, JF, d, d);
+  CUDA_TRY(cudaGetLastError());
+  blend_split_kernel<<<(B * T + 7) / 8, 256, 0, s>>>(static_cast<const __half*>(hres16_dev), g16, scale_dev, B, S, T, s_off, d,
+                                                     halves);
+  CUDA_TRY(cudaGetLastError());
+  CUtensorMap m_g16, m_wout;
+  TRY(make_map(&m_g16, g16, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
+  TRY(make_map(&m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
+  EpiOutStep::Params p;
+  p.bias = b_out_dev;
+  p.x_t = x_t_dev;
+  p.noise = noise_dev;
+  p.x_out = x_out_dev;
+  p.pred_xstart = pred_xstart_dev;
+  p.inpaint_mask = inpaint_mask_dev;
+  p.inpaint_motion = inpaint_motion_dev;
+  p.sched = sched_row_dev;
+  p.state = st;
+  p.noise_batch_stride = (flags & B200MDM_FLAG_CONST_NOISE) ? 0 : static_cast<long long>(JF) * T;
+  p.B = B; p.S = T; p.T = T; p.J = JF; p.mode = mode;      // g16 rows are frames: row = b*T + t
+  p.s_off = 0;
+  p.clip_denoised = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  return launch_gemm<96, EpiOutStep>(m_g16, m_wout, m_g16, B * T, N_out_pad, 3 * d, p, s, sms);
+}
+
 extern "C" int b200mdm_test_attention(const void* qkv16_dev, void* out16_dev, const int32_t* kvlen_dev,
                                       int32_t n_samples, int32_t S, int32_t d, int32_t impl, void* stream) {
   if (!qkv16_dev || !out16_dev || !kvlen_dev || n_samples <= 0 || S <= 0) return fail(B200MDM_EINVAL, "bad argument");
   TRY(init_kernel_attrs());
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (impl != 0) return fail(B200MDM_EINVAL, "impl 0 is the only attention kernel");
+  if (impl != 0 && impl != 1) return fail(B200MDM_EINVAL, "impl must be 0 (fp16 output) or 1 ([hi | lo] output)");
   if (S > ATC_MAX_KEYS) return fail(B200MDM_EINVAL, "attention handles at most %d tokens", ATC_MAX_KEYS);
   CUtensorMap mkv;
   TRY(make_map_3d(&mkv, qkv16_dev, n_samples, S, 3 * d, 3 * d, (S + 15) & ~15));
   return launch_attention_tc(mkv, static_cast<const __half*>(qkv16_dev), static_cast<__half*>(out16_dev), kvlen_dev, n_samples,
-                             S, d, d / ATC_DH, s);
+                             S, d, d / ATC_DH, s, impl == 1);
 }
 
 extern "C" int b200mdm_test_cross_attention(const void* q16_dev, const void* kv16_dev, const unsigned char* mask_dev,

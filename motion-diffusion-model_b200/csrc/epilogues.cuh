@@ -44,9 +44,12 @@ __device__ __forceinline__ void join_hi_lo8(const uint4& h, const uint4& l, floa
 }
 
 // exact (erf) GELU, torch F.gelu default (reference model/mdm.py:80 activation="gelu"):  gelu(x) = x * Phi(x).
-// Phi(-t) = 2^q(t) with q a degree-6 minimax fit of log2(0.5*erfc(t/sqrt 2)) on [0, 5.5] (|Phi error| < 1.5e-7,
-// |gelu error| < 8e-7 over all x, checked against torch fp64 in tests); Phi(t) = 1 - Phi(-t).  11 FP32 ops + one
-// MUFU.EX2 instead of the ~25 of erff() -- the epilogue of the FFN up-projection runs 26 M of these per layer.
+// Phi(-t) = 2^q(t) with q a degree-6 minimax fit of log2(0.5*erfc(t/sqrt 2)) on [0, 5.5] (|Phi error| < 1.5e-7);
+// Phi(t) = 1 - Phi(-t).  Below x = -5.5 the result is 0: |gelu(x)| < |gelu(-5.5)| = 1.1e-7 there, while the clamped
+// polynomial would return x * Phi(-5.5), an error that grows with |x| (1.8e-5 at x = -1000).  |gelu error| < 8e-7 +
+// 2^-22 |gelu(x)| over all x: tests/test_epilogues_gpu.py::test_gelu_sweep checks it against fp64 erfc from -1008 to 6.
+// 11 FP32 ops + one MUFU.EX2 instead of the ~25 of erff() -- the epilogue of the FFN up-projection runs 26 M of these
+// per layer.
 __device__ __forceinline__ float gelu_erf(float x) {
   const float t = fminf(fabsf(x), 5.5f);
   float q = 1.9175331544829533e-05f;
@@ -58,7 +61,7 @@ __device__ __forceinline__ float gelu_erf(float x) {
   q = fmaf(q, t, -0.9999997019767761f);
   float a;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(a) : "f"(q));
-  const float phi = (x >= 0.f) ? (1.0f - a) : a;
+  const float phi = (x >= 0.f) ? (1.0f - a) : (x < -5.5f ? 0.f : a);
   return x * phi;
 }
 

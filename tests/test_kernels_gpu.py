@@ -1,6 +1,7 @@
 """GPU: each hand-written kernel against a plain torch fp32 restatement of the same op (through the C ABI)."""
 import ctypes
 
+import numpy as np
 import pytest
 import torch
 
@@ -114,6 +115,103 @@ def test_attention(n, S, kv, impl):
     ref = (torch.softmax(s, -1) @ v).permute(0, 2, 1, 3).reshape(n * S, d)
     assert torch.isfinite(out.float()).all()
     assert (out.float() - ref).abs().max().item() < 5e-3
+
+
+def _half_ulp16(v):
+    """Half the fp16 spacing at |v| (the larger spacing at a binade edge)."""
+    h = v.abs().float().clamp(max=65504.0).half().double()
+    _, e = torch.frexp(h)
+    e = torch.where(h == 0, torch.full_like(e, -13), e)
+    return torch.ldexp(torch.ones_like(h), (e - 1).clamp(min=-14) - 11)
+
+
+def _attn_emulate(s, v, valid, max_keys, c):
+    """fp64 restatement of attention_tc_kernel for exact fp32 logits s [n, H, S, S] (raw q.k) and v [n, H, S, dh]:
+    offset m = fp32(max over `max_keys` of s * c), p = 2^fp32(s c - m) (fmaf: one rounding), P = fp16(p) in P V, the row
+    sum of the unrounded p.  Returns O, A = sum P |v| / l (the magnitude the accumulation works at) and F = sum over the
+    keys whose p lies within the ex2.approx error (2^-21 relative) of an fp16 rounding boundary of ulp16(p) |v| / l
+    (those may round either way)."""
+    m = s.masked_fill(~max_keys, float("-inf")).amax(-1, keepdim=True)
+    off = (m * c).float().double()
+    p = torch.exp2((s * c - off).float().double()).masked_fill(~valid, 0.0)
+    P = p.float().half().double()
+    l = p.sum(-1, keepdim=True)
+    d = 2.0 ** -21
+    flip = (p * (1 + d)).float().half() != (p * (1 - d)).float().half()
+    U = torch.where(flip, 2 * _half_ulp16(p), torch.zeros_like(p))
+    va = v.abs()
+    return (P @ v) / l, (P @ va) / l, (U @ va) / l
+
+
+@pytest.mark.parametrize("impl", [0, 1])
+@pytest.mark.parametrize("n,S,kv", [(4, 60, [60, 1, 16, 17]), (5, 197, [197, 1, 16, 17, 150]), (3, 209, [209, 17, 200]),
+                                    (4, 256, [256, 1, 16, 129]), (256, 60, "mixed")])
+def test_attention_peaked(n, S, kv, impl):
+    """Both attention_tc_kernel variants (impl 0: fp16 out, the encoder; impl 1: [hi | lo] out, DiP) on peaked softmax
+    rows, against an fp64 restatement of the kernel's arithmetic.  q = integers in [-6, 6], k = halves in [-3, 3]: every
+    logit is exact in fp32, so the only differences are ex2.approx, the fp32 row sum and P V accumulation, and the output
+    rounding.  Logits span about +-30 / sqrt(128)-scaled; the first masked key of every sample (key kvlen) carries the
+    row's largest logit (~100), so a kernel that lets a masked key into the maximum or the sum fails.  S = 209 is above
+    the 208 keys two CTAs per SM hold; S > 128 has a second query tile."""
+    L, lib = _lib()
+    d, H, dh = 512, 4, 128
+    if kv == "mixed":
+        kv = [[60, 1, 16, 17, 33, 59][i % 6] for i in range(n)]
+    g = torch.Generator(device="cuda").manual_seed(S * 31 + n)
+    sign = torch.randint(0, 2, (n, 1, H, dh), device="cuda", generator=g).float() * 2 - 1
+    q = sign * torch.randint(0, 7, (n, S, H, dh), device="cuda", generator=g).float()
+    k = torch.randint(-6, 7, (n, S, H, dh), device="cuda", generator=g).float() / 2
+    kvlen = torch.tensor(kv, device="cuda", dtype=torch.int32)
+    for i, kl in enumerate(kv):
+        if kl < S:
+            k[i, kl] = 3 * sign[i, 0]                          # aligned with every query row of the sample: the largest logit
+    v = torch.randn(n, S, H, dh, device="cuda", generator=g)
+    qkv = torch.cat([q.reshape(n * S, d), k.reshape(n * S, d), v.reshape(n * S, d)], 1).half().contiguous()
+    out = torch.full((n * S, (2 if impl else 1) * d), float("nan"), device="cuda", dtype=torch.float16)
+    L.check(lib.b200mdm_test_attention(_p(qkv), _p(out), _p(kvlen), n, S, d, impl, _stream()))
+    torch.cuda.synchronize()
+
+    qq, kk, vv = (t.double().permute(0, 2, 1, 3) for t in (q, k, qkv[:, 2 * d:].view(n, S, H, dh)))
+    s = qq @ kk.transpose(-1, -2)                              # exact: multiples of 1/2 below 2^12
+    c = float(np.float32(np.float32(1.4426950408889634) / np.sqrt(np.float32(128.0))))
+    key = torch.arange(S, device="cuda")
+    valid = (key[None, :] < kvlen[:, None])[:, None, None, :]
+    O, A, F = _attn_emulate(s, vv, valid, valid, c)
+    blocks = ((kvlen.clamp(max=S) + 15) // 16).double()[:, None, None, None]
+    # P V over 16*blocks keys (accumulator updates every ACC_CHUNK = 4 products, 2^-23 each, of a partial sum <= A l);
+    # row sum: 4 fp32 adds per block + 2 shuffles; ex2.approx 2^-21 on l; 1/l, O * (1/l) and hi + lo: 4 roundings
+    rel = 4 * blocks * 2.0 ** -23 + (4 * blocks + 2) * 2.0 ** -24 + 2.0 ** -21 + 4 * 2.0 ** -24
+    slack = rel * A + F
+    mx = _attn_emulate(s, vv, valid, (key < S)[None, None, None, :].expand_as(valid), c)[0]
+    plus1 = (key[None, :] < (kvlen.clamp(max=S - 1) + 1)[:, None])[:, None, None, :]
+    k1 = _attn_emulate(s, vv, plus1, plus1, c)[0]
+
+    def rows(t):                                               # [n, H, S, dh] -> [n*S, d]
+        return t.permute(0, 2, 1, 3).reshape(n * S, d)
+    O, slack, mx, k1 = rows(O), rows(slack), rows(mx), rows(k1)
+    if impl == 0:
+        got = out.double()
+        bound = _half_ulp16(O.abs() + slack) + slack
+        mutants = {"max over all keys": (mx.float().half().double() - O).abs(),
+                   "kvlen + 1 keys": (k1.float().half().double() - O).abs()}
+    else:
+        hi = out[:, :d].double()
+        got = hi + out[:, d:].double()
+        bound = slack + 2.0 ** -22 * O.abs() + 2.0 ** -25
+        mutants = {"max over all keys": (mx - O).abs(), "kvlen + 1 keys": (k1 - O).abs(), "lo half zeroed": (hi - O).abs()}
+    err = (got - O).abs()
+    ratio = (err / bound).max().item()
+    msg = ["attention impl=%d n=%d S=%d: kernel error / bound = %.3g" % (impl, n, S, ratio)]
+    bad = []
+    for name, me in mutants.items():
+        mr = (me / bound).max().item()
+        msg.append("  mutant %-20s error / bound = %.3g" % (name + ":", mr))
+        if not mr >= 8:
+            bad.append(name)
+    print("\n".join(msg))
+    assert torch.isfinite(got).all()
+    assert ratio <= 1.0, ratio
+    assert not bad, bad
 
 
 @pytest.mark.parametrize("n,S,kv,ld", [(3, 197, [197, 121, 58], 1024), (2, 41, [41, 1], 512), (4, 61, [61, 46, 31, 2], 512),
