@@ -236,6 +236,14 @@ static int set_gemm_attr() {
                                 GemmSmem<BN, Epi, RES>::TOTAL));
   return B200MDM_OK;
 }
+template <int KEYS>
+static int set_attention_attr() {
+  CUDA_TRY(cudaFuncSetAttribute(attention_tc_kernel<KEYS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                AttnTcSmem::total(KEYS)));
+  CUDA_TRY(cudaFuncSetAttribute(attention_tc_kernel<KEYS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                AttnTcSmem::total(KEYS)));
+  return B200MDM_OK;
+}
 static int init_kernel_attrs() {
   // function attributes are per device: track which ordinals have been initialised
   static unsigned long long done_mask = 0;
@@ -253,10 +261,9 @@ static int init_kernel_attrs() {
   CUDA_TRY(cudaFuncSetAttribute(gemm_resid_ln_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmLnSmem::TOTAL));
   TRY((set_gemm_attr<128, EpiEmbed>()));
   TRY((set_gemm_attr<96, EpiOutStep>()));
-  CUDA_TRY(cudaFuncSetAttribute(attention_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                AttnTcSmem::total(ATC_MAX_KEYS)));
-  CUDA_TRY(cudaFuncSetAttribute(attention_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                AttnTcSmem::total(ATC_MAX_KEYS)));
+  TRY((set_attention_attr<64>()));
+  TRY((set_attention_attr<208>()));
+  TRY((set_attention_attr<256>()));
   if (dev < 64) done_mask |= 1ull << dev;
   return B200MDM_OK;
 }
@@ -342,16 +349,27 @@ static int launch_gemm_resid_ln(const CUtensorMap& a, const CUtensorMap& w256, c
 }
 
 // attention core for sequences of up to 256 tokens (every configuration of the reference: 197 / 61 / 60)
-// map_kv: qkv viewed per sample, box {64, round_up(S, 16), 1} (make_map_3d)
+// map_kv: qkv viewed per sample, box {64, atc_keys(S), 1} (make_attention_kv_map)
+static int make_attention_kv_map(CUtensorMap* m, const void* qkv, int n_samples, int S, int ld) {
+  return make_map_3d(m, qkv, n_samples, S, ld, ld, atc_keys(S));
+}
+template <int KEYS>
+static cudaError_t launch_attention_keys(const CUtensorMap& map_kv, const __half* qkv, __half* out, const int* kvlen,
+                                         dim3 grid, int S, int d, float scale_log2, cudaStream_t s, bool wide) {
+  return launch_k(wide ? attention_tc_kernel<KEYS, true> : attention_tc_kernel<KEYS, false>, grid, dim3(ATC_THREADS),
+                  AttnTcSmem::total(KEYS), s, map_kv, qkv, out, kvlen, S, d, scale_log2);
+}
 static int launch_attention_tc(const CUtensorMap& map_kv, const __half* qkv, __half* out, const int* kvlen, int n_samples,
                                int S, int d, int H, cudaStream_t s, bool wide = false) {
   if (d != H * ATC_DH) return fail(B200MDM_ENOTIMPL, "attention: head_dim must be 128");
   if (S > ATC_MAX_KEYS) return fail(B200MDM_ENOTIMPL, "attention: at most %d tokens per sample", ATC_MAX_KEYS);
-  const int keys = (S + 15) & ~15;
   const float scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(ATC_DH));
-  const dim3 grid(H, n_samples, (S + ATC_QROWS - 1) / ATC_QROWS);
-  CUDA_TRY(launch_k(wide ? attention_tc_kernel<true> : attention_tc_kernel<false>, grid, dim3(ATC_THREADS), AttnTcSmem::total(keys),
-                    s, map_kv, qkv, out, kvlen, S, d, keys, scale_log2));
+  const int tiles = (S + ATC_QROWS - 1) / ATC_QROWS;
+  const dim3 grid(H, n_samples, (tiles + ATC_TILES_PER_CTA - 1) / ATC_TILES_PER_CTA);
+  const int keys = atc_keys(S);
+  if (keys == 64) CUDA_TRY(launch_attention_keys<64>(map_kv, qkv, out, kvlen, grid, S, d, scale_log2, s, wide));
+  else if (keys == 208) CUDA_TRY(launch_attention_keys<208>(map_kv, qkv, out, kvlen, grid, S, d, scale_log2, s, wide));
+  else CUDA_TRY(launch_attention_keys<256>(map_kv, qkv, out, kvlen, grid, S, d, scale_log2, s, wide));
   return B200MDM_OK;
 }
 #ifdef B200_TRACE
@@ -703,7 +721,7 @@ static int build_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStre
   TRY(make_map(&e->m_ffn, e->ffn16, M, kw * e->ff, kw * e->ff, GEMM_BLOCK_M));
   TRY(make_map(&e->m_g16, e->g16, static_cast<size_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
   TRY(make_map_t(&e->m_qkv_st, e->qkv16, 2, M, 3 * d, 3 * d, 32));
-  TRY(make_map_3d(&e->m_qkv_kv, e->qkv16, Bp, S, 3 * d, 3 * d, (S + 15) & ~15));
+  TRY(make_attention_kv_map(&e->m_qkv_kv, e->qkv16, Bp, S, 3 * d));
   TRY(make_map_t(&e->m_ffn_st, e->ffn16, 2, M, kw * e->ff, kw * e->ff, 32));
   TRY(make_map_res(&e->m_res_c, e->hres, MB, d));
   TRY(make_map_res(&e->m_res_u, e->hres + (halves == 2 ? MB * d * 2 : 0), MB, d));
@@ -1397,7 +1415,7 @@ extern "C" int b200mdm_test_attention(const void* qkv16_dev, void* out16_dev, co
   if (impl != 0 && impl != 1) return fail(B200MDM_EINVAL, "impl must be 0 (fp16 output) or 1 ([hi | lo] output)");
   if (S > ATC_MAX_KEYS) return fail(B200MDM_EINVAL, "attention handles at most %d tokens", ATC_MAX_KEYS);
   CUtensorMap mkv;
-  TRY(make_map_3d(&mkv, qkv16_dev, n_samples, S, 3 * d, 3 * d, (S + 15) & ~15));
+  TRY(make_attention_kv_map(&mkv, qkv16_dev, n_samples, S, 3 * d));
   return launch_attention_tc(mkv, static_cast<const __half*>(qkv16_dev), static_cast<__half*>(out16_dev), kvlen_dev, n_samples,
                              S, d, d / ATC_DH, s, impl == 1);
 }
@@ -1441,7 +1459,7 @@ extern "C" int b200mdm_test_qkv_attention(const void* h16_dev, int32_t ld, const
   if (r == B200MDM_OK) r = make_map(&mb, wqkv16_dev, 1536, 512, 512, 128);
   if (r == B200MDM_OK) r = make_map_t(&mc, qkv, 2, M, 1536, 1536, 32);
   if (r == B200MDM_OK) r = launch_gemm_bias<false>(ma, mb, mc, M, 1536, 512, bqkv_dev, s, sms);
-  if (r == B200MDM_OK) r = make_map_3d(&mkv, qkv, n_samples, S, 1536, 1536, (S + 15) & ~15);
+  if (r == B200MDM_OK) r = make_attention_kv_map(&mkv, qkv, n_samples, S, 1536);
   if (r == B200MDM_OK)
     r = launch_attention_tc(mkv, qkv, static_cast<__half*>(out16_dev), kvlen_dev, n_samples, S, 512, 4, s);
   CUDA_TRY(cudaFreeAsync(qkv, s));

@@ -170,6 +170,18 @@ __device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
+// The same for an MN-major operand (the transposed B of wgmma: N contiguous, e.g. V [key][dh] as the B of P V), 128-byte
+// swizzle: an atom is 64 N-elements (128 B) x 8 K-rows 128 B apart, as a TMA load with a 64-element box width writes it.
+//   leading byte offset = bytes between atoms along N (mn_atom_bytes)    stride byte offset = 1024 B between 8-row K groups
+// Advancing 16 rows along K is +2048 B on the start address.
+__device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(uint32_t smem_addr, uint32_t mn_atom_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>((mn_atom_bytes >> 4) & 0x3FFF) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -187,6 +199,10 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[NR]) {
 // registers.  Fragment of thread t of the warpgroup (warp w = t / 32, lane l): d[i] holds row 16 w + l / 4 + 8 ((i / 2) % 2),
 // column 8 (i / 4) + 2 (l % 4) + (i % 2).
 template <int N> struct Wgmma;
+// D[64 x N] (+)= A[64 x 16] * B, A from registers: warp w holds rows [16 w, +16) in the mma.sync m16n8k16 A fragment.  For
+// 16-bit A this is the accumulator fragment above rounded pairwise (d[8j..8j+7] of columns [16 j, +16) -> four .b32), so
+// an fp32 result can feed the next wgmma without a shuffle.
+template <int N, int TRANS_B> struct WgmmaRA;
 #include "wgmma_ops.inc"
 
 // ------------------------------------------------------------------ mma.sync / ldmatrix (warp-level tiles)
