@@ -70,8 +70,17 @@ typedef struct b200mdm_config {
   int32_t pos_embed_max_len; /* args.pos_embed_max_len: rows of the positional table */
   int32_t temb_rows;         /* model timesteps to pre-embed (>= original_num_steps of the diffusion) */
   int32_t context_len;       /* trans_dec (DiP) prefix completion: args.context_len frames precede x (model/mdm.py:58-61) */
-  int32_t reserved[6];
+  /* Target-location conditioning (args.multi_target_cond, model/mdm.py:64-73,197-199); 0 / 0 / 0 = none. */
+  int32_t target_encoder;    /* B200MDM_TARGET_*          (args.multi_encoder_type) */
+  int32_t target_enc_layers; /* args.target_enc_layers (single / split; the multi encoder always has one hidden layer) */
+  int32_t target_joints;     /* n_ext = len(all_goal_joint_names) + 2 ('traj', 'heading'): 8 for HumanML3D */
+  int32_t reserved[3];
 } b200mdm_config;
+
+#define B200MDM_TARGET_NONE 0
+#define B200MDM_TARGET_SINGLE 1 /* EmbedTargetLocSingle: one MLP on cat(target, valid) [4 n_ext] */
+#define B200MDM_TARGET_MULTI 2  /* EmbedTargetLocMulti: an MLP per valid joint, combined by WeightedSum */
+#define B200MDM_TARGET_SPLIT 3  /* EmbedTargetLocSplit: a mini-MLP of width d / n_ext per joint, concatenated */
 
 const char* b200mdm_last_error(void);
 int b200mdm_version(void);
@@ -83,7 +92,9 @@ int b200mdm_destroy(b200mdm_engine* e);
 /* load_model_wo_clip / load_state_dict(strict=False) (utils/model_util.py:8-15): one call per state_dict entry,
  * `name` is the reference key (SURVEY.md A.4), data fp32, host or device memory.  "sequence_pos_encoder.pe"
  * ([max_len, d]; the buffer the reference recomputes in PositionalEncoding.__init__, model/mdm.py:301-308) is
- * accepted here as well.  Unknown names -> B200MDM_EINVAL (the reference asserts no unexpected keys). */
+ * accepted here as well.  Unknown names -> B200MDM_EINVAL (the reference asserts no unexpected keys).
+ * With target_encoder != 0 the embed_target_cond.* keys are accepted too; the multi encoder's per-joint keys name the
+ * joint by its position in the extended joint list: "embed_target_cond.target_loc_emb.<index>.{0,2}.{weight,bias}". */
 int b200mdm_load_weight(b200mdm_engine* e, const char* name, const float* data, const int64_t* shape, int32_t ndim);
 
 /* Repack for the tensor cores (fp16 K-major copies, hi/lo split of the in/out projections), precompute the
@@ -122,6 +133,17 @@ int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, cons
                          const float* scale_dev, int32_t force_uncond, void* stream);
 /* y['prefix'] [batch, njoints, nfeats, context_len] fp32 device: the frames x is a continuation of. */
 int b200mdm_set_prefix(b200mdm_engine* e, const float* prefix_dev, void* stream);
+
+/* Target-location conditioning (model/mdm.py:197-199) for an engine created with target_encoder != 0.  Call it after
+ * b200mdm_set_cond / b200mdm_set_cond_dec (they size the workspace, and clear any previous target):
+ *   target_dev : y['target_cond'] [batch, target_joints, 3] fp32 device
+ *   valid_host : uint8 [batch, target_joints], 1 for each joint named in y['target_joint_names'][b], plus 'heading'
+ *                when y['is_heading'][b]
+ * g = embed_target_cond(target, valid) [batch, d] is evaluated here, in fp32, once per loop.  Every forward then adds
+ * it to the timestep embedding, in both halves of a CFG pair: the conditioning token is cond + (temb[t] + g[b]) for
+ * trans_enc, each text-memory token text_emb + (temb[t] + g[b]) for DiP.  y['target_uncond'] = True is a call that is
+ * never made. */
+int b200mdm_set_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, void* stream);
 
 /* y['inpainting_mask'] (bool as uint8) / y['inpainted_motion'] [B,J,F,T] device pointers
  * (gaussian_diffusion.py:300-304); NULL, NULL clears. */
@@ -243,6 +265,10 @@ int b200mdm_test_qkv_attention(const void* h16_dev, int32_t ld, const void* wqkv
  * 16-byte aligned. */
 int b200mdm_test_gemm_resid_ln(const void* a16_dev, const void* w16_dev, const float* bias_dev, const float* gamma_dev,
                                const float* beta_dev, void* hres16_dev, int32_t M, int32_t K, void* stream);
+/* The target encoder of b200mdm_set_target on the engine's finalised weights, for any batch, through a scratch buffer
+ * allocated on `stream`: out fp32 [batch, d] = embed_target_cond(target [batch, target_joints, 3], valid uint8 host). */
+int b200mdm_test_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, int32_t batch,
+                        float* out_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -11,6 +11,7 @@ LIB_PATH = os.environ.get("B200MDM_LIB") or os.path.join(HERE, "lib", "libb200md
 OK, EINVAL, ECUDA, ESTATE, ENOTIMPL = 0, -1, -2, -3, -4
 ARCH = {"trans_enc": 0, "trans_dec": 1}
 COND_NONE, COND_TEXT, COND_ACTION = 0, 1, 2
+TARGET = {"single": 1, "multi": 2, "split": 3}   # args.multi_encoder_type -> b200mdm_config.target_encoder (0: none)
 MODE_X0, MODE_DDPM, MODE_DDIM = 0, 1, 2
 FLAG_CONST_NOISE, FLAG_CLIP_DENOISED, FLAG_PHILOX_NOISE = 1, 2, 4
 SCHED_STRIDE = 8
@@ -24,13 +25,15 @@ SYMBOLS = [
     "b200mdm_sample_loop_range", "b200mdm_set_noise_stream", "b200mdm_philox_normal",
     "b200mdm_recover_from_ric", "b200mdm_test_gemm_f16", "b200mdm_test_attention", "b200mdm_test_cross_attention", "b200mdm_test_qkv_attention",
     "b200mdm_test_gemm_resid_ln", "b200mdm_test_gemm_epi", "b200mdm_test_embed", "b200mdm_test_out_step",
+    "b200mdm_set_target", "b200mdm_test_target",
 ]
 
 
 class Config(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in (
         "arch", "latent_dim", "ff_size", "num_layers", "num_heads", "njoints", "nfeats", "cond_mode", "cond_dim",
-        "num_actions", "mask_frames", "pos_embed_max_len", "temb_rows", "context_len")] + [("reserved", ctypes.c_int32 * 6)]
+        "num_actions", "mask_frames", "pos_embed_max_len", "temb_rows", "context_len", "target_encoder",
+        "target_enc_layers", "target_joints")] + [("reserved", ctypes.c_int32 * 3)]
 
 
 class B200MDMError(RuntimeError):
@@ -85,7 +88,9 @@ def load():
     for name, args in (("b200mdm_test_gemm_epi", [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
                        ("b200mdm_test_embed", [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
                        ("b200mdm_test_out_step", [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp,
-                                                  i32, i32, i32, i32, i32, i32, vp])):
+                                                  i32, i32, i32, i32, i32, i32, vp]),
+                       ("b200mdm_set_target", [vp, vp, vp, vp]),
+                       ("b200mdm_test_target", [vp, vp, vp, i32, vp, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

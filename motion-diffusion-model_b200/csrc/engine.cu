@@ -138,9 +138,10 @@ struct LayerW {
 struct GraphKey {
   int mode = -1, B = 0, T = 0, flags = 0;
   const void *pred = nullptr, *imask = nullptr, *imotion = nullptr;
+  const void* target_g = nullptr;   // the workspace's target embedding, or nullptr when the loop has no target
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && pred == o.pred && imask == o.imask &&
-           imotion == o.imotion;
+           imotion == o.imotion && target_g == o.target_g;
   }
 };
 
@@ -167,6 +168,10 @@ struct Workspace {
   unsigned char* memmask = nullptr;                                   // [Bp, Mt] 1 = padding
   CUtensorMap m_mem, m_qc_st, m_kvc_st;
   bool prefix_set = false;
+  // target-location conditioning: validity [B, n_ext] (1.0 / 0.0) and g = embed_target_cond(...) [B, d], read by both
+  // CFG halves; target_set is cleared by every b200mdm_set_cond* call
+  float *tgt_valid = nullptr, *tgt_g = nullptr;
+  bool target_set = false;
   // captured step graph of this workspace
   cudaGraphExec_t graph_exec = nullptr;
   GraphKey graph_key;
@@ -191,6 +196,10 @@ struct b200mdm_engine : Workspace {
   __half* wkv_all = nullptr;
   float* bkv_all = nullptr;
   CUtensorMap m_wkv_all;
+  // target encoder, packed for target_embed_kernel (kernels.cuh): G groups of width tdj, first layer tin wide
+  float *tw0 = nullptr, *tb0 = nullptr, *twk = nullptr, *tbk = nullptr, *twsum = nullptr;
+  int tG = 0, tdj = 0, tin = 0, tlayers = 0;
+  std::vector<float> h_valid;
   // schedule (device tables are allocated once at `sched_cap` rows: the step graphs hold these pointers)
   float* sched = nullptr;
   int* tmap = nullptr;
@@ -403,6 +412,15 @@ extern "C" int b200mdm_create(const b200mdm_config* cfg, b200mdm_engine** out) {
                 cfg->num_heads);
   if (cfg->num_layers <= 0 || cfg->njoints <= 0 || cfg->nfeats <= 0 || cfg->pos_embed_max_len <= 0 || cfg->temb_rows <= 0)
     return fail(B200MDM_EINVAL, "bad config");
+  if (cfg->target_encoder < B200MDM_TARGET_NONE || cfg->target_encoder > B200MDM_TARGET_SPLIT)
+    return fail(B200MDM_EINVAL, "target_encoder %d: 0 none, 1 single, 2 multi, 3 split", cfg->target_encoder);
+  if (cfg->target_encoder != B200MDM_TARGET_NONE) {
+    if (cfg->target_joints <= 0 || cfg->target_joints > 64 || cfg->target_enc_layers < 0 || cfg->target_enc_layers > 16)
+      return fail(B200MDM_EINVAL, "target encoder: 1..64 joints and 0..16 layers (got %d / %d)", cfg->target_joints,
+                  cfg->target_enc_layers);
+    if (cfg->target_encoder == B200MDM_TARGET_SPLIT && cfg->latent_dim % cfg->target_joints)
+      return fail(B200MDM_EINVAL, "split target encoder: latent_dim %% target_joints != 0 (model/mdm.py:427)");
+  }
   int dev = 0;
   CUDA_TRY(cudaGetDevice(&dev));
   cudaDeviceProp prop;
@@ -447,6 +465,7 @@ static void free_workspace(Workspace* w) {
   dfree(w->tok0); dfree(w->condproj); dfree(w->proj); dfree(w->scale); dfree(w->x_work); dfree(w->pe_bias); dfree(w->eps_buf);
   dfree(w->kvlen); dfree(w->tvec); dfree(w->action);
   dfree(w->encperm); dfree(w->memtok); dfree(w->memproj); dfree(w->mem16); dfree(w->qc16); dfree(w->kvc16); dfree(w->memmask);
+  dfree(w->tgt_valid); dfree(w->tgt_g);
   *w = Workspace();
 }
 // every workspace (the one in use and the parked ones): after a weight reload or a schedule-table move their graphs
@@ -469,6 +488,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   for (auto& l : e->layers) { dfree(l.wqkv); dfree(l.wo); dfree(l.w1); dfree(l.w2); dfree(l.wq_c); dfree(l.wo_c); }
   dfree(e->w_in3); dfree(e->w_out3); dfree(e->temb_hidden); dfree(e->temb_table); dfree(e->sched); dfree(e->tmap);
   dfree(e->wkv_all); dfree(e->bkv_all);
+  dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
   if (e->work) cudaStreamDestroy(e->work);
   if (e->ev_in) cudaEventDestroy(e->ev_in);
@@ -501,6 +521,34 @@ static bool known_weight_name(const b200mdm_engine* e, const std::string& n) {
     std::string rest = n.substr(dot + 1);
     for (const char* f : per_layer)
       if (rest == f) return true;
+  }
+  if (e->cfg.target_encoder != B200MDM_TARGET_NONE) {
+    const int tl = e->cfg.target_enc_layers, nj = e->cfg.target_joints;
+    auto lin = [](const std::string& r, int max_layer) {   // "<2k>.weight" / "<2k>.bias", k = 0..max_layer
+      for (int k = 0; k <= max_layer; ++k)
+        if (r == std::to_string(2 * k) + ".weight" || r == std::to_string(2 * k) + ".bias") return true;
+      return false;
+    };
+    auto joint = [nj](const std::string& r, std::string* tail) {   // "<i>.<tail>", i = 0..nj-1
+      size_t dot = r.find('.');
+      if (dot == std::string::npos || dot == 0 || r.find_first_not_of("0123456789") != dot) return false;
+      if (atoi(r.substr(0, dot).c_str()) >= nj) return false;
+      *tail = r.substr(dot + 1);
+      return true;
+    };
+    const std::string pre = "embed_target_cond.";
+    if (n.compare(0, pre.size(), pre) != 0) return false;
+    const std::string r = n.substr(pre.size());
+    std::string tail;
+    switch (e->cfg.target_encoder) {
+      case B200MDM_TARGET_SINGLE:
+        return r.compare(0, 4, "mlp.") == 0 && lin(r.substr(4), tl);
+      case B200MDM_TARGET_SPLIT:
+        return r.compare(0, 10, "mini_mlps.") == 0 && joint(r.substr(10), &tail) && lin(tail, tl);
+      case B200MDM_TARGET_MULTI:
+        if (r == "target_all_loc_emb.weights") return true;
+        return r.compare(0, 15, "target_loc_emb.") == 0 && joint(r.substr(15), &tail) && lin(tail, 1);
+    }
   }
   return false;
 }
@@ -549,6 +597,64 @@ static int to_f16_k(const float* src, __half** dst, int N, int K, int kw, cudaSt
   if (kw == 1) return to_f16(src, dst, static_cast<size_t>(N) * K, s);
   TRY(dalloc(dst, static_cast<size_t>(N) * K * 2));
   f32_to_f16_dup_kernel<<<512, 256, 0, s>>>(src, *dst, N, K);
+  CUDA_TRY(cudaGetLastError());
+  return B200MDM_OK;
+}
+
+// embed_target_cond.* -> the packed layout of target_embed_kernel (kernels.cuh): w0 [G][dj][in], b0 [G][dj],
+// wk [layers][G][dj][dj], bk [layers][G][dj], wsum [G] (multi).  nn.Linear weights are [out, in] already.
+static int pack_target_weights(b200mdm_engine* e, cudaStream_t s) {
+  dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
+  const int enc = e->cfg.target_encoder, n = e->cfg.target_joints, d = e->d;
+  if (enc == B200MDM_TARGET_NONE) return B200MDM_OK;
+  const bool multi = enc == B200MDM_TARGET_MULTI;
+  e->tG = enc == B200MDM_TARGET_SINGLE ? 1 : n;
+  e->tdj = enc == B200MDM_TARGET_SPLIT ? d / n : d;
+  e->tin = enc == B200MDM_TARGET_SINGLE ? 4 * n : multi ? 3 : 4;
+  e->tlayers = multi ? 1 : e->cfg.target_enc_layers;
+  const int G = e->tG, dj = e->tdj, in = e->tin, L = e->tlayers;
+  TRY(dalloc(&e->tw0, static_cast<size_t>(G) * dj * in));
+  TRY(dalloc(&e->tb0, static_cast<size_t>(G) * dj));
+  TRY(dalloc(&e->twk, static_cast<size_t>(L > 0 ? L : 1) * G * dj * dj));
+  TRY(dalloc(&e->tbk, static_cast<size_t>(L > 0 ? L : 1) * G * dj));
+  for (int i = 0; i < G; ++i) {
+    const std::string p = enc == B200MDM_TARGET_SINGLE ? std::string("embed_target_cond.mlp.")
+                          : multi ? "embed_target_cond.target_loc_emb." + std::to_string(i) + "."
+                                  : "embed_target_cond.mini_mlps." + std::to_string(i) + ".";
+    const float *w, *b;
+    TRY(need(e, p + "0.weight", {dj, in}, &w));
+    TRY(need(e, p + "0.bias", {dj}, &b));
+    CUDA_TRY(cudaMemcpyAsync(e->tw0 + static_cast<size_t>(i) * dj * in, w, sizeof(float) * dj * in, cudaMemcpyDeviceToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(e->tb0 + static_cast<size_t>(i) * dj, b, sizeof(float) * dj, cudaMemcpyDeviceToDevice, s));
+    for (int l = 0; l < L; ++l) {
+      const std::string k = std::to_string(2 * (l + 1));
+      TRY(need(e, p + k + ".weight", {dj, dj}, &w));
+      TRY(need(e, p + k + ".bias", {dj}, &b));
+      CUDA_TRY(cudaMemcpyAsync(e->twk + (static_cast<size_t>(l) * G + i) * dj * dj, w, sizeof(float) * dj * dj,
+                               cudaMemcpyDeviceToDevice, s));
+      CUDA_TRY(cudaMemcpyAsync(e->tbk + (static_cast<size_t>(l) * G + i) * dj, b, sizeof(float) * dj, cudaMemcpyDeviceToDevice, s));
+    }
+  }
+  if (multi) {
+    const float* ws;
+    TRY(need(e, "embed_target_cond.target_all_loc_emb.weights", {n}, &ws));
+    TRY(dalloc(&e->twsum, n));
+    CUDA_TRY(cudaMemcpyAsync(e->twsum, ws, sizeof(float) * n, cudaMemcpyDeviceToDevice, s));
+  }
+  return B200MDM_OK;
+}
+
+// g [B, d] = embed_target_cond(target [B, n, 3], valid) on stream s; valid_dev [B, n] receives the validity as fp32
+// (staged through `staging`, which must stay alive until the copy has run)
+static int encode_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, int B, float* valid_dev,
+                         float* g_dev, std::vector<float>& staging, cudaStream_t s) {
+  const int n = e->cfg.target_joints, d = e->d;
+  staging.assign(static_cast<size_t>(B) * n, 0.f);
+  for (size_t i = 0; i < staging.size(); ++i) staging[i] = valid_host[i] ? 1.f : 0.f;
+  CUDA_TRY(cudaMemcpyAsync(valid_dev, staging.data(), staging.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+  const size_t smem = sizeof(float) * (4 * n + 2 * d);
+  target_embed_kernel<<<B, d, smem, s>>>(target_dev, valid_dev, e->tw0, e->tb0, e->twk, e->tbk, e->twsum, g_dev, n, e->tG,
+                                         e->tdj, e->tin, e->tlayers, e->cfg.target_encoder == B200MDM_TARGET_MULTI ? 1 : 0);
   CUDA_TRY(cudaGetLastError());
   return B200MDM_OK;
 }
@@ -645,6 +751,7 @@ extern "C" int b200mdm_finalize_weights(b200mdm_engine* e, void* stream) {
     }
   }
   // timestep-embedding MLP for every model timestep: temb[t] = W2 silu(W1 pe[t] + b1) + b2
+  TRY(pack_target_weights(e, s));
   const int R = e->cfg.temb_rows;
   TRY(dalloc(&e->temb_hidden, static_cast<size_t>(R) * d));
   TRY(dalloc(&e->temb_table, static_cast<size_t>(R) * d));
@@ -730,6 +837,10 @@ static int build_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStre
   pe_bias_kernel<<<S, 128, 0, s>>>(e->pe_bias, e->pe, e->b_in, S, d);   // on the caller's stream: ordered before any forward
   CUDA_TRY(cudaGetLastError());
   TRY(dalloc(&e->eps_buf, static_cast<size_t>(B) * e->JF * T));
+  if (e->cfg.target_encoder != B200MDM_TARGET_NONE) {
+    TRY(dalloc(&e->tgt_valid, static_cast<size_t>(B) * e->cfg.target_joints));
+    TRY(dalloc(&e->tgt_g, static_cast<size_t>(B) * d));
+  }
   return B200MDM_OK;
 }
 
@@ -773,6 +884,7 @@ static int select_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStr
       cur->last_use = e->use_clock;
       cur->cond_set = false;      // the caller is about to set the conditioning of this loop
       cur->prefix_set = false;
+      cur->target_set = false;
       attach_l2_window(e);
       return B200MDM_OK;
     }
@@ -848,6 +960,7 @@ extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframe
   CUDA_TRY(cudaGetLastError());
   e->launches++;
   e->cond_set = true;
+  e->target_set = false;
   return B200MDM_OK;
 }
 
@@ -908,6 +1021,17 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
   CUDA_TRY(cudaGetLastError());
   e->launches += 3;
   e->cond_set = true;
+  e->target_set = false;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, void* stream) {
+  if (!e || !target_dev || !valid_host) return fail(B200MDM_EINVAL, "null argument");
+  if (e->cfg.target_encoder == B200MDM_TARGET_NONE) return fail(B200MDM_EINVAL, "this engine has no target encoder");
+  if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
+  TRY(encode_target(e, target_dev, valid_host, e->B, e->tgt_valid, e->tgt_g, e->h_valid, static_cast<cudaStream_t>(stream)));
+  e->launches++;
+  e->target_set = true;
   return B200MDM_OK;
 }
 
@@ -972,13 +1096,14 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     TRY((launch_gemm<128, EpiEmbed>(e->m_xin, e->m_win, e->m_xin, e->MB, d, 3 * Kp, p, s, e->num_sms)));
     ++nk;
   }
+  const float* target_g = e->target_set ? e->tgt_g : nullptr;   // timestep embedding + target (model/mdm.py:197-199)
   if (!e->dec) {
     CUDA_TRY(launch_k(tok0_rows_kernel, dim3(e->Bp), dim3(128), 0, s, e->hres, e->condproj, e->temb_table, e->pe,
-                      a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, B, S, d, e->cfg.temb_rows));
+                      a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, target_g, B, S, d, e->cfg.temb_rows));
   } else {
     // cross-attention memory of this step: text tokens + timestep embedding (model/mdm.py:218-220)
     CUDA_TRY(launch_k(mem_build_kernel, dim3(e->Mt, e->Bp), dim3(128), 0, s, e->mem16, e->memproj, e->temb_table,
-                      a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, B, e->Mt, d, e->cfg.temb_rows));
+                      a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, target_g, B, e->Mt, d, e->cfg.temb_rows));
     // ... and its key / value projections for every layer in one GEMM (N = L * 2d; hi half of the memory, K = d)
     EpiBiasF16Global::Params p{e->bkv_all};
     TRY((launch_gemm<128, EpiBiasF16Global>(e->m_mem, e->m_wkv_all, e->m_kvc_st, e->Bp * e->Mt, e->L * 2 * d, d, p, s, e->num_sms)));
@@ -1139,6 +1264,7 @@ extern "C" int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_
     GraphKey key;
     key.mode = mode; key.B = e->B; key.T = e->T; key.flags = flags;
     key.imask = e->inpaint_mask; key.imotion = e->inpaint_motion;
+    key.target_g = e->target_set ? e->tgt_g : nullptr;
     if (!e->graph_exec || !(key == e->graph_key)) {
       drop_graph(e);
       cudaGraph_t graph = nullptr;
@@ -1499,4 +1625,19 @@ extern "C" int b200mdm_recover_from_ric(const float* data_dev, int64_t stride_b,
   recover_from_ric_kernel<<<batch, 256, smem, static_cast<cudaStream_t>(stream)>>>(a);
   CUDA_TRY(cudaGetLastError());
   return B200MDM_OK;
+}
+
+extern "C" int b200mdm_test_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, int32_t batch,
+                                   float* out_dev, void* stream) {
+  if (!e || !target_dev || !valid_host || !out_dev || batch <= 0) return fail(B200MDM_EINVAL, "bad argument");
+  if (e->cfg.target_encoder == B200MDM_TARGET_NONE) return fail(B200MDM_EINVAL, "this engine has no target encoder");
+  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  float* valid = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&valid), static_cast<size_t>(batch) * e->cfg.target_joints * sizeof(float), s));
+  std::vector<float> staging;
+  const int r = encode_target(e, target_dev, valid_host, batch, valid, out_dev, staging, s);
+  cudaFreeAsync(valid, s);
+  CUDA_TRY(cudaStreamSynchronize(s));   // `staging` is local
+  return r;
 }

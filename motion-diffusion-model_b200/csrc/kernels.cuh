@@ -43,12 +43,14 @@ __global__ void pack_input_kernel(const float* __restrict__ x, __half* __restric
 // Conditioning-token rows of the sequence (reference model/mdm.py:195,218-220,251-252):
 //   h[b', s=0, :] = (condproj[b', :] + temb_table[t(b'), :]) + pe[0, :]
 //   t(b') = tvec[b' % B] when tvec != nullptr (model called with explicit timesteps), else timestep_map[state->cur]
+// With a target embedding g [B, d] (model/mdm.py:197-199, both CFG halves): (condproj + (temb + g[b' % B])) + pe[0].
 // Runs right after the embedding GEMM (which leaves placeholder values in these rows).
 // The residual stream is an fp16 [hi | lo] pair per element (row = 2d halves, hi + lo carries ~22 bits).
 __global__ void tok0_rows_kernel(__half* __restrict__ hres, const float* __restrict__ condproj,
                                  const float* __restrict__ temb_table, const float* __restrict__ pe,
                                  const int* __restrict__ tvec, const int* __restrict__ tmap,
-                                 const StepState* __restrict__ state, int B, int S, int d, int temb_rows) {
+                                 const StepState* __restrict__ state, const float* __restrict__ g, int B, int S, int d,
+                                 int temb_rows) {
   pdl_launch_dependents();
   pdl_wait();
   const int bp = blockIdx.x;
@@ -56,7 +58,9 @@ __global__ void tok0_rows_kernel(__half* __restrict__ hres, const float* __restr
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = static_cast<size_t>(bp) * S;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
-    const float v = (condproj[static_cast<size_t>(bp) * d + c] + temb_table[static_cast<size_t>(t) * d + c]) + pe[c];
+    float te = temb_table[static_cast<size_t>(t) * d + c];
+    if (g != nullptr) te = te + g[static_cast<size_t>(bp % B) * d + c];
+    const float v = (condproj[static_cast<size_t>(bp) * d + c] + te) + pe[c];
     const __half hi = __float2half_rn(v);
     hres[row * 2 * d + c] = hi;
     hres[row * 2 * d + d + c] = __float2half_rn(v - __half2float(hi));
@@ -241,6 +245,66 @@ __global__ void small_linear_kernel(const float* __restrict__ x, const float* __
   }
 }
 
+// Target-location encoder g[b, :] = embed_target_cond(target[b], valid[b]) (model/mdm.py:399-480), fp32, once per loop.
+// The three encoders share one packed weight layout of G groups of width dj:
+//   w0 [G][dj][in_dim], b0 [G][dj]: the first Linear; wk [layers][G][dj][dj], bk [layers][G][dj]: [SiLU, Linear] x layers
+//   single (EmbedTargetLocSingle): G = 1, dj = d, in_dim = 4 n: one MLP on cat(target, valid) [4 n]
+//   split  (EmbedTargetLocSplit) : G = n, dj = d / n, in_dim = 4: joint i's mini-MLP on (x, y, z, valid_i) writes
+//                                  columns [i dj, (i+1) dj)
+//   multi  (EmbedTargetLocMulti) : G = n, dj = d, in_dim = 3, layers = 1: joint i's MLP on (x, y, z), for valid joints
+//                                  only (an invalid joint's row is zero), rows combined by WeightedSum:
+//                                  g = sum_i (wsum[i] / sum(wsum)) row_i   (utils/misc.py:5-16)
+// target [B, n, 3], valid [B, n] (1.0 / 0.0).  One CTA per sample, blockDim.x == d; dynamic shared memory (4 n + 2 d) floats.
+__global__ void __launch_bounds__(512) target_embed_kernel(const float* __restrict__ target, const float* __restrict__ valid,
+                                                           const float* __restrict__ w0, const float* __restrict__ b0,
+                                                           const float* __restrict__ wk, const float* __restrict__ bk,
+                                                           const float* __restrict__ wsum, float* __restrict__ g, int n,
+                                                           int G, int dj, int in_dim, int layers, int multi) {
+  extern __shared__ float tsm[];
+  const int d = blockDim.x, b = blockIdx.x, c = threadIdx.x;
+  float* x = tsm;          // [n][4] = (x, y, z, valid) of this sample
+  float* s = x + 4 * n;    // SiLU of the hidden layer
+  float* o = s + d;        // next hidden layer
+  for (int k = c; k < 4 * n; k += d) {
+    const int j = k >> 2, q = k & 3;
+    x[k] = q < 3 ? target[(static_cast<size_t>(b) * n + j) * 3 + q] : valid[static_cast<size_t>(b) * n + j];
+  }
+  __syncthreads();
+  float wtot = 0.f;
+  if (multi)
+    for (int i = 0; i < G; ++i) wtot += wsum[i];
+  const int warp = c >> 5, lane = c & 31, nwarp = d >> 5;
+  float acc = 0.f;
+  for (int p = 0; p < (multi ? G : 1); ++p) {
+    if (multi && x[4 * p + 3] == 0.f) continue;   // (uniform over the CTA)
+    const int grp = multi ? p : c / dj, cl = multi ? c : c % dj;
+    const float* xi = x + 4 * grp;
+    const float* wr = w0 + (static_cast<size_t>(grp) * dj + cl) * in_dim;
+    float h = 0.f;
+    for (int k = 0; k < in_dim; ++k) h = fmaf(wr[k], xi[k], h);
+    h += b0[grp * dj + cl];
+    for (int l = 0; l < layers; ++l) {
+      s[c] = h / (1.f + expf(-h));
+      __syncthreads();
+      // one warp per output q, reading its weight row contiguously
+      for (int q = warp; q < d; q += nwarp) {
+        const int gq = multi ? p : q / dj, ql = multi ? q : q % dj;
+        const float* wq = wk + ((static_cast<size_t>(l) * G + gq) * dj + ql) * dj;
+        const float* sq = s + (multi ? 0 : gq * dj);
+        float a = 0.f;
+        for (int k = lane; k < dj; k += 32) a = fmaf(wq[k], sq[k], a);
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) a += __shfl_xor_sync(0xffffffffu, a, off);
+        if (lane == 0) o[q] = a + bk[(static_cast<size_t>(l) * G + gq) * dj + ql];
+      }
+      __syncthreads();
+      h = o[c];
+    }
+    acc = multi ? fmaf(wsum[p] / wtot, h, acc) : h;
+  }
+  g[static_cast<size_t>(b) * d + c] = acc;
+}
+
 // condproj rows for the packed batch: first B rows conditional, next B rows unconditional.
 //   text  : cond = (W clip + b) already in proj[B, d];  uncond = bias          (mask_cond zeros => bias only)
 //   action: cond = action_embedding[a[b]];              uncond = 0             (model/mdm.py:225-227)
@@ -279,10 +343,11 @@ namespace b200 {
 
 // mem16[b', m, :] = [hi | lo] fp16 of ( memproj[b', m, :] + temb_table[t(b'), :] )   (emb = text_emb + time_emb,
 // mdm.py:218-220; the time embedding is broadcast over the text tokens).  Rows are 2d wide.  grid = (Mt, Bp)
+// With a target embedding g [B, d] (mdm.py:197-199, both CFG halves): memproj + (temb + g[b' % B]).
 __global__ void mem_build_kernel(__half* __restrict__ mem16, const float* __restrict__ memproj,
                                  const float* __restrict__ temb_table, const int* __restrict__ tvec,
-                                 const int* __restrict__ tmap, const StepState* __restrict__ state, int B, int Mt, int d,
-                                 int temb_rows) {
+                                 const int* __restrict__ tmap, const StepState* __restrict__ state,
+                                 const float* __restrict__ g, int B, int Mt, int d, int temb_rows) {
   pdl_launch_dependents();
   pdl_wait();
   const int m = blockIdx.x, bp = blockIdx.y;
@@ -290,7 +355,9 @@ __global__ void mem_build_kernel(__half* __restrict__ mem16, const float* __rest
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = static_cast<size_t>(bp) * Mt + m;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
-    const float v = memproj[row * d + c] + temb_table[static_cast<size_t>(t) * d + c];
+    float te = temb_table[static_cast<size_t>(t) * d + c];
+    if (g != nullptr) te = te + g[static_cast<size_t>(bp % B) * d + c];
+    const float v = memproj[row * d + c] + te;
     const __half hi = __float2half_rn(v);
     mem16[row * 2 * d + c] = hi;
     mem16[row * 2 * d + d + c] = __float2half_rn(v - __half2float(hi));

@@ -21,11 +21,42 @@ def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def canonical_target(y, batch, joint_names):
+    """(target [B, n_ext, 3] fp32 tensor, validity uint8 [B, n_ext] numpy) from the reference's y keys: validity is 1
+    for each joint named in y['target_joint_names'][b], plus 'heading' when y['is_heading'][b] (model/mdm.py:410-416).
+    An unknown joint name raises ValueError (the reference's list.index)."""
+    tc = y["target_cond"]
+    if not torch.is_tensor(tc):
+        tc = torch.as_tensor(np.asarray(tc, dtype=np.float32))
+    n = len(joint_names)
+    if tuple(tc.shape) != (batch, n, 3):
+        raise ValueError("y['target_cond'] must be [batch, %d, 3] (got %s)" % (n, tuple(tc.shape)))
+    names, heading = y.get("target_joint_names"), y.get("is_heading")
+    if names is None or heading is None:
+        raise ValueError("y['target_cond'] needs y['target_joint_names'] and y['is_heading']")
+    if torch.is_tensor(heading):
+        heading = heading.detach().cpu().numpy()
+    heading = np.asarray(heading).reshape(-1)
+    if len(names) != batch or heading.shape[0] != batch:
+        raise ValueError("y['target_joint_names'] and y['is_heading'] need one entry per sample")
+    valid = np.zeros((batch, n), dtype=np.uint8)
+    for b in range(batch):
+        sample = [str(j) for j in np.asarray(names[b], dtype=object).reshape(-1)]
+        if heading[b]:
+            sample.append("heading")
+        for j in sample:
+            if j not in joint_names:
+                raise ValueError("unknown target joint %r (known: %s)" % (j, ", ".join(joint_names)))
+            valid[b, joint_names.index(j)] = 1
+    return tc, valid
+
+
 class Engine:
     """One engine per model instance (weights + workspace live on the current CUDA device)."""
 
     def __init__(self, *, arch, latent_dim, ff_size, num_layers, num_heads, njoints, nfeats, cond_mode, cond_dim,
-                 num_actions, mask_frames, pos_embed_max_len, temb_rows, context_len=0):
+                 num_actions, mask_frames, pos_embed_max_len, temb_rows, context_len=0, target_encoder=None,
+                 target_enc_layers=1, target_joint_names=()):
         self.lib = _lib.load()
         if not torch.cuda.is_available():
             raise RuntimeError("b200mdm needs a CUDA device (sm_90a); there is no CPU fallback")
@@ -33,7 +64,12 @@ class Engine:
         self.cfg = _lib.Config(arch=_lib.ARCH[arch], latent_dim=latent_dim, ff_size=ff_size, num_layers=num_layers,
                                num_heads=num_heads, njoints=njoints, nfeats=nfeats, cond_mode=cm, cond_dim=cond_dim,
                                num_actions=num_actions, mask_frames=int(bool(mask_frames)),
-                               pos_embed_max_len=pos_embed_max_len, temb_rows=temb_rows, context_len=context_len)
+                               pos_embed_max_len=pos_embed_max_len, temb_rows=temb_rows, context_len=context_len,
+                               target_encoder=_lib.TARGET[target_encoder] if target_encoder else 0,
+                               target_enc_layers=target_enc_layers if target_encoder else 0,
+                               target_joints=len(target_joint_names) if target_encoder else 0)
+        self.target_encoder = target_encoder
+        self.target_joint_names = list(target_joint_names)     # extended list: goal joints + ['traj', 'heading']
         self.dec = arch == "trans_dec"
         self.context_len = context_len
         h = ctypes.c_void_p()
@@ -61,6 +97,11 @@ class Engine:
         for name, t in sd.items():
             if not torch.is_tensor(t):
                 continue
+            if self.target_encoder == "multi" and name.startswith("embed_target_cond.target_loc_emb."):
+                # the C ABI names the multi encoder's per-joint MLP by the joint's index in the extended list
+                joint, _, rest = name[len("embed_target_cond.target_loc_emb."):].partition(".")
+                if joint in self.target_joint_names:
+                    name = "embed_target_cond.target_loc_emb.%d.%s" % (self.target_joint_names.index(joint), rest)
             t = t.detach().to(torch.float32).contiguous()
             shape = (ctypes.c_int64 * t.dim())(*t.shape)
             check(self.lib.b200mdm_load_weight(self.h, name.encode(), _ptr(t), shape, t.dim()))
@@ -81,9 +122,39 @@ class Engine:
     # ------------------------------------------------------------------ conditioning
     def set_cond(self, batch, nframes, y, guided, device):
         """Canonicalise model_kwargs['y'] (data_loaders/tensors.py:22-64 schema).  `guided` => CFG pair."""
-        text_embed = y.get("text_embed") if y is not None else None
         if self.dec:
-            return self._set_cond_dec(batch, nframes, y, guided, device)
+            self._set_cond_dec(batch, nframes, y, guided, device)
+        else:
+            self._set_cond_enc(batch, nframes, y, guided, device)
+        self._set_target(batch, y if y is not None else {}, device)
+
+    def _set_target(self, batch, y, device):
+        """y['target_cond'] [B, n_ext, 3], y['target_joint_names'] (per sample, a list or array of joint names),
+        y['is_heading'] [B] (model/mdm.py:197-199).  Both CFG halves carry the target (the guidance wrapper never sets
+        target_uncond, utils/sampler_util.py:27-34); y['target_uncond'] = True samples without it, as does a y without
+        'target_cond' (the b200mdm_set_cond* call above has cleared the previous target)."""
+        self._keep.pop("target", None)
+        if "target_cond" not in y or bool(y.get("target_uncond", False)):
+            return
+        if not self.target_encoder:
+            raise ValueError("y['target_cond'] was given, but the model has no target encoder (multi_target_cond=False)")
+        tc, valid = canonical_target(y, batch, self.target_joint_names)
+        tc = tc.to(device=device, dtype=torch.float32).contiguous()
+        check(self.lib.b200mdm_set_target(self.h, _ptr(tc), valid.ctypes.data_as(ctypes.c_void_p), _stream()))
+        self._keep["target"] = tc
+
+    def test_target(self, target, valid):
+        """The device target encoder alone (b200mdm_test_target): g [B, d] for target [B, n_ext, 3] (device fp32) and
+        valid uint8 [B, n_ext] (numpy)."""
+        target = target.to(torch.float32).contiguous()
+        valid = np.ascontiguousarray(valid, dtype=np.uint8)
+        out = torch.empty(target.shape[0], self.cfg.latent_dim, device=target.device, dtype=torch.float32)
+        check(self.lib.b200mdm_test_target(self.h, _ptr(target), valid.ctypes.data_as(ctypes.c_void_p), target.shape[0],
+                                           _ptr(out), _stream()))
+        return out
+
+    def _set_cond_enc(self, batch, nframes, y, guided, device):
+        text_embed = y.get("text_embed") if y is not None else None
         if isinstance(text_embed, tuple):
             raise NotImplementedError("BERT (tokens, mask) conditioning belongs to the trans_dec path")
         lengths = y.get("lengths") if y is not None else None

@@ -7,9 +7,10 @@ It uploads them once into the H100 engine (fp16 repack) and calls `b200mdm_denoi
 
 Implemented: arch='trans_enc' with cond_mode in {no_cond, text (CLIP features), action}; arch='trans_dec' with
 text_encoder_type='bert' (DiP: BERT token memory, prefix completion, model/mdm.py:203-206,255-270); hml_vec / rot6d /
-xyz data_rep.
-Not implemented (raise): arch 'gru', data_rep 'rot_vel', multi-target conditioning (CLoSD), emb_trans_dec,
-emb_policy != 'add', trans_dec with CLIP features.
+xyz data_rep; target-location conditioning (multi_target_cond, the single / multi / split encoders, model/mdm.py:64-73,
+197-199,399-480) with either arch.
+Not implemented (raise): arch 'gru', data_rep 'rot_vel', emb_trans_dec, emb_policy != 'add', trans_dec with CLIP
+features.
 """
 import numpy as np
 import torch
@@ -71,7 +72,33 @@ def _spec(arch, d, ff, layers, input_feats, cond_mode, cond_dim, num_actions):
     return s
 
 
+def _target_spec(encoder, joint_names, d, layers):
+    """(key, shape, init) of embed_target_cond (model/mdm.py:399-480; WeightedSum, utils/misc.py:5-16).  A Linear's
+    weight and bias are both U(+-1/sqrt(fan_in)): init ("fan", fan_in)."""
+    n = len(joint_names)
+
+    def mlp(prefix, d_in, width, n_hidden):
+        s = [(prefix + "0.weight", (width, d_in), ("fan", d_in)), (prefix + "0.bias", (width,), ("fan", d_in))]
+        for k in range(1, n_hidden + 1):
+            s += [(prefix + "%d.weight" % (2 * k), (width, width), ("fan", width)),
+                  (prefix + "%d.bias" % (2 * k), (width,), ("fan", width))]
+        return s
+    if encoder == "single":
+        return mlp("embed_target_cond.mlp.", 4 * n, d, layers)
+    if encoder == "split":
+        if d % n:
+            raise AssertionError("split target encoder: latent_dim %% %d joints != 0 (model/mdm.py:427)" % n)
+        return [e for i in range(n) for e in mlp("embed_target_cond.mini_mlps.%d." % i, 4, d // n, layers)]
+    if encoder == "multi":
+        return ([e for j in joint_names for e in mlp("embed_target_cond.target_loc_emb.%s." % j, 3, d, 1)] +
+                [("embed_target_cond.target_all_loc_emb.weights", (n,), "normal")])
+    raise ValueError("multi_encoder_type=%r: 'single', 'multi' or 'split' (model/mdm.py:67-73)" % (encoder,))
+
+
 def _init(shape, kind):
+    if isinstance(kind, tuple):                 # ("fan", fan_in): nn.Linear's default weight and bias init
+        bound = 1.0 / kind[1] ** 0.5
+        return torch.empty(shape).uniform_(-bound, bound)
     if kind == "zero":
         return torch.zeros(shape)
     if kind == "one":
@@ -107,6 +134,9 @@ class MDM(_Bag):
         self.is_prefix_comp = self.total_len > 0
         self.all_goal_joint_names = kargs.get("all_goal_joint_names", [])
         self.multi_target_cond = kargs.get("multi_target_cond", False)
+        self.multi_encoder_type = kargs.get("multi_encoder_type", "multi")
+        self.target_enc_layers = kargs.get("target_enc_layers", 1)
+        self.extended_goal_joint_names = list(self.all_goal_joint_names) + ["traj", "heading"]
         self.text_encoder_type = kargs.get("text_encoder_type", "clip")
         self.pos_embed_max_len = kargs.get("pos_embed_max_len", 5000)
         self.temb_rows = min(self.pos_embed_max_len, kargs.get("num_model_timesteps", 1000))
@@ -118,8 +148,8 @@ class MDM(_Bag):
                                       "an ablation and out of scope" % (arch,))
         if activation != "gelu":
             raise NotImplementedError("the fused FFN epilogue implements exact GELU only (model_util.py:63)")
-        if data_rep == "rot_vel" or self.multi_target_cond or self.emb_policy != "add":
-            raise NotImplementedError("rot_vel / multi-target / emb_policy='cat' variants are outside the hot path")
+        if data_rep == "rot_vel" or self.emb_policy != "add":
+            raise NotImplementedError("rot_vel / emb_policy='cat' variants are outside the hot path")
         if arch == "trans_enc":
             if self.is_prefix_comp:
                 raise NotImplementedError("prefix completion is implemented for arch='trans_dec' (DiP) only")
@@ -134,6 +164,10 @@ class MDM(_Bag):
         for key, shape, kind in _spec(arch, latent_dim, ff_size, num_layers, self.input_feats, self.cond_mode,
                                       self.clip_dim, num_actions):
             self.add(key, _init(shape, kind))
+        if self.multi_target_cond:
+            for key, shape, kind in _target_spec(self.multi_encoder_type, self.extended_goal_joint_names, latent_dim,
+                                                 self.target_enc_layers):
+                self.add(key, _init(shape, kind))
         self.add("sequence_pos_encoder.pe", positional_table(self.pos_embed_max_len, latent_dim).unsqueeze(1), buffer=True)
         self._engine = None
         self._engine_dirty = True
@@ -186,7 +220,10 @@ class MDM(_Bag):
                                       nfeats=self.nfeats, cond_mode=self.cond_mode, cond_dim=self.clip_dim,
                                       num_actions=max(1, self.num_actions), mask_frames=self.mask_frames,
                                       pos_embed_max_len=self.pos_embed_max_len, temb_rows=self.temb_rows,
-                                      context_len=self.context_len if self.arch == "trans_dec" else 0)
+                                      context_len=self.context_len if self.arch == "trans_dec" else 0,
+                                      target_encoder=self.multi_encoder_type if self.multi_target_cond else None,
+                                      target_enc_layers=self.target_enc_layers,
+                                      target_joint_names=self.extended_goal_joint_names)
             self._engine_device = dev
             self._engine_dirty = True
         if self._engine_dirty:

@@ -21,8 +21,15 @@ def _normal(rng, shape, std):
     return torch.from_numpy((rng.standard_normal(size=shape) * std).astype(np.float32))
 
 
+HML_TARGET_JOINTS = ["pelvis", "left_foot", "right_foot", "left_wrist", "right_wrist", "head", "traj", "heading"]
+
+
 def synthetic_state_dict(arch="trans_enc", latent_dim=512, ff_size=1024, num_layers=8, input_feats=263,
-                         cond_dim=512, cond_mode="text", num_actions=1, seed=0):
+                         cond_dim=512, cond_mode="text", num_actions=1, seed=0, target_encoder=None, target_enc_layers=1,
+                         target_joints=HML_TARGET_JOINTS):
+    """target_encoder ('single' / 'multi' / 'split', args.multi_encoder_type) adds the embed_target_cond.* tensors of
+    that encoder (model/mdm.py:399-480) for the extended joint list `target_joints`, drawn from a stream of their own:
+    every other tensor is the same as without them."""
     rng = np.random.default_rng(seed)
     d = latent_dim
     sd = {}
@@ -70,7 +77,48 @@ def synthetic_state_dict(arch="trans_enc", latent_dim=512, ff_size=1024, num_lay
     else:
         raise ValueError("unsupported arch %r" % (arch,))
     linear("output_process.poseFinal", input_feats, d)
+    if target_encoder is not None:
+        rng = np.random.default_rng([seed, 0x7a5])
+        n = len(target_joints)
+
+        def mlp(prefix, d_in, width, n_hidden):
+            linear(prefix + ".0", width, d_in)
+            for k in range(1, n_hidden + 1):
+                linear(prefix + ".%d" % (2 * k), width, width)
+        if target_encoder == "single":
+            mlp("embed_target_cond.mlp", 4 * n, d, target_enc_layers)
+        elif target_encoder == "split":
+            for i in range(n):
+                mlp("embed_target_cond.mini_mlps.%d" % i, 4, d // n, target_enc_layers)
+        elif target_encoder == "multi":
+            for j in target_joints:
+                mlp("embed_target_cond.target_loc_emb." + j, 3, d, 1)
+            # WeightedSum weights (randn init): kept away from a zero sum so that w / w.sum() stays moderate
+            sd["embed_target_cond.target_all_loc_emb.weights"] = torch.from_numpy(
+                rng.uniform(0.25, 1.0, size=n).astype(np.float32) * np.where(np.arange(n) % 3 == 2, -0.5, 1.0).astype(np.float32))
+        else:
+            raise ValueError("unsupported target encoder %r" % (target_encoder,))
     return sd
+
+
+def synthetic_target_inputs(batch, joint_names=HML_TARGET_JOINTS, seed=5):
+    """Deterministic target-location conditioning in the reference's y schema (model/mdm.py:197-199):
+    target_cond [B, n_ext, 3] fp32 (every joint has values, valid or not), target_joint_names (per sample, a numpy array
+    of names: the layout CLoSD passes), is_heading [B] bool.  The joint sets cycle through mixed choices, some with
+    heading; the last sample (of a batch of 3 or more) has no joint and no heading."""
+    rng = np.random.default_rng(seed)
+    target = torch.from_numpy(rng.standard_normal(size=(batch, len(joint_names), 3)).astype(np.float32))
+    goal = [j for j in joint_names if j not in ("heading",)]
+    choices = [["pelvis", "head"], ["traj"], ["left_wrist", "right_wrist", "left_foot"], goal, ["right_foot"]]
+    names, heading = [], []
+    for b in range(batch):
+        if batch >= 3 and b == batch - 1:
+            names.append(np.array([], dtype="<U16"))
+            heading.append(False)
+            continue
+        names.append(np.array([j for j in choices[b % len(choices)] if j in joint_names]))
+        heading.append(b % 2 == 0)
+    return dict(target_cond=target, target_joint_names=names, is_heading=torch.tensor(heading))
 
 
 def synthetic_inputs(batch, njoints=263, nfeats=1, nframes=196, steps=50, cond_dim=512, seed=10,

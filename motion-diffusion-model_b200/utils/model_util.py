@@ -39,7 +39,8 @@ def get_model_args(args, data):
         "text_encoder_type": args.text_encoder_type, "pos_embed_max_len": args.pos_embed_max_len,
         "mask_frames": args.mask_frames, "pred_len": args.pred_len, "context_len": args.context_len,
         "emb_policy": extra.get("emb_policy", "add"), "all_goal_joint_names": goal_names,
-        "multi_target_cond": extra.get("multi_target_cond", False),
+        # apply_rules (reference utils/parser_util.py:51-53): a target-location loss implies the target encoder
+        "multi_target_cond": extra.get("multi_target_cond", False) or extra.get("lambda_target_loc", 0.0) > 0.0,
         "multi_encoder_type": extra.get("multi_encoder_type", "multi"),
         "target_enc_layers": extra.get("target_enc_layers", 1),
         # engine-only knob: how many model timesteps get a pre-computed timestep embedding
