@@ -48,16 +48,16 @@ def split16(x):
 
 
 def acc_bound(a, w):
-    """Bound on the fp32 accumulation error of a @ w.T on the tensor cores, from the exact operands (fp64) a [M, K] and
-    w [N, K] in the kernel's k order.  The fp16 x fp16 products are exact in fp32; the accumulator takes them ACC_CHUNK
-    at a time and each update is off by at most 2^-23 (one fp32 ulp: truncation allowed as well as round-to-nearest) of
-    |previous partial sum| + sum |products of the chunk|.  The partial sums are computed in fp64."""
-    s = torch.zeros(a.shape[0], w.shape[0], dtype=F64, device=a.device)
+    """Bound on the fp32 accumulation error of a @ w.T on the tensor cores, from the exact operands (fp64) a [..., M, K]
+    and w [..., N, K] in the kernel's k order.  The fp16 x fp16 products are exact in fp32; the accumulator takes them
+    ACC_CHUNK at a time and each update is off by at most 2^-23 (one fp32 ulp: truncation allowed as well as
+    round-to-nearest) of |previous partial sum| + sum |products of the chunk|.  The partial sums are computed in fp64."""
+    s = torch.zeros(*a.shape[:-1], w.shape[-2], dtype=F64, device=a.device)
     tot = torch.zeros_like(s)
-    for k0 in range(0, a.shape[1], ACC_CHUNK):
-        ab, wb = a[:, k0:k0 + ACC_CHUNK], w[:, k0:k0 + ACC_CHUNK]
-        tot += s.abs() + ab.abs() @ wb.abs().t()
-        s += ab @ wb.t()
+    for k0 in range(0, a.shape[-1], ACC_CHUNK):
+        ab, wb = a[..., k0:k0 + ACC_CHUNK], w[..., k0:k0 + ACC_CHUNK].transpose(-1, -2)
+        tot += s.abs() + ab.abs() @ wb.abs()
+        s += ab @ wb
     return tot * 2.0 ** -23
 
 
@@ -94,11 +94,12 @@ def check(name, err, bound, mutants, where=None):
 
 
 def grid_operands(M, N, K, g):
-    """fp16 A [M, K] = i/8 (|i| <= 16), W [N, K] = j/256 (|j| <= 8): every product is a multiple of 2^-11 below 2^-4
-    and every partial sum (K <= 1024) a multiple of 2^-11 below 2^6 -- 17 bits, exact in fp32 in any order.  The
-    accumulation is then exact and the bounds below are the epilogue's alone."""
-    assert K <= 1024
-    a = (torch.randint(-16, 17, (M, K), device="cuda", generator=g).float() / 8).half()
+    """fp16 A [M, K] = i/8 (|i| <= 16, narrowed to 16384 / K above K = 1024), W [N, K] = j/256 (|j| <= 8): every product
+    is a multiple of 2^-11 and every partial sum a multiple of 2^-11 below 2^6 -- 17 bits, exact in fp32 in any order.
+    The accumulation is then exact and the bounds below are the epilogue's alone."""
+    assert K <= 2048
+    imax = min(16, 16384 // K)
+    a = (torch.randint(-imax, imax + 1, (M, K), device="cuda", generator=g).float() / 8).half()
     w = (torch.randint(-8, 9, (N, K), device="cuda", generator=g).float() / 256).half()
     return a, w
 
