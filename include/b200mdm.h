@@ -218,7 +218,7 @@ int b200mdm_test_gemm_f16(const void* a16_dev, const void* w16_dev, const float*
  *   epi 0: EpiBiasF16Wide<GELU> (the DiP FFN up-projection): out16 fp16 [M, 2N], columns [0, N) = hi, [N, 2N) = lo with
  *          hi + lo = gelu(A W^T + bias) to ~22 bits.  N % 64 == 0, N <= 2048.
  *   epi 1: EpiBiasF16Global (the DiP K/V projection of all layers): out16 fp16 [M, N] = fp16(A W^T + bias), bias read
- *          from global memory per chunk, so N is not limited by the staged-vector size.  N % 32 == 0. */
+ *          from global memory per tile, so N is not limited by the staged-vector size.  N % 32 == 0. */
 int b200mdm_test_gemm_epi(const void* a16_dev, const void* w16_dev, const float* bias_dev, void* out16_dev, int32_t M,
                           int32_t N, int32_t K, int32_t epi, void* stream);
 /* The embedding launches of the step (InputProcess + positional encoding, model/mdm.py:238,252,343-349) through scratch

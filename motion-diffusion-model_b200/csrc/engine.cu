@@ -20,6 +20,7 @@
 #include "epilogues.cuh"
 #include "gemm.cuh"
 #include "gemm_ln.cuh"
+#include "gemm_pingpong.cuh"
 #include "postprocess.cuh"
 #include "kernels.cuh"
 
@@ -245,6 +246,11 @@ static int set_gemm_attr() {
                                 GemmSmem<BN, Epi, RES>::TOTAL));
   return B200MDM_OK;
 }
+template <class Epi>
+static int set_pingpong_attr() {
+  CUDA_TRY(cudaFuncSetAttribute(gemm_f16_pingpong<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, PP_SMEM_BYTES));
+  return B200MDM_OK;
+}
 template <int KEYS>
 static int set_attention_attr() {
   CUDA_TRY(cudaFuncSetAttribute(attention_tc_kernel<KEYS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -259,14 +265,14 @@ static int init_kernel_attrs() {
   int dev = 0;
   CUDA_TRY(cudaGetDevice(&dev));
   if (dev < 64 && ((done_mask >> dev) & 1ull)) return B200MDM_OK;
-  TRY((set_gemm_attr<128, EpiBiasF16<false>>()));
-  TRY((set_gemm_attr<128, EpiBiasF16<true>>()));
+  TRY((set_pingpong_attr<EpiBiasF16<false>>()));
+  TRY((set_pingpong_attr<EpiBiasF16<true>>()));
+  TRY((set_pingpong_attr<EpiBiasF16Wide<true>>()));
+  TRY((set_pingpong_attr<EpiBiasF16Global>()));
   TRY((set_gemm_attr<256, EpiBiasF16<false>>()));
   TRY((set_gemm_attr<256, EpiBiasF16<true>>()));
   TRY((set_gemm_attr<64, EpiBiasF16<false>, true>()));
   TRY((set_gemm_attr<64, EpiBiasF16<true>, true>()));
-  TRY((set_gemm_attr<128, EpiBiasF16Wide<true>>()));
-  TRY((set_gemm_attr<128, EpiBiasF16Global>()));
   CUDA_TRY(cudaFuncSetAttribute(gemm_resid_ln_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmLnSmem::TOTAL));
   TRY((set_gemm_attr<128, EpiEmbed>()));
   TRY((set_gemm_attr<96, EpiOutStep>()));
@@ -336,12 +342,24 @@ static int launch_gemm_resident(const CUtensorMap& a, const CUtensorMap& b, cons
   CUDA_TRY(launch_k(gemm_f16_wgmma<BN, Epi, true>, dim3(grid), dim3(GEMM_THREADS), GemmSmem<BN, Epi, true>::TOTAL, s, a, b, c, M, N, K, p));
   return B200MDM_OK;
 }
-// out16 = fp16(act(A W^T + bias)), 128 x 128 tiles (b: W map with box 128 rows)
+// projection GEMMs of the step (gemm_pingpong.cuh): 128 x 128 tiles, the two consumer warpgroups take turns (b: W map
+// with box 128 rows; c: output map with box 32 rows x 64 columns)
+template <class Epi>
+static int launch_gemm_pp(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& c, int M, int N, int K,
+                          const typename Epi::Params& p, cudaStream_t s, int num_sms) {
+  if (!epi_unstaged<PP_BLOCK_N, Epi>::value && N * 4 > GEMM_BIAS_BYTES)
+    return fail(B200MDM_ENOTIMPL, "GEMM epilogue vectors are staged for N <= %d", GEMM_BIAS_BYTES / 4);
+  const int tiles = ((M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M) * ((N + PP_BLOCK_N - 1) / PP_BLOCK_N);
+  const int grid = tiles < num_sms ? tiles : num_sms;
+  CUDA_TRY(launch_k(gemm_f16_pingpong<Epi>, dim3(grid), dim3(GEMM_THREADS), PP_SMEM_BYTES, s, a, b, c, M, N, K, p));
+  return B200MDM_OK;
+}
+// out16 = fp16(act(A W^T + bias))
 template <bool GELU>
 static int launch_gemm_bias(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& c, int M, int N, int K,
                             const float* bias, cudaStream_t s, int num_sms) {
   typename EpiBiasF16<GELU>::Params p{bias};
-  return launch_gemm<128, EpiBiasF16<GELU>>(a, b, c, M, N, K, p, s, num_sms);
+  return launch_gemm_pp<EpiBiasF16<GELU>>(a, b, c, M, N, K, p, s, num_sms);
 }
 
 // h <- LayerNorm(h + A W^T + bias), 2-CTA cluster splitting the 512 columns, LayerNorm statistics exchanged through
@@ -1106,7 +1124,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
                       a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, target_g, B, e->Mt, d, e->cfg.temb_rows));
     // ... and its key / value projections for every layer in one GEMM (N = L * 2d; hi half of the memory, K = d)
     EpiBiasF16Global::Params p{e->bkv_all};
-    TRY((launch_gemm<128, EpiBiasF16Global>(e->m_mem, e->m_wkv_all, e->m_kvc_st, e->Bp * e->Mt, e->L * 2 * d, d, p, s, e->num_sms)));
+    TRY((launch_gemm_pp<EpiBiasF16Global>(e->m_mem, e->m_wkv_all, e->m_kvc_st, e->Bp * e->Mt, e->L * 2 * d, d, p, s, e->num_sms)));
     ++nk;
   }
   ++nk;
@@ -1146,7 +1164,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     }
     if (wide) {
       EpiBiasF16Wide<true>::Params p{w.b1, ff};
-      TRY((launch_gemm<128, EpiBiasF16Wide<true>>(e->m_h16, w.m_w1, e->m_ffn_st, e->M, ff, kw * d, p, s, e->num_sms)));
+      TRY((launch_gemm_pp<EpiBiasF16Wide<true>>(e->m_h16, w.m_w1, e->m_ffn_st, e->M, ff, kw * d, p, s, e->num_sms)));
     } else if (!B200_SKIP(4)) {
       TRY((launch_gemm_bias<true>(e->m_h16, w.m_w1, e->m_ffn_st, e->M, ff, d, w.b1, s, e->num_sms)));
     }
@@ -1379,6 +1397,9 @@ static int test_gemm_bn(const void* a16, const void* w16, const float* bias, voi
   if constexpr (RES)
     return act ? launch_gemm_resident<BN, EpiBiasF16<true>>(ma, mb, mc, M, N, K, pg, s, sms)
                : launch_gemm_resident<BN, EpiBiasF16<false>>(ma, mb, mc, M, N, K, pn, s, sms);
+  else if constexpr (BN == PP_BLOCK_N)   // the step's projection kernel
+    return act ? launch_gemm_pp<EpiBiasF16<true>>(ma, mb, mc, M, N, K, pg, s, sms)
+               : launch_gemm_pp<EpiBiasF16<false>>(ma, mb, mc, M, N, K, pn, s, sms);
   else
     return act ? launch_gemm<BN, EpiBiasF16<true>>(ma, mb, mc, M, N, K, pg, s, sms)
                : launch_gemm<BN, EpiBiasF16<false>>(ma, mb, mc, M, N, K, pn, s, sms);
@@ -1439,13 +1460,13 @@ extern "C" int b200mdm_test_gemm_epi(const void* a16_dev, const void* w16_dev, c
     if (N % 64) return fail(B200MDM_EINVAL, "EpiBiasF16Wide needs N %% 64 == 0");
     TRY(make_map_t(&mc, out16_dev, 2, M, 2 * static_cast<uint64_t>(N), 2 * static_cast<uint64_t>(N), 32));
     EpiBiasF16Wide<true>::Params p{bias_dev, N};
-    return launch_gemm<128, EpiBiasF16Wide<true>>(ma, mb, mc, M, N, K, p, s, sms);
+    return launch_gemm_pp<EpiBiasF16Wide<true>>(ma, mb, mc, M, N, K, p, s, sms);
   }
   if (epi == 1) {
     if (N % 32) return fail(B200MDM_EINVAL, "EpiBiasF16Global needs N %% 32 == 0");
     TRY(make_map_t(&mc, out16_dev, 2, M, N, N, 32));
     EpiBiasF16Global::Params p{bias_dev};
-    return launch_gemm<128, EpiBiasF16Global>(ma, mb, mc, M, N, K, p, s, sms);
+    return launch_gemm_pp<EpiBiasF16Global>(ma, mb, mc, M, N, K, p, s, sms);
   }
   return fail(B200MDM_EINVAL, "epi must be 0 (EpiBiasF16Wide<GELU>) or 1 (EpiBiasF16Global)");
 }

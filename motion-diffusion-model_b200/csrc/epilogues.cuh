@@ -1,4 +1,6 @@
-// Fused GEMM epilogues (see gemm.cuh for the calling protocol).  Thread = accumulator row.
+// Fused GEMM epilogues (see gemm.cuh for the calling protocol).  Thread = accumulator row.  The projection epilogues
+// (EpiBiasF16, EpiBiasF16Global, EpiBiasF16Wide) also provide the fragment interface of gemm_pingpong.cuh (pp_*: one
+// column pair of the wgmma accumulator fragment at a time, same arithmetic).
 //
 // Row-major outputs are written as 128-byte-per-row slabs (32 rows of the warp x 64 fp16 or 32 fp32 columns = 4 KB)
 // staged in warp-private shared memory in the TMA 128-byte swizzle and shipped with cp.async.bulk.tensor stores;
@@ -153,15 +155,37 @@ struct EpiBiasF16 {
     if (ctx.lane == 0) bulk_wait_group<0>();
     __syncwarp();
   }
+
+  // ---- fragment interface (gemm_pingpong.cuh): one column pair of one accumulator row at a time
+  static constexpr int PP_ROUND_COLS = 128;   // a round fills two 64-column slabs (16 KB each) of the warpgroup's 128 rows
+  // the bias of the tile's 128 columns (col_t = first column): here a view of the CTA's staged vector
+  static __device__ __forceinline__ const float* pp_tile_bias(const Params&, const float* bias_all, float*, int col_t, int, int) {
+    return bias_all + col_t;
+  }
+  static __device__ __forceinline__ void pp_pair(const Params&, float2 b, float a0, float a1, uint8_t* dst) {
+    float x0 = a0 + b.x, x1 = a1 + b.y;
+    if (GELU) {
+      x0 = gelu_erf(x0); x1 = gelu_erf(x1);
+    }
+    *reinterpret_cast<uint32_t*>(dst) = pack_half2(x0, x1);
+  }
+  static __device__ __forceinline__ void pp_store(const CUtensorMap* map_c, const Params&, const uint8_t* box, int col, int row) {
+    tma_store_2d(map_c, box, col, row);
+  }
 };
 
 // EpiBiasF16 for a GEMM wider than the staged-vector limit (the cross-attention K/V projection of all decoder layers
-// at once, N = L * 2d = 8192): the bias is read from global memory per chunk (one broadcast float4 per 4 columns).
+// at once, N = L * 2d = 8192): the bias is read from global memory, one float2 per column pair.  Fragment interface
+// only (gemm_f16_pingpong).
 struct EpiBiasF16Global : EpiBiasF16<false> {
   static constexpr bool UNSTAGED = true;
   static __device__ __forceinline__ void preload(const Params&, float*, int, int, int) {}
-  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0, int) {
-    chunk_bias(ctx, p.bias + col0, raw, row0, col0);
+  // thread `tid` (0..127) of the warpgroup copies one column of the tile's bias into the warpgroup's 128-float scratch
+  // (visible to the warpgroup after its next named barrier)
+  static __device__ __forceinline__ const float* pp_tile_bias(const Params& p, const float*, float* scratch, int col_t, int N,
+                                                              int tid) {
+    scratch[tid] = col_t + tid < N ? __ldg(p.bias + col_t + tid) : 0.f;
+    return scratch;
   }
 };
 
@@ -169,9 +193,9 @@ struct EpiBiasF16Global : EpiBiasF16<false> {
 // EpiBiasF16 with the result kept as a [hi | lo] fp16 pair: out16[row, col] = hi, out16[row, lo_col + col] = lo with
 // hi + lo = act(acc + bias) to ~22 bits (trans_dec engine, where guidance 7.5 amplifies activation rounding; the
 // consumer GEMM runs over K = 2N against [W | W]).  map_c: fp16 [M, 2N], box {64 cols, 32 rows}, SWIZZLE_128B.
+// Fragment interface only (gemm_f16_pingpong).
 template <bool GELU>
 struct EpiBiasF16Wide {
-  static constexpr int SMEM_PER_WARP = 2 * 4096;   // one hi slab + one lo slab
   struct Params {
     const float* bias;
     int lo_col;
@@ -179,51 +203,24 @@ struct EpiBiasF16Wide {
   static __device__ __forceinline__ void preload(const Params& p, float* dst, int N, int tid, int nthreads) {
     for (int i = tid; i < N; i += nthreads) dst[i] = p.bias[i];
   }
-  static __device__ __forceinline__ void tile_begin(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0,
-                                               int) {
-    const int half = (col0 >> 5) & 1;
-    uint8_t* slab_hi = ctx.smem;
-    uint8_t* slab_lo = ctx.smem + 4096;
-    if (half == 0) {
-      if (ctx.lane == 0) bulk_wait_group_read<0>();
-      __syncwarp();
-    }
-    const float* bs = ctx.bias_all + col0;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      uint32_t hi[4], lo[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        float x0 = __uint_as_float(raw[8 * j + 2 * i]) + bs[8 * j + 2 * i];
-        float x1 = __uint_as_float(raw[8 * j + 2 * i + 1]) + bs[8 * j + 2 * i + 1];
-        if (GELU) {
-          x0 = gelu_erf(x0); x1 = gelu_erf(x1);
-        }
-        const __half2 h = __floats2half2_rn(x0, x1);
-        const float2 f = __half22float2(h);
-        const __half2 l = __floats2half2_rn(x0 - f.x, x1 - f.y);
-        hi[i] = *reinterpret_cast<const uint32_t*>(&h);
-        lo[i] = *reinterpret_cast<const uint32_t*>(&l);
-      }
-      *reinterpret_cast<uint4*>(slab_hi + slab_off(ctx.lane, half * 4 + j)) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-      *reinterpret_cast<uint4*>(slab_lo + slab_off(ctx.lane, half * 4 + j)) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-    }
-    if (half == 1 || col0 + 32 >= ctx.N) {
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (ctx.lane == 0) {
-        tma_store_2d(ctx.map_c, slab_hi, col0 - 32 * half, row0);
-        tma_store_2d(ctx.map_c, slab_lo, p.lo_col + col0 - 32 * half, row0);
-        bulk_commit_group();
-      }
-      ctx.seq++;
-    }
+  static constexpr int PP_ROUND_COLS = 64;    // a round fills one 64-column hi slab (16 KB) and its lo slab, 16 KB further
+  static __device__ __forceinline__ const float* pp_tile_bias(const Params&, const float* bias_all, float*, int col_t, int, int) {
+    return bias_all + col_t;
   }
-  static __device__ __forceinline__ void tile_end(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void finish(EpiCtx& ctx) {
-    if (ctx.lane == 0) bulk_wait_group<0>();
-    __syncwarp();
+  static __device__ __forceinline__ void pp_pair(const Params&, float2 b, float a0, float a1, uint8_t* dst) {
+    float x0 = a0 + b.x, x1 = a1 + b.y;
+    if (GELU) {
+      x0 = gelu_erf(x0); x1 = gelu_erf(x1);
+    }
+    const __half2 h = __floats2half2_rn(x0, x1);
+    const float2 f = __half22float2(h);
+    const __half2 l = __floats2half2_rn(x0 - f.x, x1 - f.y);
+    *reinterpret_cast<__half2*>(dst) = h;
+    *reinterpret_cast<__half2*>(dst + 16384) = l;
+  }
+  static __device__ __forceinline__ void pp_store(const CUtensorMap* map_c, const Params& p, const uint8_t* box, int col, int row) {
+    tma_store_2d(map_c, box, col, row);
+    tma_store_2d(map_c, box + 16384, p.lo_col + col, row);
   }
 };
 

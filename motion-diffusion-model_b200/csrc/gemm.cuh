@@ -11,9 +11,11 @@
 // 128-byte-per-row output slab in warp-private shared memory (128B swizzle) and ships it with a TMA store.
 //
 // Tiles are statically strided over the persistent grid (tile = blockIdx.x + k * gridDim.x, N fastest so concurrently
-// running CTAs share the same A rows in L2).  The step runs BLOCK_N = 128 (96 for the output projection); BLOCK_N = 256
-// and the W-resident variant are measured alternatives reached only through b200mdm_test_gemm_f16 (both slower at the
-// step's shapes, DESIGN.md section 4).  W-resident variant (RESIDENT, K <= 512): CTA c owns column block
+// running CTAs share the same A rows in L2).  The step runs this kernel for the embedding (BLOCK_N = 128) and the output
+// projection (96), once per step each; the per-layer projections run on gemm_f16_pingpong (gemm_pingpong.cuh), which
+// takes its epilogue from the accumulator fragment.  BLOCK_N = 256 and the W-resident variant are measured alternatives
+// reached only through b200mdm_test_gemm_f16 (both slower at the step's shapes, DESIGN.md section 4).  W-resident
+// variant (RESIDENT, K <= 512): CTA c owns column block
 // c % tiles_n for the whole launch and, among the CTAs of that block, every m_step-th row block starting at c / tiles_n;
 // it loads its [BLOCK_N x K] W tile into shared memory once (k-block by k-block, so the first tile still pipelines) and
 // streams only A.  A is [M,K] row-major (K contiguous), W is the torch nn.Linear layout

@@ -107,6 +107,10 @@ __device__ __forceinline__ void bulk_wait_group() {
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// signal a named barrier without waiting on it (the other nthreads - 32k threads wait with named_bar_sync)
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // ---- programmatic dependent launch (PDL): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may
 // start while its stream predecessor is still running.  pdl_launch_dependents() lets the successor's CTAs be scheduled
