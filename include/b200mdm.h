@@ -177,6 +177,26 @@ int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_t first_ind
                               float* x_out_dev, const float* noise_tape_dev, int64_t noise_step_stride, int32_t flags,
                               int32_t use_graph, void* stream);
 
+/* plms_sample_loop (gaussian_diffusion.py:1076-1187) without returning to the host: schedule indices first_index,
+ * first_index-1, ... (n_run of them) on the engine's working buffer, order 1..4.  x_in_dev != NULL starts a fresh loop
+ * from it, whose first step is the pseudo improved-Euler step (two forwards, the second at index i - 1, wrapping to
+ * n_steps - 1 at i = 0); every later step is one Adams-Bashforth forward (one CUDA graph, replayed, when use_graph != 0).
+ * A fresh loop of order 1 -> B200MDM_EINVAL (the reference fails on its missing history).  x_in_dev NULL continues
+ * the PLMS loop the previous call of the same order left in the engine; x_out_dev NULL leaves the result there.
+ * flags: B200MDM_FLAG_CLIP_DENOISED or 0.  No noise is drawn.  The eps history (3 x [B, JF, T] fp32), a scratch sample
+ * and a pred_xstart buffer are allocated in the workspace on first use. */
+int b200mdm_plms_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index, int32_t n_run, const float* x_in_dev,
+                            float* x_out_dev, int32_t flags, int32_t use_graph, void* stream);
+
+/* One plms_sample (gaussian_diffusion.py:992-1074) at schedule index `index`: old_eps_dev is a host array of n_old
+ * device pointers to [B, JF, T] fp32 eps, oldest first (old_out['old_eps']), and may be empty (n_old == 0: one
+ * Adams-Bashforth forward at cur_order 1, as the reference does for an empty history).  old_eps_dev NULL (with
+ * n_old == 0) is old_out = None: the improved-Euler step, order 2..4.  x_out_dev (may alias x_t_dev) receives the sample, pred_xstart_dev (may be NULL) the first
+ * evaluation's x0, eps_out_dev (may be NULL) this step's eps -- the entry the caller appends to its history. */
+int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order, const float* x_t_dev, const float* const* old_eps_dev,
+                      int32_t n_old, int32_t flags, float* x_out_dev, float* pred_xstart_dev, float* eps_out_dev,
+                      void* stream);
+
 /* The engine's own noise stream (no reference counterpart: the reference draws from torch's global generator).
  * Philox4x32-10 keyed by `seed`, counter = (element/4, schedule index of the consuming step, global sample index);
  * Box-Muller on the 4 output words (exact recipe: csrc/kernels.cuh, restated in oracle/philox_oracle.py).  A sample's

@@ -25,7 +25,7 @@ SYMBOLS = [
     "b200mdm_sample_loop_range", "b200mdm_set_noise_stream", "b200mdm_philox_normal",
     "b200mdm_recover_from_ric", "b200mdm_test_gemm_f16", "b200mdm_test_attention", "b200mdm_test_cross_attention", "b200mdm_test_qkv_attention",
     "b200mdm_test_gemm_resid_ln", "b200mdm_test_gemm_epi", "b200mdm_test_embed", "b200mdm_test_out_step",
-    "b200mdm_set_target", "b200mdm_test_target",
+    "b200mdm_set_target", "b200mdm_test_target", "b200mdm_plms_loop_range", "b200mdm_plms_step",
 ]
 
 
@@ -90,7 +90,9 @@ def load():
                        ("b200mdm_test_out_step", [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp,
                                                   i32, i32, i32, i32, i32, i32, vp]),
                        ("b200mdm_set_target", [vp, vp, vp, vp]),
-                       ("b200mdm_test_target", [vp, vp, vp, i32, vp, vp])):
+                       ("b200mdm_test_target", [vp, vp, vp, i32, vp, vp]),
+                       ("b200mdm_plms_loop_range", [vp, i32, i32, i32, vp, vp, i32, i32, vp]),
+                       ("b200mdm_plms_step", [vp, i32, i32, vp, ctypes.POINTER(vp), i32, i32, vp, vp, vp, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

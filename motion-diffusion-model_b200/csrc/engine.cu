@@ -138,11 +138,12 @@ struct LayerW {
 
 struct GraphKey {
   int mode = -1, B = 0, T = 0, flags = 0;
+  int order = 0;                    // PLMS (Adams-Bashforth step): the order; 0 for DDPM / DDIM
   const void *pred = nullptr, *imask = nullptr, *imotion = nullptr;
   const void* target_g = nullptr;   // the workspace's target embedding, or nullptr when the loop has no target
   bool operator==(const GraphKey& o) const {
-    return mode == o.mode && B == o.B && T == o.T && flags == o.flags && pred == o.pred && imask == o.imask &&
-           imotion == o.imotion && target_g == o.target_g;
+    return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
+           imask == o.imask && imotion == o.imotion && target_g == o.target_g;
   }
 };
 
@@ -173,6 +174,10 @@ struct Workspace {
   // CFG halves; target_set is cleared by every b200mdm_set_cond* call
   float *tgt_valid = nullptr, *tgt_g = nullptr;
   bool target_set = false;
+  // PLMS, allocated on first use: eps history ring [PLMS_RING, B, JF, T], the improved-Euler step's mean1 (the input of
+  // its second forward) and its first x0.  plms_done = evaluations of the PLMS loop in flight (-1: none to continue).
+  float *plms_ring = nullptr, *plms_mid = nullptr, *plms_pred = nullptr;
+  int plms_done = -1, plms_order = 0;
   // captured step graph of this workspace
   cudaGraphExec_t graph_exec = nullptr;
   GraphKey graph_key;
@@ -276,6 +281,7 @@ static int init_kernel_attrs() {
   CUDA_TRY(cudaFuncSetAttribute(gemm_resid_ln_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmLnSmem::TOTAL));
   TRY((set_gemm_attr<128, EpiEmbed>()));
   TRY((set_gemm_attr<96, EpiOutStep>()));
+  TRY((set_gemm_attr<96, EpiOutPlms>()));
   TRY((set_attention_attr<64>()));
   TRY((set_attention_attr<208>()));
   TRY((set_attention_attr<256>()));
@@ -484,6 +490,7 @@ static void free_workspace(Workspace* w) {
   dfree(w->kvlen); dfree(w->tvec); dfree(w->action);
   dfree(w->encperm); dfree(w->memtok); dfree(w->memproj); dfree(w->mem16); dfree(w->qc16); dfree(w->kvc16); dfree(w->memmask);
   dfree(w->tgt_valid); dfree(w->tgt_g);
+  dfree(w->plms_ring); dfree(w->plms_mid); dfree(w->plms_pred);
   *w = Workspace();
 }
 // every workspace (the one in use and the parked ones): after a weight reload or a schedule-table move their graphs
@@ -1087,6 +1094,9 @@ struct StepArgs {
   float* pred = nullptr;
   bool explicit_t = false;        // use e->tvec instead of timestep_map[state.cur]
   bool philox = false;            // eps of this step is generated into e->eps_buf by the first kernel of the step
+  int back = 0;                   // evaluate schedule index cur - back (PLMS improved Euler, second forward: 1)
+  const float* x_step = nullptr;  // PLMS mode 5: x_t of the step
+  int order = 0;                  // PLMS mode 3
 };
 
 // Enqueue one denoiser forward (+ fused sampler step) on stream s.  Returns the number of kernels launched.
@@ -1117,11 +1127,11 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
   const float* target_g = e->target_set ? e->tgt_g : nullptr;   // timestep embedding + target (model/mdm.py:197-199)
   if (!e->dec) {
     CUDA_TRY(launch_k(tok0_rows_kernel, dim3(e->Bp), dim3(128), 0, s, e->hres, e->condproj, e->temb_table, e->pe,
-                      a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, target_g, B, S, d, e->cfg.temb_rows));
+                      a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, target_g, B, S, d, e->cfg.temb_rows, a.back));
   } else {
     // cross-attention memory of this step: text tokens + timestep embedding (model/mdm.py:218-220)
     CUDA_TRY(launch_k(mem_build_kernel, dim3(e->Mt, e->Bp), dim3(128), 0, s, e->mem16, e->memproj, e->temb_table,
-                      a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, target_g, B, e->Mt, d, e->cfg.temb_rows));
+                      a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, target_g, B, e->Mt, d, e->cfg.temb_rows, a.back));
     // ... and its key / value projections for every layer in one GEMM (N = L * 2d; hi half of the memory, K = d)
     EpiBiasF16Global::Params p{e->bkv_all};
     TRY((launch_gemm_pp<EpiBiasF16Global>(e->m_mem, e->m_wkv_all, e->m_kvc_st, e->Bp * e->Mt, e->L * 2 * d, d, p, s, e->num_sms)));
@@ -1176,7 +1186,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
                     e->halves));
   ++nk;
   {
-    EpiOutStep::Params p;
+    EpiOutPlms::Params p;   // EpiOutStep's parameters + the PLMS fields
     p.bias = e->b_out;
     p.x_t = a.x_in;
     p.noise = a.noise;
@@ -1190,7 +1200,16 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     p.B = B; p.S = T; p.T = T; p.J = JF; p.mode = a.mode;      // g16 rows are frames: row = b*T + t
     p.s_off = 0;
     p.clip_denoised = a.clip;
-    TRY((launch_gemm<96, EpiOutStep>(e->m_g16, e->m_wout, e->m_g16, B * T, e->N_out_pad, 3 * d, p, s, e->num_sms)));
+    if (a.mode <= B200MDM_MODE_DDIM) {
+      const EpiOutStep::Params& ps = p;
+      TRY((launch_gemm<96, EpiOutStep>(e->m_g16, e->m_wout, e->m_g16, B * T, e->N_out_pad, 3 * d, ps, s, e->num_sms)));
+    } else {
+      p.eps_ring = e->plms_ring;
+      p.x_step = a.x_step;
+      p.order = a.order;
+      p.back = a.back;
+      TRY((launch_gemm<96, EpiOutPlms>(e->m_g16, e->m_wout, e->m_g16, B * T, e->N_out_pad, 3 * d, p, s, e->num_sms)));
+    }
     ++nk;
   }
   *n_kernels = nk;
@@ -1235,7 +1254,7 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
   if (index < 0 || index >= e->n_steps) return fail(B200MDM_EINVAL, "schedule index out of range");
   if (!x_t_dev || !noise_dev || !x_out_dev) return fail(B200MDM_EINVAL, "null tensor");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, index, nullptr, 0, e->noise_seed, e->noise_sample_base);
+  step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, index, nullptr, 0, e->noise_seed, e->noise_sample_base, e->n_steps);
   CUDA_TRY(cudaGetLastError());
   StepArgs a;
   a.mode = mode;
@@ -1247,6 +1266,53 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
   a.pred = pred_xstart_dev;
   int nk = 0;
   TRY(enqueue_forward(e, a, s, &nk));
+  e->launches += nk + 1;
+  return B200MDM_OK;
+}
+
+// Make the workspace's step graph (one forward + step_advance, captured on the engine stream) the graph of `key`.
+static int ensure_step_graph(b200mdm_engine* e, const GraphKey& key, const StepArgs& a) {
+  if (e->graph_exec && key == e->graph_key) return B200MDM_OK;
+  drop_graph(e);
+  cudaGraph_t graph = nullptr;
+  CUDA_TRY(cudaStreamBeginCapture(e->work, cudaStreamCaptureModeThreadLocal));
+  int nk = 0;
+  int r = enqueue_forward(e, a, e->work, &nk);
+  if (r == B200MDM_OK) {
+    PdlScope pdl_scope;
+    if (launch_k(step_advance_kernel, dim3(1), dim3(1), 0, e->work, e->state) != cudaSuccess)
+      r = fail(B200MDM_ECUDA, "step_advance launch failed during capture");
+  }
+  cudaError_t ce = cudaStreamEndCapture(e->work, &graph);
+  if (r != B200MDM_OK) {
+    if (graph) cudaGraphDestroy(graph);
+    return r;
+  }
+  if (ce != cudaSuccess) return fail(B200MDM_ECUDA, "graph capture failed: %s", cudaGetErrorString(ce));
+  ce = cudaGraphInstantiate(&e->graph_exec, graph, 0);
+  cudaGraphDestroy(graph);
+  if (ce != cudaSuccess) {
+    e->graph_exec = nullptr;
+    return fail(B200MDM_ECUDA, "graph instantiate failed: %s", cudaGetErrorString(ce));
+  }
+  e->graph_key = key;
+  e->graph_kernels = nk + 1;
+  return B200MDM_OK;
+}
+
+// One step of a loop on s: a replay of the step graph, or the same forward + step_advance as plain launches.
+static int enqueue_step(b200mdm_engine* e, const StepArgs& a, cudaStream_t s, bool use_graph) {
+  if (use_graph) {
+    CUDA_TRY(cudaGraphLaunch(e->graph_exec, s));
+    e->launches += e->graph_kernels;
+    return B200MDM_OK;
+  }
+  int nk = 0;
+  TRY(enqueue_forward(e, a, s, &nk));
+  {
+    PdlScope pdl_scope;
+    CUDA_TRY(launch_k(step_advance_kernel, dim3(1), dim3(1), 0, s, e->state));
+  }
   e->launches += nk + 1;
   return B200MDM_OK;
 }
@@ -1283,53 +1349,17 @@ extern "C" int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_
     key.mode = mode; key.B = e->B; key.T = e->T; key.flags = flags;
     key.imask = e->inpaint_mask; key.imotion = e->inpaint_motion;
     key.target_g = e->target_set ? e->tgt_g : nullptr;
-    if (!e->graph_exec || !(key == e->graph_key)) {
-      drop_graph(e);
-      cudaGraph_t graph = nullptr;
-      CUDA_TRY(cudaStreamBeginCapture(e->work, cudaStreamCaptureModeThreadLocal));
-      int nk = 0;
-      int r = enqueue_forward(e, a, e->work, &nk);
-      if (r == B200MDM_OK) {
-        PdlScope pdl_scope;
-        if (launch_k(step_advance_kernel, dim3(1), dim3(1), 0, e->work, e->state) != cudaSuccess)
-          r = fail(B200MDM_ECUDA, "step_advance launch failed during capture");
-      }
-      cudaError_t ce = cudaStreamEndCapture(e->work, &graph);
-      if (r != B200MDM_OK) {
-        if (graph) cudaGraphDestroy(graph);
-        return r;
-      }
-      if (ce != cudaSuccess) return fail(B200MDM_ECUDA, "graph capture failed: %s", cudaGetErrorString(ce));
-      ce = cudaGraphInstantiate(&e->graph_exec, graph, 0);
-      cudaGraphDestroy(graph);
-      if (ce != cudaSuccess) {
-        e->graph_exec = nullptr;
-        return fail(B200MDM_ECUDA, "graph instantiate failed: %s", cudaGetErrorString(ce));
-      }
-      e->graph_key = key;
-      e->graph_kernels = nk + 1;
-    }
+    TRY(ensure_step_graph(e, key, a));
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
     CUDA_TRY(cudaStreamWaitEvent(e->work, e->ev_in, 0));
   }
+  e->plms_done = -1;   // x_work no longer holds a PLMS loop to continue
   if (x_in_dev) CUDA_TRY(cudaMemcpyAsync(e->x_work, x_in_dev, x_bytes, cudaMemcpyDeviceToDevice, s));
-  step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, first_index, noise_tape_dev, noise_step_stride, e->noise_seed, e->noise_sample_base);
+  step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, first_index, noise_tape_dev, noise_step_stride, e->noise_seed, e->noise_sample_base,
+                                  e->n_steps);
   CUDA_TRY(cudaGetLastError());
   e->launches += 1;
-  if (use_graph) {
-    for (int k = 0; k < n_run; ++k) CUDA_TRY(cudaGraphLaunch(e->graph_exec, s));
-    e->launches += static_cast<long long>(n_run) * e->graph_kernels;
-  } else {
-    for (int k = 0; k < n_run; ++k) {
-      int nk = 0;
-      TRY(enqueue_forward(e, a, s, &nk));
-      {
-        PdlScope pdl_scope;
-        CUDA_TRY(launch_k(step_advance_kernel, dim3(1), dim3(1), 0, s, e->state));
-      }
-      e->launches += nk + 1;
-    }
-  }
+  for (int k = 0; k < n_run; ++k) TRY(enqueue_step(e, a, s, use_graph));
   if (x_out_dev) CUDA_TRY(cudaMemcpyAsync(x_out_dev, e->x_work, x_bytes, cudaMemcpyDeviceToDevice, s));
   if (use_graph) {
     CUDA_TRY(cudaEventRecord(e->ev_out, e->work));
@@ -1346,6 +1376,147 @@ extern "C" int b200mdm_sample_loop(b200mdm_engine* e, int32_t mode, int32_t skip
   if (!x_T_dev || !x_0_dev) return fail(B200MDM_EINVAL, "null tensor");
   return b200mdm_sample_loop_range(e, mode, e->n_steps - 1 - skip_timesteps, e->n_steps - skip_timesteps, x_T_dev, x_0_dev,
                                    noise_tape_dev, noise_step_stride, flags, use_graph, stream);
+}
+
+// ------------------------------------------------------------------------------------------------ PLMS
+static int ensure_plms(b200mdm_engine* e) {
+  if (e->plms_ring && e->plms_mid && e->plms_pred) return B200MDM_OK;
+  const size_t n = static_cast<size_t>(e->B) * e->JF * e->T;
+  int r = B200MDM_OK;
+  if (!e->plms_ring) r = dalloc(&e->plms_ring, PLMS_RING * n);
+  if (r == B200MDM_OK && !e->plms_mid) r = dalloc(&e->plms_mid, n);
+  if (r == B200MDM_OK && !e->plms_pred) r = dalloc(&e->plms_pred, n);
+  if (r != B200MDM_OK) {   // all or nothing: no later call may find a partial set
+    dfree(e->plms_ring); dfree(e->plms_mid); dfree(e->plms_pred);
+  }
+  return r;
+}
+
+// The pseudo improved-Euler step (gaussian_diffusion.py:1042-1049) at the schedule index the step state holds:
+// forward 1 at (x_t, i) leaves eps0 in the ring, x0 in plms_pred and mean1 in plms_mid; forward 2 at (mean1, i - 1)
+// writes the sample to x_out.  Then the step state advances.
+static int enqueue_plms_euler(b200mdm_engine* e, const StepArgs& base, const float* x_t, float* x_out, cudaStream_t s) {
+  StepArgs a = base;
+  a.mode = 4;
+  a.x_in = x_t;
+  a.x_out = e->plms_mid;
+  a.pred = e->plms_pred;
+  int nk1 = 0, nk2 = 0;
+  TRY(enqueue_forward(e, a, s, &nk1));
+  a.mode = 5;
+  a.x_in = e->plms_mid;
+  a.x_step = x_t;
+  a.x_out = x_out;
+  a.back = 1;
+  TRY(enqueue_forward(e, a, s, &nk2));
+  {
+    PdlScope pdl_scope;
+    CUDA_TRY(launch_k(step_advance_kernel, dim3(1), dim3(1), 0, s, e->state));
+  }
+  e->launches += nk1 + nk2 + 1;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_plms_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index, int32_t n_run,
+                                       const float* x_in_dev, float* x_out_dev, int32_t flags, int32_t use_graph,
+                                       void* stream) {
+  if (order < 1 || order > 4) return fail(B200MDM_EINVAL, "PLMS order %d is not an integer from 1 to 4", order);
+  if (flags & ~B200MDM_FLAG_CLIP_DENOISED) return fail(B200MDM_EINVAL, "PLMS takes no flag but B200MDM_FLAG_CLIP_DENOISED");
+  if (x_in_dev && order == 1)
+    return fail(B200MDM_EINVAL, "a PLMS loop of order 1 has no first step (the reference needs old_out there)");
+  if (n_run <= 0) return fail(B200MDM_EINVAL, "bad step range");
+  TRY(check_ready(e, true));
+  if (first_index >= e->n_steps || first_index - n_run + 1 < 0) return fail(B200MDM_EINVAL, "bad step range");
+  if (!x_in_dev && (e->plms_done < 0 || e->plms_order != order))
+    return fail(B200MDM_ESTATE, "no PLMS loop of order %d to continue (pass x_in_dev)", order);
+  TRY(ensure_plms(e));
+  cudaStream_t user = static_cast<cudaStream_t>(stream);
+  const size_t x_bytes = static_cast<size_t>(e->B) * e->JF * e->T * sizeof(float);
+  StepArgs a;
+  a.mode = 3;
+  a.order = order;
+  a.x_in = e->x_work;
+  a.x_out = e->x_work;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  cudaStream_t s = use_graph ? e->work : user;
+  if (!use_graph) attach_l2_window(e, user);
+  if (use_graph) {
+    // the Adams-Bashforth step: the same launches as a DDIM step, one graph for every order-`order` step
+    GraphKey key;
+    key.mode = a.mode; key.B = e->B; key.T = e->T; key.flags = flags; key.order = order;
+    key.imask = e->inpaint_mask; key.imotion = e->inpaint_motion;
+    key.target_g = e->target_set ? e->tgt_g : nullptr;
+    TRY(ensure_step_graph(e, key, a));
+    CUDA_TRY(cudaEventRecord(e->ev_in, user));
+    CUDA_TRY(cudaStreamWaitEvent(e->work, e->ev_in, 0));
+  }
+  const int done = x_in_dev ? 0 : e->plms_done;
+  if (x_in_dev) CUDA_TRY(cudaMemcpyAsync(e->x_work, x_in_dev, x_bytes, cudaMemcpyDeviceToDevice, s));
+  step_set_kernel<<<1, 1, 0, s>>>(e->state, done, first_index, nullptr, 0, e->noise_seed, e->noise_sample_base, e->n_steps);
+  CUDA_TRY(cudaGetLastError());
+  e->launches += 1;
+  int k = 0;
+  if (done == 0) {
+    TRY(enqueue_plms_euler(e, a, e->x_work, e->x_work, s));
+    k = 1;
+  }
+  for (; k < n_run; ++k) TRY(enqueue_step(e, a, s, use_graph));
+  e->plms_done = done + n_run;
+  e->plms_order = order;
+  if (x_out_dev) CUDA_TRY(cudaMemcpyAsync(x_out_dev, e->x_work, x_bytes, cudaMemcpyDeviceToDevice, s));
+  if (use_graph) {
+    CUDA_TRY(cudaEventRecord(e->ev_out, e->work));
+    CUDA_TRY(cudaStreamWaitEvent(user, e->ev_out, 0));
+  }
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order, const float* x_t_dev,
+                                 const float* const* old_eps_dev, int32_t n_old, int32_t flags, float* x_out_dev,
+                                 float* pred_xstart_dev, float* eps_out_dev, void* stream) {
+  if (order < 1 || order > 4) return fail(B200MDM_EINVAL, "PLMS order %d is not an integer from 1 to 4", order);
+  if (flags & ~B200MDM_FLAG_CLIP_DENOISED) return fail(B200MDM_EINVAL, "PLMS takes no flag but B200MDM_FLAG_CLIP_DENOISED");
+  // old_eps_dev NULL = no old_out (the improved-Euler step); non-NULL = old_out['old_eps'], which may be empty: the
+  // reference then takes the Adams-Bashforth branch at cur_order 1 (gaussian_diffusion.py:1042-1056)
+  const bool euler = old_eps_dev == nullptr;
+  if (n_old < 0 || (euler && n_old != 0))
+    return fail(B200MDM_EINVAL, "bad eps history (n_old %d with %s array)", n_old, euler ? "a null" : "an");
+  if (euler && order == 1)
+    return fail(B200MDM_EINVAL, "PLMS of order 1 needs an eps history (the reference needs old_out there)");
+  if (!x_t_dev || !x_out_dev) return fail(B200MDM_EINVAL, "null tensor");
+  const int h = n_old < PLMS_RING ? n_old : PLMS_RING;   // the newest h entries are all AB4 can use
+  for (int j = 0; j < h; ++j)
+    if (!old_eps_dev[n_old - h + j]) return fail(B200MDM_EINVAL, "null eps history entry %d", n_old - h + j);
+  TRY(check_ready(e, true));
+  if (index < 0 || index >= e->n_steps) return fail(B200MDM_EINVAL, "schedule index out of range");
+  TRY(ensure_plms(e));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t n = static_cast<size_t>(e->B) * e->JF * e->T, x_bytes = n * sizeof(float);
+  // the history goes into ring slots 0..h-1, oldest first, as a loop that had made h evaluations would hold it
+  for (int j = 0; j < h; ++j)
+    CUDA_TRY(cudaMemcpyAsync(e->plms_ring + j * n, old_eps_dev[n_old - h + j], x_bytes, cudaMemcpyDeviceToDevice, s));
+  step_set_kernel<<<1, 1, 0, s>>>(e->state, h, index, nullptr, 0, e->noise_seed, e->noise_sample_base, e->n_steps);
+  CUDA_TRY(cudaGetLastError());
+  e->launches += 1;
+  e->plms_done = -1;
+  StepArgs a;
+  a.order = order;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  if (euler) {
+    TRY(enqueue_plms_euler(e, a, x_t_dev, x_out_dev, s));
+    if (pred_xstart_dev) CUDA_TRY(cudaMemcpyAsync(pred_xstart_dev, e->plms_pred, x_bytes, cudaMemcpyDeviceToDevice, s));
+  } else {
+    a.mode = 3;
+    a.x_in = x_t_dev;
+    a.x_out = x_out_dev;
+    a.pred = pred_xstart_dev;
+    int nk = 0;
+    TRY(enqueue_forward(e, a, s, &nk));
+    e->launches += nk;
+  }
+  if (eps_out_dev)
+    CUDA_TRY(cudaMemcpyAsync(eps_out_dev, e->plms_ring + (h % PLMS_RING) * n, x_bytes, cudaMemcpyDeviceToDevice, s));
+  return B200MDM_OK;
 }
 
 // Counter-based noise stream of the engine (Philox4x32-10 + Box-Muller, kernels.cuh): eps of schedule index i for

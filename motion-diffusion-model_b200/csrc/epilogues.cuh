@@ -289,19 +289,36 @@ struct EpiEmbed {
 //   mode 0: out = x0                       (model forward only)
 //   mode 1: DDPM   x_{t-1} = c1*x0 + c2*x_t + (nz*sigma)*eps
 //   mode 2: DDIM   eps_hat = (sr*x_t - x0)/srm1 ; x_{t-1} = x0*sqrt_abp + coef*eps_hat + (nz*sigma)*eps
+// PLMS (gaussian_diffusion.py:992-1074), eps = (sr*x - x0)/srm1 as in DDIM; sqrt_abp / sqrt(1 - abp) are columns 5 / 6
+// of an eta = 0 table (sigma = 0 exactly, so 1 - abp - sigma^2 == 1 - abp).  eps of the k-th evaluation of the loop
+// (k = StepState::done) lives in slot k % 3 of an eps history ring:
+//   mode 3: Adams-Bashforth  eps' = combine(eps, ring[k-1], ring[k-2], ring[k-3]) at cur_order = min(order, k + 1);
+//           ring[k] = eps; pred' = sr*x_t - srm1*eps'; x_{t-1} = (pred'*sqrt_abp + s1*eps')*nz + x0*(1 - nz)
+//   mode 4: improved Euler, first evaluation: ring[k] = eps0; pred_xstart = x0; x_out = x0*sqrt_abp + s1*eps0 (mean1)
+//   mode 5: improved Euler, second evaluation, of x_t = mean1 at schedule index i - 1 (`back` = 1): eps2 from the row
+//           of i - 1; eps' = (ring[k] + eps2)/2; pred' from x_step (the step's x_t) and the row of i; the sample as
+//           in mode 3 with x0 = pred_xstart (the first evaluation's)
 // Per-step scalars come from a device table indexed by the device-side step state, so the very same launch
 // (and CUDA graph) serves every step of the loop.
 constexpr int SCHED_STRIDE = 8;  // floats per schedule row: c1 c2 sig_ddpm sr srm1 sqrt_abp coef_eps sig_ddim
+constexpr int PLMS_RING = 3;     // eps history slots: AB4 combines this step's eps with the three before it
 struct StepState {
-  int done;      // steps completed so far (indexes the noise tape)
+  int done;      // steps completed so far (indexes the noise tape; PLMS: the evaluation count k)
   int cur;       // schedule index i of the step in flight
   int start;     // schedule index of the first step (num_timesteps - 1 - skip)
-  int pad;
+  int n_steps;   // schedule length (index i - 1 of the PLMS improved-Euler step wraps to n_steps - 1 at i = 0)
   const float* noise;            // loop mode: base of the noise tape (set per loop, so the step graph is reusable)
   long long noise_step_stride;   // loop mode: elements between consecutive steps of the tape
   unsigned long long seed;       // in-engine Philox noise (philox_normal_kernel): stream seed ...
   long long sample_base;         // ... and the global index of this workspace's sample 0
 };
+
+// Schedule index a forward evaluates: the step's own (back = 0) or the one before it (back = 1, PLMS improved Euler).
+// At i = 0, i - 1 = -1 indexes the reference's timestep map and tables from the end (gaussian_diffusion.py:1046).
+__device__ __forceinline__ int eval_index(const StepState& st, int back) {
+  const int i = st.cur - back;
+  return i < 0 ? i + st.n_steps : i;
+}
 
 struct EpiOutStep {
   static constexpr int SMEM_PER_WARP = 1024;  // unused
@@ -371,6 +388,108 @@ struct EpiOutStep {
           }
           p.x_out[idx] = o;
         }
+      }
+    }
+  }
+
+  static __device__ __forceinline__ void tile_end(EpiCtx&, const Params&, int, int) {}
+  static __device__ __forceinline__ void finish(EpiCtx&) {}
+};
+
+// EpiOutStep's PLMS modes 3-5 (a GEMM kernel of their own: the DDPM / DDIM kernel stays as it was), in the reference's
+// operation order with no contraction (bit-exact fp32).  x_out, x_t, x_step and the ring slots may alias one another
+// across steps: every load of a chunk is issued before its first store, and an element is only ever read and written by
+// the thread that owns it.
+struct EpiOutPlms : EpiOutStep {
+  struct Params : EpiOutStep::Params {
+    float* eps_ring;          // [PLMS_RING, B, J, T]
+    const float* x_step;      // mode 5: x_t of the step (x_t above is mean1 there)
+    int order;                // mode 3: 1..4
+    int back;                 // this forward evaluates schedule index eval_index(state, back)
+  };
+  static __device__ __forceinline__ void tile_begin(EpiCtx&, const Params&, int, int) {}
+  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0,
+                                               int) {
+    const int row = row0 + ctx.lane;
+    if (row >= ctx.M) return;
+    const int b = row / p.S, s = row - b * p.S;
+    if (s < p.s_off) return;
+    const int t = s - p.s_off;
+    const StepState st = *p.state;
+    const int k = st.done;
+    const float* row_s = p.sched + static_cast<size_t>(st.cur) * SCHED_STRIDE;
+    const float* row_e = p.sched + static_cast<size_t>(eval_index(st, p.back)) * SCHED_STRIDE;
+    const float sr = row_s[3], srm1 = row_s[4], sq = row_s[5], s1 = row_s[6];
+    const float sr_e = row_e[3], srm1_e = row_e[4];
+    const float nzf = st.cur != 0 ? 1.f : 0.f;                  // (t != 0), gaussian_diffusion.py:1071
+    const int cur_order = min(p.order, k + 1);
+    const size_t slot = static_cast<size_t>(p.B) * p.J * p.T;
+    const float* h1 = p.eps_ring + static_cast<size_t>((k + PLMS_RING - 1) % PLMS_RING) * slot;
+    const float* h2 = p.eps_ring + static_cast<size_t>((k + PLMS_RING - 2) % PLMS_RING) * slot;
+    const float* h3 = p.eps_ring + static_cast<size_t>(k % PLMS_RING) * slot;   // k - 3
+    float* own = p.eps_ring + static_cast<size_t>(k % PLMS_RING) * slot;
+    const size_t base = static_cast<size_t>(b) * p.J * p.T + t;
+#pragma unroll
+    for (int h = 0; h < 32; h += 16) {
+      // mode 3: e1..e3 = eps of evaluations k-1..k-3;  mode 5: e1 = eps0, e2 = x_step, e3 = x0 of the first evaluation
+      float xv[16], e1[16], e2[16], e3[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = col0 + h + j;
+        const size_t idx = base + static_cast<size_t>(col) * p.T;
+        const bool in = col < p.J;
+        xv[j] = in ? p.x_t[idx] : 0.f;
+        e1[j] = e2[j] = e3[j] = 0.f;
+        if (in && p.mode == 3) {
+          if (cur_order >= 2) e1[j] = h1[idx];
+          if (cur_order >= 3) e2[j] = h2[idx];
+          if (cur_order >= 4) e3[j] = h3[idx];
+        } else if (in && p.mode == 5) {
+          e1[j] = own[idx];
+          e2[j] = p.x_step[idx];
+          e3[j] = p.pred_xstart[idx];
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = col0 + h + j;
+        if (col >= p.J) continue;
+        const size_t idx = base + static_cast<size_t>(col) * p.T;
+        float x0 = __uint_as_float(raw[h + j]) + __ldg(p.bias + col);
+        if (p.inpaint_mask != nullptr && p.inpaint_mask[idx]) x0 = p.inpaint_motion[idx];
+        if (p.clip_denoised) x0 = fminf(fmaxf(x0, -1.f), 1.f);
+        // _predict_eps_from_xstart (gaussian_diffusion.py:400-404) at the index this forward evaluates
+        const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sr_e, xv[j]), x0), srm1_e);
+        if (p.mode == 4) {
+          own[idx] = eps;
+          p.pred_xstart[idx] = x0;
+          p.x_out[idx] = __fadd_rn(__fmul_rn(x0, sq), __fmul_rn(s1, eps));   // :1045
+          continue;
+        }
+        float ep, x_t = xv[j], x0s = x0;
+        if (p.mode == 5) {
+          ep = __fdiv_rn(__fadd_rn(e1[j], eps), 2.f);                          // :1047
+          x_t = e2[j];
+          x0s = e3[j];
+        } else {
+          if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
+          if (cur_order == 1) {                                                // :1055-1062
+            ep = eps;
+          } else if (cur_order == 2) {
+            ep = __fdiv_rn(__fsub_rn(__fmul_rn(3.f, eps), e1[j]), 2.f);
+          } else if (cur_order == 3) {
+            ep = __fdiv_rn(__fadd_rn(__fsub_rn(__fmul_rn(23.f, eps), __fmul_rn(16.f, e1[j])), __fmul_rn(5.f, e2[j])), 12.f);
+          } else {
+            ep = __fdiv_rn(__fsub_rn(__fadd_rn(__fsub_rn(__fmul_rn(55.f, eps), __fmul_rn(59.f, e1[j])), __fmul_rn(37.f, e2[j])),
+                                     __fmul_rn(9.f, e3[j])),
+                           24.f);
+          }
+          own[idx] = eps;                                                      // replaces evaluation k - 3
+        }
+        // _predict_xstart_from_eps (:381-388), then the mean and the (t != 0) blend (:1065-1072)
+        const float pp = __fsub_rn(__fmul_rn(sr, x_t), __fmul_rn(srm1, ep));
+        const float mean = __fadd_rn(__fmul_rn(pp, sq), __fmul_rn(s1, ep));
+        p.x_out[idx] = __fadd_rn(__fmul_rn(mean, nzf), __fmul_rn(x0s, __fsub_rn(1.f, nzf)));
       }
     }
   }

@@ -42,7 +42,8 @@ __global__ void pack_input_kernel(const float* __restrict__ x, __half* __restric
 // ---------------------------------------------------------------------------------------------------------
 // Conditioning-token rows of the sequence (reference model/mdm.py:195,218-220,251-252):
 //   h[b', s=0, :] = (condproj[b', :] + temb_table[t(b'), :]) + pe[0, :]
-//   t(b') = tvec[b' % B] when tvec != nullptr (model called with explicit timesteps), else timestep_map[state->cur]
+//   t(b') = tvec[b' % B] when tvec != nullptr (model called with explicit timesteps), else timestep_map[i] with
+//   i = eval_index(state, back): the step in flight, or the one before it (PLMS improved Euler)
 // With a target embedding g [B, d] (model/mdm.py:197-199, both CFG halves): (condproj + (temb + g[b' % B])) + pe[0].
 // Runs right after the embedding GEMM (which leaves placeholder values in these rows).
 // The residual stream is an fp16 [hi | lo] pair per element (row = 2d halves, hi + lo carries ~22 bits).
@@ -50,11 +51,11 @@ __global__ void tok0_rows_kernel(__half* __restrict__ hres, const float* __restr
                                  const float* __restrict__ temb_table, const float* __restrict__ pe,
                                  const int* __restrict__ tvec, const int* __restrict__ tmap,
                                  const StepState* __restrict__ state, const float* __restrict__ g, int B, int S, int d,
-                                 int temb_rows) {
+                                 int temb_rows, int back) {
   pdl_launch_dependents();
   pdl_wait();
   const int bp = blockIdx.x;
-  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[state->cur];
+  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(*state, back)];
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = static_cast<size_t>(bp) * S;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
@@ -81,10 +82,11 @@ __global__ void step_advance_kernel(StepState* state) {
   state->cur -= 1;
 }
 __global__ void step_set_kernel(StepState* state, int done, int cur, const float* noise, long long noise_step_stride,
-                                unsigned long long seed, long long sample_base) {
+                                unsigned long long seed, long long sample_base, int n_steps) {
   state->done = done;
   state->cur = cur;
   state->start = cur;
+  state->n_steps = n_steps;
   state->noise = noise;
   state->noise_step_stride = noise_step_stride;
   state->seed = seed;
@@ -347,11 +349,11 @@ namespace b200 {
 __global__ void mem_build_kernel(__half* __restrict__ mem16, const float* __restrict__ memproj,
                                  const float* __restrict__ temb_table, const int* __restrict__ tvec,
                                  const int* __restrict__ tmap, const StepState* __restrict__ state,
-                                 const float* __restrict__ g, int B, int Mt, int d, int temb_rows) {
+                                 const float* __restrict__ g, int B, int Mt, int d, int temb_rows, int back) {
   pdl_launch_dependents();
   pdl_wait();
   const int m = blockIdx.x, bp = blockIdx.y;
-  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[state->cur];
+  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(*state, back)];
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = static_cast<size_t>(bp) * Mt + m;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {

@@ -2,10 +2,10 @@
 
 Same constructor keywords, same public attributes (fp64 numpy tables) and the same sampling entry points
 (`p_sample_loop`, `p_sample_loop_progressive`, `ddim_sample_loop`, `ddim_sample_loop_progressive`, `p_sample`,
-`ddim_sample`, `q_sample`), but the per-step arithmetic is not here: a loop is ONE call into libb200mdm.so which
+`ddim_sample`, `plms_sample_loop`, `plms_sample_loop_progressive`, `plms_sample`, `q_sample`), but the per-step arithmetic is not here: a loop is ONE call into libb200mdm.so which
 enqueues every step (denoiser + CFG + posterior/noise epilogue) without returning to Python.
 
-Training losses / VLB / PLMS of the reference are out of scope (SURVEY.md section 8) and raise.
+Training losses / VLB of the reference are out of scope (SURVEY.md section 8) and raise.
 """
 import enum
 import math
@@ -361,11 +361,88 @@ class GaussianDiffusion:
                                      device, skip_timesteps, init_image, randomize_class, cond_fn_with_grad, False, eta,
                                      noise_tape)
 
+    # ------------------------------------------------------------------ PLMS
+    @staticmethod
+    def _plms_order(order, old_out=None):
+        """The reference's order check (:1010-1011) plus the two failures it only meets later, raised before any engine
+        work: a non-integer order (2.5 passes the reference's check and fails with a RuntimeError inside the step) is a
+        ValueError here; order 1 without old_out is the reference's TypeError on None['old_eps'] (:1052)."""
+        if not isinstance(order, (int, float, np.integer, np.floating)) or order != int(order) or not 1 <= order <= 4:
+            raise ValueError("order is invalid (should be int from 1-4).")
+        if int(order) == 1 and old_out is None:
+            raise TypeError("PLMS of order 1 needs old_out: its first step has no eps history ('NoneType' object is "
+                            "not subscriptable in the reference)")
+        return int(order)
+
+    def plms_sample(self, model, x, t, clip_denoised=True, denoised_fn=None, cond_fn=None, model_kwargs=None,
+                    cond_fn_with_grad=False, order=2, old_out=None):
+        """reference gaussian_diffusion.py:992-1074: one pseudo linear multistep step.  old_out None (order 2-4) is the
+        pseudo improved-Euler step, two forwards; any other old_out, an empty history included, is Adams-Bashforth on
+        old_out['old_eps'], which is extended with this step's eps and trimmed in place as in the reference.  order must be an integer from 1 to 4
+        (ValueError otherwise, including non-integers such as 2.5)."""
+        order = self._plms_order(order, old_out)
+        self._reject_hooks(denoised_fn, cond_fn, False, cond_fn_with_grad)
+        idx = int(t.reshape(-1)[0].item())
+        assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch (gaussian_diffusion.py:1166)"
+        eng = self._prepare(model, x.shape, model_kwargs, x.device, 0.0)
+        old_eps = old_out["old_eps"] if old_out is not None else None     # [] is a history too (:1050-1056)
+        sample, pred, eps = eng.plms_step(idx, order, x, old_eps, 2 if clip_denoised else 0)
+        if old_out is None:
+            old_eps = [eps]
+        else:
+            old_eps.append(eps)
+        if len(old_eps) >= order:                    # :1068-1069
+            old_eps.pop(0)
+        return {"sample": sample, "pred_xstart": pred, "old_eps": old_eps}
+
+    def plms_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
+                         model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
+                         randomize_class=False, cond_fn_with_grad=False, order=2, use_graph=True, noise_seed=None,
+                         sample_index_base=0, noise_tape=None):
+        """reference gaussian_diffusion.py:1076-1116, as one engine call (every step on the device, the later ones as
+        replays of one CUDA graph).  PLMS draws no per-step noise: the only draw is x_T, from torch's generator or, with
+        `noise_seed` (+ `sample_index_base`), from the engine's Philox stream.  order: see plms_sample."""
+        order = self._plms_order(order)
+        if noise_tape is not None:
+            raise ValueError("PLMS draws no per-step noise: a noise_tape has no use (sample it with noise_mode='philox')")
+        self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
+        assert isinstance(shape, (tuple, list))
+        if device is None:
+            device = next(model.parameters()).device
+        eng = self._prepare(model, shape, model_kwargs, device, 0.0)
+        if noise_seed is not None and noise is None:
+            noise = eng.philox_normal(shape, noise_seed, sample_index_base, -1, device)
+        img = self._initial(eng, shape, noise, device, skip_timesteps, init_image)
+        n_run = self.num_timesteps - skip_timesteps
+        out = torch.empty_like(img)
+        eng.plms_loop_range(order, n_run - 1, n_run, img, out, 2 if clip_denoised else 0, use_graph)
+        eng._keep["loop"] = (img,)
+        return out
+
+    def plms_sample_loop_progressive(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
+                                     model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
+                                     randomize_class=False, cond_fn_with_grad=False, order=2):
+        """reference gaussian_diffusion.py:1118-1187: generator of {'sample', 'pred_xstart', 'old_eps'} per step."""
+        order = self._plms_order(order)
+        self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
+        assert isinstance(shape, (tuple, list))
+        if device is None:
+            device = next(model.parameters()).device
+        eng = self._prepare(model, shape, model_kwargs, device, 0.0)
+        img = self._initial(eng, shape, noise, device, skip_timesteps, init_image)
+        flags = 2 if clip_denoised else 0
+        old_eps = None                               # then one list, extended and trimmed in place as in the reference
+        for i in range(self.num_timesteps - skip_timesteps)[::-1]:
+            img, pred, eps = eng.plms_step(i, order, img, old_eps, flags)
+            old_eps = [] if old_eps is None else old_eps
+            old_eps.append(eps)
+            if len(old_eps) >= order:
+                old_eps.pop(0)
+            yield {"sample": img, "pred_xstart": pred, "old_eps": old_eps}
+
     # ------------------------------------------------------------------ out of scope
     def training_losses(self, *a, **k):
         raise NotImplementedError("training is outside the H100 sampling engine (SURVEY.md section 8)")
-
-    plms_sample_loop = training_losses
 
 
 def eng_device():

@@ -290,6 +290,25 @@ class Engine:
         check(self.lib.b200mdm_sample_loop_range(self.h, mode, first_index, n_run, _ptr(x_in), _ptr(x_out), _ptr(tape),
                                                  tape.stride(0) if tape is not None else 0, flags, int(use_graph), _stream()))
 
+    def plms_loop_range(self, order, first_index, n_run, x_in, x_out, flags=0, use_graph=True):
+        """PLMS steps first_index .. first_index-n_run+1 on the engine's working buffer (b200mdm_plms_loop_range).
+        x_in None: continue the previous PLMS loop; x_out None: leave the state in the engine."""
+        check(self.lib.b200mdm_plms_loop_range(self.h, order, first_index, n_run, _ptr(x_in), _ptr(x_out), flags,
+                                               int(use_graph), _stream()))
+
+    def plms_step(self, index, order, x_t, old_eps, flags=0):
+        """One plms_sample step (b200mdm_plms_step): old_eps = list of [B,J,F,T] eps, oldest first, possibly empty
+        (an Adams-Bashforth step), or None (no old_out: the improved-Euler step).
+        Returns (sample, pred_xstart, eps of this step)."""
+        x_t = x_t.to(torch.float32).contiguous()
+        old = [o.to(torch.float32).contiguous() for o in old_eps] if old_eps is not None else []
+        ptrs = (ctypes.c_void_p * max(1, len(old)))(*[o.data_ptr() for o in old]) if old_eps is not None else None
+        out, pred, eps = torch.empty_like(x_t), torch.empty_like(x_t), torch.empty_like(x_t)
+        check(self.lib.b200mdm_plms_step(self.h, index, order, _ptr(x_t), ptrs, len(old), flags, _ptr(out), _ptr(pred),
+                                         _ptr(eps), _stream()))
+        self._keep["plms"] = (x_t, old)
+        return out, pred, eps
+
     def set_noise_stream(self, seed, sample_index_base=0):
         check(self.lib.b200mdm_set_noise_stream(self.h, ctypes.c_uint64(int(seed) & (2 ** 64 - 1)), int(sample_index_base)))
 
