@@ -43,6 +43,8 @@ extern "C" {
 #define B200MDM_MODE_X0 0   /* model output only */
 #define B200MDM_MODE_DDPM 1 /* p_sample */
 #define B200MDM_MODE_DDIM 2 /* ddim_sample */
+/* (3-5: the PLMS steps inside b200mdm_plms_loop_range / b200mdm_plms_step; not valid modes of the calls below) */
+#define B200MDM_MODE_DDIM_REVERSE 6 /* ddim_reverse_sample: b200mdm_sample_step only (noise_dev may be NULL) */
 
 #define B200MDM_FLAG_CONST_NOISE 1   /* p_sample(const_noise=True): eps row 0 repeated (gaussian_diffusion.py:527-528) */
 #define B200MDM_FLAG_CLIP_DENOISED 2 /* clip_denoised=True: clamp x0 to [-1,1] (gaussian_diffusion.py:348-352) */
@@ -110,6 +112,14 @@ int b200mdm_finalize_weights(b200mdm_engine* e, void* stream);
  * timestep_map_host: _WrappedModel's map (respace.py:125-127), n_steps int32.  Synchronous copy. */
 int b200mdm_set_schedule(b200mdm_engine* e, int32_t n_steps, const float* rows_host, const int32_t* timestep_map_host);
 
+/* The DDIM inversion's table (ddim_reverse_sample, gaussian_diffusion.py:866-872), n_steps rows of
+ *   [0] sqrt(alphas_cumprod_next)  [1] sqrt(1 - alphas_cumprod_next)
+ * with alphas_cumprod_next cast fp64 -> fp32 first, then fp32 arithmetic (the last row is 0, 1).  n_steps must equal
+ * the current schedule's; every b200mdm_set_schedule makes the table stale, and a reverse call against a stale table
+ * fails with B200MDM_ESTATE.  Synchronous copy. */
+#define B200MDM_SCHED_NEXT_STRIDE 2
+int b200mdm_set_schedule_next(b200mdm_engine* e, int32_t n_steps, const float* rows_host);
+
 /* Canonicalises model_kwargs['y'] (data_loaders/tensors.py:22-64 + callers) once per loop and (re)builds the
  * workspace for (batch, nframes):
  *   cond_embed_dev : y['text_embed'][0]  [batch, cond_dim] fp32 device, or NULL (cond_mode none / action)
@@ -154,7 +164,11 @@ int b200mdm_set_inpaint(b200mdm_engine* e, const uint8_t* mask_dev, const float*
 int b200mdm_denoise(b200mdm_engine* e, const float* x_dev, const int32_t* timesteps_host, float* out_dev, void* stream);
 
 /* One p_sample / ddim_sample (gaussian_diffusion.py:489-541 / 729-779) at schedule index `index`:
- * x_out = step(x_t, eps).  pred_xstart_dev may be NULL.  x_out_dev may alias x_t_dev. */
+ * x_out = step(x_t, eps).  pred_xstart_dev may be NULL.  x_out_dev may alias x_t_dev.
+ * mode B200MDM_MODE_DDIM_REVERSE: one ddim_reverse_sample (gaussian_diffusion.py:838-874, eta = 0), x at index i ->
+ * x at index i + 1: eps = (sr*x - x0)/srm1, x_out = x0*sqrt(abn) + sqrt(1 - abn)*eps.  noise_dev is not read (may be
+ * NULL), the only valid flag is B200MDM_FLAG_CLIP_DENOISED, and b200mdm_set_schedule_next must have been called for
+ * the current schedule. */
 int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t index, const float* x_t_dev, const float* noise_dev,
                         int32_t flags, float* x_out_dev, float* pred_xstart_dev, void* stream);
 
@@ -176,6 +190,13 @@ int b200mdm_sample_loop(b200mdm_engine* e, int32_t mode, int32_t skip_timesteps,
 int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_t first_index, int32_t n_run, const float* x_in_dev,
                               float* x_out_dev, const float* noise_tape_dev, int64_t noise_step_stride, int32_t flags,
                               int32_t use_graph, void* stream);
+
+/* ddim_reverse_sample (gaussian_diffusion.py:838-874) repeated without returning to the host: schedule indices
+ * first_index, first_index+1, ... (n_run of them, up to n_steps - 1) on the engine's working buffer, one CUDA graph of a
+ * single step replayed when use_graph != 0.  x_in_dev / x_out_dev NULL as in b200mdm_sample_loop_range.  flags:
+ * B200MDM_FLAG_CLIP_DENOISED or 0.  No noise is drawn.  Needs b200mdm_set_schedule_next for the current schedule. */
+int b200mdm_ddim_reverse_loop_range(b200mdm_engine* e, int32_t first_index, int32_t n_run, const float* x_in_dev,
+                                    float* x_out_dev, int32_t flags, int32_t use_graph, void* stream);
 
 /* plms_sample_loop (gaussian_diffusion.py:1076-1187) without returning to the host: schedule indices first_index,
  * first_index-1, ... (n_run of them) on the engine's working buffer, order 1..4.  x_in_dev != NULL starts a fresh loop

@@ -13,8 +13,10 @@ ARCH = {"trans_enc": 0, "trans_dec": 1}
 COND_NONE, COND_TEXT, COND_ACTION = 0, 1, 2
 TARGET = {"single": 1, "multi": 2, "split": 3}   # args.multi_encoder_type -> b200mdm_config.target_encoder (0: none)
 MODE_X0, MODE_DDPM, MODE_DDIM = 0, 1, 2
+MODE_DDIM_REVERSE = 6   # (3-5 are the PLMS steps inside the PLMS calls)
 FLAG_CONST_NOISE, FLAG_CLIP_DENOISED, FLAG_PHILOX_NOISE = 1, 2, 4
 SCHED_STRIDE = 8
+SCHED_NEXT_STRIDE = 2
 
 # every symbol include/b200mdm.h declares (tests check that the library exports all of them)
 SYMBOLS = [
@@ -26,6 +28,7 @@ SYMBOLS = [
     "b200mdm_recover_from_ric", "b200mdm_test_gemm_f16", "b200mdm_test_attention", "b200mdm_test_cross_attention", "b200mdm_test_qkv_attention",
     "b200mdm_test_gemm_resid_ln", "b200mdm_test_gemm_epi", "b200mdm_test_embed", "b200mdm_test_out_step",
     "b200mdm_set_target", "b200mdm_test_target", "b200mdm_plms_loop_range", "b200mdm_plms_step",
+    "b200mdm_set_schedule_next", "b200mdm_ddim_reverse_loop_range",
 ]
 
 
@@ -92,7 +95,9 @@ def load():
                        ("b200mdm_set_target", [vp, vp, vp, vp]),
                        ("b200mdm_test_target", [vp, vp, vp, i32, vp, vp]),
                        ("b200mdm_plms_loop_range", [vp, i32, i32, i32, vp, vp, i32, i32, vp]),
-                       ("b200mdm_plms_step", [vp, i32, i32, vp, ctypes.POINTER(vp), i32, i32, vp, vp, vp, vp])):
+                       ("b200mdm_plms_step", [vp, i32, i32, vp, ctypes.POINTER(vp), i32, i32, vp, vp, vp, vp]),
+                       ("b200mdm_set_schedule_next", [vp, i32, vp]),
+                       ("b200mdm_ddim_reverse_loop_range", [vp, i32, i32, vp, vp, i32, i32, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

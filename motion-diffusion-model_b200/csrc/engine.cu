@@ -210,6 +210,10 @@ struct b200mdm_engine : Workspace {
   float* sched = nullptr;
   int* tmap = nullptr;
   int n_steps = 0, sched_cap = 0;
+  // DDIM inversion: sqrt(abn), sqrt(1 - abn) per row (b200mdm_set_schedule_next), allocated with `sched`; every
+  // b200mdm_set_schedule makes it stale until the next b200mdm_set_schedule_next
+  float* sched_next = nullptr;
+  bool sched_next_fresh = false;
   // parked workspaces (see Workspace)
   std::vector<Workspace> pool;
   unsigned long long use_clock = 0;
@@ -282,6 +286,7 @@ static int init_kernel_attrs() {
   TRY((set_gemm_attr<128, EpiEmbed>()));
   TRY((set_gemm_attr<96, EpiOutStep>()));
   TRY((set_gemm_attr<96, EpiOutPlms>()));
+  TRY((set_gemm_attr<96, EpiOutReverse>()));
   TRY((set_attention_attr<64>()));
   TRY((set_attention_attr<208>()));
   TRY((set_attention_attr<256>()));
@@ -512,6 +517,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   for (auto& kv : e->store) cudaFree(kv.second.dev);
   for (auto& l : e->layers) { dfree(l.wqkv); dfree(l.wo); dfree(l.w1); dfree(l.w2); dfree(l.wq_c); dfree(l.wo_c); }
   dfree(e->w_in3); dfree(e->w_out3); dfree(e->temb_hidden); dfree(e->temb_table); dfree(e->sched); dfree(e->tmap);
+  dfree(e->sched_next);
   dfree(e->wkv_all); dfree(e->bkv_all);
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
@@ -805,14 +811,31 @@ extern "C" int b200mdm_set_schedule(b200mdm_engine* e, int32_t n_steps, const fl
     drop_all_graphs(e);
     dfree(e->sched);
     dfree(e->tmap);
+    dfree(e->sched_next);
+    e->sched_cap = 0;
     const int cap = n_steps > 1000 ? n_steps : 1000;
     TRY(dalloc(&e->sched, static_cast<size_t>(cap) * SCHED_STRIDE));
     TRY(dalloc(&e->tmap, cap));
+    TRY(dalloc(&e->sched_next, static_cast<size_t>(cap) * SCHED_NEXT_STRIDE));
     e->sched_cap = cap;
   }
   e->n_steps = n_steps;
+  e->sched_next_fresh = false;
   CUDA_TRY(cudaMemcpy(e->sched, rows_host, static_cast<size_t>(n_steps) * SCHED_STRIDE * sizeof(float), cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(e->tmap, timestep_map_host, static_cast<size_t>(n_steps) * sizeof(int), cudaMemcpyHostToDevice));
+  return B200MDM_OK;
+}
+
+static_assert(SCHED_NEXT_STRIDE == B200MDM_SCHED_NEXT_STRIDE, "the reverse table's row layout is part of the ABI");
+extern "C" int b200mdm_set_schedule_next(b200mdm_engine* e, int32_t n_steps, const float* rows_host) {
+  if (!e || !rows_host) return fail(B200MDM_EINVAL, "bad argument");
+  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
+  if (n_steps != e->n_steps)
+    return fail(B200MDM_EINVAL, "n_steps %d differs from the schedule's %d", n_steps, e->n_steps);
+  CUDA_TRY(cudaDeviceSynchronize());  // a reverse loop still in flight may be reading the old rows
+  CUDA_TRY(cudaMemcpy(e->sched_next, rows_host, static_cast<size_t>(n_steps) * SCHED_NEXT_STRIDE * sizeof(float),
+                      cudaMemcpyHostToDevice));
+  e->sched_next_fresh = true;
   return B200MDM_OK;
 }
 
@@ -1203,6 +1226,11 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     if (a.mode <= B200MDM_MODE_DDIM) {
       const EpiOutStep::Params& ps = p;
       TRY((launch_gemm<96, EpiOutStep>(e->m_g16, e->m_wout, e->m_g16, B * T, e->N_out_pad, 3 * d, ps, s, e->num_sms)));
+    } else if (a.mode == B200MDM_MODE_DDIM_REVERSE) {
+      EpiOutReverse::Params pr;
+      static_cast<EpiOutStep::Params&>(pr) = p;
+      pr.sched_next = e->sched_next;
+      TRY((launch_gemm<96, EpiOutReverse>(e->m_g16, e->m_wout, e->m_g16, B * T, e->N_out_pad, 3 * d, pr, s, e->num_sms)));
     } else {
       p.eps_ring = e->plms_ring;
       p.x_step = a.x_step;
@@ -1250,9 +1278,14 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
                                    const float* noise_dev, int32_t flags, float* x_out_dev,
                                    float* pred_xstart_dev, void* stream) {
   TRY(check_ready(e, true));
-  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM) return fail(B200MDM_EINVAL, "bad mode");
+  const bool reverse = mode == B200MDM_MODE_DDIM_REVERSE;
+  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM && !reverse) return fail(B200MDM_EINVAL, "bad mode");
   if (index < 0 || index >= e->n_steps) return fail(B200MDM_EINVAL, "schedule index out of range");
-  if (!x_t_dev || !noise_dev || !x_out_dev) return fail(B200MDM_EINVAL, "null tensor");
+  if (!x_t_dev || (!noise_dev && !reverse) || !x_out_dev) return fail(B200MDM_EINVAL, "null tensor");
+  if (reverse && (flags & ~B200MDM_FLAG_CLIP_DENOISED))
+    return fail(B200MDM_EINVAL, "DDIM inversion takes no flag but B200MDM_FLAG_CLIP_DENOISED");
+  if (reverse && !e->sched_next_fresh)
+    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_next has not been called for the current schedule");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, index, nullptr, 0, e->noise_seed, e->noise_sample_base, e->n_steps);
   CUDA_TRY(cudaGetLastError());
@@ -1270,6 +1303,13 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
   return B200MDM_OK;
 }
 
+// Move the step state to the next step of the loop: down the schedule, or up it for the DDIM inversion.
+static cudaError_t launch_advance(b200mdm_engine* e, const StepArgs& a, cudaStream_t s) {
+  PdlScope pdl_scope;
+  if (a.mode == B200MDM_MODE_DDIM_REVERSE) return launch_k(step_advance_up_kernel, dim3(1), dim3(1), 0, s, e->state);
+  return launch_k(step_advance_kernel, dim3(1), dim3(1), 0, s, e->state);
+}
+
 // Make the workspace's step graph (one forward + step_advance, captured on the engine stream) the graph of `key`.
 static int ensure_step_graph(b200mdm_engine* e, const GraphKey& key, const StepArgs& a) {
   if (e->graph_exec && key == e->graph_key) return B200MDM_OK;
@@ -1278,11 +1318,8 @@ static int ensure_step_graph(b200mdm_engine* e, const GraphKey& key, const StepA
   CUDA_TRY(cudaStreamBeginCapture(e->work, cudaStreamCaptureModeThreadLocal));
   int nk = 0;
   int r = enqueue_forward(e, a, e->work, &nk);
-  if (r == B200MDM_OK) {
-    PdlScope pdl_scope;
-    if (launch_k(step_advance_kernel, dim3(1), dim3(1), 0, e->work, e->state) != cudaSuccess)
-      r = fail(B200MDM_ECUDA, "step_advance launch failed during capture");
-  }
+  if (r == B200MDM_OK && launch_advance(e, a, e->work) != cudaSuccess)
+    r = fail(B200MDM_ECUDA, "step_advance launch failed during capture");
   cudaError_t ce = cudaStreamEndCapture(e->work, &graph);
   if (r != B200MDM_OK) {
     if (graph) cudaGraphDestroy(graph);
@@ -1309,44 +1346,25 @@ static int enqueue_step(b200mdm_engine* e, const StepArgs& a, cudaStream_t s, bo
   }
   int nk = 0;
   TRY(enqueue_forward(e, a, s, &nk));
-  {
-    PdlScope pdl_scope;
-    CUDA_TRY(launch_k(step_advance_kernel, dim3(1), dim3(1), 0, s, e->state));
-  }
+  CUDA_TRY(launch_advance(e, a, s));
   e->launches += nk + 1;
   return B200MDM_OK;
 }
 
-// Schedule indices first_index, first_index-1, ... (n_run of them) on the engine's working buffer.  x_in_dev == NULL
-// continues from the state the previous call left there; x_out_dev == NULL leaves the result there.
-extern "C" int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_t first_index, int32_t n_run,
-                                         const float* x_in_dev, float* x_out_dev, const float* noise_tape_dev,
-                                         int64_t noise_step_stride, int32_t flags, int32_t use_graph, void* stream) {
-  TRY(check_ready(e, true));
-  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM) return fail(B200MDM_EINVAL, "bad mode");
-  if (n_run <= 0 || first_index >= e->n_steps || first_index - n_run + 1 < 0) return fail(B200MDM_EINVAL, "bad step range");
-  const bool philox = (flags & B200MDM_FLAG_PHILOX_NOISE) != 0;
-  if (!philox && !noise_tape_dev) return fail(B200MDM_EINVAL, "null noise tape (or pass B200MDM_FLAG_PHILOX_NOISE)");
+// n_run steps of `a` from schedule index first_index on the engine's working buffer (a.x_in == a.x_out == x_work).
+// x_in_dev == NULL continues from the state the previous call left there; x_out_dev == NULL leaves the result there.
+static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t first_index, int32_t n_run,
+                    const float* x_in_dev, float* x_out_dev, const float* noise_tape_dev, int64_t noise_step_stride,
+                    int32_t use_graph, void* stream) {
   cudaStream_t user = static_cast<cudaStream_t>(stream);
   const size_t x_bytes = static_cast<size_t>(e->B) * e->JF * e->T * sizeof(float);
-  // The loop runs in place on an engine-owned buffer (fixed address => the captured step graph never changes);
-  // every element is read and written by the same thread of the fused output epilogue.
-  StepArgs a;
-  a.mode = mode;
-  a.x_in = e->x_work;
-  a.x_out = e->x_work;
-  a.noise = philox ? e->eps_buf : nullptr;
-  a.philox = philox;
-  a.const_noise = flags & B200MDM_FLAG_CONST_NOISE;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-
   // The graph path runs on the engine's own stream (the caller's may be the legacy default stream, which cannot be
   // captured), ordered after / before the caller's stream with events.
   cudaStream_t s = use_graph ? e->work : user;
   if (!use_graph) attach_l2_window(e, user);   // plain launches: the residual-stream window goes on the caller's stream
   if (use_graph) {
     GraphKey key;
-    key.mode = mode; key.B = e->B; key.T = e->T; key.flags = flags;
+    key.mode = a.mode; key.B = e->B; key.T = e->T; key.flags = flags;
     key.imask = e->inpaint_mask; key.imotion = e->inpaint_motion;
     key.target_g = e->target_set ? e->tgt_g : nullptr;
     TRY(ensure_step_graph(e, key, a));
@@ -1368,6 +1386,28 @@ extern "C" int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_
   return B200MDM_OK;
 }
 
+// Schedule indices first_index, first_index-1, ... (n_run of them) on the engine's working buffer.
+extern "C" int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_t first_index, int32_t n_run,
+                                         const float* x_in_dev, float* x_out_dev, const float* noise_tape_dev,
+                                         int64_t noise_step_stride, int32_t flags, int32_t use_graph, void* stream) {
+  TRY(check_ready(e, true));
+  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM) return fail(B200MDM_EINVAL, "bad mode");
+  if (n_run <= 0 || first_index >= e->n_steps || first_index - n_run + 1 < 0) return fail(B200MDM_EINVAL, "bad step range");
+  const bool philox = (flags & B200MDM_FLAG_PHILOX_NOISE) != 0;
+  if (!philox && !noise_tape_dev) return fail(B200MDM_EINVAL, "null noise tape (or pass B200MDM_FLAG_PHILOX_NOISE)");
+  // The loop runs in place on an engine-owned buffer (fixed address => the captured step graph never changes);
+  // every element is read and written by the same thread of the fused output epilogue.
+  StepArgs a;
+  a.mode = mode;
+  a.x_in = e->x_work;
+  a.x_out = e->x_work;
+  a.noise = philox ? e->eps_buf : nullptr;
+  a.philox = philox;
+  a.const_noise = flags & B200MDM_FLAG_CONST_NOISE;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  return run_loop(e, a, flags, first_index, n_run, x_in_dev, x_out_dev, noise_tape_dev, noise_step_stride, use_graph, stream);
+}
+
 extern "C" int b200mdm_sample_loop(b200mdm_engine* e, int32_t mode, int32_t skip_timesteps, const float* x_T_dev,
                                    float* x_0_dev, const float* noise_tape_dev, int64_t noise_step_stride,
                                    int32_t flags, int32_t use_graph, void* stream) {
@@ -1376,6 +1416,26 @@ extern "C" int b200mdm_sample_loop(b200mdm_engine* e, int32_t mode, int32_t skip
   if (!x_T_dev || !x_0_dev) return fail(B200MDM_EINVAL, "null tensor");
   return b200mdm_sample_loop_range(e, mode, e->n_steps - 1 - skip_timesteps, e->n_steps - skip_timesteps, x_T_dev, x_0_dev,
                                    noise_tape_dev, noise_step_stride, flags, use_graph, stream);
+}
+
+// ------------------------------------------------------------------------------------------------ DDIM inversion
+// ddim_reverse_sample at schedule indices first_index, first_index+1, ... (n_run of them) on the engine's working
+// buffer: the loop of b200mdm_sample_loop_range with the reverse epilogue, no noise and an upward step counter.
+extern "C" int b200mdm_ddim_reverse_loop_range(b200mdm_engine* e, int32_t first_index, int32_t n_run, const float* x_in_dev,
+                                               float* x_out_dev, int32_t flags, int32_t use_graph, void* stream) {
+  if (flags & ~B200MDM_FLAG_CLIP_DENOISED)
+    return fail(B200MDM_EINVAL, "DDIM inversion takes no flag but B200MDM_FLAG_CLIP_DENOISED");
+  if (n_run <= 0 || first_index < 0) return fail(B200MDM_EINVAL, "bad step range");
+  TRY(check_ready(e, true));
+  if (n_run > e->n_steps - first_index) return fail(B200MDM_EINVAL, "bad step range");
+  if (!e->sched_next_fresh)
+    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_next has not been called for the current schedule");
+  StepArgs a;
+  a.mode = B200MDM_MODE_DDIM_REVERSE;
+  a.x_in = e->x_work;
+  a.x_out = e->x_work;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  return run_loop(e, a, flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0, use_graph, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ PLMS

@@ -497,4 +497,53 @@ struct EpiOutPlms : EpiOutStep {
   static __device__ __forceinline__ void finish(EpiCtx&) {}
 };
 
+// ddim_reverse_sample (gaussian_diffusion.py:838-874), mode 6 (a GEMM kernel of its own, as EpiOutPlms): x at schedule
+// index i -> x at index i + 1 along the deterministic DDIM ODE.
+//   eps = (sr*x - x0)/srm1 (row i of sched); x_next = x0*sqrt(abn) + sqrt(1 - abn)*eps (row i of sched_next)
+// fp32, unfused, in the reference's operation order.  No noise and no history: x_t is the only load.  x_out may alias
+// x_t (the in-place loop): every load of a chunk is issued before its first store.
+constexpr int SCHED_NEXT_STRIDE = 2;   // floats per row of the reverse table: sqrt(abn) sqrt(1 - abn)
+struct EpiOutReverse : EpiOutStep {
+  struct Params : EpiOutStep::Params {
+    const float* sched_next;  // [n_steps, SCHED_NEXT_STRIDE]
+  };
+  static __device__ __forceinline__ void tile_begin(EpiCtx&, const Params&, int, int) {}
+  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0,
+                                               int) {
+    const int row = row0 + ctx.lane;
+    if (row >= ctx.M) return;
+    const int b = row / p.S, s = row - b * p.S;
+    if (s < p.s_off) return;
+    const int t = s - p.s_off;
+    const int i = p.state->cur;
+    const float* row_s = p.sched + static_cast<size_t>(i) * SCHED_STRIDE;
+    const float* row_n = p.sched_next + static_cast<size_t>(i) * SCHED_NEXT_STRIDE;
+    const float sr = row_s[3], srm1 = row_s[4], sa = row_n[0], sb = row_n[1];
+    const size_t base = static_cast<size_t>(b) * p.J * p.T + t;
+#pragma unroll
+    for (int h = 0; h < 32; h += 16) {
+      float xv[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = col0 + h + j;
+        xv[j] = col < p.J ? p.x_t[base + static_cast<size_t>(col) * p.T] : 0.f;
+      }
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = col0 + h + j;
+        if (col >= p.J) continue;
+        const size_t idx = base + static_cast<size_t>(col) * p.T;
+        float x0 = __uint_as_float(raw[h + j]) + __ldg(p.bias + col);
+        if (p.inpaint_mask != nullptr && p.inpaint_mask[idx]) x0 = p.inpaint_motion[idx];
+        if (p.clip_denoised) x0 = fminf(fmaxf(x0, -1.f), 1.f);
+        if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
+        const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sr, xv[j]), x0), srm1);     // :862-865
+        p.x_out[idx] = __fadd_rn(__fmul_rn(x0, sa), __fmul_rn(sb, eps));              // :869-872
+      }
+    }
+  }
+  static __device__ __forceinline__ void tile_end(EpiCtx&, const Params&, int, int) {}
+  static __device__ __forceinline__ void finish(EpiCtx&) {}
+};
+
 }  // namespace b200

@@ -81,6 +81,13 @@ __global__ void step_advance_kernel(StepState* state) {
   state->done += 1;
   state->cur -= 1;
 }
+// The DDIM inversion walks the schedule upwards (x at index i -> x at index i + 1).
+__global__ void step_advance_up_kernel(StepState* state) {
+  pdl_launch_dependents();
+  pdl_wait();
+  state->done += 1;
+  state->cur += 1;
+}
 __global__ void step_set_kernel(StepState* state, int done, int cur, const float* noise, long long noise_step_stride,
                                 unsigned long long seed, long long sample_base, int n_steps) {
   state->done = done;

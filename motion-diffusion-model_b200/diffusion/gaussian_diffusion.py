@@ -2,7 +2,8 @@
 
 Same constructor keywords, same public attributes (fp64 numpy tables) and the same sampling entry points
 (`p_sample_loop`, `p_sample_loop_progressive`, `ddim_sample_loop`, `ddim_sample_loop_progressive`, `p_sample`,
-`ddim_sample`, `plms_sample_loop`, `plms_sample_loop_progressive`, `plms_sample`, `q_sample`), but the per-step arithmetic is not here: a loop is ONE call into libb200mdm.so which
+`ddim_sample`, `plms_sample_loop`, `plms_sample_loop_progressive`, `plms_sample`, `ddim_reverse_sample`, `q_sample`),
+plus the DDIM inversion loops `ddim_reverse_sample_loop` / `ddim_reverse_sample_loop_progressive`, but the per-step arithmetic is not here: a loop is ONE call into libb200mdm.so which
 enqueues every step (denoiser + CFG + posterior/noise epilogue) without returning to Python.
 
 Training losses / VLB of the reference are out of scope (SURVEY.md section 8) and raise.
@@ -127,6 +128,16 @@ class GaussianDiffusion:
             rows[:, 6] = np.sqrt(one - abp - sigma ** 2)
         rows[:, 7] = nz * sigma
         return rows.astype(np.float32)
+
+    def schedule_next_rows(self):
+        """[n, 2] fp32 rows sqrt(abn), sqrt(1 - abn) for b200mdm_set_schedule_next: ddim_reverse_sample's
+        th.sqrt(alpha_bar_next) and th.sqrt(1 - alpha_bar_next) (:866-872), alphas_cumprod_next cast to fp32 first
+        (:1612), then fp32 arithmetic.  The last row is (0, 1)."""
+        abn = _f32(self.alphas_cumprod_next)
+        rows = np.empty((self.num_timesteps, _lib.SCHED_NEXT_STRIDE), dtype=np.float32)
+        rows[:, 0] = np.sqrt(abn)
+        rows[:, 1] = np.sqrt(np.float32(1.0) - abn)
+        return rows
 
     def _timestep_map(self):
         return list(range(self.num_timesteps))
@@ -360,6 +371,66 @@ class GaussianDiffusion:
         yield from self._progressive(_lib.MODE_DDIM, model, shape, noise, clip_denoised, denoised_fn, cond_fn, model_kwargs,
                                      device, skip_timesteps, init_image, randomize_class, cond_fn_with_grad, False, eta,
                                      noise_tape)
+
+    # ------------------------------------------------------------------ DDIM inversion
+    def _prepare_reverse(self, model, shape, model_kwargs, device):
+        eng = self._prepare(model, shape, model_kwargs, device, 0.0)
+        eng.set_schedule_next(self.schedule_next_rows(), key=(id(self), self.num_timesteps))
+        return eng
+
+    def _reverse_range(self, first_index, n_steps):
+        """Schedule indices of an inversion loop (default: the whole schedule); ValueError before any engine work."""
+        n = self.num_timesteps
+        if n_steps is None:
+            n_steps = n - first_index if isinstance(first_index, (int, np.integer)) else None
+        for name, v in (("first_index", first_index), ("n_steps", n_steps)):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+                raise ValueError("%s must be an integer (got %r)" % (name, v))
+        if not (0 <= first_index < n and 1 <= n_steps <= n - first_index):
+            raise ValueError("the inversion runs schedule indices first_index .. first_index + n_steps - 1 within [0, %d) "
+                             "(got first_index=%d, n_steps=%d)" % (n, first_index, n_steps))
+        return int(first_index), int(n_steps)
+
+    def ddim_reverse_sample(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None, eta=0.0):
+        """reference gaussian_diffusion.py:838-874: x at schedule index t -> x at index t + 1 along the deterministic
+        DDIM ODE.  Returns {'sample', 'pred_xstart'}."""
+        if eta != 0.0:
+            raise AssertionError("Reverse ODE only for deterministic path")
+        self._reject_hooks(denoised_fn, None, False, False)
+        idx = int(t.reshape(-1)[0].item())
+        assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch"
+        eng = self._prepare_reverse(model, x.shape, model_kwargs, x.device)
+        out, pred = eng.sample_step(_lib.MODE_DDIM_REVERSE, idx, x, None, 2 if clip_denoised else 0, want_pred=True)
+        return {"sample": out, "pred_xstart": pred}
+
+    def ddim_reverse_sample_loop(self, model, x_start, clip_denoised=True, model_kwargs=None, device=None, first_index=0,
+                                 n_steps=None, use_graph=True):
+        """DDIM inversion (no reference counterpart as a loop): exactly the reference step ddim_reverse_sample
+        iterated for i = first_index ... first_index + n_steps - 1 (default: the whole schedule, 0 ... n - 1), as one
+        engine call (every step a replay of one CUDA graph).  Returns the last step's sample; x_start is not modified."""
+        first, n_run = self._reverse_range(first_index, n_steps)
+        if device is None:
+            device = next(model.parameters()).device
+        eng = self._prepare_reverse(model, x_start.shape, model_kwargs, device)
+        img = x_start.to(device=device, dtype=torch.float32).contiguous()
+        out = torch.empty_like(img)
+        eng.ddim_reverse_loop_range(first, n_run, img, out, 2 if clip_denoised else 0, use_graph)
+        eng._keep["loop"] = (img,)
+        return out
+
+    def ddim_reverse_sample_loop_progressive(self, model, x_start, clip_denoised=True, model_kwargs=None, device=None,
+                                             first_index=0, n_steps=None):
+        """ddim_reverse_sample_loop as a generator of the reference step's {'sample', 'pred_xstart'}, one step call per
+        yield, for i = first_index ... first_index + n_steps - 1."""
+        first, n_run = self._reverse_range(first_index, n_steps)
+        if device is None:
+            device = next(model.parameters()).device
+        eng = self._prepare_reverse(model, x_start.shape, model_kwargs, device)
+        img = x_start.to(device=device, dtype=torch.float32).contiguous()
+        flags = 2 if clip_denoised else 0
+        for i in range(first, first + n_run):
+            img, pred = eng.sample_step(_lib.MODE_DDIM_REVERSE, i, img, None, flags, want_pred=True)
+            yield {"sample": img, "pred_xstart": pred}
 
     # ------------------------------------------------------------------ PLMS
     @staticmethod

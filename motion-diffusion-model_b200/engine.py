@@ -79,6 +79,7 @@ class Engine:
         self._keep = {}
         self._cond_key = None
         self._sched_key = None
+        self._next_key = None
         self.batch = self.nframes = 0
 
     def close(self):
@@ -118,6 +119,16 @@ class Engine:
         check(self.lib.b200mdm_set_schedule(self.h, len(tmap), rows.ctypes.data_as(ctypes.c_void_p),
                                             tmap.ctypes.data_as(ctypes.c_void_p)))
         self._sched_key = key
+        self._next_key = None                     # the engine marks the reverse table stale
+
+    def set_schedule_next(self, rows, key=None):
+        """[n_steps, 2] fp32 rows sqrt(abn), sqrt(1 - abn) of the current schedule (b200mdm_set_schedule_next)."""
+        if key is not None and key == self._next_key:
+            return
+        rows = np.ascontiguousarray(rows, dtype=np.float32)
+        assert rows.ndim == 2 and rows.shape[1] == _lib.SCHED_NEXT_STRIDE
+        check(self.lib.b200mdm_set_schedule_next(self.h, rows.shape[0], rows.ctypes.data_as(ctypes.c_void_p)))
+        self._next_key = key
 
     # ------------------------------------------------------------------ conditioning
     def set_cond(self, batch, nframes, y, guided, device):
@@ -260,8 +271,9 @@ class Engine:
         return out
 
     def sample_step(self, mode, index, x_t, noise, flags=0, want_pred=True):
+        """noise may be None for MODE_DDIM_REVERSE, which draws none."""
         x_t = x_t.to(torch.float32).contiguous()
-        noise = noise.to(torch.float32).contiguous()
+        noise = noise.to(torch.float32).contiguous() if noise is not None else None
         out = torch.empty_like(x_t)
         pred = torch.empty_like(x_t) if want_pred else None
         check(self.lib.b200mdm_sample_step(self.h, mode, index, _ptr(x_t), _ptr(noise), flags, _ptr(out), _ptr(pred),
@@ -289,6 +301,12 @@ class Engine:
             flags |= _lib.FLAG_PHILOX_NOISE
         check(self.lib.b200mdm_sample_loop_range(self.h, mode, first_index, n_run, _ptr(x_in), _ptr(x_out), _ptr(tape),
                                                  tape.stride(0) if tape is not None else 0, flags, int(use_graph), _stream()))
+
+    def ddim_reverse_loop_range(self, first_index, n_run, x_in, x_out, flags=0, use_graph=True):
+        """DDIM inversion steps first_index .. first_index+n_run-1 on the engine's working buffer
+        (b200mdm_ddim_reverse_loop_range).  x_in None: continue; x_out None: leave the state in the engine."""
+        check(self.lib.b200mdm_ddim_reverse_loop_range(self.h, first_index, n_run, _ptr(x_in), _ptr(x_out), flags,
+                                                       int(use_graph), _stream()))
 
     def plms_loop_range(self, order, first_index, n_run, x_in, x_out, flags=0, use_graph=True):
         """PLMS steps first_index .. first_index-n_run+1 on the engine's working buffer (b200mdm_plms_loop_range).
