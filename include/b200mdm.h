@@ -270,7 +270,7 @@ int b200mdm_test_gemm_epi(const void* a16_dev, const void* w16_dev, const float*
 int b200mdm_test_embed(const float* x_dev, const float* w_in_dev, const float* b_in_dev, const float* pe_dev, void* hres16_dev,
                        int32_t B, int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream);
 /* The output launches of the step through scratch buffers allocated on `stream`: blend_split of the residual stream, then
- * the split-weight EpiOutStep GEMM (BLOCK_N 96) with the sampler update, schedule row `sched_row` (8 floats, device; see
+ * the split-weight EpiOut<OutStep> GEMM (BLOCK_N 96) with the sampler update, schedule row `sched_row` (8 floats, device; see
  * b200mdm_set_schedule) as a one-row table at index 0.
  * hres16 fp16 [halves*B*S, 2d] = [hi | lo] (S = T + s_off; rows s >= s_off are frames); scale fp32 [B] (NULL when
  * halves == 1); w_out fp32 [JF, d]; b_out fp32 [JF]; x_t, noise, x_out, pred_xstart fp32 [B, JF, T] (x_out may alias

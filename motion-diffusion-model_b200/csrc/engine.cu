@@ -284,9 +284,9 @@ static int init_kernel_attrs() {
   TRY((set_gemm_attr<64, EpiBiasF16<true>, true>()));
   CUDA_TRY(cudaFuncSetAttribute(gemm_resid_ln_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmLnSmem::TOTAL));
   TRY((set_gemm_attr<128, EpiEmbed>()));
-  TRY((set_gemm_attr<96, EpiOutStep>()));
-  TRY((set_gemm_attr<96, EpiOutPlms>()));
-  TRY((set_gemm_attr<96, EpiOutReverse>()));
+  TRY((set_gemm_attr<96, EpiOut<OutStep>>()));
+  TRY((set_gemm_attr<96, EpiOut<OutPlms>>()));
+  TRY((set_gemm_attr<96, EpiOut<OutReverse>>()));
   TRY((set_attention_attr<64>()));
   TRY((set_attention_attr<208>()));
   TRY((set_attention_attr<256>()));
@@ -827,6 +827,9 @@ extern "C" int b200mdm_set_schedule(b200mdm_engine* e, int32_t n_steps, const fl
 }
 
 static_assert(SCHED_NEXT_STRIDE == B200MDM_SCHED_NEXT_STRIDE, "the reverse table's row layout is part of the ABI");
+static_assert(MODE_X0 == B200MDM_MODE_X0 && MODE_DDPM == B200MDM_MODE_DDPM && MODE_DDIM == B200MDM_MODE_DDIM &&
+                  MODE_DDIM_REVERSE == B200MDM_MODE_DDIM_REVERSE,
+              "the output epilogue's modes are the public ones");
 extern "C" int b200mdm_set_schedule_next(b200mdm_engine* e, int32_t n_steps, const float* rows_host) {
   if (!e || !rows_host) return fail(B200MDM_EINVAL, "bad argument");
   if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
@@ -1118,9 +1121,29 @@ struct StepArgs {
   bool explicit_t = false;        // use e->tvec instead of timestep_map[state.cur]
   bool philox = false;            // eps of this step is generated into e->eps_buf by the first kernel of the step
   int back = 0;                   // evaluate schedule index cur - back (PLMS improved Euler, second forward: 1)
-  const float* x_step = nullptr;  // PLMS mode 5: x_t of the step
-  int order = 0;                  // PLMS mode 3
+  const float* x_step = nullptr;  // MODE_PLMS_EULER2: x_t of the step
+  int order = 0;                  // MODE_PLMS_AB
 };
+
+// The output projection of the CFG-blended g16 rows with the update of a.mode fused into its epilogue (p: the tables,
+// the step state and the inpainting inputs), launched on the mode's GEMM instantiation.
+static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, int B, int T, int JF, int d,
+                           const StepArgs& a, EpiOutParams p, cudaStream_t s, int sms) {
+  p.x_t = a.x_in;
+  p.noise = a.noise;
+  p.x_out = a.x_out;
+  p.pred_xstart = a.pred;
+  p.x_step = a.x_step;
+  p.noise_batch_stride = a.const_noise ? 0 : static_cast<long long>(JF) * T;
+  p.B = B; p.T = T; p.J = JF; p.mode = a.mode;
+  p.clip_denoised = a.clip;
+  p.order = a.order;
+  p.back = a.back;
+  const int M = B * T, N = ((JF + 95) / 96) * 96, K = 3 * d;
+  if (a.mode <= MODE_DDIM) return launch_gemm<96, EpiOut<OutStep>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
+  if (a.mode == MODE_DDIM_REVERSE) return launch_gemm<96, EpiOut<OutReverse>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
+  return launch_gemm<96, EpiOut<OutPlms>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
+}
 
 // Enqueue one denoiser forward (+ fused sampler step) on stream s.  Returns the number of kernels launched.
 static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s, int* n_kernels) {
@@ -1209,35 +1232,15 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
                     e->halves));
   ++nk;
   {
-    EpiOutPlms::Params p;   // EpiOutStep's parameters + the PLMS fields
+    EpiOutParams p{};
     p.bias = e->b_out;
-    p.x_t = a.x_in;
-    p.noise = a.noise;
-    p.x_out = a.x_out;
-    p.pred_xstart = a.pred;
     p.inpaint_mask = e->inpaint_mask;
     p.inpaint_motion = e->inpaint_motion;
     p.sched = e->sched;
+    p.sched_next = e->sched_next;
+    p.eps_ring = e->plms_ring;
     p.state = e->state;
-    p.noise_batch_stride = a.const_noise ? 0 : static_cast<long long>(JF) * T;
-    p.B = B; p.S = T; p.T = T; p.J = JF; p.mode = a.mode;      // g16 rows are frames: row = b*T + t
-    p.s_off = 0;
-    p.clip_denoised = a.clip;
-    if (a.mode <= B200MDM_MODE_DDIM) {
-      const EpiOutStep::Params& ps = p;
-      TRY((launch_gemm<96, EpiOutStep>(e->m_g16, e->m_wout, e->m_g16, B * T, e->N_out_pad, 3 * d, ps, s, e->num_sms)));
-    } else if (a.mode == B200MDM_MODE_DDIM_REVERSE) {
-      EpiOutReverse::Params pr;
-      static_cast<EpiOutStep::Params&>(pr) = p;
-      pr.sched_next = e->sched_next;
-      TRY((launch_gemm<96, EpiOutReverse>(e->m_g16, e->m_wout, e->m_g16, B * T, e->N_out_pad, 3 * d, pr, s, e->num_sms)));
-    } else {
-      p.eps_ring = e->plms_ring;
-      p.x_step = a.x_step;
-      p.order = a.order;
-      p.back = a.back;
-      TRY((launch_gemm<96, EpiOutPlms>(e->m_g16, e->m_wout, e->m_g16, B * T, e->N_out_pad, 3 * d, p, s, e->num_sms)));
-    }
+    TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, a, p, s, e->num_sms));
     ++nk;
   }
   *n_kernels = nk;
@@ -1306,8 +1309,7 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
 // Move the step state to the next step of the loop: down the schedule, or up it for the DDIM inversion.
 static cudaError_t launch_advance(b200mdm_engine* e, const StepArgs& a, cudaStream_t s) {
   PdlScope pdl_scope;
-  if (a.mode == B200MDM_MODE_DDIM_REVERSE) return launch_k(step_advance_up_kernel, dim3(1), dim3(1), 0, s, e->state);
-  return launch_k(step_advance_kernel, dim3(1), dim3(1), 0, s, e->state);
+  return launch_k(step_advance_kernel, dim3(1), dim3(1), 0, s, e->state, a.mode == MODE_DDIM_REVERSE ? 1 : -1);
 }
 
 // Make the workspace's step graph (one forward + step_advance, captured on the engine stream) the graph of `key`.
@@ -1351,11 +1353,35 @@ static int enqueue_step(b200mdm_engine* e, const StepArgs& a, cudaStream_t s, bo
   return B200MDM_OK;
 }
 
-// n_run steps of `a` from schedule index first_index on the engine's working buffer (a.x_in == a.x_out == x_work).
-// x_in_dev == NULL continues from the state the previous call left there; x_out_dev == NULL leaves the result there.
+// The pseudo improved-Euler step (gaussian_diffusion.py:1042-1049) at the schedule index the step state holds:
+// forward 1 at (x_t, i) leaves eps0 in the ring, x0 in plms_pred and mean1 in plms_mid; forward 2 at (mean1, i - 1)
+// writes the sample to x_out.  Then the step state advances.
+static int enqueue_plms_euler(b200mdm_engine* e, const StepArgs& base, const float* x_t, float* x_out, cudaStream_t s) {
+  StepArgs a = base;
+  a.mode = MODE_PLMS_EULER1;
+  a.x_in = x_t;
+  a.x_out = e->plms_mid;
+  a.pred = e->plms_pred;
+  int nk1 = 0, nk2 = 0;
+  TRY(enqueue_forward(e, a, s, &nk1));
+  a.mode = MODE_PLMS_EULER2;
+  a.x_in = e->plms_mid;
+  a.x_step = x_t;
+  a.x_out = x_out;
+  a.back = 1;
+  TRY(enqueue_forward(e, a, s, &nk2));
+  CUDA_TRY(launch_advance(e, a, s));
+  e->launches += nk1 + nk2 + 1;
+  return B200MDM_OK;
+}
+
+// n_run steps of `a` from schedule index first_index on the engine's working buffer (a.x_in == a.x_out == x_work), with
+// the step counter starting at `done`; plms_euler: the first step is the PLMS improved-Euler step (two forwards, never
+// a graph), the rest are steps of `a`.  x_in_dev == NULL continues from the state the previous call left there;
+// x_out_dev == NULL leaves the result there.
 static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t first_index, int32_t n_run,
                     const float* x_in_dev, float* x_out_dev, const float* noise_tape_dev, int64_t noise_step_stride,
-                    int32_t use_graph, void* stream) {
+                    int32_t use_graph, void* stream, int done = 0, bool plms_euler = false) {
   cudaStream_t user = static_cast<cudaStream_t>(stream);
   const size_t x_bytes = static_cast<size_t>(e->B) * e->JF * e->T * sizeof(float);
   // The graph path runs on the engine's own stream (the caller's may be the legacy default stream, which cannot be
@@ -1364,7 +1390,7 @@ static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t
   if (!use_graph) attach_l2_window(e, user);   // plain launches: the residual-stream window goes on the caller's stream
   if (use_graph) {
     GraphKey key;
-    key.mode = a.mode; key.B = e->B; key.T = e->T; key.flags = flags;
+    key.mode = a.mode; key.B = e->B; key.T = e->T; key.flags = flags; key.order = a.order;
     key.imask = e->inpaint_mask; key.imotion = e->inpaint_motion;
     key.target_g = e->target_set ? e->tgt_g : nullptr;
     TRY(ensure_step_graph(e, key, a));
@@ -1373,11 +1399,20 @@ static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t
   }
   e->plms_done = -1;   // x_work no longer holds a PLMS loop to continue
   if (x_in_dev) CUDA_TRY(cudaMemcpyAsync(e->x_work, x_in_dev, x_bytes, cudaMemcpyDeviceToDevice, s));
-  step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, first_index, noise_tape_dev, noise_step_stride, e->noise_seed, e->noise_sample_base,
-                                  e->n_steps);
+  step_set_kernel<<<1, 1, 0, s>>>(e->state, done, first_index, noise_tape_dev, noise_step_stride, e->noise_seed,
+                                  e->noise_sample_base, e->n_steps);
   CUDA_TRY(cudaGetLastError());
   e->launches += 1;
-  for (int k = 0; k < n_run; ++k) TRY(enqueue_step(e, a, s, use_graph));
+  int k = 0;
+  if (plms_euler) {
+    TRY(enqueue_plms_euler(e, a, e->x_work, e->x_work, s));
+    k = 1;
+  }
+  for (; k < n_run; ++k) TRY(enqueue_step(e, a, s, use_graph));
+  if (a.mode == MODE_PLMS_AB) {
+    e->plms_done = done + n_run;
+    e->plms_order = a.order;
+  }
   if (x_out_dev) CUDA_TRY(cudaMemcpyAsync(x_out_dev, e->x_work, x_bytes, cudaMemcpyDeviceToDevice, s));
   if (use_graph) {
     CUDA_TRY(cudaEventRecord(e->ev_out, e->work));
@@ -1452,31 +1487,6 @@ static int ensure_plms(b200mdm_engine* e) {
   return r;
 }
 
-// The pseudo improved-Euler step (gaussian_diffusion.py:1042-1049) at the schedule index the step state holds:
-// forward 1 at (x_t, i) leaves eps0 in the ring, x0 in plms_pred and mean1 in plms_mid; forward 2 at (mean1, i - 1)
-// writes the sample to x_out.  Then the step state advances.
-static int enqueue_plms_euler(b200mdm_engine* e, const StepArgs& base, const float* x_t, float* x_out, cudaStream_t s) {
-  StepArgs a = base;
-  a.mode = 4;
-  a.x_in = x_t;
-  a.x_out = e->plms_mid;
-  a.pred = e->plms_pred;
-  int nk1 = 0, nk2 = 0;
-  TRY(enqueue_forward(e, a, s, &nk1));
-  a.mode = 5;
-  a.x_in = e->plms_mid;
-  a.x_step = x_t;
-  a.x_out = x_out;
-  a.back = 1;
-  TRY(enqueue_forward(e, a, s, &nk2));
-  {
-    PdlScope pdl_scope;
-    CUDA_TRY(launch_k(step_advance_kernel, dim3(1), dim3(1), 0, s, e->state));
-  }
-  e->launches += nk1 + nk2 + 1;
-  return B200MDM_OK;
-}
-
 extern "C" int b200mdm_plms_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index, int32_t n_run,
                                        const float* x_in_dev, float* x_out_dev, int32_t flags, int32_t use_graph,
                                        void* stream) {
@@ -1490,45 +1500,15 @@ extern "C" int b200mdm_plms_loop_range(b200mdm_engine* e, int32_t order, int32_t
   if (!x_in_dev && (e->plms_done < 0 || e->plms_order != order))
     return fail(B200MDM_ESTATE, "no PLMS loop of order %d to continue (pass x_in_dev)", order);
   TRY(ensure_plms(e));
-  cudaStream_t user = static_cast<cudaStream_t>(stream);
-  const size_t x_bytes = static_cast<size_t>(e->B) * e->JF * e->T * sizeof(float);
+  // every step after the improved-Euler one is an Adams-Bashforth step: the launches of a DDIM step, one graph per order
   StepArgs a;
-  a.mode = 3;
+  a.mode = MODE_PLMS_AB;
   a.order = order;
   a.x_in = e->x_work;
   a.x_out = e->x_work;
   a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-  cudaStream_t s = use_graph ? e->work : user;
-  if (!use_graph) attach_l2_window(e, user);
-  if (use_graph) {
-    // the Adams-Bashforth step: the same launches as a DDIM step, one graph for every order-`order` step
-    GraphKey key;
-    key.mode = a.mode; key.B = e->B; key.T = e->T; key.flags = flags; key.order = order;
-    key.imask = e->inpaint_mask; key.imotion = e->inpaint_motion;
-    key.target_g = e->target_set ? e->tgt_g : nullptr;
-    TRY(ensure_step_graph(e, key, a));
-    CUDA_TRY(cudaEventRecord(e->ev_in, user));
-    CUDA_TRY(cudaStreamWaitEvent(e->work, e->ev_in, 0));
-  }
   const int done = x_in_dev ? 0 : e->plms_done;
-  if (x_in_dev) CUDA_TRY(cudaMemcpyAsync(e->x_work, x_in_dev, x_bytes, cudaMemcpyDeviceToDevice, s));
-  step_set_kernel<<<1, 1, 0, s>>>(e->state, done, first_index, nullptr, 0, e->noise_seed, e->noise_sample_base, e->n_steps);
-  CUDA_TRY(cudaGetLastError());
-  e->launches += 1;
-  int k = 0;
-  if (done == 0) {
-    TRY(enqueue_plms_euler(e, a, e->x_work, e->x_work, s));
-    k = 1;
-  }
-  for (; k < n_run; ++k) TRY(enqueue_step(e, a, s, use_graph));
-  e->plms_done = done + n_run;
-  e->plms_order = order;
-  if (x_out_dev) CUDA_TRY(cudaMemcpyAsync(x_out_dev, e->x_work, x_bytes, cudaMemcpyDeviceToDevice, s));
-  if (use_graph) {
-    CUDA_TRY(cudaEventRecord(e->ev_out, e->work));
-    CUDA_TRY(cudaStreamWaitEvent(user, e->ev_out, 0));
-  }
-  return B200MDM_OK;
+  return run_loop(e, a, flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0, use_graph, stream, done, done == 0);
 }
 
 extern "C" int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order, const float* x_t_dev,
@@ -1566,7 +1546,7 @@ extern "C" int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order
     TRY(enqueue_plms_euler(e, a, x_t_dev, x_out_dev, s));
     if (pred_xstart_dev) CUDA_TRY(cudaMemcpyAsync(pred_xstart_dev, e->plms_pred, x_bytes, cudaMemcpyDeviceToDevice, s));
   } else {
-    a.mode = 3;
+    a.mode = MODE_PLMS_AB;
     a.x_in = x_t_dev;
     a.x_out = x_out_dev;
     a.pred = pred_xstart_dev;
@@ -1768,21 +1748,21 @@ extern "C" int b200mdm_test_out_step(const void* hres16_dev, const float* scale_
   CUtensorMap m_g16, m_wout;
   TRY(make_map(&m_g16, g16, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
   TRY(make_map(&m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
-  EpiOutStep::Params p;
+  EpiOutParams p{};
   p.bias = b_out_dev;
-  p.x_t = x_t_dev;
-  p.noise = noise_dev;
-  p.x_out = x_out_dev;
-  p.pred_xstart = pred_xstart_dev;
   p.inpaint_mask = inpaint_mask_dev;
   p.inpaint_motion = inpaint_motion_dev;
   p.sched = sched_row_dev;
   p.state = st;
-  p.noise_batch_stride = (flags & B200MDM_FLAG_CONST_NOISE) ? 0 : static_cast<long long>(JF) * T;
-  p.B = B; p.S = T; p.T = T; p.J = JF; p.mode = mode;      // g16 rows are frames: row = b*T + t
-  p.s_off = 0;
-  p.clip_denoised = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-  return launch_gemm<96, EpiOutStep>(m_g16, m_wout, m_g16, B * T, N_out_pad, 3 * d, p, s, sms);
+  StepArgs a;
+  a.mode = mode;
+  a.x_in = x_t_dev;
+  a.noise = noise_dev;
+  a.const_noise = flags & B200MDM_FLAG_CONST_NOISE;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  a.x_out = x_out_dev;
+  a.pred = pred_xstart_dev;
+  return launch_out_gemm(m_g16, m_wout, B, T, JF, d, a, p, s, sms);
 }
 
 extern "C" int b200mdm_test_attention(const void* qkv16_dev, void* out16_dev, const int32_t* kvlen_dev,

@@ -283,9 +283,11 @@ struct EpiEmbed {
 };
 
 // ---------------------------------------------------------------------------------------------------------
-// OutputProcess + (inpainting) + sampler arithmetic fused (reference model/mdm.py:372-386,
-// diffusion/gaussian_diffusion.py:300-304, 254-257, 525-540, 757-778).  GEMM rows are (b, s) over B*S; row s>=1
-// is frame t = s-1; column j < J is a feature.  All tensors are the reference layout [B, J*F, T].
+// OutputProcess + (inpainting) + sampler update fused (reference model/mdm.py:372-386,
+// diffusion/gaussian_diffusion.py:300-304, 254-257, 525-540, 757-778, 838-874, 992-1074).  GEMM rows are frames:
+// row = b*T + t; column j < J is a feature.  All tensors are the reference layout [B, J*F, T].
+// x0 = acc + bias, then the inpainting blend, then the clamp; then the update of `mode`, in fp32 in the reference's
+// operation order with no contraction (bit-exact):
 //   mode 0: out = x0                       (model forward only)
 //   mode 1: DDPM   x_{t-1} = c1*x0 + c2*x_t + (nz*sigma)*eps
 //   mode 2: DDIM   eps_hat = (sr*x_t - x0)/srm1 ; x_{t-1} = x0*sqrt_abp + coef*eps_hat + (nz*sigma)*eps
@@ -298,14 +300,21 @@ struct EpiEmbed {
 //   mode 5: improved Euler, second evaluation, of x_t = mean1 at schedule index i - 1 (`back` = 1): eps2 from the row
 //           of i - 1; eps' = (ring[k] + eps2)/2; pred' from x_step (the step's x_t) and the row of i; the sample as
 //           in mode 3 with x0 = pred_xstart (the first evaluation's)
+// DDIM inversion (ddim_reverse_sample, gaussian_diffusion.py:838-874): x at schedule index i -> x at index i + 1
+//   mode 6: eps = (sr*x - x0)/srm1 (row i of sched); x_next = x0*sqrt(abn) + sqrt(1 - abn)*eps (row i of sched_next)
 // Per-step scalars come from a device table indexed by the device-side step state, so the very same launch
 // (and CUDA graph) serves every step of the loop.
-constexpr int SCHED_STRIDE = 8;  // floats per schedule row: c1 c2 sig_ddpm sr srm1 sqrt_abp coef_eps sig_ddim
-constexpr int PLMS_RING = 3;     // eps history slots: AB4 combines this step's eps with the three before it
+constexpr int SCHED_STRIDE = 8;       // floats per schedule row: c1 c2 sig_ddpm sr srm1 sqrt_abp coef_eps sig_ddim
+constexpr int SCHED_NEXT_STRIDE = 2;  // floats per row of the reverse table: sqrt(abn) sqrt(1 - abn)
+constexpr int PLMS_RING = 3;          // eps history slots: AB4 combines this step's eps with the three before it
+enum OutMode : int {
+  MODE_X0 = 0, MODE_DDPM = 1, MODE_DDIM = 2,                      // B200MDM_MODE_*
+  MODE_PLMS_AB = 3, MODE_PLMS_EULER1 = 4, MODE_PLMS_EULER2 = 5,   // internal: the steps of the PLMS loop
+  MODE_DDIM_REVERSE = 6,                                          // B200MDM_MODE_DDIM_REVERSE
+};
 struct StepState {
   int done;      // steps completed so far (indexes the noise tape; PLMS: the evaluation count k)
   int cur;       // schedule index i of the step in flight
-  int start;     // schedule index of the first step (num_timesteps - 1 - skip)
   int n_steps;   // schedule length (index i - 1 of the PLMS improved-Euler step wraps to n_steps - 1 at i = 0)
   const float* noise;            // loop mode: base of the noise tape (set per loop, so the step graph is reusable)
   long long noise_step_stride;   // loop mode: elements between consecutive steps of the tape
@@ -320,213 +329,175 @@ __device__ __forceinline__ int eval_index(const StepState& st, int back) {
   return i < 0 ? i + st.n_steps : i;
 }
 
-struct EpiOutStep {
-  static constexpr int SMEM_PER_WARP = 1024;  // unused
-  template <class P> static __device__ __forceinline__ void preload(const P&, float*, int, int, int) {}
-  struct Params {
-    const float* bias;        // [J]
-    const float* x_t;         // [B, J, T]
-    const float* noise;       // explicit eps for one step; nullptr => tape described by *state (loop mode)
-    float* x_out;             // [B, J, T]
-    float* pred_xstart;       // nullable
-    const unsigned char* inpaint_mask;  // nullable, bool [B, J, T]
-    const float* inpaint_motion;        // [B, J, T]
-    const float* sched;       // [n_steps, SCHED_STRIDE]
-    const StepState* state;
-    long long noise_batch_stride;  // J*T normally, 0 for const_noise
-    int B, S, T, J, mode;
-    int s_off;                // rows s < s_off of a sequence are not frames of x (cond token / DiP prefix); t = s - s_off
-    int clip_denoised;        // clamp x0 to [-1, 1] after the inpainting blend (gaussian_diffusion.py:348-352)
-  };
-  static __device__ __forceinline__ void tile_begin(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0,
-                                               int) {
-    const int row = row0 + ctx.lane;
-    if (row >= ctx.M) return;
-    const int b = row / p.S, s = row - b * p.S;
-    if (s < p.s_off) return;
-    const int t = s - p.s_off;
-    float c1 = 0.f, c2 = 0.f, sg = 0.f, sr = 0.f, srm1 = 1.f, sq = 0.f, ce = 0.f;
-    const float* nz = nullptr;
-    if (p.mode != 0) {
-      const StepState st = *p.state;
-      const float* row_s = p.sched + static_cast<size_t>(st.cur) * SCHED_STRIDE;
-      c1 = row_s[0]; c2 = row_s[1]; sr = row_s[3]; srm1 = row_s[4]; sq = row_s[5]; ce = row_s[6];
-      sg = (p.mode == 1) ? row_s[2] : row_s[7];
-      nz = (p.noise != nullptr ? p.noise : st.noise + static_cast<long long>(st.done) * st.noise_step_stride) +
-           static_cast<long long>(b) * p.noise_batch_stride;
-    }
-    // x_out may alias x_t (in-place loop): batch every load of the chunk before the first store so that they are
-    // all in flight together (consecutive lanes = consecutive frames => each load/store is one coalesced line)
-    const size_t base = static_cast<size_t>(b) * p.J * p.T + t;
-#pragma unroll
-    for (int h = 0; h < 32; h += 16) {
-      float xv[16], nv[16];
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int col = col0 + h + j;
-        xv[j] = (p.mode != 0 && col < p.J) ? p.x_t[base + static_cast<size_t>(col) * p.T] : 0.f;
-        nv[j] = (p.mode != 0 && col < p.J) ? nz[static_cast<size_t>(col) * p.T + t] : 0.f;
-      }
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int col = col0 + h + j;
-        if (col < p.J) {
-          const size_t idx = base + static_cast<size_t>(col) * p.T;
-          float x0 = __uint_as_float(raw[h + j]) + __ldg(p.bias + col);
-          if (p.inpaint_mask != nullptr && p.inpaint_mask[idx]) x0 = p.inpaint_motion[idx];
-          if (p.clip_denoised) x0 = fminf(fmaxf(x0, -1.f), 1.f);
-          if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
-          float o = x0;
-          if (p.mode == 1) {
-            const float mean = __fadd_rn(__fmul_rn(c1, x0), __fmul_rn(c2, xv[j]));
-            o = __fadd_rn(mean, __fmul_rn(sg, nv[j]));
-          } else if (p.mode == 2) {
-            const float eh = __fdiv_rn(__fsub_rn(__fmul_rn(sr, xv[j]), x0), srm1);
-            const float mean = __fadd_rn(__fmul_rn(x0, sq), __fmul_rn(ce, eh));
-            o = __fadd_rn(mean, __fmul_rn(sg, nv[j]));
-          }
-          p.x_out[idx] = o;
-        }
-      }
-    }
-  }
-
-  static __device__ __forceinline__ void tile_end(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void finish(EpiCtx&) {}
+struct EpiOutParams {
+  const float* bias;        // [J]
+  const float* x_t;         // [B, J, T]
+  const float* noise;       // modes 1-2: explicit eps for one step; nullptr => tape described by *state (loop mode)
+  float* x_out;             // [B, J, T]
+  float* pred_xstart;       // nullable, except in modes 4 and 5
+  const unsigned char* inpaint_mask;  // nullable, bool [B, J, T]
+  const float* inpaint_motion;        // [B, J, T]
+  const float* sched;       // [n_steps, SCHED_STRIDE]
+  const float* sched_next;  // mode 6: [n_steps, SCHED_NEXT_STRIDE]
+  float* eps_ring;          // modes 3-5: [PLMS_RING, B, J, T]
+  const float* x_step;      // mode 5: x_t of the step (x_t above is mean1 there)
+  const StepState* state;
+  long long noise_batch_stride;  // J*T normally, 0 for const_noise
+  int B, T, J, mode;
+  int clip_denoised;        // clamp x0 to [-1, 1] after the inpainting blend (gaussian_diffusion.py:348-352)
+  int order;                // mode 3: 1..4
+  int back;                 // modes 3-5: this forward evaluates schedule index eval_index(state, back)
 };
 
-// EpiOutStep's PLMS modes 3-5 (a GEMM kernel of their own: the DDPM / DDIM kernel stays as it was), in the reference's
-// operation order with no contraction (bit-exact fp32).  x_out, x_t, x_step and the ring slots may alias one another
-// across steps: every load of a chunk is issued before its first store, and an element is only ever read and written by
-// the thread that owns it.
-struct EpiOutPlms : EpiOutStep {
-  struct Params : EpiOutStep::Params {
-    float* eps_ring;          // [PLMS_RING, B, J, T]
-    const float* x_step;      // mode 5: x_t of the step (x_t above is mean1 there)
-    int order;                // mode 3: 1..4
-    int back;                 // this forward evaluates schedule index eval_index(state, back)
-  };
-  static __device__ __forceinline__ void tile_begin(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0,
-                                               int) {
-    const int row = row0 + ctx.lane;
-    if (row >= ctx.M) return;
-    const int b = row / p.S, s = row - b * p.S;
-    if (s < p.s_off) return;
-    const int t = s - p.s_off;
+// The update policies of EpiOut: the constructor reads the chunk's scalars, load() the extra inputs of one element
+// (In), store() writes its outputs from x0.
+struct OutStep {   // modes 0-2
+  float c1 = 0.f, c2 = 0.f, sg = 0.f, sr = 0.f, srm1 = 1.f, sq = 0.f, ce = 0.f;
+  const float* nz = nullptr;
+  struct In { float x, n; };
+  __device__ __forceinline__ OutStep(const EpiOutParams& p, int b) {
+    if (p.mode == MODE_X0) return;
+    const StepState st = *p.state;
+    const float* row_s = p.sched + static_cast<size_t>(st.cur) * SCHED_STRIDE;
+    c1 = row_s[0]; c2 = row_s[1]; sr = row_s[3]; srm1 = row_s[4]; sq = row_s[5]; ce = row_s[6];
+    sg = (p.mode == MODE_DDPM) ? row_s[2] : row_s[7];
+    nz = (p.noise != nullptr ? p.noise : st.noise + static_cast<long long>(st.done) * st.noise_step_stride) +
+         static_cast<long long>(b) * p.noise_batch_stride;
+  }
+  __device__ __forceinline__ In load(const EpiOutParams& p, bool in, size_t idx, int col, int t) const {
+    in = in && p.mode != MODE_X0;
+    return {in ? p.x_t[idx] : 0.f, in ? nz[static_cast<size_t>(col) * p.T + t] : 0.f};
+  }
+  __device__ __forceinline__ void store(const EpiOutParams& p, size_t idx, float x0, const In& v) const {
+    if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
+    float o = x0;
+    if (p.mode == MODE_DDPM) {
+      const float mean = __fadd_rn(__fmul_rn(c1, x0), __fmul_rn(c2, v.x));
+      o = __fadd_rn(mean, __fmul_rn(sg, v.n));
+    } else if (p.mode == MODE_DDIM) {
+      const float eh = __fdiv_rn(__fsub_rn(__fmul_rn(sr, v.x), x0), srm1);
+      const float mean = __fadd_rn(__fmul_rn(x0, sq), __fmul_rn(ce, eh));
+      o = __fadd_rn(mean, __fmul_rn(sg, v.n));
+    }
+    p.x_out[idx] = o;
+  }
+};
+
+struct OutPlms {   // modes 3-5
+  float sr, srm1, sq, s1, sr_e, srm1_e, nzf;
+  int cur_order;
+  const float *h1, *h2, *h3;
+  float* own;
+  // mode 3: e1..e3 = eps of evaluations k-1..k-3;  mode 5: e1 = eps0, e2 = x_step, e3 = x0 of the first evaluation
+  struct In { float x, e1, e2, e3; };
+  __device__ __forceinline__ OutPlms(const EpiOutParams& p, int) {
     const StepState st = *p.state;
     const int k = st.done;
     const float* row_s = p.sched + static_cast<size_t>(st.cur) * SCHED_STRIDE;
     const float* row_e = p.sched + static_cast<size_t>(eval_index(st, p.back)) * SCHED_STRIDE;
-    const float sr = row_s[3], srm1 = row_s[4], sq = row_s[5], s1 = row_s[6];
-    const float sr_e = row_e[3], srm1_e = row_e[4];
-    const float nzf = st.cur != 0 ? 1.f : 0.f;                  // (t != 0), gaussian_diffusion.py:1071
-    const int cur_order = min(p.order, k + 1);
+    sr = row_s[3]; srm1 = row_s[4]; sq = row_s[5]; s1 = row_s[6];
+    sr_e = row_e[3]; srm1_e = row_e[4];
+    nzf = st.cur != 0 ? 1.f : 0.f;                  // (t != 0), gaussian_diffusion.py:1071
+    cur_order = min(p.order, k + 1);
     const size_t slot = static_cast<size_t>(p.B) * p.J * p.T;
-    const float* h1 = p.eps_ring + static_cast<size_t>((k + PLMS_RING - 1) % PLMS_RING) * slot;
-    const float* h2 = p.eps_ring + static_cast<size_t>((k + PLMS_RING - 2) % PLMS_RING) * slot;
-    const float* h3 = p.eps_ring + static_cast<size_t>(k % PLMS_RING) * slot;   // k - 3
-    float* own = p.eps_ring + static_cast<size_t>(k % PLMS_RING) * slot;
-    const size_t base = static_cast<size_t>(b) * p.J * p.T + t;
-#pragma unroll
-    for (int h = 0; h < 32; h += 16) {
-      // mode 3: e1..e3 = eps of evaluations k-1..k-3;  mode 5: e1 = eps0, e2 = x_step, e3 = x0 of the first evaluation
-      float xv[16], e1[16], e2[16], e3[16];
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int col = col0 + h + j;
-        const size_t idx = base + static_cast<size_t>(col) * p.T;
-        const bool in = col < p.J;
-        xv[j] = in ? p.x_t[idx] : 0.f;
-        e1[j] = e2[j] = e3[j] = 0.f;
-        if (in && p.mode == 3) {
-          if (cur_order >= 2) e1[j] = h1[idx];
-          if (cur_order >= 3) e2[j] = h2[idx];
-          if (cur_order >= 4) e3[j] = h3[idx];
-        } else if (in && p.mode == 5) {
-          e1[j] = own[idx];
-          e2[j] = p.x_step[idx];
-          e3[j] = p.pred_xstart[idx];
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int col = col0 + h + j;
-        if (col >= p.J) continue;
-        const size_t idx = base + static_cast<size_t>(col) * p.T;
-        float x0 = __uint_as_float(raw[h + j]) + __ldg(p.bias + col);
-        if (p.inpaint_mask != nullptr && p.inpaint_mask[idx]) x0 = p.inpaint_motion[idx];
-        if (p.clip_denoised) x0 = fminf(fmaxf(x0, -1.f), 1.f);
-        // _predict_eps_from_xstart (gaussian_diffusion.py:400-404) at the index this forward evaluates
-        const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sr_e, xv[j]), x0), srm1_e);
-        if (p.mode == 4) {
-          own[idx] = eps;
-          p.pred_xstart[idx] = x0;
-          p.x_out[idx] = __fadd_rn(__fmul_rn(x0, sq), __fmul_rn(s1, eps));   // :1045
-          continue;
-        }
-        float ep, x_t = xv[j], x0s = x0;
-        if (p.mode == 5) {
-          ep = __fdiv_rn(__fadd_rn(e1[j], eps), 2.f);                          // :1047
-          x_t = e2[j];
-          x0s = e3[j];
-        } else {
-          if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
-          if (cur_order == 1) {                                                // :1055-1062
-            ep = eps;
-          } else if (cur_order == 2) {
-            ep = __fdiv_rn(__fsub_rn(__fmul_rn(3.f, eps), e1[j]), 2.f);
-          } else if (cur_order == 3) {
-            ep = __fdiv_rn(__fadd_rn(__fsub_rn(__fmul_rn(23.f, eps), __fmul_rn(16.f, e1[j])), __fmul_rn(5.f, e2[j])), 12.f);
-          } else {
-            ep = __fdiv_rn(__fsub_rn(__fadd_rn(__fsub_rn(__fmul_rn(55.f, eps), __fmul_rn(59.f, e1[j])), __fmul_rn(37.f, e2[j])),
-                                     __fmul_rn(9.f, e3[j])),
-                           24.f);
-          }
-          own[idx] = eps;                                                      // replaces evaluation k - 3
-        }
-        // _predict_xstart_from_eps (:381-388), then the mean and the (t != 0) blend (:1065-1072)
-        const float pp = __fsub_rn(__fmul_rn(sr, x_t), __fmul_rn(srm1, ep));
-        const float mean = __fadd_rn(__fmul_rn(pp, sq), __fmul_rn(s1, ep));
-        p.x_out[idx] = __fadd_rn(__fmul_rn(mean, nzf), __fmul_rn(x0s, __fsub_rn(1.f, nzf)));
-      }
-    }
+    h1 = p.eps_ring + static_cast<size_t>((k + PLMS_RING - 1) % PLMS_RING) * slot;
+    h2 = p.eps_ring + static_cast<size_t>((k + PLMS_RING - 2) % PLMS_RING) * slot;
+    h3 = p.eps_ring + static_cast<size_t>(k % PLMS_RING) * slot;   // k - 3
+    own = p.eps_ring + static_cast<size_t>(k % PLMS_RING) * slot;
   }
-  static __device__ __forceinline__ void tile_end(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void finish(EpiCtx&) {}
+  __device__ __forceinline__ In load(const EpiOutParams& p, bool in, size_t idx, int, int) const {
+    In v{in ? p.x_t[idx] : 0.f, 0.f, 0.f, 0.f};
+    if (in && p.mode == MODE_PLMS_AB) {
+      if (cur_order >= 2) v.e1 = h1[idx];
+      if (cur_order >= 3) v.e2 = h2[idx];
+      if (cur_order >= 4) v.e3 = h3[idx];
+    } else if (in && p.mode == MODE_PLMS_EULER2) {
+      v.e1 = own[idx];
+      v.e2 = p.x_step[idx];
+      v.e3 = p.pred_xstart[idx];
+    }
+    return v;
+  }
+  __device__ __forceinline__ void store(const EpiOutParams& p, size_t idx, float x0, const In& v) const {
+    // _predict_eps_from_xstart (gaussian_diffusion.py:400-404) at the index this forward evaluates
+    const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sr_e, v.x), x0), srm1_e);
+    if (p.mode == MODE_PLMS_EULER1) {
+      own[idx] = eps;
+      p.pred_xstart[idx] = x0;
+      p.x_out[idx] = __fadd_rn(__fmul_rn(x0, sq), __fmul_rn(s1, eps));   // :1045
+      return;
+    }
+    float ep, x_t = v.x, x0s = x0;
+    if (p.mode == MODE_PLMS_EULER2) {
+      ep = __fdiv_rn(__fadd_rn(v.e1, eps), 2.f);                          // :1047
+      x_t = v.e2;
+      x0s = v.e3;
+    } else {
+      if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
+      if (cur_order == 1) {                                               // :1055-1062
+        ep = eps;
+      } else if (cur_order == 2) {
+        ep = __fdiv_rn(__fsub_rn(__fmul_rn(3.f, eps), v.e1), 2.f);
+      } else if (cur_order == 3) {
+        ep = __fdiv_rn(__fadd_rn(__fsub_rn(__fmul_rn(23.f, eps), __fmul_rn(16.f, v.e1)), __fmul_rn(5.f, v.e2)), 12.f);
+      } else {
+        ep = __fdiv_rn(__fsub_rn(__fadd_rn(__fsub_rn(__fmul_rn(55.f, eps), __fmul_rn(59.f, v.e1)), __fmul_rn(37.f, v.e2)),
+                                 __fmul_rn(9.f, v.e3)),
+                       24.f);
+      }
+      own[idx] = eps;                                                     // replaces evaluation k - 3
+    }
+    // _predict_xstart_from_eps (:381-388), then the mean and the (t != 0) blend (:1065-1072)
+    const float pp = __fsub_rn(__fmul_rn(sr, x_t), __fmul_rn(srm1, ep));
+    const float mean = __fadd_rn(__fmul_rn(pp, sq), __fmul_rn(s1, ep));
+    p.x_out[idx] = __fadd_rn(__fmul_rn(mean, nzf), __fmul_rn(x0s, __fsub_rn(1.f, nzf)));
+  }
 };
 
-// ddim_reverse_sample (gaussian_diffusion.py:838-874), mode 6 (a GEMM kernel of its own, as EpiOutPlms): x at schedule
-// index i -> x at index i + 1 along the deterministic DDIM ODE.
-//   eps = (sr*x - x0)/srm1 (row i of sched); x_next = x0*sqrt(abn) + sqrt(1 - abn)*eps (row i of sched_next)
-// fp32, unfused, in the reference's operation order.  No noise and no history: x_t is the only load.  x_out may alias
-// x_t (the in-place loop): every load of a chunk is issued before its first store.
-constexpr int SCHED_NEXT_STRIDE = 2;   // floats per row of the reverse table: sqrt(abn) sqrt(1 - abn)
-struct EpiOutReverse : EpiOutStep {
-  struct Params : EpiOutStep::Params {
-    const float* sched_next;  // [n_steps, SCHED_NEXT_STRIDE]
-  };
+struct OutReverse {   // mode 6: no noise and no history
+  float sr, srm1, sa, sb;
+  struct In { float x; };
+  __device__ __forceinline__ OutReverse(const EpiOutParams& p, int) {
+    const int i = p.state->cur;
+    const float* row_s = p.sched + static_cast<size_t>(i) * SCHED_STRIDE;
+    const float* row_n = p.sched_next + static_cast<size_t>(i) * SCHED_NEXT_STRIDE;
+    sr = row_s[3]; srm1 = row_s[4]; sa = row_n[0]; sb = row_n[1];
+  }
+  __device__ __forceinline__ In load(const EpiOutParams& p, bool in, size_t idx, int, int) const {
+    return {in ? p.x_t[idx] : 0.f};
+  }
+  __device__ __forceinline__ void store(const EpiOutParams& p, size_t idx, float x0, const In& v) const {
+    if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
+    const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sr, v.x), x0), srm1);    // :862-865
+    p.x_out[idx] = __fadd_rn(__fmul_rn(x0, sa), __fmul_rn(sb, eps));          // :869-872
+  }
+};
+
+// One GEMM instantiation per update family, so that the PLMS and inversion epilogues leave the DDPM / DDIM kernel as
+// it is.
+template <class Update>
+struct EpiOut {
+  static constexpr int SMEM_PER_WARP = 1024;  // unused
+  using Params = EpiOutParams;
+  static __device__ __forceinline__ void preload(const Params&, float*, int, int, int) {}
   static __device__ __forceinline__ void tile_begin(EpiCtx&, const Params&, int, int) {}
   static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0,
                                                int) {
     const int row = row0 + ctx.lane;
     if (row >= ctx.M) return;
-    const int b = row / p.S, s = row - b * p.S;
-    if (s < p.s_off) return;
-    const int t = s - p.s_off;
-    const int i = p.state->cur;
-    const float* row_s = p.sched + static_cast<size_t>(i) * SCHED_STRIDE;
-    const float* row_n = p.sched_next + static_cast<size_t>(i) * SCHED_NEXT_STRIDE;
-    const float sr = row_s[3], srm1 = row_s[4], sa = row_n[0], sb = row_n[1];
+    const int b = row / p.T, t = row - b * p.T;
+    const Update u(p, b);
+    // x_out may alias x_t, x_step and the ring slots (in-place loop): every load of a 16-column group is issued before
+    // its first store, so that they are all in flight together (consecutive lanes = consecutive frames => each load /
+    // store is one coalesced line), and an element is only ever read and written by the thread that owns it.
     const size_t base = static_cast<size_t>(b) * p.J * p.T + t;
 #pragma unroll
     for (int h = 0; h < 32; h += 16) {
-      float xv[16];
+      typename Update::In v[16];
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int col = col0 + h + j;
-        xv[j] = col < p.J ? p.x_t[base + static_cast<size_t>(col) * p.T] : 0.f;
+        v[j] = u.load(p, col < p.J, base + static_cast<size_t>(col) * p.T, col, t);
       }
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
@@ -536,9 +507,7 @@ struct EpiOutReverse : EpiOutStep {
         float x0 = __uint_as_float(raw[h + j]) + __ldg(p.bias + col);
         if (p.inpaint_mask != nullptr && p.inpaint_mask[idx]) x0 = p.inpaint_motion[idx];
         if (p.clip_denoised) x0 = fminf(fmaxf(x0, -1.f), 1.f);
-        if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
-        const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sr, xv[j]), x0), srm1);     // :862-865
-        p.x_out[idx] = __fadd_rn(__fmul_rn(x0, sa), __fmul_rn(sb, eps));              // :869-872
+        u.store(p, idx, x0, v[j]);
       }
     }
   }

@@ -75,24 +75,17 @@ __global__ void pe_bias_kernel(float* __restrict__ out, const float* __restrict_
   for (int c = threadIdx.x; c < d; c += blockDim.x) out[static_cast<size_t>(s) * d + c] = bias[c] + pe[static_cast<size_t>(s) * d + c];
 }
 
-__global__ void step_advance_kernel(StepState* state) {
+// dir = -1 walks the schedule down (sampling), +1 up (DDIM inversion: x at index i -> x at index i + 1).
+__global__ void step_advance_kernel(StepState* state, int dir) {
   pdl_launch_dependents();
   pdl_wait();
   state->done += 1;
-  state->cur -= 1;
-}
-// The DDIM inversion walks the schedule upwards (x at index i -> x at index i + 1).
-__global__ void step_advance_up_kernel(StepState* state) {
-  pdl_launch_dependents();
-  pdl_wait();
-  state->done += 1;
-  state->cur += 1;
+  state->cur += dir;
 }
 __global__ void step_set_kernel(StepState* state, int done, int cur, const float* noise, long long noise_step_stride,
                                 unsigned long long seed, long long sample_base, int n_steps) {
   state->done = done;
   state->cur = cur;
-  state->start = cur;
   state->n_steps = n_steps;
   state->noise = noise;
   state->noise_step_stride = noise_step_stride;
