@@ -47,6 +47,21 @@ struct GemmLnSmem {
   static_assert(TOTAL <= 227 * 1024, "shared memory budget");
 };
 
+#ifdef B200_TRACE
+// Instrumented build only: %globaltimer stamps per tile, [CTA][tile iteration][role][event], role 0 the producer thread,
+// 1 + wg the store thread of consumer warpgroup wg; read (and cleared) by b200mdm_debug_ln_trace, see tools/ln_phases.py
+// for the events.  Without B200_TRACE the stamps compile to nothing.
+constexpr int GLN_TRACE_CTAS = 264, GLN_TRACE_ITERS = 16, GLN_TRACE_ROLES = 3, GLN_TRACE_EVENTS = 8;
+__device__ uint64_t g_gln_trace[GLN_TRACE_CTAS * GLN_TRACE_ITERS * GLN_TRACE_ROLES * GLN_TRACE_EVENTS];
+__device__ __forceinline__ void gln_stamp(int it, int role, int ev) {
+  if (blockIdx.x < GLN_TRACE_CTAS && it < GLN_TRACE_ITERS)
+    g_gln_trace[((blockIdx.x * GLN_TRACE_ITERS + it) * GLN_TRACE_ROLES + role) * GLN_TRACE_EVENTS + ev] = globaltimer_ns();
+}
+#define GLN_STAMP(cond, it, role, ev) if (cond) gln_stamp(it, role, ev)
+#else
+#define GLN_STAMP(cond, it, role, ev)
+#endif
+
 struct GemmLnParams {
   const float* bias;    // [512]
   const float* gamma;   // [512]
@@ -110,8 +125,10 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
+        GLN_STAMP(true, (tile - cluster_id) / num_clusters, 0, 0);
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
+          GLN_STAMP(kb == 0, (tile - cluster_id) / num_clusters, 0, 1);
           uint8_t* sa = tiles + stage * GLN_STAGE_BYTES;
           mbar_expect_tx(&full_bar[stage], GLN_STAGE_BYTES);
           tma_load_2d(sa, &map_a, &full_bar[stage], kb * GEMM_BLOCK_K, tile * GEMM_BLOCK_M);
@@ -134,6 +151,7 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
           }
           if (++stage == GLN_STAGES) { stage = 0; phase ^= 1; }
         }
+        GLN_STAMP(true, (tile - cluster_id) / num_clusters, 0, 2);
       }
     }
   } else {
@@ -159,9 +177,11 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
       const int as = it & 1;
       const uint32_t aphase = (it >> 1) & 1;
       if (lane == 0) mbar_expect_tx(&xbar[as * 8 + cw], 16 * 8);   // the peer's partials of this warp's 16 rows
+      GLN_STAMP(store_thread, it, 1 + wg, 0);
       int prev_stage = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
+        GLN_STAMP(kb == 0 && store_thread, it, 1 + wg, 1);
         const uint32_t sa = smem_u32(tiles + stage * GLN_STAGE_BYTES);
         const uint64_t da = wgmma_desc_k_sw128(sa + wg * 64 * 128);
         const uint64_t db = wgmma_desc_k_sw128(sa + 16384);
@@ -178,6 +198,7 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
       }
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
+      GLN_STAMP(store_thread, it, 1 + wg, 2);
       if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
       // the residual groups sit in the next GLN_GROUPS ring stages: group grp in stage (rs0 + grp) % GLN_STAGES
       const int rs0 = stage;
@@ -190,6 +211,7 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
         const int grp = j >> 3, jj = j & 7;
         const int rs = (rs0 + grp) % GLN_STAGES;
         if (jj == 0) mbar_wait(&full_bar[rs], rph0 ^ (rs0 + grp >= GLN_STAGES ? 1u : 0u));
+        GLN_STAMP(jj == 0 && (grp == 0 || grp == GLN_GROUPS - 1) && store_thread, it, 1 + wg, grp == 0 ? 3 : 4);
         const uint8_t* slab = tiles + rs * GLN_STAGE_BYTES + toff + ((jj ^ g) << 4);
         const int c = 8 * j + 2 * t;                   // local column of acc[4j], acc[4j+1] (and of acc[4j+2..3], row b)
         const float2 bb = *reinterpret_cast<const float2*>(bias_s + c);
@@ -229,6 +251,7 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
         st_async_f32x2(mapa_shared(smem_u32(&rem[lrow + 8]), peer), sb, qb, pbar);
       }
       mbar_wait_cluster(&xbar[as * 8 + cw], aphase);   // the peer's lanes have delivered this warp's 16 partials
+      GLN_STAMP(store_thread, it, 1 + wg, 5);
       const float2 pa = rem[lrow], pb = rem[lrow + 8];
       const float mean_a = (sa + pa.x) * (1.f / GLN_D), mean_b = (sb + pb.x) * (1.f / GLN_D);
       const float rstd_a = rsqrtf(fmaxf((qa + pa.y) * (1.f / GLN_D) - mean_a * mean_a, 0.f) + lp.eps);
@@ -258,6 +281,7 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
           *reinterpret_cast<__half2*>(slab + GLN_RES_HALF + 1024) = __floats2half2_rn(y0 - f.x, y1 - f.y);
         }
         if (jj == 7) {   // the warpgroup's 64 rows of this group are complete
+          GLN_STAMP(grp == GLN_GROUPS - 1 && store_thread, it, 1 + wg, 6);
           fence_proxy_async_smem();
           named_bar_sync(1 + wg, 128);
           if (store_thread) {
@@ -269,6 +293,7 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
               bulk_commit_group();
             }
             bulk_wait_group_read<0>();                   // the store has read the slab: the stage may be refilled
+            GLN_STAMP(grp == GLN_GROUPS - 1, it, 1 + wg, 7);
             mbar_arrive_cnt(&empty_bar[rs], 4);
           }
         }

@@ -104,6 +104,12 @@ __device__ __forceinline__ void bulk_wait_group() {
 }
 
 // ------------------------------------------------------------------ misc
+// nanoseconds, one clock for every SM (instrumented builds: phase stamps that are compared across CTAs)
+__device__ __forceinline__ uint64_t globaltimer_ns() {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
