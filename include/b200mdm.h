@@ -76,8 +76,18 @@ typedef struct b200mdm_config {
   int32_t target_encoder;    /* B200MDM_TARGET_*          (args.multi_encoder_type) */
   int32_t target_enc_layers; /* args.target_enc_layers (single / split; the multi encoder always has one hidden layer) */
   int32_t target_joints;     /* n_ext = len(all_goal_joint_names) + 2 ('traj', 'heading'): 8 for HumanML3D */
-  int32_t reserved[3];
+  /* trans_dec only (model/mdm.py:241-270); 0 / 0 = DiP: BERT token memory, no timestep token. */
+  int32_t emb_trans_dec;     /* args.emb_trans_dec: the timestep embedding is sequence token 0 (pe[0]), frames follow */
+  int32_t dec_memory;        /* B200MDM_DEC_MEMORY_*: what the cross-attention of every decoder layer attends to */
+  int32_t reserved[1];
 } b200mdm_config;
+
+/* Decoder memory kinds.  trans_dec accepts MEMORY_CLIP only with emb_trans_dec = 1 and context_len = 0 (the
+ * humanml-decoder-with-emb checkpoint), and emb_trans_dec = 1 only with MEMORY_CLIP; other pairs -> B200MDM_ENOTIMPL. */
+#define B200MDM_DEC_MEMORY_TOKENS 0 /* text-token features + padding mask (DiP, text_encoder_type 'bert') */
+#define B200MDM_DEC_MEMORY_CLIP 1   /* one CLIP feature row per sample: memory = embed_text(clip) + time_emb (mdm.py:262-264).
+                                       A softmax over one key is 1, so each layer's cross-attention block reduces to
+                                       the per-sample row c_l = out_proj(W_v m + b_v), added before norm2. */
 
 #define B200MDM_TARGET_NONE 0
 #define B200MDM_TARGET_SINGLE 1 /* EmbedTargetLocSingle: one MLP on cat(target, valid) [4 n_ext] */
@@ -137,7 +147,12 @@ int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframes, const fl
  *   enc_text_dev   : y['text_embed'][0], BERT token features [n_tokens, batch, cond_dim] fp32 device (reference layout)
  *   text_mask_host : y['text_embed'][1], uint8 [batch, n_tokens], 1 = padding (memory_key_padding_mask)
  *   nframes        : frames of x (pred_len); the sequence is context_len + nframes tokens, no conditioning token
- * lengths / scale / force_uncond as in b200mdm_set_cond.  Must be followed by b200mdm_set_prefix when context_len > 0. */
+ * lengths / scale / force_uncond as in b200mdm_set_cond.  Must be followed by b200mdm_set_prefix when context_len > 0.
+ * dec_memory = B200MDM_DEC_MEMORY_CLIP (emb_trans_dec): enc_text_dev is y['text_embed'] [1, batch, 512], the CLIP row
+ * as the one memory token; n_tokens must be 1 (else B200MDM_EINVAL) and text_mask_host all zero (the reference passes
+ * no memory mask).  The sequence is the timestep token + nframes frames; with cfg.mask_frames and lengths, token 0
+ * and `lengths` frames are valid keys (mdm.py:241-247).  The per-sample part of every layer's cross-attention row,
+ * out_proj(W_v (embed_text(clip) + g) + b_v), is evaluated here (and again by b200mdm_set_target), in fp32. */
 int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* enc_text_dev,
                          const uint8_t* text_mask_host, int32_t n_tokens, const int64_t* lengths_host,
                          const float* scale_dev, int32_t force_uncond, void* stream);
@@ -310,6 +325,15 @@ int b200mdm_test_gemm_resid_ln(const void* a16_dev, const void* w16_dev, const f
  * allocated on `stream`: out fp32 [batch, d] = embed_target_cond(target [batch, target_joints, 3], valid uint8 host). */
 int b200mdm_test_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, int32_t batch,
                         float* out_dev, void* stream);
+/* The per-step cross-attention rows of a B200MDM_DEC_MEMORY_CLIP engine for its current workspace (after
+ * b200mdm_set_cond_dec, and b200mdm_set_target when used), every sample at model timestep `timestep`:
+ * out fp32 [num_layers, Bp, 512], Bp = 2 x batch with CFG (conditional rows, then unconditional), else batch;
+ * row (l, b') = out_proj_l(W_v,l (embed_text(clip[b'] or 0) + temb[timestep] + g[b' mod batch]) + b_v,l). */
+int b200mdm_test_cross_rows(b200mdm_engine* e, int32_t timestep, float* out_dev, void* stream);
+/* The step's row-bias LayerNorm of such an engine: h[r] <- LayerNorm(h[r] + c[r / S]; gamma, beta, 1e-5) in place, for
+ * r < M; h fp16 [M, 1024] = [hi | lo] (value hi + lo, d = 512), c fp32 [(M + S - 1) / S, 512]. */
+int b200mdm_test_row_bias_ln(void* hres16_dev, const float* c_dev, const float* gamma_dev, const float* beta_dev,
+                             int32_t M, int32_t S, void* stream);
 
 #ifdef __cplusplus
 }

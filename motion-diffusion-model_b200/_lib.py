@@ -28,15 +28,17 @@ SYMBOLS = [
     "b200mdm_recover_from_ric", "b200mdm_test_gemm_f16", "b200mdm_test_attention", "b200mdm_test_cross_attention", "b200mdm_test_qkv_attention",
     "b200mdm_test_gemm_resid_ln", "b200mdm_test_gemm_epi", "b200mdm_test_embed", "b200mdm_test_out_step",
     "b200mdm_set_target", "b200mdm_test_target", "b200mdm_plms_loop_range", "b200mdm_plms_step",
-    "b200mdm_set_schedule_next", "b200mdm_ddim_reverse_loop_range",
+    "b200mdm_set_schedule_next", "b200mdm_ddim_reverse_loop_range", "b200mdm_test_cross_rows",
+    "b200mdm_test_row_bias_ln",
 ]
+DEC_MEMORY_TOKENS, DEC_MEMORY_CLIP = 0, 1   # b200mdm_config.dec_memory (trans_dec)
 
 
 class Config(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in (
         "arch", "latent_dim", "ff_size", "num_layers", "num_heads", "njoints", "nfeats", "cond_mode", "cond_dim",
         "num_actions", "mask_frames", "pos_embed_max_len", "temb_rows", "context_len", "target_encoder",
-        "target_enc_layers", "target_joints")] + [("reserved", ctypes.c_int32 * 3)]
+        "target_enc_layers", "target_joints", "emb_trans_dec", "dec_memory")] + [("reserved", ctypes.c_int32 * 1)]
 
 
 class B200MDMError(RuntimeError):
@@ -97,7 +99,9 @@ def load():
                        ("b200mdm_plms_loop_range", [vp, i32, i32, i32, vp, vp, i32, i32, vp]),
                        ("b200mdm_plms_step", [vp, i32, i32, vp, ctypes.POINTER(vp), i32, i32, vp, vp, vp, vp]),
                        ("b200mdm_set_schedule_next", [vp, i32, vp]),
-                       ("b200mdm_ddim_reverse_loop_range", [vp, i32, i32, vp, vp, i32, i32, vp])):
+                       ("b200mdm_ddim_reverse_loop_range", [vp, i32, i32, vp, vp, i32, i32, vp]),
+                       ("b200mdm_test_cross_rows", [vp, i32, vp, vp]),
+                       ("b200mdm_test_row_bias_ln", [vp, vp, vp, vp, i32, i32, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

@@ -134,6 +134,8 @@ struct LayerW {
   __half *wq_c = nullptr, *wo_c = nullptr;           // (the K/V rows of all layers live in engine->wkv_all)
   const float *bq_c = nullptr, *bo_c = nullptr, *g3 = nullptr, *be3 = nullptr;
   CUtensorMap m_wq_c, m_wo_c_256;
+  // trans_dec with a CLIP memory: the value rows W_v [d, d], b_v and W_o of multihead_attn in fp32 (weight store)
+  const float *wv_c32 = nullptr, *bv_c32 = nullptr, *wo_c32 = nullptr;
 };
 
 struct GraphKey {
@@ -170,6 +172,9 @@ struct Workspace {
   unsigned char* memmask = nullptr;                                   // [Bp, Mt] 1 = padding
   CUtensorMap m_mem, m_qc_st, m_kvc_st;
   bool prefix_set = false;
+  // trans_dec with a CLIP memory (kernels.cuh, cross_rows_kernel): the memory rows' per-sample part mb [Bp, d], a GEMV
+  // scratch [Bp, d], cb [L, Bp, d] (per loop) and the step's cross-attention rows c [L, Bp, d]
+  float *cross_mb = nullptr, *cross_u = nullptr, *cross_b = nullptr, *cross_c = nullptr;
   // target-location conditioning: validity [B, n_ext] (1.0 / 0.0) and g = embed_target_cond(...) [B, d], read by both
   // CFG halves; target_set is cleared by every b200mdm_set_cond* call
   float *tgt_valid = nullptr, *tgt_g = nullptr;
@@ -222,6 +227,10 @@ struct b200mdm_engine : Workspace {
   std::vector<unsigned char> h_mask;
   // trans_dec (DiP)
   bool dec = false;
+  // trans_dec with emb_trans_dec and a CLIP memory: sequence = timestep token + frames, cross-attention = a per-sample
+  // row (kernels.cuh, cross_rows_kernel); cross_t = W_o,l W_v,l temb[t] for every layer and model timestep [L, R, d]
+  bool dec_clip = false;
+  float* cross_t = nullptr;
   int ctx = 0, s_off = 1;
   int kw = 1;   // 2: fp16 activations between the layer GEMMs are [hi | lo] pairs along K (trans_dec engine)
   const unsigned char* inpaint_mask = nullptr;
@@ -436,6 +445,17 @@ extern "C" int b200mdm_create(const b200mdm_config* cfg, b200mdm_engine** out) {
     return fail(B200MDM_ENOTIMPL, "arch %d: trans_enc and trans_dec are implemented", cfg->arch);
   if (cfg->arch == B200MDM_ARCH_TRANS_DEC && (cfg->cond_mode != B200MDM_COND_TEXT || cfg->context_len < 0))
     return fail(B200MDM_ENOTIMPL, "trans_dec needs text-token conditioning (BERT) and context_len >= 0");
+  if (cfg->emb_trans_dec < 0 || cfg->emb_trans_dec > 1 || cfg->dec_memory < B200MDM_DEC_MEMORY_TOKENS ||
+      cfg->dec_memory > B200MDM_DEC_MEMORY_CLIP)
+    return fail(B200MDM_EINVAL, "emb_trans_dec must be 0 or 1 and dec_memory 0 (tokens) or 1 (CLIP) (got %d / %d)",
+                cfg->emb_trans_dec, cfg->dec_memory);
+  if (cfg->arch == B200MDM_ARCH_TRANS_ENC && (cfg->emb_trans_dec || cfg->dec_memory))
+    return fail(B200MDM_EINVAL, "emb_trans_dec and dec_memory are trans_dec fields");
+  if (cfg->arch == B200MDM_ARCH_TRANS_DEC && (cfg->dec_memory == B200MDM_DEC_MEMORY_CLIP) != (cfg->emb_trans_dec == 1))
+    return fail(B200MDM_ENOTIMPL, "trans_dec implements the BERT token memory without the timestep token (DiP) and the CLIP "
+                "memory with it (emb_trans_dec); got dec_memory %d, emb_trans_dec %d", cfg->dec_memory, cfg->emb_trans_dec);
+  if (cfg->dec_memory == B200MDM_DEC_MEMORY_CLIP && cfg->context_len != 0)
+    return fail(B200MDM_ENOTIMPL, "trans_dec with a CLIP memory has no prefix completion (context_len %d)", cfg->context_len);
   if (cfg->latent_dim != 512 || cfg->num_heads != 4 || cfg->ff_size % 64 || cfg->ff_size <= 0)
     return fail(B200MDM_ENOTIMPL, "kernels are specialised for latent_dim 512 / 4 heads (got %d / %d)", cfg->latent_dim,
                 cfg->num_heads);
@@ -469,12 +489,14 @@ extern "C" int b200mdm_create(const b200mdm_config* cfg, b200mdm_engine** out) {
   e->num_sms = prop.multiProcessorCount;
   e->layers.resize(e->L);
   e->dec = cfg->arch == B200MDM_ARCH_TRANS_DEC;
+  e->dec_clip = e->dec && cfg->dec_memory == B200MDM_DEC_MEMORY_CLIP;
   e->ctx = e->dec ? cfg->context_len : 0;
-  e->s_off = e->dec ? e->ctx : 1;
+  e->s_off = (e->dec && !e->dec_clip) ? e->ctx : 1;   // token 0: the encoder's conditioning / the decoder's timestep
   // DiP samples with guidance 7.5 (three times the encoder's 2.5): the CFG blend multiplies every activation rounding
   // error by ~10.  Its fp16 activations are therefore kept as hi + lo pairs; at 60-token sequences the doubled K of
-  // the layer GEMMs is free.
-  e->kw = e->dec ? 2 : 1;
+  // the layer GEMMs is free.  The CLIP decoder runs 197-token sequences, where it is not, and holds the 1e-3 bound
+  // with plain fp16 activations (DESIGN.md section 2).
+  e->kw = (e->dec && !e->dec_clip) ? 2 : 1;
   CUDA_TRY(cudaStreamCreateWithFlags(&e->work, cudaStreamNonBlocking));
   CUDA_TRY(cudaEventCreateWithFlags(&e->ev_in, cudaEventDisableTiming));
   CUDA_TRY(cudaEventCreateWithFlags(&e->ev_out, cudaEventDisableTiming));
@@ -494,6 +516,7 @@ static void free_workspace(Workspace* w) {
   dfree(w->tok0); dfree(w->condproj); dfree(w->proj); dfree(w->scale); dfree(w->x_work); dfree(w->pe_bias); dfree(w->eps_buf);
   dfree(w->kvlen); dfree(w->tvec); dfree(w->action);
   dfree(w->encperm); dfree(w->memtok); dfree(w->memproj); dfree(w->mem16); dfree(w->qc16); dfree(w->kvc16); dfree(w->memmask);
+  dfree(w->cross_mb); dfree(w->cross_u); dfree(w->cross_b); dfree(w->cross_c);
   dfree(w->tgt_valid); dfree(w->tgt_g);
   dfree(w->plms_ring); dfree(w->plms_mid); dfree(w->plms_pred);
   *w = Workspace();
@@ -518,7 +541,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   for (auto& l : e->layers) { dfree(l.wqkv); dfree(l.wo); dfree(l.w1); dfree(l.w2); dfree(l.wq_c); dfree(l.wo_c); }
   dfree(e->w_in3); dfree(e->w_out3); dfree(e->temb_hidden); dfree(e->temb_table); dfree(e->sched); dfree(e->tmap);
   dfree(e->sched_next);
-  dfree(e->wkv_all); dfree(e->bkv_all);
+  dfree(e->wkv_all); dfree(e->bkv_all); dfree(e->cross_t);
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
   if (e->work) cudaStreamDestroy(e->work);
@@ -719,6 +742,7 @@ extern "C" int b200mdm_finalize_weights(b200mdm_engine* e, void* stream) {
   free_all_workspaces(e);
   for (auto& l : e->layers) { dfree(l.wqkv); dfree(l.wo); dfree(l.w1); dfree(l.w2); dfree(l.wq_c); dfree(l.wo_c); }
   dfree(e->w_in3); dfree(e->w_out3); dfree(e->temb_hidden); dfree(e->temb_table); dfree(e->wkv_all); dfree(e->bkv_all);
+  dfree(e->cross_t);
 
   // split-precision in / out projections: W' = [hi | hi | lo], zero padded
   const int Kp = e->Kp_in;
@@ -765,6 +789,12 @@ extern "C" int b200mdm_finalize_weights(b200mdm_engine* e, void* stream) {
       TRY(need(e, p + "multihead_attn.out_proj.bias", {d}, &w.bo_c));
       TRY(need(e, p + "norm3.weight", {d}, &w.g3));
       TRY(need(e, p + "norm3.bias", {d}, &w.be3));
+      if (e->dec_clip) {   // one memory token: only the value rows and the output projection matter, in fp32
+        w.wv_c32 = wc + static_cast<size_t>(2) * d * d;
+        w.bv_c32 = bc + 2 * d;
+        w.wo_c32 = woc;
+        continue;
+      }
       w.bq_c = bc;
       TRY(to_f16_k(wc, &w.wq_c, d, d, kw, s));
       if (l == 0) {
@@ -792,6 +822,19 @@ extern "C" int b200mdm_finalize_weights(b200mdm_engine* e, void* stream) {
   CUDA_TRY(cudaGetLastError());
   small_linear_kernel<0><<<blocks, 256, 0, s>>>(e->temb_hidden, t2w, t2b, e->temb_table, R, d, d, d);
   CUDA_TRY(cudaGetLastError());
+  if (e->dec_clip) {
+    // the timestep part of every layer's cross-attention row: cross_t[l, t] = W_o,l (W_v,l temb[t]) (temb_hidden is
+    // free again and holds the inner product)
+    TRY(dalloc(&e->cross_t, static_cast<size_t>(e->L) * R * d));
+    for (int l = 0; l < e->L; ++l) {
+      const LayerW& w = e->layers[l];
+      small_linear_kernel<0><<<blocks, 256, 0, s>>>(e->temb_table, w.wv_c32, nullptr, e->temb_hidden, R, d, d, d);
+      CUDA_TRY(cudaGetLastError());
+      small_linear_kernel<0><<<blocks, 256, 0, s>>>(e->temb_hidden, w.wo_c32, nullptr, e->cross_t + static_cast<size_t>(l) * R * d,
+                                                    R, d, d, d);
+      CUDA_TRY(cudaGetLastError());
+    }
+  }
   CUDA_TRY(cudaStreamSynchronize(s));
   e->finalized = true;
   return B200MDM_OK;
@@ -863,7 +906,13 @@ static int build_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStre
   TRY(dalloc(&e->kvlen, Bp));
   TRY(dalloc(&e->tvec, B, true));
   TRY(dalloc(&e->action, B, true));
-  if (e->dec) {
+  if (e->dec_clip) {
+    const size_t rows = static_cast<size_t>(Bp) * d, all = static_cast<size_t>(e->L) * Bp * d;
+    TRY(dalloc(&e->cross_mb, rows));
+    TRY(dalloc(&e->cross_u, rows));
+    TRY(dalloc(&e->cross_b, all));
+    TRY(dalloc(&e->cross_c, all));
+  } else if (e->dec) {
     TRY(dalloc(&e->qc16, M * d));
     TRY(make_map_t(&e->m_qc_st, e->qc16, 2, M, d, d, 32));
     e->Mt = 0;              // the text-memory buffers are sized by the packed batch: b200mdm_set_cond_dec rebuilds them
@@ -1020,6 +1069,67 @@ extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframe
   return B200MDM_OK;
 }
 
+// cb_l[b'] = W_o,l (W_v,l mb[b'] + b_v,l) + b_o,l with mb = condproj (+ g): the per-sample part of the cross-attention rows
+// of a CLIP-memory decoder, once per loop (kernels.cuh, cross_rows_kernel).
+static int cross_rows_per_sample(b200mdm_engine* e, const float* g, cudaStream_t s) {
+  const int d = e->d, Bp = e->Bp;
+  cross_mem_kernel<<<Bp, 128, 0, s>>>(e->cross_mb, e->condproj, g, e->B, d);
+  CUDA_TRY(cudaGetLastError());
+  const int blocks = static_cast<int>((static_cast<size_t>(Bp) * d * 32 + 255) / 256);
+  for (int l = 0; l < e->L; ++l) {
+    const LayerW& w = e->layers[l];
+    small_linear_kernel<0><<<blocks, 256, 0, s>>>(e->cross_mb, w.wv_c32, w.bv_c32, e->cross_u, Bp, d, d, d);
+    CUDA_TRY(cudaGetLastError());
+    small_linear_kernel<0><<<blocks, 256, 0, s>>>(e->cross_u, w.wo_c32, w.bo_c, e->cross_b + static_cast<size_t>(l) * Bp * d,
+                                                  Bp, d, d, d);
+    CUDA_TRY(cudaGetLastError());
+  }
+  e->launches += 1 + 2 * e->L;
+  return B200MDM_OK;
+}
+
+// ---- trans_dec with emb_trans_dec and a CLIP memory: y['text_embed'] [1, B, C] is the one memory token of every sample
+static int set_cond_dec_clip(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* clip_dev,
+                             const uint8_t* text_mask_host, int32_t n_tokens, const int64_t* lengths_host,
+                             const float* scale_dev, int32_t force_uncond, cudaStream_t s) {
+  if (n_tokens != 1) return fail(B200MDM_EINVAL, "a CLIP-memory decoder takes one memory token per sample (n_tokens %d)", n_tokens);
+  if (batch <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
+  if (!clip_dev || !text_mask_host) return fail(B200MDM_EINVAL, "the CLIP decoder needs y['text_embed'] and an all-zero mask");
+  for (int b = 0; b < batch; ++b)
+    if (text_mask_host[b]) return fail(B200MDM_EINVAL, "the CLIP memory has no padding mask (model/mdm.py:262-263)");
+  if (nframes + 1 > e->cfg.pos_embed_max_len) return fail(B200MDM_EINVAL, "sequence longer than the positional table");
+  if (nframes + 1 > ATC_MAX_KEYS) return fail(B200MDM_ENOTIMPL, "sequences of more than %d tokens", ATC_MAX_KEYS);
+  const int halves = scale_dev ? 2 : 1;
+  TRY(select_workspace(e, batch, nframes, halves, s));
+  const int d = e->d, B = batch, S = e->S;
+  // key mask: the timestep token, then `lengths` frames (model/mdm.py:241-247, the False column prepended)
+  std::vector<int>& kv = e->h_kv;
+  kv.assign(e->Bp, S);
+  if (e->cfg.mask_frames && lengths_host && nframes > 1) {
+    for (int b = 0; b < e->Bp; ++b) {
+      long long len = lengths_host[b % B];
+      if (len < 0) len = 0;
+      if (len > nframes) len = nframes;
+      kv[b] = static_cast<int>(len) + 1;
+    }
+  }
+  CUDA_TRY(cudaMemcpyAsync(e->kvlen, kv.data(), kv.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  if (scale_dev) CUDA_TRY(cudaMemcpyAsync(e->scale, scale_dev, B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  // text_emb = embed_text(mask_cond(clip)) (model/mdm.py:218): conditional rows W clip + b, unconditional rows b
+  const size_t warps = static_cast<size_t>(B) * d;
+  small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(clip_dev, e->w_txt, e->b_txt, e->proj, B, d,
+                                                                                     e->cfg.cond_dim, e->cfg.cond_dim);
+  CUDA_TRY(cudaGetLastError());
+  condproj_fill_kernel<<<e->Bp, 128, 0, s>>>(e->condproj, e->proj, e->b_txt, nullptr, nullptr, B, d, e->Bp,
+                                             (halves == 1 && force_uncond) ? 1 : 0, B200MDM_COND_TEXT);
+  CUDA_TRY(cudaGetLastError());
+  e->launches += 2;
+  TRY(cross_rows_per_sample(e, nullptr, s));
+  e->cond_set = true;
+  e->target_set = false;
+  return B200MDM_OK;
+}
+
 // ---- trans_dec (DiP) conditioning: BERT token features + padding mask as the cross-attention memory, prefix frames
 extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* enc_text_dev,
                                     const uint8_t* text_mask_host, int32_t n_tokens, const int64_t* lengths_host,
@@ -1027,6 +1137,9 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
   if (!e) return fail(B200MDM_EINVAL, "null engine");
   if (!e->dec) return fail(B200MDM_EINVAL, "b200mdm_set_cond_dec is for trans_dec engines");
   if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
+  if (e->dec_clip)
+    return set_cond_dec_clip(e, batch, nframes, enc_text_dev, text_mask_host, n_tokens, lengths_host, scale_dev, force_uncond,
+                             static_cast<cudaStream_t>(stream));
   if (batch <= 0 || nframes <= 0 || n_tokens <= 0 || n_tokens > 64) return fail(B200MDM_EINVAL, "bad batch / nframes / n_tokens (1..64)");
   if (nframes + e->ctx > e->cfg.pos_embed_max_len) return fail(B200MDM_EINVAL, "sequence longer than the positional table");
   if (nframes + e->ctx > ATC_MAX_KEYS) return fail(B200MDM_ENOTIMPL, "sequences of more than %d tokens", ATC_MAX_KEYS);
@@ -1087,6 +1200,8 @@ extern "C" int b200mdm_set_target(b200mdm_engine* e, const float* target_dev, co
   if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
   TRY(encode_target(e, target_dev, valid_host, e->B, e->tgt_valid, e->tgt_g, e->h_valid, static_cast<cudaStream_t>(stream)));
   e->launches++;
+  // the CLIP decoder's memory row carries g as well (model/mdm.py:199,262): its per-sample cross-attention part again
+  if (e->dec_clip) TRY(cross_rows_per_sample(e, e->tgt_g, static_cast<cudaStream_t>(stream)));
   e->target_set = true;
   return B200MDM_OK;
 }
@@ -1176,9 +1291,17 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     ++nk;
   }
   const float* target_g = e->target_set ? e->tgt_g : nullptr;   // timestep embedding + target (model/mdm.py:197-199)
-  if (!e->dec) {
-    CUDA_TRY(launch_k(tok0_rows_kernel, dim3(e->Bp), dim3(128), 0, s, e->hres, e->condproj, e->temb_table, e->pe,
-                      a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, target_g, B, S, d, e->cfg.temb_rows, a.back));
+  if (!e->dec || e->dec_clip) {
+    // token 0: cond + (temb + g) (encoder), or the decoder's timestep token (temb + g) without the text (mdm.py:256)
+    CUDA_TRY(launch_k(tok0_rows_kernel, dim3(e->Bp), dim3(128), 0, s, e->hres, e->dec_clip ? nullptr : e->condproj,
+                      e->temb_table, e->pe, a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, target_g, B, S, d,
+                      e->cfg.temb_rows, a.back));
+    if (e->dec_clip) {
+      // every layer's cross-attention row of this step: c_l[b'] = cb_l[b'] + ct_l[t]
+      CUDA_TRY(launch_k(cross_rows_kernel, dim3(e->Bp, e->L), dim3(128), 0, s, e->cross_c, e->cross_b, e->cross_t,
+                        a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, B, e->Bp, d, e->cfg.temb_rows, a.back));
+      ++nk;
+    }
   } else {
     // cross-attention memory of this step: text tokens + timestep embedding (model/mdm.py:218-220)
     CUDA_TRY(launch_k(mem_build_kernel, dim3(e->Mt, e->Bp), dim3(128), 0, s, e->mem16, e->memproj, e->temb_table,
@@ -1205,7 +1328,12 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
       TRY(launch_attention_tc(e->m_qkv_kv, e->qkv16, e->att16, e->kvlen, e->Bp, S, d, e->H, s, wide));
     }
     if (!B200_SKIP(2)) TRY(launch_gemm_resid_ln(e->m_att, w.m_wo_256, e->m_hres, e->M, kw * d, w.bo, w.g1, w.be1, s, e->num_sms));
-    if (e->dec) {
+    if (e->dec_clip) {
+      // cross-attention block over the one-token memory + norm2: h <- LN2(h + c_l[b'])
+      CUDA_TRY(launch_k(row_bias_ln_kernel, dim3((e->M + RBLN_ROWS_PER_CTA - 1) / RBLN_ROWS_PER_CTA), dim3(32 * RBLN_ROWS_PER_CTA),
+                        0, s, e->hres, e->cross_c + static_cast<size_t>(l) * e->Bp * d, w.g2, w.be2, e->M, S, 1e-5f));
+      ++nk;
+    } else if (e->dec) {
       // cross-attention block of nn.TransformerDecoderLayer: q from the sequence, k/v from the text memory
       TRY((launch_gemm_bias<false>(e->m_h16, w.m_wq_c, e->m_qc_st, e->M, d, d, w.bq_c, s, e->num_sms)));
       {
@@ -1843,6 +1971,33 @@ extern "C" int b200mdm_test_gemm_resid_ln(const void* a16_dev, const void* w16_d
   TRY(make_map(&mb, w16_dev, GLN_D, K, K, 256));
   TRY(make_hres_map(&mh, hres16_dev, M));
   return launch_gemm_resid_ln(ma, mb, mh, M, K, bias_dev, gamma_dev, beta_dev, static_cast<cudaStream_t>(stream), sms);
+}
+
+extern "C" int b200mdm_test_cross_rows(b200mdm_engine* e, int32_t timestep, float* out_dev, void* stream) {
+  if (!e || !out_dev) return fail(B200MDM_EINVAL, "bad argument");
+  if (!e->dec_clip) return fail(B200MDM_EINVAL, "cross-attention rows belong to trans_dec engines with a CLIP memory");
+  if (!e->finalized || !e->cond_set) return fail(B200MDM_ESTATE, "weights and b200mdm_set_cond_dec first");
+  if (timestep < 0 || timestep >= e->cfg.temb_rows) return fail(B200MDM_EINVAL, "timestep outside [0, %d)", e->cfg.temb_rows);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<int> t(e->B, timestep);
+  CUDA_TRY(cudaMemcpyAsync(e->tvec, t.data(), e->B * sizeof(int), cudaMemcpyHostToDevice, s));
+  cross_rows_kernel<<<dim3(e->Bp, e->L), 128, 0, s>>>(out_dev, e->cross_b, e->cross_t, e->tvec, e->tmap, e->state, e->B, e->Bp,
+                                                      e->d, e->cfg.temb_rows, 0);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaStreamSynchronize(s));   // `t` is local
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_test_row_bias_ln(void* hres16_dev, const float* c_dev, const float* gamma_dev, const float* beta_dev,
+                                        int32_t M, int32_t S, void* stream) {
+  if (!hres16_dev || !c_dev || !gamma_dev || !beta_dev || M <= 0 || S <= 0) return fail(B200MDM_EINVAL, "bad argument");
+  if ((reinterpret_cast<uintptr_t>(hres16_dev) | reinterpret_cast<uintptr_t>(c_dev) | reinterpret_cast<uintptr_t>(gamma_dev) |
+       reinterpret_cast<uintptr_t>(beta_dev)) & 15)
+    return fail(B200MDM_EINVAL, "operands must be 16-byte aligned");
+  row_bias_ln_kernel<<<(M + RBLN_ROWS_PER_CTA - 1) / RBLN_ROWS_PER_CTA, 32 * RBLN_ROWS_PER_CTA, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<__half*>(hres16_dev), c_dev, gamma_dev, beta_dev, M, S, 1e-5f);
+  CUDA_TRY(cudaGetLastError());
+  return B200MDM_OK;
 }
 
 #ifdef B200_TRACE

@@ -45,6 +45,7 @@ __global__ void pack_input_kernel(const float* __restrict__ x, __half* __restric
 //   t(b') = tvec[b' % B] when tvec != nullptr (model called with explicit timesteps), else timestep_map[i] with
 //   i = eval_index(state, back): the step in flight, or the one before it (PLMS improved Euler)
 // With a target embedding g [B, d] (model/mdm.py:197-199, both CFG halves): (condproj + (temb + g[b' % B])) + pe[0].
+// condproj == nullptr (the timestep token of trans_dec with emb_trans_dec, mdm.py:256): (temb + g) + pe[0], no text.
 // Runs right after the embedding GEMM (which leaves placeholder values in these rows).
 // The residual stream is an fp16 [hi | lo] pair per element (row = 2d halves, hi + lo carries ~22 bits).
 __global__ void tok0_rows_kernel(__half* __restrict__ hres, const float* __restrict__ condproj,
@@ -61,7 +62,7 @@ __global__ void tok0_rows_kernel(__half* __restrict__ hres, const float* __restr
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
     float te = temb_table[static_cast<size_t>(t) * d + c];
     if (g != nullptr) te = te + g[static_cast<size_t>(bp % B) * d + c];
-    const float v = (condproj[static_cast<size_t>(bp) * d + c] + te) + pe[c];
+    const float v = (condproj != nullptr ? condproj[static_cast<size_t>(bp) * d + c] + te : te) + pe[c];
     const __half hi = __float2half_rn(v);
     hres[row * 2 * d + c] = hi;
     hres[row * 2 * d + d + c] = __float2half_rn(v - __half2float(hi));
@@ -382,6 +383,117 @@ __global__ void permute_mbc_kernel(const float* __restrict__ src, float* __restr
   const int m = blockIdx.x, b = blockIdx.y;
   for (int c = threadIdx.x; c < C; c += blockDim.x)
     dst[(static_cast<size_t>(b) * Mt + m) * C + c] = src[(static_cast<size_t>(m) * B + b) * C + c];
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// trans_dec with a CLIP memory and the timestep token (emb_trans_dec, model/mdm.py:256-264).  The memory is ONE token
+// per sample, m[b'] = textproj[b'] + (temb[t] + g[b]), without a mask: the softmax over a single key is exactly 1, so
+// each layer's cross-attention block returns the same row for every query of the sample,
+//   c_l[b'] = W_o,l (W_v,l m[b'] + b_v,l) + b_o,l .
+// It is linear in m, so it splits into a per-sample part and a per-timestep part, both in fp32:
+//   cb_l[b'] = W_o,l (W_v,l (textproj[b'] + g[b]) + b_v,l) + b_o,l   once per loop (set_cond_dec / set_target)
+//   ct_l[t]  = W_o,l (W_v,l temb[t])                                  once per weight load, every model timestep
+// and the step only adds them (cross_rows_kernel).  Against the reference's order this moves the fp32 rounding of the
+// two GEMVs, a few ulp of each dot product (tests/test_dec_emb_gpu.py bounds it against fp64).
+
+// mb[b', :] = textproj[b', :] + g[b' % B, :] (g == nullptr: textproj), the per-sample part of the memory row.
+__global__ void cross_mem_kernel(float* __restrict__ mb, const float* __restrict__ textproj, const float* __restrict__ g,
+                                 int B, int d) {
+  const int bp = blockIdx.x;
+  for (int c = threadIdx.x; c < d; c += blockDim.x) {
+    const float p = textproj[static_cast<size_t>(bp) * d + c];
+    mb[static_cast<size_t>(bp) * d + c] = g != nullptr ? p + g[static_cast<size_t>(bp % B) * d + c] : p;
+  }
+}
+
+// c[l, b', :] = cb[l, b', :] + ct[l, t(b'), :]   (t as in tok0_rows_kernel).  grid = (Bp, L)
+__global__ void cross_rows_kernel(float* __restrict__ c, const float* __restrict__ cb, const float* __restrict__ ct,
+                                  const int* __restrict__ tvec, const int* __restrict__ tmap,
+                                  const StepState* __restrict__ state, int B, int Bp, int d, int temb_rows, int back) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int bp = blockIdx.x, l = blockIdx.y;
+  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(*state, back)];
+  t = min(max(t, 0), temb_rows - 1);
+  const size_t row = (static_cast<size_t>(l) * Bp + bp) * d, trow = (static_cast<size_t>(l) * temb_rows + t) * d;
+  for (int i = threadIdx.x; i < d / 4; i += blockDim.x) {
+    const float4 a = reinterpret_cast<const float4*>(cb + row)[i], b = reinterpret_cast<const float4*>(ct + trow)[i];
+    reinterpret_cast<float4*>(c + row)[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+  }
+}
+
+// h[r] <- LayerNorm(h[r] + c[r / S]; gamma, beta, eps) in place on the residual stream fp16 [M, 2 RBLN_D] = [hi | lo]
+// (norm2 of the decoder layer with the cross-attention row c_l of the sample).  One warp per row; lane j holds columns
+// [8j, 8j + 8) and [256 + 8j, 256 + 8j + 8) of both halves in 16-byte loads.  v = (hi + lo) + c in fp32; the mean and
+// then the variance Σ(v - mean)² / d are two passes over the registers (no mean² cancellation);
+// y = (v - mean) rstd gamma + beta, written back as hi = fp16(y), lo = fp16(y - hi).
+constexpr int RBLN_D = 512;
+constexpr int RBLN_ROWS_PER_CTA = 8;
+__global__ void __launch_bounds__(32 * RBLN_ROWS_PER_CTA) row_bias_ln_kernel(__half* __restrict__ hres,
+                                                                            const float* __restrict__ c,
+                                                                            const float* __restrict__ gamma,
+                                                                            const float* __restrict__ beta, int M, int S,
+                                                                            float eps) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int lane = threadIdx.x & 31;
+  const int r = blockIdx.x * RBLN_ROWS_PER_CTA + (threadIdx.x >> 5);
+  if (r >= M) return;
+  __half* hrow = hres + static_cast<size_t>(r) * 2 * RBLN_D;
+  const float* crow = c + static_cast<size_t>(r / S) * RBLN_D;
+  float v[16];
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const int col = k * (RBLN_D / 2) + 8 * lane;
+    const uint4 hv = *reinterpret_cast<const uint4*>(hrow + col);
+    const uint4 lv = *reinterpret_cast<const uint4*>(hrow + RBLN_D + col);
+    const float4 c0 = *reinterpret_cast<const float4*>(crow + col), c1 = *reinterpret_cast<const float4*>(crow + col + 4);
+    const __half2* h2 = reinterpret_cast<const __half2*>(&hv);
+    const __half2* l2 = reinterpret_cast<const __half2*>(&lv);
+    const float cc[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 a = __half22float2(h2[j]), b = __half22float2(l2[j]);
+      v[8 * k + 2 * j] = (a.x + b.x) + cc[2 * j];
+      v[8 * k + 2 * j + 1] = (a.y + b.y) + cc[2 * j + 1];
+    }
+  }
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) s += v[i];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const float mean = s * (1.f / RBLN_D);
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const float dv = v[i] - mean;
+    q = fmaf(dv, dv, q);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+  const float rstd = rsqrtf(q * (1.f / RBLN_D) + eps);
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const int col = k * (RBLN_D / 2) + 8 * lane;
+    const float4 g0 = *reinterpret_cast<const float4*>(gamma + col), g1 = *reinterpret_cast<const float4*>(gamma + col + 4);
+    const float4 b0 = *reinterpret_cast<const float4*>(beta + col), b1 = *reinterpret_cast<const float4*>(beta + col + 4);
+    const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+    uint4 ho, lo;
+    __half2* h2 = reinterpret_cast<__half2*>(&ho);
+    __half2* l2 = reinterpret_cast<__half2*>(&lo);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float y0 = (v[8 * k + 2 * j] - mean) * rstd * gg[2 * j] + bb[2 * j];
+      const float y1 = (v[8 * k + 2 * j + 1] - mean) * rstd * gg[2 * j + 1] + bb[2 * j + 1];
+      h2[j] = __floats2half2_rn(y0, y1);
+      const float2 hf = __half22float2(h2[j]);
+      l2[j] = __floats2half2_rn(y0 - hf.x, y1 - hf.y);
+    }
+    *reinterpret_cast<uint4*>(hrow + col) = ho;
+    *reinterpret_cast<uint4*>(hrow + RBLN_D + col) = lo;
+  }
 }
 
 // Cross-attention core: softmax(q k^T / sqrt(128) + mask) v with a handful of memory tokens (Mt <= 64).

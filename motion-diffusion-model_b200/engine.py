@@ -56,7 +56,7 @@ class Engine:
 
     def __init__(self, *, arch, latent_dim, ff_size, num_layers, num_heads, njoints, nfeats, cond_mode, cond_dim,
                  num_actions, mask_frames, pos_embed_max_len, temb_rows, context_len=0, target_encoder=None,
-                 target_enc_layers=1, target_joint_names=()):
+                 target_enc_layers=1, target_joint_names=(), emb_trans_dec=False, dec_memory=_lib.DEC_MEMORY_TOKENS):
         self.lib = _lib.load()
         if not torch.cuda.is_available():
             raise RuntimeError("b200mdm needs a CUDA device (sm_90a); there is no CPU fallback")
@@ -67,10 +67,12 @@ class Engine:
                                pos_embed_max_len=pos_embed_max_len, temb_rows=temb_rows, context_len=context_len,
                                target_encoder=_lib.TARGET[target_encoder] if target_encoder else 0,
                                target_enc_layers=target_enc_layers if target_encoder else 0,
-                               target_joints=len(target_joint_names) if target_encoder else 0)
+                               target_joints=len(target_joint_names) if target_encoder else 0,
+                               emb_trans_dec=int(bool(emb_trans_dec)), dec_memory=dec_memory)
         self.target_encoder = target_encoder
         self.target_joint_names = list(target_joint_names)     # extended list: goal joints + ['traj', 'heading']
         self.dec = arch == "trans_dec"
+        self.dec_clip = self.dec and dec_memory == _lib.DEC_MEMORY_CLIP
         self.context_len = context_len
         h = ctypes.c_void_p()
         check(self.lib.b200mdm_create(ctypes.byref(self.cfg), ctypes.byref(h)))
@@ -164,6 +166,13 @@ class Engine:
                                            _ptr(out), _stream()))
         return out
 
+    def test_cross_rows(self, timestep, halves, device):
+        """The CLIP decoder's per-step cross-attention rows (b200mdm_test_cross_rows) for the conditioning last set:
+        [num_layers, halves * batch, d] fp32 at model timestep `timestep`."""
+        out = torch.empty(self.cfg.num_layers, halves * self.batch, self.cfg.latent_dim, device=device, dtype=torch.float32)
+        check(self.lib.b200mdm_test_cross_rows(self.h, int(timestep), _ptr(out), _stream()))
+        return out
+
     def _set_cond_enc(self, batch, nframes, y, guided, device):
         text_embed = y.get("text_embed") if y is not None else None
         if isinstance(text_embed, tuple):
@@ -205,23 +214,10 @@ class Engine:
         self._keep["cond"] = (te, sc)
         self.batch, self.nframes = batch, nframes
 
-    def _set_cond_dec(self, batch, nframes, y, guided, device):
-        """DiP: y['text_embed'] = (BERT tokens [Mt,B,768], padding mask [B,Mt] True = pad), y['prefix'] [B,J,F,ctx]
-        (reference model/mdm.py:203-206,210-217,264)."""
-        te = y.get("text_embed")
-        if not isinstance(te, tuple):
-            raise RuntimeError("trans_dec (DiP) needs y['text_embed'] = (tokens, mask) from bert_encode_text "
-                               "(model/mdm.py:180-187)")
-        enc, tmask = te
-        enc = enc.detach().to(device=device, dtype=torch.float32)
-        if enc.shape[1] == 1 and batch > 1:
-            enc = enc.expand(-1, batch, -1)
-        enc = enc.contiguous()
-        if tmask.shape[0] == 1 and batch > 1:                  # model/mdm.py:215-216
-            tmask = torch.repeat_interleave(tmask, batch, dim=0)
-        Mt = enc.shape[0]
-        assert enc.shape == (Mt, batch, self.cfg.cond_dim) and tuple(tmask.shape) == (batch, Mt), (enc.shape, tmask.shape)
-        tm = np.ascontiguousarray(tmask.detach().cpu().numpy().astype(np.uint8))
+    @staticmethod
+    def _lengths_and_scale(batch, y, guided, device):
+        """(lengths int64 numpy or None, scale fp32 device tensor or None) from y['lengths'] / y['mask'] / y['scale']:
+        no key mask when the mask has one column (model/mdm.py:242), lengths from a prefix mask (tensors.py:3-6)."""
         lengths, mask = y.get("lengths"), y.get("mask")
         if mask is not None and mask.shape[-1] <= 1:
             lengths = None
@@ -238,6 +234,54 @@ class Engine:
         if scale is not None:
             sc = scale.detach().to(device=device, dtype=torch.float32).reshape(-1).contiguous()
             assert sc.shape[0] == batch
+        return ln, sc
+
+    def _set_cond_dec_clip(self, batch, nframes, y, guided, device):
+        """trans_dec with emb_trans_dec (humanml-decoder-with-emb): y['text_embed'] = CLIP features [1, B, 512] (or
+        [1, 1, 512] for the whole batch) is the one memory token of each sample (model/mdm.py:218-220,262-264)."""
+        te = y.get("text_embed")
+        if isinstance(te, tuple):
+            raise NotImplementedError("BERT (tokens, mask) conditioning belongs to the DiP decoder (text_encoder_type='bert')")
+        uncond = bool(y.get("uncond", False))
+        if te is None and uncond and not guided:              # mask_cond zeroes the features (model/mdm.py:218)
+            te = torch.zeros(batch, self.cfg.cond_dim, device=device)
+        if te is None:
+            raise RuntimeError("the CLIP decoder needs y['text_embed'] [1, B, %d] (or y['text'] with a text encoder "
+                               "attached)" % self.cfg.cond_dim)
+        te = te.detach().to(device=device, dtype=torch.float32)
+        te = te.reshape(-1, te.shape[-1])
+        if te.shape[0] == 1 and batch > 1:                     # single prompt for the whole batch (sample/predict.py)
+            te = te.expand(batch, -1)
+        te = te.contiguous()
+        assert te.shape == (batch, self.cfg.cond_dim), (te.shape, batch, self.cfg.cond_dim)
+        ln, sc = self._lengths_and_scale(batch, y, guided, device)
+        no_pad = np.zeros((batch, 1), dtype=np.uint8)           # the reference passes no memory mask
+        check(self.lib.b200mdm_set_cond_dec(self.h, batch, nframes, _ptr(te), no_pad.ctypes.data_as(ctypes.c_void_p), 1,
+                                            None if ln is None else ln.ctypes.data_as(ctypes.c_void_p), _ptr(sc),
+                                            int(uncond), _stream()))
+        self._keep["cond"] = (te, sc)
+        self.batch, self.nframes = batch, nframes
+
+    def _set_cond_dec(self, batch, nframes, y, guided, device):
+        """DiP: y['text_embed'] = (BERT tokens [Mt,B,768], padding mask [B,Mt] True = pad), y['prefix'] [B,J,F,ctx]
+        (reference model/mdm.py:203-206,210-217,264)."""
+        if self.dec_clip:
+            return self._set_cond_dec_clip(batch, nframes, y, guided, device)
+        te = y.get("text_embed")
+        if not isinstance(te, tuple):
+            raise RuntimeError("trans_dec (DiP) needs y['text_embed'] = (tokens, mask) from bert_encode_text "
+                               "(model/mdm.py:180-187)")
+        enc, tmask = te
+        enc = enc.detach().to(device=device, dtype=torch.float32)
+        if enc.shape[1] == 1 and batch > 1:
+            enc = enc.expand(-1, batch, -1)
+        enc = enc.contiguous()
+        if tmask.shape[0] == 1 and batch > 1:                  # model/mdm.py:215-216
+            tmask = torch.repeat_interleave(tmask, batch, dim=0)
+        Mt = enc.shape[0]
+        assert enc.shape == (Mt, batch, self.cfg.cond_dim) and tuple(tmask.shape) == (batch, Mt), (enc.shape, tmask.shape)
+        tm = np.ascontiguousarray(tmask.detach().cpu().numpy().astype(np.uint8))
+        ln, sc = self._lengths_and_scale(batch, y, guided, device)
         check(self.lib.b200mdm_set_cond_dec(self.h, batch, nframes, _ptr(enc), tm.ctypes.data_as(ctypes.c_void_p), Mt,
                                             None if ln is None else ln.ctypes.data_as(ctypes.c_void_p), _ptr(sc),
                                             int(bool(y.get("uncond", False))), _stream()))

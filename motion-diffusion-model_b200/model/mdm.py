@@ -6,17 +6,22 @@ shapes, so reference checkpoints load with the reference's own `load_state_dict(
 It uploads them once into the H100 engine (fp16 repack) and calls `b200mdm_denoise`.
 
 Implemented: arch='trans_enc' with cond_mode in {no_cond, text (CLIP features), action}; arch='trans_dec' with
-text_encoder_type='bert' (DiP: BERT token memory, prefix completion, model/mdm.py:203-206,255-270); hml_vec / rot6d /
+text_encoder_type='bert' (DiP: BERT token memory, prefix completion, model/mdm.py:203-206,255-270); arch='trans_dec'
+with text_encoder_type='clip' and emb_trans_dec=True (the humanml-decoder-with-emb checkpoint: timestep token 0, the
+CLIP row + timestep embedding as a one-token memory, mdm.py:256-270; y takes the encoder's keys); hml_vec / rot6d /
 xyz data_rep; target-location conditioning (multi_target_cond, the single / multi / split encoders, model/mdm.py:64-73,
-197-199,399-480) with either arch.
-Not implemented (raise): arch 'gru', data_rep 'rot_vel', emb_trans_dec, emb_policy != 'add', trans_dec with CLIP
-features.
+197-199,399-480) with any of them.
+Not implemented (raise): arch 'gru', data_rep 'rot_vel', emb_policy != 'add', trans_dec with CLIP features and
+emb_trans_dec=False, trans_dec with BERT and emb_trans_dec=True, trans_dec with action / no_cond conditioning.
 """
 import numpy as np
 import torch
 import torch.nn as nn
 
+from .. import _lib
 from ..engine import Engine
+
+_DEC_MEMORY = {"bert": _lib.DEC_MEMORY_TOKENS, "clip": _lib.DEC_MEMORY_CLIP}   # trans_dec: what the cross-attention reads
 
 
 def positional_table(max_len, d_model):
@@ -156,10 +161,17 @@ class MDM(_Bag):
             if "text" in self.cond_mode and self.text_encoder_type != "clip":
                 raise AssertionError("BERT text conditioning requires arch='trans_dec' (model/mdm.py:114)")
         else:
-            if "text" not in self.cond_mode or self.text_encoder_type != "bert" or emb_trans_dec:
-                raise NotImplementedError("arch='trans_dec' is implemented for the DiP configuration: cond_mode='text', "
-                                          "text_encoder_type='bert', emb_trans_dec=False")
-            self.clip_dim = 768                     # model/mdm.py:117
+            text = "text" in self.cond_mode
+            dip = text and self.text_encoder_type == "bert" and not emb_trans_dec
+            clip_dec = text and self.text_encoder_type == "clip" and emb_trans_dec
+            if not (dip or clip_dec):
+                raise NotImplementedError("arch='trans_dec' is implemented for cond_mode='text' with either "
+                                          "text_encoder_type='bert', emb_trans_dec=False (DiP) or text_encoder_type='clip', "
+                                          "emb_trans_dec=True")
+            if clip_dec and self.is_prefix_comp:
+                raise NotImplementedError("prefix completion is implemented for the DiP decoder (text_encoder_type='bert')")
+            if dip:
+                self.clip_dim = 768                 # model/mdm.py:117
 
         for key, shape, kind in _spec(arch, latent_dim, ff_size, num_layers, self.input_feats, self.cond_mode,
                                       self.clip_dim, num_actions):
@@ -223,7 +235,9 @@ class MDM(_Bag):
                                       context_len=self.context_len if self.arch == "trans_dec" else 0,
                                       target_encoder=self.multi_encoder_type if self.multi_target_cond else None,
                                       target_enc_layers=self.target_enc_layers,
-                                      target_joint_names=self.extended_goal_joint_names)
+                                      target_joint_names=self.extended_goal_joint_names,
+                                      emb_trans_dec=self.arch == "trans_dec" and self.emb_trans_dec,
+                                      dec_memory=_DEC_MEMORY[self.text_encoder_type] if self.arch == "trans_dec" else 0)
             self._engine_device = dev
             self._engine_dirty = True
         if self._engine_dirty:

@@ -36,7 +36,8 @@ def get_model_args(args, data):
         "num_layers": args.layers, "num_heads": 4, "dropout": 0.1, "activation": "gelu", "data_rep": data_rep,
         "cond_mode": get_cond_mode(args), "cond_mask_prob": args.cond_mask_prob, "action_emb": "tensor",
         "arch": args.arch, "emb_trans_dec": args.emb_trans_dec, "clip_version": "ViT-B/32", "dataset": args.dataset,
-        "text_encoder_type": args.text_encoder_type, "pos_embed_max_len": args.pos_embed_max_len,
+        # an args.json written before the BERT option has no text_encoder_type: the reference then loads CLIP
+        "text_encoder_type": extra.get("text_encoder_type", "clip"), "pos_embed_max_len": args.pos_embed_max_len,
         "mask_frames": args.mask_frames, "pred_len": args.pred_len, "context_len": args.context_len,
         "emb_policy": extra.get("emb_policy", "add"), "all_goal_joint_names": goal_names,
         # apply_rules (reference utils/parser_util.py:51-53): a target-location loss implies the target encoder
