@@ -26,10 +26,19 @@ HML_TARGET_JOINTS = ["pelvis", "left_foot", "right_foot", "left_wrist", "right_w
 
 def synthetic_state_dict(arch="trans_enc", latent_dim=512, ff_size=1024, num_layers=8, input_feats=263,
                          cond_dim=512, cond_mode="text", num_actions=1, seed=0, target_encoder=None, target_enc_layers=1,
-                         target_joints=HML_TARGET_JOINTS):
+                         target_joints=HML_TARGET_JOINTS, qk_gain=1.0, cross_qk_gain=1.0, ffn_gain=1.0, ln_outliers=0.0):
     """target_encoder ('single' / 'multi' / 'split', args.multi_encoder_type) adds the embed_target_cond.* tensors of
     that encoder (model/mdm.py:399-480) for the extended joint list `target_joints`, drawn from a stream of their own:
-    every other tensor is the same as without them."""
+    every other tensor is the same as without them.
+
+    Stress options for precision tests, applied after every draw (at their defaults the output is the init-scale
+    checkpoint above, bit for bit).  They are stress settings chosen for testing, not statistics measured on a released
+    checkpoint (none is available here); oracle/weight_families.py picks them from the statistic each one targets.
+      qk_gain: the q and k rows of every self-attention in_proj (weight and bias) are scaled by it, so every
+        self-attention logit is scaled by qk_gain**2 (sharper attention);
+      cross_qk_gain: the same for the cross-attention of trans_dec;
+      ffn_gain: linear1 (weight and bias) of every layer is scaled by it, and so is every FFN pre-activation;
+      ln_outliers: this fraction of the channels of every LayerNorm get a bias of +-U(5, 10) (own stream)."""
     rng = np.random.default_rng(seed)
     d = latent_dim
     sd = {}
@@ -98,7 +107,28 @@ def synthetic_state_dict(arch="trans_enc", latent_dim=512, ff_size=1024, num_lay
                 rng.uniform(0.25, 1.0, size=n).astype(np.float32) * np.where(np.arange(n) % 3 == 2, -0.5, 1.0).astype(np.float32))
         else:
             raise ValueError("unsupported target encoder %r" % (target_encoder,))
+    _stress(sd, seed, d, qk_gain, cross_qk_gain, ffn_gain, ln_outliers)
     return sd
+
+
+def _stress(sd, seed, d, qk_gain, cross_qk_gain, ffn_gain, ln_outliers):
+    """The stress options of synthetic_state_dict, in place."""
+    for name, t in list(sd.items()):
+        if ".linear1." in name and ffn_gain != 1.0:
+            sd[name] = t * ffn_gain
+        for key, gain in ((".self_attn.in_proj_", qk_gain), (".multihead_attn.in_proj_", cross_qk_gain)):
+            if key in name and gain != 1.0:
+                t = t.clone()
+                t[: 2 * d] *= gain                # q and k rows; v keeps its scale
+                sd[name] = t
+    if ln_outliers > 0.0:
+        rng = np.random.default_rng([seed, 0x1b5])
+        n = max(1, int(round(ln_outliers * d)))
+        for name in sorted(k for k in sd if ".norm" in k and k.endswith(".bias")):
+            ch = rng.choice(d, size=n, replace=False)
+            t = sd[name].clone()
+            t[ch] = torch.from_numpy((rng.uniform(5.0, 10.0, size=n) * rng.choice([-1.0, 1.0], size=n)).astype(np.float32))
+            sd[name] = t
 
 
 def synthetic_target_inputs(batch, joint_names=HML_TARGET_JOINTS, seed=5):

@@ -9,7 +9,8 @@ memory = text_emb + time_emb, ONE token per sample, no memory mask (:220, :262-2
 (:269-270).  The decoder layers are nn.TransformerDecoderLayer, post-norm (mdm_oracle.decoder_stack).
 
 `cast` rounds every GEMM operand through a narrower dtype, as in mdm_oracle; it exists for the precision study of
-DESIGN.md section 2 and is None for parity work.
+DESIGN.md section 2 and is None for parity work.  `cast=mo.DEC_EMB_SITES` is the site-exact fp16 emulation of the
+engine (mdm_oracle.Sites).
 """
 import torch
 
@@ -19,6 +20,15 @@ from . import mdm_oracle as mo
 def denoise_dec_emb(W, x, t_model, cond, lengths=None, mask_frames=True, uncond=False, g=None, cast=None):
     """x [B,J,F,T]; t_model python int; cond = text_embed [1,B,512] (or [1,1,512]); g [B,d] target embedding or None;
     lengths [B] valid frames or None (=> no key mask)."""
+    B, J, Fe, T = x.shape
+    h, mem, keymask = dec_emb_input(W, x, t_model, cond, lengths, mask_frames, uncond, g, cast)
+    h = mo.decoder_stack(W, h, mem, keymask, None, cast)[:, 1:]
+    out = mo._lin(h, W["output_process.poseFinal.weight"], W["output_process.poseFinal.bias"], cast)
+    return out.reshape(B, T, J, Fe).permute(0, 2, 3, 1).contiguous()
+
+
+def dec_emb_input(W, x, t_model, cond, lengths=None, mask_frames=True, uncond=False, g=None, cast=None):
+    """The decoder stack's inputs of denoise_dec_emb: (h [B, T+1, d], memory [B, 1, d], key mask or None)."""
     B, J, Fe, T = x.shape
     d = W.d
     temb = mo.timestep_embedding(W, t_model)[None, :].expand(B, d)
@@ -34,9 +44,7 @@ def denoise_dec_emb(W, x, t_model, cond, lengths=None, mask_frames=True, uncond=
     keymask = None
     if mask_frames and lengths is not None and T > 1:
         keymask = torch.arange(T + 1)[None, :] >= (lengths[:, None] + 1)
-    h = mo.decoder_stack(W, h, mem, keymask, None, cast)[:, 1:]
-    out = mo._lin(h, W["output_process.poseFinal.weight"], W["output_process.poseFinal.bias"], cast)
-    return out.reshape(B, T, J, Fe).permute(0, 2, 3, 1).contiguous()
+    return h, mem, keymask
 
 
 def cfg_denoise_dec_emb(W, x, t_model, cond, scale, lengths=None, mask_frames=True, g=None, cast=None):

@@ -16,7 +16,9 @@ Pinned against the live reference in tests/test_oracle_cpu.py::test_oracle_vs_li
 container) and by tests/golden/*.npz produced by oracle/gen_golden.py from the reference itself.
 
 `cast` (optional) rounds both GEMM operands through a narrower dtype and back; it exists only for
-the precision studies behind DESIGN.md section 2 and is None for parity work.
+the precision studies behind DESIGN.md section 2 and is None for parity work.  A `Sites` given as `cast` instead
+rounds through fp16 at the named sites alone: with ENC_SITES / DIP_SITES / DEC_EMB_SITES exactly where the engine
+keeps fp16 (the site-exact emulation); with no site it is the plain oracle, bit for bit.
 """
 import math
 
@@ -25,6 +27,34 @@ import torch
 import torch.nn.functional as F
 
 from . import schedule_oracle as so
+
+
+class Sites(frozenset):
+    """fp16 rounding sites of the site-exact emulation (every layer, both CFG halves):
+      qkv_in   the residual stream h as the A operand of the self-attention QKV GEMM
+      qk, v    q and k, and v, after their bias (self-attention)
+      p        the self-attention probabilities P = exp(s - rowmax), rounded before P V; the row sum stays unrounded
+      attn     the self-attention output (A operand of its out-projection)
+      ffn_in   h as the A operand of FFN-up
+      gelu     the GELU output (A operand of FFN-down)
+      weights  the layer weights (QKV, out-projection, linear1, linear2)
+      cross_q_in, cross_q, mem, cross_kv, cross_attn, cross_weights: the same for the trans_dec cross-attention
+               (h into its q projection, q, the memory into its k / v projection, k and v, its output, its weights).
+    Embedding and output projections, the residual stream, LayerNorm and the softmax row sums stay fp32."""
+
+
+ENC_SITES = Sites({"qkv_in", "qk", "v", "p", "attn", "ffn_in", "gelu", "weights"})
+# DiP keeps the self-attention output, the FFN-up input and the GELU output as [hi | lo] pairs (DESIGN.md section 2) and
+# feeds the cross-attention P V with P as hi + lo
+DIP_SITES = Sites({"qkv_in", "qk", "v", "p", "weights", "cross_q_in", "cross_q", "mem", "cross_kv", "cross_attn",
+                   "cross_weights"})
+# the CLIP decoder's one-token cross-attention block runs in fp32 on CUDA cores
+DEC_EMB_SITES = ENC_SITES
+
+
+def _site(z, cast, site):
+    """z through fp16 when `cast` is a Sites holding `site`."""
+    return z.to(torch.float16).float() if isinstance(cast, Sites) and site in cast else z
 
 
 class OracleWeights:
@@ -42,8 +72,10 @@ class OracleWeights:
         return self.sd[k]
 
 
-def _lin(x, w, b, cast=None):
-    if cast is not None:
+def _lin(x, w, b, cast=None, x_site=None, w_site=None):
+    if isinstance(cast, Sites):
+        x, w = _site(x, cast, x_site), _site(w, cast, w_site)
+    elif cast is not None:
         x = x.to(cast).float()
         w = w.to(cast).float()
     y = x @ w.t()
@@ -63,21 +95,29 @@ def _mha_self(h, lw, keymask, H, cast=None):
     """nn.MultiheadAttention self-attention, eval mode.  h [B,S,d]; keymask [B,S] True = ignore."""
     B, S, d = h.shape
     dh = d // H
-    qkv = _lin(h, lw["in_w"], lw["in_b"], cast)
+    qkv = _lin(h, lw["in_w"], lw["in_b"], cast, "qkv_in", "weights")
     q, k, v = qkv.split(d, dim=-1)
     q = q.view(B, S, H, dh).transpose(1, 2)
     k = k.view(B, S, H, dh).transpose(1, 2)
     v = v.view(B, S, H, dh).transpose(1, 2)
-    if cast is not None:
+    if isinstance(cast, Sites):
+        q, k, v = _site(q, cast, "qk"), _site(k, cast, "qk"), _site(v, cast, "v")
+    elif cast is not None:
         q, k, v = (z.to(cast).float() for z in (q, k, v))
     s = (q @ k.transpose(-1, -2)) / math.sqrt(dh)
     if keymask is not None:
         s = s.masked_fill(keymask[:, None, None, :], float("-inf"))
-    p = torch.softmax(s, dim=-1)
-    if cast is not None:
-        p = p.to(cast).float()
-    a = (p @ v).transpose(1, 2).reshape(B, S, d)
-    return _lin(a, lw["out_w"], lw["out_b"], cast)
+    if isinstance(cast, Sites) and "p" in cast:
+        # the engine's attention core: fp16 P against the row maximum, the row sum over the unrounded p
+        e = torch.exp(s - s.amax(-1, keepdim=True))
+        o = (_site(e, cast, "p") @ v) / e.sum(-1, keepdim=True)
+    else:
+        p = torch.softmax(s, dim=-1)
+        if cast is not None and not isinstance(cast, Sites):
+            p = p.to(cast).float()
+        o = p @ v
+    a = o.transpose(1, 2).reshape(B, S, d)
+    return _lin(a, lw["out_w"], lw["out_b"], cast, "attn", "weights")
 
 
 def encoder_stack(W, h, keymask, cast=None):
@@ -89,10 +129,13 @@ def encoder_stack(W, h, keymask, cast=None):
                   out_w=W[p + "self_attn.out_proj.weight"], out_b=W[p + "self_attn.out_proj.bias"])
         a = _mha_self(h, lw, keymask, W.H, cast)
         h = F.layer_norm(h + a, (d,), W[p + "norm1.weight"], W[p + "norm1.bias"], 1e-5)
-        f = F.gelu(_lin(h, W[p + "linear1.weight"], W[p + "linear1.bias"], cast))
-        f = _lin(f, W[p + "linear2.weight"], W[p + "linear2.bias"], cast)
-        h = F.layer_norm(h + f, (d,), W[p + "norm2.weight"], W[p + "norm2.bias"], 1e-5)
+        h = F.layer_norm(h + _ffn(W, p, h, cast), (d,), W[p + "norm2.weight"], W[p + "norm2.bias"], 1e-5)
     return h
+
+
+def _ffn(W, p, h, cast):
+    f = F.gelu(_lin(h, W[p + "linear1.weight"], W[p + "linear1.bias"], cast, "ffn_in", "weights"))
+    return _lin(f, W[p + "linear2.weight"], W[p + "linear2.bias"], cast, "gelu", "weights")
 
 
 def denoise_enc(W, x, t_model, cond, lengths=None, mask_frames=True, uncond=False, action=None, cast=None):
@@ -101,6 +144,15 @@ def denoise_enc(W, x, t_model, cond, lengths=None, mask_frames=True, uncond=Fals
     x [B,J,F,T] fp32; t_model python int (same for the whole batch, gaussian_diffusion.py:709);
     cond: text_embed [1,B,C] (cond_mode text), or None (no_cond); action: [B,1] ints (cond_mode
     action); lengths [B] or None (=> no key mask, mdm.py:241-247)."""
+    B, J, Fe, T = x.shape
+    h, keymask = enc_input(W, x, t_model, cond, lengths, mask_frames, uncond, action, cast)
+    h = encoder_stack(W, h, keymask, cast)[:, 1:]                           # mdm.py:253
+    out = _lin(h, W["output_process.poseFinal.weight"], W["output_process.poseFinal.bias"], cast)
+    return out.reshape(B, T, J, Fe).permute(0, 2, 3, 1).contiguous()        # mdm.py:384-385
+
+
+def enc_input(W, x, t_model, cond, lengths=None, mask_frames=True, uncond=False, action=None, cast=None):
+    """The encoder stack's input of denoise_enc: (h [B, T+1, d], key mask [B, T+1] or None)."""
     B, J, Fe, T = x.shape
     d = W.d
     temb = timestep_embedding(W, t_model)                                   # [d]
@@ -120,9 +172,7 @@ def denoise_enc(W, x, t_model, cond, lengths=None, mask_frames=True, uncond=Fals
     keymask = None
     if mask_frames and lengths is not None and T > 1:                       # mdm.py:241-247
         keymask = torch.arange(T + 1)[None, :] >= (lengths[:, None] + 1)
-    h = encoder_stack(W, h, keymask, cast)[:, 1:]                           # mdm.py:253
-    out = _lin(h, W["output_process.poseFinal.weight"], W["output_process.poseFinal.bias"], cast)
-    return out.reshape(B, T, J, Fe).permute(0, 2, 3, 1).contiguous()        # mdm.py:384-385
+    return h, keymask
 
 
 def cfg_denoise_enc(W, x, t_model, cond, scale, lengths=None, mask_frames=True, action=None, cast=None):
@@ -205,14 +255,14 @@ def _mha_cross(h, mem, lw, mem_mask, H, cast=None):
     dh = d // H
     wq, wk, wv = lw["in_w"].split(d, dim=0)
     bq, bk, bv = lw["in_b"].split(d, dim=0)
-    q = _lin(h, wq, bq, cast).view(B, S, H, dh).transpose(1, 2)
-    k = _lin(mem, wk, bk, cast).view(B, Mt, H, dh).transpose(1, 2)
-    v = _lin(mem, wv, bv, cast).view(B, Mt, H, dh).transpose(1, 2)
+    q = _site(_lin(h, wq, bq, cast, "cross_q_in", "cross_weights"), cast, "cross_q").view(B, S, H, dh).transpose(1, 2)
+    k = _site(_lin(mem, wk, bk, cast, "mem", "cross_weights"), cast, "cross_kv").view(B, Mt, H, dh).transpose(1, 2)
+    v = _site(_lin(mem, wv, bv, cast, "mem", "cross_weights"), cast, "cross_kv").view(B, Mt, H, dh).transpose(1, 2)
     s = (q @ k.transpose(-1, -2)) / math.sqrt(dh)
     if mem_mask is not None:
         s = s.masked_fill(mem_mask[:, None, None, :], float("-inf"))
     a = (torch.softmax(s, dim=-1) @ v).transpose(1, 2).reshape(B, S, d)
-    return _lin(a, lw["out_w"], lw["out_b"], cast)
+    return _lin(a, lw["out_w"], lw["out_b"], cast, "cross_attn", "cross_weights")
 
 
 def decoder_stack(W, h, mem, tgt_keymask, mem_keymask, cast=None):
@@ -225,8 +275,7 @@ def decoder_stack(W, h, mem, tgt_keymask, mem_keymask, cast=None):
                   out_w=W[p + "multihead_attn.out_proj.weight"], out_b=W[p + "multihead_attn.out_proj.bias"])
         h = F.layer_norm(h + _mha_self(h, sa, tgt_keymask, W.H, cast), (d,), W[p + "norm1.weight"], W[p + "norm1.bias"], 1e-5)
         h = F.layer_norm(h + _mha_cross(h, mem, ca, mem_keymask, W.H, cast), (d,), W[p + "norm2.weight"], W[p + "norm2.bias"], 1e-5)
-        f = _lin(F.gelu(_lin(h, W[p + "linear1.weight"], W[p + "linear1.bias"], cast)), W[p + "linear2.weight"], W[p + "linear2.bias"], cast)
-        h = F.layer_norm(h + f, (d,), W[p + "norm3.weight"], W[p + "norm3.bias"], 1e-5)
+        h = F.layer_norm(h + _ffn(W, p, h, cast), (d,), W[p + "norm3.weight"], W[p + "norm3.bias"], 1e-5)
     return h
 
 
@@ -235,6 +284,16 @@ def denoise_dec(W, x, t_model, enc_text, text_mask, prefix, lengths=None, mask_f
 
     x [B,J,F,pred]; prefix [B,J,F,ctx]; enc_text [Mt,B,768]; text_mask [B,Mt] True = padding;
     lengths [B] valid frames of x (the context frames are always valid, mdm.py:204-206)."""
+    B, J, Fe, Tp = x.shape
+    ctx = prefix.shape[-1]
+    h, mem, keymask = dec_input(W, x, t_model, enc_text, prefix, lengths, mask_frames, uncond, cast)
+    h = decoder_stack(W, h, mem, keymask, text_mask, cast)[:, ctx:]
+    out = _lin(h, W["output_process.poseFinal.weight"], W["output_process.poseFinal.bias"], cast)
+    return out.reshape(B, Tp, J, Fe).permute(0, 2, 3, 1).contiguous()
+
+
+def dec_input(W, x, t_model, enc_text, prefix, lengths=None, mask_frames=True, uncond=False, cast=None):
+    """The decoder stack's inputs of denoise_dec: (h [B, ctx+pred, d], memory [B, Mt, d], key mask or None)."""
     B, J, Fe, Tp = x.shape
     ctx = prefix.shape[-1]
     d = W.d
@@ -248,9 +307,7 @@ def denoise_dec(W, x, t_model, enc_text, text_mask, prefix, lengths=None, mask_f
     keymask = None
     if mask_frames and lengths is not None and T > 1:
         keymask = torch.arange(T)[None, :] >= (lengths[:, None] + ctx)
-    h = decoder_stack(W, h, mem, keymask, text_mask, cast)[:, ctx:]
-    out = _lin(h, W["output_process.poseFinal.weight"], W["output_process.poseFinal.bias"], cast)
-    return out.reshape(B, Tp, J, Fe).permute(0, 2, 3, 1).contiguous()
+    return h, mem, keymask
 
 
 def cfg_denoise_dec(W, x, t_model, enc_text, text_mask, prefix, scale, lengths=None, mask_frames=True, cast=None):
