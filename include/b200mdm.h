@@ -147,6 +147,9 @@ int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframes, const fl
  *   enc_text_dev   : y['text_embed'][0], BERT token features [n_tokens, batch, cond_dim] fp32 device (reference layout)
  *   text_mask_host : y['text_embed'][1], uint8 [batch, n_tokens], 1 = padding (memory_key_padding_mask)
  *   nframes        : frames of x (pred_len); the sequence is context_len + nframes tokens, no conditioning token
+ *   n_tokens       : 1..512 (DistilBERT's position limit; B200MDM_EINVAL above).  Up to 64 tokens the cross-attention
+ *                    core holds a sample's keys in registers; above, it streams them in blocks of 64.  The text-memory
+ *                    buffers grow linearly in n_tokens (at 512 tokens and 128 guided rows, ~1.4 GB).
  * lengths / scale / force_uncond as in b200mdm_set_cond.  Must be followed by b200mdm_set_prefix when context_len > 0.
  * dec_memory = B200MDM_DEC_MEMORY_CLIP (emb_trans_dec): enc_text_dev is y['text_embed'] [1, batch, 512], the CLIP row
  * as the one memory token; n_tokens must be 1 (else B200MDM_EINVAL) and text_mask_host all zero (the reference passes
@@ -305,7 +308,9 @@ int b200mdm_test_attention(const void* qkv16_dev, void* out16_dev, const int32_t
 /* Cross-attention core of the trans_dec (DiP) layers, nn.MultiheadAttention(query = sequence, key = value = text memory)
  * between its in- and out-projections (model/mdm.py:219-224 via nn.TransformerDecoderLayer): d = 512, 4 heads.
  * q16 fp16 [n*S, 512]; kv16 fp16 rows (sample, token) of pitch ld_kv >= 1024 holding k | v; mask uint8 [n, n_tokens]
- * (1 = padding token); out16 fp16 [n*S, 1024]: columns [0, 512) are written.  n_tokens <= 64. */
+ * (1 = padding token, any pattern); out16 fp16 [n*S, 1024]: columns [0, 512) are written.  1 <= n_tokens <= 512: the
+ * engine's dispatch, cross_attention_kernel for n_tokens <= 64 and cross_attention_long_kernel above.  Invalid arguments
+ * return B200MDM_EINVAL before any CUDA call. */
 int b200mdm_test_cross_attention(const void* q16_dev, const void* kv16_dev, const unsigned char* mask_dev, void* out16_dev,
                                  int32_t n_samples, int32_t S, int32_t n_tokens, int32_t ld_kv, void* stream);
 /* QKV projection + attention core of an encoder layer (nn.MultiheadAttention up to its output projection,

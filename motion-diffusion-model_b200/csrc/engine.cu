@@ -247,7 +247,11 @@ struct b200mdm_engine : Workspace {
 
 template <class T>
 static int dalloc(T** p, size_t n, bool zero = false) {
-  CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
+  const cudaError_t err = cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T));
+  if (err != cudaSuccess) {
+    cudaGetLastError();   // an out-of-memory error is not sticky: clear it so that later launches do not report it
+    return fail(B200MDM_ECUDA, "cudaMalloc of %zu bytes failed: %s", n * sizeof(T), cudaGetErrorString(err));
+  }
   if (zero) CUDA_TRY(cudaMemset(*p, 0, n * sizeof(T)));
   return B200MDM_OK;
 }
@@ -299,6 +303,7 @@ static int init_kernel_attrs() {
   TRY((set_attention_attr<64>()));
   TRY((set_attention_attr<208>()));
   TRY((set_attention_attr<256>()));
+  CUDA_TRY(cudaFuncSetAttribute(cross_attention_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XAL_SMEM));
   if (dev < 64) done_mask |= 1ull << dev;
   return B200MDM_OK;
 }
@@ -1140,7 +1145,9 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
   if (e->dec_clip)
     return set_cond_dec_clip(e, batch, nframes, enc_text_dev, text_mask_host, n_tokens, lengths_host, scale_dev, force_uncond,
                              static_cast<cudaStream_t>(stream));
-  if (batch <= 0 || nframes <= 0 || n_tokens <= 0 || n_tokens > 64) return fail(B200MDM_EINVAL, "bad batch / nframes / n_tokens (1..64)");
+  if (batch <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
+  if (n_tokens <= 0 || n_tokens > XAL_MAX_MT)
+    return fail(B200MDM_EINVAL, "n_tokens %d: a text memory holds 1..%d tokens (DistilBERT's position limit)", n_tokens, XAL_MAX_MT);
   if (nframes + e->ctx > e->cfg.pos_embed_max_len) return fail(B200MDM_EINVAL, "sequence longer than the positional table");
   if (nframes + e->ctx > ATC_MAX_KEYS) return fail(B200MDM_ENOTIMPL, "sequences of more than %d tokens", ATC_MAX_KEYS);
   if (!enc_text_dev || !text_mask_host) return fail(B200MDM_EINVAL, "DiP needs y['text_embed'] = (tokens, mask)");
@@ -1152,6 +1159,7 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
     CUDA_TRY(cudaDeviceSynchronize());
     drop_graph(e);
     dfree(e->encperm); dfree(e->memtok); dfree(e->memproj); dfree(e->mem16); dfree(e->kvc16); dfree(e->memmask);
+    e->Mt = 0;   // until every buffer below exists: a failed allocation leaves the next call to rebuild them
     TRY(dalloc(&e->encperm, static_cast<size_t>(B) * Mt * C));
     TRY(dalloc(&e->memtok, static_cast<size_t>(B) * Mt * d));
     TRY(dalloc(&e->memproj, static_cast<size_t>(Bp) * Mt * d));
@@ -1345,8 +1353,11 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
           CUDA_TRY(launch_k(cross_attention_kernel<2>, cg, cb, 0, s, e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
         else if (e->Mt <= 32)
           CUDA_TRY(launch_k(cross_attention_kernel<4>, cg, cb, 0, s, e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
-        else
+        else if (e->Mt <= 64)
           CUDA_TRY(launch_k(cross_attention_kernel<8>, cg, cb, 0, s, e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
+        else
+          CUDA_TRY(launch_k(cross_attention_long_kernel, dim3(e->H, e->Bp, (S + XAL_ROWS - 1) / XAL_ROWS), cb, XAL_SMEM, s,
+                            e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
       }
       TRY(launch_gemm_resid_ln(e->m_att, w.m_wo_c_256, e->m_hres, e->M, d, w.bo_c, w.g2, w.be2, s, e->num_sms));   // cross-attention output: hi half
       nk += 3;
@@ -1915,7 +1926,7 @@ extern "C" int b200mdm_test_cross_attention(const void* q16_dev, const void* kv1
                                             void* out16_dev, int32_t n_samples, int32_t S, int32_t n_tokens, int32_t ld_kv,
                                             void* stream) {
   const int d = 512;
-  if (!q16_dev || !kv16_dev || !mask_dev || !out16_dev || n_samples <= 0 || S <= 0 || n_tokens <= 0 || n_tokens > 64 ||
+  if (!q16_dev || !kv16_dev || !mask_dev || !out16_dev || n_samples <= 0 || S <= 0 || n_tokens <= 0 || n_tokens > XAL_MAX_MT ||
       ld_kv < 2 * d || ld_kv % 8)
     return fail(B200MDM_EINVAL, "bad argument");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1926,7 +1937,12 @@ extern "C" int b200mdm_test_cross_attention(const void* q16_dev, const void* kv1
   __half* o = static_cast<__half*>(out16_dev);
   if (n_tokens <= 16) CUDA_TRY(launch_k(cross_attention_kernel<2>, cg, cb, 0, s, q, kv, mask_dev, o, S, n_tokens, d, ld_kv, sl2));
   else if (n_tokens <= 32) CUDA_TRY(launch_k(cross_attention_kernel<4>, cg, cb, 0, s, q, kv, mask_dev, o, S, n_tokens, d, ld_kv, sl2));
-  else CUDA_TRY(launch_k(cross_attention_kernel<8>, cg, cb, 0, s, q, kv, mask_dev, o, S, n_tokens, d, ld_kv, sl2));
+  else if (n_tokens <= 64) CUDA_TRY(launch_k(cross_attention_kernel<8>, cg, cb, 0, s, q, kv, mask_dev, o, S, n_tokens, d, ld_kv, sl2));
+  else {
+    TRY(init_kernel_attrs());
+    CUDA_TRY(launch_k(cross_attention_long_kernel, dim3(d / 128, n_samples, (S + XAL_ROWS - 1) / XAL_ROWS), cb, XAL_SMEM, s, q, kv,
+                      mask_dev, o, S, n_tokens, d, ld_kv, sl2));
+  }
   return B200MDM_OK;
 }
 

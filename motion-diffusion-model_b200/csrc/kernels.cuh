@@ -623,4 +623,182 @@ __global__ void __launch_bounds__(128) cross_attention_kernel(const __half* __re
   }
 }
 
+// Cross-attention core for long text memories (64 < Mt <= 512, DistilBERT's position limit): the interface of
+// cross_attention_kernel, with the keys taken in blocks of 64 instead of all at once in registers.
+//   * each block's K and V rows are staged in shared memory by cp.async, double-buffered: block kb + 1 is in flight
+//     while block kb is used; keys past Mt are zero-filled (never read from global memory) and masked;
+//   * scores: m16n8k16 with the q fragments held in registers for the whole launch.  Thread t of a quad owns the
+//     16-byte chunks t, t + 4, t + 8, t + 12 of the 128 columns, for q and k alike (a dot product does not care about
+//     the order of its terms), so a K row is read as four 16-byte shared-memory loads;
+//   * online softmax in fp32 per query row: a running max m and sum l.  When a block raises m, O and l are scaled by
+//     2^(m_old - m_new) (exactly 1 when m does not move, 0 when m_old = -inf).  While every key so far is masked m
+//     stays -inf and the exponent offset is 0, so p = 0 and no -inf - -inf appears;
+//   * P feeds P.V as hi + lo fp16 like the short core, V fragments come from row-major V by ldmatrix.trans, and O
+//     [16 rows x 128] stays in registers across the blocks (16 n-tiles x 4 fp32 per thread).
+// Shared-memory rows are unpadded: K chunk c of row r sits at c ^ 4 (r & 1), V chunk c at c ^ (r & 7), so a quad pair's
+// 16-byte K loads and an ldmatrix's 8 row addresses each fall in distinct banks.
+// A fully masked row yields 0.  grid = (heads, n_samples, ceil(S / 64)): one 64-row pass per CTA, so every CTA holds
+// one warp tile of O and S = 196 runs as four CTAs per (sample, head), each streaming that head's K / V blocks from L2.
+// block = 128 (4 warps x 16 rows), dynamic shared memory XAL_SMEM.
+constexpr int XAL_KEYS = 64;                 // keys per block
+constexpr int XAL_MAX_MT = 512;
+constexpr int XAL_ROWS = 64;                 // query rows per CTA
+constexpr int XAL_TILE = XAL_KEYS * 128;     // halves of one staged K or V block
+constexpr size_t XAL_SMEM = 2 * 2 * XAL_TILE * sizeof(__half) + 2 * XAL_KEYS * sizeof(float);
+
+__device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
+
+__global__ void __launch_bounds__(128) cross_attention_long_kernel(const __half* __restrict__ q16, const __half* __restrict__ kv16,
+                                                                   const unsigned char* __restrict__ mask,
+                                                                   __half* __restrict__ out16, int S, int Mt, int d, int ld_kv,
+                                                                   float scale_log2) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ __align__(16) unsigned char xal_smem[];
+  __half* sK = reinterpret_cast<__half*>(xal_smem);                    // [2][64 keys][128]
+  __half* sV = sK + 2 * XAL_TILE;                                      // [2][64 keys][128]
+  float* sBias = reinterpret_cast<float*>(sV + 2 * XAL_TILE);          // [2][64]
+  const int h = blockIdx.x, smp = blockIdx.y;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const __half* kv = kv16 + static_cast<size_t>(smp) * Mt * ld_kv + h * 128;
+  const unsigned char* mk = mask + static_cast<size_t>(smp) * Mt;
+  const int nb = (Mt + XAL_KEYS - 1) / XAL_KEYS;
+
+  auto stage = [&](int kb) {
+    const int buf = kb & 1;
+    const uint32_t ks = smem_u32(sK + buf * XAL_TILE), vs = smem_u32(sV + buf * XAL_TILE);
+    for (int i = threadIdx.x; i < XAL_KEYS * 16; i += 128) {
+      const int r = i >> 4, c = i & 15, key = kb * XAL_KEYS + r;
+      const bool in = key < Mt;
+      const __half* src = kv + static_cast<size_t>(in ? key : 0) * ld_kv + c * 8;
+      cp_async16_zfill(ks + 2 * (r * 128 + 8 * (c ^ ((r & 1) << 2))), src, in);
+      cp_async16_zfill(vs + 2 * (r * 128 + 8 * (c ^ (r & 7))), src + d, in);
+    }
+    if (threadIdx.x < XAL_KEYS) {
+      const int key = kb * XAL_KEYS + threadIdx.x;
+      sBias[buf * XAL_KEYS + threadIdx.x] = (key < Mt && !mk[key]) ? 0.f : -INFINITY;
+    }
+    cp_async_commit();
+  };
+  stage(0);
+
+  const int m0 = blockIdx.z * XAL_ROWS + warp * 16, r0 = m0 + g, r1 = r0 + 8;
+  const bool active = m0 < S;                  // idle warps still stage blocks and meet the barriers
+  uint32_t qa[16], qb[16];
+  {
+    const size_t row0 = static_cast<size_t>(smp) * S + min(r0, S - 1), row1 = static_cast<size_t>(smp) * S + min(r1, S - 1);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint4 a = *reinterpret_cast<const uint4*>(q16 + row0 * d + h * 128 + 8 * (4 * i + t));
+      const uint4 b = *reinterpret_cast<const uint4*>(q16 + row1 * d + h * 128 + 8 * (4 * i + t));
+      qa[4 * i] = a.x; qa[4 * i + 1] = a.y; qa[4 * i + 2] = a.z; qa[4 * i + 3] = a.w;
+      qb[4 * i] = b.x; qb[4 * i + 1] = b.y; qb[4 * i + 2] = b.z; qb[4 * i + 3] = b.w;
+    }
+  }
+  float o[16][4];
+#pragma unroll
+  for (int nd = 0; nd < 16; ++nd) o[nd][0] = o[nd][1] = o[nd][2] = o[nd][3] = 0.f;
+  float mx0 = -INFINITY, mx1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // l: this thread's share of the row sums
+
+  for (int kb = 0; kb < nb; ++kb) {
+    if (kb + 1 < nb) {
+      stage(kb + 1);
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    if (active) {
+      const int buf = kb & 1;
+      const __half* kbuf = sK + buf * XAL_TILE;
+      const float* bias = sBias + buf * XAL_KEYS;
+      float sc[8][4];
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        sc[nt][0] = sc[nt][1] = sc[nt][2] = sc[nt][3] = 0.f;
+        const __half* krow = kbuf + (nt * 8 + g) * 128;
+        uint32_t kw[16];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const uint4 a = *reinterpret_cast<const uint4*>(krow + 8 * ((4 * i + t) ^ ((g & 1) << 2)));
+          kw[4 * i] = a.x; kw[4 * i + 1] = a.y; kw[4 * i + 2] = a.z; kw[4 * i + 3] = a.w;
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) mma_m16n8k16(sc[nt], qa[2 * j], qb[2 * j], qa[2 * j + 1], qb[2 * j + 1], kw[2 * j], kw[2 * j + 1]);
+      }
+      // thread holds keys nt*8 + 2t, +1 of rows g (c0, c1) and g+8 (c2, c3)
+      float bm0 = -INFINITY, bm1 = -INFINITY;
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        const float b0 = bias[nt * 8 + 2 * t], b1 = bias[nt * 8 + 2 * t + 1];
+        sc[nt][0] = fmaf(sc[nt][0], scale_log2, b0); sc[nt][1] = fmaf(sc[nt][1], scale_log2, b1);
+        sc[nt][2] = fmaf(sc[nt][2], scale_log2, b0); sc[nt][3] = fmaf(sc[nt][3], scale_log2, b1);
+        bm0 = fmaxf(bm0, fmaxf(sc[nt][0], sc[nt][1]));
+        bm1 = fmaxf(bm1, fmaxf(sc[nt][2], sc[nt][3]));
+      }
+      bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1)); bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
+      bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1)); bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
+      const float mn0 = fmaxf(mx0, bm0), mn1 = fmaxf(mx1, bm1);
+      const float al0 = (mn0 == mx0) ? 1.f : exp2f(mx0 - mn0), al1 = (mn1 == mx1) ? 1.f : exp2f(mx1 - mn1);
+      mx0 = mn0; mx1 = mn1;
+      const float off0 = (mn0 == -INFINITY) ? 0.f : mn0, off1 = (mn1 == -INFINITY) ? 0.f : mn1;
+      float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        sc[nt][0] = exp2f(sc[nt][0] - off0); sc[nt][1] = exp2f(sc[nt][1] - off0);
+        sc[nt][2] = exp2f(sc[nt][2] - off1); sc[nt][3] = exp2f(sc[nt][3] - off1);
+        s0 += sc[nt][0] + sc[nt][1]; s1 += sc[nt][2] + sc[nt][3];
+      }
+      l0 = l0 * al0 + s0; l1 = l1 * al1 + s1;
+#pragma unroll
+      for (int nd = 0; nd < 16; ++nd) {
+        o[nd][0] *= al0; o[nd][1] *= al0; o[nd][2] *= al1; o[nd][3] *= al1;
+      }
+      // P.V: lane addresses row (lane & 7) of ldmatrix matrix lane >> 3 = (keys +8 if odd, columns +8 if >= 2)
+      const uint32_t vbuf = smem_u32(sV + buf * XAL_TILE);
+      const int mi = lane >> 3, lr = lane & 7;
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        uint32_t ph[4], pl[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float x = sc[2 * kk + (j >> 1)][2 * (j & 1)], y = sc[2 * kk + (j >> 1)][2 * (j & 1) + 1];
+          const __half2 hv = __floats2half2_rn(x, y);
+          const float2 hf = __half22float2(hv);
+          ph[j] = *reinterpret_cast<const uint32_t*>(&hv);
+          pl[j] = pack_half2_u32(x - hf.x, y - hf.y);
+        }
+        const int vr = 16 * kk + 8 * (mi & 1) + lr;
+#pragma unroll
+        for (int nd = 0; nd < 16; nd += 2) {
+          uint32_t b[4];
+          ldmatrix_x4_trans(b, vbuf + 2 * (vr * 128 + 8 * ((nd + (mi >> 1)) ^ lr)));
+          mma_16816(o[nd], ph, b[0], b[1]);
+          mma_16816(o[nd], pl, b[0], b[1]);
+          mma_16816(o[nd + 1], ph, b[2], b[3]);
+          mma_16816(o[nd + 1], pl, b[2], b[3]);
+        }
+      }
+    }
+    __syncthreads();   // the next iteration stages block kb + 2 into this buffer
+  }
+  if (!active) return;
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv0 = (mx0 == -INFINITY || !(l0 > 0.f)) ? 0.f : 1.f / l0;
+  const float inv1 = (mx1 == -INFINITY || !(l1 > 0.f)) ? 0.f : 1.f / l1;
+  __half* o0 = out16 + (static_cast<size_t>(smp) * S + r0) * 2 * d + h * 128 + 2 * t;
+  __half* o1 = out16 + (static_cast<size_t>(smp) * S + r1) * 2 * d + h * 128 + 2 * t;
+#pragma unroll
+  for (int nd = 0; nd < 16; ++nd) {
+    if (r0 < S) *reinterpret_cast<__half2*>(o0 + nd * 8) = __floats2half2_rn(o[nd][0] * inv0, o[nd][1] * inv0);
+    if (r1 < S) *reinterpret_cast<__half2*>(o1 + nd * 8) = __floats2half2_rn(o[nd][2] * inv1, o[nd][3] * inv1);
+  }
+}
+
 }  // namespace b200
