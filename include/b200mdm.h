@@ -340,6 +340,35 @@ int b200mdm_test_cross_rows(b200mdm_engine* e, int32_t timestep, float* out_dev,
 int b200mdm_test_row_bias_ln(void* hres16_dev, const float* c_dev, const float* gamma_dev, const float* beta_dev,
                              int32_t M, int32_t S, void* stream);
 
+/* Stage taps of the engine's own forward: one b200mdm_denoise (the same launches, programmatic dependent launch as
+ * configured), and after the launch that produces tap point k the engine copies the workspace buffer behind it into
+ * tap_dev[k] (a caller device buffer of the size below, or NULL to skip it) on `stream`.  Per-layer points (L_*) are taken
+ * for layer `layer` only.  Nothing else changes: no graph, no loop state, no launch count.  A non-NULL buffer for a point
+ * the model does not have, a bad layer or n_taps outside 0..B200MDM_TAP_COUNT return B200MDM_EINVAL before any CUDA call.
+ * Synchronises the stream once (like b200mdm_denoise) before the forward is enqueued.
+ * Sizes, with M = halves*B*S rows (S = T + 1, or context_len + T for DiP), Bp = halves*B, kw = 2 for DiP else 1, Mt the
+ * text tokens, ff = ff_size, d = 512; h = fp16, f = fp32; hres rows are [hi | lo]: */
+#define B200MDM_TAP_EMBED 0     /* h [M, 2d]  residual stream after the embedding GEMM, before token 0 */
+#define B200MDM_TAP_TOK0 1      /* h [M, 2d]  after token 0 / the DiP memory build / the CLIP decoder's cross rows */
+#define B200MDM_TAP_CONDPROJ 2  /* f [Bp, d]  conditioning rows (not DiP) */
+#define B200MDM_TAP_TEMB 3      /* f [B, d]   timestep-embedding rows temb[timesteps[b]] */
+#define B200MDM_TAP_MEM16 4     /* h [Bp*Mt, 2d] DiP: text memory + temb, [hi | lo] */
+#define B200MDM_TAP_CROSS_C 5   /* f [L, Bp, d] CLIP decoder: every layer's cross-attention row of this step */
+#define B200MDM_TAP_KVC16 6     /* h [Bp*Mt, L*2d] DiP: the K | V projections of every layer */
+#define B200MDM_TAP_L_IN 7      /* h [M, 2d]  residual stream at the layer's entry */
+#define B200MDM_TAP_L_QKV 8     /* h [M, 3d]  after the QKV GEMM */
+#define B200MDM_TAP_L_ATT 9     /* h [M, kw*d] after the self-attention core */
+#define B200MDM_TAP_L_LN1 10    /* h [M, 2d]  after out-proj + LN1 */
+#define B200MDM_TAP_L_QC 11     /* h [M, d]   DiP: after the cross-attention Q GEMM */
+#define B200MDM_TAP_L_XATT 12   /* h [M, kw*d] DiP: after the cross-attention core (columns [0, d)) */
+#define B200MDM_TAP_L_LN2 13    /* h [M, 2d]  decoders: after cross out-proj + LN2 (DiP) / the row-bias LN2 (CLIP) */
+#define B200MDM_TAP_L_FFN 14    /* h [M, kw*ff] after FFN-up (GELU) */
+#define B200MDM_TAP_L_LN3 15    /* h [M, 2d]  after FFN-down + LN (norm2, decoders norm3) */
+#define B200MDM_TAP_BLEND 16    /* h [B*T, 3d] CFG blend [hi | lo | hi], the output GEMM's A operand */
+#define B200MDM_TAP_COUNT 17
+int b200mdm_test_forward_taps(b200mdm_engine* e, const float* x_dev, const int32_t* timesteps_host, float* out_dev,
+                              int32_t layer, void* const* tap_dev, int32_t n_taps, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

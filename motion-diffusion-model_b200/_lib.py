@@ -29,8 +29,11 @@ SYMBOLS = [
     "b200mdm_test_gemm_resid_ln", "b200mdm_test_gemm_epi", "b200mdm_test_embed", "b200mdm_test_out_step",
     "b200mdm_set_target", "b200mdm_test_target", "b200mdm_plms_loop_range", "b200mdm_plms_step",
     "b200mdm_set_schedule_next", "b200mdm_ddim_reverse_loop_range", "b200mdm_test_cross_rows",
-    "b200mdm_test_row_bias_ln",
+    "b200mdm_test_row_bias_ln", "b200mdm_test_forward_taps",
 ]
+# tap points of b200mdm_test_forward_taps (B200MDM_TAP_*)
+TAPS = ["EMBED", "TOK0", "CONDPROJ", "TEMB", "MEM16", "CROSS_C", "KVC16", "L_IN", "L_QKV", "L_ATT", "L_LN1", "L_QC",
+        "L_XATT", "L_LN2", "L_FFN", "L_LN3", "BLEND"]
 DEC_MEMORY_TOKENS, DEC_MEMORY_CLIP = 0, 1   # b200mdm_config.dec_memory (trans_dec)
 
 
@@ -101,7 +104,8 @@ def load():
                        ("b200mdm_set_schedule_next", [vp, i32, vp]),
                        ("b200mdm_ddim_reverse_loop_range", [vp, i32, i32, vp, vp, i32, i32, vp]),
                        ("b200mdm_test_cross_rows", [vp, i32, vp, vp]),
-                       ("b200mdm_test_row_bias_ln", [vp, vp, vp, vp, i32, i32, vp])):
+                       ("b200mdm_test_row_bias_ln", [vp, vp, vp, vp, i32, i32, vp]),
+                       ("b200mdm_test_forward_taps", [vp, vp, vp, vp, i32, ctypes.POINTER(vp), i32, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

@@ -1273,8 +1273,70 @@ static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, 
   return launch_gemm<96, EpiOut<OutPlms>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
 }
 
+// Stage outputs requested by b200mdm_test_forward_taps: dst[id] (B200MDM_TAP_*) receives a device copy of the
+// workspace buffer behind tap point id right after the launch that produces it; per-layer points only at `layer`.
+struct ForwardTaps {
+  int layer = 0;
+  void* const* dst = nullptr;
+  int n = 0;
+  const int32_t* t_host = nullptr;   // the forward's timesteps: which temb_table rows B200MDM_TAP_TEMB gathers
+};
+
+// (source, bytes) of tap point id in the current workspace; bytes 0: the model kind has no such buffer.
+static void tap_source(const b200mdm_engine* e, int id, const void** src, size_t* bytes) {
+  const size_t M = e->M, d = e->d, h = sizeof(__half), f = sizeof(float), kw = e->kw, mem = static_cast<size_t>(e->Bp) * e->Mt;
+  const bool dip = e->dec && !e->dec_clip;
+  *src = nullptr;
+  *bytes = 0;
+  switch (id) {
+    case B200MDM_TAP_EMBED: case B200MDM_TAP_TOK0: case B200MDM_TAP_L_IN: case B200MDM_TAP_L_LN1: case B200MDM_TAP_L_LN3:
+      *src = e->hres; *bytes = M * 2 * d * h; break;
+    case B200MDM_TAP_L_LN2:
+      if (e->dec) { *src = e->hres; *bytes = M * 2 * d * h; }
+      break;
+    case B200MDM_TAP_CONDPROJ:
+      if (!dip) { *src = e->condproj; *bytes = static_cast<size_t>(e->Bp) * d * f; }
+      break;
+    case B200MDM_TAP_TEMB: *src = e->temb_table; *bytes = static_cast<size_t>(e->B) * d * f; break;
+    case B200MDM_TAP_MEM16: if (dip) { *src = e->mem16; *bytes = mem * 2 * d * h; } break;
+    case B200MDM_TAP_KVC16: if (dip) { *src = e->kvc16; *bytes = mem * 2 * d * e->L * h; } break;
+    case B200MDM_TAP_CROSS_C:
+      if (e->dec_clip) { *src = e->cross_c; *bytes = static_cast<size_t>(e->L) * e->Bp * d * f; }
+      break;
+    case B200MDM_TAP_L_QKV: *src = e->qkv16; *bytes = M * 3 * d * h; break;
+    case B200MDM_TAP_L_ATT: *src = e->att16; *bytes = M * kw * d * h; break;
+    case B200MDM_TAP_L_QC: if (dip) { *src = e->qc16; *bytes = M * d * h; } break;
+    case B200MDM_TAP_L_XATT: if (dip) { *src = e->att16; *bytes = M * kw * d * h; } break;
+    case B200MDM_TAP_L_FFN: *src = e->ffn16; *bytes = M * kw * e->ff * h; break;
+    case B200MDM_TAP_BLEND: *src = e->g16; *bytes = static_cast<size_t>(e->B) * e->T * 3 * d * h; break;
+  }
+}
+
+// Copy tap points first..last (layer l, or -1 outside the layer loop) into the caller's buffers, on stream s.
+static int take_taps(const b200mdm_engine* e, const ForwardTaps& tp, int first, int last, int l, cudaStream_t s) {
+  if (l >= 0 && l != tp.layer) return B200MDM_OK;
+  for (int id = first; id <= last && id < tp.n; ++id) {
+    if (!tp.dst[id]) continue;
+    const void* src;
+    size_t bytes;
+    tap_source(e, id, &src, &bytes);
+    if (bytes == 0) continue;   // (b200mdm_test_forward_taps rejects such requests up front)
+    if (id == B200MDM_TAP_TEMB) {   // the rows temb_table[t_b] of this forward, b = 0..B-1
+      const size_t row = static_cast<size_t>(e->d) * sizeof(float);
+      for (int b = 0; b < e->B; ++b)
+        CUDA_TRY(cudaMemcpyAsync(static_cast<char*>(tp.dst[id]) + b * row, e->temb_table + static_cast<size_t>(tp.t_host[b]) * e->d,
+                                 row, cudaMemcpyDeviceToDevice, s));
+      continue;
+    }
+    CUDA_TRY(cudaMemcpyAsync(tp.dst[id], src, bytes, cudaMemcpyDeviceToDevice, s));
+  }
+  return B200MDM_OK;
+}
+
 // Enqueue one denoiser forward (+ fused sampler step) on stream s.  Returns the number of kernels launched.
-static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s, int* n_kernels) {
+// taps: stage copies for b200mdm_test_forward_taps, nullptr everywhere else.
+static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s, int* n_kernels,
+                           const ForwardTaps* taps = nullptr) {
   const int d = e->d, ff = e->ff, B = e->B, T = e->T, S = e->S, JF = e->JF, Kp = e->Kp_in;
   int nk = 0;
   PdlScope pdl_scope;
@@ -1298,6 +1360,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     TRY((launch_gemm<128, EpiEmbed>(e->m_xin, e->m_win, e->m_xin, e->MB, d, 3 * Kp, p, s, e->num_sms)));
     ++nk;
   }
+  if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_EMBED, B200MDM_TAP_EMBED, -1, s));
   const float* target_g = e->target_set ? e->tgt_g : nullptr;   // timestep embedding + target (model/mdm.py:197-199)
   if (!e->dec || e->dec_clip) {
     // token 0: cond + (temb + g) (encoder), or the decoder's timestep token (temb + g) without the text (mdm.py:256)
@@ -1320,10 +1383,12 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     ++nk;
   }
   ++nk;
+  if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_TOK0, B200MDM_TAP_KVC16, -1, s));
   const int kw = e->kw;
   const bool wide = kw == 2;
   for (int l = 0; l < e->L; ++l) {
     const LayerW& w = e->layers[l];
+    if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_IN, B200MDM_TAP_L_IN, l, s));
     if (B200_SKIP(1)) {
       ++nk;
     } else {
@@ -1333,9 +1398,12 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
         // projections below read the hi half alone: K = d against the first d columns of [W | W]
         TRY((launch_gemm_bias<false>(e->m_h16, w.m_wqkv, e->m_qkv_st, e->M, 3 * d, d, w.bqkv, s, e->num_sms)));
       }
+      if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_QKV, B200MDM_TAP_L_QKV, l, s));
       TRY(launch_attention_tc(e->m_qkv_kv, e->qkv16, e->att16, e->kvlen, e->Bp, S, d, e->H, s, wide));
+      if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_ATT, B200MDM_TAP_L_ATT, l, s));
     }
     if (!B200_SKIP(2)) TRY(launch_gemm_resid_ln(e->m_att, w.m_wo_256, e->m_hres, e->M, kw * d, w.bo, w.g1, w.be1, s, e->num_sms));
+    if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_LN1, B200MDM_TAP_L_LN1, l, s));
     if (e->dec_clip) {
       // cross-attention block over the one-token memory + norm2: h <- LN2(h + c_l[b'])
       CUDA_TRY(launch_k(row_bias_ln_kernel, dim3((e->M + RBLN_ROWS_PER_CTA - 1) / RBLN_ROWS_PER_CTA), dim3(32 * RBLN_ROWS_PER_CTA),
@@ -1344,6 +1412,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     } else if (e->dec) {
       // cross-attention block of nn.TransformerDecoderLayer: q from the sequence, k/v from the text memory
       TRY((launch_gemm_bias<false>(e->m_h16, w.m_wq_c, e->m_qc_st, e->M, d, d, w.bq_c, s, e->num_sms)));
+      if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_QC, B200MDM_TAP_L_QC, l, s));
       {
         const float sl2 = 1.4426950408889634f / sqrtf(128.0f);
         const dim3 cg(e->H, e->Bp), cb(128);
@@ -1359,22 +1428,27 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
           CUDA_TRY(launch_k(cross_attention_long_kernel, dim3(e->H, e->Bp, (S + XAL_ROWS - 1) / XAL_ROWS), cb, XAL_SMEM, s,
                             e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
       }
+      if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_XATT, B200MDM_TAP_L_XATT, l, s));
       TRY(launch_gemm_resid_ln(e->m_att, w.m_wo_c_256, e->m_hres, e->M, d, w.bo_c, w.g2, w.be2, s, e->num_sms));   // cross-attention output: hi half
       nk += 3;
     }
+    if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_LN2, B200MDM_TAP_L_LN2, l, s));
     if (wide) {
       EpiBiasF16Wide<true>::Params p{w.b1, ff};
       TRY((launch_gemm_pp<EpiBiasF16Wide<true>>(e->m_h16, w.m_w1, e->m_ffn_st, e->M, ff, kw * d, p, s, e->num_sms)));
     } else if (!B200_SKIP(4)) {
       TRY((launch_gemm_bias<true>(e->m_h16, w.m_w1, e->m_ffn_st, e->M, ff, d, w.b1, s, e->num_sms)));
     }
+    if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_FFN, B200MDM_TAP_L_FFN, l, s));
     if (!B200_SKIP(8)) TRY(launch_gemm_resid_ln(e->m_ffn, w.m_w2_256, e->m_hres, e->M, kw * ff, w.b2, e->dec ? w.g3 : w.g2,
                              e->dec ? w.be3 : w.be2, s, e->num_sms));
+    if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_LN3, B200MDM_TAP_L_LN3, l, s));
     nk += 5;
   }
   CUDA_TRY(launch_k(blend_split_kernel, dim3((B * T + 7) / 8), dim3(256), 0, s, e->hres, e->g16, e->scale, B, S, T, e->s_off, d,
                     e->halves));
   ++nk;
+  if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_BLEND, B200MDM_TAP_BLEND, -1, s));
   {
     EpiOutParams p{};
     p.bias = e->b_out;
@@ -1400,14 +1474,16 @@ static int check_ready(b200mdm_engine* e, bool need_sched) {
   return B200MDM_OK;
 }
 
-extern "C" int b200mdm_denoise(b200mdm_engine* e, const float* x_dev, const int32_t* timesteps_host, float* out_dev,
-                               void* stream) {
-  TRY(check_ready(e, false));
-  if (!x_dev || !timesteps_host || !out_dev) return fail(B200MDM_EINVAL, "null tensor");
+static int check_timesteps(const b200mdm_engine* e, const int32_t* timesteps_host) {
   for (int b = 0; b < e->B; ++b)
     if (timesteps_host[b] < 0 || timesteps_host[b] >= e->cfg.temb_rows)
       return fail(B200MDM_EINVAL, "timestep %d outside the pre-embedded range [0, %d)", timesteps_host[b], e->cfg.temb_rows);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  return B200MDM_OK;
+}
+
+// One model forward at explicit per-sample timesteps (b200mdm_denoise; with taps, b200mdm_test_forward_taps).
+static int denoise_forward(b200mdm_engine* e, const float* x_dev, const int32_t* timesteps_host, float* out_dev,
+                           cudaStream_t s, const ForwardTaps* taps, int* n_kernels) {
   CUDA_TRY(cudaMemcpyAsync(e->tvec, timesteps_host, e->B * sizeof(int), cudaMemcpyHostToDevice, s));
   CUDA_TRY(cudaStreamSynchronize(s));  // timesteps_host is caller memory
   StepArgs a;
@@ -1415,10 +1491,41 @@ extern "C" int b200mdm_denoise(b200mdm_engine* e, const float* x_dev, const int3
   a.x_in = x_dev;
   a.x_out = out_dev;
   a.explicit_t = true;
+  return enqueue_forward(e, a, s, n_kernels, taps);
+}
+
+extern "C" int b200mdm_denoise(b200mdm_engine* e, const float* x_dev, const int32_t* timesteps_host, float* out_dev,
+                               void* stream) {
+  TRY(check_ready(e, false));
+  if (!x_dev || !timesteps_host || !out_dev) return fail(B200MDM_EINVAL, "null tensor");
+  TRY(check_timesteps(e, timesteps_host));
   int nk = 0;
-  TRY(enqueue_forward(e, a, s, &nk));
+  TRY(denoise_forward(e, x_dev, timesteps_host, out_dev, static_cast<cudaStream_t>(stream), nullptr, &nk));
   e->launches += nk;
   return B200MDM_OK;
+}
+
+extern "C" int b200mdm_test_forward_taps(b200mdm_engine* e, const float* x_dev, const int32_t* timesteps_host, float* out_dev,
+                                         int32_t layer, void* const* tap_dev, int32_t n_taps, void* stream) {
+  if (!e || !x_dev || !timesteps_host || !out_dev) return fail(B200MDM_EINVAL, "null argument");
+  if (n_taps < 0 || n_taps > B200MDM_TAP_COUNT || (n_taps > 0 && !tap_dev))
+    return fail(B200MDM_EINVAL, "n_taps %d: 0..%d tap buffers (tap_dev may be NULL only with n_taps 0)", n_taps, B200MDM_TAP_COUNT);
+  TRY(check_ready(e, false));
+  if (layer < 0 || layer >= e->L) return fail(B200MDM_EINVAL, "layer %d outside [0, %d)", layer, e->L);
+  TRY(check_timesteps(e, timesteps_host));
+  for (int id = 0; id < n_taps; ++id) {
+    const void* src;
+    size_t bytes;
+    tap_source(e, id, &src, &bytes);
+    if (tap_dev[id] && bytes == 0) return fail(B200MDM_EINVAL, "tap point %d does not exist in this model", id);
+  }
+  ForwardTaps tp;
+  tp.layer = layer;
+  tp.dst = tap_dev;
+  tp.n = n_taps;
+  tp.t_host = timesteps_host;
+  int nk = 0;
+  return denoise_forward(e, x_dev, timesteps_host, out_dev, static_cast<cudaStream_t>(stream), &tp, &nk);
 }
 
 extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t index, const float* x_t_dev,

@@ -82,7 +82,8 @@ class Engine:
         self._cond_key = None
         self._sched_key = None
         self._next_key = None
-        self.batch = self.nframes = 0
+        self.batch = self.nframes = self.n_tokens = 0
+        self.halves = 1
 
     def close(self):
         if getattr(self, "h", None):
@@ -212,7 +213,7 @@ class Engine:
                                         int(uncond), None if ac is None else ac.ctypes.data_as(ctypes.c_void_p),
                                         _stream()))
         self._keep["cond"] = (te, sc)
-        self.batch, self.nframes = batch, nframes
+        self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 2 if sc is not None else 1, 1
 
     @staticmethod
     def _lengths_and_scale(batch, y, guided, device):
@@ -260,7 +261,7 @@ class Engine:
                                             None if ln is None else ln.ctypes.data_as(ctypes.c_void_p), _ptr(sc),
                                             int(uncond), _stream()))
         self._keep["cond"] = (te, sc)
-        self.batch, self.nframes = batch, nframes
+        self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 2 if sc is not None else 1, 1
 
     def _set_cond_dec(self, batch, nframes, y, guided, device):
         """DiP: y['text_embed'] = (BERT tokens [Mt,B,768], padding mask [B,Mt] True = pad), y['prefix'] [B,J,F,ctx]
@@ -293,7 +294,7 @@ class Engine:
             assert tuple(pf.shape) == (batch, self.cfg.njoints, self.cfg.nfeats, self.context_len), pf.shape
             check(self.lib.b200mdm_set_prefix(self.h, _ptr(pf), _stream()))
         self._keep["cond"] = (enc, sc, pf)
-        self.batch, self.nframes = batch, nframes
+        self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 2 if sc is not None else 1, Mt
 
     def set_inpaint(self, mask, motion):
         if mask is None:
@@ -313,6 +314,41 @@ class Engine:
         out = torch.empty_like(x)
         check(self.lib.b200mdm_denoise(self.h, _ptr(x), ts.ctypes.data_as(ctypes.c_void_p), _ptr(out), _stream()))
         return out
+
+    def tap_shapes(self):
+        """{tap name: (shape, dtype)} of every b200mdm_test_forward_taps point the current model and workspace have
+        (include/b200mdm.h, B200MDM_TAP_*)."""
+        c = self.cfg
+        d, ff, L, B, T, Bp = c.latent_dim, c.ff_size, c.num_layers, self.batch, self.nframes, self.halves * self.batch
+        dip = self.dec and not self.dec_clip
+        S = T + (self.context_len if dip else 1)
+        M, kw, mem, h, f = Bp * S, 2 if dip else 1, Bp * self.n_tokens, torch.float16, torch.float32
+        out = dict(EMBED=((M, 2 * d), h), TOK0=((M, 2 * d), h), TEMB=((B, d), f), L_IN=((M, 2 * d), h),
+                   L_QKV=((M, 3 * d), h), L_ATT=((M, kw * d), h), L_LN1=((M, 2 * d), h), L_FFN=((M, kw * ff), h),
+                   L_LN3=((M, 2 * d), h), BLEND=((B * T, 3 * d), h))
+        if not dip:
+            out["CONDPROJ"] = ((Bp, d), f)
+        if self.dec:
+            out["L_LN2"] = ((M, 2 * d), h)
+        if self.dec_clip:
+            out["CROSS_C"] = ((L, Bp, d), f)
+        if dip:
+            out.update(MEM16=((mem, 2 * d), h), KVC16=((mem, L * 2 * d), h), L_QC=((M, d), h), L_XATT=((M, kw * d), h))
+        return out
+
+    def forward_taps(self, x, timesteps, layer, names=None):
+        """One forward as denoise() does, with the stage outputs of b200mdm_test_forward_taps: (out, {tap name: tensor})
+        for the points in `names` (default: every point of this model), per-layer points at `layer`."""
+        x = x.to(torch.float32).contiguous()
+        ts = np.ascontiguousarray(timesteps.detach().reshape(-1).cpu().numpy().astype(np.int32))
+        assert ts.shape[0] == x.shape[0]
+        shapes = self.tap_shapes()
+        taps = {n: torch.empty(*shapes[n][0], device=x.device, dtype=shapes[n][1]) for n in (names or shapes)}
+        ptrs = (ctypes.c_void_p * len(_lib.TAPS))(*[taps[n].data_ptr() if n in taps else None for n in _lib.TAPS])
+        out = torch.empty_like(x)
+        check(self.lib.b200mdm_test_forward_taps(self.h, _ptr(x), ts.ctypes.data_as(ctypes.c_void_p), _ptr(out), int(layer),
+                                                 ptrs, len(_lib.TAPS), _stream()))
+        return out, taps
 
     def sample_step(self, mode, index, x_t, noise, flags=0, want_pred=True):
         """noise may be None for MODE_DDIM_REVERSE, which draws none."""

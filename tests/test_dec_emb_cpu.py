@@ -3,6 +3,8 @@ emb_trans_dec=True) -- the fp32 oracle against the reference's fixtures, the hos
 config layout, the configurations that still raise and the C-ABI rejections that happen before any CUDA call."""
 import ctypes
 import importlib
+import os
+import re
 from types import SimpleNamespace
 
 import numpy as np
@@ -11,7 +13,7 @@ import torch
 
 import b200mdm
 from b200mdm import _lib
-from conftest import default_args, rel_err
+from conftest import ROOT, default_args, rel_err
 from oracle import dec_emb_oracle as deo, mdm_oracle as mo, schedule_oracle as so, target_oracle as to
 
 syn = importlib.import_module("motion-diffusion-model_b200.synthetic")
@@ -161,3 +163,19 @@ def test_test_hooks_reject_bad_arguments_without_gpu():
     lib = _lib.load()
     assert lib.b200mdm_test_cross_rows(None, 0, None, None) == _lib.EINVAL
     assert lib.b200mdm_test_row_bias_ln(None, None, None, None, 8, 4, None) == _lib.EINVAL
+
+
+def test_forward_taps_rejects_bad_arguments_without_gpu():
+    """b200mdm_test_forward_taps validates its arguments before any CUDA call; the tap ids are the header's."""
+    lib = _lib.load()
+    hdr = open(os.path.join(ROOT, "include", "b200mdm.h")).read()
+    ids = {m[0]: int(m[1]) for m in re.findall(r"#define B200MDM_TAP_([A-Z0-9_]+) (\d+)", hdr)}
+    assert ids.pop("COUNT") == len(_lib.TAPS) and ids == {n: i for i, n in enumerate(_lib.TAPS)}
+    buf = (ctypes.c_float * 4)()
+    ts = (ctypes.c_int32 * 1)()
+    taps = (ctypes.c_void_p * len(_lib.TAPS))()
+    fn = lib.b200mdm_test_forward_taps
+    assert fn(None, buf, ts, buf, 0, taps, len(_lib.TAPS), None) == _lib.EINVAL
+    assert b"null" in lib.b200mdm_last_error()
+    for x, t, out in ((None, ts, buf), (buf, None, buf), (buf, ts, None)):
+        assert fn(None, x, t, out, 0, taps, 1, None) == _lib.EINVAL
