@@ -43,7 +43,8 @@ extern "C" {
 #define B200MDM_MODE_X0 0   /* model output only */
 #define B200MDM_MODE_DDPM 1 /* p_sample */
 #define B200MDM_MODE_DDIM 2 /* ddim_sample */
-/* (3-5: the PLMS steps inside b200mdm_plms_loop_range / b200mdm_plms_step; not valid modes of the calls below) */
+/* (3-5: the PLMS steps inside b200mdm_plms_loop_range / b200mdm_plms_step, 7: the DPM-Solver++ step inside
+ * b200mdm_dpm_loop_range; not valid modes of the calls below) */
 #define B200MDM_MODE_DDIM_REVERSE 6 /* ddim_reverse_sample: b200mdm_sample_step only (noise_dev may be NULL) */
 
 #define B200MDM_FLAG_CONST_NOISE 1   /* p_sample(const_noise=True): eps row 0 repeated (gaussian_diffusion.py:527-528) */
@@ -129,6 +130,15 @@ int b200mdm_set_schedule(b200mdm_engine* e, int32_t n_steps, const float* rows_h
  * fails with B200MDM_ESTATE.  Synchronous copy. */
 #define B200MDM_SCHED_NEXT_STRIDE 2
 int b200mdm_set_schedule_next(b200mdm_engine* e, int32_t n_steps, const float* rows_host);
+
+/* The DPM-Solver++ table (no reference counterpart; DESIGN.md section 1), n_steps rows of
+ *   [0] c_x = sigma_{i-1}/sigma_i  [1] c0 = alpha_{i-1} - alpha_i*sigma_{i-1}/sigma_i  [2] c_cur = c0*(1 + 1/(2r))
+ *   [3] c_prev = -c0/(2r)
+ * with alpha = sqrt(ac), sigma = sqrt(1 - ac), target index i - 1 taken from alphas_cumprod_prev, r = h_prev / h the
+ * ratio of the log-SNR steps, every value computed in fp64 and rounded once.  Row 0 is (0, 1, ., .).  Staleness as for
+ * b200mdm_set_schedule_next.  Synchronous copy. */
+#define B200MDM_SCHED_DPM_STRIDE 4
+int b200mdm_set_schedule_dpm(b200mdm_engine* e, int32_t n_steps, const float* rows_host);
 
 /* Canonicalises model_kwargs['y'] (data_loaders/tensors.py:22-64 + callers) once per loop and (re)builds the
  * workspace for (batch, nframes):
@@ -236,6 +246,21 @@ int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order, const flo
                       int32_t n_old, int32_t flags, float* x_out_dev, float* pred_xstart_dev, float* eps_out_dev,
                       void* stream);
 
+/* Multistep DPM-Solver++ in its data-prediction form (Lu et al. 2022, Algorithm 2; no reference counterpart) without
+ * returning to the host: schedule indices first_index, first_index-1, ... (n_run of them) on the engine's working
+ * buffer, order 1 or 2, each step one forward (one CUDA graph per order, replayed, when use_graph != 0).  Step k of a
+ * loop at index i: x0 as the DDIM step forms it (CFG, inpainting, clamp), kept in slot k % 2 of an x0 history, then
+ *   x_out = fmaf(c0, x0, c_x*x)                                   at k == 0, i == 0 or order 1,
+ *   x_out = fmaf(c_prev, x0 of step k - 1, fmaf(c_cur, x0, c_x*x)) otherwise (2M),
+ * from row i of the b200mdm_set_schedule_dpm table (stale table -> B200MDM_ESTATE).  x_in_dev != NULL starts a fresh
+ * loop (k = 0); NULL continues the DPM-Solver++ loop the previous call of the same order left in the engine, history
+ * included; x_out_dev NULL leaves the result there.  flags: B200MDM_FLAG_CLIP_DENOISED or 0.  No noise is drawn.  The
+ * history (2 x [B, JF, T] fp32) is allocated in the workspace on first use. */
+int b200mdm_dpm_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index, int32_t n_run, const float* x_in_dev,
+                           float* x_out_dev, int32_t flags, int32_t use_graph, void* stream);
+/* out_dev [B, JF, T] fp32 <- the x0 (pred_xstart) of the last step of that loop.  Enqueued on `stream`. */
+int b200mdm_dpm_pred_xstart(b200mdm_engine* e, float* out_dev, void* stream);
+
 /* The engine's own noise stream (no reference counterpart: the reference draws from torch's global generator).
  * Philox4x32-10 keyed by `seed`, counter = (element/4, schedule index of the consuming step, global sample index);
  * Box-Muller on the 4 output words (exact recipe: csrc/kernels.cuh, restated in oracle/philox_oracle.py).  A sample's
@@ -299,6 +324,16 @@ int b200mdm_test_out_step(const void* hres16_dev, const float* scale_dev, const 
                           const uint8_t* inpaint_mask_dev, const float* inpaint_motion_dev, float* x_out_dev,
                           float* pred_xstart_dev, int32_t B, int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves,
                           void* stream);
+/* The same output launches with the EpiOut<OutDpm> epilogue of b200mdm_dpm_loop_range, as step `step` (k) of a loop of
+ * order 1 or 2 at schedule index `index`: dpm_row (4 floats, device; see b200mdm_set_schedule_dpm) is row `index` of
+ * the table.  x0_hist fp32 [2, B, JF, T]: slot (k - 1) % 2 is read as the previous x0 (second-order steps only), slot
+ * k % 2 receives this step's x0; x_out [B, JF, T] (may alias x_t) the update.  flags: B200MDM_FLAG_CLIP_DENOISED or 0;
+ * other arguments as in b200mdm_test_out_step.  Invalid arguments return B200MDM_EINVAL before any CUDA call. */
+int b200mdm_test_out_dpm(const void* hres16_dev, const float* scale_dev, const float* w_out_dev, const float* b_out_dev,
+                         const float* x_t_dev, const float* dpm_row_dev, int32_t index, int32_t step, int32_t order,
+                         int32_t flags, const uint8_t* inpaint_mask_dev, const float* inpaint_motion_dev,
+                         float* x0_hist_dev, float* x_out_dev, int32_t B, int32_t JF, int32_t T, int32_t d, int32_t s_off,
+                         int32_t halves, void* stream);
 /* Self-attention core (tensor-core kernel, S <= 256): softmax(q k^T / sqrt(128) + mask) v per (sample, head);
  * qkv16 [n*S, 3d]; kvlen int32 [n] device (valid keys per sample, a prefix).
  * impl 0: out16 fp16 [n*S, d] (the encoder); impl 1: out16 fp16 [n*S, 2d] = [hi | lo] with hi + lo = the fp32 result

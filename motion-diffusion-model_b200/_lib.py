@@ -17,6 +17,7 @@ MODE_DDIM_REVERSE = 6   # (3-5 are the PLMS steps inside the PLMS calls)
 FLAG_CONST_NOISE, FLAG_CLIP_DENOISED, FLAG_PHILOX_NOISE = 1, 2, 4
 SCHED_STRIDE = 8
 SCHED_NEXT_STRIDE = 2
+SCHED_DPM_STRIDE = 4
 
 # every symbol include/b200mdm.h declares (tests check that the library exports all of them)
 SYMBOLS = [
@@ -30,6 +31,7 @@ SYMBOLS = [
     "b200mdm_set_target", "b200mdm_test_target", "b200mdm_plms_loop_range", "b200mdm_plms_step",
     "b200mdm_set_schedule_next", "b200mdm_ddim_reverse_loop_range", "b200mdm_test_cross_rows",
     "b200mdm_test_row_bias_ln", "b200mdm_test_forward_taps",
+    "b200mdm_set_schedule_dpm", "b200mdm_dpm_loop_range", "b200mdm_dpm_pred_xstart", "b200mdm_test_out_dpm",
 ]
 # tap points of b200mdm_test_forward_taps (B200MDM_TAP_*)
 TAPS = ["EMBED", "TOK0", "CONDPROJ", "TEMB", "MEM16", "CROSS_C", "KVC16", "L_IN", "L_QKV", "L_ATT", "L_LN1", "L_QC",
@@ -105,7 +107,12 @@ def load():
                        ("b200mdm_ddim_reverse_loop_range", [vp, i32, i32, vp, vp, i32, i32, vp]),
                        ("b200mdm_test_cross_rows", [vp, i32, vp, vp]),
                        ("b200mdm_test_row_bias_ln", [vp, vp, vp, vp, i32, i32, vp]),
-                       ("b200mdm_test_forward_taps", [vp, vp, vp, vp, i32, ctypes.POINTER(vp), i32, vp])):
+                       ("b200mdm_test_forward_taps", [vp, vp, vp, vp, i32, ctypes.POINTER(vp), i32, vp]),
+                       ("b200mdm_set_schedule_dpm", [vp, i32, vp]),
+                       ("b200mdm_dpm_loop_range", [vp, i32, i32, i32, vp, vp, i32, i32, vp]),
+                       ("b200mdm_dpm_pred_xstart", [vp, vp, vp]),
+                       ("b200mdm_test_out_dpm", [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp,
+                                                 i32, i32, i32, i32, i32, i32, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

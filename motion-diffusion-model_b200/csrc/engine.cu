@@ -183,6 +183,10 @@ struct Workspace {
   // its second forward) and its first x0.  plms_done = evaluations of the PLMS loop in flight (-1: none to continue).
   float *plms_ring = nullptr, *plms_mid = nullptr, *plms_pred = nullptr;
   int plms_done = -1, plms_order = 0;
+  // DPM-Solver++, allocated on first use: x0 history [DPM_SLOTS, B, JF, T].  dpm_done = evaluations of the DPM loop in
+  // flight (-1: none to continue).
+  float* dpm_hist = nullptr;
+  int dpm_done = -1, dpm_order = 0;
   // captured step graph of this workspace
   cudaGraphExec_t graph_exec = nullptr;
   GraphKey graph_key;
@@ -219,6 +223,10 @@ struct b200mdm_engine : Workspace {
   // b200mdm_set_schedule makes it stale until the next b200mdm_set_schedule_next
   float* sched_next = nullptr;
   bool sched_next_fresh = false;
+  // DPM-Solver++: c_x, c0, c_cur, c_prev per row (b200mdm_set_schedule_dpm), allocated with `sched`, stale in the same
+  // way as sched_next
+  float* sched_dpm = nullptr;
+  bool sched_dpm_fresh = false;
   // parked workspaces (see Workspace)
   std::vector<Workspace> pool;
   unsigned long long use_clock = 0;
@@ -300,6 +308,7 @@ static int init_kernel_attrs() {
   TRY((set_gemm_attr<96, EpiOut<OutStep>>()));
   TRY((set_gemm_attr<96, EpiOut<OutPlms>>()));
   TRY((set_gemm_attr<96, EpiOut<OutReverse>>()));
+  TRY((set_gemm_attr<96, EpiOut<OutDpm>>()));
   TRY((set_attention_attr<64>()));
   TRY((set_attention_attr<208>()));
   TRY((set_attention_attr<256>()));
@@ -524,6 +533,7 @@ static void free_workspace(Workspace* w) {
   dfree(w->cross_mb); dfree(w->cross_u); dfree(w->cross_b); dfree(w->cross_c);
   dfree(w->tgt_valid); dfree(w->tgt_g);
   dfree(w->plms_ring); dfree(w->plms_mid); dfree(w->plms_pred);
+  dfree(w->dpm_hist);
   *w = Workspace();
 }
 // every workspace (the one in use and the parked ones): after a weight reload or a schedule-table move their graphs
@@ -545,7 +555,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   for (auto& kv : e->store) cudaFree(kv.second.dev);
   for (auto& l : e->layers) { dfree(l.wqkv); dfree(l.wo); dfree(l.w1); dfree(l.w2); dfree(l.wq_c); dfree(l.wo_c); }
   dfree(e->w_in3); dfree(e->w_out3); dfree(e->temb_hidden); dfree(e->temb_table); dfree(e->sched); dfree(e->tmap);
-  dfree(e->sched_next);
+  dfree(e->sched_next); dfree(e->sched_dpm);
   dfree(e->wkv_all); dfree(e->bkv_all); dfree(e->cross_t);
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
@@ -860,15 +870,18 @@ extern "C" int b200mdm_set_schedule(b200mdm_engine* e, int32_t n_steps, const fl
     dfree(e->sched);
     dfree(e->tmap);
     dfree(e->sched_next);
+    dfree(e->sched_dpm);
     e->sched_cap = 0;
     const int cap = n_steps > 1000 ? n_steps : 1000;
     TRY(dalloc(&e->sched, static_cast<size_t>(cap) * SCHED_STRIDE));
     TRY(dalloc(&e->tmap, cap));
     TRY(dalloc(&e->sched_next, static_cast<size_t>(cap) * SCHED_NEXT_STRIDE));
+    TRY(dalloc(&e->sched_dpm, static_cast<size_t>(cap) * SCHED_DPM_STRIDE));
     e->sched_cap = cap;
   }
   e->n_steps = n_steps;
   e->sched_next_fresh = false;
+  e->sched_dpm_fresh = false;
   CUDA_TRY(cudaMemcpy(e->sched, rows_host, static_cast<size_t>(n_steps) * SCHED_STRIDE * sizeof(float), cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(e->tmap, timestep_map_host, static_cast<size_t>(n_steps) * sizeof(int), cudaMemcpyHostToDevice));
   return B200MDM_OK;
@@ -887,6 +900,19 @@ extern "C" int b200mdm_set_schedule_next(b200mdm_engine* e, int32_t n_steps, con
   CUDA_TRY(cudaMemcpy(e->sched_next, rows_host, static_cast<size_t>(n_steps) * SCHED_NEXT_STRIDE * sizeof(float),
                       cudaMemcpyHostToDevice));
   e->sched_next_fresh = true;
+  return B200MDM_OK;
+}
+
+static_assert(SCHED_DPM_STRIDE == B200MDM_SCHED_DPM_STRIDE, "the DPM-Solver++ table's row layout is part of the ABI");
+extern "C" int b200mdm_set_schedule_dpm(b200mdm_engine* e, int32_t n_steps, const float* rows_host) {
+  if (!e || !rows_host) return fail(B200MDM_EINVAL, "bad argument");
+  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
+  if (n_steps != e->n_steps)
+    return fail(B200MDM_EINVAL, "n_steps %d differs from the schedule's %d", n_steps, e->n_steps);
+  CUDA_TRY(cudaDeviceSynchronize());  // a DPM loop still in flight may be reading the old rows
+  CUDA_TRY(cudaMemcpy(e->sched_dpm, rows_host, static_cast<size_t>(n_steps) * SCHED_DPM_STRIDE * sizeof(float),
+                      cudaMemcpyHostToDevice));
+  e->sched_dpm_fresh = true;
   return B200MDM_OK;
 }
 
@@ -1270,6 +1296,7 @@ static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, 
   const int M = B * T, N = ((JF + 95) / 96) * 96, K = 3 * d;
   if (a.mode <= MODE_DDIM) return launch_gemm<96, EpiOut<OutStep>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
   if (a.mode == MODE_DDIM_REVERSE) return launch_gemm<96, EpiOut<OutReverse>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
+  if (a.mode == MODE_DPM) return launch_gemm<96, EpiOut<OutDpm>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
   return launch_gemm<96, EpiOut<OutPlms>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
 }
 
@@ -1456,7 +1483,9 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     p.inpaint_motion = e->inpaint_motion;
     p.sched = e->sched;
     p.sched_next = e->sched_next;
+    p.sched_dpm = e->sched_dpm;
     p.eps_ring = e->plms_ring;
+    p.x0_hist = e->dpm_hist;
     p.state = e->state;
     TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, a, p, s, e->num_sms));
     ++nk;
@@ -1648,7 +1677,8 @@ static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
     CUDA_TRY(cudaStreamWaitEvent(e->work, e->ev_in, 0));
   }
-  e->plms_done = -1;   // x_work no longer holds a PLMS loop to continue
+  e->plms_done = -1;   // x_work no longer holds a PLMS or DPM-Solver++ loop to continue
+  e->dpm_done = -1;
   if (x_in_dev) CUDA_TRY(cudaMemcpyAsync(e->x_work, x_in_dev, x_bytes, cudaMemcpyDeviceToDevice, s));
   step_set_kernel<<<1, 1, 0, s>>>(e->state, done, first_index, noise_tape_dev, noise_step_stride, e->noise_seed,
                                   e->noise_sample_base, e->n_steps);
@@ -1663,6 +1693,9 @@ static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t
   if (a.mode == MODE_PLMS_AB) {
     e->plms_done = done + n_run;
     e->plms_order = a.order;
+  } else if (a.mode == MODE_DPM) {
+    e->dpm_done = done + n_run;
+    e->dpm_order = a.order;
   }
   if (x_out_dev) CUDA_TRY(cudaMemcpyAsync(x_out_dev, e->x_work, x_bytes, cudaMemcpyDeviceToDevice, s));
   if (use_graph) {
@@ -1807,6 +1840,43 @@ extern "C" int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order
   }
   if (eps_out_dev)
     CUDA_TRY(cudaMemcpyAsync(eps_out_dev, e->plms_ring + (h % PLMS_RING) * n, x_bytes, cudaMemcpyDeviceToDevice, s));
+  return B200MDM_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ DPM-Solver++
+// Multistep DPM-Solver++ (data prediction) at schedule indices first_index, first_index-1, ... (n_run of them) on the
+// engine's working buffer: the launches of a DDIM step without the noise draw, one graph per order.  The step counter
+// k = StepState::done selects the history slots and the first-order first step.
+extern "C" int b200mdm_dpm_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index, int32_t n_run,
+                                      const float* x_in_dev, float* x_out_dev, int32_t flags, int32_t use_graph,
+                                      void* stream) {
+  if (order < 1 || order > 2) return fail(B200MDM_EINVAL, "DPM-Solver++ order %d is not 1 or 2", order);
+  if (flags & ~B200MDM_FLAG_CLIP_DENOISED)
+    return fail(B200MDM_EINVAL, "DPM-Solver++ takes no flag but B200MDM_FLAG_CLIP_DENOISED");
+  if (n_run <= 0) return fail(B200MDM_EINVAL, "bad step range");
+  TRY(check_ready(e, true));
+  if (first_index >= e->n_steps || first_index - n_run + 1 < 0) return fail(B200MDM_EINVAL, "bad step range");
+  if (!e->sched_dpm_fresh)
+    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_dpm has not been called for the current schedule");
+  if (!x_in_dev && (e->dpm_done < 0 || e->dpm_order != order))
+    return fail(B200MDM_ESTATE, "no DPM-Solver++ loop of order %d to continue (pass x_in_dev)", order);
+  if (!e->dpm_hist) TRY(dalloc(&e->dpm_hist, DPM_SLOTS * static_cast<size_t>(e->B) * e->JF * e->T));
+  StepArgs a;
+  a.mode = MODE_DPM;
+  a.order = order;
+  a.x_in = e->x_work;
+  a.x_out = e->x_work;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  const int done = x_in_dev ? 0 : e->dpm_done;
+  return run_loop(e, a, flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0, use_graph, stream, done);
+}
+
+extern "C" int b200mdm_dpm_pred_xstart(b200mdm_engine* e, float* out_dev, void* stream) {
+  if (!e || !out_dev) return fail(B200MDM_EINVAL, "null argument");
+  if (e->dpm_done <= 0 || !e->dpm_hist) return fail(B200MDM_ESTATE, "no DPM-Solver++ loop has run a step");
+  const size_t n = static_cast<size_t>(e->B) * e->JF * e->T;
+  CUDA_TRY(cudaMemcpyAsync(out_dev, e->dpm_hist + static_cast<size_t>((e->dpm_done - 1) & 1) * n, n * sizeof(float),
+                           cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
   return B200MDM_OK;
 }
 
@@ -2013,6 +2083,57 @@ extern "C" int b200mdm_test_out_step(const void* hres16_dev, const float* scale_
   a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
   a.x_out = x_out_dev;
   a.pred = pred_xstart_dev;
+  return launch_out_gemm(m_g16, m_wout, B, T, JF, d, a, p, s, sms);
+}
+
+extern "C" int b200mdm_test_out_dpm(const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
+                                    const float* b_out_dev, const float* x_t_dev, const float* dpm_row_dev, int32_t index,
+                                    int32_t step, int32_t order, int32_t flags, const uint8_t* inpaint_mask_dev,
+                                    const float* inpaint_motion_dev, float* x0_hist_dev, float* x_out_dev, int32_t B,
+                                    int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream) {
+  if (!hres16_dev || !w_out_dev || !b_out_dev || !x_t_dev || !dpm_row_dev || !x0_hist_dev || !x_out_dev || B <= 0 ||
+      JF <= 0 || T <= 0 || s_off < 0 || d <= 0 || d % 64 || (halves != 1 && halves != 2) || (halves == 2 && !scale_dev) ||
+      index < 0 || step < 0 || (order != 1 && order != 2) || (flags & ~B200MDM_FLAG_CLIP_DENOISED) ||
+      (inpaint_mask_dev == nullptr) != (inpaint_motion_dev == nullptr))
+    return fail(B200MDM_EINVAL, "bad argument");
+  TRY(init_kernel_attrs());
+  int sms = 132;
+  TRY(device_sms(&sms));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int S = T + s_off, N_out_pad = ((JF + 95) / 96) * 96;
+  StreamScratch scr(s);
+  __half *g16 = nullptr, *w_out3 = nullptr;
+  float* table = nullptr;
+  StepState* st = nullptr;
+  TRY(scr.alloc(&g16, static_cast<size_t>(B) * T * 3 * d));
+  TRY(scr.alloc(&w_out3, static_cast<size_t>(N_out_pad) * 3 * d, true));
+  TRY(scr.alloc(&table, static_cast<size_t>(index + 1) * SCHED_DPM_STRIDE, true));   // the row at `index`, zeros above
+  TRY(scr.alloc(&st, 1, true));
+  CUDA_TRY(cudaMemcpyAsync(table + static_cast<size_t>(index) * SCHED_DPM_STRIDE, dpm_row_dev, SCHED_DPM_STRIDE * sizeof(float),
+                           cudaMemcpyDeviceToDevice, s));
+  step_set_kernel<<<1, 1, 0, s>>>(st, step, index, nullptr, 0, 0, 0, index + 1);
+  CUDA_TRY(cudaGetLastError());
+  split_weight_kernel<<<JF, 128, 0, s>>>(w_out_dev, w_out3, JF, d, d);
+  CUDA_TRY(cudaGetLastError());
+  blend_split_kernel<<<(B * T + 7) / 8, 256, 0, s>>>(static_cast<const __half*>(hres16_dev), g16, scale_dev, B, S, T, s_off, d,
+                                                     halves);
+  CUDA_TRY(cudaGetLastError());
+  CUtensorMap m_g16, m_wout;
+  TRY(make_map(&m_g16, g16, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
+  TRY(make_map(&m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
+  EpiOutParams p{};
+  p.bias = b_out_dev;
+  p.inpaint_mask = inpaint_mask_dev;
+  p.inpaint_motion = inpaint_motion_dev;
+  p.sched_dpm = table;
+  p.x0_hist = x0_hist_dev;
+  p.state = st;
+  StepArgs a;
+  a.mode = MODE_DPM;
+  a.order = order;
+  a.x_in = x_t_dev;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  a.x_out = x_out_dev;
   return launch_out_gemm(m_g16, m_wout, B, T, JF, d, a, p, s, sms);
 }
 

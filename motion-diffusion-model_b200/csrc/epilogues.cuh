@@ -302,15 +302,22 @@ struct EpiEmbed {
 //           in mode 3 with x0 = pred_xstart (the first evaluation's)
 // DDIM inversion (ddim_reverse_sample, gaussian_diffusion.py:838-874): x at schedule index i -> x at index i + 1
 //   mode 6: eps = (sr*x - x0)/srm1 (row i of sched); x_next = x0*sqrt(abn) + sqrt(1 - abn)*eps (row i of sched_next)
+// DPM-Solver++ multistep, data prediction (Lu et al. 2022, Algorithm 2; DESIGN.md section 1): x0 of evaluation k lives in
+// slot k % 2 of an x0 history, row i of the DPM table holds (c_x, c0, c_cur, c_prev)
+//   mode 7: cur_order = (k == 0 || i == 0) ? 1 : order;  history[k % 2] = x0;
+//           order 1: x_out = fmaf(c0, x0, c_x*x);  order 2: x_out = fmaf(c_prev, history[(k-1) % 2], fmaf(c_cur, x0, c_x*x))
 // Per-step scalars come from a device table indexed by the device-side step state, so the very same launch
 // (and CUDA graph) serves every step of the loop.
 constexpr int SCHED_STRIDE = 8;       // floats per schedule row: c1 c2 sig_ddpm sr srm1 sqrt_abp coef_eps sig_ddim
 constexpr int SCHED_NEXT_STRIDE = 2;  // floats per row of the reverse table: sqrt(abn) sqrt(1 - abn)
+constexpr int SCHED_DPM_STRIDE = 4;   // floats per row of the DPM-Solver++ table: c_x c0 c_cur c_prev
 constexpr int PLMS_RING = 3;          // eps history slots: AB4 combines this step's eps with the three before it
+constexpr int DPM_SLOTS = 2;          // x0 history slots: 2M combines this step's x0 with the one before it
 enum OutMode : int {
   MODE_X0 = 0, MODE_DDPM = 1, MODE_DDIM = 2,                      // B200MDM_MODE_*
   MODE_PLMS_AB = 3, MODE_PLMS_EULER1 = 4, MODE_PLMS_EULER2 = 5,   // internal: the steps of the PLMS loop
   MODE_DDIM_REVERSE = 6,                                          // B200MDM_MODE_DDIM_REVERSE
+  MODE_DPM = 7,                                                   // internal: the step of the DPM-Solver++ loop
 };
 struct StepState {
   int done;      // steps completed so far (indexes the noise tape; PLMS: the evaluation count k)
@@ -339,13 +346,15 @@ struct EpiOutParams {
   const float* inpaint_motion;        // [B, J, T]
   const float* sched;       // [n_steps, SCHED_STRIDE]
   const float* sched_next;  // mode 6: [n_steps, SCHED_NEXT_STRIDE]
+  const float* sched_dpm;   // mode 7: [n_steps, SCHED_DPM_STRIDE]
   float* eps_ring;          // modes 3-5: [PLMS_RING, B, J, T]
+  float* x0_hist;           // mode 7: [DPM_SLOTS, B, J, T]
   const float* x_step;      // mode 5: x_t of the step (x_t above is mean1 there)
   const StepState* state;
   long long noise_batch_stride;  // J*T normally, 0 for const_noise
   int B, T, J, mode;
   int clip_denoised;        // clamp x0 to [-1, 1] after the inpainting blend (gaussian_diffusion.py:348-352)
-  int order;                // mode 3: 1..4
+  int order;                // mode 3: 1..4; mode 7: 1..2
   int back;                 // modes 3-5: this forward evaluates schedule index eval_index(state, back)
 };
 
@@ -473,8 +482,35 @@ struct OutReverse {   // mode 6: no noise and no history
   }
 };
 
-// One GEMM instantiation per update family, so that the PLMS and inversion epilogues leave the DDPM / DDIM kernel as
-// it is.
+struct OutDpm {   // mode 7: no noise; the x0 history replaces PLMS's eps ring
+  float cx, c0, cc, cp;
+  bool second;            // this step is second order
+  const float* prev;      // x0 of evaluation k - 1
+  float* own;             // slot of evaluation k
+  struct In { float x, h; };
+  __device__ __forceinline__ OutDpm(const EpiOutParams& p, int) {
+    const StepState st = *p.state;
+    const int k = st.done, i = st.cur;
+    const float* row = p.sched_dpm + static_cast<size_t>(i) * SCHED_DPM_STRIDE;
+    cx = row[0]; c0 = row[1]; cc = row[2]; cp = row[3];
+    second = p.order == 2 && k != 0 && i != 0;
+    const size_t slot = static_cast<size_t>(p.B) * p.J * p.T;
+    own = p.x0_hist + static_cast<size_t>(k & 1) * slot;
+    prev = p.x0_hist + static_cast<size_t>((k + 1) & 1) * slot;
+  }
+  __device__ __forceinline__ In load(const EpiOutParams& p, bool in, size_t idx, int, int) const {
+    return {in ? p.x_t[idx] : 0.f, in && second ? prev[idx] : 0.f};
+  }
+  __device__ __forceinline__ void store(const EpiOutParams& p, size_t idx, float x0, const In& v) const {
+    own[idx] = x0;
+    if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
+    const float base = __fmul_rn(cx, v.x);
+    p.x_out[idx] = second ? __fmaf_rn(cp, v.h, __fmaf_rn(cc, x0, base)) : __fmaf_rn(c0, x0, base);
+  }
+};
+
+// One GEMM instantiation per update family, so that the PLMS, inversion and DPM-Solver++ epilogues leave the DDPM /
+// DDIM kernel as it is.
 template <class Update>
 struct EpiOut {
   static constexpr int SMEM_PER_WARP = 1024;  // unused

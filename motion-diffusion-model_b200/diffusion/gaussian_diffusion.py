@@ -3,7 +3,8 @@
 Same constructor keywords, same public attributes (fp64 numpy tables) and the same sampling entry points
 (`p_sample_loop`, `p_sample_loop_progressive`, `ddim_sample_loop`, `ddim_sample_loop_progressive`, `p_sample`,
 `ddim_sample`, `plms_sample_loop`, `plms_sample_loop_progressive`, `plms_sample`, `ddim_reverse_sample`, `q_sample`),
-plus the DDIM inversion loops `ddim_reverse_sample_loop` / `ddim_reverse_sample_loop_progressive`, but the per-step arithmetic is not here: a loop is ONE call into libb200mdm.so which
+plus the DDIM inversion loops `ddim_reverse_sample_loop` / `ddim_reverse_sample_loop_progressive` and the DPM-Solver++
+loops `dpm_solver_sample_loop` / `dpm_solver_sample_loop_progressive`, but the per-step arithmetic is not here: a loop is ONE call into libb200mdm.so which
 enqueues every step (denoiser + CFG + posterior/noise epilogue) without returning to Python.
 
 Training losses / VLB of the reference are out of scope (SURVEY.md section 8) and raise.
@@ -138,6 +139,30 @@ class GaussianDiffusion:
         rows[:, 0] = np.sqrt(abn)
         rows[:, 1] = np.sqrt(np.float32(1.0) - abn)
         return rows
+
+    def schedule_dpm_rows(self):
+        """[n, 4] fp32 rows c_x, c0, c_cur, c_prev for b200mdm_set_schedule_dpm (DESIGN.md section 1).  With
+        alpha = sqrt(ac), sigma = sqrt(1 - ac) and lambda = log(alpha) - log(sigma): step i goes from index i to the
+        target alphas_cumprod_prev[i], h = lambda_target - lambda_i, c_x = sigma_target / sigma_i,
+        c0 = -alpha_target * expm1(-h); the second-order pair uses r = h_prev / h with h_prev the step from i + 1 to i:
+        c_cur = c0 * (1 + 1/(2r)), c_prev = -c0 / (2r).  Everything in fp64 from the fp64 tables, rounded once.
+        Row 0 (target alpha 1, sigma 0) is (0, 1, 1, 0); row n - 1 has no previous step (c_cur = c0, c_prev = 0)."""
+        ac, acp = self.alphas_cumprod, self.alphas_cumprod_prev
+        n = self.num_timesteps
+        lam = 0.5 * (np.log(ac) - np.log1p(-ac))                 # log(alpha) - log(sigma)
+        rows = np.zeros((n, 4), dtype=np.float64)
+        rows[0] = (0.0, 1.0, 1.0, 0.0)
+        for i in range(1, n):
+            h = 0.5 * (np.log(acp[i]) - np.log1p(-acp[i])) - lam[i]
+            c0 = -np.sqrt(acp[i]) * np.expm1(-h)
+            rows[i, 0] = np.sqrt(1.0 - acp[i]) / np.sqrt(1.0 - ac[i])
+            rows[i, 1] = c0
+            if i + 1 < n:
+                r = (lam[i] - lam[i + 1]) / h
+                rows[i, 2], rows[i, 3] = c0 * (1.0 + 1.0 / (2.0 * r)), -c0 / (2.0 * r)
+            else:
+                rows[i, 2], rows[i, 3] = c0, 0.0
+        return rows.astype(np.float32)
 
     def _timestep_map(self):
         return list(range(self.num_timesteps))
@@ -510,6 +535,70 @@ class GaussianDiffusion:
             if len(old_eps) >= order:
                 old_eps.pop(0)
             yield {"sample": img, "pred_xstart": pred, "old_eps": old_eps}
+
+    # ------------------------------------------------------------------ DPM-Solver++
+    @staticmethod
+    def _dpm_order(order):
+        if isinstance(order, bool) or not isinstance(order, (int, np.integer)):
+            raise TypeError("DPM-Solver++ order must be an int (got %r)" % (order,))
+        if order not in (1, 2):
+            raise ValueError("DPM-Solver++ order must be 1 or 2 (got %d)" % order)
+        return int(order)
+
+    def _dpm_begin(self, model, shape, noise, clip_denoised, denoised_fn, cond_fn, model_kwargs, device, skip_timesteps,
+                   init_image, randomize_class, cond_fn_with_grad, dump_steps, const_noise, order, noise_tape,
+                   noise_seed, sample_index_base):
+        """Argument checks (before any engine work), the tables, conditioning and x_T of a DPM-Solver++ loop."""
+        order = self._dpm_order(order)
+        if noise_tape is not None:
+            raise ValueError("DPM-Solver++ draws no per-step noise: a noise_tape has no use")
+        if dump_steps is not None or const_noise:
+            raise NotImplementedError()
+        self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
+        assert isinstance(shape, (tuple, list))
+        if device is None:
+            device = next(model.parameters()).device
+        eng = self._prepare(model, shape, model_kwargs, device, 0.0)
+        eng.set_schedule_dpm(self.schedule_dpm_rows(), key=(id(self), self.num_timesteps))
+        if noise_seed is not None and noise is None:
+            noise = eng.philox_normal(shape, noise_seed, sample_index_base, -1, device)
+        img = self._initial(eng, shape, noise, device, skip_timesteps, init_image)
+        return eng, img, order, 2 if clip_denoised else 0, self.num_timesteps - skip_timesteps
+
+    def dpm_solver_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
+                               model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
+                               randomize_class=False, cond_fn_with_grad=False, dump_steps=None, const_noise=False,
+                               order=2, use_graph=True, noise_tape=None, noise_seed=None, sample_index_base=0):
+        """Multistep DPM-Solver++ in its data-prediction form (Lu et al. 2022, Algorithm 2; no reference counterpart) on
+        this diffusion's own (possibly respaced) schedule, as one engine call: order 2 is the "2M" solver, order 1 is
+        DDIM with eta = 0.  The keywords mirror ddim_sample_loop.  No per-step noise is drawn: the only draw is x_T, from
+        torch's generator or, with `noise_seed` (+ `sample_index_base`), from the engine's Philox stream; a noise_tape
+        raises ValueError.  order: an int, 1 or 2 (TypeError / ValueError otherwise)."""
+        eng, img, order, flags, n_run = self._dpm_begin(
+            model, shape, noise, clip_denoised, denoised_fn, cond_fn, model_kwargs, device, skip_timesteps, init_image,
+            randomize_class, cond_fn_with_grad, dump_steps, const_noise, order, noise_tape, noise_seed, sample_index_base)
+        out = torch.empty_like(img)
+        eng.dpm_loop_range(order, n_run - 1, n_run, img, out, flags, use_graph)
+        eng._keep["loop"] = (img,)
+        return out
+
+    def dpm_solver_sample_loop_progressive(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None,
+                                           cond_fn=None, model_kwargs=None, device=None, progress=False,
+                                           skip_timesteps=0, init_image=None, randomize_class=False,
+                                           cond_fn_with_grad=False, order=2, use_graph=True, noise_tape=None):
+        """dpm_solver_sample_loop as a generator of {'sample', 'pred_xstart'} per step: the same loop, continued one
+        step per yield, so the samples are those of the loop bit for bit."""
+        eng, img, order, flags, n_run = self._dpm_begin(
+            model, shape, noise, clip_denoised, denoised_fn, cond_fn, model_kwargs, device, skip_timesteps, init_image,
+            randomize_class, cond_fn_with_grad, None, False, order, noise_tape, None, 0)
+        x_in = img
+        for k in range(n_run):
+            sample, pred = torch.empty_like(img), torch.empty_like(img)
+            eng.dpm_loop_range(order, n_run - 1 - k, 1, x_in, sample, flags, use_graph)
+            eng.dpm_pred_xstart(pred)
+            eng._keep["loop"] = (img,)
+            x_in = None
+            yield {"sample": sample, "pred_xstart": pred}
 
     # ------------------------------------------------------------------ out of scope
     def training_losses(self, *a, **k):

@@ -122,7 +122,8 @@ class Engine:
         check(self.lib.b200mdm_set_schedule(self.h, len(tmap), rows.ctypes.data_as(ctypes.c_void_p),
                                             tmap.ctypes.data_as(ctypes.c_void_p)))
         self._sched_key = key
-        self._next_key = None                     # the engine marks the reverse table stale
+        self._next_key = None                     # the engine marks the reverse and DPM-Solver++ tables stale
+        self._dpm_key = None
 
     def set_schedule_next(self, rows, key=None):
         """[n_steps, 2] fp32 rows sqrt(abn), sqrt(1 - abn) of the current schedule (b200mdm_set_schedule_next)."""
@@ -132,6 +133,15 @@ class Engine:
         assert rows.ndim == 2 and rows.shape[1] == _lib.SCHED_NEXT_STRIDE
         check(self.lib.b200mdm_set_schedule_next(self.h, rows.shape[0], rows.ctypes.data_as(ctypes.c_void_p)))
         self._next_key = key
+
+    def set_schedule_dpm(self, rows, key=None):
+        """[n_steps, 4] fp32 rows c_x, c0, c_cur, c_prev of the current schedule (b200mdm_set_schedule_dpm)."""
+        if key is not None and key == self._dpm_key:
+            return
+        rows = np.ascontiguousarray(rows, dtype=np.float32)
+        assert rows.ndim == 2 and rows.shape[1] == _lib.SCHED_DPM_STRIDE
+        check(self.lib.b200mdm_set_schedule_dpm(self.h, rows.shape[0], rows.ctypes.data_as(ctypes.c_void_p)))
+        self._dpm_key = key
 
     # ------------------------------------------------------------------ conditioning
     def set_cond(self, batch, nframes, y, guided, device):
@@ -393,6 +403,17 @@ class Engine:
         x_in None: continue the previous PLMS loop; x_out None: leave the state in the engine."""
         check(self.lib.b200mdm_plms_loop_range(self.h, order, first_index, n_run, _ptr(x_in), _ptr(x_out), flags,
                                                int(use_graph), _stream()))
+
+    def dpm_loop_range(self, order, first_index, n_run, x_in, x_out, flags=0, use_graph=True):
+        """DPM-Solver++ steps first_index .. first_index-n_run+1 on the engine's working buffer (b200mdm_dpm_loop_range).
+        x_in None: continue the previous DPM-Solver++ loop of this order; x_out None: leave the state in the engine."""
+        check(self.lib.b200mdm_dpm_loop_range(self.h, order, first_index, n_run, _ptr(x_in), _ptr(x_out), flags,
+                                              int(use_graph), _stream()))
+
+    def dpm_pred_xstart(self, out):
+        """out <- the x0 of the last step of the DPM-Solver++ loop in the engine (b200mdm_dpm_pred_xstart)."""
+        check(self.lib.b200mdm_dpm_pred_xstart(self.h, _ptr(out), _stream()))
+        return out
 
     def plms_step(self, index, order, x_t, old_eps, flags=0):
         """One plms_sample step (b200mdm_plms_step): old_eps = list of [B,J,F,T] eps, oldest first, possibly empty
