@@ -148,12 +148,15 @@ int b200mdm_set_schedule_dpm(b200mdm_engine* e, int32_t n_steps, const float* ro
  *                    packed into one batch of 2*batch, utils/sampler_util.py:27-34); NULL => single forward
  *   force_uncond   : y.get('uncond', False) for the single-forward case (model/mdm.py:208)
  *   action_host    : y['action'][:,0] int64 [batch] or NULL
- * The text projection embed_text(mask_cond(.)) (model/mdm.py:218) is evaluated here, once. */
+ * The text projection embed_text(mask_cond(.)) (model/mdm.py:218) is evaluated here, once.  Every call starts a new
+ * loop's conditioning: it clears the target (b200mdm_set_target) and the inpainting inputs (b200mdm_set_inpaint), also
+ * at an unchanged shape; a PLMS / DPM-Solver++ loop of the selected workspace can still be continued. */
 int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* cond_embed_dev,
                      const int64_t* lengths_host, const float* scale_dev, int32_t force_uncond,
                      const int64_t* action_host, void* stream);
 
-/* trans_dec (DiP, model/mdm.py:203-206,255-270): conditioning for arch = B200MDM_ARCH_TRANS_DEC.
+/* Like b200mdm_set_cond, it clears the target (b200mdm_set_target) and the inpainting inputs (b200mdm_set_inpaint).
+ * trans_dec (DiP, model/mdm.py:203-206,255-270): conditioning for arch = B200MDM_ARCH_TRANS_DEC.
  *   enc_text_dev   : y['text_embed'][0], BERT token features [n_tokens, batch, cond_dim] fp32 device (reference layout)
  *   text_mask_host : y['text_embed'][1], uint8 [batch, n_tokens], 1 = padding (memory_key_padding_mask)
  *   nframes        : frames of x (pred_len); the sequence is context_len + nframes tokens, no conditioning token
@@ -184,11 +187,15 @@ int b200mdm_set_prefix(b200mdm_engine* e, const float* prefix_dev, void* stream)
 int b200mdm_set_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, void* stream);
 
 /* y['inpainting_mask'] (bool as uint8) / y['inpainted_motion'] [B,J,F,T] device pointers
- * (gaussian_diffusion.py:300-304); NULL, NULL clears. */
+ * (gaussian_diffusion.py:300-304); NULL, NULL clears.  Call it after b200mdm_set_cond / b200mdm_set_cond_dec, which
+ * clear it.  The pointers are read by every sampler step and loop (and so the pred_xstart of b200mdm_sample_step, as the
+ * reference's p_mean_variance forms it), never by b200mdm_denoise or b200mdm_test_forward_taps, and must stay valid
+ * until the work enqueued with them has completed. */
 int b200mdm_set_inpaint(b200mdm_engine* e, const uint8_t* mask_dev, const float* motion_dev);
 
 /* MDM.forward / ClassifierFreeSampleModel.forward (model/mdm.py:189-283, utils/sampler_util.py:27-34):
- * out = model(x, timesteps, y).  timesteps_host: int32 [batch] MODEL timesteps (already mapped). */
+ * out = model(x, timesteps, y), without inpainting (the sampler's, not the model's).  timesteps_host: int32 [batch] MODEL
+ * timesteps (already mapped). */
 int b200mdm_denoise(b200mdm_engine* e, const float* x_dev, const int32_t* timesteps_host, float* out_dev, void* stream);
 
 /* One p_sample / ddim_sample (gaussian_diffusion.py:489-541 / 729-779) at schedule index `index`:
@@ -233,7 +240,11 @@ int b200mdm_ddim_reverse_loop_range(b200mdm_engine* e, int32_t first_index, int3
  * A fresh loop of order 1 -> B200MDM_EINVAL (the reference fails on its missing history).  x_in_dev NULL continues
  * the PLMS loop the previous call of the same order left in the engine; x_out_dev NULL leaves the result there.
  * flags: B200MDM_FLAG_CLIP_DENOISED or 0.  No noise is drawn.  The eps history (3 x [B, JF, T] fp32), a scratch sample
- * and a pred_xstart buffer are allocated in the workspace on first use. */
+ * and a pred_xstart buffer are allocated in the workspace on first use.  The loop to continue is the workspace's: a
+ * b200mdm_set_cond* that selects another (batch, nframes, CFG) and then this one again, a b200mdm_set_cond* at the same
+ * shape, b200mdm_denoise, b200mdm_sample_step, b200mdm_set_schedule and loops on other workspaces keep it; any other loop
+ * on this workspace, b200mdm_plms_step, a weight reload and the eviction of the parked workspace from the pool end it
+ * (B200MDM_ESTATE). */
 int b200mdm_plms_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index, int32_t n_run, const float* x_in_dev,
                             float* x_out_dev, int32_t flags, int32_t use_graph, void* stream);
 
@@ -255,7 +266,8 @@ int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order, const flo
  * from row i of the b200mdm_set_schedule_dpm table (stale table -> B200MDM_ESTATE).  x_in_dev != NULL starts a fresh
  * loop (k = 0); NULL continues the DPM-Solver++ loop the previous call of the same order left in the engine, history
  * included; x_out_dev NULL leaves the result there.  flags: B200MDM_FLAG_CLIP_DENOISED or 0.  No noise is drawn.  The
- * history (2 x [B, JF, T] fp32) is allocated in the workspace on first use. */
+ * history (2 x [B, JF, T] fp32) is allocated in the workspace on first use.  What keeps and what ends the loop to
+ * continue is as for b200mdm_plms_loop_range, except that b200mdm_plms_step does not end it. */
 int b200mdm_dpm_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index, int32_t n_run, const float* x_in_dev,
                            float* x_out_dev, int32_t flags, int32_t use_graph, void* stream);
 /* out_dev [B, JF, T] fp32 <- the x0 (pred_xstart) of the last step of that loop.  Enqueued on `stream`. */

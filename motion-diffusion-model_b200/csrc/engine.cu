@@ -1097,6 +1097,8 @@ extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframe
   e->launches++;
   e->cond_set = true;
   e->target_set = false;
+  e->inpaint_mask = nullptr;   // a new loop's conditioning: the previous loop's inpainting inputs no longer apply
+  e->inpaint_motion = nullptr;
   return B200MDM_OK;
 }
 
@@ -1158,6 +1160,8 @@ static int set_cond_dec_clip(b200mdm_engine* e, int32_t batch, int32_t nframes, 
   TRY(cross_rows_per_sample(e, nullptr, s));
   e->cond_set = true;
   e->target_set = false;
+  e->inpaint_mask = nullptr;   // a new loop's conditioning: the previous loop's inpainting inputs no longer apply
+  e->inpaint_motion = nullptr;
   return B200MDM_OK;
 }
 
@@ -1225,6 +1229,8 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
   e->launches += 3;
   e->cond_set = true;
   e->target_set = false;
+  e->inpaint_mask = nullptr;   // a new loop's conditioning: the previous loop's inpainting inputs no longer apply
+  e->inpaint_motion = nullptr;
   return B200MDM_OK;
 }
 
@@ -1277,6 +1283,7 @@ struct StepArgs {
   int back = 0;                   // evaluate schedule index cur - back (PLMS improved Euler, second forward: 1)
   const float* x_step = nullptr;  // MODE_PLMS_EULER2: x_t of the step
   int order = 0;                  // MODE_PLMS_AB
+  bool model_only = false;        // b200mdm_denoise: the bare model output, without the engine's inpainting
 };
 
 // The output projection of the CFG-blended g16 rows with the update of a.mode fused into its epilogue (p: the tables,
@@ -1479,8 +1486,9 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
   {
     EpiOutParams p{};
     p.bias = e->b_out;
-    p.inpaint_mask = e->inpaint_mask;
-    p.inpaint_motion = e->inpaint_motion;
+    // inpainting belongs to the sampler (p_mean_variance, gaussian_diffusion.py:300-304), not to MDM.forward
+    p.inpaint_mask = a.model_only ? nullptr : e->inpaint_mask;
+    p.inpaint_motion = a.model_only ? nullptr : e->inpaint_motion;
     p.sched = e->sched;
     p.sched_next = e->sched_next;
     p.sched_dpm = e->sched_dpm;
@@ -1520,6 +1528,7 @@ static int denoise_forward(b200mdm_engine* e, const float* x_dev, const int32_t*
   a.x_in = x_dev;
   a.x_out = out_dev;
   a.explicit_t = true;
+  a.model_only = true;
   return enqueue_forward(e, a, s, n_kernels, taps);
 }
 
