@@ -304,9 +304,8 @@ int b200mdm_recover_from_ric(const float* data_dev, int64_t stride_b, int64_t st
 
 /* ---- kernel-level entry points (used by tests/ to check each kernel against a torch fp32 restatement) ---- */
 /* out16[M,N] = fp16(act(A16[M,K] @ W16[N,K]^T + bias)); act: 0 none, 1 exact GELU.  K % 8 == 0, N % 8 == 0,
- * block_n: 128 = 128 x 128 tiles (the kernel every projection GEMM of the step runs on), 512 = 128 x 256 tiles,
- * 513 = W-resident kernel, 128 x 64 tiles, each CTA keeping its W tile in shared memory for the whole launch (K <= 512
- * and N <= 64 x the number of SMs, B200MDM_ENOTIMPL otherwise). */
+ * block_n must be 128: 128 x 128 tiles, the kernel every projection GEMM of the step runs on (B200MDM_EINVAL
+ * otherwise, before the device is touched). */
 int b200mdm_test_gemm_f16(const void* a16_dev, const void* w16_dev, const float* bias_dev, void* out16_dev, int32_t M,
                           int32_t N, int32_t K, int32_t act, int32_t block_n, void* stream);
 /* The two projection-GEMM epilogues b200mdm_test_gemm_f16 does not reach, on 128 x 128 tiles; a16 [M,K], w16 [N,K] fp16,

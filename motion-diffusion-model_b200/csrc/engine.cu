@@ -61,21 +61,26 @@ static int resolve_driver() {
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   return B200MDM_OK;
 }
+// One cuTensorMapEncodeTiled call: `rank` dimensions gdim (innermost first) with rank - 1 byte pitches, no interleave,
+// 256-byte L2 promotion, out-of-bounds elements read as zero.
+static int encode_map(CUtensorMap* m, CUtensorMapDataType dtype, uint32_t rank, const void* ptr, const cuuint64_t* gdim,
+                      const cuuint64_t* gstride_bytes, const cuuint32_t* box, CUtensorMapSwizzle swizzle, const char* what) {
+  TRY(resolve_driver());
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || gstride_bytes[0] % 16) return fail(B200MDM_EINVAL, "TMA operand misaligned");
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = g_encode(m, dtype, rank, const_cast<void*>(ptr), gdim, gstride_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(B200MDM_ECUDA, "cuTensorMapEncodeTiled%s failed (%d)", what, static_cast<int>(r));
+  return B200MDM_OK;
+}
 // fp16 matrix [rows, cols] with leading dimension ld (elements); box = box_rows x 64 columns, 128-byte swizzle.
 // elem_bytes 2 = fp16, 4 = fp32; the box is always 128 bytes wide (64 fp16 / 32 fp32 columns) x box_rows.
 static int make_map_t(CUtensorMap* m, const void* ptr, int elem_bytes, uint64_t rows, uint64_t cols, uint64_t ld,
                       uint32_t box_rows) {
-  TRY(resolve_driver());
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (ld * elem_bytes) % 16) return fail(B200MDM_EINVAL, "TMA operand misaligned");
-  cuuint64_t gdim[2] = {cols, rows};
-  cuuint64_t gstr[1] = {ld * elem_bytes};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / elem_bytes), box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode(m, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
-                        const_cast<void*>(ptr), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B200MDM_ECUDA, "cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
-  return B200MDM_OK;
+  const cuuint64_t gdim[2] = {cols, rows}, gstr[1] = {ld * elem_bytes};
+  const cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / elem_bytes), box_rows};
+  return encode_map(m, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, ptr, gdim, gstr,
+                    box, CU_TENSOR_MAP_SWIZZLE_128B, "");
 }
 static int make_map(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
   return make_map_t(m, ptr, 2, rows, cols, ld, box_rows);
@@ -84,17 +89,9 @@ static int make_map(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t col
 // The middle dimension is bounded per sample, so tiles that run past the last token of a sample are zero-filled.
 static int make_map_3d(CUtensorMap* m, const void* ptr, uint64_t n, uint64_t rows, uint64_t cols, uint64_t ld,
                        uint32_t box_rows) {
-  TRY(resolve_driver());
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (ld * 2) % 16) return fail(B200MDM_EINVAL, "TMA operand misaligned");
-  cuuint64_t gdim[3] = {cols, rows, n};
-  cuuint64_t gstr[2] = {ld * 2, rows * ld * 2};
-  cuuint32_t box[3] = {64, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(ptr), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B200MDM_ECUDA, "cuTensorMapEncodeTiled(3d) failed (%d)", static_cast<int>(r));
-  return B200MDM_OK;
+  const cuuint64_t gdim[3] = {cols, rows, n}, gstr[2] = {ld * 2, rows * ld * 2};
+  const cuuint32_t box[3] = {64, box_rows, 1};
+  return encode_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, ptr, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_128B, "(3d)");
 }
 
 // Residual stream [M, 2 x 512] fp16 as the residual + LayerNorm GEMM moves it: box 64 columns x GLN_RES_BOX_ROWS rows.
@@ -105,17 +102,9 @@ static int make_hres_map(CUtensorMap* m, const void* hres, uint64_t rows) {
 // Residual stream fp16 [rows, 2d] = [hi | lo]: box {32 cols, 32 rows} with 64-byte rows and the 64-byte swizzle; an
 // epilogue chunk of 32 columns moves one such box from the hi half and one from the lo half.
 static int make_map_res(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t d) {
-  TRY(resolve_driver());
-  if (reinterpret_cast<uintptr_t>(ptr) & 15) return fail(B200MDM_EINVAL, "TMA operand misaligned");
-  cuuint64_t gdim[2] = {2 * d, rows};
-  cuuint64_t gstr[1] = {d * 4};
-  cuuint32_t box[2] = {32, 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B200MDM_ECUDA, "cuTensorMapEncodeTiled(residual) failed (%d)", static_cast<int>(r));
-  return B200MDM_OK;
+  const cuuint64_t gdim[2] = {2 * d, rows}, gstr[1] = {d * 4};
+  const cuuint32_t box[2] = {32, 32};
+  return encode_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, gdim, gstr, box, CU_TENSOR_MAP_SWIZZLE_64B, "(residual)");
 }
 
 // ------------------------------------------------------------------------------------------------ engine
@@ -270,10 +259,9 @@ static void dfree(T*& p) {
 }
 
 // ------------------------------------------------------------------------------------------------ launchers
-template <int BN, class Epi, bool RES = false>
+template <int BN, class Epi>
 static int set_gemm_attr() {
-  CUDA_TRY(cudaFuncSetAttribute(gemm_f16_wgmma<BN, Epi, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                GemmSmem<BN, Epi, RES>::TOTAL));
+  CUDA_TRY(cudaFuncSetAttribute(gemm_f16_wgmma<BN, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmSmem<BN, Epi>::TOTAL));
   return B200MDM_OK;
 }
 template <class Epi>
@@ -299,10 +287,6 @@ static int init_kernel_attrs() {
   TRY((set_pingpong_attr<EpiBiasF16<true>>()));
   TRY((set_pingpong_attr<EpiBiasF16Wide<true>>()));
   TRY((set_pingpong_attr<EpiBiasF16Global>()));
-  TRY((set_gemm_attr<256, EpiBiasF16<false>>()));
-  TRY((set_gemm_attr<256, EpiBiasF16<true>>()));
-  TRY((set_gemm_attr<64, EpiBiasF16<false>, true>()));
-  TRY((set_gemm_attr<64, EpiBiasF16<true>, true>()));
   CUDA_TRY(cudaFuncSetAttribute(gemm_resid_ln_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmLnSmem::TOTAL));
   TRY((set_gemm_attr<128, EpiEmbed>()));
   TRY((set_gemm_attr<96, EpiOut<OutStep>>()));
@@ -351,29 +335,17 @@ static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(std::forward<Args>(args))...);
 }
 
-template <int BN, class Epi, class = void> struct epi_unstaged : std::false_type {};
-template <int BN, class Epi> struct epi_unstaged<BN, Epi, std::enable_if_t<Epi::UNSTAGED>> : std::true_type {};
+template <class Epi, class = void> struct epi_unstaged : std::false_type {};
+template <class Epi> struct epi_unstaged<Epi, std::enable_if_t<Epi::UNSTAGED>> : std::true_type {};
 
 template <int BN, class Epi>
 static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& c, int M, int N, int K,
                        const typename Epi::Params& p, cudaStream_t s, int num_sms) {
-  if (!epi_unstaged<BN, Epi>::value && N * 4 > GEMM_BIAS_BYTES)
+  if (!epi_unstaged<Epi>::value && N * 4 > GEMM_BIAS_BYTES)
     return fail(B200MDM_ENOTIMPL, "GEMM epilogue vectors are staged for N <= %d", GEMM_BIAS_BYTES / 4);
   const int tiles = ((M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M) * ((N + BN - 1) / BN);
   const int grid = tiles < num_sms ? tiles : num_sms;
   CUDA_TRY(launch_k(gemm_f16_wgmma<BN, Epi>, dim3(grid), dim3(GEMM_THREADS), GemmSmem<BN, Epi>::TOTAL, s, a, b, c, M, N, K, p));
-  return B200MDM_OK;
-}
-// W-resident GEMM (gemm.cuh, RESIDENT): K <= 512 and every column block owned by at least one CTA
-template <int BN, class Epi>
-static int launch_gemm_resident(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& c, int M, int N, int K,
-                                const typename Epi::Params& p, cudaStream_t s, int num_sms) {
-  const int tiles_n = (N + BN - 1) / BN;
-  const int tiles = ((M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M) * tiles_n;
-  const int grid = tiles < num_sms ? tiles : num_sms;
-  if (K > GEMM_RES_KB_MAX * GEMM_BLOCK_K || tiles_n > grid || N * 4 > GEMM_BIAS_BYTES)
-    return fail(B200MDM_ENOTIMPL, "W-resident GEMM needs K <= %d and N <= %d", GEMM_RES_KB_MAX * GEMM_BLOCK_K, grid * BN);
-  CUDA_TRY(launch_k(gemm_f16_wgmma<BN, Epi, true>, dim3(grid), dim3(GEMM_THREADS), GemmSmem<BN, Epi, true>::TOTAL, s, a, b, c, M, N, K, p));
   return B200MDM_OK;
 }
 // projection GEMMs of the step (gemm_pingpong.cuh): 128 x 128 tiles, the two consumer warpgroups take turns (b: W map
@@ -381,7 +353,7 @@ static int launch_gemm_resident(const CUtensorMap& a, const CUtensorMap& b, cons
 template <class Epi>
 static int launch_gemm_pp(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& c, int M, int N, int K,
                           const typename Epi::Params& p, cudaStream_t s, int num_sms) {
-  if (!epi_unstaged<PP_BLOCK_N, Epi>::value && N * 4 > GEMM_BIAS_BYTES)
+  if (!epi_unstaged<Epi>::value && N * 4 > GEMM_BIAS_BYTES)
     return fail(B200MDM_ENOTIMPL, "GEMM epilogue vectors are staged for N <= %d", GEMM_BIAS_BYTES / 4);
   const int tiles = ((M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M) * ((N + PP_BLOCK_N - 1) / PP_BLOCK_N);
   const int grid = tiles < num_sms ? tiles : num_sms;
@@ -431,6 +403,60 @@ static int launch_attention_tc(const CUtensorMap& map_kv, const __half* qkv, __h
   if (keys == 64) CUDA_TRY(launch_attention_keys<64>(map_kv, qkv, out, kvlen, grid, S, d, scale_log2, s, wide));
   else if (keys == 208) CUDA_TRY(launch_attention_keys<208>(map_kv, qkv, out, kvlen, grid, S, d, scale_log2, s, wide));
   else CUDA_TRY(launch_attention_keys<256>(map_kv, qkv, out, kvlen, grid, S, d, scale_log2, s, wide));
+  return B200MDM_OK;
+}
+// cross-attention core of a trans_dec layer over a text memory of Mt tokens: q16 [n*S, d]; kv rows (sample, token) of
+// pitch ld_kv holding k | v; mask [n, Mt], 1 = padding.  Up to 64 tokens every key of a head sits in registers, longer
+// memories take the key-blocked kernel.
+static int launch_cross_attention(const __half* q16, const __half* kv, const unsigned char* mask, __half* out, int n_samples,
+                                  int S, int Mt, int d, int H, int ld_kv, cudaStream_t s) {
+  const float sl2 = 1.4426950408889634f / sqrtf(128.0f);
+  const dim3 cg(H, n_samples), cb(128);
+  if (Mt <= 16)
+    CUDA_TRY(launch_k(cross_attention_kernel<2>, cg, cb, 0, s, q16, kv, mask, out, S, Mt, d, ld_kv, sl2));
+  else if (Mt <= 32)
+    CUDA_TRY(launch_k(cross_attention_kernel<4>, cg, cb, 0, s, q16, kv, mask, out, S, Mt, d, ld_kv, sl2));
+  else if (Mt <= 64)
+    CUDA_TRY(launch_k(cross_attention_kernel<8>, cg, cb, 0, s, q16, kv, mask, out, S, Mt, d, ld_kv, sl2));
+  else
+    CUDA_TRY(launch_k(cross_attention_long_kernel, dim3(H, n_samples, (S + XAL_ROWS - 1) / XAL_ROWS), cb, XAL_SMEM, s, q16, kv,
+                      mask, out, S, Mt, d, ld_kv, sl2));
+  return B200MDM_OK;
+}
+// h <- LayerNorm(h + c[row / S]) over the [hi | lo] residual stream (the CLIP decoder's one-token cross-attention block)
+static int launch_row_bias_ln(__half* hres, const float* c, const float* gamma, const float* beta, int M, int S, cudaStream_t s) {
+  CUDA_TRY(launch_k(row_bias_ln_kernel, dim3((M + RBLN_ROWS_PER_CTA - 1) / RBLN_ROWS_PER_CTA), dim3(32 * RBLN_ROWS_PER_CTA), 0, s,
+                    hres, c, gamma, beta, M, S, 1e-5f));
+  return B200MDM_OK;
+}
+// eps [B, n] of the counter-based noise stream; state != nullptr: seed, sample base and step come from the step state
+static int launch_philox(float* out, int B, long long n, unsigned long long seed, long long sample_base, uint32_t step_id,
+                         const StepState* state, cudaStream_t s) {
+  const long long quads = (n + 3) / 4 * B;
+  const int blocks = static_cast<int>(quads / 256 + 1 < 1184 ? quads / 256 + 1 : 1184);
+  CUDA_TRY(launch_k(philox_normal_kernel, dim3(blocks), dim3(256), 0, s, out, B, n, seed, sample_base, step_id, state));
+  return B200MDM_OK;
+}
+// x [B, JF, cols] -> rows row_off .. row_off + cols of every S-row sequence of the embedding GEMM's A operand [hi | hi | lo]
+static int launch_pack_input(const float* x, __half* xin16, int B, int JF, int cols, int S, int Kp, int row_off, cudaStream_t s) {
+  CUDA_TRY(launch_k(pack_input_kernel, dim3((cols + 31) / 32, (JF + 31) / 32, B), dim3(32, 8), 0, s, x, xin16, B, JF, cols, S,
+                    Kp, 3 * Kp, row_off));
+  return B200MDM_OK;
+}
+// residual stream <- xin16 W_in3^T + pe_bias[s], stored to the rows of both CFG halves (EpiEmbed)
+static int launch_embed_gemm(const CUtensorMap& m_xin, const CUtensorMap& m_win, const CUtensorMap& m_res_c,
+                             const CUtensorMap& m_res_u, const float* pe_bias, int MB, int S, int d, int Kp, int halves,
+                             cudaStream_t s, int num_sms) {
+  EpiEmbed::Params p;
+  p.res_c = m_res_c; p.res_u = m_res_u;
+  p.pe_bias = pe_bias;
+  p.S = S; p.d = d; p.halves = halves;
+  return launch_gemm<128, EpiEmbed>(m_xin, m_win, m_xin, MB, d, 3 * Kp, p, s, num_sms);
+}
+// g16 [B*T, 3d] = [hi | hi | lo] of the CFG blend of the frame rows of hres
+static int launch_blend_split(const __half* hres, __half* g16, const float* scale, int B, int S, int T, int s_off, int d,
+                              int halves, cudaStream_t s) {
+  CUDA_TRY(launch_k(blend_split_kernel, dim3((B * T + 7) / 8), dim3(256), 0, s, hres, g16, scale, B, S, T, s_off, d, halves));
   return B200MDM_OK;
 }
 #ifdef B200_TRACE
@@ -548,15 +574,20 @@ static void drop_all_graphs(b200mdm_engine* e) {
   for (auto& w : e->pool) drop_graph(&w);
 }
 
+// the fp16 / packed copies b200mdm_finalize_weights derives from the weight store
+static void free_repacks(b200mdm_engine* e) {
+  for (auto& l : e->layers) { dfree(l.wqkv); dfree(l.wo); dfree(l.w1); dfree(l.w2); dfree(l.wq_c); dfree(l.wo_c); }
+  dfree(e->w_in3); dfree(e->w_out3); dfree(e->temb_hidden); dfree(e->temb_table); dfree(e->wkv_all); dfree(e->bkv_all);
+  dfree(e->cross_t);
+}
+
 extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   if (!e) return B200MDM_OK;
   cudaDeviceSynchronize();
   free_all_workspaces(e);
   for (auto& kv : e->store) cudaFree(kv.second.dev);
-  for (auto& l : e->layers) { dfree(l.wqkv); dfree(l.wo); dfree(l.w1); dfree(l.w2); dfree(l.wq_c); dfree(l.wo_c); }
-  dfree(e->w_in3); dfree(e->w_out3); dfree(e->temb_hidden); dfree(e->temb_table); dfree(e->sched); dfree(e->tmap);
-  dfree(e->sched_next); dfree(e->sched_dpm);
-  dfree(e->wkv_all); dfree(e->bkv_all); dfree(e->cross_t);
+  free_repacks(e);
+  dfree(e->sched); dfree(e->tmap); dfree(e->sched_next); dfree(e->sched_dpm);
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
   if (e->work) cudaStreamDestroy(e->work);
@@ -755,9 +786,7 @@ extern "C" int b200mdm_finalize_weights(b200mdm_engine* e, void* stream) {
   // the next one
   CUDA_TRY(cudaDeviceSynchronize());
   free_all_workspaces(e);
-  for (auto& l : e->layers) { dfree(l.wqkv); dfree(l.wo); dfree(l.w1); dfree(l.w2); dfree(l.wq_c); dfree(l.wo_c); }
-  dfree(e->w_in3); dfree(e->w_out3); dfree(e->temb_hidden); dfree(e->temb_table); dfree(e->wkv_all); dfree(e->bkv_all);
-  dfree(e->cross_t);
+  free_repacks(e);
 
   // split-precision in / out projections: W' = [hi | hi | lo], zero padded
   const int Kp = e->Kp_in;
@@ -1039,6 +1068,59 @@ static int select_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStr
   return r;
 }
 
+// ---- what the three conditioning entry points share
+// a sequence of n_tokens tokens fits the positional table and the attention kernels
+static int check_seq_len(const b200mdm_engine* e, int n_tokens) {
+  if (n_tokens > e->cfg.pos_embed_max_len) return fail(B200MDM_EINVAL, "sequence longer than the positional table");
+  if (n_tokens > ATC_MAX_KEYS)
+    return fail(B200MDM_ENOTIMPL, "sequences of more than %d tokens (the attention kernels keep all keys of a sample on chip; "
+                "every dataset of the reference stops at 196 frames)", ATC_MAX_KEYS);
+  return B200MDM_OK;
+}
+// Valid-key counts of the current workspace's packed batch -- the seq_extra tokens ahead of the frames are always valid,
+// then `lengths` frames (model/mdm.py:241-247; lengths_to_mask, data_loaders/tensors.py:3-6), all keys unless `clamp` --
+// and the guidance scales, uploaded on s.  The host staging lives in the engine until the next call, so the asynchronous
+// copy needs no stream synchronisation.
+static int upload_kvlen_scale(b200mdm_engine* e, int nframes, int seq_extra, bool clamp, const int64_t* lengths_host,
+                              const float* scale_dev, cudaStream_t s) {
+  std::vector<int>& kv = e->h_kv;
+  kv.assign(e->Bp, e->S);
+  if (e->cfg.mask_frames && lengths_host && clamp) {
+    for (int b = 0; b < e->Bp; ++b) {
+      long long len = lengths_host[b % e->B];
+      if (len < 0) len = 0;
+      if (len > nframes) len = nframes;
+      kv[b] = static_cast<int>(len) + seq_extra;
+    }
+  }
+  CUDA_TRY(cudaMemcpyAsync(e->kvlen, kv.data(), kv.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  if (scale_dev) CUDA_TRY(cudaMemcpyAsync(e->scale, scale_dev, e->B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return B200MDM_OK;
+}
+// condproj rows of the packed batch: proj = embed_text(text) [B, d] when the model is text-conditioned and a text is given
+// (model/mdm.py:218), then the conditional / unconditional rows of the model's conditioning mode (condproj_fill_kernel)
+static int fill_condproj(b200mdm_engine* e, const float* text_dev, bool uncond, cudaStream_t s) {
+  const int B = e->B, d = e->d;
+  if (e->cfg.cond_mode == B200MDM_COND_TEXT && text_dev) {
+    const size_t warps = static_cast<size_t>(B) * d;
+    small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(text_dev, e->w_txt, e->b_txt, e->proj, B, d,
+                                                                                       e->cfg.cond_dim, e->cfg.cond_dim);
+    CUDA_TRY(cudaGetLastError());
+    e->launches++;
+  }
+  condproj_fill_kernel<<<e->Bp, 128, 0, s>>>(e->condproj, e->proj, e->b_txt, e->act_emb, e->action, B, d, e->Bp, uncond ? 1 : 0,
+                                             e->cfg.cond_mode);
+  CUDA_TRY(cudaGetLastError());
+  e->launches++;
+  return B200MDM_OK;
+}
+// a new loop's conditioning is in place: the previous loop's target and inpainting inputs no longer apply
+static void end_cond(b200mdm_engine* e) {
+  e->cond_set = true;
+  e->target_set = false;
+  e->inpaint_mask = nullptr;
+  e->inpaint_motion = nullptr;
+}
 
 extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* cond_embed_dev,
                                 const int64_t* lengths_host, const float* scale_dev, int32_t force_uncond,
@@ -1047,10 +1129,7 @@ extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframe
   if (e->dec) return fail(B200MDM_EINVAL, "trans_dec engines take their conditioning through b200mdm_set_cond_dec");
   if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
   if (batch <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
-  if (nframes + 1 > e->cfg.pos_embed_max_len) return fail(B200MDM_EINVAL, "sequence longer than the positional table");
-  if (nframes + 1 > ATC_MAX_KEYS)
-    return fail(B200MDM_ENOTIMPL, "sequences of more than %d tokens (the attention kernels keep all keys of a sample on chip; "
-                "every dataset of the reference stops at 196 frames)", ATC_MAX_KEYS);
+  TRY(check_seq_len(e, nframes + 1));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int halves = scale_dev ? 2 : 1;
   if (e->cfg.cond_mode == B200MDM_COND_TEXT && !cond_embed_dev && !(halves == 1 && force_uncond))
@@ -1060,21 +1139,8 @@ extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframe
   if (halves == 2 && e->cfg.cond_mode == B200MDM_COND_NONE)
     return fail(B200MDM_EINVAL, "classifier-free guidance needs a conditioned model (sampler_util.py:29)");
   TRY(select_workspace(e, batch, nframes, halves, s));
-  const int d = e->d, B = batch, S = nframes + 1;
-  // key mask -> valid-key counts (model/mdm.py:241-247; lengths_to_mask, data_loaders/tensors.py:3-6)
-  // (host staging lives in the engine until the next call, so the asynchronous copies need no stream synchronisation)
-  std::vector<int>& kv = e->h_kv;
-  kv.assign(e->Bp, S);
-  if (e->cfg.mask_frames && lengths_host && nframes > 1) {
-    for (int b = 0; b < e->Bp; ++b) {
-      long long len = lengths_host[b % B];
-      if (len < 0) len = 0;
-      if (len > nframes) len = nframes;
-      kv[b] = static_cast<int>(len) + 1;
-    }
-  }
-  CUDA_TRY(cudaMemcpyAsync(e->kvlen, kv.data(), kv.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-  if (scale_dev) CUDA_TRY(cudaMemcpyAsync(e->scale, scale_dev, B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  const int B = batch;
+  TRY(upload_kvlen_scale(e, nframes, 1, nframes > 1, lengths_host, scale_dev, s));
   if (e->cfg.cond_mode == B200MDM_COND_ACTION && action_host) {
     std::vector<int>& a = e->h_action;
     a.assign(B, 0);
@@ -1084,21 +1150,8 @@ extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframe
     }
     CUDA_TRY(cudaMemcpyAsync(e->action, a.data(), B * sizeof(int), cudaMemcpyHostToDevice, s));
   }
-  if (e->cfg.cond_mode == B200MDM_COND_TEXT && cond_embed_dev) {
-    const size_t warps = static_cast<size_t>(B) * d;
-    small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(cond_embed_dev, e->w_txt, e->b_txt, e->proj, B,
-                                                                                       d, e->cfg.cond_dim, e->cfg.cond_dim);
-    CUDA_TRY(cudaGetLastError());
-    e->launches++;
-  }
-  condproj_fill_kernel<<<e->Bp, 128, 0, s>>>(e->condproj, e->proj, e->b_txt, e->act_emb, e->action, B, d, e->Bp,
-                                             (halves == 1 && force_uncond) ? 1 : 0, e->cfg.cond_mode);
-  CUDA_TRY(cudaGetLastError());
-  e->launches++;
-  e->cond_set = true;
-  e->target_set = false;
-  e->inpaint_mask = nullptr;   // a new loop's conditioning: the previous loop's inpainting inputs no longer apply
-  e->inpaint_motion = nullptr;
+  TRY(fill_condproj(e, cond_embed_dev, halves == 1 && force_uncond, s));
+  end_cond(e);
   return B200MDM_OK;
 }
 
@@ -1130,38 +1183,15 @@ static int set_cond_dec_clip(b200mdm_engine* e, int32_t batch, int32_t nframes, 
   if (!clip_dev || !text_mask_host) return fail(B200MDM_EINVAL, "the CLIP decoder needs y['text_embed'] and an all-zero mask");
   for (int b = 0; b < batch; ++b)
     if (text_mask_host[b]) return fail(B200MDM_EINVAL, "the CLIP memory has no padding mask (model/mdm.py:262-263)");
-  if (nframes + 1 > e->cfg.pos_embed_max_len) return fail(B200MDM_EINVAL, "sequence longer than the positional table");
-  if (nframes + 1 > ATC_MAX_KEYS) return fail(B200MDM_ENOTIMPL, "sequences of more than %d tokens", ATC_MAX_KEYS);
+  TRY(check_seq_len(e, nframes + 1));
   const int halves = scale_dev ? 2 : 1;
   TRY(select_workspace(e, batch, nframes, halves, s));
-  const int d = e->d, B = batch, S = e->S;
-  // key mask: the timestep token, then `lengths` frames (model/mdm.py:241-247, the False column prepended)
-  std::vector<int>& kv = e->h_kv;
-  kv.assign(e->Bp, S);
-  if (e->cfg.mask_frames && lengths_host && nframes > 1) {
-    for (int b = 0; b < e->Bp; ++b) {
-      long long len = lengths_host[b % B];
-      if (len < 0) len = 0;
-      if (len > nframes) len = nframes;
-      kv[b] = static_cast<int>(len) + 1;
-    }
-  }
-  CUDA_TRY(cudaMemcpyAsync(e->kvlen, kv.data(), kv.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-  if (scale_dev) CUDA_TRY(cudaMemcpyAsync(e->scale, scale_dev, B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  // key mask: the timestep token, then `lengths` frames (the False column prepended, model/mdm.py:241-247)
+  TRY(upload_kvlen_scale(e, nframes, 1, nframes > 1, lengths_host, scale_dev, s));
   // text_emb = embed_text(mask_cond(clip)) (model/mdm.py:218): conditional rows W clip + b, unconditional rows b
-  const size_t warps = static_cast<size_t>(B) * d;
-  small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(clip_dev, e->w_txt, e->b_txt, e->proj, B, d,
-                                                                                     e->cfg.cond_dim, e->cfg.cond_dim);
-  CUDA_TRY(cudaGetLastError());
-  condproj_fill_kernel<<<e->Bp, 128, 0, s>>>(e->condproj, e->proj, e->b_txt, nullptr, nullptr, B, d, e->Bp,
-                                             (halves == 1 && force_uncond) ? 1 : 0, B200MDM_COND_TEXT);
-  CUDA_TRY(cudaGetLastError());
-  e->launches += 2;
+  TRY(fill_condproj(e, clip_dev, halves == 1 && force_uncond, s));
   TRY(cross_rows_per_sample(e, nullptr, s));
-  e->cond_set = true;
-  e->target_set = false;
-  e->inpaint_mask = nullptr;   // a new loop's conditioning: the previous loop's inpainting inputs no longer apply
-  e->inpaint_motion = nullptr;
+  end_cond(e);
   return B200MDM_OK;
 }
 
@@ -1178,13 +1208,12 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
   if (batch <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
   if (n_tokens <= 0 || n_tokens > XAL_MAX_MT)
     return fail(B200MDM_EINVAL, "n_tokens %d: a text memory holds 1..%d tokens (DistilBERT's position limit)", n_tokens, XAL_MAX_MT);
-  if (nframes + e->ctx > e->cfg.pos_embed_max_len) return fail(B200MDM_EINVAL, "sequence longer than the positional table");
-  if (nframes + e->ctx > ATC_MAX_KEYS) return fail(B200MDM_ENOTIMPL, "sequences of more than %d tokens", ATC_MAX_KEYS);
+  TRY(check_seq_len(e, nframes + e->ctx));
   if (!enc_text_dev || !text_mask_host) return fail(B200MDM_EINVAL, "DiP needs y['text_embed'] = (tokens, mask)");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int halves = scale_dev ? 2 : 1;
   TRY(select_workspace(e, batch, nframes, halves, s));
-  const int d = e->d, B = batch, S = e->S, Bp = e->Bp, Mt = n_tokens, C = e->cfg.cond_dim;
+  const int d = e->d, B = batch, Bp = e->Bp, Mt = n_tokens, C = e->cfg.cond_dim;
   if (Mt != e->Mt) {
     CUDA_TRY(cudaDeviceSynchronize());
     drop_graph(e);
@@ -1201,23 +1230,12 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
     e->Mt = Mt;
   }
   // key mask of the frames: the context frames are always valid (model/mdm.py:204-206), then `lengths` frames of x
-  std::vector<int>& kv = e->h_kv;
-  kv.assign(Bp, S);
-  if (e->cfg.mask_frames && lengths_host && S > 1) {
-    for (int b = 0; b < Bp; ++b) {
-      long long len = lengths_host[b % B];
-      if (len < 0) len = 0;
-      if (len > nframes) len = nframes;
-      kv[b] = static_cast<int>(len) + e->ctx;
-    }
-  }
+  TRY(upload_kvlen_scale(e, nframes, e->ctx, e->S > 1, lengths_host, scale_dev, s));
   std::vector<unsigned char>& mk = e->h_mask;
   mk.assign(static_cast<size_t>(Bp) * Mt, 0);
   for (int b = 0; b < Bp; ++b)
     for (int m = 0; m < Mt; ++m) mk[static_cast<size_t>(b) * Mt + m] = text_mask_host[static_cast<size_t>(b % B) * Mt + m] ? 1 : 0;
-  CUDA_TRY(cudaMemcpyAsync(e->kvlen, kv.data(), kv.size() * sizeof(int), cudaMemcpyHostToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(e->memmask, mk.data(), mk.size(), cudaMemcpyHostToDevice, s));
-  if (scale_dev) CUDA_TRY(cudaMemcpyAsync(e->scale, scale_dev, B * sizeof(float), cudaMemcpyDeviceToDevice, s));
   // text_emb = embed_text(mask_cond(enc_text)) per token (model/mdm.py:218), once per loop
   permute_mbc_kernel<<<dim3(Mt, B), 128, 0, s>>>(enc_text_dev, e->encperm, Mt, B, C);
   CUDA_TRY(cudaGetLastError());
@@ -1227,10 +1245,7 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
   memproj_fill_kernel<<<dim3(Mt, Bp), 128, 0, s>>>(e->memproj, e->memtok, e->b_txt, B, Mt, d, Bp, (halves == 1 && force_uncond) ? 1 : 0);
   CUDA_TRY(cudaGetLastError());
   e->launches += 3;
-  e->cond_set = true;
-  e->target_set = false;
-  e->inpaint_mask = nullptr;   // a new loop's conditioning: the previous loop's inpainting inputs no longer apply
-  e->inpaint_motion = nullptr;
+  end_cond(e);
   return B200MDM_OK;
 }
 
@@ -1252,10 +1267,7 @@ extern "C" int b200mdm_set_prefix(b200mdm_engine* e, const float* prefix_dev, vo
   if (!e || !prefix_dev) return fail(B200MDM_EINVAL, "null argument");
   if (!e->dec || e->ctx <= 0) return fail(B200MDM_EINVAL, "this engine has no prefix (context_len == 0)");
   if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond_dec first (it sizes the workspace)");
-  dim3 grid((e->ctx + 31) / 32, (e->JF + 31) / 32, e->B), block(32, 8);
-  pack_input_kernel<<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(prefix_dev, e->xin16, e->B, e->JF, e->ctx, e->S, e->Kp_in,
-                                                                          3 * e->Kp_in, 0);
-  CUDA_TRY(cudaGetLastError());
+  TRY(launch_pack_input(prefix_dev, e->xin16, e->B, e->JF, e->ctx, e->S, e->Kp_in, 0, static_cast<cudaStream_t>(stream)));
   e->launches++;
   e->prefix_set = true;
   return B200MDM_OK;
@@ -1367,6 +1379,13 @@ static int take_taps(const b200mdm_engine* e, const ForwardTaps& tp, int first, 
   return B200MDM_OK;
 }
 
+// The CLIP decoder's cross-attention rows of all layers at the step's timestep (tvec, or the step state's): out [L, Bp, d]
+static int launch_cross_rows(const b200mdm_engine* e, float* out, const int* tvec, int back, cudaStream_t s) {
+  CUDA_TRY(launch_k(cross_rows_kernel, dim3(e->Bp, e->L), dim3(128), 0, s, out, e->cross_b, e->cross_t, tvec, e->tmap, e->state,
+                    e->B, e->Bp, e->d, e->cfg.temb_rows, back));
+  return B200MDM_OK;
+}
+
 // Enqueue one denoiser forward (+ fused sampler step) on stream s.  Returns the number of kernels launched.
 // taps: stage copies for b200mdm_test_forward_taps, nullptr everywhere else.
 static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s, int* n_kernels,
@@ -1375,25 +1394,12 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
   int nk = 0;
   PdlScope pdl_scope;
   if (a.philox) {
-    const long long quads = (static_cast<long long>(JF) * T + 3) / 4 * B;
-    const int blocks = static_cast<int>(quads / 256 + 1 < 1184 ? quads / 256 + 1 : 1184);
-    CUDA_TRY(launch_k(philox_normal_kernel, dim3(blocks), dim3(256), 0, s, e->eps_buf, B, static_cast<long long>(JF) * T,
-                      0ull, 0ll, 0u, e->state));
+    TRY(launch_philox(e->eps_buf, B, static_cast<long long>(JF) * T, 0ull, 0ll, 0u, e->state, s));
     ++nk;
   }
-  {
-    dim3 grid((T + 31) / 32, (JF + 31) / 32, B), block(32, 8);
-    CUDA_TRY(launch_k(pack_input_kernel, grid, block, 0, s, a.x_in, e->xin16, B, JF, T, S, Kp, 3 * Kp, e->s_off));
-    ++nk;
-  }
-  {
-    EpiEmbed::Params p;
-    p.res_c = e->m_res_c; p.res_u = e->m_res_u;
-    p.pe_bias = e->pe_bias;
-    p.S = S; p.d = d; p.halves = e->halves;
-    TRY((launch_gemm<128, EpiEmbed>(e->m_xin, e->m_win, e->m_xin, e->MB, d, 3 * Kp, p, s, e->num_sms)));
-    ++nk;
-  }
+  TRY(launch_pack_input(a.x_in, e->xin16, B, JF, T, S, Kp, e->s_off, s));
+  TRY(launch_embed_gemm(e->m_xin, e->m_win, e->m_res_c, e->m_res_u, e->pe_bias, e->MB, S, d, Kp, e->halves, s, e->num_sms));
+  nk += 2;
   if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_EMBED, B200MDM_TAP_EMBED, -1, s));
   const float* target_g = e->target_set ? e->tgt_g : nullptr;   // timestep embedding + target (model/mdm.py:197-199)
   if (!e->dec || e->dec_clip) {
@@ -1403,8 +1409,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
                       e->cfg.temb_rows, a.back));
     if (e->dec_clip) {
       // every layer's cross-attention row of this step: c_l[b'] = cb_l[b'] + ct_l[t]
-      CUDA_TRY(launch_k(cross_rows_kernel, dim3(e->Bp, e->L), dim3(128), 0, s, e->cross_c, e->cross_b, e->cross_t,
-                        a.explicit_t ? e->tvec : nullptr, e->tmap, e->state, B, e->Bp, d, e->cfg.temb_rows, a.back));
+      TRY(launch_cross_rows(e, e->cross_c, a.explicit_t ? e->tvec : nullptr, a.back, s));
       ++nk;
     }
   } else {
@@ -1440,28 +1445,15 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_LN1, B200MDM_TAP_L_LN1, l, s));
     if (e->dec_clip) {
       // cross-attention block over the one-token memory + norm2: h <- LN2(h + c_l[b'])
-      CUDA_TRY(launch_k(row_bias_ln_kernel, dim3((e->M + RBLN_ROWS_PER_CTA - 1) / RBLN_ROWS_PER_CTA), dim3(32 * RBLN_ROWS_PER_CTA),
-                        0, s, e->hres, e->cross_c + static_cast<size_t>(l) * e->Bp * d, w.g2, w.be2, e->M, S, 1e-5f));
+      TRY(launch_row_bias_ln(e->hres, e->cross_c + static_cast<size_t>(l) * e->Bp * d, w.g2, w.be2, e->M, S, s));
       ++nk;
     } else if (e->dec) {
       // cross-attention block of nn.TransformerDecoderLayer: q from the sequence, k/v from the text memory
       TRY((launch_gemm_bias<false>(e->m_h16, w.m_wq_c, e->m_qc_st, e->M, d, d, w.bq_c, s, e->num_sms)));
       if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_QC, B200MDM_TAP_L_QC, l, s));
-      {
-        const float sl2 = 1.4426950408889634f / sqrtf(128.0f);
-        const dim3 cg(e->H, e->Bp), cb(128);
-        const __half* kvl = e->kvc16 + static_cast<size_t>(l) * 2 * d;      // this layer's k | v columns
-        const int ldkv = e->L * 2 * d;
-        if (e->Mt <= 16)
-          CUDA_TRY(launch_k(cross_attention_kernel<2>, cg, cb, 0, s, e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
-        else if (e->Mt <= 32)
-          CUDA_TRY(launch_k(cross_attention_kernel<4>, cg, cb, 0, s, e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
-        else if (e->Mt <= 64)
-          CUDA_TRY(launch_k(cross_attention_kernel<8>, cg, cb, 0, s, e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
-        else
-          CUDA_TRY(launch_k(cross_attention_long_kernel, dim3(e->H, e->Bp, (S + XAL_ROWS - 1) / XAL_ROWS), cb, XAL_SMEM, s,
-                            e->qc16, kvl, e->memmask, e->att16, S, e->Mt, d, ldkv, sl2));
-      }
+      // kv: this layer's k | v columns of the all-layer memory projection
+      TRY(launch_cross_attention(e->qc16, e->kvc16 + static_cast<size_t>(l) * 2 * d, e->memmask, e->att16, e->Bp, S, e->Mt, d,
+                                 e->H, e->L * 2 * d, s));
       if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_XATT, B200MDM_TAP_L_XATT, l, s));
       TRY(launch_gemm_resid_ln(e->m_att, w.m_wo_c_256, e->m_hres, e->M, d, w.bo_c, w.g2, w.be2, s, e->num_sms));   // cross-attention output: hi half
       nk += 3;
@@ -1479,8 +1471,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_LN3, B200MDM_TAP_L_LN3, l, s));
     nk += 5;
   }
-  CUDA_TRY(launch_k(blend_split_kernel, dim3((B * T + 7) / 8), dim3(256), 0, s, e->hres, e->g16, e->scale, B, S, T, e->s_off, d,
-                    e->halves));
+  TRY(launch_blend_split(e->hres, e->g16, e->scale, B, S, T, e->s_off, d, e->halves, s));
   ++nk;
   if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_BLEND, B200MDM_TAP_BLEND, -1, s));
   {
@@ -1900,12 +1891,8 @@ extern "C" int b200mdm_set_noise_stream(b200mdm_engine* e, uint64_t seed, int64_
 extern "C" int b200mdm_philox_normal(float* out_dev, int32_t batch, int64_t n_per_sample, uint64_t seed,
                                      int64_t sample_index_base, int32_t step_id, void* stream) {
   if (!out_dev || batch <= 0 || n_per_sample <= 0) return fail(B200MDM_EINVAL, "bad argument");
-  const long long quads = (n_per_sample + 3) / 4 * batch;
-  const int blocks = static_cast<int>(quads / 256 + 1 < 1184 ? quads / 256 + 1 : 1184);
-  philox_normal_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(out_dev, batch, n_per_sample, seed, sample_index_base,
-                                                                             static_cast<uint32_t>(step_id), nullptr);
-  CUDA_TRY(cudaGetLastError());
-  return B200MDM_OK;
+  return launch_philox(out_dev, batch, n_per_sample, seed, sample_index_base, static_cast<uint32_t>(step_id), nullptr,
+                       static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b200mdm_q_sample(b200mdm_engine* e, float sqrt_ac, float sqrt_1mac, const float* x_start_dev,
@@ -1926,39 +1913,29 @@ extern "C" int64_t b200mdm_launch_count(b200mdm_engine* e, int32_t reset) {
 }
 
 // ------------------------------------------------------------------------------------------------ kernel tests
-template <int BN, bool RES = false>
-static int test_gemm_bn(const void* a16, const void* w16, const float* bias, void* out16, int M, int N, int K, int act,
-                        cudaStream_t s, int sms) {
-  CUtensorMap ma, mb, mc;
-  TRY(make_map(&ma, a16, M, K, K, GEMM_BLOCK_M));
-  TRY(make_map(&mb, w16, N, K, K, BN));
-  TRY(make_map_t(&mc, out16, 2, M, N, N, 32));
-  EpiBiasF16<true>::Params pg{bias};
-  EpiBiasF16<false>::Params pn{bias};
-  if constexpr (RES)
-    return act ? launch_gemm_resident<BN, EpiBiasF16<true>>(ma, mb, mc, M, N, K, pg, s, sms)
-               : launch_gemm_resident<BN, EpiBiasF16<false>>(ma, mb, mc, M, N, K, pn, s, sms);
-  else if constexpr (BN == PP_BLOCK_N)   // the step's projection kernel
-    return act ? launch_gemm_pp<EpiBiasF16<true>>(ma, mb, mc, M, N, K, pg, s, sms)
-               : launch_gemm_pp<EpiBiasF16<false>>(ma, mb, mc, M, N, K, pn, s, sms);
-  else
-    return act ? launch_gemm<BN, EpiBiasF16<true>>(ma, mb, mc, M, N, K, pg, s, sms)
-               : launch_gemm<BN, EpiBiasF16<false>>(ma, mb, mc, M, N, K, pn, s, sms);
+static int device_sms(int* sms) {
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  CUDA_TRY(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+  return B200MDM_OK;
 }
 
 extern "C" int b200mdm_test_gemm_f16(const void* a16_dev, const void* w16_dev, const float* bias_dev, void* out16_dev,
                                      int32_t M, int32_t N, int32_t K, int32_t act, int32_t block_n, void* stream) {
   if (!a16_dev || !w16_dev || !bias_dev || !out16_dev || M <= 0 || N <= 0 || K <= 0 || K % 8 || N % 8)
     return fail(B200MDM_EINVAL, "bad argument (K %% 8 == 0, N %% 8 == 0 required)");
+  if (block_n != PP_BLOCK_N)
+    return fail(B200MDM_EINVAL, "block_n must be 128 (the 128 x 128 tiles of the step's ping-pong projection kernel)");
   TRY(init_kernel_attrs());
-  int dev = 0, sms = 132;
-  CUDA_TRY(cudaGetDevice(&dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms = 132;
+  TRY(device_sms(&sms));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (block_n == 128) return test_gemm_bn<128>(a16_dev, w16_dev, bias_dev, out16_dev, M, N, K, act, s, sms);
-  if (block_n == 512) return test_gemm_bn<256>(a16_dev, w16_dev, bias_dev, out16_dev, M, N, K, act, s, sms);
-  if (block_n == 513) return test_gemm_bn<64, true>(a16_dev, w16_dev, bias_dev, out16_dev, M, N, K, act, s, sms);
-  return fail(B200MDM_EINVAL, "block_n must be 128 (128 x 128 tiles), 512 (128 x 256 tiles) or 513 (W-resident, 128 x 64 tiles)");
+  CUtensorMap ma, mb, mc;
+  TRY(make_map(&ma, a16_dev, M, K, K, GEMM_BLOCK_M));
+  TRY(make_map(&mb, w16_dev, N, K, K, PP_BLOCK_N));
+  TRY(make_map_t(&mc, out16_dev, 2, M, N, N, 32));
+  return act ? launch_gemm_bias<true>(ma, mb, mc, M, N, K, bias_dev, s, sms)
+             : launch_gemm_bias<false>(ma, mb, mc, M, N, K, bias_dev, s, sms);
 }
 
 // Scratch device memory of a kernel-test entry point, allocated and freed in the order of `s`.
@@ -1977,13 +1954,6 @@ struct StreamScratch {
     return B200MDM_OK;
   }
 };
-
-static int device_sms(int* sms) {
-  int dev = 0;
-  CUDA_TRY(cudaGetDevice(&dev));
-  CUDA_TRY(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
-  return B200MDM_OK;
-}
 
 extern "C" int b200mdm_test_gemm_epi(const void* a16_dev, const void* w16_dev, const float* bias_dev, void* out16_dev,
                                      int32_t M, int32_t N, int32_t K, int32_t epi, void* stream) {
@@ -2029,24 +1999,41 @@ extern "C" int b200mdm_test_embed(const float* x_dev, const float* w_in_dev, con
   TRY(scr.alloc(&xin16, static_cast<size_t>(MB) * 3 * Kp, true));   // rows s < s_off and the pad columns stay zero
   TRY(scr.alloc(&w_in3, static_cast<size_t>(d) * 3 * Kp, true));
   TRY(scr.alloc(&pe_bias, static_cast<size_t>(S) * d));
-  {
-    dim3 grid((T + 31) / 32, (JF + 31) / 32, B), block(32, 8);
-    pack_input_kernel<<<grid, block, 0, s>>>(x_dev, xin16, B, JF, T, S, Kp, 3 * Kp, s_off);
-    CUDA_TRY(cudaGetLastError());
-  }
+  TRY(launch_pack_input(x_dev, xin16, B, JF, T, S, Kp, s_off, s));
   split_weight_kernel<<<d, 128, 0, s>>>(w_in_dev, w_in3, d, JF, Kp);
   CUDA_TRY(cudaGetLastError());
   pe_bias_kernel<<<S, 128, 0, s>>>(pe_bias, pe_dev, b_in_dev, S, d);
   CUDA_TRY(cudaGetLastError());
-  CUtensorMap m_xin, m_win;
+  CUtensorMap m_xin, m_win, m_res_c, m_res_u;
   TRY(make_map(&m_xin, xin16, MB, 3 * Kp, 3 * Kp, GEMM_BLOCK_M));
   TRY(make_map(&m_win, w_in3, d, 3 * Kp, 3 * Kp, 128));
-  EpiEmbed::Params p;
-  TRY(make_map_res(&p.res_c, hres16_dev, MB, d));
-  TRY(make_map_res(&p.res_u, static_cast<__half*>(hres16_dev) + (halves == 2 ? static_cast<size_t>(MB) * d * 2 : 0), MB, d));
-  p.pe_bias = pe_bias;
-  p.S = S; p.d = d; p.halves = halves;
-  return launch_gemm<128, EpiEmbed>(m_xin, m_win, m_xin, MB, d, 3 * Kp, p, s, sms);
+  TRY(make_map_res(&m_res_c, hres16_dev, MB, d));
+  TRY(make_map_res(&m_res_u, static_cast<__half*>(hres16_dev) + (halves == 2 ? static_cast<size_t>(MB) * d * 2 : 0), MB, d));
+  return launch_embed_gemm(m_xin, m_win, m_res_c, m_res_u, pe_bias, MB, S, d, Kp, halves, s, sms);
+}
+
+// What the two output-step hooks share, on scratch memory of `scr`: g16 = the CFG blend of hres, the split output
+// weight, the maps of both, and the bias / inpainting fields of the epilogue parameters.
+struct OutHook {
+  CUtensorMap m_g16, m_wout;
+  EpiOutParams p{};
+};
+static int out_hook_setup(StreamScratch& scr, OutHook* o, const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
+                          const float* b_out_dev, const uint8_t* inpaint_mask_dev, const float* inpaint_motion_dev, int B, int JF,
+                          int T, int d, int s_off, int halves) {
+  const int N_out_pad = ((JF + 95) / 96) * 96;
+  __half *g16 = nullptr, *w_out3 = nullptr;
+  TRY(scr.alloc(&g16, static_cast<size_t>(B) * T * 3 * d));
+  TRY(scr.alloc(&w_out3, static_cast<size_t>(N_out_pad) * 3 * d, true));
+  split_weight_kernel<<<JF, 128, 0, scr.s>>>(w_out_dev, w_out3, JF, d, d);
+  CUDA_TRY(cudaGetLastError());
+  TRY(launch_blend_split(static_cast<const __half*>(hres16_dev), g16, scale_dev, B, T + s_off, T, s_off, d, halves, scr.s));
+  TRY(make_map(&o->m_g16, g16, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
+  TRY(make_map(&o->m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
+  o->p.bias = b_out_dev;
+  o->p.inpaint_mask = inpaint_mask_dev;
+  o->p.inpaint_motion = inpaint_motion_dev;
+  return B200MDM_OK;
 }
 
 extern "C" int b200mdm_test_out_step(const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
@@ -2063,27 +2050,14 @@ extern "C" int b200mdm_test_out_step(const void* hres16_dev, const float* scale_
   int sms = 132;
   TRY(device_sms(&sms));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int S = T + s_off, N_out_pad = ((JF + 95) / 96) * 96;
   StreamScratch scr(s);
-  __half *g16 = nullptr, *w_out3 = nullptr;
+  OutHook o;
+  TRY(out_hook_setup(scr, &o, hres16_dev, scale_dev, w_out_dev, b_out_dev, inpaint_mask_dev, inpaint_motion_dev, B, JF, T, d,
+                     s_off, halves));
   StepState* st = nullptr;
-  TRY(scr.alloc(&g16, static_cast<size_t>(B) * T * 3 * d));
-  TRY(scr.alloc(&w_out3, static_cast<size_t>(N_out_pad) * 3 * d, true));
   TRY(scr.alloc(&st, 1, true));   // cur = 0: the one-row schedule table
-  split_weight_kernel<<<JF, 128, 0, s>>>(w_out_dev, w_out3, JF, d, d);
-  CUDA_TRY(cudaGetLastError());
-  blend_split_kernel<<<(B * T + 7) / 8, 256, 0, s>>>(static_cast<const __half*>(hres16_dev), g16, scale_dev, B, S, T, s_off, d,
-                                                     halves);
-  CUDA_TRY(cudaGetLastError());
-  CUtensorMap m_g16, m_wout;
-  TRY(make_map(&m_g16, g16, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
-  TRY(make_map(&m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
-  EpiOutParams p{};
-  p.bias = b_out_dev;
-  p.inpaint_mask = inpaint_mask_dev;
-  p.inpaint_motion = inpaint_motion_dev;
-  p.sched = sched_row_dev;
-  p.state = st;
+  o.p.sched = sched_row_dev;
+  o.p.state = st;
   StepArgs a;
   a.mode = mode;
   a.x_in = x_t_dev;
@@ -2092,7 +2066,7 @@ extern "C" int b200mdm_test_out_step(const void* hres16_dev, const float* scale_
   a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
   a.x_out = x_out_dev;
   a.pred = pred_xstart_dev;
-  return launch_out_gemm(m_g16, m_wout, B, T, JF, d, a, p, s, sms);
+  return launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms);
 }
 
 extern "C" int b200mdm_test_out_dpm(const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
@@ -2109,41 +2083,28 @@ extern "C" int b200mdm_test_out_dpm(const void* hres16_dev, const float* scale_d
   int sms = 132;
   TRY(device_sms(&sms));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int S = T + s_off, N_out_pad = ((JF + 95) / 96) * 96;
   StreamScratch scr(s);
-  __half *g16 = nullptr, *w_out3 = nullptr;
+  OutHook o;
+  TRY(out_hook_setup(scr, &o, hres16_dev, scale_dev, w_out_dev, b_out_dev, inpaint_mask_dev, inpaint_motion_dev, B, JF, T, d,
+                     s_off, halves));
   float* table = nullptr;
   StepState* st = nullptr;
-  TRY(scr.alloc(&g16, static_cast<size_t>(B) * T * 3 * d));
-  TRY(scr.alloc(&w_out3, static_cast<size_t>(N_out_pad) * 3 * d, true));
   TRY(scr.alloc(&table, static_cast<size_t>(index + 1) * SCHED_DPM_STRIDE, true));   // the row at `index`, zeros above
   TRY(scr.alloc(&st, 1, true));
   CUDA_TRY(cudaMemcpyAsync(table + static_cast<size_t>(index) * SCHED_DPM_STRIDE, dpm_row_dev, SCHED_DPM_STRIDE * sizeof(float),
                            cudaMemcpyDeviceToDevice, s));
   step_set_kernel<<<1, 1, 0, s>>>(st, step, index, nullptr, 0, 0, 0, index + 1);
   CUDA_TRY(cudaGetLastError());
-  split_weight_kernel<<<JF, 128, 0, s>>>(w_out_dev, w_out3, JF, d, d);
-  CUDA_TRY(cudaGetLastError());
-  blend_split_kernel<<<(B * T + 7) / 8, 256, 0, s>>>(static_cast<const __half*>(hres16_dev), g16, scale_dev, B, S, T, s_off, d,
-                                                     halves);
-  CUDA_TRY(cudaGetLastError());
-  CUtensorMap m_g16, m_wout;
-  TRY(make_map(&m_g16, g16, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
-  TRY(make_map(&m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
-  EpiOutParams p{};
-  p.bias = b_out_dev;
-  p.inpaint_mask = inpaint_mask_dev;
-  p.inpaint_motion = inpaint_motion_dev;
-  p.sched_dpm = table;
-  p.x0_hist = x0_hist_dev;
-  p.state = st;
+  o.p.sched_dpm = table;
+  o.p.x0_hist = x0_hist_dev;
+  o.p.state = st;
   StepArgs a;
   a.mode = MODE_DPM;
   a.order = order;
   a.x_in = x_t_dev;
   a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
   a.x_out = x_out_dev;
-  return launch_out_gemm(m_g16, m_wout, B, T, JF, d, a, p, s, sms);
+  return launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms);
 }
 
 extern "C" int b200mdm_test_attention(const void* qkv16_dev, void* out16_dev, const int32_t* kvlen_dev,
@@ -2166,21 +2127,10 @@ extern "C" int b200mdm_test_cross_attention(const void* q16_dev, const void* kv1
   if (!q16_dev || !kv16_dev || !mask_dev || !out16_dev || n_samples <= 0 || S <= 0 || n_tokens <= 0 || n_tokens > XAL_MAX_MT ||
       ld_kv < 2 * d || ld_kv % 8)
     return fail(B200MDM_EINVAL, "bad argument");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const float sl2 = 1.4426950408889634f / sqrtf(128.0f);
-  const dim3 cg(d / 128, n_samples), cb(128);
-  const __half* q = static_cast<const __half*>(q16_dev);
-  const __half* kv = static_cast<const __half*>(kv16_dev);
-  __half* o = static_cast<__half*>(out16_dev);
-  if (n_tokens <= 16) CUDA_TRY(launch_k(cross_attention_kernel<2>, cg, cb, 0, s, q, kv, mask_dev, o, S, n_tokens, d, ld_kv, sl2));
-  else if (n_tokens <= 32) CUDA_TRY(launch_k(cross_attention_kernel<4>, cg, cb, 0, s, q, kv, mask_dev, o, S, n_tokens, d, ld_kv, sl2));
-  else if (n_tokens <= 64) CUDA_TRY(launch_k(cross_attention_kernel<8>, cg, cb, 0, s, q, kv, mask_dev, o, S, n_tokens, d, ld_kv, sl2));
-  else {
-    TRY(init_kernel_attrs());
-    CUDA_TRY(launch_k(cross_attention_long_kernel, dim3(d / 128, n_samples, (S + XAL_ROWS - 1) / XAL_ROWS), cb, XAL_SMEM, s, q, kv,
-                      mask_dev, o, S, n_tokens, d, ld_kv, sl2));
-  }
-  return B200MDM_OK;
+  TRY(init_kernel_attrs());
+  return launch_cross_attention(static_cast<const __half*>(q16_dev), static_cast<const __half*>(kv16_dev), mask_dev,
+                                static_cast<__half*>(out16_dev), n_samples, S, n_tokens, d, d / 128, ld_kv,
+                                static_cast<cudaStream_t>(stream));
 }
 
 // QKV projection + attention core of an encoder layer, the two launches the step makes, through a scratch qkv buffer.
@@ -2191,9 +2141,8 @@ extern "C" int b200mdm_test_qkv_attention(const void* h16_dev, int32_t ld, const
       ld < 512 || ld % 8)
     return fail(B200MDM_EINVAL, "bad argument");
   TRY(init_kernel_attrs());
-  int dev = 0, sms = 132;
-  CUDA_TRY(cudaGetDevice(&dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms = 132;
+  TRY(device_sms(&sms));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int M = n_samples * S;
   __half* qkv = nullptr;
@@ -2216,9 +2165,8 @@ extern "C" int b200mdm_test_gemm_resid_ln(const void* a16_dev, const void* w16_d
   if (!a16_dev || !w16_dev || !bias_dev || !gamma_dev || !beta_dev || !hres16_dev || M <= 0 || K <= 0 || K % 8)
     return fail(B200MDM_EINVAL, "bad argument");
   TRY(init_kernel_attrs());
-  int dev = 0, sms = 132;
-  CUDA_TRY(cudaGetDevice(&dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms = 132;
+  TRY(device_sms(&sms));
   CUtensorMap ma, mb, mh;
   TRY(make_map(&ma, a16_dev, M, K, K, GEMM_BLOCK_M));
   TRY(make_map(&mb, w16_dev, GLN_D, K, K, 256));
@@ -2234,9 +2182,7 @@ extern "C" int b200mdm_test_cross_rows(b200mdm_engine* e, int32_t timestep, floa
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   std::vector<int> t(e->B, timestep);
   CUDA_TRY(cudaMemcpyAsync(e->tvec, t.data(), e->B * sizeof(int), cudaMemcpyHostToDevice, s));
-  cross_rows_kernel<<<dim3(e->Bp, e->L), 128, 0, s>>>(out_dev, e->cross_b, e->cross_t, e->tvec, e->tmap, e->state, e->B, e->Bp,
-                                                      e->d, e->cfg.temb_rows, 0);
-  CUDA_TRY(cudaGetLastError());
+  TRY(launch_cross_rows(e, out_dev, e->tvec, 0, s));
   CUDA_TRY(cudaStreamSynchronize(s));   // `t` is local
   return B200MDM_OK;
 }
@@ -2247,10 +2193,7 @@ extern "C" int b200mdm_test_row_bias_ln(void* hres16_dev, const float* c_dev, co
   if ((reinterpret_cast<uintptr_t>(hres16_dev) | reinterpret_cast<uintptr_t>(c_dev) | reinterpret_cast<uintptr_t>(gamma_dev) |
        reinterpret_cast<uintptr_t>(beta_dev)) & 15)
     return fail(B200MDM_EINVAL, "operands must be 16-byte aligned");
-  row_bias_ln_kernel<<<(M + RBLN_ROWS_PER_CTA - 1) / RBLN_ROWS_PER_CTA, 32 * RBLN_ROWS_PER_CTA, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<__half*>(hres16_dev), c_dev, gamma_dev, beta_dev, M, S, 1e-5f);
-  CUDA_TRY(cudaGetLastError());
-  return B200MDM_OK;
+  return launch_row_bias_ln(static_cast<__half*>(hres16_dev), c_dev, gamma_dev, beta_dev, M, S, static_cast<cudaStream_t>(stream));
 }
 
 #ifdef B200_TRACE

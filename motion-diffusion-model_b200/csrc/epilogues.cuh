@@ -1,6 +1,6 @@
 // Fused GEMM epilogues (see gemm.cuh for the calling protocol).  Thread = accumulator row.  The projection epilogues
-// (EpiBiasF16, EpiBiasF16Global, EpiBiasF16Wide) also provide the fragment interface of gemm_pingpong.cuh (pp_*: one
-// column pair of the wgmma accumulator fragment at a time, same arithmetic).
+// (EpiBiasF16, EpiBiasF16Global, EpiBiasF16Wide) provide the fragment interface of gemm_pingpong.cuh instead (pp_*:
+// one column pair of the wgmma accumulator fragment at a time).
 //
 // Row-major outputs are written as 128-byte-per-row slabs (32 rows of the warp x 64 fp16 or 32 fp32 columns = 4 KB)
 // staged in warp-private shared memory in the TMA 128-byte swizzle and shipped with cp.async.bulk.tensor stores;
@@ -67,27 +67,6 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return x * phi;
 }
 
-// Stage the bias of the tile in flight (up to 256 columns) in warp-private shared memory so that the row-owning
-// threads read it with broadcast LDS instead of dependent global loads inside the chunk loop.
-__device__ __forceinline__ void stage_bias(float* bs, const float* bias, int col_base, int N, int lane) {
-  __syncwarp();
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int idx = i * 128 + lane * 4;
-    const int col = col_base + idx;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (col + 3 < N) {
-      v = __ldg(reinterpret_cast<const float4*>(bias + col));
-    } else {
-      if (col + 0 < N) v.x = bias[col + 0];
-      if (col + 1 < N) v.y = bias[col + 1];
-      if (col + 2 < N) v.z = bias[col + 2];
-    }
-    *reinterpret_cast<float4*>(bs + idx) = v;
-  }
-  __syncwarp();
-}
-
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
@@ -95,15 +74,10 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
 
 // ---------------------------------------------------------------------------------------------------------
 // out16[row, col] = fp16( act(acc + bias[col]) )          (QKV projection, FFN up-projection)
-// Two 32-column chunks fill one 64-column (128-byte) slab; slabs are double-buffered.  map_c: fp16 [M, N],
-// box {64 cols, 32 rows}, SWIZZLE_128B.
+// map_c: fp16 [M, N], box {64 cols, 32 rows}, SWIZZLE_128B.  Fragment interface only (gemm_f16_pingpong), like
+// EpiBiasF16Wide / EpiBiasF16Global.
 template <bool GELU>
 struct EpiBiasF16 {
-  // one output slab + the tile's bias: with 8 epilogue warps the wait for the previous slab's TMA store overlaps the
-  // other warps' work, and the 4 KB saved per warp buy one more operand pipeline stage (the layer GEMMs are bound
-  // by operand bytes in flight)
-  static constexpr int NSLAB = 1;
-  static constexpr int SMEM_PER_WARP = NSLAB * 4096;
   struct Params {
     const float* bias;
   };
@@ -112,51 +86,7 @@ struct EpiBiasF16 {
   static __device__ __forceinline__ void preload(const Params& p, float* dst, int N, int tid, int nthreads) {
     for (int i = tid; i < N; i += nthreads) dst[i] = p.bias[i];
   }
-  static __device__ __forceinline__ void tile_begin(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params&, uint32_t (&raw)[32], int row0, int col0, int) {
-    chunk_bias(ctx, ctx.bias_all + col0, raw, row0, col0);   // chunk() is only called for col0 < N, N % 32 == 0 here
-  }
-  static __device__ __forceinline__ void chunk_bias(EpiCtx& ctx, const float* bs, uint32_t (&raw)[32], int row0, int col0) {
-    const int half = (col0 >> 5) & 1;
-    uint8_t* slab = ctx.smem + (ctx.seq % NSLAB) * 4096;
-    if (half == 0) {
-      // the store that last read this buffer (NSLAB slabs ago) must have finished reading
-      if (ctx.lane == 0) bulk_wait_group_read<NSLAB - 1>();
-      __syncwarp();
-    }
-    uint32_t pk[16];
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      const float4 b = *reinterpret_cast<const float4*>(bs + j);
-      float x0 = __uint_as_float(raw[j + 0]) + b.x, x1 = __uint_as_float(raw[j + 1]) + b.y;
-      float x2 = __uint_as_float(raw[j + 2]) + b.z, x3 = __uint_as_float(raw[j + 3]) + b.w;
-      if (GELU) {
-        x0 = gelu_erf(x0); x1 = gelu_erf(x1); x2 = gelu_erf(x2); x3 = gelu_erf(x3);
-      }
-      pk[j / 2] = pack_half2(x0, x1);
-      pk[j / 2 + 1] = pack_half2(x2, x3);
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      *reinterpret_cast<uint4*>(slab + slab_off(ctx.lane, half * 4 + j)) =
-          make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-    if (half == 1 || col0 + 32 >= ctx.N) {
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (ctx.lane == 0) {
-        tma_store_2d(ctx.map_c, slab, col0 - 32 * half, row0);
-        bulk_commit_group();
-      }
-      ctx.seq++;
-    }
-  }
-  static __device__ __forceinline__ void tile_end(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void finish(EpiCtx& ctx) {
-    if (ctx.lane == 0) bulk_wait_group<0>();
-    __syncwarp();
-  }
-
-  // ---- fragment interface (gemm_pingpong.cuh): one column pair of one accumulator row at a time
+  // one column pair of one accumulator row at a time
   static constexpr int PP_ROUND_COLS = 128;   // a round fills two 64-column slabs (16 KB each) of the warpgroup's 128 rows
   // the bias of the tile's 128 columns (col_t = first column): here a view of the CTA's staged vector
   static __device__ __forceinline__ const float* pp_tile_bias(const Params&, const float* bias_all, float*, int col_t, int, int) {

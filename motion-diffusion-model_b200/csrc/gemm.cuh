@@ -6,22 +6,17 @@
 //                      tile, accumulators in registers, and then runs the fused epilogue of those rows itself.
 //
 // Epilogue: the accumulator fragment is staged through a warpgroup-private fp32 tile in shared memory so that the fused
-// epilogue functors see it as "thread = row" -- warp w of the warpgroup owns rows [32 (w & 1), +32) and every other
-// 64-column block (part = w >> 1), lane = row; each 32-column chunk is handed to the functor, which stages its
+// epilogue functors see it as "thread = row" -- warp w of the warpgroup owns rows [32 (w & 1), +32) and the
+// 64-column block part = w >> 1 of the tile (BLOCK_N <= 128), lane = row; each 32-column chunk is handed to the functor, which stages its
 // 128-byte-per-row output slab in warp-private shared memory (128B swizzle) and ships it with a TMA store.
 //
 // Tiles are statically strided over the persistent grid (tile = blockIdx.x + k * gridDim.x, N fastest so concurrently
 // running CTAs share the same A rows in L2).  The step runs this kernel for the embedding (BLOCK_N = 128) and the output
 // projection (96), once per step each; the per-layer projections run on gemm_f16_pingpong (gemm_pingpong.cuh), which
-// takes its epilogue from the accumulator fragment.  BLOCK_N = 256 and the W-resident variant are measured alternatives
-// reached only through b200mdm_test_gemm_f16 (both slower at the step's shapes, DESIGN.md section 4).  W-resident
-// variant (RESIDENT, K <= 512): CTA c owns column block
-// c % tiles_n for the whole launch and, among the CTAs of that block, every m_step-th row block starting at c / tiles_n;
-// it loads its [BLOCK_N x K] W tile into shared memory once (k-block by k-block, so the first tile still pipelines) and
-// streams only A.  A is [M,K] row-major (K contiguous), W is the torch nn.Linear layout
-// [N,K] row-major -- both K-major wgmma operands, no transposes anywhere.  While the consumers run the epilogue of tile
-// i the producer already streams the operands of tile i+1.  K tails / M tails / N tails rely on TMA out-of-bounds zero
-// fill (loads) and clipping (stores).
+// takes its epilogue from the accumulator fragment.  A is [M,K] row-major (K contiguous), W is the torch nn.Linear
+// layout [N,K] row-major -- both K-major wgmma operands, no transposes anywhere.  While the consumers run the epilogue
+// of tile i the producer already streams the operands of tile i+1.  K tails / M tails / N tails rely on TMA
+// out-of-bounds zero fill (loads) and clipping (stores).
 #pragma once
 #include "ptx.cuh"
 
@@ -34,28 +29,24 @@ constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_BAR_BYTES = 1024;
 constexpr int GEMM_BIAS_BYTES = 8192;   // per-column epilogue vector (bias) of the whole GEMM, staged once per CTA: N <= 2048
 
-constexpr int GEMM_RES_KB_MAX = 8;   // W-resident variant: k-blocks of 64 kept in shared memory, K <= 512
 // setmaxnreg: the producer warpgroup hands its registers to the consumers (40 + 2 x 232 <= 3 x 168, the pool of a
-// 384-thread CTA), which a 256-wide tile needs for its 128 accumulators per thread
+// 384-thread CTA).  The values are the ones the measured numbers in DESIGN.md section 5 were taken with.
 constexpr int GEMM_REGS_PRODUCER = 40, GEMM_REGS_CONSUMER = 232;
 
-// the accumulator is staged for the epilogue in rounds of at most 128 columns
 template <int BLOCK_N>
-constexpr int gemm_stage_cols() { return BLOCK_N < 128 ? BLOCK_N : 128; }
-template <int BLOCK_N>
-constexpr int gemm_stage_ld() { return gemm_stage_cols<BLOCK_N>() + 4; }   // fp32 row pitch of the staging tile (bank spread)
+constexpr int gemm_stage_ld() { return BLOCK_N + 4; }   // fp32 row pitch of the staging tile (bank spread)
 
-template <int BLOCK_N, class Epi, bool RESIDENT = false>
+template <int BLOCK_N, class Epi>
 struct GemmSmem {
+  static_assert(BLOCK_N <= 128, "the whole accumulator tile is staged for the epilogue at once");
   static constexpr int A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;  // 16 KB
   static constexpr int B_BYTES = BLOCK_N * GEMM_BLOCK_K * 2;       // one k-block of the W tile
-  static constexpr int STAGE_BYTES = A_BYTES + (RESIDENT ? 0 : B_BYTES);
-  static constexpr int W_BYTES = RESIDENT ? GEMM_RES_KB_MAX * B_BYTES : 0;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int ACC_BYTES = 2 * 64 * gemm_stage_ld<BLOCK_N>() * 4;   // one staging tile per consumer warpgroup
   static constexpr int EPI_BYTES = GEMM_EPI_WARPS * Epi::SMEM_PER_WARP;  // SMEM_PER_WARP is a multiple of 1024
-  static constexpr int budget = 227 * 1024 - 1024 /*alignment slack*/ - W_BYTES - ACC_BYTES - EPI_BYTES - GEMM_BIAS_BYTES - GEMM_BAR_BYTES;
+  static constexpr int budget = 227 * 1024 - 1024 /*alignment slack*/ - ACC_BYTES - EPI_BYTES - GEMM_BIAS_BYTES - GEMM_BAR_BYTES;
   static constexpr int STAGES = (budget / STAGE_BYTES) > 6 ? 6 : (budget / STAGE_BYTES);
-  static constexpr int TOTAL = 1024 + W_BYTES + STAGES * STAGE_BYTES + EPI_BYTES + ACC_BYTES + GEMM_BIAS_BYTES + GEMM_BAR_BYTES;
+  static constexpr int TOTAL = 1024 + STAGES * STAGE_BYTES + EPI_BYTES + ACC_BYTES + GEMM_BIAS_BYTES + GEMM_BAR_BYTES;
   static_assert(STAGES >= 2, "not enough shared memory for a pipeline");
   static_assert(Epi::SMEM_PER_WARP % 1024 == 0, "epilogue slabs must keep 1024-byte alignment (128B swizzle)");
   static_assert(B_BYTES % 1024 == 0, "W tiles must keep 1024-byte alignment (128B swizzle)");
@@ -73,18 +64,15 @@ struct EpiCtx {
   uint32_t seq;         // running chunk / block counter (buffer rotation), functor-defined
 };
 
-// Write columns [c0, c0 + gemm_stage_cols) of a warpgroup's accumulator fragment (rows [0, 64) of its half tile) into the
-// fp32 staging tile (c0 is a compile-time multiple of 128 after unrolling).
+// Write a warpgroup's accumulator fragment (rows [0, 64) of its half tile) into the fp32 staging tile.
 template <int BLOCK_N>
-__device__ __forceinline__ void stage_acc(float* st, const float (&acc)[BLOCK_N / 2], int c0, int wq, int lane) {
+__device__ __forceinline__ void stage_acc(float* st, const float (&acc)[BLOCK_N / 2], int wq, int lane) {
   constexpr int LD = gemm_stage_ld<BLOCK_N>();
-  constexpr int NJ = gemm_stage_cols<BLOCK_N>() / 8;
   const int r = 16 * wq + (lane >> 2), c = 2 * (lane & 3);
 #pragma unroll
-  for (int jj = 0; jj < NJ; ++jj) {
-    const int j = c0 / 8 + jj;
-    *reinterpret_cast<float2*>(st + r * LD + 8 * jj + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
-    *reinterpret_cast<float2*>(st + (r + 8) * LD + 8 * jj + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    *reinterpret_cast<float2*>(st + r * LD + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(st + (r + 8) * LD + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
   }
 }
 // thread = row: 32 consecutive fp32 accumulator columns of row `row` of the staging tile
@@ -108,12 +96,12 @@ __device__ __forceinline__ void load_row32(const float* st, int row, int col, ui
 //                                                   next_col0 = first column of this warp's next chunk in the tile, or -1
 //   tile_end(ctx, p, row0, col_base)                after the last chunk
 //   finish(ctx)                                     once, before the CTA exits (drain async stores)
-template <int BLOCK_N, class Epi, bool RESIDENT = false>
+template <int BLOCK_N, class Epi>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_c, int M, int N, int K,
                const __grid_constant__ typename Epi::Params ep) {
-  using SM = GemmSmem<BLOCK_N, Epi, RESIDENT>;
+  using SM = GemmSmem<BLOCK_N, Epi>;
   using MMA = Wgmma<BLOCK_N>;
   constexpr int STAGES = SM::STAGES;
   constexpr int NREG = BLOCK_N / 2;
@@ -121,27 +109,20 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* wres = smem;                                   // RESIDENT: [KB_MAX][BLOCK_N rows x 128 B]
-  uint8_t* tiles = smem + SM::W_BYTES;
+  uint8_t* tiles = smem;
   uint8_t* epi_smem = tiles + STAGES * SM::STAGE_BYTES;
   float* acc_stage = reinterpret_cast<float*>(epi_smem + SM::EPI_BYTES);
   float* bias_all = reinterpret_cast<float*>(epi_smem + SM::EPI_BYTES + SM::ACC_BYTES);
   uint64_t* bars = reinterpret_cast<uint64_t*>(epi_smem + SM::EPI_BYTES + SM::ACC_BYTES + GEMM_BIAS_BYTES);
   uint64_t* full_bar = bars;                    // [STAGES]
   uint64_t* empty_bar = bars + STAGES;          // [STAGES]  one arrival per consumer warp
-  uint64_t* w_full = bars + 2 * STAGES;         // [KB_MAX]  RESIDENT: W k-block landed (armed once)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int tiles_m = (M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M;
   const int tiles_n = (N + BLOCK_N - 1) / BLOCK_N;
   const int num_tiles = tiles_m * tiles_n;
-  const int num_kb = (K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;   // RESIDENT: the launcher guarantees <= KB_MAX
-  // tile order: strided (tile = first + k * step, N fastest), or RESIDENT: one column block per CTA (launcher guarantees
-  // tiles_n <= gridDim.x), its row blocks m_first, m_first + m_step, ...
-  const int res_n = blockIdx.x % tiles_n;
-  const int first = RESIDENT ? (blockIdx.x / tiles_n) * tiles_n + res_n : blockIdx.x;
-  const int step = RESIDENT ? ((gridDim.x - res_n + tiles_n - 1) / tiles_n) * tiles_n : gridDim.x;
+  const int num_kb = (K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
 
   pdl_launch_dependents();
   Epi::preload(ep, bias_all, N, threadIdx.x, blockDim.x);   // visible to the consumers after the barrier below
@@ -153,8 +134,6 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], GEMM_EPI_WARPS);
     }
-    if (RESIDENT)
-      for (int s = 0; s < GEMM_RES_KB_MAX; ++s) mbar_init(&w_full[s], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -166,22 +145,16 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     if (warp == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      bool first_tile = true;
-      for (int tile = first; tile < num_tiles; tile += step) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_blk = tile / tiles_n, n_blk = tile % tiles_n;
         for (int kb = 0; kb < num_kb; ++kb) {
-          if (RESIDENT && first_tile) {   // resident W k-block: its own buffer, loaded once, no slot to wait for
-            mbar_expect_tx(&w_full[kb], SM::B_BYTES);
-            tma_load_2d(wres + kb * SM::B_BYTES, &map_b, &w_full[kb], kb * GEMM_BLOCK_K, n_blk * BLOCK_N);
-          }
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = tiles + stage * SM::STAGE_BYTES;
           mbar_expect_tx(&full_bar[stage], SM::STAGE_BYTES);
           tma_load_2d(sa, &map_a, &full_bar[stage], kb * GEMM_BLOCK_K, m_blk * GEMM_BLOCK_M);
-          if (!RESIDENT) tma_load_2d(sa + SM::A_BYTES, &map_b, &full_bar[stage], kb * GEMM_BLOCK_K, n_blk * BLOCK_N);
+          tma_load_2d(sa + SM::A_BYTES, &map_b, &full_bar[stage], kb * GEMM_BLOCK_K, n_blk * BLOCK_N);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        first_tile = false;
       }
     }
   } else {
@@ -203,17 +176,15 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     int stage = 0;
     uint32_t phase = 0;
     float acc[NREG];
-    bool first_tile = true;
-    for (int tile = first; tile < num_tiles; tile += step) {
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile / tiles_n, n_blk = tile % tiles_n;
       const int col_base = n_blk * BLOCK_N;
       // ---- main loop: one wgmma group in flight while the next stage is awaited
       int prev_stage = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
-        if (RESIDENT && first_tile) mbar_wait(&w_full[kb], 0);   // W k-block has landed (first tile only)
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(tiles + stage * SM::STAGE_BYTES) + wg * 64 * 128;
-        const uint32_t sb = RESIDENT ? smem_u32(wres + kb * SM::B_BYTES) : smem_u32(tiles + stage * SM::STAGE_BYTES) + SM::A_BYTES;
+        const uint32_t sb = smem_u32(tiles + stage * SM::STAGE_BYTES) + SM::A_BYTES;
         const uint64_t da = wgmma_desc_k_sw128(sa);
         const uint64_t db = wgmma_desc_k_sw128(sb);
         wgmma_fence_acc(acc);
@@ -230,7 +201,6 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-      first_tile = false;
       // ---- epilogue
       const int row0 = m_blk * GEMM_BLOCK_M + 64 * wg + rh;
       const bool live = row0 < M;  // warp-uniform: this warp's 32 rows exist
@@ -238,25 +208,21 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       ctx.col_end = col_base + BLOCK_N;
       if (live) Epi::tile_begin(ctx, ep, row0, col_base);
       uint32_t raw[32];
-      auto run = [&](int c0, int c, int cn) {
+      auto run = [&](int c, int cn) {
         if (live && col_base + c < N) {
-          load_row32<BLOCK_N>(st, rh + lane, c - c0, raw);
+          load_row32<BLOCK_N>(st, rh + lane, c, raw);
           Epi::chunk(ctx, ep, raw, row0, col_base + c, (cn < BLOCK_N && col_base + cn < N) ? col_base + cn : -1);
         }
       };
-      constexpr int SC = gemm_stage_cols<BLOCK_N>();
-#pragma unroll
-      for (int c0 = 0; c0 < BLOCK_N; c0 += SC) {   // staging rounds of up to 128 columns: this warp owns one 64-column block each
-        named_bar_sync(1 + wg, 128);   // the previous round's staging tile has been read by every warp of the warpgroup
-        stage_acc<BLOCK_N>(st, acc, c0, wq, lane);
-        named_bar_sync(1 + wg, 128);
-        const int c = c0 + part * 64;
-        if (c < c0 + SC && c < BLOCK_N) {
-          const bool two = c + 32 < BLOCK_N;                     // (BLOCK_N = 96: the last block is a single chunk)
-          const int cnext = c + 128;
-          run(c0, c, two ? c + 32 : cnext);
-          if (two) run(c0, c + 32, cnext);
-        }
+      named_bar_sync(1 + wg, 128);   // the previous tile's staging tile has been read by every warp of the warpgroup
+      stage_acc<BLOCK_N>(st, acc, wq, lane);
+      named_bar_sync(1 + wg, 128);
+      const int c = part * 64;   // this warp owns one 64-column block of the tile
+      if (c < BLOCK_N) {
+        const bool two = c + 32 < BLOCK_N;                     // (BLOCK_N = 96: the last block is a single chunk)
+        const int cnext = c + 128;
+        run(c, two ? c + 32 : cnext);
+        if (two) run(c + 32, cnext);
       }
       if (live) Epi::tile_end(ctx, ep, row0, col_base);
     }

@@ -146,11 +146,12 @@ class Engine:
     # ------------------------------------------------------------------ conditioning
     def set_cond(self, batch, nframes, y, guided, device):
         """Canonicalise model_kwargs['y'] (data_loaders/tensors.py:22-64 schema).  `guided` => CFG pair."""
+        y = y or {}
         if self.dec:
             self._set_cond_dec(batch, nframes, y, guided, device)
         else:
             self._set_cond_enc(batch, nframes, y, guided, device)
-        self._set_target(batch, y if y is not None else {}, device)
+        self._set_target(batch, y, device)
 
     def _set_target(self, batch, y, device):
         """y['target_cond'] [B, n_ext, 3], y['target_joint_names'] (per sample, a list or array of joint names),
@@ -185,36 +186,15 @@ class Engine:
         return out
 
     def _set_cond_enc(self, batch, nframes, y, guided, device):
-        text_embed = y.get("text_embed") if y is not None else None
+        text_embed = y.get("text_embed")
         if isinstance(text_embed, tuple):
             raise NotImplementedError("BERT (tokens, mask) conditioning belongs to the trans_dec path")
-        lengths = y.get("lengths") if y is not None else None
-        mask = y.get("mask") if y is not None else None
-        if mask is not None and mask.shape[-1] <= 1:      # model/mdm.py:242 "is_valid_mask"
-            lengths = None
-        elif lengths is None and mask is not None:        # prefix mask -> lengths (tensors.py:3-6)
-            lengths = mask.reshape(mask.shape[0], -1).sum(-1)
-        scale = y.get("scale") if (guided and y is not None) else None
-        if guided and scale is None:
-            raise AssertionError("ClassifierFreeSampleModel needs y['scale'] (sampler_util.py:34)")
-        uncond = bool(y.get("uncond", False)) if y is not None else False
-        action = y.get("action") if y is not None else None
+        ln, sc = self._lengths_and_scale(batch, y, guided, device)
+        uncond = bool(y.get("uncond", False))
+        action = y.get("action")
         te = None
         if text_embed is not None and self.cond_mode == _lib.COND_TEXT:
-            te = text_embed.detach().to(device=device, dtype=torch.float32)
-            te = te.reshape(-1, te.shape[-1])
-            if te.shape[0] == 1 and batch > 1:             # single prompt for the whole batch (sample/predict.py)
-                te = te.expand(batch, -1)
-            te = te.contiguous()
-            assert te.shape == (batch, self.cfg.cond_dim), (te.shape, batch, self.cfg.cond_dim)
-        ln = None
-        if lengths is not None:
-            ln = np.ascontiguousarray(lengths.detach().reshape(-1).cpu().numpy().astype(np.int64))
-            assert ln.shape[0] == batch
-        sc = None
-        if scale is not None:
-            sc = scale.detach().to(device=device, dtype=torch.float32).reshape(-1).contiguous()
-            assert sc.shape[0] == batch
+            te = self._text_rows(text_embed, batch, device)
         ac = None
         if action is not None and self.cond_mode == _lib.COND_ACTION:
             ac = np.ascontiguousarray(action.detach().reshape(batch, -1)[:, 0].cpu().numpy().astype(np.int64))
@@ -224,6 +204,17 @@ class Engine:
                                         _stream()))
         self._keep["cond"] = (te, sc)
         self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 2 if sc is not None else 1, 1
+
+    def _text_rows(self, te, batch, device):
+        """y['text_embed'] [1, B, cond_dim] (or [1, 1, cond_dim]: one prompt for the whole batch, sample/predict.py) as
+        contiguous fp32 rows [batch, cond_dim] on `device`."""
+        te = te.detach().to(device=device, dtype=torch.float32)
+        te = te.reshape(-1, te.shape[-1])
+        if te.shape[0] == 1 and batch > 1:
+            te = te.expand(batch, -1)
+        te = te.contiguous()
+        assert te.shape == (batch, self.cfg.cond_dim), (te.shape, batch, self.cfg.cond_dim)
+        return te
 
     @staticmethod
     def _lengths_and_scale(batch, y, guided, device):
@@ -259,12 +250,7 @@ class Engine:
         if te is None:
             raise RuntimeError("the CLIP decoder needs y['text_embed'] [1, B, %d] (or y['text'] with a text encoder "
                                "attached)" % self.cfg.cond_dim)
-        te = te.detach().to(device=device, dtype=torch.float32)
-        te = te.reshape(-1, te.shape[-1])
-        if te.shape[0] == 1 and batch > 1:                     # single prompt for the whole batch (sample/predict.py)
-            te = te.expand(batch, -1)
-        te = te.contiguous()
-        assert te.shape == (batch, self.cfg.cond_dim), (te.shape, batch, self.cfg.cond_dim)
+        te = self._text_rows(te, batch, device)
         ln, sc = self._lengths_and_scale(batch, y, guided, device)
         no_pad = np.zeros((batch, 1), dtype=np.uint8)           # the reference passes no memory mask
         check(self.lib.b200mdm_set_cond_dec(self.h, batch, nframes, _ptr(te), no_pad.ctypes.data_as(ctypes.c_void_p), 1,

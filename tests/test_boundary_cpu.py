@@ -136,6 +136,10 @@ def test_c_abi_error_contract_without_gpu():
     assert lib.b200mdm_recover_from_ric(None, 0, 0, 0, None, None, buf, 0, 0, 0, 1, 1, 22, None) < 0
     assert lib.b200mdm_recover_from_ric(buf, 1, 1, 1, buf, None, buf, 1, 1, 1, 1, 1, 22, None) < 0 and b"mean and std" in lib.b200mdm_last_error()
     assert lib.b200mdm_recover_from_ric(buf, 1, 1, 1, None, None, buf, 1, 1, 1, 1, 100000, 22, None) < 0 and b"frames" in lib.b200mdm_last_error()
+    # kernel-test hook of the projection GEMM: block_n is 128 (128 x 128 tiles) or the call is refused
+    for bn in (512, 513, 64, 0):
+        assert lib.b200mdm_test_gemm_f16(buf, buf, buf, buf, 128, 128, 64, 0, bn, None) == _lib.EINVAL
+        assert b"block_n must be 128" in lib.b200mdm_last_error()
     for fn in (lib.b200mdm_set_cond_dec, lib.b200mdm_set_prefix):
         assert fn.argtypes is not None
     assert lib.b200mdm_set_prefix(None, None, None) < 0

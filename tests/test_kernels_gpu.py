@@ -45,24 +45,23 @@ def run_gemm_f16(a, w, bias, act, bn):
     (394, 288, 1536, 128, 0),        # N tail inside a 128-wide tile, 64-column slab clipped by the TMA store
     (394, 264, 1536, 128, 0),        # N tail that ends inside a 32-column chunk
     (5, 16, 8, 128, 1),              # tiny
-    (256, 256, 64, 512, 0),          # 128 x 256 tiles: two row tiles, one k-block
-    (700, 512, 512, 512, 0),         # 256-wide: M tail inside the second warpgroup's rows (700 = 5*128 + 60), pipeline wraps
-    (25216 // 8, 1536, 512, 512, 0), # 256-wide: QKV shape
-    (3000, 1024, 512, 512, 1),       # 256-wide: FFN up + GELU, two staging rounds per tile
-    (130, 512, 1024, 512, 0),        # 256-wide: last row tile holds 2 live rows only
-    (100, 264, 512, 512, 0),         # 256-wide: second warpgroup entirely out of range, N tail in the second tile
-    (256, 256, 64, 513, 0),          # W-resident kernel (128 x 64 tiles): one resident k-block
-    (700, 512, 512, 513, 0),         # W-resident: M tail, one row tile per CTA
-    (25216 // 8, 1536, 512, 513, 0), # W-resident: QKV shape, 24 column blocks
-    (25216, 1024, 512, 513, 1),      # W-resident: the FFN up-projection at BASELINE config 2 (the A ring wraps for many
-                                     # rounds while W stays put) + GELU
-    (40000, 512, 320, 513, 0),       # W-resident: 5 k-blocks, many rounds
-    (5000, 768, 200, 513, 1),        # W-resident: K tail inside the last k-block (200 = 3*64 + 8)
-    (100, 264, 512, 513, 0),         # W-resident: second warpgroup entirely out of range, N tail
+    (256, 256, 64, 128, 0),          # two row tiles, one k-block
+    (256, 256, 64, 128, 1),
+    (700, 512, 512, 128, 0),         # M tail of 60 rows in the last row tile (700 = 5*128 + 60), pipeline wraps
+    (700, 512, 512, 128, 1),
+    (25216 // 8, 1536, 512, 128, 1), # QKV shape through the GELU epilogue
+    (3000, 1024, 512, 128, 1),       # FFN up + GELU, M tail of 56 rows
+    (130, 512, 1024, 128, 0),        # last row tile holds 2 live rows only
+    (130, 512, 1024, 128, 1),
+    (100, 264, 512, 128, 0),         # one partial row tile, N tail of 8 columns in the third column tile
+    (100, 264, 512, 128, 1),
+    (25216, 1024, 512, 128, 1),      # the FFN up-projection at BASELINE config 2 + GELU
+    (40000, 512, 320, 128, 0),       # 5 k-blocks, ten tiles per CTA
+    (5000, 768, 200, 128, 1),        # K tail inside the last k-block (200 = 3*64 + 8)
 ])
 def test_gemm_tcgen05(M, N, K, bn, act):
-    """EpiBiasF16<act> behind the 128 x 128, 128 x 256 and W-resident GEMMs, on grid operands (the fp32 accumulation is
-    exact).  act = 0: fp16(fp32(acc + bias)) bit for bit.  act = 1: fp16(gelu_erf(fp32(acc + bias))) against fp64
+    """EpiBiasF16<act> behind the 128 x 128 projection GEMM (block_n = 128, the only tile shape), on grid operands (the
+    fp32 accumulation is exact).  act = 0: fp16(fp32(acc + bias)) bit for bit.  act = 1: fp16(gelu_erf(fp32(acc + bias))) against fp64
     gelu(acc + bias) within half an fp16 ulp + gelu_erf's bound + the fp32 bias add (|gelu'| <= 1.13)."""
     g = torch.Generator(device="cuda").manual_seed(M * 7 + N * 3 + K)
     a, w = grid_operands(M, N, K, g)
