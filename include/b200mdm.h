@@ -44,7 +44,7 @@ extern "C" {
 #define B200MDM_MODE_DDPM 1 /* p_sample */
 #define B200MDM_MODE_DDIM 2 /* ddim_sample */
 /* (3-5: the PLMS steps inside b200mdm_plms_loop_range / b200mdm_plms_step, 7: the DPM-Solver++ step inside
- * b200mdm_dpm_loop_range; not valid modes of the calls below) */
+ * b200mdm_dpm_loop_range, 8: the bound step inside b200mdm_vb_loop_range; not valid modes of the calls below) */
 #define B200MDM_MODE_DDIM_REVERSE 6 /* ddim_reverse_sample: b200mdm_sample_step only (noise_dev may be NULL) */
 
 #define B200MDM_FLAG_CONST_NOISE 1   /* p_sample(const_noise=True): eps row 0 repeated (gaussian_diffusion.py:527-528) */
@@ -139,6 +139,17 @@ int b200mdm_set_schedule_next(b200mdm_engine* e, int32_t n_steps, const float* r
  * b200mdm_set_schedule_next.  Synchronous copy. */
 #define B200MDM_SCHED_DPM_STRIDE 4
 int b200mdm_set_schedule_dpm(b200mdm_engine* e, int32_t n_steps, const float* rows_host);
+
+/* The variational-bound table (calc_bpd_loop), n_steps rows of fp32 values as the reference's fp32 tensors hold them:
+ *   [0] posterior_mean_coef1  [1] posterior_mean_coef2  [2] posterior_log_variance_clipped  [3] the model's fixed
+ *   log-variance (FIXED_SMALL: = [2]; FIXED_LARGE: log(append(posterior_variance[1], betas[1:])))
+ *   [4] sqrt_recip_alphas_cumprod  [5] sqrt_recipm1_alphas_cumprod  [6] sqrt_alphas_cumprod
+ *   [7] sqrt_one_minus_alphas_cumprod  [8] ((-1 + [3]) - [2]) + exp([2] - [3])  [9] exp(-[3])  [10] exp(-(0.5 * [3]))
+ *   [11] (-1 - log(1 - ac)) + exp(log(1 - ac))
+ * ([8]-[11] in fp32 arithmetic from the fp32 entries; DESIGN.md section 1).  Staleness as for b200mdm_set_schedule_next.
+ * Synchronous copy. */
+#define B200MDM_SCHED_VB_STRIDE 12
+int b200mdm_set_schedule_vb(b200mdm_engine* e, int32_t n_steps, const float* rows_host);
 
 /* Canonicalises model_kwargs['y'] (data_loaders/tensors.py:22-64 + callers) once per loop and (re)builds the
  * workspace for (batch, nframes):
@@ -273,6 +284,23 @@ int b200mdm_dpm_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index
 /* out_dev [B, JF, T] fp32 <- the x0 (pred_xstart) of the last step of that loop.  Enqueued on `stream`. */
 int b200mdm_dpm_pred_xstart(b200mdm_engine* e, float* out_dev, void* stream);
 
+/* The variational lower bound (calc_bpd_loop, gaussian_diffusion.py:1544-1599) at schedule indices first_index,
+ * first_index-1, ... (n_run of them), each step one forward (one CUDA graph, replayed, when use_graph != 0):
+ *   x_t = sqrt_ac*x_start + sqrt_1mac*eps (eps: step k of noise_tape_dev, or the engine's Philox stream with
+ *   B200MDM_FLAG_PHILOX_NOISE, as in b200mdm_sample_loop_range); x0 as p_mean_variance forms it (CFG, inpainting, clamp
+ *   under B200MDM_FLAG_CLIP_DENOISED); the KL term (the decoder NLL at index 0) in bits, (x0 - x_start)^2 and
+ *   (eps(x_t, x0) - eps)^2, each averaged over the sample (padded frames included) with per-chunk partial sums in fixed
+ *   slots and a fixed-order final sum: two runs on the same inputs give the same bits.
+ * x_start_dev != NULL starts a fresh loop (x_start [B, JF, T] is copied in and never overwritten; every column is
+ * cleared); NULL continues the bound loop left in the engine (b200mdm_set_cond* ends it).  terms_dev (nullable)
+ * [3, B, n_steps] fp32 receives vb, xstart_mse, mse with column c = schedule index n_steps - 1 - c (columns no call of
+ * this loop has reached hold 0).  bpd_dev (nullable) [2, B] receives total_bpd = the sum of the vb row (columns in order)
+ * + prior_bpd, and prior_bpd, when this call ends at schedule index 0.  Stale bound table -> B200MDM_ESTATE.  The
+ * buffers (about 2 x [B, JF, T] fp32) are allocated in the workspace on first use. */
+int b200mdm_vb_loop_range(b200mdm_engine* e, int32_t first_index, int32_t n_run, const float* x_start_dev,
+                          const float* noise_tape_dev, int64_t noise_step_stride, int32_t flags, float* terms_dev,
+                          float* bpd_dev, int32_t use_graph, void* stream);
+
 /* The engine's own noise stream (no reference counterpart: the reference draws from torch's global generator).
  * Philox4x32-10 keyed by `seed`, counter = (element/4, schedule index of the consuming step, global sample index);
  * Box-Muller on the 4 output words (exact recipe: csrc/kernels.cuh, restated in oracle/philox_oracle.py).  A sample's
@@ -345,6 +373,17 @@ int b200mdm_test_out_dpm(const void* hres16_dev, const float* scale_dev, const f
                          int32_t flags, const uint8_t* inpaint_mask_dev, const float* inpaint_motion_dev,
                          float* x0_hist_dev, float* x_out_dev, int32_t B, int32_t JF, int32_t T, int32_t d, int32_t s_off,
                          int32_t halves, void* stream);
+/* The same output launches with the EpiOut<OutVb> epilogue of b200mdm_vb_loop_range and its per-sample reduction, as
+ * the bound step at schedule index `index` of an n_steps schedule: vb_row (12 floats, device; see b200mdm_set_schedule_vb)
+ * is row `index` of the table; x_t, x_start, noise [B, JF, T].  pred_xstart (nullable) receives x0, elem (nullable)
+ * [3, B, JF, T] the per-element terms before averaging, terms [3, B, n_steps] column n_steps - 1 - index the per-sample
+ * means (the other columns are left as they are).  flags: B200MDM_FLAG_CLIP_DENOISED or 0; other arguments as in
+ * b200mdm_test_out_step.  Invalid arguments return B200MDM_EINVAL before any CUDA call. */
+int b200mdm_test_out_vb(const void* hres16_dev, const float* scale_dev, const float* w_out_dev, const float* b_out_dev,
+                        const float* x_t_dev, const float* x_start_dev, const float* noise_dev, const float* vb_row_dev,
+                        int32_t index, int32_t n_steps, int32_t flags, const uint8_t* inpaint_mask_dev,
+                        const float* inpaint_motion_dev, float* pred_xstart_dev, float* elem_dev, float* terms_dev, int32_t B,
+                        int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream);
 /* Self-attention core (tensor-core kernel, S <= 256): softmax(q k^T / sqrt(128) + mask) v per (sample, head);
  * qkv16 [n*S, 3d]; kvlen int32 [n] device (valid keys per sample, a prefix).
  * impl 0: out16 fp16 [n*S, d] (the encoder); impl 1: out16 fp16 [n*S, 2d] = [hi | lo] with hi + lo = the fp32 result

@@ -18,6 +18,7 @@ FLAG_CONST_NOISE, FLAG_CLIP_DENOISED, FLAG_PHILOX_NOISE = 1, 2, 4
 SCHED_STRIDE = 8
 SCHED_NEXT_STRIDE = 2
 SCHED_DPM_STRIDE = 4
+SCHED_VB_STRIDE = 12
 
 # every symbol include/b200mdm.h declares (tests check that the library exports all of them)
 SYMBOLS = [
@@ -32,6 +33,7 @@ SYMBOLS = [
     "b200mdm_set_schedule_next", "b200mdm_ddim_reverse_loop_range", "b200mdm_test_cross_rows",
     "b200mdm_test_row_bias_ln", "b200mdm_test_forward_taps",
     "b200mdm_set_schedule_dpm", "b200mdm_dpm_loop_range", "b200mdm_dpm_pred_xstart", "b200mdm_test_out_dpm",
+    "b200mdm_set_schedule_vb", "b200mdm_vb_loop_range", "b200mdm_test_out_vb",
 ]
 # tap points of b200mdm_test_forward_taps (B200MDM_TAP_*)
 TAPS = ["EMBED", "TOK0", "CONDPROJ", "TEMB", "MEM16", "CROSS_C", "KVC16", "L_IN", "L_QKV", "L_ATT", "L_LN1", "L_QC",
@@ -112,7 +114,11 @@ def load():
                        ("b200mdm_dpm_loop_range", [vp, i32, i32, i32, vp, vp, i32, i32, vp]),
                        ("b200mdm_dpm_pred_xstart", [vp, vp, vp]),
                        ("b200mdm_test_out_dpm", [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp,
-                                                 i32, i32, i32, i32, i32, i32, vp])):
+                                                 i32, i32, i32, i32, i32, i32, vp]),
+                       ("b200mdm_set_schedule_vb", [vp, i32, vp]),
+                       ("b200mdm_vb_loop_range", [vp, i32, i32, vp, vp, i64, i32, vp, vp, i32, vp]),
+                       ("b200mdm_test_out_vb", [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp,
+                                                i32, i32, i32, i32, i32, i32, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

@@ -176,6 +176,12 @@ struct Workspace {
   // flight (-1: none to continue).
   float* dpm_hist = nullptr;
   int dpm_done = -1, dpm_order = 0;
+  // variational-bound loop, allocated on first use: x_start [B, JF, T] (the loop state, never overwritten), the
+  // per-(row, 32-column chunk) sums of the output epilogue [VB_TERMS, B*T, vb_chunks] and the per-step means
+  // [VB_TERMS, B, vb_cap] (column n_steps - 1 - i for schedule index i).  vb_live: a bound loop that may be continued.
+  float *vb_xs = nullptr, *vb_part = nullptr, *vb_terms = nullptr;
+  int vb_cap = 0;
+  bool vb_live = false;
   // captured step graph of this workspace
   cudaGraphExec_t graph_exec = nullptr;
   GraphKey graph_key;
@@ -216,6 +222,9 @@ struct b200mdm_engine : Workspace {
   // way as sched_next
   float* sched_dpm = nullptr;
   bool sched_dpm_fresh = false;
+  // variational bound: the VB_* columns per row (b200mdm_set_schedule_vb), allocated with `sched`, stale in the same way
+  float* sched_vb = nullptr;
+  bool sched_vb_fresh = false;
   // parked workspaces (see Workspace)
   std::vector<Workspace> pool;
   unsigned long long use_clock = 0;
@@ -293,6 +302,7 @@ static int init_kernel_attrs() {
   TRY((set_gemm_attr<96, EpiOut<OutPlms>>()));
   TRY((set_gemm_attr<96, EpiOut<OutReverse>>()));
   TRY((set_gemm_attr<96, EpiOut<OutDpm>>()));
+  TRY((set_gemm_attr<96, EpiOut<OutVb>>()));
   TRY((set_attention_attr<64>()));
   TRY((set_attention_attr<208>()));
   TRY((set_attention_attr<256>()));
@@ -453,6 +463,20 @@ static int launch_embed_gemm(const CUtensorMap& m_xin, const CUtensorMap& m_win,
   p.S = S; p.d = d; p.halves = halves;
   return launch_gemm<128, EpiEmbed>(m_xin, m_win, m_xin, MB, d, 3 * Kp, p, s, num_sms);
 }
+// the bound step's x_t into x_t [B, n] from x_start and the step's eps (noise, or the tape of the step state)
+static int launch_vb_xt(float* x_t, const float* x_start, const float* noise, const float* sched_vb, const StepState* state,
+                        size_t n, cudaStream_t s) {
+  const int blocks = static_cast<int>(n / 256 + 1 < 1184 ? n / 256 + 1 : 1184);
+  CUDA_TRY(launch_k(vb_xt_kernel, dim3(blocks), dim3(256), 0, s, x_t, x_start, noise, sched_vb, state, n));
+  return B200MDM_OK;
+}
+// the bound step's per-sample means of its three terms from the epilogue's partial sums -> column n_steps - 1 - cur of terms
+static int launch_vb_reduce(float* terms, int ld_terms, const float* part, int B, int T, int JF, const StepState* state,
+                            cudaStream_t s) {
+  CUDA_TRY(launch_k(vb_reduce_kernel, dim3(B, VB_TERMS), dim3(VB_REDUCE_THREADS), 0, s, terms, ld_terms, part, B,
+                    T * ((JF + 31) / 32), static_cast<float>(JF) * static_cast<float>(T), state));
+  return B200MDM_OK;
+}
 // g16 [B*T, 3d] = [hi | hi | lo] of the CFG blend of the frame rows of hres
 static int launch_blend_split(const __half* hres, __half* g16, const float* scale, int B, int S, int T, int s_off, int d,
                               int halves, cudaStream_t s) {
@@ -560,6 +584,7 @@ static void free_workspace(Workspace* w) {
   dfree(w->tgt_valid); dfree(w->tgt_g);
   dfree(w->plms_ring); dfree(w->plms_mid); dfree(w->plms_pred);
   dfree(w->dpm_hist);
+  dfree(w->vb_xs); dfree(w->vb_part); dfree(w->vb_terms);
   *w = Workspace();
 }
 // every workspace (the one in use and the parked ones): after a weight reload or a schedule-table move their graphs
@@ -588,6 +613,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   for (auto& kv : e->store) cudaFree(kv.second.dev);
   free_repacks(e);
   dfree(e->sched); dfree(e->tmap); dfree(e->sched_next); dfree(e->sched_dpm);
+  dfree(e->sched_vb);
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
   if (e->work) cudaStreamDestroy(e->work);
@@ -900,17 +926,20 @@ extern "C" int b200mdm_set_schedule(b200mdm_engine* e, int32_t n_steps, const fl
     dfree(e->tmap);
     dfree(e->sched_next);
     dfree(e->sched_dpm);
+    dfree(e->sched_vb);
     e->sched_cap = 0;
     const int cap = n_steps > 1000 ? n_steps : 1000;
     TRY(dalloc(&e->sched, static_cast<size_t>(cap) * SCHED_STRIDE));
     TRY(dalloc(&e->tmap, cap));
     TRY(dalloc(&e->sched_next, static_cast<size_t>(cap) * SCHED_NEXT_STRIDE));
     TRY(dalloc(&e->sched_dpm, static_cast<size_t>(cap) * SCHED_DPM_STRIDE));
+    TRY(dalloc(&e->sched_vb, static_cast<size_t>(cap) * SCHED_VB_STRIDE));
     e->sched_cap = cap;
   }
   e->n_steps = n_steps;
   e->sched_next_fresh = false;
   e->sched_dpm_fresh = false;
+  e->sched_vb_fresh = false;
   CUDA_TRY(cudaMemcpy(e->sched, rows_host, static_cast<size_t>(n_steps) * SCHED_STRIDE * sizeof(float), cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(e->tmap, timestep_map_host, static_cast<size_t>(n_steps) * sizeof(int), cudaMemcpyHostToDevice));
   return B200MDM_OK;
@@ -942,6 +971,19 @@ extern "C" int b200mdm_set_schedule_dpm(b200mdm_engine* e, int32_t n_steps, cons
   CUDA_TRY(cudaMemcpy(e->sched_dpm, rows_host, static_cast<size_t>(n_steps) * SCHED_DPM_STRIDE * sizeof(float),
                       cudaMemcpyHostToDevice));
   e->sched_dpm_fresh = true;
+  return B200MDM_OK;
+}
+
+static_assert(SCHED_VB_STRIDE == B200MDM_SCHED_VB_STRIDE, "the bound table's row layout is part of the ABI");
+extern "C" int b200mdm_set_schedule_vb(b200mdm_engine* e, int32_t n_steps, const float* rows_host) {
+  if (!e || !rows_host) return fail(B200MDM_EINVAL, "bad argument");
+  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
+  if (n_steps != e->n_steps)
+    return fail(B200MDM_EINVAL, "n_steps %d differs from the schedule's %d", n_steps, e->n_steps);
+  CUDA_TRY(cudaDeviceSynchronize());  // a bound loop still in flight may be reading the old rows
+  CUDA_TRY(cudaMemcpy(e->sched_vb, rows_host, static_cast<size_t>(n_steps) * SCHED_VB_STRIDE * sizeof(float),
+                      cudaMemcpyHostToDevice));
+  e->sched_vb_fresh = true;
   return B200MDM_OK;
 }
 
@@ -1120,6 +1162,7 @@ static void end_cond(b200mdm_engine* e) {
   e->target_set = false;
   e->inpaint_mask = nullptr;
   e->inpaint_motion = nullptr;
+  e->vb_live = false;
 }
 
 extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* cond_embed_dev,
@@ -1309,6 +1352,7 @@ static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, 
   p.x_step = a.x_step;
   p.noise_batch_stride = a.const_noise ? 0 : static_cast<long long>(JF) * T;
   p.B = B; p.T = T; p.J = JF; p.mode = a.mode;
+  p.vb_chunks = (JF + 31) / 32;
   p.clip_denoised = a.clip;
   p.order = a.order;
   p.back = a.back;
@@ -1316,6 +1360,7 @@ static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, 
   if (a.mode <= MODE_DDIM) return launch_gemm<96, EpiOut<OutStep>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
   if (a.mode == MODE_DDIM_REVERSE) return launch_gemm<96, EpiOut<OutReverse>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
   if (a.mode == MODE_DPM) return launch_gemm<96, EpiOut<OutDpm>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
+  if (a.mode == MODE_VB) return launch_gemm<96, EpiOut<OutVb>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
   return launch_gemm<96, EpiOut<OutPlms>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
 }
 
@@ -1395,6 +1440,10 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
   PdlScope pdl_scope;
   if (a.philox) {
     TRY(launch_philox(e->eps_buf, B, static_cast<long long>(JF) * T, 0ull, 0ll, 0u, e->state, s));
+    ++nk;
+  }
+  if (a.mode == MODE_VB) {   // x_t = q_sample(x_start, i, eps): the denoiser's input
+    TRY(launch_vb_xt(e->x_work, e->vb_xs, a.noise, e->sched_vb, e->state, static_cast<size_t>(B) * JF * T, s));
     ++nk;
   }
   TRY(launch_pack_input(a.x_in, e->xin16, B, JF, T, S, Kp, e->s_off, s));
@@ -1485,8 +1534,15 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     p.sched_dpm = e->sched_dpm;
     p.eps_ring = e->plms_ring;
     p.x0_hist = e->dpm_hist;
+    p.sched_vb = e->sched_vb;
+    p.x_start = e->vb_xs;
+    p.vb_part = e->vb_part;
     p.state = e->state;
     TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, a, p, s, e->num_sms));
+    ++nk;
+  }
+  if (a.mode == MODE_VB) {
+    TRY(launch_vb_reduce(e->vb_terms, e->vb_cap, e->vb_part, B, T, JF, e->state, s));
     ++nk;
   }
   *n_kernels = nk;
@@ -1880,6 +1936,76 @@ extern "C" int b200mdm_dpm_pred_xstart(b200mdm_engine* e, float* out_dev, void* 
   return B200MDM_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ variational bound
+static int ensure_vb(b200mdm_engine* e) {
+  const size_t n = static_cast<size_t>(e->B) * e->JF * e->T;
+  if (e->vb_xs && e->vb_part && e->vb_terms && e->vb_cap >= e->n_steps) return B200MDM_OK;
+  if (e->vb_terms && e->vb_cap < e->n_steps) {   // a longer schedule: the step graph holds the old pointer
+    drop_graph(e);
+    dfree(e->vb_terms);
+    e->vb_live = false;
+  }
+  int r = B200MDM_OK;
+  if (!e->vb_xs) r = dalloc(&e->vb_xs, n);
+  if (r == B200MDM_OK && !e->vb_part)
+    r = dalloc(&e->vb_part, static_cast<size_t>(VB_TERMS) * e->B * e->T * ((e->JF + 31) / 32));
+  if (r == B200MDM_OK && !e->vb_terms) {
+    r = dalloc(&e->vb_terms, static_cast<size_t>(VB_TERMS) * e->B * e->sched_cap);
+    e->vb_cap = r == B200MDM_OK ? e->sched_cap : 0;
+  }
+  if (r != B200MDM_OK) {   // all or nothing
+    dfree(e->vb_xs); dfree(e->vb_part); dfree(e->vb_terms);
+    e->vb_cap = 0;
+    e->vb_live = false;
+  }
+  return r;
+}
+
+// The bound loop (calc_bpd_loop) at schedule indices first_index, first_index-1, ... (n_run of them): per step
+// vb_xt_kernel, the forward with the EpiOut<OutVb> epilogue and vb_reduce_kernel, one graph.  The step state's `done`
+// indexes this call's noise tape.
+extern "C" int b200mdm_vb_loop_range(b200mdm_engine* e, int32_t first_index, int32_t n_run, const float* x_start_dev,
+                                     const float* noise_tape_dev, int64_t noise_step_stride, int32_t flags,
+                                     float* terms_dev, float* bpd_dev, int32_t use_graph, void* stream) {
+  if (flags & ~(B200MDM_FLAG_CLIP_DENOISED | B200MDM_FLAG_PHILOX_NOISE))
+    return fail(B200MDM_EINVAL, "the bound loop takes no flag but B200MDM_FLAG_CLIP_DENOISED and B200MDM_FLAG_PHILOX_NOISE");
+  const bool philox = (flags & B200MDM_FLAG_PHILOX_NOISE) != 0;
+  if (!philox && !noise_tape_dev) return fail(B200MDM_EINVAL, "null noise tape (or pass B200MDM_FLAG_PHILOX_NOISE)");
+  if (n_run <= 0) return fail(B200MDM_EINVAL, "bad step range");
+  TRY(check_ready(e, true));
+  if (first_index >= e->n_steps || first_index - n_run + 1 < 0) return fail(B200MDM_EINVAL, "bad step range");
+  if (!e->sched_vb_fresh)
+    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_vb has not been called for the current schedule");
+  if (!x_start_dev && !e->vb_live) return fail(B200MDM_ESTATE, "no bound loop to continue (pass x_start_dev)");
+  TRY(ensure_vb(e));
+  if (!x_start_dev && !e->vb_live)   // ensure_vb reallocated the tables for a longer schedule: nothing to continue
+    return fail(B200MDM_ESTATE, "the schedule outgrew the bound loop's tables: no bound loop to continue (pass x_start_dev)");
+  cudaStream_t user = static_cast<cudaStream_t>(stream);
+  const size_t n = static_cast<size_t>(e->B) * e->JF * e->T;
+  if (x_start_dev) {   // a fresh loop: x_start in, every column of the tables cleared
+    CUDA_TRY(cudaMemcpyAsync(e->vb_xs, x_start_dev, n * sizeof(float), cudaMemcpyDeviceToDevice, user));
+    CUDA_TRY(cudaMemsetAsync(e->vb_terms, 0, static_cast<size_t>(VB_TERMS) * e->B * e->vb_cap * sizeof(float), user));
+  }
+  e->vb_live = true;
+  StepArgs a;
+  a.mode = MODE_VB;
+  a.x_in = e->x_work;
+  a.noise = philox ? e->eps_buf : nullptr;
+  a.philox = philox;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  TRY(run_loop(e, a, flags, first_index, n_run, nullptr, nullptr, noise_tape_dev, noise_step_stride, use_graph, stream));
+  if (terms_dev)
+    CUDA_TRY(cudaMemcpy2DAsync(terms_dev, e->n_steps * sizeof(float), e->vb_terms, e->vb_cap * sizeof(float),
+                               e->n_steps * sizeof(float), static_cast<size_t>(VB_TERMS) * e->B, cudaMemcpyDeviceToDevice, user));
+  if (bpd_dev && first_index - n_run + 1 == 0) {
+    vb_final_kernel<<<e->B, VB_REDUCE_THREADS, 0, user>>>(bpd_dev, e->vb_terms, e->vb_cap, e->vb_xs, e->sched_vb, e->n_steps,
+                                                           e->B, e->JF * e->T);
+    CUDA_TRY(cudaGetLastError());
+    e->launches += 1;
+  }
+  return B200MDM_OK;
+}
+
 // Counter-based noise stream of the engine (Philox4x32-10 + Box-Muller, kernels.cuh): eps of schedule index i for
 // global sample g depends on (seed, i, g, element) only -- not on the batch split, the GPU count or the chunking.
 extern "C" int b200mdm_set_noise_stream(b200mdm_engine* e, uint64_t seed, int64_t sample_index_base) {
@@ -2105,6 +2231,49 @@ extern "C" int b200mdm_test_out_dpm(const void* hres16_dev, const float* scale_d
   a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
   a.x_out = x_out_dev;
   return launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms);
+}
+
+extern "C" int b200mdm_test_out_vb(const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
+                                   const float* b_out_dev, const float* x_t_dev, const float* x_start_dev, const float* noise_dev,
+                                   const float* vb_row_dev, int32_t index, int32_t n_steps, int32_t flags,
+                                   const uint8_t* inpaint_mask_dev, const float* inpaint_motion_dev, float* pred_xstart_dev,
+                                   float* elem_dev, float* terms_dev, int32_t B, int32_t JF, int32_t T, int32_t d, int32_t s_off,
+                                   int32_t halves, void* stream) {
+  if (!hres16_dev || !w_out_dev || !b_out_dev || !x_t_dev || !x_start_dev || !noise_dev || !vb_row_dev || !terms_dev ||
+      B <= 0 || JF <= 0 || T <= 0 || s_off < 0 || d <= 0 || d % 64 || (halves != 1 && halves != 2) ||
+      (halves == 2 && !scale_dev) || index < 0 || index >= n_steps || (flags & ~B200MDM_FLAG_CLIP_DENOISED) ||
+      (inpaint_mask_dev == nullptr) != (inpaint_motion_dev == nullptr))
+    return fail(B200MDM_EINVAL, "bad argument");
+  TRY(init_kernel_attrs());
+  int sms = 132;
+  TRY(device_sms(&sms));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  StreamScratch scr(s);
+  OutHook o;
+  TRY(out_hook_setup(scr, &o, hres16_dev, scale_dev, w_out_dev, b_out_dev, inpaint_mask_dev, inpaint_motion_dev, B, JF, T, d,
+                     s_off, halves));
+  float *table = nullptr, *part = nullptr;
+  StepState* st = nullptr;
+  TRY(scr.alloc(&table, static_cast<size_t>(index + 1) * SCHED_VB_STRIDE, true));   // the row at `index`, zeros above
+  TRY(scr.alloc(&part, static_cast<size_t>(VB_TERMS) * B * T * ((JF + 31) / 32)));
+  TRY(scr.alloc(&st, 1, true));
+  CUDA_TRY(cudaMemcpyAsync(table + static_cast<size_t>(index) * SCHED_VB_STRIDE, vb_row_dev, SCHED_VB_STRIDE * sizeof(float),
+                           cudaMemcpyDeviceToDevice, s));
+  step_set_kernel<<<1, 1, 0, s>>>(st, 0, index, nullptr, 0, 0, 0, n_steps);
+  CUDA_TRY(cudaGetLastError());
+  o.p.sched_vb = table;
+  o.p.x_start = x_start_dev;
+  o.p.vb_part = part;
+  o.p.vb_elem = elem_dev;
+  o.p.state = st;
+  StepArgs a;
+  a.mode = MODE_VB;
+  a.x_in = x_t_dev;
+  a.noise = noise_dev;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  a.pred = pred_xstart_dev;
+  TRY(launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms));
+  return launch_vb_reduce(terms_dev, n_steps, part, B, T, JF, st, s);
 }
 
 extern "C" int b200mdm_test_attention(const void* qkv16_dev, void* out16_dev, const int32_t* kvlen_dev,

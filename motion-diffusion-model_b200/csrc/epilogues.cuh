@@ -236,11 +236,30 @@ struct EpiEmbed {
 // slot k % 2 of an x0 history, row i of the DPM table holds (c_x, c0, c_cur, c_prev)
 //   mode 7: cur_order = (k == 0 || i == 0) ? 1 : order;  history[k % 2] = x0;
 //           order 1: x_out = fmaf(c0, x0, c_x*x);  order 2: x_out = fmaf(c_prev, history[(k-1) % 2], fmaf(c_cur, x0, c_x*x))
+// Variational bound (calc_bpd_loop / _vb_terms_bpd, gaussian_diffusion.py:1189-1222, 1544-1599; diffusion/losses.py):
+// x_t = q_sample(x_start, i, eps) was formed by vb_xt_kernel at the head of the step; row i of the bound table (VB_*)
+//   mode 8: mean = c1*x0 + c2*x_t;  i > 0: true_mean = c1*x_start + c2*x_t, term = normal_kl(true_mean, lv_true, mean,
+//           lv_model);  i == 0: term = -discretized_gaussian_log_likelihood(x_start, mean, 0.5*lv_model);
+//           xm = (x0 - x_start)^2;  em = ((sr*x_t - x0)/srm1 - eps)^2.  The three are summed per (row, 32-column chunk)
+//           in column order into fixed slots of a partial-sum buffer (vb_reduce_kernel finishes the per-sample means)
 // Per-step scalars come from a device table indexed by the device-side step state, so the very same launch
 // (and CUDA graph) serves every step of the loop.
 constexpr int SCHED_STRIDE = 8;       // floats per schedule row: c1 c2 sig_ddpm sr srm1 sqrt_abp coef_eps sig_ddim
 constexpr int SCHED_NEXT_STRIDE = 2;  // floats per row of the reverse table: sqrt(abn) sqrt(1 - abn)
 constexpr int SCHED_DPM_STRIDE = 4;   // floats per row of the DPM-Solver++ table: c_x c0 c_cur c_prev
+// floats per row of the bound table (b200mdm_set_schedule_vb), every entry fp32 as the reference's tensors hold it:
+constexpr int SCHED_VB_STRIDE = 12;
+enum VbCol : int {
+  VB_C1 = 0, VB_C2 = 1,          // posterior_mean_coef1 / 2
+  VB_LV_TRUE = 2, VB_LV_MODEL = 3,   // posterior_log_variance_clipped; the model's fixed log-variance
+  VB_SR = 4, VB_SRM1 = 5,        // sqrt_recip_alphas_cumprod, sqrt_recipm1_alphas_cumprod
+  VB_SQ = 6, VB_SQM1 = 7,        // sqrt_alphas_cumprod, sqrt_one_minus_alphas_cumprod (q_sample)
+  VB_KL_C = 8,                   // ((-1 + lv_model) - lv_true) + exp(lv_true - lv_model)   (normal_kl's per-row part)
+  VB_EXP_NEG_LV = 9,             // exp(-lv_model)
+  VB_INV_STD = 10,               // exp(-(0.5 * lv_model))   (discretized_gaussian_log_likelihood's inv_stdv)
+  VB_PRIOR_C = 11,               // (-1 - log(1 - ac)) + exp(log(1 - ac))   (the prior term's normal_kl part, _prior_bpd)
+};
+constexpr int VB_TERMS = 3;           // vb, xstart_mse, mse
 constexpr int PLMS_RING = 3;          // eps history slots: AB4 combines this step's eps with the three before it
 constexpr int DPM_SLOTS = 2;          // x0 history slots: 2M combines this step's x0 with the one before it
 enum OutMode : int {
@@ -248,6 +267,7 @@ enum OutMode : int {
   MODE_PLMS_AB = 3, MODE_PLMS_EULER1 = 4, MODE_PLMS_EULER2 = 5,   // internal: the steps of the PLMS loop
   MODE_DDIM_REVERSE = 6,                                          // B200MDM_MODE_DDIM_REVERSE
   MODE_DPM = 7,                                                   // internal: the step of the DPM-Solver++ loop
+  MODE_VB = 8,                                                    // internal: the step of the bound loop
 };
 struct StepState {
   int done;      // steps completed so far (indexes the noise tape; PLMS: the evaluation count k)
@@ -258,6 +278,24 @@ struct StepState {
   unsigned long long seed;       // in-engine Philox noise (philox_normal_kernel): stream seed ...
   long long sample_base;         // ... and the global index of this workspace's sample 0
 };
+
+// The step state as of the last step_set / step_advance.  Every reader goes through L2 (ld.global.cg), never through
+// the SM's L1 / read-only cache: under programmatic dependent launch a kernel is resident on an SM before the
+// step_advance it depends on has written the state, and an L1 line of the previous step's state -- brought in by another
+// kernel still running on that SM, e.g. a reader through a const __restrict__ pointer (LDG.CONSTANT) -- is not
+// invalidated by griddepcontrol.wait.  Such a line once served the previous schedule index to the first kernel of the
+// next step (DESIGN.md section 1, "Step state").
+__device__ __forceinline__ StepState load_step_state(const StepState* s) {
+  StepState st;
+  st.done = __ldcg(&s->done);
+  st.cur = __ldcg(&s->cur);
+  st.n_steps = __ldcg(&s->n_steps);
+  st.noise = reinterpret_cast<const float*>(__ldcg(reinterpret_cast<const unsigned long long*>(&s->noise)));
+  st.noise_step_stride = __ldcg(&s->noise_step_stride);
+  st.seed = __ldcg(&s->seed);
+  st.sample_base = __ldcg(&s->sample_base);
+  return st;
+}
 
 // Schedule index a forward evaluates: the step's own (back = 0) or the one before it (back = 1, PLMS improved Euler).
 // At i = 0, i - 1 = -1 indexes the reference's timestep map and tables from the end (gaussian_diffusion.py:1046).
@@ -280,6 +318,11 @@ struct EpiOutParams {
   float* eps_ring;          // modes 3-5: [PLMS_RING, B, J, T]
   float* x0_hist;           // mode 7: [DPM_SLOTS, B, J, T]
   const float* x_step;      // mode 5: x_t of the step (x_t above is mean1 there)
+  const float* sched_vb;    // mode 8: [n_steps, SCHED_VB_STRIDE]
+  const float* x_start;     // mode 8: [B, J, T]
+  float* vb_part;           // mode 8: [VB_TERMS, B*T, vb_chunks] per-(row, 32-column chunk) sums
+  float* vb_elem;           // mode 8, nullable: [VB_TERMS, B, J, T] the per-element terms (kernel tests)
+  int vb_chunks;            // mode 8: ceil(J / 32)
   const StepState* state;
   long long noise_batch_stride;  // J*T normally, 0 for const_noise
   int B, T, J, mode;
@@ -296,7 +339,7 @@ struct OutStep {   // modes 0-2
   struct In { float x, n; };
   __device__ __forceinline__ OutStep(const EpiOutParams& p, int b) {
     if (p.mode == MODE_X0) return;
-    const StepState st = *p.state;
+    const StepState st = load_step_state(p.state);
     const float* row_s = p.sched + static_cast<size_t>(st.cur) * SCHED_STRIDE;
     c1 = row_s[0]; c2 = row_s[1]; sr = row_s[3]; srm1 = row_s[4]; sq = row_s[5]; ce = row_s[6];
     sg = (p.mode == MODE_DDPM) ? row_s[2] : row_s[7];
@@ -320,6 +363,7 @@ struct OutStep {   // modes 0-2
     }
     p.x_out[idx] = o;
   }
+  __device__ __forceinline__ void end(const EpiOutParams&, int, int) const {}
 };
 
 struct OutPlms {   // modes 3-5
@@ -330,7 +374,7 @@ struct OutPlms {   // modes 3-5
   // mode 3: e1..e3 = eps of evaluations k-1..k-3;  mode 5: e1 = eps0, e2 = x_step, e3 = x0 of the first evaluation
   struct In { float x, e1, e2, e3; };
   __device__ __forceinline__ OutPlms(const EpiOutParams& p, int) {
-    const StepState st = *p.state;
+    const StepState st = load_step_state(p.state);
     const int k = st.done;
     const float* row_s = p.sched + static_cast<size_t>(st.cur) * SCHED_STRIDE;
     const float* row_e = p.sched + static_cast<size_t>(eval_index(st, p.back)) * SCHED_STRIDE;
@@ -391,13 +435,14 @@ struct OutPlms {   // modes 3-5
     const float mean = __fadd_rn(__fmul_rn(pp, sq), __fmul_rn(s1, ep));
     p.x_out[idx] = __fadd_rn(__fmul_rn(mean, nzf), __fmul_rn(x0s, __fsub_rn(1.f, nzf)));
   }
+  __device__ __forceinline__ void end(const EpiOutParams&, int, int) const {}
 };
 
 struct OutReverse {   // mode 6: no noise and no history
   float sr, srm1, sa, sb;
   struct In { float x; };
   __device__ __forceinline__ OutReverse(const EpiOutParams& p, int) {
-    const int i = p.state->cur;
+    const int i = load_step_state(p.state).cur;
     const float* row_s = p.sched + static_cast<size_t>(i) * SCHED_STRIDE;
     const float* row_n = p.sched_next + static_cast<size_t>(i) * SCHED_NEXT_STRIDE;
     sr = row_s[3]; srm1 = row_s[4]; sa = row_n[0]; sb = row_n[1];
@@ -410,6 +455,7 @@ struct OutReverse {   // mode 6: no noise and no history
     const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sr, v.x), x0), srm1);    // :862-865
     p.x_out[idx] = __fadd_rn(__fmul_rn(x0, sa), __fmul_rn(sb, eps));          // :869-872
   }
+  __device__ __forceinline__ void end(const EpiOutParams&, int, int) const {}
 };
 
 struct OutDpm {   // mode 7: no noise; the x0 history replaces PLMS's eps ring
@@ -419,7 +465,7 @@ struct OutDpm {   // mode 7: no noise; the x0 history replaces PLMS's eps ring
   float* own;             // slot of evaluation k
   struct In { float x, h; };
   __device__ __forceinline__ OutDpm(const EpiOutParams& p, int) {
-    const StepState st = *p.state;
+    const StepState st = load_step_state(p.state);
     const int k = st.done, i = st.cur;
     const float* row = p.sched_dpm + static_cast<size_t>(i) * SCHED_DPM_STRIDE;
     cx = row[0]; c0 = row[1]; cc = row[2]; cp = row[3];
@@ -437,10 +483,84 @@ struct OutDpm {   // mode 7: no noise; the x0 history replaces PLMS's eps ring
     const float base = __fmul_rn(cx, v.x);
     p.x_out[idx] = second ? __fmaf_rn(cp, v.h, __fmaf_rn(cc, x0, base)) : __fmaf_rn(c0, x0, base);
   }
+  __device__ __forceinline__ void end(const EpiOutParams&, int, int) const {}
 };
 
-// One GEMM instantiation per update family, so that the PLMS, inversion and DPM-Solver++ epilogues leave the DDPM /
-// DDIM kernel as it is.
+// approx_standard_normal_cdf (diffusion/losses.py:42-47) in fp32 in torch's operation order: pow(x, 3) = (x*x)*x
+__device__ __forceinline__ float vb_approx_cdf(float x) {
+  const float x3 = __fmul_rn(__fmul_rn(x, x), x);
+  const float in = __fmul_rn(0.7978845608028654f, __fadd_rn(x, __fmul_rn(0.044715f, x3)));
+  return __fmul_rn(0.5f, __fadd_rn(1.f, tanhf(in)));
+}
+// -discretized_gaussian_log_likelihood(x, mean, log_scales) for one element (losses.py:50-77); inv_std = exp(-log_scales)
+__device__ __forceinline__ float vb_decoder_nll(float x, float mean, float inv_std) {
+  const float c = __fsub_rn(x, mean);
+  const float cdf_plus = vb_approx_cdf(__fmul_rn(inv_std, __fadd_rn(c, 1.0f / 255.0f)));
+  const float cdf_min = vb_approx_cdf(__fmul_rn(inv_std, __fsub_rn(c, 1.0f / 255.0f)));
+  float lp;
+  if (x < -0.999f) lp = logf(fmaxf(cdf_plus, 1e-12f));
+  else if (x > 0.999f) lp = logf(fmaxf(__fsub_rn(1.f, cdf_min), 1e-12f));
+  else lp = logf(fmaxf(__fsub_rn(cdf_plus, cdf_min), 1e-12f));
+  return -lp;
+}
+
+struct OutVb {   // mode 8: writes no sample; the three terms of each element go into the chunk's sums
+  float c1, c2, sr, srm1, klc, elv, isd;
+  bool t0;
+  const float* nz;
+  mutable float s_vb = 0.f, s_x = 0.f, s_e = 0.f;
+  struct In { float x, xs, n; };
+  __device__ __forceinline__ OutVb(const EpiOutParams& p, int b) {
+    const StepState st = load_step_state(p.state);
+    const float* r = p.sched_vb + static_cast<size_t>(st.cur) * SCHED_VB_STRIDE;
+    c1 = r[VB_C1]; c2 = r[VB_C2]; sr = r[VB_SR]; srm1 = r[VB_SRM1];
+    klc = r[VB_KL_C]; elv = r[VB_EXP_NEG_LV]; isd = r[VB_INV_STD];
+    t0 = st.cur == 0;
+    nz = (p.noise != nullptr ? p.noise : st.noise + static_cast<long long>(st.done) * st.noise_step_stride) +
+         static_cast<long long>(b) * p.noise_batch_stride;
+  }
+  __device__ __forceinline__ In load(const EpiOutParams& p, bool in, size_t idx, int col, int t) const {
+    return {in ? p.x_t[idx] : 0.f, in ? p.x_start[idx] : 0.f, in ? nz[static_cast<size_t>(col) * p.T + t] : 0.f};
+  }
+  __device__ __forceinline__ void store(const EpiOutParams& p, size_t idx, float x0, const In& v) const {
+    if (p.pred_xstart != nullptr) p.pred_xstart[idx] = x0;
+    const float mean = __fadd_rn(__fmul_rn(c1, x0), __fmul_rn(c2, v.x));           // q_posterior of x0 (:254-257)
+    float term;
+    if (t0) {
+      term = vb_decoder_nll(v.xs, mean, isd);
+    } else {   // normal_kl (losses.py:12-39): 0.5 * (((-1 + lv2) - lv1) + exp(lv1 - lv2) + (m1 - m2)^2 * exp(-lv2))
+      const float tm = __fadd_rn(__fmul_rn(c1, v.xs), __fmul_rn(c2, v.x));
+      const float d = __fsub_rn(tm, mean);
+      term = __fmul_rn(0.5f, __fadd_rn(klc, __fmul_rn(__fmul_rn(d, d), elv)));
+    }
+    const float dx = __fsub_rn(x0, v.xs);
+    const float xm = __fmul_rn(dx, dx);
+    const float eps = __fdiv_rn(__fsub_rn(__fmul_rn(sr, v.x), x0), srm1);           // _predict_eps_from_xstart
+    const float de = __fsub_rn(eps, v.n);
+    const float em = __fmul_rn(de, de);
+    s_vb = __fadd_rn(s_vb, term);
+    s_x = __fadd_rn(s_x, xm);
+    s_e = __fadd_rn(s_e, em);
+    if (p.vb_elem != nullptr) {
+      const size_t slot = static_cast<size_t>(p.B) * p.J * p.T;
+      p.vb_elem[idx] = term;
+      p.vb_elem[slot + idx] = xm;
+      p.vb_elem[2 * slot + idx] = em;
+    }
+  }
+  // the chunk's sums into slot (row, col0 / 32) of each term: every slot has exactly one writer
+  __device__ __forceinline__ void end(const EpiOutParams& p, int row, int col0) const {
+    if (col0 >= p.J) return;
+    const size_t rows = static_cast<size_t>(p.B) * p.T * p.vb_chunks;
+    const size_t i = static_cast<size_t>(row) * p.vb_chunks + col0 / 32;
+    p.vb_part[i] = s_vb;
+    p.vb_part[rows + i] = s_x;
+    p.vb_part[2 * rows + i] = s_e;
+  }
+};
+
+// One GEMM instantiation per update family, so that the PLMS, inversion, DPM-Solver++ and bound epilogues leave the
+// DDPM / DDIM kernel as it is.
 template <class Update>
 struct EpiOut {
   static constexpr int SMEM_PER_WARP = 1024;  // unused
@@ -476,6 +596,7 @@ struct EpiOut {
         u.store(p, idx, x0, v[j]);
       }
     }
+    u.end(p, row, col0);
   }
   static __device__ __forceinline__ void tile_end(EpiCtx&, const Params&, int, int) {}
   static __device__ __forceinline__ void finish(EpiCtx&) {}

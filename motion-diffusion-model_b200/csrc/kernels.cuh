@@ -56,7 +56,7 @@ __global__ void tok0_rows_kernel(__half* __restrict__ hres, const float* __restr
   pdl_launch_dependents();
   pdl_wait();
   const int bp = blockIdx.x;
-  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(*state, back)];
+  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(load_step_state(state), back)];
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = static_cast<size_t>(bp) * S;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
@@ -80,8 +80,9 @@ __global__ void pe_bias_kernel(float* __restrict__ out, const float* __restrict_
 __global__ void step_advance_kernel(StepState* state, int dir) {
   pdl_launch_dependents();
   pdl_wait();
-  state->done += 1;
-  state->cur += dir;
+  const StepState st = load_step_state(state);
+  state->done = st.done + 1;
+  state->cur = st.cur + dir;
 }
 __global__ void step_set_kernel(StepState* state, int done, int cur, const float* noise, long long noise_step_stride,
                                 unsigned long long seed, long long sample_base, int n_steps) {
@@ -119,9 +120,10 @@ __global__ void philox_normal_kernel(float* __restrict__ out, int B, long long n
   pdl_launch_dependents();
   pdl_wait();
   if (state != nullptr) {
-    seed = state->seed;
-    sample_base = state->sample_base;
-    step_id = static_cast<uint32_t>(state->cur);
+    const StepState st = load_step_state(state);
+    seed = st.seed;
+    sample_base = st.sample_base;
+    step_id = static_cast<uint32_t>(st.cur);
   }
   const long long qn = (n + 3) / 4, total = qn * B;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
@@ -338,6 +340,87 @@ __global__ void q_sample_kernel(float* __restrict__ out, const float* __restrict
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// The variational-bound loop (b200mdm_vb_loop_range).  Per step: vb_xt_kernel, the forward with the EpiOut<OutVb>
+// epilogue, vb_reduce_kernel; after the last step, vb_final_kernel.
+constexpr int VB_REDUCE_THREADS = 256;
+
+// x_t = sqrt_ac[i] * x_start + sqrt_1mac[i] * eps at the step's schedule index (q_sample, gaussian_diffusion.py:226-244)
+// eps: `noise` (one step, [B, n]) or the tape the step state describes
+__global__ void vb_xt_kernel(float* __restrict__ x_t, const float* __restrict__ x_start, const float* noise,
+                             const float* __restrict__ sched_vb, const StepState* __restrict__ state, size_t n) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const StepState st = load_step_state(state);
+  const float* r = sched_vb + static_cast<size_t>(st.cur) * SCHED_VB_STRIDE;
+  const float a = r[VB_SQ], b = r[VB_SQM1];
+  const float* nz = noise != nullptr ? noise : st.noise + static_cast<long long>(st.done) * st.noise_step_stride;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    x_t[i] = __fadd_rn(__fmul_rn(a, x_start[i]), __fmul_rn(b, nz[i]));
+}
+
+// Deterministic block sum of v[0 .. n): thread k adds v[k], v[k + 256], ... in that order, then a fixed shared-memory
+// tree (stride 128, 64, ..., 1).  The result is in sh[0] after the call; every thread must call it.
+__device__ __forceinline__ float vb_block_sum(float acc, float* sh) {
+  sh[threadIdx.x] = acc;
+  __syncthreads();
+#pragma unroll
+  for (int s = VB_REDUCE_THREADS / 2; s > 0; s >>= 1) {
+    if (static_cast<int>(threadIdx.x) < s) sh[threadIdx.x] = __fadd_rn(sh[threadIdx.x], sh[threadIdx.x + s]);
+    __syncthreads();
+  }
+  return sh[0];
+}
+
+// terms[k, b, n_steps - 1 - cur] = mean over the sample's J*T elements of term k (the sample's T*chunks partial sums, in
+// the order of vb_block_sum), the vb term divided by log(2) (mean_flat(.) / np.log(2.0)).  grid (B, VB_TERMS).
+__global__ void __launch_bounds__(VB_REDUCE_THREADS) vb_reduce_kernel(float* __restrict__ terms, int ld_terms,
+                                                                     const float* __restrict__ part, int B, int per_sample,
+                                                                     float count, const StepState* __restrict__ state) {
+  __shared__ float sh[VB_REDUCE_THREADS];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x, k = blockIdx.y;
+  const float* v = part + (static_cast<size_t>(k) * B + b) * per_sample;
+  float acc = 0.f;
+  for (int i = threadIdx.x; i < per_sample; i += VB_REDUCE_THREADS) acc = __fadd_rn(acc, v[i]);
+  const float sum = vb_block_sum(acc, sh);
+  if (threadIdx.x == 0) {
+    float m = __fdiv_rn(sum, count);
+    if (k == 0) m = __fdiv_rn(m, 0.6931471805599453f);
+    const StepState st = load_step_state(state);
+    terms[(static_cast<size_t>(k) * B + b) * ld_terms + (st.n_steps - 1 - st.cur)] = m;
+  }
+}
+
+// _prior_bpd and total_bpd (gaussian_diffusion.py:1527-1542, 1593): bpd[b] = sum_c vb[b, c] (c = 0 .. n - 1 in order) +
+// prior[b], bpd[B + b] = prior[b] = mean(0.5 * (prior_c + (sqrt_ac * x_start)^2)) / log(2) with row n - 1 of the table.
+// grid B.
+__global__ void __launch_bounds__(VB_REDUCE_THREADS) vb_final_kernel(float* __restrict__ bpd, const float* __restrict__ terms,
+                                                                    int ld_terms, const float* __restrict__ x_start,
+                                                                    const float* __restrict__ sched_vb, int n_steps, int B,
+                                                                    int per_sample) {
+  __shared__ float sh[VB_REDUCE_THREADS];
+  const int b = blockIdx.x;
+  const float* r = sched_vb + static_cast<size_t>(n_steps - 1) * SCHED_VB_STRIDE;
+  const float sq = r[VB_SQ], pc = r[VB_PRIOR_C];
+  const float* xs = x_start + static_cast<size_t>(b) * per_sample;
+  float acc = 0.f;
+  for (int i = threadIdx.x; i < per_sample; i += VB_REDUCE_THREADS) {
+    const float m = __fmul_rn(sq, xs[i]);
+    acc = __fadd_rn(acc, __fmul_rn(0.5f, __fadd_rn(pc, __fmul_rn(m, m))));
+  }
+  const float sum = vb_block_sum(acc, sh);
+  if (threadIdx.x == 0) {
+    const float prior = __fdiv_rn(__fdiv_rn(sum, static_cast<float>(per_sample)), 0.6931471805599453f);
+    const float* vb = terms + static_cast<size_t>(b) * ld_terms;
+    float tot = 0.f;
+    for (int c = 0; c < n_steps; ++c) tot = __fadd_rn(tot, vb[c]);
+    bpd[b] = __fadd_rn(tot, prior);
+    bpd[B + b] = prior;
+  }
+}
+
 }  // namespace b200
 
 // ===================================================================================================================
@@ -354,7 +437,7 @@ __global__ void mem_build_kernel(__half* __restrict__ mem16, const float* __rest
   pdl_launch_dependents();
   pdl_wait();
   const int m = blockIdx.x, bp = blockIdx.y;
-  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(*state, back)];
+  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(load_step_state(state), back)];
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = static_cast<size_t>(bp) * Mt + m;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
@@ -413,7 +496,7 @@ __global__ void cross_rows_kernel(float* __restrict__ c, const float* __restrict
   pdl_launch_dependents();
   pdl_wait();
   const int bp = blockIdx.x, l = blockIdx.y;
-  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(*state, back)];
+  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(load_step_state(state), back)];
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = (static_cast<size_t>(l) * Bp + bp) * d, trow = (static_cast<size_t>(l) * temb_rows + t) * d;
   for (int i = threadIdx.x; i < d / 4; i += blockDim.x) {

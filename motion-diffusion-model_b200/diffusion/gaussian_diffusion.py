@@ -5,9 +5,11 @@ Same constructor keywords, same public attributes (fp64 numpy tables) and the sa
 `ddim_sample`, `plms_sample_loop`, `plms_sample_loop_progressive`, `plms_sample`, `ddim_reverse_sample`, `q_sample`),
 plus the DDIM inversion loops `ddim_reverse_sample_loop` / `ddim_reverse_sample_loop_progressive` and the DPM-Solver++
 loops `dpm_solver_sample_loop` / `dpm_solver_sample_loop_progressive`, but the per-step arithmetic is not here: a loop is ONE call into libb200mdm.so which
-enqueues every step (denoiser + CFG + posterior/noise epilogue) without returning to Python.
+enqueues every step (denoiser + CFG + posterior/noise epilogue) without returning to Python.  The variational bound
+`calc_bpd_loop` is such a loop too; `p_mean_variance`, `q_mean_variance` and `q_posterior_mean_variance` are there for
+callers that build on them.
 
-Training losses / VLB of the reference are out of scope (SURVEY.md section 8) and raise.
+Training losses of the reference are out of scope (SURVEY.md section 8) and raise.
 """
 import enum
 import math
@@ -164,6 +166,29 @@ class GaussianDiffusion:
                 rows[i, 2], rows[i, 3] = c0, 0.0
         return rows.astype(np.float32)
 
+    def schedule_vb_rows(self):
+        """[n, 12] fp32 rows for b200mdm_set_schedule_vb (include/b200mdm.h): the fp32 tables the reference's
+        _vb_terms_bpd / _prior_bpd read (fp64 table -> fp32, :1612), and the per-row parts of normal_kl and of the decoder
+        likelihood formed from them in fp32 in the reference's operation order (diffusion/losses.py:12-77)."""
+        n = self.num_timesteps
+        rows = np.zeros((n, _lib.SCHED_VB_STRIDE), dtype=np.float32)
+        lvt, lvm = _f32(self.posterior_log_variance_clipped), _f32(self._model_log_variance())
+        lq = _f32(self.log_one_minus_alphas_cumprod)
+        one, half = np.float32(1.0), np.float32(0.5)
+        rows[:, 0] = _f32(self.posterior_mean_coef1)
+        rows[:, 1] = _f32(self.posterior_mean_coef2)
+        rows[:, 2] = lvt
+        rows[:, 3] = lvm
+        rows[:, 4] = _f32(self.sqrt_recip_alphas_cumprod)
+        rows[:, 5] = _f32(self.sqrt_recipm1_alphas_cumprod)
+        rows[:, 6] = _f32(self.sqrt_alphas_cumprod)
+        rows[:, 7] = _f32(self.sqrt_one_minus_alphas_cumprod)
+        rows[:, 8] = ((-one + lvm) - lvt) + np.exp(lvt - lvm)
+        rows[:, 9] = np.exp(-lvm)
+        rows[:, 10] = np.exp(-(half * lvm))
+        rows[:, 11] = (-one - lq) + np.exp(lq)
+        return rows
+
     def _timestep_map(self):
         return list(range(self.num_timesteps))
 
@@ -224,9 +249,10 @@ class GaussianDiffusion:
     # NOISE_CHUNK steps at a time on a side stream into three rotating buffers, while the engine runs the previous chunk.
     NOISE_CHUNK = 16
 
-    def _run_generator_loop(self, eng, mode, img, n_run, first, flags, use_graph, noise_fn=None):
+    def _run_generator_loop(self, eng, mode, img, n_run, first, flags, use_graph, noise_fn=None, run_range=None):
         """noise_fn(buf, k0): fill buf[j] with the eps of the (k0+j)-th executed step, j < len(buf) (runs on the side
-        stream); default = one `normal_()` per step from torch's default generator."""
+        stream); default = one `normal_()` per step from torch's default generator.  run_range(first_index, n, x_in,
+        last, buf) replaces the sampling loop's engine call per chunk (x_in None: continue; last: the final chunk)."""
         dev = img.device
         chunk = max(1, min(self.NOISE_CHUNK, n_run))
         nbuf = 3 if n_run > 2 * chunk else (2 if n_run > chunk else 1)
@@ -258,8 +284,11 @@ class GaussianDiffusion:
                 draw(c + 1)                          # overlaps loop chunk c-1 / c on the engine stream
             b, n = c % nbuf, min(chunk, n_run - c * chunk)
             main.wait_event(ready[b])
-            eng.sample_loop_range(mode, first - done, n, img if c == 0 else None, out if c == n_chunks - 1 else None,
-                                  bufs[b], flags, use_graph)
+            if run_range is not None:
+                run_range(first - done, n, img if c == 0 else None, c == n_chunks - 1, bufs[b])
+            else:
+                eng.sample_loop_range(mode, first - done, n, img if c == 0 else None, out if c == n_chunks - 1 else None,
+                                      bufs[b], flags, use_graph)
             free[b] = torch.cuda.Event()
             free[b].record(main)                     # main has been made to wait for the engine stream by the call
             done += n
@@ -599,6 +628,77 @@ class GaussianDiffusion:
             eng._keep["loop"] = (img,)
             x_in = None
             yield {"sample": sample, "pred_xstart": pred}
+
+    # ------------------------------------------------------------------ posterior / variational bound
+    def q_mean_variance(self, x_start, t):
+        """reference gaussian_diffusion.py:209-224: (mean, variance, log_variance) of q(x_t | x_0), table gathers."""
+        mean = _extract_into_tensor(self.sqrt_alphas_cumprod, t, x_start.shape) * x_start
+        variance = _extract_into_tensor(1.0 - self.alphas_cumprod, t, x_start.shape)
+        log_variance = _extract_into_tensor(self.log_one_minus_alphas_cumprod, t, x_start.shape)
+        return mean, variance, log_variance
+
+    def q_posterior_mean_variance(self, x_start, x_t, t):
+        """reference gaussian_diffusion.py:246-268: (mean, variance, log_variance_clipped) of q(x_{t-1} | x_t, x_0)."""
+        assert x_start.shape == x_t.shape
+        mean = (_extract_into_tensor(self.posterior_mean_coef1, t, x_t.shape) * x_start
+                + _extract_into_tensor(self.posterior_mean_coef2, t, x_t.shape) * x_t)
+        variance = _extract_into_tensor(self.posterior_variance, t, x_t.shape)
+        log_variance = _extract_into_tensor(self.posterior_log_variance_clipped, t, x_t.shape)
+        return mean, variance, log_variance
+
+    def _model_variance(self):
+        if self.model_var_type == ModelVarType.FIXED_LARGE:
+            return np.append(self.posterior_variance[1], self.betas[1:])
+        return self.posterior_variance
+
+    def p_mean_variance(self, model, x, t, clip_denoised=True, denoised_fn=None, model_kwargs=None):
+        """reference gaussian_diffusion.py:270-381: {'mean', 'variance', 'log_variance', 'pred_xstart'} of p(x_{t-1} | x_t).
+        One engine forward: the DDPM step at zero noise, whose sample is the model mean (bit for bit that step's mean)
+        and whose pred_xstart is p_sample's.  t: LongTensor [B] of one schedule index."""
+        self._reject_hooks(denoised_fn, None, False, False)
+        idx = int(t.reshape(-1)[0].item())
+        assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch (gaussian_diffusion.py:709)"
+        log_variance = self._model_log_variance()           # NotImplementedError for learned variances
+        eng = self._prepare(model, x.shape, model_kwargs, x.device, 0.0)
+        x = x.to(torch.float32).contiguous()
+        mean, pred = eng.sample_step(_lib.MODE_DDPM, idx, x, torch.zeros_like(x), 2 if clip_denoised else 0, want_pred=True)
+        return {"mean": mean, "variance": _extract_into_tensor(self._model_variance(), t, x.shape),
+                "log_variance": _extract_into_tensor(log_variance, t, x.shape), "pred_xstart": pred}
+
+    def calc_bpd_loop(self, model, x_start, clip_denoised=True, model_kwargs=None, noise_tape=None, noise_seed=None,
+                      sample_index_base=0, use_graph=True):
+        """reference gaussian_diffusion.py:1544-1599: the variational lower bound in bits per dimension, as one engine
+        call (every step a replay of one CUDA graph; DESIGN.md section 1).  Returns {'total_bpd' [B], 'prior_bpd' [B],
+        'vb', 'xstart_mse', 'mse' [B, num_timesteps]}, column 0 = schedule index num_timesteps - 1.  The noise of step t
+        is th.randn_like(x_start) from torch's generator in the reference's order (drawn NOISE_CHUNK steps at a time);
+        `noise_tape` [num_timesteps, *x_start.shape] replaces the draws, `noise_seed` (+ `sample_index_base`) switches
+        them to the engine's Philox stream (the eps a sampling loop of that seed would draw at the same index)."""
+        if noise_tape is not None and noise_seed is not None:
+            raise ValueError("noise_seed excludes noise_tape")
+        self._model_log_variance()                           # NotImplementedError for learned variances
+        device = x_start.device
+        eng = self._prepare(model, x_start.shape, model_kwargs, device, 0.0)
+        eng.set_schedule_vb(self.schedule_vb_rows(), key=(id(self), self.num_timesteps, self.model_var_type))
+        xs = x_start.to(device=device, dtype=torch.float32).contiguous()
+        n, B = self.num_timesteps, int(xs.shape[0])
+        terms = torch.empty((3, B, n), device=device, dtype=torch.float32)
+        bpd = torch.empty((2, B), device=device, dtype=torch.float32)
+        flags = 2 if clip_denoised else 0
+        if noise_seed is not None:
+            eng.set_noise_stream(noise_seed, sample_index_base)
+            eng.vb_loop_range(n - 1, n, xs, None, flags, terms, bpd, use_graph)
+            eng._keep["loop"] = (xs,)
+        elif noise_tape is not None:
+            tape = noise_tape.to(device=device, dtype=torch.float32).contiguous()
+            assert tape.shape[0] == n and tuple(tape.shape[1:]) == tuple(xs.shape), (tape.shape, xs.shape)
+            eng.vb_loop_range(n - 1, n, xs, tape, flags, terms, bpd, use_graph)
+            eng._keep["loop"] = (xs, tape)
+        else:
+            def run(first_index, n_run, x_in, last, buf):
+                eng.vb_loop_range(first_index, n_run, x_in, buf, flags, terms if last else None, bpd if last else None,
+                                  use_graph)
+            self._run_generator_loop(eng, None, xs, n, n - 1, flags, use_graph, run_range=run)
+        return {"total_bpd": bpd[0], "prior_bpd": bpd[1], "vb": terms[0], "xstart_mse": terms[1], "mse": terms[2]}
 
     # ------------------------------------------------------------------ out of scope
     def training_losses(self, *a, **k):

@@ -122,8 +122,9 @@ class Engine:
         check(self.lib.b200mdm_set_schedule(self.h, len(tmap), rows.ctypes.data_as(ctypes.c_void_p),
                                             tmap.ctypes.data_as(ctypes.c_void_p)))
         self._sched_key = key
-        self._next_key = None                     # the engine marks the reverse and DPM-Solver++ tables stale
+        self._next_key = None                     # the engine marks the reverse, DPM-Solver++ and bound tables stale
         self._dpm_key = None
+        self._vb_key = None
 
     def set_schedule_next(self, rows, key=None):
         """[n_steps, 2] fp32 rows sqrt(abn), sqrt(1 - abn) of the current schedule (b200mdm_set_schedule_next)."""
@@ -142,6 +143,15 @@ class Engine:
         assert rows.ndim == 2 and rows.shape[1] == _lib.SCHED_DPM_STRIDE
         check(self.lib.b200mdm_set_schedule_dpm(self.h, rows.shape[0], rows.ctypes.data_as(ctypes.c_void_p)))
         self._dpm_key = key
+
+    def set_schedule_vb(self, rows, key=None):
+        """[n_steps, 12] fp32 rows of the variational-bound table of the current schedule (b200mdm_set_schedule_vb)."""
+        if key is not None and key == getattr(self, "_vb_key", None):
+            return
+        rows = np.ascontiguousarray(rows, dtype=np.float32)
+        assert rows.ndim == 2 and rows.shape[1] == _lib.SCHED_VB_STRIDE
+        check(self.lib.b200mdm_set_schedule_vb(self.h, rows.shape[0], rows.ctypes.data_as(ctypes.c_void_p)))
+        self._vb_key = key
 
     # ------------------------------------------------------------------ conditioning
     def set_cond(self, batch, nframes, y, guided, device):
@@ -395,6 +405,17 @@ class Engine:
         x_in None: continue the previous DPM-Solver++ loop of this order; x_out None: leave the state in the engine."""
         check(self.lib.b200mdm_dpm_loop_range(self.h, order, first_index, n_run, _ptr(x_in), _ptr(x_out), flags,
                                               int(use_graph), _stream()))
+
+    def vb_loop_range(self, first_index, n_run, x_start, tape, flags=0, terms=None, bpd=None, use_graph=True):
+        """Bound steps first_index .. first_index-n_run+1 (b200mdm_vb_loop_range).  x_start None: continue the bound loop in
+        the engine; tape None: B200MDM_FLAG_PHILOX_NOISE; terms [3, B, n_steps] / bpd [2, B] fp32 outputs or None."""
+        if tape is not None:
+            assert tape.is_contiguous() and tape.dtype == torch.float32 and tape.shape[0] >= n_run
+        else:
+            flags |= _lib.FLAG_PHILOX_NOISE
+        check(self.lib.b200mdm_vb_loop_range(self.h, first_index, n_run, _ptr(x_start), _ptr(tape),
+                                             tape.stride(0) if tape is not None else 0, flags, _ptr(terms), _ptr(bpd),
+                                             int(use_graph), _stream()))
 
     def dpm_pred_xstart(self, out):
         """out <- the x0 of the last step of the DPM-Solver++ loop in the engine (b200mdm_dpm_pred_xstart)."""
