@@ -204,6 +204,22 @@ int b200mdm_set_target(b200mdm_engine* e, const float* target_dev, const uint8_t
  * until the work enqueued with them has completed. */
 int b200mdm_set_inpaint(b200mdm_engine* e, const uint8_t* mask_dev, const float* motion_dev);
 
+/* Long motions from chained windows (DoubleTake's first take, Shafir et al.; this project's definition, DESIGN.md):
+ * batch sample b is a window of n_b = lengths_host[b] <= nframes frames (all nframes when lengths_host is NULL);
+ * motion_start_host uint8 [batch] marks the windows that begin a motion (NULL: the whole batch is one motion), and
+ * window 0 must begin one.  For a window b that does not, with p = b - 1, handshake position j = 0 .. h-1 pairs frame
+ * n_p - h + j of p with frame j of b; both frames of the model output (x0 after classifier-free guidance) become
+ *   H_j = (1 - a_j) D[p, n_p - h + j] + a_j D[b, j],   a_j = (j + 1) / (h + 1).
+ * The blend is part of the model output, so it applies to every forward of the engine (b200mdm_denoise,
+ * b200mdm_sample_step, b200mdm_plms_step and the DDPM / DDIM, PLMS and DPM-Solver++ loops), ahead of inpainting and the
+ * clamp; the DDIM-inversion and variational-bound entry points return B200MDM_ENOTIMPL while it is set.  Call it after
+ * b200mdm_set_cond / b200mdm_set_cond_dec, which clear it; h == 0 (or a batch of single-window motions) clears it too.
+ * h < 0, a length outside [0, nframes], a chained window with n < h, a window with a predecessor and a successor and
+ * n < 2h, or motion_start_host[0] == 0 return B200MDM_EINVAL before any CUDA call; a prefix-completion (DiP) engine
+ * B200MDM_ENOTIMPL.  The descriptor is uploaded on `stream`; a step graph captured with it reads it at every replay. */
+int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t* lengths_host, const uint8_t* motion_start_host,
+                          void* stream);
+
 /* MDM.forward / ClassifierFreeSampleModel.forward (model/mdm.py:189-283, utils/sampler_util.py:27-34):
  * out = model(x, timesteps, y), without inpainting (the sampler's, not the model's).  timesteps_host: int32 [batch] MODEL
  * timesteps (already mapped). */
@@ -384,6 +400,13 @@ int b200mdm_test_out_vb(const void* hres16_dev, const float* scale_dev, const fl
                         int32_t index, int32_t n_steps, int32_t flags, const uint8_t* inpaint_mask_dev,
                         const float* inpaint_motion_dev, float* pred_xstart_dev, float* elem_dev, float* terms_dev, int32_t B,
                         int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream);
+/* The blend launch of the step alone (blend_split_kernel) with the handshakes of b200mdm_set_handshake for h,
+ * lengths_host and motion_start_host (validated as there, B200MDM_EINVAL before any CUDA call): g16 fp16 [B*T, 3d]
+ * receives [hi | lo | hi] of the CFG blend (halves 2, scale fp32 [B]) or of the rows themselves (halves 1) of the frame
+ * rows of hres16 (as in b200mdm_test_out_step), handshake frames blended.  Synchronises `stream`. */
+int b200mdm_test_blend_handshake(const void* hres16_dev, const float* scale_dev, void* g16_dev, int32_t B, int32_t T,
+                                 int32_t d, int32_t s_off, int32_t halves, int32_t h, const int64_t* lengths_host,
+                                 const uint8_t* motion_start_host, void* stream);
 /* Self-attention core (tensor-core kernel, S <= 256): softmax(q k^T / sqrt(128) + mask) v per (sample, head);
  * qkv16 [n*S, 3d]; kvlen int32 [n] device (valid keys per sample, a prefix).
  * impl 0: out16 fp16 [n*S, d] (the encoder); impl 1: out16 fp16 [n*S, 2d] = [hi | lo] with hi + lo = the fp32 result

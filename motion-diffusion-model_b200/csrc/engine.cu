@@ -132,9 +132,10 @@ struct GraphKey {
   int order = 0;                    // PLMS (Adams-Bashforth step): the order; 0 for DDPM / DDIM
   const void *pred = nullptr, *imask = nullptr, *imotion = nullptr;
   const void* target_g = nullptr;   // the workspace's target embedding, or nullptr when the loop has no target
+  const void* hs = nullptr;         // the workspace's handshake descriptor, or nullptr when the loop has none
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
-           imask == o.imask && imotion == o.imotion && target_g == o.target_g;
+           imask == o.imask && imotion == o.imotion && target_g == o.target_g && hs == o.hs;
   }
 };
 
@@ -168,6 +169,10 @@ struct Workspace {
   // CFG halves; target_set is cleared by every b200mdm_set_cond* call
   float *tgt_valid = nullptr, *tgt_g = nullptr;
   bool target_set = false;
+  // handshakes between chained windows (b200mdm_set_handshake): the blend kernel's descriptor [1 + 2B] int32 (layout
+  // HS_* in kernels.cuh), allocated on first use; hs_set is cleared by every b200mdm_set_cond* call
+  int* hs_desc = nullptr;
+  bool hs_set = false;
   // PLMS, allocated on first use: eps history ring [PLMS_RING, B, JF, T], the improved-Euler step's mean1 (the input of
   // its second forward) and its first x0.  plms_done = evaluations of the PLMS loop in flight (-1: none to continue).
   float *plms_ring = nullptr, *plms_mid = nullptr, *plms_pred = nullptr;
@@ -231,6 +236,7 @@ struct b200mdm_engine : Workspace {
   // host staging for b200mdm_set_cond* (kept alive until the next call: no stream synchronisation needed)
   std::vector<int> h_kv, h_action;
   std::vector<unsigned char> h_mask;
+  std::vector<int> h_hs;
   // trans_dec (DiP)
   bool dec = false;
   // trans_dec with emb_trans_dec and a CLIP memory: sequence = timestep token + frames, cross-attention = a per-sample
@@ -477,10 +483,42 @@ static int launch_vb_reduce(float* terms, int ld_terms, const float* part, int B
                     T * ((JF + 31) / 32), static_cast<float>(JF) * static_cast<float>(T), state));
   return B200MDM_OK;
 }
-// g16 [B*T, 3d] = [hi | hi | lo] of the CFG blend of the frame rows of hres
+// g16 [B*T, 3d] = [hi | hi | lo] of the CFG blend of the frame rows of hres, with the handshakes of descriptor hs
+// (nullptr: none)
 static int launch_blend_split(const __half* hres, __half* g16, const float* scale, int B, int S, int T, int s_off, int d,
-                              int halves, cudaStream_t s) {
-  CUDA_TRY(launch_k(blend_split_kernel, dim3((B * T + 7) / 8), dim3(256), 0, s, hres, g16, scale, B, S, T, s_off, d, halves));
+                              int halves, const int* hs, cudaStream_t s) {
+  CUDA_TRY(launch_k(blend_split_kernel, dim3((B * T + 7) / 8), dim3(256), 0, s, hres, g16, scale, B, S, T, s_off, d, halves, hs));
+  return B200MDM_OK;
+}
+
+// The blend kernel's handshake descriptor (HS_* in kernels.cuh) for B windows of T frames: window b has lengths[b]
+// frames (all T without lengths) and continues window b - 1 unless motion_start[b] (without motion_start, the batch is
+// one motion).  desc is left empty when nothing is blended (h == 0, or every window begins a motion).  Host-only: bad
+// arguments return B200MDM_EINVAL before any CUDA call.
+static int handshake_desc(int h, int B, int T, const int64_t* lengths, const uint8_t* motion_start, std::vector<int>* desc) {
+  desc->clear();
+  if (h < 0) return fail(B200MDM_EINVAL, "handshake size %d < 0", h);
+  if (B <= 0 || T <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
+  if (motion_start && !motion_start[0]) return fail(B200MDM_EINVAL, "window 0 must begin a motion (motion_start[0])");
+  if (h == 0) return B200MDM_OK;
+  std::vector<int> d(1 + 2 * static_cast<size_t>(B), 0);
+  d[HS_H] = h;
+  bool any = false;
+  for (int b = 0; b < B; ++b) {
+    const long long n = lengths ? lengths[b] : T;
+    if (n < 0 || n > T) return fail(B200MDM_EINVAL, "window %d: length %lld outside [0, %d]", b, n, T);
+    d[HS_LEN(b)] = static_cast<int>(n);
+    d[HS_CHAIN(b)] = (b > 0 && !(motion_start && motion_start[b])) ? 1 : 0;
+    any = any || d[HS_CHAIN(b)];
+  }
+  for (int b = 0; b < B; ++b) {
+    const bool prev = d[HS_CHAIN(b)] != 0, next = b + 1 < B && d[HS_CHAIN(b + 1)] != 0;
+    const int n = d[HS_LEN(b)];
+    if ((prev || next) && n < h) return fail(B200MDM_EINVAL, "chained window %d has %d frames < handshake size %d", b, n, h);
+    if (prev && next && n < 2 * h)
+      return fail(B200MDM_EINVAL, "window %d has %d frames < 2 x handshake size %d: its two handshakes would overlap", b, n, h);
+  }
+  if (any) desc->swap(d);
   return B200MDM_OK;
 }
 #ifdef B200_TRACE
@@ -581,7 +619,7 @@ static void free_workspace(Workspace* w) {
   dfree(w->kvlen); dfree(w->tvec); dfree(w->action);
   dfree(w->encperm); dfree(w->memtok); dfree(w->memproj); dfree(w->mem16); dfree(w->qc16); dfree(w->kvc16); dfree(w->memmask);
   dfree(w->cross_mb); dfree(w->cross_u); dfree(w->cross_b); dfree(w->cross_c);
-  dfree(w->tgt_valid); dfree(w->tgt_g);
+  dfree(w->tgt_valid); dfree(w->tgt_g); dfree(w->hs_desc);
   dfree(w->plms_ring); dfree(w->plms_mid); dfree(w->plms_pred);
   dfree(w->dpm_hist);
   dfree(w->vb_xs); dfree(w->vb_part); dfree(w->vb_terms);
@@ -1162,6 +1200,7 @@ static void end_cond(b200mdm_engine* e) {
   e->target_set = false;
   e->inpaint_mask = nullptr;
   e->inpaint_motion = nullptr;
+  e->hs_set = false;
   e->vb_live = false;
 }
 
@@ -1321,6 +1360,23 @@ extern "C" int b200mdm_set_inpaint(b200mdm_engine* e, const uint8_t* mask_dev, c
   if ((mask_dev == nullptr) != (motion_dev == nullptr)) return fail(B200MDM_EINVAL, "inpainting needs both mask and motion");
   e->inpaint_mask = mask_dev;
   e->inpaint_motion = motion_dev;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t* lengths_host,
+                                     const uint8_t* motion_start_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (h < 0) return fail(B200MDM_EINVAL, "handshake size %d < 0", h);
+  if (e->dec && !e->dec_clip) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented for prefix-completion (DiP) models");
+  if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
+  TRY(handshake_desc(h, e->B, e->T, lengths_host, motion_start_host, &e->h_hs));
+  e->hs_set = false;
+  if (e->h_hs.empty()) return B200MDM_OK;   // nothing to blend: the plain forward
+  if (!e->hs_desc) TRY(dalloc(&e->hs_desc, e->h_hs.size()));
+  // the host staging lives in the engine until the next call (as b200mdm_set_cond's): no stream synchronisation
+  CUDA_TRY(cudaMemcpyAsync(e->hs_desc, e->h_hs.data(), e->h_hs.size() * sizeof(int), cudaMemcpyHostToDevice,
+                           static_cast<cudaStream_t>(stream)));
+  e->hs_set = true;
   return B200MDM_OK;
 }
 
@@ -1520,7 +1576,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_LN3, B200MDM_TAP_L_LN3, l, s));
     nk += 5;
   }
-  TRY(launch_blend_split(e->hres, e->g16, e->scale, B, S, T, e->s_off, d, e->halves, s));
+  TRY(launch_blend_split(e->hres, e->g16, e->scale, B, S, T, e->s_off, d, e->halves, e->hs_set ? e->hs_desc : nullptr, s));
   ++nk;
   if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_BLEND, B200MDM_TAP_BLEND, -1, s));
   {
@@ -1625,6 +1681,7 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
     return fail(B200MDM_EINVAL, "DDIM inversion takes no flag but B200MDM_FLAG_CLIP_DENOISED");
   if (reverse && !e->sched_next_fresh)
     return fail(B200MDM_ESTATE, "b200mdm_set_schedule_next has not been called for the current schedule");
+  if (reverse && e->hs_set) return fail(B200MDM_ENOTIMPL, "DDIM inversion with handshakes is not implemented");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, index, nullptr, 0, e->noise_seed, e->noise_sample_base, e->n_steps);
   CUDA_TRY(cudaGetLastError());
@@ -1729,6 +1786,7 @@ static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t
     key.mode = a.mode; key.B = e->B; key.T = e->T; key.flags = flags; key.order = a.order;
     key.imask = e->inpaint_mask; key.imotion = e->inpaint_motion;
     key.target_g = e->target_set ? e->tgt_g : nullptr;
+    key.hs = e->hs_set ? e->hs_desc : nullptr;
     TRY(ensure_step_graph(e, key, a));
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
     CUDA_TRY(cudaStreamWaitEvent(e->work, e->ev_in, 0));
@@ -1805,6 +1863,7 @@ extern "C" int b200mdm_ddim_reverse_loop_range(b200mdm_engine* e, int32_t first_
   if (n_run > e->n_steps - first_index) return fail(B200MDM_EINVAL, "bad step range");
   if (!e->sched_next_fresh)
     return fail(B200MDM_ESTATE, "b200mdm_set_schedule_next has not been called for the current schedule");
+  if (e->hs_set) return fail(B200MDM_ENOTIMPL, "DDIM inversion with handshakes is not implemented");
   StepArgs a;
   a.mode = B200MDM_MODE_DDIM_REVERSE;
   a.x_in = e->x_work;
@@ -1977,6 +2036,7 @@ extern "C" int b200mdm_vb_loop_range(b200mdm_engine* e, int32_t first_index, int
   if (!e->sched_vb_fresh)
     return fail(B200MDM_ESTATE, "b200mdm_set_schedule_vb has not been called for the current schedule");
   if (!x_start_dev && !e->vb_live) return fail(B200MDM_ESTATE, "no bound loop to continue (pass x_start_dev)");
+  if (e->hs_set) return fail(B200MDM_ENOTIMPL, "the variational bound with handshakes is not implemented");
   TRY(ensure_vb(e));
   if (!x_start_dev && !e->vb_live)   // ensure_vb reallocated the tables for a longer schedule: nothing to continue
     return fail(B200MDM_ESTATE, "the schedule outgrew the bound loop's tables: no bound loop to continue (pass x_start_dev)");
@@ -2153,7 +2213,7 @@ static int out_hook_setup(StreamScratch& scr, OutHook* o, const void* hres16_dev
   TRY(scr.alloc(&w_out3, static_cast<size_t>(N_out_pad) * 3 * d, true));
   split_weight_kernel<<<JF, 128, 0, scr.s>>>(w_out_dev, w_out3, JF, d, d);
   CUDA_TRY(cudaGetLastError());
-  TRY(launch_blend_split(static_cast<const __half*>(hres16_dev), g16, scale_dev, B, T + s_off, T, s_off, d, halves, scr.s));
+  TRY(launch_blend_split(static_cast<const __half*>(hres16_dev), g16, scale_dev, B, T + s_off, T, s_off, d, halves, nullptr, scr.s));
   TRY(make_map(&o->m_g16, g16, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
   TRY(make_map(&o->m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
   o->p.bias = b_out_dev;
@@ -2274,6 +2334,27 @@ extern "C" int b200mdm_test_out_vb(const void* hres16_dev, const float* scale_de
   a.pred = pred_xstart_dev;
   TRY(launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms));
   return launch_vb_reduce(terms_dev, n_steps, part, B, T, JF, st, s);
+}
+
+extern "C" int b200mdm_test_blend_handshake(const void* hres16_dev, const float* scale_dev, void* g16_dev, int32_t B,
+                                            int32_t T, int32_t d, int32_t s_off, int32_t halves, int32_t h,
+                                            const int64_t* lengths_host, const uint8_t* motion_start_host, void* stream) {
+  if (!hres16_dev || !g16_dev || B <= 0 || T <= 0 || s_off < 0 || d <= 0 || d % 64 || (halves != 1 && halves != 2) ||
+      (halves == 2 && !scale_dev))
+    return fail(B200MDM_EINVAL, "bad argument");
+  std::vector<int> desc;
+  TRY(handshake_desc(h, B, T, lengths_host, motion_start_host, &desc));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  StreamScratch scr(s);
+  int* hs = nullptr;
+  if (!desc.empty()) {
+    TRY(scr.alloc(&hs, desc.size()));
+    CUDA_TRY(cudaMemcpyAsync(hs, desc.data(), desc.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
+  TRY(launch_blend_split(static_cast<const __half*>(hres16_dev), static_cast<__half*>(g16_dev), scale_dev, B, T + s_off, T,
+                         s_off, d, halves, hs, s));
+  CUDA_TRY(cudaStreamSynchronize(s));   // `desc` is local
+  return B200MDM_OK;
 }
 
 extern "C" int b200mdm_test_attention(const void* qkv16_dev, void* out16_dev, const int32_t* kvlen_dev,

@@ -159,8 +159,30 @@ __global__ void philox_normal_kernel(float* __restrict__ out, int B, long long n
 //   v = h_u + scale[b] * (h_c - h_u)   (same expression as utils/sampler_util.py:34, applied before the linear
 //   OutputProcess: W(h_u + s(h_c-h_u)) + b == out_u + s(out_c - out_u) exactly in real arithmetic)
 //   halves == 1: v = h.       g16 row layout: [hi | lo | hi], ld = 3*d.
+// Handshakes between chained windows (hs != nullptr; layout HS_* below): window b continues window p = b - 1 when
+// hs[HS_CHAIN(b)] != 0; handshake position j = 0 .. h-1 pairs frame n_p - h + j of p with frame j of b, and both rows
+// receive H_j = (1 - a_j) v_p + a_j v_b with a_j = (j + 1) / (h + 1), each v the CFG blend of its own window (its own
+// scale).  OutputProcess is linear per frame and the weights sum to 1, so this is the blend of the two x0 rows.  The two
+// copies of a handshake frame evaluate the same expression on the same operands in the same order: identical g16 rows.
+#define HS_H 0
+#define HS_LEN(b) (1 + 2 * (b))
+#define HS_CHAIN(b) (2 + 2 * (b))
+__device__ __forceinline__ float2 cfg_blend_pair(const __half* hc, const __half* hu, float sc, int d, int c, bool guided) {
+  const float2 ah = __half22float2(*reinterpret_cast<const __half2*>(hc + c));
+  const float2 al = __half22float2(*reinterpret_cast<const __half2*>(hc + d + c));
+  float2 a = make_float2(ah.x + al.x, ah.y + al.y);
+  if (guided) {
+    const float2 uh = __half22float2(*reinterpret_cast<const __half2*>(hu + c));
+    const float2 ul = __half22float2(*reinterpret_cast<const __half2*>(hu + d + c));
+    const float2 u = make_float2(uh.x + ul.x, uh.y + ul.y);
+    a.x = __fadd_rn(u.x, __fmul_rn(sc, __fsub_rn(a.x, u.x)));
+    a.y = __fadd_rn(u.y, __fmul_rn(sc, __fsub_rn(a.y, u.y)));
+  }
+  return a;
+}
 __global__ void blend_split_kernel(const __half* __restrict__ hres, __half* __restrict__ g16,
-                                   const float* __restrict__ scale, int B, int S, int T, int s_off, int d, int halves) {
+                                   const float* __restrict__ scale, int B, int S, int T, int s_off, int d, int halves,
+                                   const int* __restrict__ hs) {
   pdl_launch_dependents();
   pdl_wait();
   // one warp per FRAME row: the rows s < s_off of a sequence (condition token / DiP prefix) never reach x, so g16
@@ -169,22 +191,48 @@ __global__ void blend_split_kernel(const __half* __restrict__ hres, __half* __re
   const int lane = threadIdx.x & 31;
   if (orow >= B * T) return;
   const int b = orow / T;
-  const int row = b * S + s_off + (orow - b * T);
+  const int f = orow - b * T;
+  // handshake: (earlier window wa, its frame fa) and (later window wb, its frame fb), weight a of the later one
+  int wa = -1, fa = 0, wb = 0, fb = 0;
+  float alpha = 0.f;
+  if (hs != nullptr) {
+    const int h = hs[HS_H];
+    const int nb = hs[HS_LEN(b)];
+    if (f < h && hs[HS_CHAIN(b)]) {                                      // prefix of b: partner is p's suffix
+      wa = b - 1; fa = hs[HS_LEN(b - 1)] - h + f; wb = b; fb = f;
+    } else if (b + 1 < B && hs[HS_CHAIN(b + 1)] && f >= nb - h && f < nb) {   // suffix of b: partner is b+1's prefix
+      wa = b; fa = f; wb = b + 1; fb = f - (nb - h);
+    }
+    if (wa >= 0) alpha = __fdiv_rn(static_cast<float>(fb + 1), static_cast<float>(h + 1));
+  }
+  const bool guided = halves == 2;
+  __half* dst = g16 + static_cast<size_t>(orow) * 3 * d;
+  if (wa >= 0) {
+    const int ra = wa * S + s_off + fa, rb = wb * S + s_off + fb;
+    const __half *hca = hres + static_cast<size_t>(ra) * 2 * d, *hua = hres + (static_cast<size_t>(B) * S + ra) * 2 * d;
+    const __half *hcb = hres + static_cast<size_t>(rb) * 2 * d, *hub = hres + (static_cast<size_t>(B) * S + rb) * 2 * d;
+    const float sa = guided ? scale[wa] : 0.f, sb = guided ? scale[wb] : 0.f;
+    const float beta = __fsub_rn(1.f, alpha);
+    for (int c = lane * 2; c < d; c += 64) {
+      const float2 va = cfg_blend_pair(hca, hua, sa, d, c, guided);
+      const float2 vb = cfg_blend_pair(hcb, hub, sb, d, c, guided);
+      const float2 a = make_float2(__fadd_rn(__fmul_rn(beta, va.x), __fmul_rn(alpha, vb.x)),
+                                   __fadd_rn(__fmul_rn(beta, va.y), __fmul_rn(alpha, vb.y)));
+      const __half2 hi = __floats2half2_rn(a.x, a.y);
+      const float2 hif = __half22float2(hi);
+      const __half2 lo = __floats2half2_rn(a.x - hif.x, a.y - hif.y);
+      *reinterpret_cast<__half2*>(dst + c) = hi;
+      *reinterpret_cast<__half2*>(dst + d + c) = lo;
+      *reinterpret_cast<__half2*>(dst + 2 * d + c) = hi;
+    }
+    return;
+  }
+  const int row = b * S + s_off + f;
   const __half* hc = hres + static_cast<size_t>(row) * 2 * d;                         // [hi | lo] rows
   const __half* hu = hres + (static_cast<size_t>(B) * S + row) * 2 * d;
-  const float sc = (halves == 2) ? scale[b] : 0.f;
-  __half* dst = g16 + static_cast<size_t>(orow) * 3 * d;
+  const float sc = guided ? scale[b] : 0.f;
   for (int c = lane * 2; c < d; c += 64) {
-    const float2 ah = __half22float2(*reinterpret_cast<const __half2*>(hc + c));
-    const float2 al = __half22float2(*reinterpret_cast<const __half2*>(hc + d + c));
-    float2 a = make_float2(ah.x + al.x, ah.y + al.y);
-    if (halves == 2) {
-      const float2 uh = __half22float2(*reinterpret_cast<const __half2*>(hu + c));
-      const float2 ul = __half22float2(*reinterpret_cast<const __half2*>(hu + d + c));
-      const float2 u = make_float2(uh.x + ul.x, uh.y + ul.y);
-      a.x = __fadd_rn(u.x, __fmul_rn(sc, __fsub_rn(a.x, u.x)));
-      a.y = __fadd_rn(u.y, __fmul_rn(sc, __fsub_rn(a.y, u.y)));
-    }
+    const float2 a = cfg_blend_pair(hc, hu, sc, d, c, guided);
     const __half2 hi = __floats2half2_rn(a.x, a.y);
     const float2 hif = __half22float2(hi);
     const __half2 lo = __floats2half2_rn(a.x - hif.x, a.y - hif.y);

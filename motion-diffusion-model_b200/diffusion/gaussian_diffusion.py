@@ -204,6 +204,15 @@ class GaussianDiffusion:
         from ..model.mdm import engine_for
         return engine_for(model)
 
+    @staticmethod
+    def _handshake_of(model):
+        from ..model.mdm import handshake_of
+        return handshake_of(model)
+
+    def _reject_handshake(self, model, what):
+        if self._handshake_of(model) is not None:
+            raise NotImplementedError("%s with HandshakeSampleModel is not implemented" % what)
+
     def _prepare(self, model, shape, model_kwargs, device, eta):
         self._check_supported()
         eng, guided = self._engine_of(model)
@@ -214,6 +223,9 @@ class GaussianDiffusion:
         eng.set_schedule(self.schedule_rows(eta), self._timestep_map(), key=(id(self), float(eta), self.num_timesteps))
         B, T = int(shape[0]), int(shape[-1])
         eng.set_cond(B, T, y, guided, device)
+        hs = self._handshake_of(model)
+        if hs is not None and hs.handshake_size > 0:
+            eng.set_handshake(hs.handshake_size, B, T, y)
         if "inpainting_mask" in y and "inpainted_motion" in y:
             assert tuple(y["inpainting_mask"].shape) == tuple(shape) == tuple(y["inpainted_motion"].shape)
             eng.set_inpaint(y["inpainting_mask"].to(device), y["inpainted_motion"].to(device))
@@ -450,6 +462,7 @@ class GaussianDiffusion:
         DDIM ODE.  Returns {'sample', 'pred_xstart'}."""
         if eta != 0.0:
             raise AssertionError("Reverse ODE only for deterministic path")
+        self._reject_handshake(model, "DDIM inversion")
         self._reject_hooks(denoised_fn, None, False, False)
         idx = int(t.reshape(-1)[0].item())
         assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch"
@@ -462,6 +475,7 @@ class GaussianDiffusion:
         """DDIM inversion (no reference counterpart as a loop): exactly the reference step ddim_reverse_sample
         iterated for i = first_index ... first_index + n_steps - 1 (default: the whole schedule, 0 ... n - 1), as one
         engine call (every step a replay of one CUDA graph).  Returns the last step's sample; x_start is not modified."""
+        self._reject_handshake(model, "DDIM inversion")
         first, n_run = self._reverse_range(first_index, n_steps)
         if device is None:
             device = next(model.parameters()).device
@@ -476,6 +490,7 @@ class GaussianDiffusion:
                                              first_index=0, n_steps=None):
         """ddim_reverse_sample_loop as a generator of the reference step's {'sample', 'pred_xstart'}, one step call per
         yield, for i = first_index ... first_index + n_steps - 1."""
+        self._reject_handshake(model, "DDIM inversion")
         first, n_run = self._reverse_range(first_index, n_steps)
         if device is None:
             device = next(model.parameters()).device
@@ -673,6 +688,7 @@ class GaussianDiffusion:
         is th.randn_like(x_start) from torch's generator in the reference's order (drawn NOISE_CHUNK steps at a time);
         `noise_tape` [num_timesteps, *x_start.shape] replaces the draws, `noise_seed` (+ `sample_index_base`) switches
         them to the engine's Philox stream (the eps a sampling loop of that seed would draw at the same index)."""
+        self._reject_handshake(model, "The variational bound")
         if noise_tape is not None and noise_seed is not None:
             raise ValueError("noise_seed excludes noise_tape")
         self._model_log_variance()                           # NotImplementedError for learned variances

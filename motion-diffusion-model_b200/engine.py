@@ -312,6 +312,17 @@ class Engine:
         check(self.lib.b200mdm_set_inpaint(self.h, _ptr(m8), _ptr(mo)))
         self._keep["inpaint"] = (m8, mo)
 
+    def set_handshake(self, handshake_size, batch, nframes, y):
+        """Handshakes between the chained windows of the batch (b200mdm_set_handshake) from y['lengths'] and
+        y['motion_start']; after set_cond, which clears them.  ValueError (before the engine is touched) as
+        utils/sampler_util.handshake_layout raises it."""
+        from .utils.sampler_util import handshake_layout
+        y = y or {}
+        n, ms = handshake_layout(batch, nframes, handshake_size, y.get("lengths"), y.get("motion_start"))
+        n, ms = np.ascontiguousarray(n), np.ascontiguousarray(ms.astype(np.uint8))
+        check(self.lib.b200mdm_set_handshake(self.h, int(handshake_size), n.ctypes.data_as(ctypes.c_void_p),
+                                             ms.ctypes.data_as(ctypes.c_void_p), _stream()))
+
     # ------------------------------------------------------------------ compute
     def denoise(self, x, timesteps):
         x = x.to(torch.float32).contiguous()

@@ -260,27 +260,44 @@ def _identity_rot2xyz(x, mask=None, pose_rep="xyz", **kw):
     return x
 
 
-def _run_model(model, x, timesteps, y, guided):
+def _run_model(model, x, timesteps, y, guided, handshake=0):
     eng = model.engine()
     B, T = x.shape[0], x.shape[-1]
     with torch.cuda.device(x.device):
         eng.set_cond(B, T, y if y is not None else {}, guided, x.device)
+        if handshake:
+            eng.set_handshake(handshake, B, T, y if y is not None else {})
         eng.set_inpaint(None, None)
         return eng.denoise(x, timesteps)
 
 
+def _unwrap(model):
+    """(innermost model, HandshakeSampleModel or None) behind respace._WrappedModel and a HandshakeSampleModel."""
+    from ..utils.sampler_util import HandshakeSampleModel
+    from ..diffusion.respace import _WrappedModel
+    inner = model
+    while isinstance(inner, _WrappedModel):
+        inner = inner.model
+    if isinstance(inner, HandshakeSampleModel):
+        return inner.model, inner
+    return inner, None
+
+
+def handshake_of(model):
+    """The HandshakeSampleModel a sampler was given (possibly behind respace._WrappedModel), or None."""
+    return _unwrap(model)[1]
+
+
 def engine_for(model):
-    """(engine, guided) for a bare MDM or a ClassifierFreeSampleModel wrapper (possibly behind respace._WrappedModel).
+    """(engine, guided) for a bare MDM or a ClassifierFreeSampleModel wrapper (possibly behind respace._WrappedModel
+    and a HandshakeSampleModel, whose handshake the sampler sets with handshake_of).
 
     Only wrappers this package knows are looked through: an unknown object that merely has a `.model` attribute (for
     instance a guidance wrapper class from another import of this package, or the reference's own
     ClassifierFreeSampleModel) would otherwise be unwrapped down to the bare denoiser and sampled WITHOUT guidance,
     silently."""
     from ..utils.sampler_util import ClassifierFreeSampleModel
-    from ..diffusion.respace import _WrappedModel
-    inner = model
-    while isinstance(inner, _WrappedModel):
-        inner = inner.model
+    inner = _unwrap(model)[0]
     if isinstance(inner, ClassifierFreeSampleModel):
         if not isinstance(inner.model, MDM):
             raise TypeError("ClassifierFreeSampleModel must wrap a b200mdm MDM (got %r)" % type(inner.model))

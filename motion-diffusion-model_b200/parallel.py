@@ -62,12 +62,20 @@ def gather_objects(obj, group=None):
 
 
 _BATCH_KEYS = ("mask", "lengths", "scale", "action", "inpainting_mask", "inpainted_motion", "prefix", "target_cond",
-               "is_heading")
+               "is_heading", "motion_start")
 
 
 def shard_model_kwargs(model_kwargs, lo, hi):
-    """Slice the reference's `y` dict (data_loaders/tensors.py:22-64 schema) along the batch dimension."""
+    """Slice the reference's `y` dict (data_loaders/tensors.py:22-64 schema) along the batch dimension.  With
+    y['motion_start'] (chained windows, HandshakeSampleModel) both ends of the slice must be motion boundaries: a motion
+    is never split across shards (ValueError)."""
     y = model_kwargs["y"]
+    if y.get("motion_start") is not None:
+        ms = np.asarray(y["motion_start"].detach().cpu() if torch.is_tensor(y["motion_start"]) else y["motion_start"]).astype(bool)
+        for edge in (lo, hi):
+            if 0 < edge < ms.shape[0] and not ms[edge]:
+                raise ValueError("shard [%d, %d) cuts a motion: window %d continues window %d (y['motion_start'])"
+                                 % (lo, hi, edge, edge - 1))
     out = {}
     for k, v in y.items():
         if k == "text_embed" and torch.is_tensor(v):
@@ -79,7 +87,7 @@ def shard_model_kwargs(model_kwargs, lo, hi):
             out[k] = v[lo:hi].contiguous()
         elif k in ("text", "tokens", "target_joint_names") and isinstance(v, (list, tuple)):
             out[k] = list(v[lo:hi])
-        elif k in ("target_cond", "is_heading", "target_joint_names") and isinstance(v, np.ndarray):
+        elif k in ("target_cond", "is_heading", "target_joint_names", "motion_start") and isinstance(v, np.ndarray):
             out[k] = v[lo:hi]
         else:
             out[k] = v
@@ -103,6 +111,10 @@ def sample_sharded(sample_fn, model, shape, model_kwargs, *, n_steps, noise_mode
         raise ValueError("global batch %d is smaller than the number of ranks %d" % (B, world))
     lo, hi = shard_range(B, rank, world)
     y = model_kwargs["y"]
+    from .model.mdm import handshake_of
+    if world > 1 and handshake_of(model) is not None and y.get("motion_start") is None:
+        raise ValueError("chained windows without y['motion_start'] are one motion, which cannot be split over %d ranks"
+                         % world)
     if torch.is_tensor(y.get("text_embed")) or isinstance(y.get("text_embed"), tuple):
         broadcast_text_embed(y["text_embed"], 0, group)
     local_kwargs = shard_model_kwargs(model_kwargs, lo, hi)

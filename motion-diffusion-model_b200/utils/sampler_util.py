@@ -1,4 +1,5 @@
 """Sampling-time model wrappers (host mirror of the reference's utils/sampler_util.py)."""
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -34,6 +35,108 @@ class ClassifierFreeSampleModel(nn.Module):
 
     def __getattr__(self, name, default=None):
         return wrapped_getattr(self, name, default=None)
+
+
+def handshake_layout(batch, nframes, handshake_size, lengths=None, motion_start=None):
+    """(lengths int64 [batch], motion_start bool [batch]) numpy arrays of a batch of chained windows (DESIGN.md,
+    "Long motions from chained windows"): window b has lengths[b] <= nframes frames (all nframes without lengths) and
+    begins a new motion where motion_start[b] (without motion_start, the batch is one motion).  ValueError for h < 0, a
+    shape mismatch, a length outside [0, nframes], motion_start[0] False, a chained window with fewer than h frames, or a
+    window with a predecessor and a successor and fewer than 2h frames (its two handshakes would overlap)."""
+    h = int(handshake_size)
+    if h < 0:
+        raise ValueError("handshake_size must be >= 0 (got %d)" % h)
+    n = np.full(batch, nframes, dtype=np.int64) if lengths is None else \
+        np.asarray(lengths.detach().cpu() if torch.is_tensor(lengths) else lengths, dtype=np.int64).reshape(-1)
+    if motion_start is None:
+        ms = np.zeros(batch, dtype=bool)
+        ms[0] = True
+    else:
+        ms = np.asarray(motion_start.detach().cpu() if torch.is_tensor(motion_start) else motion_start).astype(bool).reshape(-1)
+    if n.shape != (batch,) or ms.shape != (batch,):
+        raise ValueError("lengths and motion_start need one entry per window (batch %d; got %s and %s)"
+                         % (batch, n.shape, ms.shape))
+    if ((n < 0) | (n > nframes)).any():
+        raise ValueError("window lengths must lie in [0, %d] (got %s)" % (nframes, n.tolist()))
+    if not ms[0]:
+        raise ValueError("motion_start[0] must be True: the first window begins a motion")
+    if h > 0:
+        chained_prev = ~ms
+        chained_next = np.append(~ms[1:], False)
+        for b in range(batch):
+            if (chained_prev[b] or chained_next[b]) and n[b] < h:
+                raise ValueError("window %d is chained but has %d frames < handshake_size %d" % (b, n[b], h))
+            if chained_prev[b] and chained_next[b] and n[b] < 2 * h:
+                raise ValueError("window %d has %d frames < 2 x handshake_size %d: its two handshakes would overlap"
+                                 % (b, n[b], h))
+    return n, ms
+
+
+def _inner_mdm(model):
+    from ..model.mdm import MDM
+    inner = model.model if isinstance(model, ClassifierFreeSampleModel) else model
+    if not isinstance(inner, MDM):
+        raise TypeError("HandshakeSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(model))
+    return inner
+
+
+class HandshakeSampleModel(nn.Module):
+    """Long motions from chained windows (DoubleTake's first take, Shafir et al., "Human Motion Diffusion as a
+    Generative Prior"), with this project's weights (DESIGN.md): the batch is a list of windows, y['lengths'] their
+    lengths and y['motion_start'] (bool [B]) marks the windows that begin a motion (absent: the whole batch is one
+    motion).  The last h = handshake_size frames of every window and the first h frames of the next window of the same
+    motion are replaced, in the model output, by
+
+        H_j = (1 - a_j) * D[p, n_p - h + j] + a_j * D[b, j],   a_j = (j + 1) / (h + 1),   j = 0 .. h-1,
+
+    so every denoising step forces the two to agree.  `model` is a b200mdm MDM or ClassifierFreeSampleModel; the blend
+    runs inside the engine's guidance-blend kernel, in every sampler (DDPM, DDIM, PLMS, DPM-Solver++).  Stitch the
+    final windows with `stitch_handshake`.  Prefix-completion (DiP) models, DDIM inversion and the variational bound are
+    not supported (NotImplementedError)."""
+
+    def __init__(self, model, handshake_size):
+        super().__init__()
+        inner = _inner_mdm(model)
+        if inner.is_prefix_comp or (inner.arch == "trans_dec" and not inner.emb_trans_dec):
+            raise NotImplementedError("handshakes are not implemented for prefix-completion (DiP) models")
+        if int(handshake_size) < 0:
+            raise ValueError("handshake_size must be >= 0 (got %d)" % int(handshake_size))
+        self.model = model
+        self.handshake_size = int(handshake_size)
+        self.rot2xyz = self.model.rot2xyz
+        self.translation = self.model.translation
+        self.njoints = self.model.njoints
+        self.nfeats = self.model.nfeats
+        self.data_rep = self.model.data_rep
+        self.cond_mode = self.model.cond_mode
+        self.encode_text = self.model.encode_text
+
+    def forward(self, x, timesteps, y=None):
+        from ..model.mdm import _run_model
+        guided = isinstance(self.model, ClassifierFreeSampleModel)
+        if guided:
+            assert self.model.model.cond_mode in ["text", "action"]
+        return _run_model(_inner_mdm(self.model), x, timesteps, y, guided=guided, handshake=self.handshake_size)
+
+    def __getattr__(self, name, default=None):
+        return wrapped_getattr(self, name, default=None)
+
+
+def stitch_handshake(sample, lengths, handshake_size, motion_start=None):
+    """The motions of a batch of chained windows (HandshakeSampleModel): for each motion, its first window's frames
+    [:n], then each later window's [h:n].  sample [B, njoints, nfeats, T]; lengths [B] (None: all T); returns a list of
+    [njoints, nfeats, L_k] tensors, L_k = sum(n) - (windows - 1) * h."""
+    B, T = int(sample.shape[0]), int(sample.shape[-1])
+    n, ms = handshake_layout(B, T, handshake_size, lengths, motion_start)
+    h = int(handshake_size)
+    motions = []
+    for b in range(B):
+        piece = sample[b, ..., : int(n[b])] if ms[b] else sample[b, ..., h: int(n[b])]
+        if ms[b]:
+            motions.append([piece])
+        else:
+            motions[-1].append(piece)
+    return [torch.cat(p, dim=-1) for p in motions]
 
 
 class AutoRegressiveSampler:
