@@ -203,6 +203,14 @@ int b200mdm_set_target(b200mdm_engine* e, const float* target_dev, const uint8_t
  * reference's p_mean_variance forms it), never by b200mdm_denoise or b200mdm_test_forward_taps, and must stay valid
  * until the work enqueued with them has completed. */
 int b200mdm_set_inpaint(b200mdm_engine* e, const uint8_t* mask_dev, const float* motion_dev);
+/* Soft inpainting (this project's definition, DESIGN.md "Refined transitions"): weight_dev fp32 [B,J,F,T] with values in
+ * [0, 1] (1 = keep the motion) and motion_dev fp32 [B,J,F,T] device pointers; NULL, NULL clears.  Where the bool mask
+ * replaces x0, the weight blends it: w >= 1 gives the motion, w <= 0 leaves x0, otherwise x0 <- (1 - w) x0 + w motion in
+ * fp32, each operation rounded, before the clamp of clip_denoised.  Setting a weight clears a bool mask and
+ * b200mdm_set_inpaint clears a weight; otherwise the same rules as b200mdm_set_inpaint apply (cleared by
+ * b200mdm_set_cond*, read by every sampler step and loop, never by b200mdm_denoise).  One NULL pointer returns
+ * B200MDM_EINVAL before any CUDA call. */
+int b200mdm_set_inpaint_weight(b200mdm_engine* e, const float* weight_dev, const float* motion_dev);
 
 /* Long motions from chained windows (DoubleTake's first take, Shafir et al.; this project's definition, DESIGN.md):
  * batch sample b is a window of n_b = lengths_host[b] <= nframes frames (all nframes when lengths_host is NULL);
@@ -404,6 +412,16 @@ int b200mdm_test_out_vb(const void* hres16_dev, const float* scale_dev, const fl
  * lengths_host and motion_start_host (validated as there, B200MDM_EINVAL before any CUDA call): g16 fp16 [B*T, 3d]
  * receives [hi | lo | hi] of the CFG blend (halves 2, scale fp32 [B]) or of the rows themselves (halves 1) of the frame
  * rows of hres16 (as in b200mdm_test_out_step), handshake frames blended.  Synchronises `stream`. */
+/* x0 of the output launch with soft inpainting (weight, motion fp32 [B, JF, T], both or neither) on the GEMM
+ * instantiation of an update family, launched as the step launches it: mode B200MDM_MODE_X0 / DDPM / DDIM (the DDPM /
+ * DDIM epilogue), 3 (PLMS), B200MDM_MODE_DDIM_REVERSE, 7 (DPM-Solver++) or 8 (the variational bound).  pred_xstart fp32
+ * [B, JF, T] receives x0 after the blend and the clamp (flags: B200MDM_FLAG_CLIP_DENOISED or 0); the family's other
+ * inputs are zero and its other outputs are discarded.  Other arguments as in b200mdm_test_out_step; invalid arguments
+ * return B200MDM_EINVAL before any CUDA call. */
+int b200mdm_test_out_weight(const void* hres16_dev, const float* scale_dev, const float* w_out_dev, const float* b_out_dev,
+                            const float* x_t_dev, int32_t mode, int32_t flags, const float* weight_dev,
+                            const float* motion_dev, float* pred_xstart_dev, int32_t B, int32_t JF, int32_t T, int32_t d,
+                            int32_t s_off, int32_t halves, void* stream);
 int b200mdm_test_blend_handshake(const void* hres16_dev, const float* scale_dev, void* g16_dev, int32_t B, int32_t T,
                                  int32_t d, int32_t s_off, int32_t halves, int32_t h, const int64_t* lengths_host,
                                  const uint8_t* motion_start_host, void* stream);

@@ -14,6 +14,7 @@ COND_NONE, COND_TEXT, COND_ACTION = 0, 1, 2
 TARGET = {"single": 1, "multi": 2, "split": 3}   # args.multi_encoder_type -> b200mdm_config.target_encoder (0: none)
 MODE_X0, MODE_DDPM, MODE_DDIM = 0, 1, 2
 MODE_DDIM_REVERSE = 6   # (3-5 are the PLMS steps inside the PLMS calls)
+MODE_PLMS_AB, MODE_DPM, MODE_VB = 3, 7, 8   # update families of b200mdm_test_out_weight
 FLAG_CONST_NOISE, FLAG_CLIP_DENOISED, FLAG_PHILOX_NOISE = 1, 2, 4
 SCHED_STRIDE = 8
 SCHED_NEXT_STRIDE = 2
@@ -34,7 +35,7 @@ SYMBOLS = [
     "b200mdm_test_row_bias_ln", "b200mdm_test_forward_taps",
     "b200mdm_set_schedule_dpm", "b200mdm_dpm_loop_range", "b200mdm_dpm_pred_xstart", "b200mdm_test_out_dpm",
     "b200mdm_set_schedule_vb", "b200mdm_vb_loop_range", "b200mdm_test_out_vb",
-    "b200mdm_set_handshake", "b200mdm_test_blend_handshake",
+    "b200mdm_set_handshake", "b200mdm_test_blend_handshake", "b200mdm_set_inpaint_weight", "b200mdm_test_out_weight",
 ]
 # tap points of b200mdm_test_forward_taps (B200MDM_TAP_*)
 TAPS = ["EMBED", "TOK0", "CONDPROJ", "TEMB", "MEM16", "CROSS_C", "KVC16", "L_IN", "L_QKV", "L_ATT", "L_LN1", "L_QC",
@@ -121,7 +122,10 @@ def load():
                        ("b200mdm_test_out_vb", [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp,
                                                 i32, i32, i32, i32, i32, i32, vp]),
                        ("b200mdm_set_handshake", [vp, i32, vp, vp, vp]),
-                       ("b200mdm_test_blend_handshake", [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp])):
+                       ("b200mdm_test_blend_handshake", [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]),
+                       ("b200mdm_set_inpaint_weight", [vp, vp, vp]),
+                       ("b200mdm_test_out_weight", [vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32,
+                                                    vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

@@ -130,12 +130,12 @@ struct LayerW {
 struct GraphKey {
   int mode = -1, B = 0, T = 0, flags = 0;
   int order = 0;                    // PLMS (Adams-Bashforth step): the order; 0 for DDPM / DDIM
-  const void *pred = nullptr, *imask = nullptr, *imotion = nullptr;
+  const void *pred = nullptr, *imask = nullptr, *iweight = nullptr, *imotion = nullptr;
   const void* target_g = nullptr;   // the workspace's target embedding, or nullptr when the loop has no target
   const void* hs = nullptr;         // the workspace's handshake descriptor, or nullptr when the loop has none
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
-           imask == o.imask && imotion == o.imotion && target_g == o.target_g && hs == o.hs;
+           imask == o.imask && iweight == o.iweight && imotion == o.imotion && target_g == o.target_g && hs == o.hs;
   }
 };
 
@@ -246,6 +246,7 @@ struct b200mdm_engine : Workspace {
   int ctx = 0, s_off = 1;
   int kw = 1;   // 2: fp16 activations between the layer GEMMs are [hi | lo] pairs along K (trans_dec engine)
   const unsigned char* inpaint_mask = nullptr;
+  const float* inpaint_weight = nullptr;   // soft inpainting (b200mdm_set_inpaint_weight); never set with the mask
   const float* inpaint_motion = nullptr;
   // in-engine noise (B200MDM_FLAG_PHILOX_NOISE): counter-based Philox4x32-10 keyed by (seed, schedule index, global sample)
   unsigned long long noise_seed = 0;
@@ -1199,6 +1200,7 @@ static void end_cond(b200mdm_engine* e) {
   e->cond_set = true;
   e->target_set = false;
   e->inpaint_mask = nullptr;
+  e->inpaint_weight = nullptr;
   e->inpaint_motion = nullptr;
   e->hs_set = false;
   e->vb_live = false;
@@ -1359,6 +1361,16 @@ extern "C" int b200mdm_set_inpaint(b200mdm_engine* e, const uint8_t* mask_dev, c
   if (!e) return fail(B200MDM_EINVAL, "null engine");
   if ((mask_dev == nullptr) != (motion_dev == nullptr)) return fail(B200MDM_EINVAL, "inpainting needs both mask and motion");
   e->inpaint_mask = mask_dev;
+  e->inpaint_weight = nullptr;
+  e->inpaint_motion = motion_dev;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_inpaint_weight(b200mdm_engine* e, const float* weight_dev, const float* motion_dev) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if ((weight_dev == nullptr) != (motion_dev == nullptr)) return fail(B200MDM_EINVAL, "soft inpainting needs both weight and motion");
+  e->inpaint_mask = nullptr;
+  e->inpaint_weight = weight_dev;
   e->inpaint_motion = motion_dev;
   return B200MDM_OK;
 }
@@ -1584,6 +1596,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     p.bias = e->b_out;
     // inpainting belongs to the sampler (p_mean_variance, gaussian_diffusion.py:300-304), not to MDM.forward
     p.inpaint_mask = a.model_only ? nullptr : e->inpaint_mask;
+    p.inpaint_weight = a.model_only ? nullptr : e->inpaint_weight;
     p.inpaint_motion = a.model_only ? nullptr : e->inpaint_motion;
     p.sched = e->sched;
     p.sched_next = e->sched_next;
@@ -1784,7 +1797,7 @@ static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t
   if (use_graph) {
     GraphKey key;
     key.mode = a.mode; key.B = e->B; key.T = e->T; key.flags = flags; key.order = a.order;
-    key.imask = e->inpaint_mask; key.imotion = e->inpaint_motion;
+    key.imask = e->inpaint_mask; key.iweight = e->inpaint_weight; key.imotion = e->inpaint_motion;
     key.target_g = e->target_set ? e->tgt_g : nullptr;
     key.hs = e->hs_set ? e->hs_desc : nullptr;
     TRY(ensure_step_graph(e, key, a));
@@ -2206,7 +2219,7 @@ struct OutHook {
 };
 static int out_hook_setup(StreamScratch& scr, OutHook* o, const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
                           const float* b_out_dev, const uint8_t* inpaint_mask_dev, const float* inpaint_motion_dev, int B, int JF,
-                          int T, int d, int s_off, int halves) {
+                          int T, int d, int s_off, int halves, const float* inpaint_weight_dev = nullptr) {
   const int N_out_pad = ((JF + 95) / 96) * 96;
   __half *g16 = nullptr, *w_out3 = nullptr;
   TRY(scr.alloc(&g16, static_cast<size_t>(B) * T * 3 * d));
@@ -2218,6 +2231,7 @@ static int out_hook_setup(StreamScratch& scr, OutHook* o, const void* hres16_dev
   TRY(make_map(&o->m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
   o->p.bias = b_out_dev;
   o->p.inpaint_mask = inpaint_mask_dev;
+  o->p.inpaint_weight = inpaint_weight_dev;
   o->p.inpaint_motion = inpaint_motion_dev;
   return B200MDM_OK;
 }
@@ -2334,6 +2348,63 @@ extern "C" int b200mdm_test_out_vb(const void* hres16_dev, const float* scale_de
   a.pred = pred_xstart_dev;
   TRY(launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms));
   return launch_vb_reduce(terms_dev, n_steps, part, B, T, JF, st, s);
+}
+
+// x0 of the output epilogue with soft inpainting, on the GEMM instantiation of update family `mode` (B200MDM_MODE_X0 /
+// DDPM / DDIM: OutStep; 3: OutPlms, 6: OutReverse, 7: OutDpm, 8: OutVb), launched by launch_out_gemm as the step launches
+// it.  Every family writes the x0 it formed to pred_xstart; its other outputs and inputs live in zeroed scratch.
+extern "C" int b200mdm_test_out_weight(const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
+                                       const float* b_out_dev, const float* x_t_dev, int32_t mode, int32_t flags,
+                                       const float* weight_dev, const float* motion_dev, float* pred_xstart_dev, int32_t B,
+                                       int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream) {
+  const bool family = mode == MODE_X0 || mode == MODE_DDPM || mode == MODE_DDIM || mode == MODE_PLMS_AB ||
+                      mode == MODE_DDIM_REVERSE || mode == MODE_DPM || mode == MODE_VB;
+  if (!hres16_dev || !w_out_dev || !b_out_dev || !x_t_dev || !pred_xstart_dev || B <= 0 || JF <= 0 || T <= 0 ||
+      s_off < 0 || d <= 0 || d % 64 || (halves != 1 && halves != 2) || (halves == 2 && !scale_dev) || !family ||
+      (flags & ~B200MDM_FLAG_CLIP_DENOISED) || (weight_dev == nullptr) != (motion_dev == nullptr))
+    return fail(B200MDM_EINVAL, "bad argument");
+  TRY(init_kernel_attrs());
+  int sms = 132;
+  TRY(device_sms(&sms));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  StreamScratch scr(s);
+  OutHook o;
+  TRY(out_hook_setup(scr, &o, hres16_dev, scale_dev, w_out_dev, b_out_dev, nullptr, motion_dev, B, JF, T, d, s_off, halves,
+                     weight_dev));
+  const size_t n = static_cast<size_t>(B) * JF * T;
+  float *x_out = nullptr, *zeros = nullptr, *ring = nullptr, *hist = nullptr, *part = nullptr, *sched = nullptr;
+  float *next = nullptr, *dpm = nullptr, *vb = nullptr;
+  StepState* st = nullptr;
+  TRY(scr.alloc(&x_out, n));
+  TRY(scr.alloc(&zeros, n, true));                       // noise, x_start
+  TRY(scr.alloc(&ring, PLMS_RING * n, true));
+  TRY(scr.alloc(&hist, DPM_SLOTS * n, true));
+  TRY(scr.alloc(&part, static_cast<size_t>(VB_TERMS) * B * T * ((JF + 31) / 32)));
+  TRY(scr.alloc(&sched, SCHED_STRIDE, true));            // one all-zero row of each table: index 0
+  TRY(scr.alloc(&next, SCHED_NEXT_STRIDE, true));
+  TRY(scr.alloc(&dpm, SCHED_DPM_STRIDE, true));
+  TRY(scr.alloc(&vb, SCHED_VB_STRIDE, true));
+  TRY(scr.alloc(&st, 1, true));
+  step_set_kernel<<<1, 1, 0, s>>>(st, 0, 0, nullptr, 0, 0, 0, 1);
+  CUDA_TRY(cudaGetLastError());
+  o.p.sched = sched;
+  o.p.sched_next = next;
+  o.p.sched_dpm = dpm;
+  o.p.sched_vb = vb;
+  o.p.eps_ring = ring;
+  o.p.x0_hist = hist;
+  o.p.x_start = zeros;
+  o.p.vb_part = part;
+  o.p.state = st;
+  StepArgs a;
+  a.mode = mode;
+  a.order = 1;
+  a.x_in = x_t_dev;
+  a.noise = zeros;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  a.x_out = x_out;
+  a.pred = pred_xstart_dev;
+  return launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms);
 }
 
 extern "C" int b200mdm_test_blend_handshake(const void* hres16_dev, const float* scale_dev, void* g16_dev, int32_t B,

@@ -311,6 +311,7 @@ struct EpiOutParams {
   float* x_out;             // [B, J, T]
   float* pred_xstart;       // nullable, except in modes 4 and 5
   const unsigned char* inpaint_mask;  // nullable, bool [B, J, T]
+  const float* inpaint_weight;        // nullable, soft inpainting weight [B, J, T] in [0, 1]; at most one of it and the mask
   const float* inpaint_motion;        // [B, J, T]
   const float* sched;       // [n_steps, SCHED_STRIDE]
   const float* sched_next;  // mode 6: [n_steps, SCHED_NEXT_STRIDE]
@@ -559,6 +560,15 @@ struct OutVb {   // mode 8: writes no sample; the three terms of each element go
   }
 };
 
+// Soft inpainting of one x0 element (DESIGN.md, "Refined transitions"): w >= 1 takes the motion, w <= 0 keeps x0, so a
+// 0 / 1 weight gives the bool mask's bits; in between (1 - w) x0 + w m in fp32 with no contraction.  The motion is read
+// only where it is used.
+__device__ __forceinline__ float soft_inpaint(float x0, float w, const float* motion) {
+  if (w >= 1.f) return *motion;
+  if (w <= 0.f) return x0;
+  return __fadd_rn(__fmul_rn(__fsub_rn(1.f, w), x0), __fmul_rn(w, *motion));
+}
+
 // One GEMM instantiation per update family, so that the PLMS, inversion, DPM-Solver++ and bound epilogues leave the
 // DDPM / DDIM kernel as it is.
 template <class Update>
@@ -592,6 +602,7 @@ struct EpiOut {
         const size_t idx = base + static_cast<size_t>(col) * p.T;
         float x0 = __uint_as_float(raw[h + j]) + __ldg(p.bias + col);
         if (p.inpaint_mask != nullptr && p.inpaint_mask[idx]) x0 = p.inpaint_motion[idx];
+        if (p.inpaint_weight != nullptr) x0 = soft_inpaint(x0, p.inpaint_weight[idx], p.inpaint_motion + idx);
         if (p.clip_denoised) x0 = fminf(fmaxf(x0, -1.f), 1.f);
         u.store(p, idx, x0, v[j]);
       }

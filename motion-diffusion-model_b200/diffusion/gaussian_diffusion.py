@@ -213,11 +213,33 @@ class GaussianDiffusion:
         if self._handshake_of(model) is not None:
             raise NotImplementedError("%s with HandshakeSampleModel is not implemented" % what)
 
+    @staticmethod
+    def _soft_inpainting(y, shape):
+        """(weight, motion) of y['inpainting_weight'] / y['inpainted_motion'] (DESIGN.md, "Refined transitions"), or None
+        without a weight.  ValueError, before any engine work, for a weight next to y['inpainting_mask'], a weight without
+        a motion, a shape other than the sample's, a non-float weight, or a value that is not finite or outside [0, 1]."""
+        if "inpainting_weight" not in y:
+            return None
+        if "inpainting_mask" in y:
+            raise ValueError("y['inpainting_mask'] and y['inpainting_weight'] exclude each other")
+        w, motion = y["inpainting_weight"], y.get("inpainted_motion")
+        if motion is None:
+            raise ValueError("y['inpainting_weight'] needs y['inpainted_motion']")
+        if not torch.is_tensor(w) or not w.is_floating_point():
+            raise ValueError("y['inpainting_weight'] must be a float tensor")
+        if not (tuple(w.shape) == tuple(shape) == tuple(motion.shape)):
+            raise ValueError("y['inpainting_weight'] %s and y['inpainted_motion'] %s must have the sample's shape %s"
+                             % (tuple(w.shape), tuple(motion.shape), tuple(shape)))
+        if not bool((torch.isfinite(w) & (w >= 0) & (w <= 1)).all()):
+            raise ValueError("y['inpainting_weight'] must be finite and within [0, 1]")
+        return w, motion
+
     def _prepare(self, model, shape, model_kwargs, device, eta):
         self._check_supported()
-        eng, guided = self._engine_of(model)
         model_kwargs = model_kwargs if model_kwargs is not None else {}
         y = model_kwargs.get("y", {})
+        soft = self._soft_inpainting(y, shape)
+        eng, guided = self._engine_of(model)
         if "text" in y.keys():                       # encode once, mutate y like the reference (:633-635)
             y["text_embed"] = model.encode_text(y["text"])
         eng.set_schedule(self.schedule_rows(eta), self._timestep_map(), key=(id(self), float(eta), self.num_timesteps))
@@ -226,7 +248,9 @@ class GaussianDiffusion:
         hs = self._handshake_of(model)
         if hs is not None and hs.handshake_size > 0:
             eng.set_handshake(hs.handshake_size, B, T, y)
-        if "inpainting_mask" in y and "inpainted_motion" in y:
+        if soft is not None:
+            eng.set_inpaint_weight(soft[0].to(device), soft[1].to(device))
+        elif "inpainting_mask" in y and "inpainted_motion" in y:
             assert tuple(y["inpainting_mask"].shape) == tuple(shape) == tuple(y["inpainted_motion"].shape)
             eng.set_inpaint(y["inpainting_mask"].to(device), y["inpainted_motion"].to(device))
         else:

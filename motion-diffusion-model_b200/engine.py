@@ -312,6 +312,14 @@ class Engine:
         check(self.lib.b200mdm_set_inpaint(self.h, _ptr(m8), _ptr(mo)))
         self._keep["inpaint"] = (m8, mo)
 
+    def set_inpaint_weight(self, weight, motion):
+        """Soft inpainting (b200mdm_set_inpaint_weight): weight and motion [B, J, F, T], on the engine's device.  It
+        replaces a bool mask; the values are checked by the sampler (gaussian_diffusion._inpainting)."""
+        w = weight.to(torch.float32).contiguous()
+        mo = motion.to(torch.float32).contiguous()
+        check(self.lib.b200mdm_set_inpaint_weight(self.h, _ptr(w), _ptr(mo)))
+        self._keep["inpaint"] = (w, mo)
+
     def set_handshake(self, handshake_size, batch, nframes, y):
         """Handshakes between the chained windows of the batch (b200mdm_set_handshake) from y['lengths'] and
         y['motion_start']; after set_cond, which clears them.  ValueError (before the engine is touched) as

@@ -139,6 +139,141 @@ def stitch_handshake(sample, lengths, handshake_size, motion_start=None):
     return [torch.cat(p, dim=-1) for p in motions]
 
 
+# A transition is sampled as a sequence of its own: one conditioning token + Lt frames within the engine's 256 keys.
+MAX_TRANSITION_FRAMES = 255
+
+
+def transition_layout(batch, nframes, handshake_size, blend_len, lengths=None, motion_start=None,
+                      max_frames=MAX_TRANSITION_FRAMES):
+    """Host-only layout of the refined transitions between chained windows (DoubleTake's second take; DESIGN.md,
+    "Refined transitions").  For every window b that continues p = b - 1 there is one transition of Lt = 2m + h frames
+    (h = handshake_size, m = blend_len): p's last m frames before the handshake, p's copy of the handshake, then b's frames
+    h .. h + m - 1.  Returns a dict of numpy arrays:
+      pairs [n, 2] (p, b);  src_window, src_frame [n, Lt] where each transition frame comes from in the window batch;
+      weight fp32 [Lt] (1 = keep the first take: (m - f)/m, 0 over the handshake, (f - m - h + 1)/m; fp64, rounded once);
+      motion [n] the stitched motion (stitch_handshake) each transition belongs to, and paste [n, 2] the frames
+      [s - m + 1, s + h + m - 1) of that motion its frames 1 .. Lt - 2 replace, s = where b's handshake begins in it.
+    ValueError as handshake_layout raises it, and for m < 1, a chained window with n < h + m, a window chained on both
+    sides with n < 2h + 2m (its transitions would overlap), or Lt > max_frames."""
+    h, m = int(handshake_size), int(blend_len)
+    if m < 1:
+        raise ValueError("blend_len must be >= 1 (got %d)" % m)
+    n, ms = handshake_layout(batch, nframes, h, lengths, motion_start)
+    Lt = 2 * m + h
+    chained_prev = ~ms
+    chained_next = np.append(~ms[1:], False)
+    for b in range(batch):
+        if (chained_prev[b] or chained_next[b]) and n[b] < h + m:
+            raise ValueError("window %d is chained but has %d frames < handshake_size + blend_len = %d" % (b, n[b], h + m))
+        if chained_prev[b] and chained_next[b] and n[b] < 2 * h + 2 * m:
+            raise ValueError("window %d has %d frames < 2 x (handshake_size + blend_len) = %d: its two transitions would "
+                             "overlap" % (b, n[b], 2 * h + 2 * m))
+    if any(chained_prev) and Lt > max_frames:
+        raise ValueError("a transition of 2 x blend_len + handshake_size = %d frames exceeds the model's %d" % (Lt, max_frames))
+    f = np.arange(Lt)
+    w = np.zeros(Lt, dtype=np.float64)
+    w[:m] = (m - f[:m]) / m
+    w[m + h:] = (f[m + h:] - m - h + 1) / m
+    pairs, src_w, src_f, motion, paste = [], [], [], [], []
+    k, off = -1, np.zeros(batch, dtype=np.int64)               # off[b]: where window b's frame 0 lies in its motion
+    for b in range(batch):
+        if ms[b]:
+            k += 1
+            continue
+        p = b - 1
+        off[b] = off[p] + n[p] - h
+        pairs.append((p, b))
+        src_w.append(np.where(f < m + h, p, b))
+        src_f.append(np.where(f < m + h, n[p] - h - m + f, f - m))
+        motion.append(k)
+        paste.append((off[b] - m + 1, off[b] + h + m - 1))
+    shape = (len(pairs), Lt)
+    return dict(pairs=np.asarray(pairs, dtype=np.int64).reshape(-1, 2),
+                src_window=np.asarray(src_w, dtype=np.int64).reshape(shape),
+                src_frame=np.asarray(src_f, dtype=np.int64).reshape(shape), weight=w.astype(np.float32),
+                motion=np.asarray(motion, dtype=np.int64), paste=np.asarray(paste, dtype=np.int64).reshape(-1, 2))
+
+
+# per-window entries of y that a transition takes from its later window; flags that hold for the whole batch
+_PER_WINDOW_KEYS = ("text_embed", "text", "action", "scale", "target_cond", "target_joint_names", "is_heading")
+_BATCH_FLAGS = ("uncond", "target_uncond")
+
+
+def _transition_y(y, windows, Lt, device):
+    """The conditioning of each transition: window b's entries of y (windows = the b of every transition), every one of
+    the Lt frames valid.  The window batch's inpainting, lengths, mask and motion_start stay behind."""
+    idx = torch.as_tensor(windows, dtype=torch.long)
+    out = {k: y[k] for k in _BATCH_FLAGS if k in y}
+    for k in _PER_WINDOW_KEYS:
+        if k not in y:
+            continue
+        v = y[k]
+        if k == "text_embed" and torch.is_tensor(v):
+            out[k] = v if v.shape[1] == 1 else v[:, idx.to(v.device)]          # [1, B, C]; a single prompt is shared
+        elif torch.is_tensor(v):
+            out[k] = v[idx.to(v.device)]
+        elif isinstance(v, np.ndarray):
+            out[k] = v[idx.numpy()]
+        else:
+            out[k] = [v[int(b)] for b in windows]
+    n = len(windows)
+    out["mask"] = torch.ones((n, 1, 1, Lt), dtype=torch.bool, device=device)
+    out["lengths"] = torch.full((n,), Lt, dtype=torch.long, device=device)
+    return out
+
+
+def refine_transitions(sample_fn, model, windows, model_kwargs, handshake_size, blend_len, skip_timesteps,
+                       transition_kwargs=None, **sample_kw):
+    """DoubleTake's second take (Shafir et al., "Human Motion Diffusion as a Generative Prior"; this project's definition,
+    DESIGN.md "Refined transitions"): the motions of a batch of first-take windows (HandshakeSampleModel; laid out by
+    model_kwargs['y']['lengths'] / ['motion_start']) with every transition re-noised to depth skip_timesteps and denoised
+    again as a short motion of its own, its margins softly pinned to the first take.
+
+    All transitions run as ONE call sample_fn(model, (n, J, F, Lt), skip_timesteps=skip_timesteps, init_image=x_init,
+    model_kwargs={'y': y_t}, **sample_kw), y_t carrying y['inpainting_weight'] (transition_layout's weights over J and F)
+    and y['inpainted_motion'] = x_init, and by default each transition window b's conditioning (transition_kwargs replaces
+    it).  The refined frames 1 .. Lt - 2 are pasted into stitch_handshake's motions; without a chained pair those are
+    returned as they are, with no engine call.  `model` is the plain (guided) model: a HandshakeSampleModel raises
+    TypeError, a prefix-completion (DiP) model NotImplementedError; layout errors raise ValueError (transition_layout),
+    as does skip_timesteps outside [0, num_timesteps).  Gather and paste are device indexing only."""
+    from ..model.mdm import _unwrap
+    inner, hs = _unwrap(model)
+    if hs is not None:
+        raise TypeError("refine_transitions runs the plain model: pass the model a HandshakeSampleModel wraps, not the wrapper")
+    mdm = _inner_mdm(inner)
+    if mdm.is_prefix_comp or (mdm.arch == "trans_dec" and not mdm.emb_trans_dec):
+        raise NotImplementedError("transitions are not implemented for prefix-completion (DiP) models")
+    k = int(skip_timesteps)
+    n_steps = getattr(getattr(sample_fn, "__self__", None), "num_timesteps", None)
+    if k < 0 or (n_steps is not None and k >= n_steps):
+        raise ValueError("skip_timesteps must lie in [0, %s) (got %d)" % (n_steps, k))
+    y = model_kwargs["y"]
+    B, J, F, T = (int(s) for s in windows.shape)
+    h = int(handshake_size)
+    lay = transition_layout(B, T, h, blend_len, y.get("lengths"), y.get("motion_start"),
+                            min(MAX_TRANSITION_FRAMES, int(mdm.pos_embed_max_len) - 1))
+    motions = stitch_handshake(windows, y.get("lengths"), h, y.get("motion_start"))
+    n = lay["pairs"].shape[0]
+    if n == 0:
+        return motions
+    Lt, dev = lay["weight"].shape[0], windows.device
+    sw = torch.from_numpy(lay["src_window"]).to(dev)
+    sf = torch.from_numpy(lay["src_frame"]).to(dev)
+    x_init = windows[sw, :, :, sf].permute(0, 2, 3, 1).contiguous()          # [n, Lt, J, F] -> [n, J, F, Lt]
+    w = torch.from_numpy(lay["weight"]).to(dev).view(1, 1, 1, Lt).expand(n, J, F, Lt).contiguous()
+    if transition_kwargs is None:
+        kw = {"y": _transition_y(y, lay["pairs"][:, 1], Lt, dev)}
+    else:
+        kw = dict(transition_kwargs, y=dict(transition_kwargs["y"]))
+    kw["y"]["inpainting_weight"] = w
+    kw["y"]["inpainted_motion"] = x_init
+    refined = sample_fn(model, (n, J, F, Lt), skip_timesteps=k, init_image=x_init, model_kwargs=kw, **sample_kw)
+    for i in range(n):
+        a, b = (int(v) for v in lay["paste"][i])
+        motions[int(lay["motion"][i])][..., a:b] = refined[i, ..., 1:Lt - 1]
+    return motions
+
+
 class AutoRegressiveSampler:
     """DiP's outer loop (reference utils/sampler_util.py:41-81): generate `required_frames` as a chain of `pred_len`
     chunks, each a full diffusion loop of the trans_dec engine conditioned on the last `context_len` frames of the
