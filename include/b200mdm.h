@@ -308,6 +308,40 @@ int b200mdm_dpm_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index
 /* out_dev [B, JF, T] fp32 <- the x0 (pred_xstart) of the last step of that loop.  Enqueued on `stream`. */
 int b200mdm_dpm_pred_xstart(b200mdm_engine* e, float* out_dev, void* stream);
 
+/* DiP's autoregressive chain (AutoRegressiveSampler, utils/sampler_util.py) as one engine loop (DESIGN.md,
+ * "Autoregressive chain").  Chunk c = 0 .. n_chunks - 1 is a full sampling loop of pred_len frames whose prefix is the
+ * last context_len frames of chunk c - 1's sample (chunk 0: the b200mdm_set_prefix prefix); its sample lands at frames
+ * off + c * pred_len of the output [B, JF, crop] (off = context_len with include_prefix != 0, else 0), frames at or past
+ * crop dropped.  Call it after b200mdm_set_cond_dec (batch, nframes = pred_len) and b200mdm_set_prefix, which end any
+ * chain set up before.  enc_chunks_dev [n_chunks, Mt, batch, cond_dim] fp32 device and text_mask_chunks_host uint8
+ * [n_chunks, batch, Mt] (1 = padding) give every chunk a memory of its own, projected here as b200mdm_set_cond_dec
+ * projects one (Mt and the unconditional flag are b200mdm_set_cond_dec's); both NULL keep b200mdm_set_cond_dec's memory
+ * for every chunk.  B200MDM_EINVAL before any CUDA call for n_chunks <= 0, context_len outside 1 .. pred_len, crop
+ * outside 1 .. the chain's frames, or one of the two memory pointers NULL; then for an engine without a prefix or a
+ * pred_len / context_len other than the conditioning's; B200MDM_ESTATE without the conditioning and prefix.  (A DiP
+ * engine never holds handshakes: b200mdm_set_handshake refuses them.) */
+int b200mdm_chain_setup(b200mdm_engine* e, int32_t n_chunks, int32_t pred_len, int32_t context_len, int32_t include_prefix,
+                        int32_t crop, const float* enc_chunks_dev, const uint8_t* text_mask_chunks_host, void* stream);
+/* Global steps first_step .. first_step + n_run - 1 of the chain set up last; step k is step k % n_steps (schedule index
+ * n_steps - 1 - k % n_steps) of chunk k / n_steps.  mode B200MDM_MODE_DDPM / B200MDM_MODE_DDIM with order 0 (the step of
+ * b200mdm_sample_loop_range), or 7 with order 1 or 2 (the step of b200mdm_dpm_loop_range; needs a fresh
+ * b200mdm_set_schedule_dpm table).  Each chunk begins at x_T_dev + c * x_T_chunk_stride (with B200MDM_FLAG_PHILOX_NOISE
+ * and x_T_dev NULL: b200mdm_philox_normal's x_T, step_id -1, of the b200mdm_set_noise_stream seed, for every chunk); the
+ * eps of DDPM / DDIM step k is at noise_tape_dev + (k - first_step) * noise_step_stride (ignored with
+ * B200MDM_FLAG_PHILOX_NOISE).  After the last step of a chunk its sample is written to out_dev [B, JF, crop] and its last
+ * context_len frames become the next chunk's prefix, on the device.  A call continues where the previous one stopped
+ * (first_step == 0 right after b200mdm_chain_setup), so noise can be fed buffer by buffer; any other loop, a
+ * b200mdm_set_cond* or b200mdm_set_prefix ends the chain (B200MDM_ESTATE).  A chain consumes the conditioning: it
+ * replaces the memory and the prefix rows, so from its first call on every other sampling call needs
+ * b200mdm_set_cond_dec and b200mdm_set_prefix again (B200MDM_ESTATE until then).  flags: B200MDM_FLAG_CLIP_DENOISED |
+ * B200MDM_FLAG_PHILOX_NOISE.  B200MDM_EINVAL before any CUDA call for a bad mode, order or flag, a null x_T or (DDPM /
+ * DDIM) noise tape without B200MDM_FLAG_PHILOX_NOISE, a null output or an empty range; then for a non-DiP engine or
+ * steps past the chain; B200MDM_ESTATE without a schedule, with a stale DPM-Solver++ table, or for a first_step other
+ * than where the chain set up last stands.  Tapes and output must stay alive until the enqueued work has completed. */
+int b200mdm_chain_loop_range(b200mdm_engine* e, int32_t mode, int32_t order, int32_t first_step, int32_t n_run,
+                             const float* x_T_dev, int64_t x_T_chunk_stride, const float* noise_tape_dev,
+                             int64_t noise_step_stride, float* out_dev, int32_t flags, int32_t use_graph, void* stream);
+
 /* The variational lower bound (calc_bpd_loop, gaussian_diffusion.py:1544-1599) at schedule indices first_index,
  * first_index-1, ... (n_run of them), each step one forward (one CUDA graph, replayed, when use_graph != 0):
  *   x_t = sqrt_ac*x_start + sqrt_1mac*eps (eps: step k of noise_tape_dev, or the engine's Philox stream with

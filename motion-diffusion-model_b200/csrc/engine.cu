@@ -256,6 +256,17 @@ struct b200mdm_engine : Workspace {
   cudaStream_t work = nullptr;
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   long long launches = 0;
+  // DiP: whether b200mdm_set_cond_dec filled the memory's conditional rows with the unconditional projection
+  bool mem_uncond = false;
+  // autoregressive chain (b200mdm_chain_setup): per-chunk projected memories [n, Bp*Mt, d] and masks [n, Bp*Mt] (unused
+  // when every chunk keeps the memory of b200mdm_set_cond_dec), the prefix handed on [B, JF, ctx], the layout, and the
+  // global step the next b200mdm_chain_loop_range must start at (-1: no chain to run or continue)
+  float *chain_mem = nullptr, *chain_prefix = nullptr;
+  unsigned char* chain_mask = nullptr;
+  size_t chain_mem_cap = 0, chain_mask_cap = 0, chain_prefix_cap = 0;
+  std::vector<unsigned char> h_chain_mask;
+  int chain_n = 0, chain_off = 0, chain_crop = 0, chain_next = -1;
+  bool chain_mems = false;
 };
 
 template <class T>
@@ -653,6 +664,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   free_repacks(e);
   dfree(e->sched); dfree(e->tmap); dfree(e->sched_next); dfree(e->sched_dpm);
   dfree(e->sched_vb);
+  dfree(e->chain_mem); dfree(e->chain_mask); dfree(e->chain_prefix);
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
   if (e->work) cudaStreamDestroy(e->work);
@@ -1204,6 +1216,7 @@ static void end_cond(b200mdm_engine* e) {
   e->inpaint_motion = nullptr;
   e->hs_set = false;
   e->vb_live = false;
+  e->chain_next = -1;
 }
 
 extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* cond_embed_dev,
@@ -1326,7 +1339,8 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
   const size_t warps = static_cast<size_t>(B) * Mt * d;
   small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(e->encperm, e->w_txt, e->b_txt, e->memtok, B * Mt, d, C, C);
   CUDA_TRY(cudaGetLastError());
-  memproj_fill_kernel<<<dim3(Mt, Bp), 128, 0, s>>>(e->memproj, e->memtok, e->b_txt, B, Mt, d, Bp, (halves == 1 && force_uncond) ? 1 : 0);
+  e->mem_uncond = halves == 1 && force_uncond;
+  memproj_fill_kernel<<<dim3(Mt, Bp), 128, 0, s>>>(e->memproj, e->memtok, e->b_txt, B, Mt, d, Bp, e->mem_uncond ? 1 : 0);
   CUDA_TRY(cudaGetLastError());
   e->launches += 3;
   end_cond(e);
@@ -1354,6 +1368,7 @@ extern "C" int b200mdm_set_prefix(b200mdm_engine* e, const float* prefix_dev, vo
   TRY(launch_pack_input(prefix_dev, e->xin16, e->B, e->JF, e->ctx, e->S, e->Kp_in, 0, static_cast<cudaStream_t>(stream)));
   e->launches++;
   e->prefix_set = true;
+  e->chain_next = -1;   // a chain's prefix rows were replaced
   return B200MDM_OK;
 }
 
@@ -1785,14 +1800,12 @@ static int enqueue_plms_euler(b200mdm_engine* e, const StepArgs& base, const flo
 // the step counter starting at `done`; plms_euler: the first step is the PLMS improved-Euler step (two forwards, never
 // a graph), the rest are steps of `a`.  x_in_dev == NULL continues from the state the previous call left there;
 // x_out_dev == NULL leaves the result there.
-static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t first_index, int32_t n_run,
-                    const float* x_in_dev, float* x_out_dev, const float* noise_tape_dev, int64_t noise_step_stride,
-                    int32_t use_graph, void* stream, int done = 0, bool plms_euler = false) {
-  cudaStream_t user = static_cast<cudaStream_t>(stream);
-  const size_t x_bytes = static_cast<size_t>(e->B) * e->JF * e->T * sizeof(float);
-  // The graph path runs on the engine's own stream (the caller's may be the legacy default stream, which cannot be
-  // captured), ordered after / before the caller's stream with events.
-  cudaStream_t s = use_graph ? e->work : user;
+// The stream a loop of `a` runs on: the graph path runs on the engine's own stream (the caller's may be the legacy
+// default stream, which cannot be captured), ordered after the caller's stream with an event (loop_leave orders it
+// back).  x_work no longer holds a PLMS, DPM-Solver++ or chain loop to continue.
+static int loop_enter(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t use_graph, cudaStream_t user,
+                      cudaStream_t* s) {
+  *s = use_graph ? e->work : user;
   if (!use_graph) attach_l2_window(e, user);   // plain launches: the residual-stream window goes on the caller's stream
   if (use_graph) {
     GraphKey key;
@@ -1804,8 +1817,27 @@ static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
     CUDA_TRY(cudaStreamWaitEvent(e->work, e->ev_in, 0));
   }
-  e->plms_done = -1;   // x_work no longer holds a PLMS or DPM-Solver++ loop to continue
+  e->plms_done = -1;
   e->dpm_done = -1;
+  e->chain_next = -1;
+  return B200MDM_OK;
+}
+
+static int loop_leave(b200mdm_engine* e, int32_t use_graph, cudaStream_t user) {
+  if (use_graph) {
+    CUDA_TRY(cudaEventRecord(e->ev_out, e->work));
+    CUDA_TRY(cudaStreamWaitEvent(user, e->ev_out, 0));
+  }
+  return B200MDM_OK;
+}
+
+static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t first_index, int32_t n_run,
+                    const float* x_in_dev, float* x_out_dev, const float* noise_tape_dev, int64_t noise_step_stride,
+                    int32_t use_graph, void* stream, int done = 0, bool plms_euler = false) {
+  cudaStream_t user = static_cast<cudaStream_t>(stream);
+  const size_t x_bytes = static_cast<size_t>(e->B) * e->JF * e->T * sizeof(float);
+  cudaStream_t s;
+  TRY(loop_enter(e, a, flags, use_graph, user, &s));
   if (x_in_dev) CUDA_TRY(cudaMemcpyAsync(e->x_work, x_in_dev, x_bytes, cudaMemcpyDeviceToDevice, s));
   step_set_kernel<<<1, 1, 0, s>>>(e->state, done, first_index, noise_tape_dev, noise_step_stride, e->noise_seed,
                                   e->noise_sample_base, e->n_steps);
@@ -1825,11 +1857,7 @@ static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t
     e->dpm_order = a.order;
   }
   if (x_out_dev) CUDA_TRY(cudaMemcpyAsync(x_out_dev, e->x_work, x_bytes, cudaMemcpyDeviceToDevice, s));
-  if (use_graph) {
-    CUDA_TRY(cudaEventRecord(e->ev_out, e->work));
-    CUDA_TRY(cudaStreamWaitEvent(user, e->ev_out, 0));
-  }
-  return B200MDM_OK;
+  return loop_leave(e, use_graph, user);
 }
 
 // Schedule indices first_index, first_index-1, ... (n_run of them) on the engine's working buffer.
@@ -2006,6 +2034,168 @@ extern "C" int b200mdm_dpm_pred_xstart(b200mdm_engine* e, float* out_dev, void* 
   CUDA_TRY(cudaMemcpyAsync(out_dev, e->dpm_hist + static_cast<size_t>((e->dpm_done - 1) & 1) * n, n * sizeof(float),
                            cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
   return B200MDM_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ autoregressive chain
+static bool is_prefix_engine(const b200mdm_engine* e) { return e->dec && !e->dec_clip && e->ctx > 0; }
+
+template <class T>
+static int ensure_cap(T** p, size_t* cap, size_t n) {
+  if (*cap >= n) return B200MDM_OK;
+  dfree(*p);
+  *cap = 0;
+  TRY(dalloc(p, n));
+  *cap = n;
+  return B200MDM_OK;
+}
+
+// DiP's chain of prefix completions (AutoRegressiveSampler) as one engine loop: the layout, and every chunk's memory
+// projected once, here.
+extern "C" int b200mdm_chain_setup(b200mdm_engine* e, int32_t n_chunks, int32_t pred_len, int32_t context_len,
+                                   int32_t include_prefix, int32_t crop, const float* enc_chunks_dev,
+                                   const uint8_t* text_mask_chunks_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (n_chunks <= 0) return fail(B200MDM_EINVAL, "n_chunks %d <= 0", n_chunks);
+  if (pred_len <= 0 || context_len <= 0 || context_len > pred_len)
+    return fail(B200MDM_EINVAL, "pred_len %d / context_len %d: a chunk hands on 1 .. pred_len frames", pred_len, context_len);
+  const long long total = (include_prefix ? context_len : 0) + static_cast<long long>(n_chunks) * pred_len;
+  if (crop <= 0 || crop > total) return fail(B200MDM_EINVAL, "crop %d outside the chain's 1 .. %lld frames", crop, total);
+  if ((enc_chunks_dev == nullptr) != (text_mask_chunks_host == nullptr))
+    return fail(B200MDM_EINVAL, "per-chunk memories need both the token features and the masks");
+  if (!is_prefix_engine(e)) return fail(B200MDM_EINVAL, "the chain is for prefix-completion (DiP) engines");
+  if (!e->finalized || !e->cond_set || !e->prefix_set)
+    return fail(B200MDM_ESTATE, "weights, b200mdm_set_cond_dec and b200mdm_set_prefix first");
+  if (pred_len != e->T || context_len != e->ctx)
+    return fail(B200MDM_EINVAL, "pred_len %d / context_len %d differ from the conditioning's %d / the model's %d", pred_len,
+                context_len, e->T, e->ctx);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int B = e->B, Bp = e->Bp, Mt = e->Mt, d = e->d, C = e->cfg.cond_dim;
+  e->chain_next = -1;
+  if (e->chain_prefix_cap < static_cast<size_t>(B) * e->JF * e->ctx || (enc_chunks_dev && e->chain_mem_cap < static_cast<size_t>(n_chunks) * Bp * Mt * d)) {
+    CUDA_TRY(cudaDeviceSynchronize());   // a previous chain may still read the buffers being replaced
+  }
+  TRY(ensure_cap(&e->chain_prefix, &e->chain_prefix_cap, static_cast<size_t>(B) * e->JF * e->ctx));
+  e->chain_mems = enc_chunks_dev != nullptr;
+  if (e->chain_mems) {
+    const size_t mem = static_cast<size_t>(Bp) * Mt * d, msk = static_cast<size_t>(Bp) * Mt;
+    TRY(ensure_cap(&e->chain_mem, &e->chain_mem_cap, n_chunks * mem));
+    TRY(ensure_cap(&e->chain_mask, &e->chain_mask_cap, n_chunks * msk));
+    std::vector<unsigned char>& mk = e->h_chain_mask;   // staged in the engine until the next call, as b200mdm_set_cond_dec's
+    mk.assign(n_chunks * msk, 0);
+    for (int c = 0; c < n_chunks; ++c)
+      for (int b = 0; b < Bp; ++b)
+        for (int m = 0; m < Mt; ++m)
+          mk[c * msk + static_cast<size_t>(b) * Mt + m] = text_mask_chunks_host[(static_cast<size_t>(c) * B + b % B) * Mt + m] ? 1 : 0;
+    CUDA_TRY(cudaMemcpyAsync(e->chain_mask, mk.data(), mk.size(), cudaMemcpyHostToDevice, s));
+    // each chunk's text_emb, by the launches of b200mdm_set_cond_dec
+    const size_t warps = static_cast<size_t>(B) * Mt * d;
+    for (int c = 0; c < n_chunks; ++c) {
+      permute_mbc_kernel<<<dim3(Mt, B), 128, 0, s>>>(enc_chunks_dev + static_cast<size_t>(c) * Mt * B * C, e->encperm, Mt, B, C);
+      CUDA_TRY(cudaGetLastError());
+      small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(e->encperm, e->w_txt, e->b_txt, e->memtok,
+                                                                                       B * Mt, d, C, C);
+      CUDA_TRY(cudaGetLastError());
+      memproj_fill_kernel<<<dim3(Mt, Bp), 128, 0, s>>>(e->chain_mem + c * mem, e->memtok, e->b_txt, B, Mt, d, Bp, e->mem_uncond ? 1 : 0);
+      CUDA_TRY(cudaGetLastError());
+    }
+    e->launches += 3 * n_chunks;
+  }
+  e->chain_n = n_chunks;
+  e->chain_off = include_prefix ? context_len : 0;
+  e->chain_crop = crop;
+  e->chain_next = 0;
+  return B200MDM_OK;
+}
+
+// Global steps first_step .. first_step + n_run - 1 of the chain; step k is step k % N of chunk k / N (N = n_steps).  A
+// chunk starts with its memory and x_T in x_work and the step state reset (cur = N - 1, done = 0), so one step graph
+// serves every step of every chunk; after its last step chain_handoff_kernel writes the sample to the output and hands
+// its last ctx frames on as the next chunk's prefix.
+extern "C" int b200mdm_chain_loop_range(b200mdm_engine* e, int32_t mode, int32_t order, int32_t first_step, int32_t n_run,
+                                        const float* x_T_dev, int64_t x_T_chunk_stride, const float* noise_tape_dev,
+                                        int64_t noise_step_stride, float* out_dev, int32_t flags, int32_t use_graph,
+                                        void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  const bool dpm = mode == MODE_DPM;
+  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM && !dpm)
+    return fail(B200MDM_EINVAL, "chain mode %d: B200MDM_MODE_DDPM, B200MDM_MODE_DDIM or 7 (DPM-Solver++)", mode);
+  if (dpm ? (order < 1 || order > 2) : order != 0)
+    return fail(B200MDM_EINVAL, "order %d: 1 or 2 for DPM-Solver++, 0 otherwise", order);
+  if (flags & ~(B200MDM_FLAG_CLIP_DENOISED | B200MDM_FLAG_PHILOX_NOISE))
+    return fail(B200MDM_EINVAL, "a chain takes no flag but B200MDM_FLAG_CLIP_DENOISED and B200MDM_FLAG_PHILOX_NOISE");
+  const bool philox = (flags & B200MDM_FLAG_PHILOX_NOISE) != 0;
+  if (!philox && (!x_T_dev || (!dpm && !noise_tape_dev)))
+    return fail(B200MDM_EINVAL, "null x_T or noise tape (or pass B200MDM_FLAG_PHILOX_NOISE)");
+  if (!out_dev) return fail(B200MDM_EINVAL, "null output");
+  if (first_step < 0 || n_run <= 0) return fail(B200MDM_EINVAL, "bad step range");
+  if (!is_prefix_engine(e)) return fail(B200MDM_EINVAL, "the chain is for prefix-completion (DiP) engines");
+  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
+  if (dpm && !e->sched_dpm_fresh)
+    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_dpm has not been called for the current schedule");
+  if (e->chain_next < 0 || first_step != e->chain_next)
+    return fail(B200MDM_ESTATE, "no chain to run from step %d (b200mdm_chain_setup; next step %d)", first_step, e->chain_next);
+  const int N = e->n_steps;
+  if (static_cast<long long>(first_step) + n_run > static_cast<long long>(e->chain_n) * N)
+    return fail(B200MDM_EINVAL, "steps %d .. %d past the chain's %d x %d", first_step, first_step + n_run - 1, e->chain_n, N);
+  if (dpm && !e->dpm_hist) TRY(dalloc(&e->dpm_hist, DPM_SLOTS * static_cast<size_t>(e->B) * e->JF * e->T));
+  StepArgs a;
+  a.mode = mode;
+  a.order = order;
+  a.x_in = e->x_work;
+  a.x_out = e->x_work;
+  a.philox = philox && !dpm;
+  a.noise = a.philox ? e->eps_buf : nullptr;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  cudaStream_t user = static_cast<cudaStream_t>(stream), s;
+  TRY(loop_enter(e, a, flags, use_graph, user, &s));
+  // The chain consumes the conditioning: it replaces the memory (per-chunk memories) and the prefix rows, so every
+  // other call needs b200mdm_set_cond_dec and b200mdm_set_prefix again (chain_next, not cond_set, admits its own calls).
+  e->cond_set = false;
+  e->prefix_set = false;
+  const int B = e->B, JF = e->JF, T = e->T;
+  const size_t n = static_cast<size_t>(B) * JF * T, mem = static_cast<size_t>(e->Bp) * e->Mt * e->d,
+               msk = static_cast<size_t>(e->Bp) * e->Mt;
+  for (int k = first_step; k < first_step + n_run; ++k) {
+    const int c = k / N, j = k % N;
+    if (j == 0) {
+      if (e->chain_mems) {
+        CUDA_TRY(cudaMemcpyAsync(e->memproj, e->chain_mem + c * mem, mem * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        CUDA_TRY(cudaMemcpyAsync(e->memmask, e->chain_mask + c * msk, msk, cudaMemcpyDeviceToDevice, s));
+      }
+      if (x_T_dev) {
+        CUDA_TRY(cudaMemcpyAsync(e->x_work, x_T_dev + c * x_T_chunk_stride, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+      } else {   // the x_T of b200mdm_philox_normal(step_id -1): the same for every chunk, as the host chain draws it
+        TRY(launch_philox(e->x_work, B, static_cast<long long>(JF) * T, e->noise_seed, e->noise_sample_base, 0xffffffffu,
+                          nullptr, s));
+        e->launches += 1;
+      }
+    }
+    if (j == 0 || k == first_step) {
+      // DPM-Solver++ counts its steps within the chunk (first-order first step, history slots); the noise tape of the
+      // DDPM / DDIM step k is at + (k - first_step) * stride of this call's tape
+      const float* tape = noise_tape_dev && !philox ? noise_tape_dev + static_cast<long long>(k - first_step) * noise_step_stride : nullptr;
+      step_set_kernel<<<1, 1, 0, s>>>(e->state, dpm ? j : 0, N - 1 - j, tape, noise_step_stride, e->noise_seed,
+                                      e->noise_sample_base, N);
+      CUDA_TRY(cudaGetLastError());
+      e->launches += 1;
+    }
+    TRY(enqueue_step(e, a, s, use_graph));
+    if (j == N - 1) {
+      const bool last = c == e->chain_n - 1;
+      const long long rows = static_cast<long long>(B) * JF;
+      chain_handoff_kernel<<<static_cast<int>((rows * T + 255) / 256 < 1184 ? (rows * T + 255) / 256 : 1184), 256, 0, s>>>(
+          e->x_work, out_dev, last ? nullptr : e->chain_prefix, rows, T, e->ctx, e->chain_off + c * T, e->chain_crop);
+      CUDA_TRY(cudaGetLastError());
+      e->launches += 1;
+      if (!last) {
+        TRY(launch_pack_input(e->chain_prefix, e->xin16, B, JF, e->ctx, e->S, e->Kp_in, 0, s));
+        e->launches += 1;
+      }
+    }
+  }
+  const int next = first_step + n_run;
+  e->chain_next = next < e->chain_n * N ? next : -1;
+  return loop_leave(e, use_graph, user);
 }
 
 // ------------------------------------------------------------------------------------------------ variational bound

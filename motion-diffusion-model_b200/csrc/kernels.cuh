@@ -95,6 +95,24 @@ __global__ void step_set_kernel(StepState* state, int done, int cur, const float
   state->sample_base = sample_base;
 }
 
+// Hand-off of an autoregressive chain (b200mdm_chain_loop_range) after the last step of a chunk: the final sample
+// x [B, JF, T] goes to frames off .. off + T - 1 of the chain output out [B, JF, crop] (frames at or past crop are
+// dropped) and, unless prefix is null (the last chunk), its last ctx frames to prefix [B, JF, ctx], which
+// pack_input_kernel then packs into the embedding GEMM's A operand exactly as b200mdm_set_prefix packs y['prefix'].
+// A copy: every value is moved, none is computed.
+__global__ void chain_handoff_kernel(const float* __restrict__ x, float* __restrict__ out, float* __restrict__ prefix,
+                                     long long rows, int T, int ctx, int off, int crop) {
+  const long long n = rows * T;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long row = i / T;
+    const int t = static_cast<int>(i - row * T);
+    const float v = x[i];
+    if (off + t < crop) out[row * crop + off + t] = v;
+    if (prefix != nullptr && t >= T - ctx) prefix[row * ctx + t - (T - ctx)] = v;
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // The engine's own noise stream (B200MDM_FLAG_PHILOX_NOISE / b200mdm_philox_normal): replaces the reference's
 // th.randn_like(x) per step (diffusion/gaussian_diffusion.py:525, :770) when the caller asks for a stream that does not

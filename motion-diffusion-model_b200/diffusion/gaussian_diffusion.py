@@ -668,6 +668,80 @@ class GaussianDiffusion:
             x_in = None
             yield {"sample": sample, "pred_xstart": pred}
 
+    # ------------------------------------------------------------------ DiP's autoregressive chain
+    def _ar_chain(self, mode, model, shape, ys, required_frames, include_prefix, noise=None, clip_denoised=True,
+                  device=None, eta=0.0, order=0, noise_tape=None, use_graph=True, noise_seed=None, sample_index_base=0):
+        """AutoRegressiveSampler.sample's chain of len(ys) prefix completions of shape [B, J, F, pred_len] as engine loops
+        (DESIGN.md, "Autoregressive chain"), for the p_sample_loop (MODE_DDPM), ddim_sample_loop (MODE_DDIM) or
+        dpm_solver_sample_loop (MODE_DPM) keywords utils/sampler_util._chain_plan admits.  ys[c] is chunk c's y without
+        its prefix (chunk 0's y['prefix'] starts the chain); each y['text'] is encoded here, in chunk order, as the host
+        chain's _prepare encodes it.  Conditioning, memories and tables are set once; the prefix hand-off, the chunk's
+        x_T and memory run on the device.  Noise: the host chain's sources in its order -- per chunk x_T (noise[c] /
+        noise / noise_seed's Philox x_T / one torch.randn) and then its steps' eps (noise_tape[c] / Philox / one normal_()
+        each, drawn NOISE_CHUNK steps at a time).  Returns [B, J, F, required_frames], or None before any sampling when a later
+        chunk's text_embed is not a (tokens, mask) pair or the chunks' memories differ in token count (the host chain
+        runs those, and raises what it raises)."""
+        n, N = len(ys), self.num_timesteps
+        B, pred = int(shape[0]), int(shape[-1])
+        if device is None:
+            device = next(model.parameters()).device
+        for y in ys:
+            if "text" in y:
+                y["text_embed"] = model.encode_text(y["text"])
+        tes = [y.get("text_embed") for y in ys]
+        mems = None
+        if any(te is not tes[0] for te in tes[1:]):
+            if not all(isinstance(te, tuple) for te in tes):
+                return None                          # the host chain raises the conditioning's error at that chunk
+            eng, _ = self._engine_of(model)
+            mems = [eng.dec_memory(te, B, device) for te in tes]
+            if len({m[0].shape[0] for m in mems}) > 1:
+                return None
+        y0 = {k: v for k, v in ys[0].items() if k != "text"}         # encoded above
+        eng = self._prepare(model, shape, {"y": y0}, device, eta)
+        if mode == _lib.MODE_DPM:
+            eng.set_schedule_dpm(self.schedule_dpm_rows(), key=(id(self), self.num_timesteps))
+        ctx = eng.context_len
+        prefix = ys[0]["prefix"]
+        enc = None if mems is None else torch.stack([m[0] for m in mems])
+        eng.chain_setup(n, pred, include_prefix, required_frames, enc, None if mems is None else np.stack([m[1] for m in mems]))
+        out = torch.empty(tuple(shape[:-1]) + (required_frames,), device=device, dtype=torch.float32)
+        if include_prefix:
+            out[..., :ctx] = prefix[..., :min(ctx, required_frames)]
+        flags = 2 if clip_denoised else 0
+        if noise_seed is not None:
+            eng.set_noise_stream(noise_seed, sample_index_base)
+        x_T = None
+        if noise is not None:
+            x_T = (noise[:n] if noise.dim() == len(shape) + 1 else noise).to(device=device, dtype=torch.float32).contiguous()
+        draw_x_T = noise is None and noise_seed is None
+        if draw_x_T:
+            x_T = torch.empty((n,) + tuple(shape), device=device, dtype=torch.float32)
+        if mode == _lib.MODE_DPM or noise_seed is not None or noise_tape is not None:
+            if draw_x_T:
+                for c in range(n):
+                    x_T[c].normal_()                 # == torch.randn(*shape): the host chain's only draw per chunk
+            tape = None
+            if noise_tape is not None:
+                tape = noise_tape[:n].to(device=device, dtype=torch.float32).contiguous().view((n * N,) + tuple(shape))
+            eng.chain_loop_range(mode, order, 0, n * N, x_T, tape, out, flags, use_graph)
+            eng._keep["loop"] = (out, x_T, tape)
+            return out
+
+        def draw(buf, k0):                           # the host chain's order: chunk c's x_T, then its steps' eps
+            for j in range(buf.shape[0]):
+                if draw_x_T and (k0 + j) % N == 0:
+                    x_T[(k0 + j) // N].normal_()
+                buf[j].normal_()
+
+        def run(first_index, n_run, x_in, last, buf):
+            eng.chain_loop_range(mode, order, n * N - 1 - first_index, n_run, x_T, buf, out, flags, use_graph)
+
+        self._run_generator_loop(eng, mode, torch.empty(tuple(shape), device=device), n * N, n * N - 1, flags, use_graph,
+                                 noise_fn=draw, run_range=run)
+        eng._keep["loop"] = eng._keep["loop"] + (out, x_T)
+        return out
+
     # ------------------------------------------------------------------ posterior / variational bound
     def q_mean_variance(self, x_start, t):
         """reference gaussian_diffusion.py:209-224: (mean, variance, log_variance) of q(x_t | x_0), table gathers."""

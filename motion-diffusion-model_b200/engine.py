@@ -269,15 +269,9 @@ class Engine:
         self._keep["cond"] = (te, sc)
         self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 2 if sc is not None else 1, 1
 
-    def _set_cond_dec(self, batch, nframes, y, guided, device):
-        """DiP: y['text_embed'] = (BERT tokens [Mt,B,768], padding mask [B,Mt] True = pad), y['prefix'] [B,J,F,ctx]
-        (reference model/mdm.py:203-206,210-217,264)."""
-        if self.dec_clip:
-            return self._set_cond_dec_clip(batch, nframes, y, guided, device)
-        te = y.get("text_embed")
-        if not isinstance(te, tuple):
-            raise RuntimeError("trans_dec (DiP) needs y['text_embed'] = (tokens, mask) from bert_encode_text "
-                               "(model/mdm.py:180-187)")
+    def dec_memory(self, te, batch, device):
+        """(tokens [Mt, batch, cond_dim] contiguous fp32 on device, padding mask uint8 numpy [batch, Mt]) of a DiP
+        y['text_embed'] = (tokens, mask), a single prompt's [Mt, 1, C] / [1, Mt] broadcast over the batch."""
         enc, tmask = te
         enc = enc.detach().to(device=device, dtype=torch.float32)
         if enc.shape[1] == 1 and batch > 1:
@@ -287,7 +281,19 @@ class Engine:
             tmask = torch.repeat_interleave(tmask, batch, dim=0)
         Mt = enc.shape[0]
         assert enc.shape == (Mt, batch, self.cfg.cond_dim) and tuple(tmask.shape) == (batch, Mt), (enc.shape, tmask.shape)
-        tm = np.ascontiguousarray(tmask.detach().cpu().numpy().astype(np.uint8))
+        return enc, np.ascontiguousarray(tmask.detach().cpu().numpy().astype(np.uint8))
+
+    def _set_cond_dec(self, batch, nframes, y, guided, device):
+        """DiP: y['text_embed'] = (BERT tokens [Mt,B,768], padding mask [B,Mt] True = pad), y['prefix'] [B,J,F,ctx]
+        (reference model/mdm.py:203-206,210-217,264)."""
+        if self.dec_clip:
+            return self._set_cond_dec_clip(batch, nframes, y, guided, device)
+        te = y.get("text_embed")
+        if not isinstance(te, tuple):
+            raise RuntimeError("trans_dec (DiP) needs y['text_embed'] = (tokens, mask) from bert_encode_text "
+                               "(model/mdm.py:180-187)")
+        enc, tm = self.dec_memory(te, batch, device)
+        Mt = enc.shape[0]
         ln, sc = self._lengths_and_scale(batch, y, guided, device)
         check(self.lib.b200mdm_set_cond_dec(self.h, batch, nframes, _ptr(enc), tm.ctypes.data_as(ctypes.c_void_p), Mt,
                                             None if ln is None else ln.ctypes.data_as(ctypes.c_void_p), _ptr(sc),
@@ -435,6 +441,26 @@ class Engine:
         check(self.lib.b200mdm_vb_loop_range(self.h, first_index, n_run, _ptr(x_start), _ptr(tape),
                                              tape.stride(0) if tape is not None else 0, flags, _ptr(terms), _ptr(bpd),
                                              int(use_graph), _stream()))
+
+    def chain_setup(self, n_chunks, pred_len, include_prefix, crop, enc_chunks=None, mask_chunks=None):
+        """An autoregressive chain of n_chunks prefix completions after set_cond (b200mdm_chain_setup): enc_chunks
+        [n, Mt, B, C] fp32 device and mask_chunks uint8 numpy [n, B, Mt] give every chunk its memory (None: set_cond's)."""
+        mask = None if mask_chunks is None else np.ascontiguousarray(mask_chunks, dtype=np.uint8)
+        check(self.lib.b200mdm_chain_setup(self.h, int(n_chunks), int(pred_len), int(self.context_len), int(bool(include_prefix)),
+                                           int(crop), _ptr(enc_chunks), None if mask is None else mask.ctypes.data_as(ctypes.c_void_p),
+                                           _stream()))
+        self._keep["chain"] = (enc_chunks, mask)
+
+    def chain_loop_range(self, mode, order, first_step, n_run, x_T, noise, out, flags=0, use_graph=True):
+        """Global steps first_step .. first_step+n_run-1 of the chain (b200mdm_chain_loop_range).  x_T [n_chunks, ...]
+        one per chunk, [...] one for every chunk, or None (the Philox x_T); noise [>= n_run, ...] or None (Philox eps, or
+        none for DPM-Solver++).  out [B, J, F, crop] receives every chunk's frames."""
+        if x_T is None or (noise is None and mode != _lib.MODE_DPM):
+            flags |= _lib.FLAG_PHILOX_NOISE
+        xs = 0 if x_T is None or x_T.dim() == out.dim() else x_T.stride(0)
+        check(self.lib.b200mdm_chain_loop_range(self.h, mode, order, first_step, n_run, _ptr(x_T), xs, _ptr(noise),
+                                                noise.stride(0) if noise is not None else 0, _ptr(out), flags,
+                                                int(use_graph), _stream()))
 
     def dpm_pred_xstart(self, out):
         """out <- the x0 of the last step of the DPM-Solver++ loop in the engine (b200mdm_dpm_pred_xstart)."""

@@ -274,12 +274,78 @@ def refine_transitions(sample_fn, model, windows, model_kwargs, handshake_size, 
     return motions
 
 
+# the samplers whose chain runs as engine loops (GaussianDiffusion._ar_chain), and the keywords each takes there; every
+# other keyword of theirs must keep its default (hooks, init_image / skip_timesteps, dump_steps, const_noise, noise_fn)
+_CHAIN_SAMPLERS = {"p_sample_loop": "MODE_DDPM", "ddim_sample_loop": "MODE_DDIM", "dpm_solver_sample_loop": "MODE_DPM"}
+_CHAIN_KEYS = {"model_kwargs", "noise", "clip_denoised", "device", "progress", "use_graph", "noise_seed",
+               "sample_index_base", "noise_tape", "eta", "order"}
+_CHAIN_DEFAULTS = dict(denoised_fn=None, cond_fn=None, skip_timesteps=0, init_image=None, randomize_class=False,
+                       cond_fn_with_grad=False, dump_steps=None, const_noise=False, noise_fn=None)
+
+
+def _chain_plan(sample_fn, model, ar_shape, n_chunks, kargs):
+    """(diffusion, mode, keywords of GaussianDiffusion._ar_chain) when AutoRegressiveSampler.sample's chain gives the
+    same result as engine loops, else None (the host chain runs): sample_fn is p_sample_loop, ddim_sample_loop or
+    dpm_solver_sample_loop (order 1 or 2) of a b200mdm GaussianDiffusion / SpacedDiffusion, as its class defines it; the
+    model a DiP MDM or its ClassifierFreeSampleModel; no keyword outside _CHAIN_KEYS unless at its default; a noise_tape
+    only for DDPM / DDIM, without noise_seed, and every tape and x_T of the chain's shapes; a float32 y['prefix']."""
+    from ..diffusion import gaussian_diffusion as gd
+    from ..model.mdm import MDM
+    from .. import _lib
+    diffusion, func = getattr(sample_fn, "__self__", None), getattr(sample_fn, "__func__", None)
+    if not isinstance(diffusion, gd.GaussianDiffusion):
+        return None
+    name = next((k for k in _CHAIN_SAMPLERS if func is getattr(gd.GaussianDiffusion, k)), None)
+    if name is None:
+        return None
+    inner = model.model if isinstance(model, ClassifierFreeSampleModel) else model
+    if not (isinstance(inner, MDM) and inner.is_prefix_comp and inner.arch == "trans_dec" and not inner.emb_trans_dec):
+        return None
+    def at_default(k):
+        v, d = kargs[k], _CHAIN_DEFAULTS[k]
+        return v is None if d is None else (isinstance(v, (bool, int, np.integer)) and v == d)
+    if any(k not in _CHAIN_KEYS and (k not in _CHAIN_DEFAULTS or not at_default(k)) for k in kargs):
+        return None
+    if "noise_fn" in kargs and name != "p_sample_loop":          # the other two have no such keyword (TypeError)
+        return None
+    mode = getattr(_lib, _CHAIN_SAMPLERS[name])
+    kw = {k: kargs[k] for k in _CHAIN_KEYS - {"model_kwargs", "progress", "eta", "order"} if k in kargs}
+    if name == "ddim_sample_loop":
+        kw["eta"] = kargs.get("eta", 0.0)
+    elif "eta" in kargs:
+        return None
+    if name == "dpm_solver_sample_loop":
+        order = kargs.get("order", 2)
+        if isinstance(order, bool) or not isinstance(order, (int, np.integer)) or order not in (1, 2):
+            return None
+        if kw.get("noise_tape") is not None:
+            return None
+        kw["order"] = int(order)
+    elif "order" in kargs:
+        return None
+    tape, noise = kw.get("noise_tape"), kw.get("noise")
+    shape = tuple(ar_shape)
+    if tape is not None and (kw.get("noise_seed") is not None or not torch.is_tensor(tape) or tape.dim() != len(shape) + 2
+                             or tape.shape[0] < n_chunks or tape.shape[1] != diffusion.num_timesteps
+                             or tuple(tape.shape[2:]) != shape):
+        return None
+    if noise is not None and not (torch.is_tensor(noise) and (tuple(noise.shape) == shape or (
+            noise.dim() == len(shape) + 1 and noise.shape[0] >= n_chunks and tuple(noise.shape[1:]) == shape))):
+        return None
+    y = (kargs.get("model_kwargs") or {}).get("y")
+    if not isinstance(y, dict) or not torch.is_tensor(y.get("prefix")) or y["prefix"].dtype != torch.float32:
+        return None
+    return diffusion, mode, kw
+
+
 class AutoRegressiveSampler:
     """DiP's outer loop (reference utils/sampler_util.py:41-81): generate `required_frames` as a chain of `pred_len`
     chunks, each a full diffusion loop of the trans_dec engine conditioned on the last `context_len` frames of the
-    previous chunk (y['prefix']).  Host control flow only; every chunk is one `sample_fn` call, i.e. one replay of the
-    engine's captured step graph per diffusion step.  The caller's kwargs are never mutated (the reference deep-copies
-    them per chunk; here only the dicts that change are rebuilt)."""
+    previous chunk (y['prefix']).  With p_sample_loop, ddim_sample_loop or dpm_solver_sample_loop of a b200mdm diffusion
+    (_chain_plan), the whole chain runs as engine loops: the conditioning is set once, and the prefix hand-off between
+    chunks happens on the device, with the same result bit for bit (DESIGN.md, "Autoregressive chain").  Any other
+    sample_fn runs here on the host, one `sample_fn` call per chunk.  The caller's kwargs are never mutated (the
+    reference deep-copies them per chunk; here only the dicts that change are rebuilt)."""
 
     def __init__(self, args, sample_fn, required_frames=196):
         self.sample_fn = sample_fn
@@ -296,6 +362,21 @@ class AutoRegressiveSampler:
         ar_shape = list(shape)
         ar_shape[-1] = pred_len
         tape = kargs.get("noise_tape")            # b200mdm extension: one tape per chunk, [n_iterations, n_run+1, ...]
+        plan = _chain_plan(self.sample_fn, model, ar_shape, n_iterations, kargs)
+        if plan is not None:
+            ys = []
+            for i in range(n_iterations):
+                y = dict(y0)
+                if dynamic_text_mode:
+                    y["text"] = [s[i] for s in y0["text"]]
+                    if getattr(model, "text_encoder_type", "bert") != "bert":
+                        raise NotImplementedError("DiP model only supports BERT text encoder at the moment.")
+                    y["text_embed"] = (y0["text_embed"][0][:, :, i], y0["text_embed"][1][:, i])
+                ys.append(y)
+            diffusion, mode, kw = plan
+            out = diffusion._ar_chain(mode, model, ar_shape, ys, self.required_frames, bool(samples_buf), **kw)
+            if out is not None:
+                return out
         for i in range(n_iterations):
             y = dict(y0)
             y["prefix"] = cur_prefix
