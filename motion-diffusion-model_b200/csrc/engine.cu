@@ -465,7 +465,7 @@ static int launch_philox(float* out, int B, long long n, unsigned long long seed
   CUDA_TRY(launch_k(philox_normal_kernel, dim3(blocks), dim3(256), 0, s, out, B, n, seed, sample_base, step_id, state));
   return B200MDM_OK;
 }
-// x [B, JF, cols] -> rows row_off .. row_off + cols of every S-row sequence of the embedding GEMM's A operand [hi | hi | lo]
+// x [B, JF, cols] -> rows row_off .. row_off + cols of every S-row sequence of the embedding GEMM's A operand [hi | lo | hi]
 static int launch_pack_input(const float* x, __half* xin16, int B, int JF, int cols, int S, int Kp, int row_off, cudaStream_t s) {
   CUDA_TRY(launch_k(pack_input_kernel, dim3((cols + 31) / 32, (JF + 31) / 32, B), dim3(32, 8), 0, s, x, xin16, B, JF, cols, S,
                     Kp, 3 * Kp, row_off));

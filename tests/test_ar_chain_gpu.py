@@ -46,13 +46,14 @@ class FakeBert:
         return enc, present.cuda()
 
 
-def build(steps=STEPS, respacing=None, target=False, mt=6, ctx=CTX, pred=PRED, seed=21):
-    over = dict(layers=L, diffusion_steps=steps, arch="trans_dec", text_encoder_type="bert", context_len=ctx, pred_len=pred)
+def build(steps=STEPS, respacing=None, target=False, mt=6, ctx=CTX, pred=PRED, seed=21, dataset="humanml"):
+    over = dict(layers=L, diffusion_steps=steps, arch="trans_dec", text_encoder_type="bert", context_len=ctx, pred_len=pred,
+                dataset=dataset)
     if target:
         over.update(multi_target_cond=True, multi_encoder_type="multi", target_enc_layers=1)
     model, diffusion = b200mdm.create_model_and_diffusion(default_args(**over), SimpleNamespace(dataset=SimpleNamespace()))
     sd = b200mdm.synthetic_state_dict(arch="trans_dec", num_layers=L, cond_dim=C, seed=seed,
-                                      target_encoder="multi" if target else None)
+                                      target_encoder="multi" if target else None, input_feats=251 if dataset == "kit" else 263)
     b200mdm.load_model_wo_clip(model, sd)
     model.to("cuda").eval()
     model.clip_model = FakeBert(mt)
@@ -64,8 +65,8 @@ def build(steps=STEPS, respacing=None, target=False, mt=6, ctx=CTX, pred=PRED, s
     return model, diffusion, sd
 
 
-def make_y(B, n_chunks, mt=6, ctx=CTX, pred=PRED, guided=True, text="static", seed=3, host_mask=False):
-    enc, tmask, prefix = b200mdm.synthetic_dip_inputs(B, mt, ctx, seed=seed)
+def make_y(B, n_chunks, mt=6, ctx=CTX, pred=PRED, guided=True, text="static", seed=3, host_mask=False, njoints=263):
+    enc, tmask, prefix = b200mdm.synthetic_dip_inputs(B, mt, ctx, njoints=njoints, seed=seed)
     y = dict(prefix=prefix.cuda(), mask=torch.ones(B, 1, 1, pred, dtype=torch.bool).cuda(),
              lengths=torch.tensor([pred] + [pred - 1 - b % 3 for b in range(1, B)]).cuda())
     if host_mask:
@@ -252,12 +253,16 @@ def test_one_conditioning_upload_and_no_host_sync(dip, monkeypatch):
 
 
 def test_chain_against_fp32_oracle(dip):
-    model, diffusion, sd = dip
+    chain_against_fp32_oracle(*dip, 263)
+
+
+def chain_against_fp32_oracle(model, diffusion, sd, njoints):
+    """A 3-chunk chain (each chunk's prefix handed over on the device) against the fp32 oracle's chunks."""
     m = b200mdm.ClassifierFreeSampleModel(model)
     B, required = 3, 20
     n_chunks = -(-required // PRED)
-    shape = (B, 263, 1, PRED)
-    y = make_y(B, n_chunks)
+    shape = (B, njoints, 1, PRED)
+    y = make_y(B, n_chunks, njoints=njoints)
     nk = noise_kw("tape", n_chunks, STEPS, shape)
     args = SimpleNamespace(pred_len=PRED, context_len=CTX, autoregressive_include_prefix=False)
     out = b200mdm.AutoRegressiveSampler(args, diffusion.p_sample_loop, required).sample(

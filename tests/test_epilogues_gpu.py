@@ -203,7 +203,7 @@ def test_embed(B, JF, T, s_off, halves):
     x W^T + b + pe[s] (rows s < s_off: b + pe[s]); the two CFG copies bit-identical."""
     L, lib = _lib()
     d = 512
-    S, Kp = T + s_off, (JF + 7) // 8 * 8
+    S = T + s_off
     g = torch.Generator(device="cuda").manual_seed(B * 1000 + JF + s_off)
     x = torch.randn(B, JF, T, device="cuda", generator=g)
     w = torch.randn(d, JF, device="cuda", generator=g) / JF ** 0.5
@@ -216,7 +216,17 @@ def test_embed(B, JF, T, s_off, halves):
     if halves == 2:
         assert torch.equal(hres[:MB].view(torch.int16), hres[MB:].view(torch.int16)), "CFG copies differ"
     got = hres[:MB, :d].double() + hres[:MB, d:].double()
+    ref, bound, mutants = embed_reference(x, w, b, pe, s_off)
+    check("embed B=%d JF=%d T=%d s_off=%d halves=%d" % (B, JF, T, s_off, halves), (got - ref).abs(), bound, mutants)
 
+
+def embed_reference(x, w, b, pe, s_off):
+    """(fp64 x W^T + b + pe[s] of the GEMM rows (b, s), its per-element bound, errors of the mutants) for the embedding
+    hook's inputs x [B, JF, T], w [d, JF], b [d], pe; the operands as the kernel splits them, [hi | lo | hi] x
+    [hi | hi | lo] with zero pad columns up to Kp = ceil8(JF)."""
+    B, JF, T = x.shape
+    S, Kp = T + s_off, (JF + 7) // 8 * 8
+    MB = B * S
     xr = torch.zeros(B, S, JF, device="cuda")                   # GEMM rows (b, s); frame t at s = s_off + t
     xr[:, s_off:] = x.transpose(1, 2)
     xr = xr.view(MB, JF)
@@ -235,10 +245,9 @@ def test_embed(B, JF, T, s_off, halves):
     bound = (split_product_bound(xr, w) + acc_bound(a3, w3) + U32 * bpe.abs()[s_idx] + (U32 + 2.0 ** -22) * ref.abs()
              + 2.0 ** -25)
     pe_prev = b.double() + pe.double()[(s_idx - 1).clamp(min=0)]
-    check("embed B=%d JF=%d T=%d s_off=%d halves=%d" % (B, JF, T, s_off, halves), (got - ref).abs(), bound,
-          {"A_lo W_hi dropped": (p3 - padk(xl) @ padk(wh).t() - ref).abs(),
-           "A_hi W_lo dropped": (p3 - padk(xh) @ padk(wl).t() - ref).abs(),
-           "pe row s-1": (p3 - bpe[s_idx] + pe_prev - ref).abs()})
+    return ref, bound, {"A_lo W_hi dropped": (p3 - padk(xl) @ padk(wh).t() - ref).abs(),
+                        "A_hi W_lo dropped": (p3 - padk(xh) @ padk(wl).t() - ref).abs(),
+                        "pe row s-1": (p3 - bpe[s_idx] + pe_prev - ref).abs()}
 
 
 # ------------------------------------------------------------------------------------------------ EpiOutStep
@@ -302,30 +311,7 @@ def test_out_step(mode, halves, JF, B, T, s_off, flags, inpaint, alias):
                                       B, JF, T, d, s_off, halves, _stream()))
     torch.cuda.synchronize()
 
-    # frame rows of the residual stream: (b, t) -> row b*S + s_off + t of each CFG half
-    rows = (torch.arange(B, device="cuda")[:, None] * S + s_off + torch.arange(T, device="cuda")[None, :]).flatten()
-    c = (hh.double() + hl.double())[rows]
-    s = torch.zeros(B * T, 1, dtype=F64, device="cuda")
-    if halves == 2:
-        u = (hh.double() + hl.double())[B * S + rows]
-        s = scale.double().repeat_interleave(T)[:, None]
-        v = u + s * (c - u)
-        v_swapped = c + s * (u - c)                                # scale applied to the uncond half
-    else:
-        u, v = c, c
-    w64 = w.double()
-    ref = v @ w64.t() + b.double()                                 # [B*T, JF]
-    # the fp32 blend (three roundings: |dv| <= 2^-24 (2 |s| |c - u| + |v|)), the fp16 [hi|lo|hi] x [hi|hi|lo] split of
-    # v (|lo| <= 2^-11 |v|, |v - hi - lo| <= 2^-22 |v| + 2^-25) and of W, the accumulation, the fp32 bias add
-    V = v.abs() * (1 + 2.0 ** -20)
-    wh, wl = (t.double() for t in split16(w))
-    ew = w64 - wh - wl
-    dv = U32 * (2 * s.abs() * (c - u).abs() + V) * 1.01
-    vh, vl = (t.double() for t in split16(v.float()))
-    a3 = torch.cat([vh, vl, vh], 1)
-    w3 = torch.cat([wh, wh, wl], 1)
-    bound = ((dv + 2.0 ** -22 * V + 2.0 ** -25) @ w64.abs().t() + (2.0 ** -11 * 1.001 * V) @ wl.abs().t()
-             + V @ ew.abs().t() + acc_bound(a3, w3) + U32 * (ref.abs() + 1e-30))
+    ref, bound, v_swapped, vl, wh = out_reference(hh, hl, scale, w, b, B, T, s_off, halves)
 
     def to_bjt(t):
         return t.view(B, T, JF).permute(0, 2, 1)
@@ -338,7 +324,7 @@ def test_out_step(mode, halves, JF, B, T, s_off, flags, inpaint, alias):
     ref_p = post(ref)
     mutants = {"A_lo W_hi dropped": (post(ref - vl @ wh.t()) - ref_p).abs()}
     if halves == 2:
-        mutants["scale applied to the uncond half"] = (post(v_swapped @ w64.t() + b.double()) - ref_p).abs()
+        mutants["scale applied to the uncond half"] = (post(v_swapped @ w.double().t() + b.double()) - ref_p).abs()
     keep = ~mask if inpaint else None
     check("out step mode=%d halves=%d JF=%d B=%d T=%d flags=%d" % (mode, halves, JF, B, T, flags),
           (pred.double() - ref_p).abs(), to_bjt(bound), mutants, where=keep)
@@ -346,8 +332,12 @@ def test_out_step(mode, halves, JF, B, T, s_off, flags, inpaint, alias):
         assert torch.equal(pred[mask], motion[mask]), "inpainted elements must equal the motion exactly"
     if flags & CLIP:
         assert pred.abs().max().item() <= 1.0
+    check_x_out(mode, pred, xt0, noise, xout)
 
-    # x_out: bit-exact against the float32 update evaluated from what the kernel returned
+
+def check_x_out(mode, pred, xt0, noise, xout):
+    """x_out bit for bit against the float32 update evaluated from the pred_xstart the kernel returned; an FMA-contracted
+    evaluation must differ somewhere."""
     x0n, xtn = pred.cpu().numpy(), xt0.cpu().numpy()
     nzn = np.broadcast_to(noise.cpu().numpy(), xtn.shape)
     want = _step_f32(mode, x0n, xtn, nzn, SCHED_ROW)
@@ -361,3 +351,35 @@ def test_out_step(mode, halves, JF, B, T, s_off, flags, inpaint, alias):
         assert nfm > 0, "the bit-exact check would not see an FMA-contracted update"
     print(line)
     assert diff == 0
+
+
+def out_reference(hh, hl, scale, w, b, B, T, s_off, halves):
+    """(fp64 model output [B*T, JF] of the frame rows of the residual stream hh + hl (both CFG halves), its per-element
+    bound, the blend with the scale on the unconditional half, the lo part of the blend's split and the hi part of W's)
+    for the output hooks."""
+    S = T + s_off
+    # frame rows of the residual stream: (b, t) -> row b*S + s_off + t of each CFG half
+    rows = (torch.arange(B, device="cuda")[:, None] * S + s_off + torch.arange(T, device="cuda")[None, :]).flatten()
+    c = (hh.double() + hl.double())[rows]
+    s = torch.zeros(B * T, 1, dtype=F64, device="cuda")
+    if halves == 2:
+        u = (hh.double() + hl.double())[B * S + rows]
+        s = scale.double().repeat_interleave(T)[:, None]
+        v = u + s * (c - u)
+        v_swapped = c + s * (u - c)                                # scale applied to the uncond half
+    else:
+        u, v, v_swapped = c, c, None
+    w64 = w.double()
+    ref = v @ w64.t() + b.double()                                 # [B*T, JF]
+    # the fp32 blend (three roundings: |dv| <= 2^-24 (2 |s| |c - u| + |v|)), the fp16 [hi|lo|hi] x [hi|hi|lo] split of
+    # v (|lo| <= 2^-11 |v|, |v - hi - lo| <= 2^-22 |v| + 2^-25) and of W, the accumulation, the fp32 bias add
+    V = v.abs() * (1 + 2.0 ** -20)
+    wh, wl = (t.double() for t in split16(w))
+    ew = w64 - wh - wl
+    dv = U32 * (2 * s.abs() * (c - u).abs() + V) * 1.01
+    vh, vl = (t.double() for t in split16(v.float()))
+    a3 = torch.cat([vh, vl, vh], 1)
+    w3 = torch.cat([wh, wh, wl], 1)
+    bound = ((dv + 2.0 ** -22 * V + 2.0 ** -25) @ w64.abs().t() + (2.0 ** -11 * 1.001 * V) @ wl.abs().t()
+             + V @ ew.abs().t() + acc_bound(a3, w3) + U32 * (ref.abs() + 1e-30))
+    return ref, bound, v_swapped, vl, wh

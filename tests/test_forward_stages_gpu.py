@@ -125,9 +125,10 @@ def f16(w, kw=1):
 
 
 # ------------------------------------------------------------------------------------------------ model cases
-def build(kind, B, T, L, seed, guided, lengths=None, scale=None, Mt=16, ctx=20, target=None):
+def build(kind, B, T, L, seed, guided, lengths=None, scale=None, Mt=16, ctx=20, target=None, dataset=None):
     """A loaded engine with its conditioning set, and everything the checks need: weights (the model's own state dict,
-    fp32 on the GPU), inputs, y and the shape of the step."""
+    fp32 on the GPU), inputs, y and the shape of the step.  dataset="kit": a text model (trans_enc or DiP) at KIT's 251
+    features."""
     over = dict(layers=L, diffusion_steps=50)
     ds, sdkw, njoints, nfeats = {}, {}, 263, 1
     if kind == "a2m":
@@ -139,6 +140,9 @@ def build(kind, B, T, L, seed, guided, lengths=None, scale=None, Mt=16, ctx=20, 
     elif kind == "dec_emb":
         over.update(arch="trans_dec", text_encoder_type="clip", emb_trans_dec=True)
         sdkw = dict(arch="trans_dec", cond_dim=512)
+    if dataset == "kit":
+        over.update(dataset="kit")
+        sdkw["input_feats"], njoints = 251, 251
     if target:
         over.update(multi_target_cond=True, multi_encoder_type=target, target_enc_layers=1)
         sdkw.update(target_encoder=target, target_enc_layers=1)
@@ -158,7 +162,7 @@ def build(kind, B, T, L, seed, guided, lengths=None, scale=None, Mt=16, ctx=20, 
     elif kind == "a2m":
         y["action"] = torch.arange(B).remainder(12).view(B, 1)
     elif kind == "dip":
-        enc, tmask, prefix = syn.synthetic_dip_inputs(B, Mt, ctx, seed=seed + 2)
+        enc, tmask, prefix = syn.synthetic_dip_inputs(B, Mt, ctx, njoints=njoints, seed=seed + 2)
         y["text_embed"], c.Mt, c.ctx = (enc, tmask), Mt, ctx
         if ctx:
             y["prefix"] = prefix
@@ -496,6 +500,28 @@ def test_stages_trans_enc_text_cfg_b64():
     scale = torch.tensor([0.0, 1.0, 2.5, 7.5]).repeat(B // 4)
     c = build("enc", B, T, 8, 101, True, lengths=_lengths(B, T, 1), scale=scale)
     run_case(c, "trans_enc text, CFG, B=64 T=196 L=8")
+
+
+def test_stages_kit_cfg():
+    """KIT's 251 features (five zero pad columns of the input projection, no K tail, the partial output chunk at
+    [224, 256)): B = 4, T = 196, L = 2, guidance 0 / 1 / 2.5 / 7.5, lengths including 1; then a 3-step loop against the fp32
+    oracle."""
+    B, T = 4, 196
+    c = build("enc", B, T, 2, 191, True, lengths=[196, 1, 120, 57], scale=torch.tensor([0.0, 1.0, 2.5, 7.5]), dataset="kit")
+    assert c.JF == 251 and c.eng.cfg.njoints * c.eng.cfg.nfeats == 251
+    run_case(c, "KIT (251 features), CFG, B=4 T=196 L=2")
+    c.inp["scale"] = torch.tensor([0.0, 1.0, 2.5, 2.5])   # (7.5 on trans_enc: the open xfail of test_precision_margin_gpu.py)
+    c.y["scale"] = c.inp["scale"].cuda()
+    _loop_vs_oracle(c)
+
+
+def test_stages_dip_kit():
+    """DiP (BERT, ctx 20 + pred 40) at KIT's 251 features: the prefix, packed by b200mdm_set_prefix at row 0 of each
+    sequence and the frames at row 20, then a 3-step loop against the fp32 oracle."""
+    c = build("dip", 3, 40, 2, 197, True, lengths=[40, 1, 27], scale=torch.tensor([7.5, 2.5, 1.0]), Mt=16, dataset="kit")
+    assert c.JF == 251 and tuple(c.y["prefix"].shape) == (3, 251, 1, 20)
+    run_case(c, "DiP ctx 20 + 40 at 251 features, CFG, B=3 L=2")
+    _loop_vs_oracle(c)
 
 
 def test_stages_trans_enc_target():
