@@ -366,14 +366,16 @@ static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
 template <class Epi, class = void> struct epi_unstaged : std::false_type {};
 template <class Epi> struct epi_unstaged<Epi, std::enable_if_t<Epi::UNSTAGED>> : std::true_type {};
 
+// the staged GEMM (gemm.cuh) of the embedding and the output projection; the speed of both was measured with these
+// pipeline depths
+static_assert(GemmSmem<128, EpiEmbed>::STAGES == 2, "shared-memory budget: 2 operand stages for the embedding GEMM");
+static_assert(GemmSmem<96, EpiOut<OutStep>>::STAGES == 5, "shared-memory budget: 5 operand stages for the output GEMM");
 template <int BN, class Epi>
-static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& c, int M, int N, int K,
-                       const typename Epi::Params& p, cudaStream_t s, int num_sms) {
-  if (!epi_unstaged<Epi>::value && N * 4 > GEMM_BIAS_BYTES)
-    return fail(B200MDM_ENOTIMPL, "GEMM epilogue vectors are staged for N <= %d", GEMM_BIAS_BYTES / 4);
+static int launch_gemm(const CUtensorMap& a, const CUtensorMap& b, int M, int N, int K, const typename Epi::Params& p,
+                       cudaStream_t s, int num_sms) {
   const int tiles = ((M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M) * ((N + BN - 1) / BN);
   const int grid = tiles < num_sms ? tiles : num_sms;
-  CUDA_TRY(launch_k(gemm_f16_wgmma<BN, Epi>, dim3(grid), dim3(GEMM_THREADS), GemmSmem<BN, Epi>::TOTAL, s, a, b, c, M, N, K, p));
+  CUDA_TRY(launch_k(gemm_f16_wgmma<BN, Epi>, dim3(grid), dim3(GEMM_THREADS), GemmSmem<BN, Epi>::TOTAL, s, a, b, M, N, K, p));
   return B200MDM_OK;
 }
 // projection GEMMs of the step (gemm_pingpong.cuh): 128 x 128 tiles, the two consumer warpgroups take turns (b: W map
@@ -479,7 +481,7 @@ static int launch_embed_gemm(const CUtensorMap& m_xin, const CUtensorMap& m_win,
   p.res_c = m_res_c; p.res_u = m_res_u;
   p.pe_bias = pe_bias;
   p.S = S; p.d = d; p.halves = halves;
-  return launch_gemm<128, EpiEmbed>(m_xin, m_win, m_xin, MB, d, 3 * Kp, p, s, num_sms);
+  return launch_gemm<128, EpiEmbed>(m_xin, m_win, MB, d, 3 * Kp, p, s, num_sms);
 }
 // the bound step's x_t into x_t [B, n] from x_start and the step's eps (noise, or the tape of the step state)
 static int launch_vb_xt(float* x_t, const float* x_start, const float* noise, const float* sched_vb, const StepState* state,
@@ -1440,11 +1442,11 @@ static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, 
   p.order = a.order;
   p.back = a.back;
   const int M = B * T, N = ((JF + 95) / 96) * 96, K = 3 * d;
-  if (a.mode <= MODE_DDIM) return launch_gemm<96, EpiOut<OutStep>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
-  if (a.mode == MODE_DDIM_REVERSE) return launch_gemm<96, EpiOut<OutReverse>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
-  if (a.mode == MODE_DPM) return launch_gemm<96, EpiOut<OutDpm>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
-  if (a.mode == MODE_VB) return launch_gemm<96, EpiOut<OutVb>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
-  return launch_gemm<96, EpiOut<OutPlms>>(m_g16, m_wout, m_g16, M, N, K, p, s, sms);
+  if (a.mode <= MODE_DDIM) return launch_gemm<96, EpiOut<OutStep>>(m_g16, m_wout, M, N, K, p, s, sms);
+  if (a.mode == MODE_DDIM_REVERSE) return launch_gemm<96, EpiOut<OutReverse>>(m_g16, m_wout, M, N, K, p, s, sms);
+  if (a.mode == MODE_DPM) return launch_gemm<96, EpiOut<OutDpm>>(m_g16, m_wout, M, N, K, p, s, sms);
+  if (a.mode == MODE_VB) return launch_gemm<96, EpiOut<OutVb>>(m_g16, m_wout, M, N, K, p, s, sms);
+  return launch_gemm<96, EpiOut<OutPlms>>(m_g16, m_wout, M, N, K, p, s, sms);
 }
 
 // Stage outputs requested by b200mdm_test_forward_taps: dst[id] (B200MDM_TAP_*) receives a device copy of the

@@ -1,6 +1,7 @@
-// Fused GEMM epilogues (see gemm.cuh for the calling protocol).  Thread = accumulator row.  The projection epilogues
-// (EpiBiasF16, EpiBiasF16Global, EpiBiasF16Wide) provide the fragment interface of gemm_pingpong.cuh instead (pp_*:
-// one column pair of the wgmma accumulator fragment at a time).
+// Fused GEMM epilogues.  EpiEmbed and EpiOut serve the staged kernel gemm_f16_wgmma (gemm.cuh: chunk / finish, thread
+// = accumulator row, 32 columns at a time).  The projection epilogues (EpiBiasF16, EpiBiasF16Global, EpiBiasF16Wide)
+// provide the fragment interface of gemm_pingpong.cuh instead (preload, then pp_*: one column pair of the wgmma
+// accumulator fragment at a time).
 //
 // Row-major outputs are written as 128-byte-per-row slabs (32 rows of the warp x 64 fp16 or 32 fp32 columns = 4 KB)
 // staged in warp-private shared memory in the TMA 128-byte swizzle and shipped with cp.async.bulk.tensor stores;
@@ -163,16 +164,13 @@ struct EpiBiasF16Wide {
 //   Output: the residual stream as fp16 [hi | lo] (hi half = the next GEMM's A operand).
 struct EpiEmbed {
   static constexpr int SMEM_PER_WARP = 2 * 4096;  // two [hi | lo] slabs
-  template <class P> static __device__ __forceinline__ void preload(const P&, float*, int, int, int) {}
   struct Params {
     CUtensorMap res_c, res_u;                 // residual stream [rows, 2d] = [hi | lo] of the two CFG halves,
                                               // box {32 cols, 32 rows} (64-byte rows, SWIZZLE_64B)
     const float* pe_bias;                     // [S, d] = pe[s] + bias
     int S, d, halves;
   };
-  static __device__ __forceinline__ void tile_begin(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0,
-                                               int) {
+  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0) {
     uint8_t* slab = ctx.smem + (ctx.seq & 1) * 4096;
     if (ctx.lane == 0) bulk_wait_group_read<1>();  // the group that last read this slab (two chunks ago) is done
     __syncwarp();
@@ -205,7 +203,6 @@ struct EpiEmbed {
     }
     ctx.seq++;
   }
-  static __device__ __forceinline__ void tile_end(EpiCtx&, const Params&, int, int) {}
   static __device__ __forceinline__ void finish(EpiCtx& ctx) {
     if (ctx.lane == 0) bulk_wait_group<0>();
     __syncwarp();
@@ -575,10 +572,7 @@ template <class Update>
 struct EpiOut {
   static constexpr int SMEM_PER_WARP = 1024;  // unused
   using Params = EpiOutParams;
-  static __device__ __forceinline__ void preload(const Params&, float*, int, int, int) {}
-  static __device__ __forceinline__ void tile_begin(EpiCtx&, const Params&, int, int) {}
-  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0,
-                                               int) {
+  static __device__ __forceinline__ void chunk(EpiCtx& ctx, const Params& p, uint32_t (&raw)[32], int row0, int col0) {
     const int row = row0 + ctx.lane;
     if (row >= ctx.M) return;
     const int b = row / p.T, t = row - b * p.T;
@@ -609,7 +603,6 @@ struct EpiOut {
     }
     u.end(p, row, col0);
   }
-  static __device__ __forceinline__ void tile_end(EpiCtx&, const Params&, int, int) {}
   static __device__ __forceinline__ void finish(EpiCtx&) {}
 };
 

@@ -1,22 +1,24 @@
-// Persistent warp-specialised wgmma GEMM for sm_90a:   D[M,N] = A[M,K] * W[N,K]^T   (fp16 in, fp32 accumulate)
+// wgmma GEMMs for sm_90a:   D[M,N] = A[M,K] * W[N,K]^T   (fp16 in, fp32 accumulate)
 //
-//   warpgroup 0      : TMA producer (one elected thread: cp.async.bulk.tensor 2-D, 128B-swizzled tiles, STAGES-deep
-//                      mbarrier ring)
-//   warpgroups 1, 2  : consumers.  Warpgroup g issues wgmma m64 x BLOCK_N x k16 for rows [64 (g-1), +64) of the 128-row
-//                      tile, accumulators in registers, and then runs the fused epilogue of those rows itself.
+// The operand pipeline shared by the three GEMM kernels (this file's gemm_f16_wgmma, gemm_f16_pingpong in
+// gemm_pingpong.cuh, gemm_resid_ln_cluster in gemm_ln.cuh): a 384-thread CTA whose warpgroup 0 is the TMA producer
+// (one elected thread, cp.async.bulk.tensor 2-D, 128B-swizzled A and W boxes) and warpgroups 1 and 2 the wgmma
+// consumers.  The operands flow through a STAGES-deep ring of shared-memory stages, each with a `full` mbarrier (the
+// producer's expect_tx + the TMA transactions) and an `empty` mbarrier (the consumer warps' arrivals once the MMAs that
+// read the stage are done).  Ring tracks the stage and phase, produce_kblocks fills one tile's k-blocks and
+// consume_kblocks issues their MMAs with one wgmma group in flight while the next stage is awaited.  A is [M,K]
+// row-major (K contiguous), W is the torch nn.Linear layout [N,K] row-major -- both K-major wgmma operands, no
+// transposes anywhere.  K tails / M tails / N tails rely on TMA out-of-bounds zero fill (loads) and clipping (stores).
 //
-// Epilogue: the accumulator fragment is staged through a warpgroup-private fp32 tile in shared memory so that the fused
-// epilogue functors see it as "thread = row" -- warp w of the warpgroup owns rows [32 (w & 1), +32) and the
-// 64-column block part = w >> 1 of the tile (BLOCK_N <= 128), lane = row; each 32-column chunk is handed to the functor, which stages its
-// 128-byte-per-row output slab in warp-private shared memory (128B swizzle) and ships it with a TMA store.
-//
-// Tiles are statically strided over the persistent grid (tile = blockIdx.x + k * gridDim.x, N fastest so concurrently
-// running CTAs share the same A rows in L2).  The step runs this kernel for the embedding (BLOCK_N = 128) and the output
-// projection (96), once per step each; the per-layer projections run on gemm_f16_pingpong (gemm_pingpong.cuh), which
-// takes its epilogue from the accumulator fragment.  A is [M,K] row-major (K contiguous), W is the torch nn.Linear
-// layout [N,K] row-major -- both K-major wgmma operands, no transposes anywhere.  While the consumers run the epilogue
-// of tile i the producer already streams the operands of tile i+1.  K tails / M tails / N tails rely on TMA
-// out-of-bounds zero fill (loads) and clipping (stores).
+// gemm_f16_wgmma, the staged kernel: persistent, tiles statically strided over the grid (tile = blockIdx.x + k *
+// gridDim.x, N fastest so concurrently running CTAs share the same A rows in L2).  Consumer warpgroup g issues wgmma
+// m64 x BLOCK_N x k16 for rows [64 (g-1), +64) of the 128-row tile and then runs the fused epilogue of those rows
+// itself: the accumulator fragment is staged through a warpgroup-private fp32 tile in shared memory so that the
+// epilogue functors see it as "thread = row" -- warp w of the warpgroup owns rows [32 (w & 1), +32) and the 64-column
+// block part = w >> 1 of the tile (BLOCK_N <= 128), lane = row; each 32-column chunk is handed to the functor.  While
+// the consumers run the epilogue of tile i the producer already streams the operands of tile i+1.  The step runs this
+// kernel for the embedding (BLOCK_N = 128) and the output projection (96), once per step each; the per-layer
+// projections run on gemm_f16_pingpong, which takes its epilogue from the accumulator fragment.
 #pragma once
 #include "ptx.cuh"
 
@@ -27,11 +29,75 @@ constexpr int GEMM_BLOCK_K = 64;  // 64 fp16 = 128 B = one swizzle row
 constexpr int GEMM_EPI_WARPS = 8;
 constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_BAR_BYTES = 1024;
-constexpr int GEMM_BIAS_BYTES = 8192;   // per-column epilogue vector (bias) of the whole GEMM, staged once per CTA: N <= 2048
+constexpr int GEMM_BIAS_BYTES = 8192;   // gemm_f16_pingpong: per-column epilogue vector (bias), staged once per CTA: N <= 2048
 
 // setmaxnreg: the producer warpgroup hands its registers to the consumers (40 + 2 x 232 <= 3 x 168, the pool of a
 // 384-thread CTA).  The values are the ones the measured numbers in DESIGN.md section 5 were taken with.
 constexpr int GEMM_REGS_PRODUCER = 40, GEMM_REGS_CONSUMER = 232;
+
+// Bytes from smem_raw, the start of the dynamic shared memory, to its first 1024-byte boundary (128B-swizzled boxes).
+// The kernels align by adding this offset to smem_raw itself, so that the compiler still sees shared-memory pointers
+// (LDS / STS rather than generic LD / ST) and 32-bit address arithmetic.
+__device__ __forceinline__ uint32_t smem_pad1024(const uint8_t* smem_raw) {
+  return (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
+}
+
+// Position in a STAGES-deep mbarrier ring: the stage and the parity of its current phase.  A consumer waits on the
+// stage's full barrier at `phase`, the producer on its empty barrier at `phase ^ 1` (the first pass finds it free).
+template <int STAGES>
+struct Ring {
+  int stage = 0;
+  uint32_t phase = 0;
+  Ring() = default;
+  __device__ __forceinline__ explicit Ring(int pos) : stage(pos % STAGES), phase((pos / STAGES) & 1) {}
+  __device__ __forceinline__ void advance() {
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  // the position n stages further on
+  __device__ __forceinline__ Ring ahead(int n) const {
+    Ring r(stage + n);
+    r.phase ^= phase;
+    return r;
+  }
+};
+
+// Producer: one tile's num_kb k-blocks into the ring, each once its stage is free -- the A box (rows from a_row) at the
+// start of the stage, the W box (rows from w_row) w_off bytes into it, stage_bytes in all on the stage's full barrier.
+// first() runs once the first k-block's stage is free.
+template <int STAGES, class First>
+__device__ __forceinline__ void produce_kblocks(Ring<STAGES>& ring, uint8_t* tiles, int stage_bytes, uint64_t* full_bar,
+                                                uint64_t* empty_bar, const CUtensorMap* map_a, int a_row,
+                                                const CUtensorMap* map_b, int w_off, int w_row, int num_kb, First&& first) {
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1);
+    if (kb == 0) first();
+    uint8_t* s = tiles + ring.stage * stage_bytes;
+    mbar_expect_tx(&full_bar[ring.stage], stage_bytes);
+    tma_load_2d(s, map_a, &full_bar[ring.stage], kb * GEMM_BLOCK_K, a_row);
+    tma_load_2d(s + w_off, map_b, &full_bar[ring.stage], kb * GEMM_BLOCK_K, w_row);
+    ring.advance();
+  }
+}
+
+// Consumer: for each of num_kb k-blocks, wait until its stage has landed, run mma(shared address of the stage, kb) --
+// one wgmma group with its accumulator fences: fence_acc, wgmma_fence, the MMAs (accumulating unless kb == 0 in the
+// first k16 step), wgmma_commit, fence_acc -- and, once that group leaves one in flight, release the stage of the
+// k-block before it (lane 0: one arrival per warp).  Returns the last k-block's stage, which the caller releases after
+// wgmma_wait<0>.
+template <int STAGES, class Mma>
+__device__ __forceinline__ int consume_kblocks(Ring<STAGES>& ring, const uint8_t* tiles, int stage_bytes,
+                                               uint64_t* full_bar, uint64_t* empty_bar, int num_kb, int lane, Mma&& mma) {
+  int prev_stage = -1;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&full_bar[ring.stage], ring.phase);
+    mma(smem_u32(tiles + ring.stage * stage_bytes), kb);
+    wgmma_wait<1>();
+    if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);   // the group that read it is done
+    prev_stage = ring.stage;
+    ring.advance();
+  }
+  return prev_stage;
+}
 
 template <int BLOCK_N>
 constexpr int gemm_stage_ld() { return BLOCK_N + 4; }   // fp32 row pitch of the staging tile (bank spread)
@@ -44,9 +110,9 @@ struct GemmSmem {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int ACC_BYTES = 2 * 64 * gemm_stage_ld<BLOCK_N>() * 4;   // one staging tile per consumer warpgroup
   static constexpr int EPI_BYTES = GEMM_EPI_WARPS * Epi::SMEM_PER_WARP;  // SMEM_PER_WARP is a multiple of 1024
-  static constexpr int budget = 227 * 1024 - 1024 /*alignment slack*/ - ACC_BYTES - EPI_BYTES - GEMM_BIAS_BYTES - GEMM_BAR_BYTES;
+  static constexpr int budget = 227 * 1024 - 1024 /*alignment slack*/ - ACC_BYTES - EPI_BYTES - GEMM_BAR_BYTES;
   static constexpr int STAGES = (budget / STAGE_BYTES) > 6 ? 6 : (budget / STAGE_BYTES);
-  static constexpr int TOTAL = 1024 + STAGES * STAGE_BYTES + EPI_BYTES + ACC_BYTES + GEMM_BIAS_BYTES + GEMM_BAR_BYTES;
+  static constexpr int TOTAL = 1024 + STAGES * STAGE_BYTES + EPI_BYTES + ACC_BYTES + GEMM_BAR_BYTES;
   static_assert(STAGES >= 2, "not enough shared memory for a pipeline");
   static_assert(Epi::SMEM_PER_WARP % 1024 == 0, "epilogue slabs must keep 1024-byte alignment (128B swizzle)");
   static_assert(B_BYTES % 1024 == 0, "W tiles must keep 1024-byte alignment (128B swizzle)");
@@ -55,12 +121,8 @@ struct GemmSmem {
 // Per-warp epilogue context handed to the functor (lives in registers for the whole persistent loop).
 struct EpiCtx {
   uint8_t* smem;        // warp-private slab, Epi::SMEM_PER_WARP bytes, 1024-byte aligned
-  const CUtensorMap* map_c;
-  const float* bias_all; // CTA-shared copy of the functor's per-column vector for columns [0, N)
   int lane;
-  int M, N;
-  int col_base;         // first column of the tile in flight
-  int col_end;          // first column after the tile in flight (col_base + BLOCK_N)
+  int M;
   uint32_t seq;         // running chunk / block counter (buffer rotation), functor-defined
 };
 
@@ -89,17 +151,12 @@ __device__ __forceinline__ void load_row32(const float* st, int row, int col, ui
 }
 
 // Epi interface (all static, called by every lane of a consumer warp, warp-uniform arguments):
-//   SMEM_PER_WARP                                   bytes of warp-private shared memory
-//   preload(p, dst, N, tid, nthreads)               stage the per-column vector once per CTA (before the first tile)
-//   tile_begin(ctx, p, row0, col_base)              before the tile's chunks
-//   chunk(ctx, p, v, row0, col0, next_col0)         v[32] = accumulator row (row0+lane), columns [col0, col0+32);
-//                                                   next_col0 = first column of this warp's next chunk in the tile, or -1
-//   tile_end(ctx, p, row0, col_base)                after the last chunk
-//   finish(ctx)                                     once, before the CTA exits (drain async stores)
+//   SMEM_PER_WARP                    bytes of warp-private shared memory
+//   chunk(ctx, p, v, row0, col0)     v[32] = accumulator row (row0+lane), columns [col0, col0+32)
+//   finish(ctx)                      once, before the CTA exits (drain async stores)
 template <int BLOCK_N, class Epi>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-               const __grid_constant__ CUtensorMap map_c, int M, int N, int K,
+gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, int M, int N, int K,
                const __grid_constant__ typename Epi::Params ep) {
   using SM = GemmSmem<BLOCK_N, Epi>;
   using MMA = Wgmma<BLOCK_N>;
@@ -108,12 +165,10 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   static_assert(BLOCK_N % 32 == 0, "epilogue works on 32-column chunks");
 
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* tiles = smem;
+  uint8_t* tiles = smem_raw + smem_pad1024(smem_raw);
   uint8_t* epi_smem = tiles + STAGES * SM::STAGE_BYTES;
   float* acc_stage = reinterpret_cast<float*>(epi_smem + SM::EPI_BYTES);
-  float* bias_all = reinterpret_cast<float*>(epi_smem + SM::EPI_BYTES + SM::ACC_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_smem + SM::EPI_BYTES + SM::ACC_BYTES + GEMM_BIAS_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_smem + SM::EPI_BYTES + SM::ACC_BYTES);
   uint64_t* full_bar = bars;                    // [STAGES]
   uint64_t* empty_bar = bars + STAGES;          // [STAGES]  one arrival per consumer warp
 
@@ -125,11 +180,9 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   const int num_kb = (K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
 
   pdl_launch_dependents();
-  Epi::preload(ep, bias_all, N, threadIdx.x, blockDim.x);   // visible to the consumers after the barrier below
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    tma_prefetch_desc(&map_c);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], GEMM_EPI_WARPS);
@@ -139,22 +192,15 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   __syncthreads();
   pdl_wait();   // the prologue above overlapped the previous kernel's tail; its outputs are visible from here on
 
+  Ring<STAGES> ring;   // this thread's position in the operand ring
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(GEMM_REGS_PRODUCER));
     // ------------------------------------------------------------ TMA producer
     if (warp == 0 && elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_blk = tile / tiles_n, n_blk = tile % tiles_n;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = tiles + stage * SM::STAGE_BYTES;
-          mbar_expect_tx(&full_bar[stage], SM::STAGE_BYTES);
-          tma_load_2d(sa, &map_a, &full_bar[stage], kb * GEMM_BLOCK_K, m_blk * GEMM_BLOCK_M);
-          tma_load_2d(sa + SM::A_BYTES, &map_b, &full_bar[stage], kb * GEMM_BLOCK_K, n_blk * BLOCK_N);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
+        produce_kblocks(ring, tiles, SM::STAGE_BYTES, full_bar, empty_bar, &map_a, m_blk * GEMM_BLOCK_M, &map_b,
+                        SM::A_BYTES, n_blk * BLOCK_N, num_kb, [] {});
       }
     }
   } else {
@@ -167,64 +213,43 @@ gemm_f16_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     float* st = acc_stage + wg * 64 * gemm_stage_ld<BLOCK_N>();
     EpiCtx ctx;
     ctx.smem = epi_smem + (warp - 4) * Epi::SMEM_PER_WARP;
-    ctx.map_c = &map_c;
-    ctx.bias_all = bias_all;
     ctx.lane = lane;
     ctx.M = M;
-    ctx.N = N;
     ctx.seq = 0;
-    int stage = 0;
-    uint32_t phase = 0;
     float acc[NREG];
+    auto mma = [&](uint32_t s, int kb) {
+      const uint64_t da = wgmma_desc_k_sw128(s + wg * 64 * 128);
+      const uint64_t db = wgmma_desc_k_sw128(s + SM::A_BYTES);
+      wgmma_fence_acc(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) MMA::mma(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+      wgmma_commit();
+      wgmma_fence_acc(acc);
+    };
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile / tiles_n, n_blk = tile % tiles_n;
       const int col_base = n_blk * BLOCK_N;
-      // ---- main loop: one wgmma group in flight while the next stage is awaited
-      int prev_stage = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_u32(tiles + stage * SM::STAGE_BYTES) + wg * 64 * 128;
-        const uint32_t sb = smem_u32(tiles + stage * SM::STAGE_BYTES) + SM::A_BYTES;
-        const uint64_t da = wgmma_desc_k_sw128(sa);
-        const uint64_t db = wgmma_desc_k_sw128(sb);
-        wgmma_fence_acc(acc);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) MMA::mma(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
-        wgmma_commit();
-        wgmma_fence_acc(acc);
-        wgmma_wait<1>();
-        if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);   // the group that read it is done
-        prev_stage = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
+      const int last_stage = consume_kblocks(ring, tiles, SM::STAGE_BYTES, full_bar, empty_bar, num_kb, lane, mma);
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
-      if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      if (lane == 0) mbar_arrive(&empty_bar[last_stage]);
       // ---- epilogue
       const int row0 = m_blk * GEMM_BLOCK_M + 64 * wg + rh;
       const bool live = row0 < M;  // warp-uniform: this warp's 32 rows exist
-      ctx.col_base = col_base;
-      ctx.col_end = col_base + BLOCK_N;
-      if (live) Epi::tile_begin(ctx, ep, row0, col_base);
       uint32_t raw[32];
-      auto run = [&](int c, int cn) {
+      auto run = [&](int c) {
         if (live && col_base + c < N) {
           load_row32<BLOCK_N>(st, rh + lane, c, raw);
-          Epi::chunk(ctx, ep, raw, row0, col_base + c, (cn < BLOCK_N && col_base + cn < N) ? col_base + cn : -1);
+          Epi::chunk(ctx, ep, raw, row0, col_base + c);
         }
       };
       named_bar_sync(1 + wg, 128);   // the previous tile's staging tile has been read by every warp of the warpgroup
       stage_acc<BLOCK_N>(st, acc, wq, lane);
       named_bar_sync(1 + wg, 128);
-      const int c = part * 64;   // this warp owns one 64-column block of the tile
-      if (c < BLOCK_N) {
-        const bool two = c + 32 < BLOCK_N;                     // (BLOCK_N = 96: the last block is a single chunk)
-        const int cnext = c + 128;
-        run(c, two ? c + 32 : cnext);
-        if (two) run(c + 32, cnext);
-      }
-      if (live) Epi::tile_end(ctx, ep, row0, col_base);
+      const int c = part * 64;   // this warp owns one 64-column block of the tile (BLOCK_N = 96: the last is one chunk)
+      if (c < BLOCK_N) run(c);
+      if (c + 32 < BLOCK_N) run(c + 32);
     }
     Epi::finish(ctx);
   }

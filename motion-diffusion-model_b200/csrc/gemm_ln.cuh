@@ -4,12 +4,14 @@
 //     (post-norm nn.TransformerEncoderLayer of the reference, built at model/mdm.py:77-84)
 //
 // Both CTAs of a cluster work on the SAME 128 rows; CTA r owns columns [256 r, 256 r + 256) (its own 256 rows of W).
-// Warpgroup 0 is the TMA producer; consumer warpgroup g (1, 2) issues wgmma m64n256k16 for rows [64 (g-1), +64) and
-// keeps its 64 x 256 fp32 accumulator in registers (128 per thread) for the whole epilogue.
+// The operand pipeline is gemm.cuh's: warpgroup 0 is the TMA producer; consumer warpgroup g (1, 2) issues wgmma
+// m64n256k16 for rows [64 (g-1), +64) and keeps its 64 x 256 fp32 accumulator in registers (128 per thread) for the
+// whole epilogue.
 //
 // The residual moves only as bulk TMA traffic.  After a tile's last k-block the producer loads the CTA's 256 residual
 // columns as four 64-column groups, each a 128-row hi box + the matching lo box (2 x 16 KB, 128-byte swizzle), into the
-// next four stages of the operand ring, so the loads overlap the tail of the mainloop.  Epilogue:
+// next four stages of the operand ring (the same Ring: group grp at ring.ahead(grp)), so the loads overlap the tail of
+// the mainloop.  Epilogue:
 //   pass 1    v = acc + bias + residual (read from the swizzled slab in the accumulator's fragment layout: the 8 rows of a
 //             quad group land on distinct 16-byte chunks, no bank conflicts), kept in the accumulator registers;
 //             per-row partial sum / sum of squares over the CTA's 256 columns (quad shuffles)
@@ -77,10 +79,8 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GLN_THREADS, 1)
 gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                       const __grid_constant__ CUtensorMap map_h, int M, int K, const GemmLnParams lp) {
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment as an offset from smem_raw, so that the compiler still sees shared-memory pointers (LDS / STS)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* tiles = smem;
-  float* prm = reinterpret_cast<float*>(smem + GLN_STAGES * GLN_STAGE_BYTES);   // bias | gamma | beta  (this CTA's 256 cols)
+  uint8_t* tiles = smem_raw + smem_pad1024(smem_raw);
+  float* prm = reinterpret_cast<float*>(tiles + GLN_STAGES * GLN_STAGE_BYTES);   // bias | gamma | beta  (this CTA's 256 cols)
   float2* st_remote = reinterpret_cast<float2*>(prm + 3 * GLN_BN);             // [2 stages][128 rows], written by the PEER
   uint64_t* bars = reinterpret_cast<uint64_t*>(st_remote + 256);
   uint64_t* full_bar = bars;                       // [STAGES]
@@ -122,34 +122,27 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(GLN_REGS_PRODUCER));
     // ------------------------------------------------------------ TMA producer
     if (warp == 0 && elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
+      Ring<GLN_STAGES> ring;
       for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
         GLN_STAMP(true, (tile - cluster_id) / num_clusters, 0, 0);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          GLN_STAMP(kb == 0, (tile - cluster_id) / num_clusters, 0, 1);
-          uint8_t* sa = tiles + stage * GLN_STAGE_BYTES;
-          mbar_expect_tx(&full_bar[stage], GLN_STAGE_BYTES);
-          tma_load_2d(sa, &map_a, &full_bar[stage], kb * GEMM_BLOCK_K, tile * GEMM_BLOCK_M);
-          tma_load_2d(sa + 16384, &map_b, &full_bar[stage], kb * GEMM_BLOCK_K, col_cta);
-          if (++stage == GLN_STAGES) { stage = 0; phase ^= 1; }
-        }
+        produce_kblocks(ring, tiles, GLN_STAGE_BYTES, full_bar, empty_bar, &map_a, tile * GEMM_BLOCK_M, &map_b, 16384,
+                        col_cta, num_kb, [&] { GLN_STAMP(true, (tile - cluster_id) / num_clusters, 0, 1); });
         // the tile's residual, group by group, into the next ring stages (hi slab | lo slab)
         const int r0 = tile * GEMM_BLOCK_M;
         const bool two = r0 + GLN_RES_BOX_ROWS < M;   // the second warpgroup's rows exist
         for (int grp = 0; grp < GLN_GROUPS; ++grp) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sr = tiles + stage * GLN_STAGE_BYTES;
+          mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1);
+          uint64_t* fb = &full_bar[ring.stage];
+          uint8_t* sr = tiles + ring.stage * GLN_STAGE_BYTES;
           const int c = col_cta + 64 * grp;
-          mbar_expect_tx(&full_bar[stage], (two ? 4 : 2) * GLN_RES_BOX_BYTES);
-          tma_load_2d(sr, &map_h, &full_bar[stage], c, r0);
-          tma_load_2d(sr + GLN_RES_HALF, &map_h, &full_bar[stage], GLN_D + c, r0);
+          mbar_expect_tx(fb, (two ? 4 : 2) * GLN_RES_BOX_BYTES);
+          tma_load_2d(sr, &map_h, fb, c, r0);
+          tma_load_2d(sr + GLN_RES_HALF, &map_h, fb, GLN_D + c, r0);
           if (two) {
-            tma_load_2d(sr + GLN_RES_BOX_BYTES, &map_h, &full_bar[stage], c, r0 + GLN_RES_BOX_ROWS);
-            tma_load_2d(sr + GLN_RES_HALF + GLN_RES_BOX_BYTES, &map_h, &full_bar[stage], GLN_D + c, r0 + GLN_RES_BOX_ROWS);
+            tma_load_2d(sr + GLN_RES_BOX_BYTES, &map_h, fb, c, r0 + GLN_RES_BOX_ROWS);
+            tma_load_2d(sr + GLN_RES_HALF + GLN_RES_BOX_BYTES, &map_h, fb, GLN_D + c, r0 + GLN_RES_BOX_ROWS);
           }
-          if (++stage == GLN_STAGES) { stage = 0; phase ^= 1; }
+          ring.advance();
         }
         GLN_STAMP(true, (tile - cluster_id) / num_clusters, 0, 2);
       }
@@ -169,50 +162,41 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
     const float* bias_s = prm;
     const float* gamma_s = prm + GLN_BN;
     const float* beta_s = prm + 2 * GLN_BN;
-    int stage = 0;
-    uint32_t phase = 0;
+    Ring<GLN_STAGES> ring;
     float acc[128];
     int it = 0;
+    auto mma = [&](uint32_t s, int kb) {
+      GLN_STAMP(kb == 0 && store_thread, it, 1 + wg, 1);
+      const uint64_t da = wgmma_desc_k_sw128(s + wg * 64 * 128);
+      const uint64_t db = wgmma_desc_k_sw128(s + 16384);
+      wgmma_fence_acc(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) Wgmma<256>::mma(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+      wgmma_commit();
+      wgmma_fence_acc(acc);
+    };
     for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++it) {
       const int as = it & 1;
       const uint32_t aphase = (it >> 1) & 1;
       if (lane == 0) mbar_expect_tx(&xbar[as * 8 + cw], 16 * 8);   // the peer's partials of this warp's 16 rows
       GLN_STAMP(store_thread, it, 1 + wg, 0);
-      int prev_stage = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        GLN_STAMP(kb == 0 && store_thread, it, 1 + wg, 1);
-        const uint32_t sa = smem_u32(tiles + stage * GLN_STAGE_BYTES);
-        const uint64_t da = wgmma_desc_k_sw128(sa + wg * 64 * 128);
-        const uint64_t db = wgmma_desc_k_sw128(sa + 16384);
-        wgmma_fence_acc(acc);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) Wgmma<256>::mma(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
-        wgmma_commit();
-        wgmma_fence_acc(acc);
-        wgmma_wait<1>();
-        if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-        prev_stage = stage;
-        if (++stage == GLN_STAGES) { stage = 0; phase ^= 1; }
-      }
+      const int last_stage = consume_kblocks(ring, tiles, GLN_STAGE_BYTES, full_bar, empty_bar, num_kb, lane, mma);
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
       GLN_STAMP(store_thread, it, 1 + wg, 2);
-      if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-      // the residual groups sit in the next GLN_GROUPS ring stages: group grp in stage (rs0 + grp) % GLN_STAGES
-      const int rs0 = stage;
-      const uint32_t rph0 = phase;
+      if (lane == 0) mbar_arrive(&empty_bar[last_stage]);
+      // the residual groups sit in the next GLN_GROUPS ring stages: group grp at ring.ahead(grp)
 
       // ---- pass 1: v = residual + (acc + bias) in place, partial statistics of the two rows
       float sa = 0.f, qa = 0.f, sb = 0.f, qb = 0.f;
 #pragma unroll
       for (int j = 0; j < GLN_BN / 8; ++j) {
         const int grp = j >> 3, jj = j & 7;
-        const int rs = (rs0 + grp) % GLN_STAGES;
-        if (jj == 0) mbar_wait(&full_bar[rs], rph0 ^ (rs0 + grp >= GLN_STAGES ? 1u : 0u));
+        const Ring<GLN_STAGES> rg = ring.ahead(grp);
+        if (jj == 0) mbar_wait(&full_bar[rg.stage], rg.phase);
         GLN_STAMP(jj == 0 && (grp == 0 || grp == GLN_GROUPS - 1) && store_thread, it, 1 + wg, grp == 0 ? 3 : 4);
-        const uint8_t* slab = tiles + rs * GLN_STAGE_BYTES + toff + ((jj ^ g) << 4);
+        const uint8_t* slab = tiles + rg.stage * GLN_STAGE_BYTES + toff + ((jj ^ g) << 4);
         const int c = 8 * j + 2 * t;                   // local column of acc[4j], acc[4j+1] (and of acc[4j+2..3], row b)
         const float2 bb = *reinterpret_cast<const float2*>(bias_s + c);
         float2 ra, rb;
@@ -261,7 +245,7 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
 #pragma unroll
       for (int j = 0; j < GLN_BN / 8; ++j) {
         const int grp = j >> 3, jj = j & 7;
-        const int rs = (rs0 + grp) % GLN_STAGES;
+        const int rs = ring.ahead(grp).stage;
         uint8_t* slab = tiles + rs * GLN_STAGE_BYTES + toff + ((jj ^ g) << 4);
         const int c = 8 * j + 2 * t;
         const float2 gg = *reinterpret_cast<const float2*>(gamma_s + c);
@@ -298,8 +282,7 @@ gemm_resid_ln_cluster(const __grid_constant__ CUtensorMap map_a, const __grid_co
           }
         }
       }
-      for (int grp = 0; grp < GLN_GROUPS; ++grp)
-        if (++stage == GLN_STAGES) { stage = 0; phase ^= 1; }
+      ring = ring.ahead(GLN_GROUPS);
     }
     if (store_thread) bulk_wait_group<0>();   // the last stores have landed before the CTA exits
   }

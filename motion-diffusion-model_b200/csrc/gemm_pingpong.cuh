@@ -1,7 +1,6 @@
 // Projection GEMM with the epilogue under the MMAs, sm_90a:   out = epi(A[M,K] * W[N,K]^T)   (fp16 in, fp32 accumulate)
 //
-//   warpgroup 0      : TMA producer, exactly as in gemm.cuh (one elected thread, 128B-swizzled A and W tiles, one
-//                      PP_STAGES-deep mbarrier ring filled in tile order)
+//   warpgroup 0      : the TMA producer of gemm.cuh, filling one PP_STAGES-deep ring in tile order
 //   warpgroups 1, 2  : consumers.  Each owns a WHOLE 128 x 128 tile: two wgmma.m64n128k16 per k16 step (rows [0, 64) and
 //                      [64, 128) of the tile against the same W tile), 128 fp32 accumulators per thread.
 //
@@ -48,9 +47,7 @@ gemm_f16_pingpong(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   static_assert(RC == 64 || RC == 128, "a round is one or two 64-column slabs");
 
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment as an offset from smem_raw, so that the compiler still sees shared-memory pointers (LDS / STS)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* tiles = smem;
+  uint8_t* tiles = smem_raw + smem_pad1024(smem_raw);
   uint8_t* slabs = tiles + PP_STAGES * PP_STAGE_BYTES;
   float* bias_all = reinterpret_cast<float*>(slabs + 2 * PP_SLAB_BYTES);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(slabs + 2 * PP_SLAB_BYTES + GEMM_BIAS_BYTES);   // [STAGES]
@@ -83,19 +80,12 @@ gemm_f16_pingpong(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(GEMM_REGS_PRODUCER));
     // ------------------------------------------------------------ TMA producer
     if (warp == 0 && elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
+      Ring<PP_STAGES> ring;
       for (int i = 0; i < my_tiles; ++i) {
         const int tile = blockIdx.x + i * gridDim.x;
         const int m_blk = tile / tiles_n, n_blk = tile % tiles_n;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = tiles + stage * PP_STAGE_BYTES;
-          mbar_expect_tx(&full_bar[stage], PP_STAGE_BYTES);
-          tma_load_2d(sa, &map_a, &full_bar[stage], kb * GEMM_BLOCK_K, m_blk * GEMM_BLOCK_M);
-          tma_load_2d(sa + PP_A_BYTES, &map_b, &full_bar[stage], kb * GEMM_BLOCK_K, n_blk * PP_BLOCK_N);
-          if (++stage == PP_STAGES) { stage = 0; phase ^= 1; }
-        }
+        produce_kblocks(ring, tiles, PP_STAGE_BYTES, full_bar, empty_bar, &map_a, m_blk * GEMM_BLOCK_M, &map_b, PP_A_BYTES,
+                        n_blk * PP_BLOCK_N, num_kb, [] {});
       }
     }
   } else {
@@ -110,42 +100,33 @@ gemm_f16_pingpong(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     // the second 64-row half: +8192)
     const int toff = (16 * wq + g) * 128 + 4 * t;
     float acc0[64], acc1[64];   // rows [0, 64) and [64, 128) of the tile
+    auto mma = [&](uint32_t s, int kb) {
+      const uint64_t da0 = wgmma_desc_k_sw128(s);
+      const uint64_t da1 = wgmma_desc_k_sw128(s + 64 * 128);
+      const uint64_t db = wgmma_desc_k_sw128(s + PP_A_BYTES);
+      wgmma_fence_acc(acc0);
+      wgmma_fence_acc(acc1);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
+        Wgmma<128>::mma(acc0, da0 + 2 * k, db + 2 * k, (kb | k) != 0);
+        Wgmma<128>::mma(acc1, da1 + 2 * k, db + 2 * k, (kb | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_fence_acc(acc0);
+      wgmma_fence_acc(acc1);
+    };
     for (int i = wg; i < my_tiles; i += 2) {
       const int tile = blockIdx.x + i * gridDim.x;
       const int m_blk = tile / tiles_n, n_blk = tile % tiles_n;
-      const int pos = i * num_kb;   // ring position of the tile's first k-block
-      int stage = pos % PP_STAGES;
-      uint32_t phase = (pos / PP_STAGES) & 1;
+      Ring<PP_STAGES> ring(i * num_kb);   // the tile's first k-block
       if (i > 0) named_bar_sync(PP_BAR_TURN + wg, 256);   // the other warpgroup has issued tile i - 1
-      // ---- main loop: one wgmma group in flight while the next stage is awaited
-      int prev_stage = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_u32(tiles + stage * PP_STAGE_BYTES);
-        const uint64_t da0 = wgmma_desc_k_sw128(sa);
-        const uint64_t da1 = wgmma_desc_k_sw128(sa + 64 * 128);
-        const uint64_t db = wgmma_desc_k_sw128(sa + PP_A_BYTES);
-        wgmma_fence_acc(acc0);
-        wgmma_fence_acc(acc1);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
-          Wgmma<128>::mma(acc0, da0 + 2 * k, db + 2 * k, (kb | k) != 0);
-          Wgmma<128>::mma(acc1, da1 + 2 * k, db + 2 * k, (kb | k) != 0);
-        }
-        wgmma_commit();
-        wgmma_fence_acc(acc0);
-        wgmma_fence_acc(acc1);
-        wgmma_wait<1>();
-        if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);   // the group that read it is done
-        prev_stage = stage;
-        if (++stage == PP_STAGES) { stage = 0; phase ^= 1; }
-      }
+      const int last_stage = consume_kblocks(ring, tiles, PP_STAGE_BYTES, full_bar, empty_bar, num_kb, lane, mma);
       if (i + 1 < my_tiles) named_bar_arrive(PP_BAR_TURN + (wg ^ 1), 256);   // hand the ring to the other warpgroup
       wgmma_wait<0>();
       wgmma_fence_acc(acc0);
       wgmma_fence_acc(acc1);
-      if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      if (lane == 0) mbar_arrive(&empty_bar[last_stage]);
       // ---- epilogue, in rounds of RC columns
       const int row_t = m_blk * GEMM_BLOCK_M, col_t = n_blk * PP_BLOCK_N;
       // (an epilogue that writes its scratch does so after this warpgroup's last read of the previous tile's bias: the
