@@ -11,6 +11,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <map>
 #include <string>
 #include <vector>
@@ -108,6 +109,16 @@ static int make_map_res(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t
 }
 
 // ------------------------------------------------------------------------------------------------ engine
+// The schedule's row tables, one row per schedule index: the step table (b200mdm_set_schedule), the DDIM inversion's
+// sqrt(abn), sqrt(1 - abn), DPM-Solver++'s c_x, c0, c_cur, c_prev and the variational bound's VB_* columns.
+enum SchedTable { TAB_STEP, TAB_NEXT, TAB_DPM, TAB_VB, N_TABLES };
+static constexpr int TAB_STRIDE[N_TABLES] = {SCHED_STRIDE, SCHED_NEXT_STRIDE, SCHED_DPM_STRIDE, SCHED_VB_STRIDE};
+static const char* const TAB_SETTER[N_TABLES] = {"b200mdm_set_schedule", "b200mdm_set_schedule_next",
+                                                 "b200mdm_set_schedule_dpm", "b200mdm_set_schedule_vb"};
+static_assert(SCHED_STRIDE == B200MDM_SCHED_STRIDE && SCHED_NEXT_STRIDE == B200MDM_SCHED_NEXT_STRIDE &&
+                  SCHED_DPM_STRIDE == B200MDM_SCHED_DPM_STRIDE && SCHED_VB_STRIDE == B200MDM_SCHED_VB_STRIDE,
+              "the tables' row layouts are part of the ABI");
+
 struct Tensor32 {
   float* dev = nullptr;
   std::vector<int64_t> shape;
@@ -215,21 +226,12 @@ struct b200mdm_engine : Workspace {
   float *tw0 = nullptr, *tb0 = nullptr, *twk = nullptr, *tbk = nullptr, *twsum = nullptr;
   int tG = 0, tdj = 0, tin = 0, tlayers = 0;
   std::vector<float> h_valid;
-  // schedule (device tables are allocated once at `sched_cap` rows: the step graphs hold these pointers)
-  float* sched = nullptr;
+  // schedule: the row tables (SchedTable) and the timestep map, allocated once at `sched_cap` rows (the step graphs
+  // hold these pointers).  Every b200mdm_set_schedule makes the tables after TAB_STEP stale until their own setter.
+  float* tab[N_TABLES] = {};
+  bool tab_fresh[N_TABLES] = {};
   int* tmap = nullptr;
   int n_steps = 0, sched_cap = 0;
-  // DDIM inversion: sqrt(abn), sqrt(1 - abn) per row (b200mdm_set_schedule_next), allocated with `sched`; every
-  // b200mdm_set_schedule makes it stale until the next b200mdm_set_schedule_next
-  float* sched_next = nullptr;
-  bool sched_next_fresh = false;
-  // DPM-Solver++: c_x, c0, c_cur, c_prev per row (b200mdm_set_schedule_dpm), allocated with `sched`, stale in the same
-  // way as sched_next
-  float* sched_dpm = nullptr;
-  bool sched_dpm_fresh = false;
-  // variational bound: the VB_* columns per row (b200mdm_set_schedule_vb), allocated with `sched`, stale in the same way
-  float* sched_vb = nullptr;
-  bool sched_vb_fresh = false;
   // parked workspaces (see Workspace)
   std::vector<Workspace> pool;
   unsigned long long use_clock = 0;
@@ -664,8 +666,8 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   free_all_workspaces(e);
   for (auto& kv : e->store) cudaFree(kv.second.dev);
   free_repacks(e);
-  dfree(e->sched); dfree(e->tmap); dfree(e->sched_next); dfree(e->sched_dpm);
-  dfree(e->sched_vb);
+  for (float*& t : e->tab) dfree(t);
+  dfree(e->tmap);
   dfree(e->chain_mem); dfree(e->chain_mask); dfree(e->chain_prefix);
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
@@ -975,69 +977,58 @@ extern "C" int b200mdm_set_schedule(b200mdm_engine* e, int32_t n_steps, const fl
   if (n_steps > e->sched_cap) {
     // the captured step graphs hold these pointers as kernel parameters: moving the tables invalidates every graph
     drop_all_graphs(e);
-    dfree(e->sched);
+    for (float*& t : e->tab) dfree(t);
     dfree(e->tmap);
-    dfree(e->sched_next);
-    dfree(e->sched_dpm);
-    dfree(e->sched_vb);
     e->sched_cap = 0;
     const int cap = n_steps > 1000 ? n_steps : 1000;
-    TRY(dalloc(&e->sched, static_cast<size_t>(cap) * SCHED_STRIDE));
+    for (int t = 0; t < N_TABLES; ++t) TRY(dalloc(&e->tab[t], static_cast<size_t>(cap) * TAB_STRIDE[t]));
     TRY(dalloc(&e->tmap, cap));
-    TRY(dalloc(&e->sched_next, static_cast<size_t>(cap) * SCHED_NEXT_STRIDE));
-    TRY(dalloc(&e->sched_dpm, static_cast<size_t>(cap) * SCHED_DPM_STRIDE));
-    TRY(dalloc(&e->sched_vb, static_cast<size_t>(cap) * SCHED_VB_STRIDE));
     e->sched_cap = cap;
   }
   e->n_steps = n_steps;
-  e->sched_next_fresh = false;
-  e->sched_dpm_fresh = false;
-  e->sched_vb_fresh = false;
-  CUDA_TRY(cudaMemcpy(e->sched, rows_host, static_cast<size_t>(n_steps) * SCHED_STRIDE * sizeof(float), cudaMemcpyHostToDevice));
+  for (int t = 0; t < N_TABLES; ++t) e->tab_fresh[t] = t == TAB_STEP;
+  CUDA_TRY(cudaMemcpy(e->tab[TAB_STEP], rows_host, static_cast<size_t>(n_steps) * SCHED_STRIDE * sizeof(float),
+                      cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(e->tmap, timestep_map_host, static_cast<size_t>(n_steps) * sizeof(int), cudaMemcpyHostToDevice));
   return B200MDM_OK;
 }
 
-static_assert(SCHED_NEXT_STRIDE == B200MDM_SCHED_NEXT_STRIDE, "the reverse table's row layout is part of the ABI");
+// The rows of table `which` for the current schedule (b200mdm_set_schedule_next / _dpm / _vb).
+static int upload_table(b200mdm_engine* e, SchedTable which, int32_t n_steps, const float* rows_host) {
+  if (!e || !rows_host) return fail(B200MDM_EINVAL, "bad argument");
+  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
+  if (n_steps != e->n_steps)
+    return fail(B200MDM_EINVAL, "n_steps %d differs from the schedule's %d", n_steps, e->n_steps);
+  CUDA_TRY(cudaDeviceSynchronize());  // a loop still in flight may be reading the old rows
+  CUDA_TRY(cudaMemcpy(e->tab[which], rows_host, static_cast<size_t>(n_steps) * TAB_STRIDE[which] * sizeof(float),
+                      cudaMemcpyHostToDevice));
+  e->tab_fresh[which] = true;
+  return B200MDM_OK;
+}
+// ESTATE unless table `which` has been uploaded for the current schedule.
+static int need_table(const b200mdm_engine* e, SchedTable which) {
+  if (e->tab_fresh[which]) return B200MDM_OK;
+  return fail(B200MDM_ESTATE, "%s has not been called for the current schedule", TAB_SETTER[which]);
+}
+// The output epilogue's pointer to each table.
+static void set_tables(EpiOutParams* p, float* const (&tab)[N_TABLES]) {
+  p->sched = tab[TAB_STEP];
+  p->sched_next = tab[TAB_NEXT];
+  p->sched_dpm = tab[TAB_DPM];
+  p->sched_vb = tab[TAB_VB];
+}
+
 static_assert(MODE_X0 == B200MDM_MODE_X0 && MODE_DDPM == B200MDM_MODE_DDPM && MODE_DDIM == B200MDM_MODE_DDIM &&
                   MODE_DDIM_REVERSE == B200MDM_MODE_DDIM_REVERSE,
               "the output epilogue's modes are the public ones");
 extern "C" int b200mdm_set_schedule_next(b200mdm_engine* e, int32_t n_steps, const float* rows_host) {
-  if (!e || !rows_host) return fail(B200MDM_EINVAL, "bad argument");
-  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
-  if (n_steps != e->n_steps)
-    return fail(B200MDM_EINVAL, "n_steps %d differs from the schedule's %d", n_steps, e->n_steps);
-  CUDA_TRY(cudaDeviceSynchronize());  // a reverse loop still in flight may be reading the old rows
-  CUDA_TRY(cudaMemcpy(e->sched_next, rows_host, static_cast<size_t>(n_steps) * SCHED_NEXT_STRIDE * sizeof(float),
-                      cudaMemcpyHostToDevice));
-  e->sched_next_fresh = true;
-  return B200MDM_OK;
+  return upload_table(e, TAB_NEXT, n_steps, rows_host);
 }
-
-static_assert(SCHED_DPM_STRIDE == B200MDM_SCHED_DPM_STRIDE, "the DPM-Solver++ table's row layout is part of the ABI");
 extern "C" int b200mdm_set_schedule_dpm(b200mdm_engine* e, int32_t n_steps, const float* rows_host) {
-  if (!e || !rows_host) return fail(B200MDM_EINVAL, "bad argument");
-  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
-  if (n_steps != e->n_steps)
-    return fail(B200MDM_EINVAL, "n_steps %d differs from the schedule's %d", n_steps, e->n_steps);
-  CUDA_TRY(cudaDeviceSynchronize());  // a DPM loop still in flight may be reading the old rows
-  CUDA_TRY(cudaMemcpy(e->sched_dpm, rows_host, static_cast<size_t>(n_steps) * SCHED_DPM_STRIDE * sizeof(float),
-                      cudaMemcpyHostToDevice));
-  e->sched_dpm_fresh = true;
-  return B200MDM_OK;
+  return upload_table(e, TAB_DPM, n_steps, rows_host);
 }
-
-static_assert(SCHED_VB_STRIDE == B200MDM_SCHED_VB_STRIDE, "the bound table's row layout is part of the ABI");
 extern "C" int b200mdm_set_schedule_vb(b200mdm_engine* e, int32_t n_steps, const float* rows_host) {
-  if (!e || !rows_host) return fail(B200MDM_EINVAL, "bad argument");
-  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
-  if (n_steps != e->n_steps)
-    return fail(B200MDM_EINVAL, "n_steps %d differs from the schedule's %d", n_steps, e->n_steps);
-  CUDA_TRY(cudaDeviceSynchronize());  // a bound loop still in flight may be reading the old rows
-  CUDA_TRY(cudaMemcpy(e->sched_vb, rows_host, static_cast<size_t>(n_steps) * SCHED_VB_STRIDE * sizeof(float),
-                      cudaMemcpyHostToDevice));
-  e->sched_vb_fresh = true;
-  return B200MDM_OK;
+  return upload_table(e, TAB_VB, n_steps, rows_host);
 }
 
 // ------------------------------------------------------------------------------------------------ cond / workspace
@@ -1528,7 +1519,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     ++nk;
   }
   if (a.mode == MODE_VB) {   // x_t = q_sample(x_start, i, eps): the denoiser's input
-    TRY(launch_vb_xt(e->x_work, e->vb_xs, a.noise, e->sched_vb, e->state, static_cast<size_t>(B) * JF * T, s));
+    TRY(launch_vb_xt(e->x_work, e->vb_xs, a.noise, e->tab[TAB_VB], e->state, static_cast<size_t>(B) * JF * T, s));
     ++nk;
   }
   TRY(launch_pack_input(a.x_in, e->xin16, B, JF, T, S, Kp, e->s_off, s));
@@ -1615,12 +1606,9 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     p.inpaint_mask = a.model_only ? nullptr : e->inpaint_mask;
     p.inpaint_weight = a.model_only ? nullptr : e->inpaint_weight;
     p.inpaint_motion = a.model_only ? nullptr : e->inpaint_motion;
-    p.sched = e->sched;
-    p.sched_next = e->sched_next;
-    p.sched_dpm = e->sched_dpm;
+    set_tables(&p, e->tab);
     p.eps_ring = e->plms_ring;
     p.x0_hist = e->dpm_hist;
-    p.sched_vb = e->sched_vb;
     p.x_start = e->vb_xs;
     p.vb_part = e->vb_part;
     p.state = e->state;
@@ -1642,6 +1630,14 @@ static int check_ready(b200mdm_engine* e, bool need_sched) {
   if (e->dec && e->ctx > 0 && !e->prefix_set) return fail(B200MDM_ESTATE, "b200mdm_set_prefix has not been called (y['prefix'])");
   if (need_sched && e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
   return B200MDM_OK;
+}
+
+// EINVAL unless flags holds nothing outside `allowed`: B200MDM_FLAG_CLIP_DENOISED, with or without
+// B200MDM_FLAG_PHILOX_NOISE.
+static int check_flags(const char* family, int32_t flags, int32_t allowed) {
+  if (!(flags & ~allowed)) return B200MDM_OK;
+  return fail(B200MDM_EINVAL, "%s takes no flag but B200MDM_FLAG_CLIP_DENOISED%s", family,
+              (allowed & B200MDM_FLAG_PHILOX_NOISE) ? " and B200MDM_FLAG_PHILOX_NOISE" : "");
 }
 
 static int check_timesteps(const b200mdm_engine* e, const int32_t* timesteps_host) {
@@ -1707,11 +1703,11 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
   if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM && !reverse) return fail(B200MDM_EINVAL, "bad mode");
   if (index < 0 || index >= e->n_steps) return fail(B200MDM_EINVAL, "schedule index out of range");
   if (!x_t_dev || (!noise_dev && !reverse) || !x_out_dev) return fail(B200MDM_EINVAL, "null tensor");
-  if (reverse && (flags & ~B200MDM_FLAG_CLIP_DENOISED))
-    return fail(B200MDM_EINVAL, "DDIM inversion takes no flag but B200MDM_FLAG_CLIP_DENOISED");
-  if (reverse && !e->sched_next_fresh)
-    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_next has not been called for the current schedule");
-  if (reverse && e->hs_set) return fail(B200MDM_ENOTIMPL, "DDIM inversion with handshakes is not implemented");
+  if (reverse) {
+    TRY(check_flags("DDIM inversion", flags, B200MDM_FLAG_CLIP_DENOISED));
+    TRY(need_table(e, TAB_NEXT));
+    if (e->hs_set) return fail(B200MDM_ENOTIMPL, "DDIM inversion with handshakes is not implemented");
+  }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, index, nullptr, 0, e->noise_seed, e->noise_sample_base, e->n_steps);
   CUDA_TRY(cudaGetLastError());
@@ -1862,26 +1858,53 @@ static int run_loop(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32_t
   return loop_leave(e, use_graph, user);
 }
 
-// Schedule indices first_index, first_index-1, ... (n_run of them) on the engine's working buffer.
-extern "C" int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_t first_index, int32_t n_run,
-                                         const float* x_in_dev, float* x_out_dev, const float* noise_tape_dev,
-                                         int64_t noise_step_stride, int32_t flags, int32_t use_graph, void* stream) {
-  TRY(check_ready(e, true));
-  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM) return fail(B200MDM_EINVAL, "bad mode");
+// EINVAL unless schedule indices first_index, first_index - 1, ... (n_run of them) exist.
+static int check_range_down(const b200mdm_engine* e, int32_t first_index, int32_t n_run) {
   if (n_run <= 0 || first_index >= e->n_steps || first_index - n_run + 1 < 0) return fail(B200MDM_EINVAL, "bad step range");
-  const bool philox = (flags & B200MDM_FLAG_PHILOX_NOISE) != 0;
-  if (!philox && !noise_tape_dev) return fail(B200MDM_EINVAL, "null noise tape (or pass B200MDM_FLAG_PHILOX_NOISE)");
-  // The loop runs in place on an engine-owned buffer (fixed address => the captured step graph never changes);
-  // every element is read and written by the same thread of the fused output epilogue.
+  return B200MDM_OK;
+}
+
+// The StepArgs of a loop of `mode`.  The loop runs in place on an engine-owned buffer (fixed address => the captured
+// step graph never changes); every element is read and written by the same thread of the fused output epilogue.
+static StepArgs loop_args(b200mdm_engine* e, int mode, int order, int32_t flags, bool philox) {
   StepArgs a;
   a.mode = mode;
+  a.order = order;
   a.x_in = e->x_work;
   a.x_out = e->x_work;
   a.noise = philox ? e->eps_buf : nullptr;
   a.philox = philox;
   a.const_noise = flags & B200MDM_FLAG_CONST_NOISE;
   a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-  return run_loop(e, a, flags, first_index, n_run, x_in_dev, x_out_dev, noise_tape_dev, noise_step_stride, use_graph, stream);
+  return a;
+}
+
+// A loop's device buffers, all or nothing: each null pointer gets its n floats; after a failure every one of them is
+// freed, so that no later call finds a partial set.
+struct LoopBuf {
+  float** p;
+  size_t n;
+};
+static int alloc_all(std::initializer_list<LoopBuf> bufs) {
+  int r = B200MDM_OK;
+  for (const LoopBuf& b : bufs)
+    if (r == B200MDM_OK && !*b.p) r = dalloc(b.p, b.n);
+  if (r != B200MDM_OK)
+    for (const LoopBuf& b : bufs) dfree(*b.p);
+  return r;
+}
+
+// Schedule indices first_index, first_index-1, ... (n_run of them) on the engine's working buffer.
+extern "C" int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_t first_index, int32_t n_run,
+                                         const float* x_in_dev, float* x_out_dev, const float* noise_tape_dev,
+                                         int64_t noise_step_stride, int32_t flags, int32_t use_graph, void* stream) {
+  TRY(check_ready(e, true));
+  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM) return fail(B200MDM_EINVAL, "bad mode");
+  TRY(check_range_down(e, first_index, n_run));
+  const bool philox = (flags & B200MDM_FLAG_PHILOX_NOISE) != 0;
+  if (!philox && !noise_tape_dev) return fail(B200MDM_EINVAL, "null noise tape (or pass B200MDM_FLAG_PHILOX_NOISE)");
+  return run_loop(e, loop_args(e, mode, 0, flags, philox), flags, first_index, n_run, x_in_dev, x_out_dev, noise_tape_dev,
+                  noise_step_stride, use_graph, stream);
 }
 
 extern "C" int b200mdm_sample_loop(b200mdm_engine* e, int32_t mode, int32_t skip_timesteps, const float* x_T_dev,
@@ -1899,65 +1922,46 @@ extern "C" int b200mdm_sample_loop(b200mdm_engine* e, int32_t mode, int32_t skip
 // buffer: the loop of b200mdm_sample_loop_range with the reverse epilogue, no noise and an upward step counter.
 extern "C" int b200mdm_ddim_reverse_loop_range(b200mdm_engine* e, int32_t first_index, int32_t n_run, const float* x_in_dev,
                                                float* x_out_dev, int32_t flags, int32_t use_graph, void* stream) {
-  if (flags & ~B200MDM_FLAG_CLIP_DENOISED)
-    return fail(B200MDM_EINVAL, "DDIM inversion takes no flag but B200MDM_FLAG_CLIP_DENOISED");
+  TRY(check_flags("DDIM inversion", flags, B200MDM_FLAG_CLIP_DENOISED));
   if (n_run <= 0 || first_index < 0) return fail(B200MDM_EINVAL, "bad step range");
   TRY(check_ready(e, true));
   if (n_run > e->n_steps - first_index) return fail(B200MDM_EINVAL, "bad step range");
-  if (!e->sched_next_fresh)
-    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_next has not been called for the current schedule");
+  TRY(need_table(e, TAB_NEXT));
   if (e->hs_set) return fail(B200MDM_ENOTIMPL, "DDIM inversion with handshakes is not implemented");
-  StepArgs a;
-  a.mode = B200MDM_MODE_DDIM_REVERSE;
-  a.x_in = e->x_work;
-  a.x_out = e->x_work;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-  return run_loop(e, a, flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0, use_graph, stream);
+  return run_loop(e, loop_args(e, B200MDM_MODE_DDIM_REVERSE, 0, flags, false), flags, first_index, n_run, x_in_dev, x_out_dev,
+                  nullptr, 0, use_graph, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ PLMS
 static int ensure_plms(b200mdm_engine* e) {
-  if (e->plms_ring && e->plms_mid && e->plms_pred) return B200MDM_OK;
   const size_t n = static_cast<size_t>(e->B) * e->JF * e->T;
-  int r = B200MDM_OK;
-  if (!e->plms_ring) r = dalloc(&e->plms_ring, PLMS_RING * n);
-  if (r == B200MDM_OK && !e->plms_mid) r = dalloc(&e->plms_mid, n);
-  if (r == B200MDM_OK && !e->plms_pred) r = dalloc(&e->plms_pred, n);
-  if (r != B200MDM_OK) {   // all or nothing: no later call may find a partial set
-    dfree(e->plms_ring); dfree(e->plms_mid); dfree(e->plms_pred);
-  }
-  return r;
+  return alloc_all({{&e->plms_ring, PLMS_RING * n}, {&e->plms_mid, n}, {&e->plms_pred, n}});
 }
 
 extern "C" int b200mdm_plms_loop_range(b200mdm_engine* e, int32_t order, int32_t first_index, int32_t n_run,
                                        const float* x_in_dev, float* x_out_dev, int32_t flags, int32_t use_graph,
                                        void* stream) {
   if (order < 1 || order > 4) return fail(B200MDM_EINVAL, "PLMS order %d is not an integer from 1 to 4", order);
-  if (flags & ~B200MDM_FLAG_CLIP_DENOISED) return fail(B200MDM_EINVAL, "PLMS takes no flag but B200MDM_FLAG_CLIP_DENOISED");
+  TRY(check_flags("PLMS", flags, B200MDM_FLAG_CLIP_DENOISED));
   if (x_in_dev && order == 1)
     return fail(B200MDM_EINVAL, "a PLMS loop of order 1 has no first step (the reference needs old_out there)");
   if (n_run <= 0) return fail(B200MDM_EINVAL, "bad step range");
   TRY(check_ready(e, true));
-  if (first_index >= e->n_steps || first_index - n_run + 1 < 0) return fail(B200MDM_EINVAL, "bad step range");
+  TRY(check_range_down(e, first_index, n_run));
   if (!x_in_dev && (e->plms_done < 0 || e->plms_order != order))
     return fail(B200MDM_ESTATE, "no PLMS loop of order %d to continue (pass x_in_dev)", order);
   TRY(ensure_plms(e));
   // every step after the improved-Euler one is an Adams-Bashforth step: the launches of a DDIM step, one graph per order
-  StepArgs a;
-  a.mode = MODE_PLMS_AB;
-  a.order = order;
-  a.x_in = e->x_work;
-  a.x_out = e->x_work;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
   const int done = x_in_dev ? 0 : e->plms_done;
-  return run_loop(e, a, flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0, use_graph, stream, done, done == 0);
+  return run_loop(e, loop_args(e, MODE_PLMS_AB, order, flags, false), flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0,
+                  use_graph, stream, done, done == 0);
 }
 
 extern "C" int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order, const float* x_t_dev,
                                  const float* const* old_eps_dev, int32_t n_old, int32_t flags, float* x_out_dev,
                                  float* pred_xstart_dev, float* eps_out_dev, void* stream) {
   if (order < 1 || order > 4) return fail(B200MDM_EINVAL, "PLMS order %d is not an integer from 1 to 4", order);
-  if (flags & ~B200MDM_FLAG_CLIP_DENOISED) return fail(B200MDM_EINVAL, "PLMS takes no flag but B200MDM_FLAG_CLIP_DENOISED");
+  TRY(check_flags("PLMS", flags, B200MDM_FLAG_CLIP_DENOISED));
   // old_eps_dev NULL = no old_out (the improved-Euler step); non-NULL = old_out['old_eps'], which may be empty: the
   // reference then takes the Adams-Bashforth branch at cur_order 1 (gaussian_diffusion.py:1042-1056)
   const bool euler = old_eps_dev == nullptr;
@@ -2002,6 +2006,10 @@ extern "C" int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order
 }
 
 // ------------------------------------------------------------------------------------------------ DPM-Solver++
+static int ensure_dpm(b200mdm_engine* e) {
+  return alloc_all({{&e->dpm_hist, DPM_SLOTS * static_cast<size_t>(e->B) * e->JF * e->T}});
+}
+
 // Multistep DPM-Solver++ (data prediction) at schedule indices first_index, first_index-1, ... (n_run of them) on the
 // engine's working buffer: the launches of a DDIM step without the noise draw, one graph per order.  The step counter
 // k = StepState::done selects the history slots and the first-order first step.
@@ -2009,24 +2017,17 @@ extern "C" int b200mdm_dpm_loop_range(b200mdm_engine* e, int32_t order, int32_t 
                                       const float* x_in_dev, float* x_out_dev, int32_t flags, int32_t use_graph,
                                       void* stream) {
   if (order < 1 || order > 2) return fail(B200MDM_EINVAL, "DPM-Solver++ order %d is not 1 or 2", order);
-  if (flags & ~B200MDM_FLAG_CLIP_DENOISED)
-    return fail(B200MDM_EINVAL, "DPM-Solver++ takes no flag but B200MDM_FLAG_CLIP_DENOISED");
+  TRY(check_flags("DPM-Solver++", flags, B200MDM_FLAG_CLIP_DENOISED));
   if (n_run <= 0) return fail(B200MDM_EINVAL, "bad step range");
   TRY(check_ready(e, true));
-  if (first_index >= e->n_steps || first_index - n_run + 1 < 0) return fail(B200MDM_EINVAL, "bad step range");
-  if (!e->sched_dpm_fresh)
-    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_dpm has not been called for the current schedule");
+  TRY(check_range_down(e, first_index, n_run));
+  TRY(need_table(e, TAB_DPM));
   if (!x_in_dev && (e->dpm_done < 0 || e->dpm_order != order))
     return fail(B200MDM_ESTATE, "no DPM-Solver++ loop of order %d to continue (pass x_in_dev)", order);
-  if (!e->dpm_hist) TRY(dalloc(&e->dpm_hist, DPM_SLOTS * static_cast<size_t>(e->B) * e->JF * e->T));
-  StepArgs a;
-  a.mode = MODE_DPM;
-  a.order = order;
-  a.x_in = e->x_work;
-  a.x_out = e->x_work;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  TRY(ensure_dpm(e));
   const int done = x_in_dev ? 0 : e->dpm_done;
-  return run_loop(e, a, flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0, use_graph, stream, done);
+  return run_loop(e, loop_args(e, MODE_DPM, order, flags, false), flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0,
+                  use_graph, stream, done);
 }
 
 extern "C" int b200mdm_dpm_pred_xstart(b200mdm_engine* e, float* out_dev, void* stream) {
@@ -2123,8 +2124,7 @@ extern "C" int b200mdm_chain_loop_range(b200mdm_engine* e, int32_t mode, int32_t
     return fail(B200MDM_EINVAL, "chain mode %d: B200MDM_MODE_DDPM, B200MDM_MODE_DDIM or 7 (DPM-Solver++)", mode);
   if (dpm ? (order < 1 || order > 2) : order != 0)
     return fail(B200MDM_EINVAL, "order %d: 1 or 2 for DPM-Solver++, 0 otherwise", order);
-  if (flags & ~(B200MDM_FLAG_CLIP_DENOISED | B200MDM_FLAG_PHILOX_NOISE))
-    return fail(B200MDM_EINVAL, "a chain takes no flag but B200MDM_FLAG_CLIP_DENOISED and B200MDM_FLAG_PHILOX_NOISE");
+  TRY(check_flags("a chain", flags, B200MDM_FLAG_CLIP_DENOISED | B200MDM_FLAG_PHILOX_NOISE));
   const bool philox = (flags & B200MDM_FLAG_PHILOX_NOISE) != 0;
   if (!philox && (!x_T_dev || (!dpm && !noise_tape_dev)))
     return fail(B200MDM_EINVAL, "null x_T or noise tape (or pass B200MDM_FLAG_PHILOX_NOISE)");
@@ -2132,22 +2132,14 @@ extern "C" int b200mdm_chain_loop_range(b200mdm_engine* e, int32_t mode, int32_t
   if (first_step < 0 || n_run <= 0) return fail(B200MDM_EINVAL, "bad step range");
   if (!is_prefix_engine(e)) return fail(B200MDM_EINVAL, "the chain is for prefix-completion (DiP) engines");
   if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
-  if (dpm && !e->sched_dpm_fresh)
-    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_dpm has not been called for the current schedule");
+  if (dpm) TRY(need_table(e, TAB_DPM));
   if (e->chain_next < 0 || first_step != e->chain_next)
     return fail(B200MDM_ESTATE, "no chain to run from step %d (b200mdm_chain_setup; next step %d)", first_step, e->chain_next);
   const int N = e->n_steps;
   if (static_cast<long long>(first_step) + n_run > static_cast<long long>(e->chain_n) * N)
     return fail(B200MDM_EINVAL, "steps %d .. %d past the chain's %d x %d", first_step, first_step + n_run - 1, e->chain_n, N);
-  if (dpm && !e->dpm_hist) TRY(dalloc(&e->dpm_hist, DPM_SLOTS * static_cast<size_t>(e->B) * e->JF * e->T));
-  StepArgs a;
-  a.mode = mode;
-  a.order = order;
-  a.x_in = e->x_work;
-  a.x_out = e->x_work;
-  a.philox = philox && !dpm;
-  a.noise = a.philox ? e->eps_buf : nullptr;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  if (dpm) TRY(ensure_dpm(e));
+  const StepArgs a = loop_args(e, mode, order, flags, philox && !dpm);
   cudaStream_t user = static_cast<cudaStream_t>(stream), s;
   TRY(loop_enter(e, a, flags, use_graph, user, &s));
   // The chain consumes the conditioning: it replaces the memory (per-chunk memories) and the prefix rows, so every
@@ -2203,24 +2195,20 @@ extern "C" int b200mdm_chain_loop_range(b200mdm_engine* e, int32_t mode, int32_t
 // ------------------------------------------------------------------------------------------------ variational bound
 static int ensure_vb(b200mdm_engine* e) {
   const size_t n = static_cast<size_t>(e->B) * e->JF * e->T;
-  if (e->vb_xs && e->vb_part && e->vb_terms && e->vb_cap >= e->n_steps) return B200MDM_OK;
   if (e->vb_terms && e->vb_cap < e->n_steps) {   // a longer schedule: the step graph holds the old pointer
     drop_graph(e);
     dfree(e->vb_terms);
     e->vb_live = false;
   }
-  int r = B200MDM_OK;
-  if (!e->vb_xs) r = dalloc(&e->vb_xs, n);
-  if (r == B200MDM_OK && !e->vb_part)
-    r = dalloc(&e->vb_part, static_cast<size_t>(VB_TERMS) * e->B * e->T * ((e->JF + 31) / 32));
-  if (r == B200MDM_OK && !e->vb_terms) {
-    r = dalloc(&e->vb_terms, static_cast<size_t>(VB_TERMS) * e->B * e->sched_cap);
-    e->vb_cap = r == B200MDM_OK ? e->sched_cap : 0;
-  }
-  if (r != B200MDM_OK) {   // all or nothing
-    dfree(e->vb_xs); dfree(e->vb_part); dfree(e->vb_terms);
+  const bool new_terms = !e->vb_terms;
+  const int r = alloc_all({{&e->vb_xs, n},
+                           {&e->vb_part, static_cast<size_t>(VB_TERMS) * e->B * e->T * ((e->JF + 31) / 32)},
+                           {&e->vb_terms, static_cast<size_t>(VB_TERMS) * e->B * e->sched_cap}});
+  if (r != B200MDM_OK) {
     e->vb_cap = 0;
     e->vb_live = false;
+  } else if (new_terms) {
+    e->vb_cap = e->sched_cap;
   }
   return r;
 }
@@ -2231,15 +2219,13 @@ static int ensure_vb(b200mdm_engine* e) {
 extern "C" int b200mdm_vb_loop_range(b200mdm_engine* e, int32_t first_index, int32_t n_run, const float* x_start_dev,
                                      const float* noise_tape_dev, int64_t noise_step_stride, int32_t flags,
                                      float* terms_dev, float* bpd_dev, int32_t use_graph, void* stream) {
-  if (flags & ~(B200MDM_FLAG_CLIP_DENOISED | B200MDM_FLAG_PHILOX_NOISE))
-    return fail(B200MDM_EINVAL, "the bound loop takes no flag but B200MDM_FLAG_CLIP_DENOISED and B200MDM_FLAG_PHILOX_NOISE");
+  TRY(check_flags("the bound loop", flags, B200MDM_FLAG_CLIP_DENOISED | B200MDM_FLAG_PHILOX_NOISE));
   const bool philox = (flags & B200MDM_FLAG_PHILOX_NOISE) != 0;
   if (!philox && !noise_tape_dev) return fail(B200MDM_EINVAL, "null noise tape (or pass B200MDM_FLAG_PHILOX_NOISE)");
   if (n_run <= 0) return fail(B200MDM_EINVAL, "bad step range");
   TRY(check_ready(e, true));
-  if (first_index >= e->n_steps || first_index - n_run + 1 < 0) return fail(B200MDM_EINVAL, "bad step range");
-  if (!e->sched_vb_fresh)
-    return fail(B200MDM_ESTATE, "b200mdm_set_schedule_vb has not been called for the current schedule");
+  TRY(check_range_down(e, first_index, n_run));
+  TRY(need_table(e, TAB_VB));
   if (!x_start_dev && !e->vb_live) return fail(B200MDM_ESTATE, "no bound loop to continue (pass x_start_dev)");
   if (e->hs_set) return fail(B200MDM_ENOTIMPL, "the variational bound with handshakes is not implemented");
   TRY(ensure_vb(e));
@@ -2252,18 +2238,13 @@ extern "C" int b200mdm_vb_loop_range(b200mdm_engine* e, int32_t first_index, int
     CUDA_TRY(cudaMemsetAsync(e->vb_terms, 0, static_cast<size_t>(VB_TERMS) * e->B * e->vb_cap * sizeof(float), user));
   }
   e->vb_live = true;
-  StepArgs a;
-  a.mode = MODE_VB;
-  a.x_in = e->x_work;
-  a.noise = philox ? e->eps_buf : nullptr;
-  a.philox = philox;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-  TRY(run_loop(e, a, flags, first_index, n_run, nullptr, nullptr, noise_tape_dev, noise_step_stride, use_graph, stream));
+  TRY(run_loop(e, loop_args(e, MODE_VB, 0, flags, philox), flags, first_index, n_run, nullptr, nullptr, noise_tape_dev,
+               noise_step_stride, use_graph, stream));
   if (terms_dev)
     CUDA_TRY(cudaMemcpy2DAsync(terms_dev, e->n_steps * sizeof(float), e->vb_terms, e->vb_cap * sizeof(float),
                                e->n_steps * sizeof(float), static_cast<size_t>(VB_TERMS) * e->B, cudaMemcpyDeviceToDevice, user));
   if (bpd_dev && first_index - n_run + 1 == 0) {
-    vb_final_kernel<<<e->B, VB_REDUCE_THREADS, 0, user>>>(bpd_dev, e->vb_terms, e->vb_cap, e->vb_xs, e->sched_vb, e->n_steps,
+    vb_final_kernel<<<e->B, VB_REDUCE_THREADS, 0, user>>>(bpd_dev, e->vb_terms, e->vb_cap, e->vb_xs, e->tab[TAB_VB], e->n_steps,
                                                            e->B, e->JF * e->T);
     CUDA_TRY(cudaGetLastError());
     e->launches += 1;
@@ -2304,7 +2285,9 @@ extern "C" int64_t b200mdm_launch_count(b200mdm_engine* e, int32_t reset) {
 }
 
 // ------------------------------------------------------------------------------------------------ kernel tests
-static int device_sms(int* sms) {
+// What every GEMM test hook does before its launches: the kernels' attributes, and the SM count of the current device.
+static int test_prologue(int* sms) {
+  TRY(init_kernel_attrs());
   int dev = 0;
   CUDA_TRY(cudaGetDevice(&dev));
   CUDA_TRY(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
@@ -2317,9 +2300,8 @@ extern "C" int b200mdm_test_gemm_f16(const void* a16_dev, const void* w16_dev, c
     return fail(B200MDM_EINVAL, "bad argument (K %% 8 == 0, N %% 8 == 0 required)");
   if (block_n != PP_BLOCK_N)
     return fail(B200MDM_EINVAL, "block_n must be 128 (the 128 x 128 tiles of the step's ping-pong projection kernel)");
-  TRY(init_kernel_attrs());
   int sms = 132;
-  TRY(device_sms(&sms));
+  TRY(test_prologue(&sms));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CUtensorMap ma, mb, mc;
   TRY(make_map(&ma, a16_dev, M, K, K, GEMM_BLOCK_M));
@@ -2350,9 +2332,8 @@ extern "C" int b200mdm_test_gemm_epi(const void* a16_dev, const void* w16_dev, c
                                      int32_t M, int32_t N, int32_t K, int32_t epi, void* stream) {
   if (!a16_dev || !w16_dev || !bias_dev || !out16_dev || M <= 0 || N <= 0 || K <= 0 || K % 8)
     return fail(B200MDM_EINVAL, "bad argument (K %% 8 == 0 required)");
-  TRY(init_kernel_attrs());
   int sms = 132;
-  TRY(device_sms(&sms));
+  TRY(test_prologue(&sms));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CUtensorMap ma, mb, mc;
   TRY(make_map(&ma, a16_dev, M, K, K, GEMM_BLOCK_M));
@@ -2379,9 +2360,8 @@ extern "C" int b200mdm_test_embed(const float* x_dev, const float* w_in_dev, con
   if (!x_dev || !w_in_dev || !b_in_dev || !pe_dev || !hres16_dev || B <= 0 || JF <= 0 || T <= 0 || s_off < 0 ||
       d <= 0 || d % 64 || d * 4 > GEMM_BIAS_BYTES || (halves != 1 && halves != 2))
     return fail(B200MDM_EINVAL, "bad argument (d %% 64 == 0, d <= %d, halves 1 or 2)", GEMM_BIAS_BYTES / 4);
-  TRY(init_kernel_attrs());
   int sms = 132;
-  TRY(device_sms(&sms));
+  TRY(test_prologue(&sms));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int S = T + s_off, Kp = (JF + 7) & ~7, MB = B * S;
   StreamScratch scr(s);
@@ -2403,29 +2383,71 @@ extern "C" int b200mdm_test_embed(const float* x_dev, const float* w_in_dev, con
   return launch_embed_gemm(m_xin, m_win, m_res_c, m_res_u, pe_bias, MB, S, d, Kp, halves, s, sms);
 }
 
-// What the two output-step hooks share, on scratch memory of `scr`: g16 = the CFG blend of hres, the split output
-// weight, the maps of both, and the bias / inpainting fields of the epilogue parameters.
+// One output-step launch of a test hook, as the step makes it, on scratch memory: g16 = the CFG blend of hres and the
+// split output weight; each table a zeroed (index + 1)-row copy, with `row` at `index` of table `table`; the step state
+// (done, index, n_steps); and zeroed scratch for the PLMS ring, the partial sums, and the noise, DPM-Solver++ history
+// and x_start the caller leaves null.  With `terms`, launch_vb_reduce then reduces the bound's partial sums into it.
 struct OutHook {
-  CUtensorMap m_g16, m_wout;
-  EpiOutParams p{};
+  const void* hres16;
+  const float *scale, *w_out, *b_out;
+  int B, JF, T, d, s_off, halves;
+  const uint8_t* inpaint_mask;
+  const float *inpaint_weight, *inpaint_motion;
+  StepArgs a;   // mode, order, clip, const_noise, x_in, noise, x_out (scratch when null), pred
+  SchedTable table = TAB_STEP;
+  const float* row = nullptr;
+  int index = 0, done = 0, n_steps = 0;
+  float *x0_hist = nullptr, *vb_elem = nullptr, *terms = nullptr;
+  const float* x_start = nullptr;
 };
-static int out_hook_setup(StreamScratch& scr, OutHook* o, const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
-                          const float* b_out_dev, const uint8_t* inpaint_mask_dev, const float* inpaint_motion_dev, int B, int JF,
-                          int T, int d, int s_off, int halves, const float* inpaint_weight_dev = nullptr) {
+static int run_out_hook(OutHook h, cudaStream_t s) {
+  const int B = h.B, JF = h.JF, T = h.T, d = h.d;
+  if (!h.hres16 || !h.w_out || !h.b_out || !h.a.x_in || B <= 0 || JF <= 0 || T <= 0 || h.s_off < 0 || d <= 0 || d % 64 ||
+      (h.halves != 1 && h.halves != 2) || (h.halves == 2 && !h.scale) ||
+      (h.inpaint_mask == nullptr && h.inpaint_weight == nullptr) != (h.inpaint_motion == nullptr))
+    return fail(B200MDM_EINVAL, "bad argument");
+  int sms = 132;
+  TRY(test_prologue(&sms));
+  StreamScratch scr(s);
   const int N_out_pad = ((JF + 95) / 96) * 96;
+  const size_t n = static_cast<size_t>(B) * JF * T;
   __half *g16 = nullptr, *w_out3 = nullptr;
   TRY(scr.alloc(&g16, static_cast<size_t>(B) * T * 3 * d));
   TRY(scr.alloc(&w_out3, static_cast<size_t>(N_out_pad) * 3 * d, true));
-  split_weight_kernel<<<JF, 128, 0, scr.s>>>(w_out_dev, w_out3, JF, d, d);
+  split_weight_kernel<<<JF, 128, 0, s>>>(h.w_out, w_out3, JF, d, d);
   CUDA_TRY(cudaGetLastError());
-  TRY(launch_blend_split(static_cast<const __half*>(hres16_dev), g16, scale_dev, B, T + s_off, T, s_off, d, halves, nullptr, scr.s));
-  TRY(make_map(&o->m_g16, g16, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
-  TRY(make_map(&o->m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
-  o->p.bias = b_out_dev;
-  o->p.inpaint_mask = inpaint_mask_dev;
-  o->p.inpaint_weight = inpaint_weight_dev;
-  o->p.inpaint_motion = inpaint_motion_dev;
-  return B200MDM_OK;
+  TRY(launch_blend_split(static_cast<const __half*>(h.hres16), g16, h.scale, B, T + h.s_off, T, h.s_off, d, h.halves, nullptr, s));
+  CUtensorMap m_g16, m_wout;
+  TRY(make_map(&m_g16, g16, static_cast<uint64_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
+  TRY(make_map(&m_wout, w_out3, N_out_pad, 3 * d, 3 * d, 96));
+  EpiOutParams p{};
+  p.bias = h.b_out;
+  p.inpaint_mask = h.inpaint_mask;
+  p.inpaint_weight = h.inpaint_weight;
+  p.inpaint_motion = h.inpaint_motion;
+  float* tab[N_TABLES];
+  for (int t = 0; t < N_TABLES; ++t) TRY(scr.alloc(&tab[t], static_cast<size_t>(h.index + 1) * TAB_STRIDE[t], true));
+  if (h.row)
+    CUDA_TRY(cudaMemcpyAsync(tab[h.table] + static_cast<size_t>(h.index) * TAB_STRIDE[h.table], h.row,
+                             TAB_STRIDE[h.table] * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  set_tables(&p, tab);
+  StepState* st = nullptr;
+  TRY(scr.alloc(&st, 1));
+  step_set_kernel<<<1, 1, 0, s>>>(st, h.done, h.index, nullptr, 0, 0, 0, h.n_steps);
+  CUDA_TRY(cudaGetLastError());
+  p.state = st;
+  float* zeros = nullptr;
+  TRY(scr.alloc(&zeros, n, true));
+  TRY(scr.alloc(&p.eps_ring, PLMS_RING * n, true));
+  p.x0_hist = h.x0_hist;
+  if (!p.x0_hist) TRY(scr.alloc(&p.x0_hist, DPM_SLOTS * n, true));
+  TRY(scr.alloc(&p.vb_part, static_cast<size_t>(VB_TERMS) * B * T * ((JF + 31) / 32), true));
+  p.vb_elem = h.vb_elem;
+  p.x_start = h.x_start ? h.x_start : zeros;
+  if (!h.a.noise) h.a.noise = zeros;
+  if (!h.a.x_out) TRY(scr.alloc(&h.a.x_out, n));
+  TRY(launch_out_gemm(m_g16, m_wout, B, T, JF, d, h.a, p, s, sms));
+  return h.terms ? launch_vb_reduce(h.terms, h.n_steps, p.vb_part, B, T, JF, st, s) : B200MDM_OK;
 }
 
 extern "C" int b200mdm_test_out_step(const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
@@ -2433,32 +2455,19 @@ extern "C" int b200mdm_test_out_step(const void* hres16_dev, const float* scale_
                                      const float* sched_row_dev, int32_t mode, int32_t flags, const uint8_t* inpaint_mask_dev,
                                      const float* inpaint_motion_dev, float* x_out_dev, float* pred_xstart_dev, int32_t B,
                                      int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream) {
-  if (!hres16_dev || !w_out_dev || !b_out_dev || !x_t_dev || !x_out_dev || !pred_xstart_dev || B <= 0 || JF <= 0 ||
-      T <= 0 || s_off < 0 || d <= 0 || d % 64 || (halves != 1 && halves != 2) || (halves == 2 && !scale_dev) ||
-      mode < B200MDM_MODE_X0 || mode > B200MDM_MODE_DDIM || (mode != B200MDM_MODE_X0 && (!noise_dev || !sched_row_dev)) ||
-      (inpaint_mask_dev == nullptr) != (inpaint_motion_dev == nullptr))
+  if (!x_out_dev || !pred_xstart_dev || mode < B200MDM_MODE_X0 || mode > B200MDM_MODE_DDIM ||
+      (mode != B200MDM_MODE_X0 && (!noise_dev || !sched_row_dev)))
     return fail(B200MDM_EINVAL, "bad argument");
-  TRY(init_kernel_attrs());
-  int sms = 132;
-  TRY(device_sms(&sms));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  StreamScratch scr(s);
-  OutHook o;
-  TRY(out_hook_setup(scr, &o, hres16_dev, scale_dev, w_out_dev, b_out_dev, inpaint_mask_dev, inpaint_motion_dev, B, JF, T, d,
-                     s_off, halves));
-  StepState* st = nullptr;
-  TRY(scr.alloc(&st, 1, true));   // cur = 0: the one-row schedule table
-  o.p.sched = sched_row_dev;
-  o.p.state = st;
-  StepArgs a;
-  a.mode = mode;
-  a.x_in = x_t_dev;
-  a.noise = noise_dev;
-  a.const_noise = flags & B200MDM_FLAG_CONST_NOISE;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-  a.x_out = x_out_dev;
-  a.pred = pred_xstart_dev;
-  return launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms);
+  OutHook h{hres16_dev, scale_dev, w_out_dev, b_out_dev, B, JF, T, d, s_off, halves, inpaint_mask_dev, nullptr, inpaint_motion_dev};
+  h.a.mode = mode;
+  h.a.x_in = x_t_dev;
+  h.a.noise = noise_dev;
+  h.a.const_noise = flags & B200MDM_FLAG_CONST_NOISE;
+  h.a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  h.a.x_out = x_out_dev;
+  h.a.pred = pred_xstart_dev;
+  h.row = sched_row_dev;
+  return run_out_hook(h, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b200mdm_test_out_dpm(const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
@@ -2466,37 +2475,22 @@ extern "C" int b200mdm_test_out_dpm(const void* hres16_dev, const float* scale_d
                                     int32_t step, int32_t order, int32_t flags, const uint8_t* inpaint_mask_dev,
                                     const float* inpaint_motion_dev, float* x0_hist_dev, float* x_out_dev, int32_t B,
                                     int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream) {
-  if (!hres16_dev || !w_out_dev || !b_out_dev || !x_t_dev || !dpm_row_dev || !x0_hist_dev || !x_out_dev || B <= 0 ||
-      JF <= 0 || T <= 0 || s_off < 0 || d <= 0 || d % 64 || (halves != 1 && halves != 2) || (halves == 2 && !scale_dev) ||
-      index < 0 || step < 0 || (order != 1 && order != 2) || (flags & ~B200MDM_FLAG_CLIP_DENOISED) ||
-      (inpaint_mask_dev == nullptr) != (inpaint_motion_dev == nullptr))
+  if (!dpm_row_dev || !x0_hist_dev || !x_out_dev || index < 0 || step < 0 || (order != 1 && order != 2) ||
+      (flags & ~B200MDM_FLAG_CLIP_DENOISED))
     return fail(B200MDM_EINVAL, "bad argument");
-  TRY(init_kernel_attrs());
-  int sms = 132;
-  TRY(device_sms(&sms));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  StreamScratch scr(s);
-  OutHook o;
-  TRY(out_hook_setup(scr, &o, hres16_dev, scale_dev, w_out_dev, b_out_dev, inpaint_mask_dev, inpaint_motion_dev, B, JF, T, d,
-                     s_off, halves));
-  float* table = nullptr;
-  StepState* st = nullptr;
-  TRY(scr.alloc(&table, static_cast<size_t>(index + 1) * SCHED_DPM_STRIDE, true));   // the row at `index`, zeros above
-  TRY(scr.alloc(&st, 1, true));
-  CUDA_TRY(cudaMemcpyAsync(table + static_cast<size_t>(index) * SCHED_DPM_STRIDE, dpm_row_dev, SCHED_DPM_STRIDE * sizeof(float),
-                           cudaMemcpyDeviceToDevice, s));
-  step_set_kernel<<<1, 1, 0, s>>>(st, step, index, nullptr, 0, 0, 0, index + 1);
-  CUDA_TRY(cudaGetLastError());
-  o.p.sched_dpm = table;
-  o.p.x0_hist = x0_hist_dev;
-  o.p.state = st;
-  StepArgs a;
-  a.mode = MODE_DPM;
-  a.order = order;
-  a.x_in = x_t_dev;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-  a.x_out = x_out_dev;
-  return launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms);
+  OutHook h{hres16_dev, scale_dev, w_out_dev, b_out_dev, B, JF, T, d, s_off, halves, inpaint_mask_dev, nullptr, inpaint_motion_dev};
+  h.a.mode = MODE_DPM;
+  h.a.order = order;
+  h.a.x_in = x_t_dev;
+  h.a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  h.a.x_out = x_out_dev;
+  h.table = TAB_DPM;
+  h.row = dpm_row_dev;
+  h.index = index;
+  h.done = step;
+  h.n_steps = index + 1;
+  h.x0_hist = x0_hist_dev;
+  return run_out_hook(h, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b200mdm_test_out_vb(const void* hres16_dev, const float* scale_dev, const float* w_out_dev,
@@ -2505,41 +2499,23 @@ extern "C" int b200mdm_test_out_vb(const void* hres16_dev, const float* scale_de
                                    const uint8_t* inpaint_mask_dev, const float* inpaint_motion_dev, float* pred_xstart_dev,
                                    float* elem_dev, float* terms_dev, int32_t B, int32_t JF, int32_t T, int32_t d, int32_t s_off,
                                    int32_t halves, void* stream) {
-  if (!hres16_dev || !w_out_dev || !b_out_dev || !x_t_dev || !x_start_dev || !noise_dev || !vb_row_dev || !terms_dev ||
-      B <= 0 || JF <= 0 || T <= 0 || s_off < 0 || d <= 0 || d % 64 || (halves != 1 && halves != 2) ||
-      (halves == 2 && !scale_dev) || index < 0 || index >= n_steps || (flags & ~B200MDM_FLAG_CLIP_DENOISED) ||
-      (inpaint_mask_dev == nullptr) != (inpaint_motion_dev == nullptr))
+  if (!x_start_dev || !noise_dev || !vb_row_dev || !terms_dev || index < 0 || index >= n_steps ||
+      (flags & ~B200MDM_FLAG_CLIP_DENOISED))
     return fail(B200MDM_EINVAL, "bad argument");
-  TRY(init_kernel_attrs());
-  int sms = 132;
-  TRY(device_sms(&sms));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  StreamScratch scr(s);
-  OutHook o;
-  TRY(out_hook_setup(scr, &o, hres16_dev, scale_dev, w_out_dev, b_out_dev, inpaint_mask_dev, inpaint_motion_dev, B, JF, T, d,
-                     s_off, halves));
-  float *table = nullptr, *part = nullptr;
-  StepState* st = nullptr;
-  TRY(scr.alloc(&table, static_cast<size_t>(index + 1) * SCHED_VB_STRIDE, true));   // the row at `index`, zeros above
-  TRY(scr.alloc(&part, static_cast<size_t>(VB_TERMS) * B * T * ((JF + 31) / 32)));
-  TRY(scr.alloc(&st, 1, true));
-  CUDA_TRY(cudaMemcpyAsync(table + static_cast<size_t>(index) * SCHED_VB_STRIDE, vb_row_dev, SCHED_VB_STRIDE * sizeof(float),
-                           cudaMemcpyDeviceToDevice, s));
-  step_set_kernel<<<1, 1, 0, s>>>(st, 0, index, nullptr, 0, 0, 0, n_steps);
-  CUDA_TRY(cudaGetLastError());
-  o.p.sched_vb = table;
-  o.p.x_start = x_start_dev;
-  o.p.vb_part = part;
-  o.p.vb_elem = elem_dev;
-  o.p.state = st;
-  StepArgs a;
-  a.mode = MODE_VB;
-  a.x_in = x_t_dev;
-  a.noise = noise_dev;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-  a.pred = pred_xstart_dev;
-  TRY(launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms));
-  return launch_vb_reduce(terms_dev, n_steps, part, B, T, JF, st, s);
+  OutHook h{hres16_dev, scale_dev, w_out_dev, b_out_dev, B, JF, T, d, s_off, halves, inpaint_mask_dev, nullptr, inpaint_motion_dev};
+  h.a.mode = MODE_VB;
+  h.a.x_in = x_t_dev;
+  h.a.noise = noise_dev;
+  h.a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  h.a.pred = pred_xstart_dev;
+  h.table = TAB_VB;
+  h.row = vb_row_dev;
+  h.index = index;
+  h.n_steps = n_steps;
+  h.x_start = x_start_dev;
+  h.vb_elem = elem_dev;
+  h.terms = terms_dev;
+  return run_out_hook(h, static_cast<cudaStream_t>(stream));
 }
 
 // x0 of the output epilogue with soft inpainting, on the GEMM instantiation of update family `mode` (B200MDM_MODE_X0 /
@@ -2551,52 +2527,15 @@ extern "C" int b200mdm_test_out_weight(const void* hres16_dev, const float* scal
                                        int32_t JF, int32_t T, int32_t d, int32_t s_off, int32_t halves, void* stream) {
   const bool family = mode == MODE_X0 || mode == MODE_DDPM || mode == MODE_DDIM || mode == MODE_PLMS_AB ||
                       mode == MODE_DDIM_REVERSE || mode == MODE_DPM || mode == MODE_VB;
-  if (!hres16_dev || !w_out_dev || !b_out_dev || !x_t_dev || !pred_xstart_dev || B <= 0 || JF <= 0 || T <= 0 ||
-      s_off < 0 || d <= 0 || d % 64 || (halves != 1 && halves != 2) || (halves == 2 && !scale_dev) || !family ||
-      (flags & ~B200MDM_FLAG_CLIP_DENOISED) || (weight_dev == nullptr) != (motion_dev == nullptr))
-    return fail(B200MDM_EINVAL, "bad argument");
-  TRY(init_kernel_attrs());
-  int sms = 132;
-  TRY(device_sms(&sms));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  StreamScratch scr(s);
-  OutHook o;
-  TRY(out_hook_setup(scr, &o, hres16_dev, scale_dev, w_out_dev, b_out_dev, nullptr, motion_dev, B, JF, T, d, s_off, halves,
-                     weight_dev));
-  const size_t n = static_cast<size_t>(B) * JF * T;
-  float *x_out = nullptr, *zeros = nullptr, *ring = nullptr, *hist = nullptr, *part = nullptr, *sched = nullptr;
-  float *next = nullptr, *dpm = nullptr, *vb = nullptr;
-  StepState* st = nullptr;
-  TRY(scr.alloc(&x_out, n));
-  TRY(scr.alloc(&zeros, n, true));                       // noise, x_start
-  TRY(scr.alloc(&ring, PLMS_RING * n, true));
-  TRY(scr.alloc(&hist, DPM_SLOTS * n, true));
-  TRY(scr.alloc(&part, static_cast<size_t>(VB_TERMS) * B * T * ((JF + 31) / 32)));
-  TRY(scr.alloc(&sched, SCHED_STRIDE, true));            // one all-zero row of each table: index 0
-  TRY(scr.alloc(&next, SCHED_NEXT_STRIDE, true));
-  TRY(scr.alloc(&dpm, SCHED_DPM_STRIDE, true));
-  TRY(scr.alloc(&vb, SCHED_VB_STRIDE, true));
-  TRY(scr.alloc(&st, 1, true));
-  step_set_kernel<<<1, 1, 0, s>>>(st, 0, 0, nullptr, 0, 0, 0, 1);
-  CUDA_TRY(cudaGetLastError());
-  o.p.sched = sched;
-  o.p.sched_next = next;
-  o.p.sched_dpm = dpm;
-  o.p.sched_vb = vb;
-  o.p.eps_ring = ring;
-  o.p.x0_hist = hist;
-  o.p.x_start = zeros;
-  o.p.vb_part = part;
-  o.p.state = st;
-  StepArgs a;
-  a.mode = mode;
-  a.order = 1;
-  a.x_in = x_t_dev;
-  a.noise = zeros;
-  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
-  a.x_out = x_out;
-  a.pred = pred_xstart_dev;
-  return launch_out_gemm(o.m_g16, o.m_wout, B, T, JF, d, a, o.p, s, sms);
+  if (!pred_xstart_dev || !family || (flags & ~B200MDM_FLAG_CLIP_DENOISED)) return fail(B200MDM_EINVAL, "bad argument");
+  OutHook h{hres16_dev, scale_dev, w_out_dev, b_out_dev, B, JF, T, d, s_off, halves, nullptr, weight_dev, motion_dev};
+  h.a.mode = mode;
+  h.a.order = 1;
+  h.a.x_in = x_t_dev;
+  h.a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  h.a.pred = pred_xstart_dev;
+  h.n_steps = 1;
+  return run_out_hook(h, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b200mdm_test_blend_handshake(const void* hres16_dev, const float* scale_dev, void* g16_dev, int32_t B,
@@ -2653,9 +2592,8 @@ extern "C" int b200mdm_test_qkv_attention(const void* h16_dev, int32_t ld, const
   if (!h16_dev || !wqkv16_dev || !bqkv_dev || !out16_dev || !kvlen_dev || n_samples <= 0 || S <= 0 || S > ATC_MAX_KEYS ||
       ld < 512 || ld % 8)
     return fail(B200MDM_EINVAL, "bad argument");
-  TRY(init_kernel_attrs());
   int sms = 132;
-  TRY(device_sms(&sms));
+  TRY(test_prologue(&sms));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int M = n_samples * S;
   __half* qkv = nullptr;
@@ -2677,9 +2615,8 @@ extern "C" int b200mdm_test_gemm_resid_ln(const void* a16_dev, const void* w16_d
                                           int32_t K, void* stream) {
   if (!a16_dev || !w16_dev || !bias_dev || !gamma_dev || !beta_dev || !hres16_dev || M <= 0 || K <= 0 || K % 8)
     return fail(B200MDM_EINVAL, "bad argument");
-  TRY(init_kernel_attrs());
   int sms = 132;
-  TRY(device_sms(&sms));
+  TRY(test_prologue(&sms));
   CUtensorMap ma, mb, mh;
   TRY(make_map(&ma, a16_dev, M, K, K, GEMM_BLOCK_M));
   TRY(make_map(&mb, w16_dev, GLN_D, K, K, 256));

@@ -81,7 +81,7 @@ class Engine:
         self._keep = {}
         self._cond_key = None
         self._sched_key = None
-        self._next_key = None
+        self._table_keys = {}                     # "next" / "dpm" / "vb": the key of the rows uploaded for the schedule
         self.batch = self.nframes = self.n_tokens = 0
         self.halves = 1
 
@@ -122,36 +122,29 @@ class Engine:
         check(self.lib.b200mdm_set_schedule(self.h, len(tmap), rows.ctypes.data_as(ctypes.c_void_p),
                                             tmap.ctypes.data_as(ctypes.c_void_p)))
         self._sched_key = key
-        self._next_key = None                     # the engine marks the reverse, DPM-Solver++ and bound tables stale
-        self._dpm_key = None
-        self._vb_key = None
+        self._table_keys.clear()                  # the engine marks the reverse, DPM-Solver++ and bound tables stale
+
+    def _set_table(self, which, rows, key):
+        """b200mdm_set_schedule_<which>, skipped when `key` names the rows already uploaded for this schedule."""
+        if key is not None and key == self._table_keys.get(which):
+            return
+        rows = np.ascontiguousarray(rows, dtype=np.float32)
+        assert rows.ndim == 2 and rows.shape[1] == getattr(_lib, "SCHED_%s_STRIDE" % which.upper())
+        setter = getattr(self.lib, "b200mdm_set_schedule_" + which)
+        check(setter(self.h, rows.shape[0], rows.ctypes.data_as(ctypes.c_void_p)))
+        self._table_keys[which] = key
 
     def set_schedule_next(self, rows, key=None):
         """[n_steps, 2] fp32 rows sqrt(abn), sqrt(1 - abn) of the current schedule (b200mdm_set_schedule_next)."""
-        if key is not None and key == self._next_key:
-            return
-        rows = np.ascontiguousarray(rows, dtype=np.float32)
-        assert rows.ndim == 2 and rows.shape[1] == _lib.SCHED_NEXT_STRIDE
-        check(self.lib.b200mdm_set_schedule_next(self.h, rows.shape[0], rows.ctypes.data_as(ctypes.c_void_p)))
-        self._next_key = key
+        self._set_table("next", rows, key)
 
     def set_schedule_dpm(self, rows, key=None):
         """[n_steps, 4] fp32 rows c_x, c0, c_cur, c_prev of the current schedule (b200mdm_set_schedule_dpm)."""
-        if key is not None and key == self._dpm_key:
-            return
-        rows = np.ascontiguousarray(rows, dtype=np.float32)
-        assert rows.ndim == 2 and rows.shape[1] == _lib.SCHED_DPM_STRIDE
-        check(self.lib.b200mdm_set_schedule_dpm(self.h, rows.shape[0], rows.ctypes.data_as(ctypes.c_void_p)))
-        self._dpm_key = key
+        self._set_table("dpm", rows, key)
 
     def set_schedule_vb(self, rows, key=None):
         """[n_steps, 12] fp32 rows of the variational-bound table of the current schedule (b200mdm_set_schedule_vb)."""
-        if key is not None and key == getattr(self, "_vb_key", None):
-            return
-        rows = np.ascontiguousarray(rows, dtype=np.float32)
-        assert rows.ndim == 2 and rows.shape[1] == _lib.SCHED_VB_STRIDE
-        check(self.lib.b200mdm_set_schedule_vb(self.h, rows.shape[0], rows.ctypes.data_as(ctypes.c_void_p)))
-        self._vb_key = key
+        self._set_table("vb", rows, key)
 
     # ------------------------------------------------------------------ conditioning
     def set_cond(self, batch, nframes, y, guided, device):

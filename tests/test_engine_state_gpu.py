@@ -928,6 +928,24 @@ def test_caller_memory_footprint(name):
     r.set_inpaint(None)
 
 
+def test_table_setters_before_set_schedule():
+    """set_schedule_next / _dpm / _vb with a key on a fresh engine, before any set_schedule: each is refused with the
+    engine's ESTATE; after set_schedule the same calls upload."""
+    eng = Engine(**_cfg())
+    s = sched(6)
+    vb = create_gaussian_diffusion(default_args(layers=L, diffusion_steps=6)).schedule_vb_rows()
+    calls = ((eng.set_schedule_next, s.next), (eng.set_schedule_dpm, s.dpm), (eng.set_schedule_vb, vb))
+    for setter, rows in calls:
+        with pytest.raises(_lib.B200MDMError) as exc:
+            setter(rows, key="k")
+        assert exc.value.code == _lib.ESTATE, exc.value
+        assert "b200mdm_set_schedule has not been called" in str(exc.value)
+    eng.set_schedule(s.rows, s.tmap)
+    for setter, rows in calls:
+        setter(rows, key="k")
+    eng.close()
+
+
 def test_recover_from_ric_strided_output():
     """recover_from_ric into a strided view (padded rows and samples) inside guard bands: it writes exactly the
     (b, t, joint, axis) elements, each where the strides say."""
