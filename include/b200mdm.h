@@ -228,6 +228,22 @@ int b200mdm_set_inpaint_weight(b200mdm_engine* e, const float* weight_dev, const
 int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t* lengths_host, const uint8_t* motion_start_host,
                           void* stream);
 
+/* Joint-position control (this project's definition, DESIGN.md "Joint-position control"): every DDPM / DDIM step
+ * replaces the model's x0 (after classifier-free guidance) by `iters` gradient steps x0 <- x0 - step * grad G(x0),
+ *   G = 1/2 sum_{t,j} weight[b,j,t] |recover_from_ric(x0 * std + mean)[t,j] - target[b,j,:,t]|^2,
+ * before inpainting, the clamp of clip_denoised and the update.  Only the ric features (0 .. 3 + 3(J-1)) change; a free
+ * joint (weight 0) never reads its target.  mean_dev, std_dev fp32 [D]; target_dev fp32 [B, J, 3, T] (sample_to_xyz's
+ * layout and units); weight_dev fp32 [B, J, T] >= 0, with D = 263 / J = 22 (HumanML3D) or D = 251 / J = 21 (KIT).  The
+ * tensors are the caller's and must stay valid until the work enqueued with them has completed; the descriptor is
+ * uploaded on `stream`.  Call it after b200mdm_set_cond / b200mdm_set_cond_dec, which clear it.  It applies to
+ * b200mdm_sample_step (modes 1 and 2), b200mdm_sample_loop and b200mdm_sample_loop_range; the PLMS, DPM-Solver++,
+ * DDIM-inversion and variational-bound entry points return B200MDM_ENOTIMPL while it is set, and b200mdm_denoise
+ * ignores it.  Null pointers, a step that is not finite or <= 0, iters outside 1 .. 10000, or a model other than
+ * D = 263 / 251 with nfeats 1 return B200MDM_EINVAL; a prefix-completion (DiP) engine, or handshakes (set before or
+ * after), B200MDM_ENOTIMPL. */
+int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_dev, const float* std_dev, const float* target_dev,
+                               const float* weight_dev, float step, int32_t iters, void* stream);
+
 /* MDM.forward / ClassifierFreeSampleModel.forward (model/mdm.py:189-283, utils/sampler_util.py:27-34):
  * out = model(x, timesteps, y), without inpainting (the sampler's, not the model's).  timesteps_host: int32 [batch] MODEL
  * timesteps (already mapped). */
@@ -459,6 +475,13 @@ int b200mdm_test_out_weight(const void* hres16_dev, const float* scale_dev, cons
 int b200mdm_test_blend_handshake(const void* hres16_dev, const float* scale_dev, void* g16_dev, int32_t B, int32_t T,
                                  int32_t d, int32_t s_off, int32_t halves, int32_t h, const int64_t* lengths_host,
                                  const uint8_t* motion_start_host, void* stream);
+/* The guidance iterations of b200mdm_set_joint_guidance alone (joint_guidance_test_kernel, the device function the
+ * step kernel runs): x0_out fp32 [B, D, T] = x0 [B, D, T] after `iters` gradient steps; loss_out (nullable) fp32
+ * [iters + 1, B] receives G before each step and after the last.  1 <= T <= 256; other arguments as there; invalid
+ * arguments return B200MDM_EINVAL before any CUDA call. */
+int b200mdm_test_joint_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
+                                const float* weight_dev, int32_t B, int32_t T, int32_t D, float step, int32_t iters,
+                                float* x0_out_dev, float* loss_out_dev, void* stream);
 /* Self-attention core (tensor-core kernel, S <= 256): softmax(q k^T / sqrt(128) + mask) v per (sample, head);
  * qkv16 [n*S, 3d]; kvlen int32 [n] device (valid keys per sample, a prefix).
  * impl 0: out16 fp16 [n*S, d] (the encoder); impl 1: out16 fp16 [n*S, 2d] = [hi | lo] with hi + lo = the fp32 result

@@ -36,7 +36,7 @@ SYMBOLS = [
     "b200mdm_set_schedule_dpm", "b200mdm_dpm_loop_range", "b200mdm_dpm_pred_xstart", "b200mdm_test_out_dpm",
     "b200mdm_set_schedule_vb", "b200mdm_vb_loop_range", "b200mdm_test_out_vb",
     "b200mdm_set_handshake", "b200mdm_test_blend_handshake", "b200mdm_set_inpaint_weight", "b200mdm_test_out_weight",
-    "b200mdm_chain_setup", "b200mdm_chain_loop_range",
+    "b200mdm_chain_setup", "b200mdm_chain_loop_range", "b200mdm_set_joint_guidance", "b200mdm_test_joint_guidance",
 ]
 # tap points of b200mdm_test_forward_taps (B200MDM_TAP_*)
 TAPS = ["EMBED", "TOK0", "CONDPROJ", "TEMB", "MEM16", "CROSS_C", "KVC16", "L_IN", "L_QKV", "L_ATT", "L_LN1", "L_QC",
@@ -128,7 +128,9 @@ def load():
                        ("b200mdm_test_out_weight", [vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32,
                                                     vp]),
                        ("b200mdm_chain_setup", [vp, i32, i32, i32, i32, i32, vp, vp, vp]),
-                       ("b200mdm_chain_loop_range", [vp, i32, i32, i32, i32, vp, i64, vp, i64, vp, i32, i32, vp])):
+                       ("b200mdm_chain_loop_range", [vp, i32, i32, i32, i32, vp, i64, vp, i64, vp, i32, i32, vp]),
+                       ("b200mdm_set_joint_guidance", [vp, vp, vp, vp, vp, f32, i32, vp]),
+                       ("b200mdm_test_joint_guidance", [vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, vp, vp, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

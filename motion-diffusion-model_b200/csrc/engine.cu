@@ -22,6 +22,7 @@
 #include "gemm.cuh"
 #include "gemm_ln.cuh"
 #include "gemm_pingpong.cuh"
+#include "joint_guidance.cuh"
 #include "postprocess.cuh"
 #include "kernels.cuh"
 
@@ -144,9 +145,11 @@ struct GraphKey {
   const void *pred = nullptr, *imask = nullptr, *iweight = nullptr, *imotion = nullptr;
   const void* target_g = nullptr;   // the workspace's target embedding, or nullptr when the loop has no target
   const void* hs = nullptr;         // the workspace's handshake descriptor, or nullptr when the loop has none
+  bool guided = false;              // joint-position control: the step ends in joint_guidance_step_kernel
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
-           imask == o.imask && iweight == o.iweight && imotion == o.imotion && target_g == o.target_g && hs == o.hs;
+           imask == o.imask && iweight == o.iweight && imotion == o.imotion && target_g == o.target_g && hs == o.hs &&
+           guided == o.guided;
   }
 };
 
@@ -184,6 +187,9 @@ struct Workspace {
   // HS_* in kernels.cuh), allocated on first use; hs_set is cleared by every b200mdm_set_cond* call
   int* hs_desc = nullptr;
   bool hs_set = false;
+  // joint-position control (b200mdm_set_joint_guidance): the raw x0 [B, JF, T] the output GEMM hands to the guidance
+  // kernel, allocated on first use
+  float* jg_x0 = nullptr;
   // PLMS, allocated on first use: eps history ring [PLMS_RING, B, JF, T], the improved-Euler step's mean1 (the input of
   // its second forward) and its first x0.  plms_done = evaluations of the PLMS loop in flight (-1: none to continue).
   float *plms_ring = nullptr, *plms_mid = nullptr, *plms_pred = nullptr;
@@ -250,6 +256,11 @@ struct b200mdm_engine : Workspace {
   const unsigned char* inpaint_mask = nullptr;
   const float* inpaint_weight = nullptr;   // soft inpainting (b200mdm_set_inpaint_weight); never set with the mask
   const float* inpaint_motion = nullptr;
+  // joint-position control: its device descriptor (read by the step graph at every replay, allocated on first use) and
+  // the host staging of the last upload; jg_set is cleared by every b200mdm_set_cond* call
+  JointGuide* jg_desc = nullptr;
+  JointGuide h_jg{};
+  bool jg_set = false;
   // in-engine noise (B200MDM_FLAG_PHILOX_NOISE): counter-based Philox4x32-10 keyed by (seed, schedule index, global sample)
   unsigned long long noise_seed = 0;
   long long noise_sample_base = 0;
@@ -327,6 +338,9 @@ static int init_kernel_attrs() {
   TRY((set_attention_attr<208>()));
   TRY((set_attention_attr<256>()));
   CUDA_TRY(cudaFuncSetAttribute(cross_attention_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XAL_SMEM));
+  const int jg_smem = static_cast<int>(jg_smem_bytes(JG_MAX_FRAMES, JG_MAX_FEATS));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
   if (dev < 64) done_mask |= 1ull << dev;
   return B200MDM_OK;
 }
@@ -635,7 +649,7 @@ static void free_workspace(Workspace* w) {
   dfree(w->kvlen); dfree(w->tvec); dfree(w->action);
   dfree(w->encperm); dfree(w->memtok); dfree(w->memproj); dfree(w->mem16); dfree(w->qc16); dfree(w->kvc16); dfree(w->memmask);
   dfree(w->cross_mb); dfree(w->cross_u); dfree(w->cross_b); dfree(w->cross_c);
-  dfree(w->tgt_valid); dfree(w->tgt_g); dfree(w->hs_desc);
+  dfree(w->tgt_valid); dfree(w->tgt_g); dfree(w->hs_desc); dfree(w->jg_x0);
   dfree(w->plms_ring); dfree(w->plms_mid); dfree(w->plms_pred);
   dfree(w->dpm_hist);
   dfree(w->vb_xs); dfree(w->vb_part); dfree(w->vb_terms);
@@ -671,6 +685,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   dfree(e->chain_mem); dfree(e->chain_mask); dfree(e->chain_prefix);
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
+  dfree(e->jg_desc);
   if (e->work) cudaStreamDestroy(e->work);
   if (e->ev_in) cudaEventDestroy(e->ev_in);
   if (e->ev_out) cudaEventDestroy(e->ev_out);
@@ -1208,6 +1223,7 @@ static void end_cond(b200mdm_engine* e) {
   e->inpaint_weight = nullptr;
   e->inpaint_motion = nullptr;
   e->hs_set = false;
+  e->jg_set = false;
   e->vb_live = false;
   e->chain_next = -1;
 }
@@ -1389,6 +1405,7 @@ extern "C" int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t
   if (h < 0) return fail(B200MDM_EINVAL, "handshake size %d < 0", h);
   if (e->dec && !e->dec_clip) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented for prefix-completion (DiP) models");
   if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
+  if (e->jg_set) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented with joint-position control");
   TRY(handshake_desc(h, e->B, e->T, lengths_host, motion_start_host, &e->h_hs));
   e->hs_set = false;
   if (e->h_hs.empty()) return B200MDM_OK;   // nothing to blend: the plain forward
@@ -1397,6 +1414,34 @@ extern "C" int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t
   CUDA_TRY(cudaMemcpyAsync(e->hs_desc, e->h_hs.data(), e->h_hs.size() * sizeof(int), cudaMemcpyHostToDevice,
                            static_cast<cudaStream_t>(stream)));
   e->hs_set = true;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_dev, const float* std_dev,
+                                          const float* target_dev, const float* weight_dev, float step, int32_t iters,
+                                          void* stream) {
+  if (!e || !mean_dev || !std_dev || !target_dev || !weight_dev) return fail(B200MDM_EINVAL, "null argument");
+  if (!std::isfinite(step) || step <= 0.f) return fail(B200MDM_EINVAL, "guidance step %g: a finite value > 0", step);
+  if (iters < 1 || iters > 10000) return fail(B200MDM_EINVAL, "guidance iterations %d outside 1 .. 10000", iters);
+  if (e->cfg.nfeats != 1 || (e->JF != 263 && e->JF != 251))
+    return fail(B200MDM_EINVAL, "joint-position control needs the ric features of HumanML3D (263) or KIT (251) with nfeats 1 "
+                "(got %d x %d)", e->cfg.njoints, e->cfg.nfeats);
+  if (e->dec && !e->dec_clip)
+    return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented for prefix-completion (DiP) models");
+  if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
+  if (e->hs_set) return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented with handshakes");
+  if (e->T > JG_MAX_FRAMES) return fail(B200MDM_ENOTIMPL, "joint-position control: at most %d frames", JG_MAX_FRAMES);
+  if (!e->jg_desc) TRY(dalloc(&e->jg_desc, 1));
+  if (!e->jg_x0) TRY(dalloc(&e->jg_x0, static_cast<size_t>(e->B) * e->JF * e->T));
+  e->h_jg = JointGuide{mean_dev, std_dev, target_dev, weight_dev, step, iters};
+  CUDA_TRY(cudaMemcpyAsync(e->jg_desc, &e->h_jg, sizeof(JointGuide), cudaMemcpyHostToDevice, static_cast<cudaStream_t>(stream)));
+  e->jg_set = true;
+  return B200MDM_OK;
+}
+
+// ENOTIMPL for the samplers joint-position control does not support, while it is set
+static int refuse_joint_guidance(const b200mdm_engine* e, const char* what) {
+  if (e->jg_set) return fail(B200MDM_ENOTIMPL, "%s with joint-position control is not implemented", what);
   return B200MDM_OK;
 }
 
@@ -1417,10 +1462,10 @@ struct StepArgs {
   bool model_only = false;        // b200mdm_denoise: the bare model output, without the engine's inpainting
 };
 
-// The output projection of the CFG-blended g16 rows with the update of a.mode fused into its epilogue (p: the tables,
-// the step state and the inpainting inputs), launched on the mode's GEMM instantiation.
-static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, int B, int T, int JF, int d,
-                           const StepArgs& a, EpiOutParams p, cudaStream_t s, int sms) {
+// The per-step fields of the output step's parameters (p already holds the tables, the step state and the inpainting
+// inputs): the output GEMM's epilogue and the joint-guidance step kernel read the same.
+static void set_step_params(EpiOutParams* pp, const StepArgs& a, int B, int T, int JF) {
+  EpiOutParams& p = *pp;
   p.x_t = a.x_in;
   p.noise = a.noise;
   p.x_out = a.x_out;
@@ -1432,6 +1477,12 @@ static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, 
   p.clip_denoised = a.clip;
   p.order = a.order;
   p.back = a.back;
+}
+// The output projection of the CFG-blended g16 rows with the update of a.mode fused into its epilogue, launched on the
+// mode's GEMM instantiation.
+static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, int B, int T, int JF, int d,
+                           const StepArgs& a, EpiOutParams p, cudaStream_t s, int sms) {
+  set_step_params(&p, a, B, T, JF);
   const int M = B * T, N = ((JF + 95) / 96) * 96, K = 3 * d;
   if (a.mode <= MODE_DDIM) return launch_gemm<96, EpiOut<OutStep>>(m_g16, m_wout, M, N, K, p, s, sms);
   if (a.mode == MODE_DDIM_REVERSE) return launch_gemm<96, EpiOut<OutReverse>>(m_g16, m_wout, M, N, K, p, s, sms);
@@ -1612,8 +1663,27 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     p.x_start = e->vb_xs;
     p.vb_part = e->vb_part;
     p.state = e->state;
-    TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, a, p, s, e->num_sms));
-    ++nk;
+    if (e->jg_set && !a.model_only) {
+      // joint-position control: the output GEMM writes the raw x0, the guidance kernel runs the step's tail on it
+      StepArgs ax = a;
+      ax.mode = MODE_X0;
+      ax.x_out = e->jg_x0;
+      ax.pred = nullptr;
+      ax.clip = 0;
+      EpiOutParams px = p;
+      px.inpaint_mask = nullptr;
+      px.inpaint_weight = nullptr;
+      px.inpaint_motion = nullptr;
+      TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, ax, px, s, e->num_sms));
+      set_step_params(&p, a, B, T, JF);
+      const int R = 4 + 3 * ((JF == 263 ? 22 : 21) - 1);
+      CUDA_TRY(launch_k(joint_guidance_step_kernel, dim3(B), dim3(JG_THREADS), jg_smem_bytes(T, R), s,
+                        static_cast<const JointGuide*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
+      nk += 2;
+    } else {
+      TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, a, p, s, e->num_sms));
+      ++nk;
+    }
   }
   if (a.mode == MODE_VB) {
     TRY(launch_vb_reduce(e->vb_terms, e->vb_cap, e->vb_part, B, T, JF, e->state, s));
@@ -1707,6 +1777,7 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
     TRY(check_flags("DDIM inversion", flags, B200MDM_FLAG_CLIP_DENOISED));
     TRY(need_table(e, TAB_NEXT));
     if (e->hs_set) return fail(B200MDM_ENOTIMPL, "DDIM inversion with handshakes is not implemented");
+    TRY(refuse_joint_guidance(e, "DDIM inversion"));
   }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, index, nullptr, 0, e->noise_seed, e->noise_sample_base, e->n_steps);
@@ -1811,6 +1882,7 @@ static int loop_enter(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32
     key.imask = e->inpaint_mask; key.iweight = e->inpaint_weight; key.imotion = e->inpaint_motion;
     key.target_g = e->target_set ? e->tgt_g : nullptr;
     key.hs = e->hs_set ? e->hs_desc : nullptr;
+    key.guided = e->jg_set;
     TRY(ensure_step_graph(e, key, a));
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
     CUDA_TRY(cudaStreamWaitEvent(e->work, e->ev_in, 0));
@@ -1928,6 +2000,7 @@ extern "C" int b200mdm_ddim_reverse_loop_range(b200mdm_engine* e, int32_t first_
   if (n_run > e->n_steps - first_index) return fail(B200MDM_EINVAL, "bad step range");
   TRY(need_table(e, TAB_NEXT));
   if (e->hs_set) return fail(B200MDM_ENOTIMPL, "DDIM inversion with handshakes is not implemented");
+  TRY(refuse_joint_guidance(e, "DDIM inversion"));
   return run_loop(e, loop_args(e, B200MDM_MODE_DDIM_REVERSE, 0, flags, false), flags, first_index, n_run, x_in_dev, x_out_dev,
                   nullptr, 0, use_graph, stream);
 }
@@ -1950,6 +2023,7 @@ extern "C" int b200mdm_plms_loop_range(b200mdm_engine* e, int32_t order, int32_t
   TRY(check_range_down(e, first_index, n_run));
   if (!x_in_dev && (e->plms_done < 0 || e->plms_order != order))
     return fail(B200MDM_ESTATE, "no PLMS loop of order %d to continue (pass x_in_dev)", order);
+  TRY(refuse_joint_guidance(e, "PLMS"));
   TRY(ensure_plms(e));
   // every step after the improved-Euler one is an Adams-Bashforth step: the launches of a DDIM step, one graph per order
   const int done = x_in_dev ? 0 : e->plms_done;
@@ -1975,6 +2049,7 @@ extern "C" int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order
     if (!old_eps_dev[n_old - h + j]) return fail(B200MDM_EINVAL, "null eps history entry %d", n_old - h + j);
   TRY(check_ready(e, true));
   if (index < 0 || index >= e->n_steps) return fail(B200MDM_EINVAL, "schedule index out of range");
+  TRY(refuse_joint_guidance(e, "PLMS"));
   TRY(ensure_plms(e));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t n = static_cast<size_t>(e->B) * e->JF * e->T, x_bytes = n * sizeof(float);
@@ -2024,6 +2099,7 @@ extern "C" int b200mdm_dpm_loop_range(b200mdm_engine* e, int32_t order, int32_t 
   TRY(need_table(e, TAB_DPM));
   if (!x_in_dev && (e->dpm_done < 0 || e->dpm_order != order))
     return fail(B200MDM_ESTATE, "no DPM-Solver++ loop of order %d to continue (pass x_in_dev)", order);
+  TRY(refuse_joint_guidance(e, "DPM-Solver++"));
   TRY(ensure_dpm(e));
   const int done = x_in_dev ? 0 : e->dpm_done;
   return run_loop(e, loop_args(e, MODE_DPM, order, flags, false), flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0,
@@ -2228,6 +2304,7 @@ extern "C" int b200mdm_vb_loop_range(b200mdm_engine* e, int32_t first_index, int
   TRY(need_table(e, TAB_VB));
   if (!x_start_dev && !e->vb_live) return fail(B200MDM_ESTATE, "no bound loop to continue (pass x_start_dev)");
   if (e->hs_set) return fail(B200MDM_ENOTIMPL, "the variational bound with handshakes is not implemented");
+  TRY(refuse_joint_guidance(e, "the variational bound"));
   TRY(ensure_vb(e));
   if (!x_start_dev && !e->vb_live)   // ensure_vb reallocated the tables for a longer schedule: nothing to continue
     return fail(B200MDM_ESTATE, "the schedule outgrew the bound loop's tables: no bound loop to continue (pass x_start_dev)");
@@ -2663,6 +2740,23 @@ extern "C" int b200mdm_debug_ln_trace(uint64_t* host_out, int32_t* dims) {
   return B200MDM_OK;
 }
 #endif
+
+extern "C" int b200mdm_test_joint_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev,
+                                           const float* target_dev, const float* weight_dev, int32_t B, int32_t T, int32_t D,
+                                           float step, int32_t iters, float* x0_out_dev, float* loss_out_dev, void* stream) {
+  if (!x0_dev || !mean_dev || !std_dev || !target_dev || !weight_dev || !x0_out_dev) return fail(B200MDM_EINVAL, "null argument");
+  if (!std::isfinite(step) || step <= 0.f) return fail(B200MDM_EINVAL, "guidance step %g: a finite value > 0", step);
+  if (iters < 1 || iters > 10000) return fail(B200MDM_EINVAL, "guidance iterations %d outside 1 .. 10000", iters);
+  if (D != 263 && D != 251) return fail(B200MDM_EINVAL, "D %d: 263 (HumanML3D) or 251 (KIT)", D);
+  if (B < 1 || T < 1 || T > JG_MAX_FRAMES) return fail(B200MDM_EINVAL, "B %d, T %d: B >= 1, 1 <= T <= %d", B, T, JG_MAX_FRAMES);
+  TRY(init_kernel_attrs());
+  const JointGuide g{mean_dev, std_dev, target_dev, weight_dev, step, iters};
+  const int R = D == 263 ? 67 : 64;
+  joint_guidance_test_kernel<<<B, JG_THREADS, jg_smem_bytes(T, R), static_cast<cudaStream_t>(stream)>>>(
+      g, x0_dev, x0_out_dev, loss_out_dev, B, T, D);
+  CUDA_TRY(cudaGetLastError());
+  return B200MDM_OK;
+}
 
 // ------------------------------------------------------------------------------------------------ post-processing
 extern "C" int b200mdm_recover_from_ric(const float* data_dev, int64_t stride_b, int64_t stride_f, int64_t stride_t,

@@ -566,6 +566,18 @@ __device__ __forceinline__ float soft_inpaint(float x0, float w, const float* mo
   return __fadd_rn(__fmul_rn(__fsub_rn(1.f, w), x0), __fmul_rn(w, *motion));
 }
 
+// The per-element tail of the output step, after x0 is formed: inpainting (bool mask or soft weight), the clamp of
+// clip_denoised, then the update's store.  The output epilogue and the joint-guidance step kernel (joint_guidance.cuh)
+// share it.
+template <class Update>
+__device__ __forceinline__ void out_tail(const EpiOutParams& p, const Update& u, size_t idx, float x0,
+                                         const typename Update::In& v) {
+  if (p.inpaint_mask != nullptr && p.inpaint_mask[idx]) x0 = p.inpaint_motion[idx];
+  if (p.inpaint_weight != nullptr) x0 = soft_inpaint(x0, p.inpaint_weight[idx], p.inpaint_motion + idx);
+  if (p.clip_denoised) x0 = fminf(fmaxf(x0, -1.f), 1.f);
+  u.store(p, idx, x0, v);
+}
+
 // One GEMM instantiation per update family, so that the PLMS, inversion, DPM-Solver++ and bound epilogues leave the
 // DDPM / DDIM kernel as it is.
 template <class Update>
@@ -594,11 +606,7 @@ struct EpiOut {
         const int col = col0 + h + j;
         if (col >= p.J) continue;
         const size_t idx = base + static_cast<size_t>(col) * p.T;
-        float x0 = __uint_as_float(raw[h + j]) + __ldg(p.bias + col);
-        if (p.inpaint_mask != nullptr && p.inpaint_mask[idx]) x0 = p.inpaint_motion[idx];
-        if (p.inpaint_weight != nullptr) x0 = soft_inpaint(x0, p.inpaint_weight[idx], p.inpaint_motion + idx);
-        if (p.clip_denoised) x0 = fminf(fmaxf(x0, -1.f), 1.f);
-        u.store(p, idx, x0, v[j]);
+        out_tail(p, u, idx, __uint_as_float(raw[h + j]) + __ldg(p.bias + col), v[j]);
       }
     }
     u.end(p, row, col0);

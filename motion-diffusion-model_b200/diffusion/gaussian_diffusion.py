@@ -214,6 +214,12 @@ class GaussianDiffusion:
             raise NotImplementedError("%s with HandshakeSampleModel is not implemented" % what)
 
     @staticmethod
+    def _reject_joint_control(model, what):
+        from ..model.mdm import joint_control_of
+        if joint_control_of(model) is not None:
+            raise NotImplementedError("%s with joint-position control (JointControlSampleModel) is not implemented" % what)
+
+    @staticmethod
     def _soft_inpainting(y, shape):
         """(weight, motion) of y['inpainting_weight'] / y['inpainted_motion'] (DESIGN.md, "Refined transitions"), or None
         without a weight.  ValueError, before any engine work, for a weight next to y['inpainting_mask'], a weight without
@@ -239,6 +245,9 @@ class GaussianDiffusion:
         model_kwargs = model_kwargs if model_kwargs is not None else {}
         y = model_kwargs.get("y", {})
         soft = self._soft_inpainting(y, shape)
+        from ..model.mdm import joint_control_of
+        jc = joint_control_of(model)
+        joint = jc.targets(y, shape) if jc is not None else None
         eng, guided = self._engine_of(model)
         if "text" in y.keys():                       # encode once, mutate y like the reference (:633-635)
             y["text_embed"] = model.encode_text(y["text"])
@@ -255,6 +264,9 @@ class GaussianDiffusion:
             eng.set_inpaint(y["inpainting_mask"].to(device), y["inpainted_motion"].to(device))
         else:
             eng.set_inpaint(None, None)
+        if joint is not None:
+            eng.set_joint_guidance(jc.mean.to(device), jc.std.to(device), joint[0].to(device), joint[1].to(device),
+                                   jc.step_size, jc.n_iters)
         return eng
 
     @staticmethod
@@ -487,6 +499,7 @@ class GaussianDiffusion:
         if eta != 0.0:
             raise AssertionError("Reverse ODE only for deterministic path")
         self._reject_handshake(model, "DDIM inversion")
+        self._reject_joint_control(model, "DDIM inversion")
         self._reject_hooks(denoised_fn, None, False, False)
         idx = int(t.reshape(-1)[0].item())
         assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch"
@@ -500,6 +513,7 @@ class GaussianDiffusion:
         iterated for i = first_index ... first_index + n_steps - 1 (default: the whole schedule, 0 ... n - 1), as one
         engine call (every step a replay of one CUDA graph).  Returns the last step's sample; x_start is not modified."""
         self._reject_handshake(model, "DDIM inversion")
+        self._reject_joint_control(model, "DDIM inversion")
         first, n_run = self._reverse_range(first_index, n_steps)
         if device is None:
             device = next(model.parameters()).device
@@ -515,6 +529,7 @@ class GaussianDiffusion:
         """ddim_reverse_sample_loop as a generator of the reference step's {'sample', 'pred_xstart'}, one step call per
         yield, for i = first_index ... first_index + n_steps - 1."""
         self._reject_handshake(model, "DDIM inversion")
+        self._reject_joint_control(model, "DDIM inversion")
         first, n_run = self._reverse_range(first_index, n_steps)
         if device is None:
             device = next(model.parameters()).device
@@ -545,6 +560,7 @@ class GaussianDiffusion:
         old_out['old_eps'], which is extended with this step's eps and trimmed in place as in the reference.  order must be an integer from 1 to 4
         (ValueError otherwise, including non-integers such as 2.5)."""
         order = self._plms_order(order, old_out)
+        self._reject_joint_control(model, "PLMS")
         self._reject_hooks(denoised_fn, cond_fn, False, cond_fn_with_grad)
         idx = int(t.reshape(-1)[0].item())
         assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch (gaussian_diffusion.py:1166)"
@@ -567,6 +583,7 @@ class GaussianDiffusion:
         replays of one CUDA graph).  PLMS draws no per-step noise: the only draw is x_T, from torch's generator or, with
         `noise_seed` (+ `sample_index_base`), from the engine's Philox stream.  order: see plms_sample."""
         order = self._plms_order(order)
+        self._reject_joint_control(model, "PLMS")
         if noise_tape is not None:
             raise ValueError("PLMS draws no per-step noise: a noise_tape has no use (sample it with noise_mode='philox')")
         self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
@@ -588,6 +605,7 @@ class GaussianDiffusion:
                                      randomize_class=False, cond_fn_with_grad=False, order=2):
         """reference gaussian_diffusion.py:1118-1187: generator of {'sample', 'pred_xstart', 'old_eps'} per step."""
         order = self._plms_order(order)
+        self._reject_joint_control(model, "PLMS")
         self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
         assert isinstance(shape, (tuple, list))
         if device is None:
@@ -618,6 +636,7 @@ class GaussianDiffusion:
                    noise_seed, sample_index_base):
         """Argument checks (before any engine work), the tables, conditioning and x_T of a DPM-Solver++ loop."""
         order = self._dpm_order(order)
+        self._reject_joint_control(model, "DPM-Solver++")
         if noise_tape is not None:
             raise ValueError("DPM-Solver++ draws no per-step noise: a noise_tape has no use")
         if dump_steps is not None or const_noise:
@@ -768,6 +787,7 @@ class GaussianDiffusion:
         """reference gaussian_diffusion.py:270-381: {'mean', 'variance', 'log_variance', 'pred_xstart'} of p(x_{t-1} | x_t).
         One engine forward: the DDPM step at zero noise, whose sample is the model mean (bit for bit that step's mean)
         and whose pred_xstart is p_sample's.  t: LongTensor [B] of one schedule index."""
+        self._reject_joint_control(model, "p_mean_variance")
         self._reject_hooks(denoised_fn, None, False, False)
         idx = int(t.reshape(-1)[0].item())
         assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch (gaussian_diffusion.py:709)"
@@ -787,6 +807,7 @@ class GaussianDiffusion:
         `noise_tape` [num_timesteps, *x_start.shape] replaces the draws, `noise_seed` (+ `sample_index_base`) switches
         them to the engine's Philox stream (the eps a sampling loop of that seed would draw at the same index)."""
         self._reject_handshake(model, "The variational bound")
+        self._reject_joint_control(model, "The variational bound")
         if noise_tape is not None and noise_seed is not None:
             raise ValueError("noise_seed excludes noise_tape")
         self._model_log_variance()                           # NotImplementedError for learned variances

@@ -51,6 +51,19 @@ def canonical_target(y, batch, joint_names):
     return tc, valid
 
 
+def joint_guidance_hook(x0, mean, std, target, weight, step, iters):
+    """The guidance iterations of joint-position control alone (b200mdm_test_joint_guidance), on x0's device:
+    (guided x0 [B, D, T], loss [iters + 1, B])."""
+    lib = _lib.load()
+    x0, mean, std, target, weight = (t.to(torch.float32).contiguous() for t in (x0, mean, std, target, weight))
+    B, D, T = int(x0.shape[0]), int(x0.shape[1]), int(x0.shape[-1])
+    out = torch.empty_like(x0)
+    loss = torch.empty((int(iters) + 1, B), device=x0.device, dtype=torch.float32)
+    check(lib.b200mdm_test_joint_guidance(_ptr(x0), _ptr(mean), _ptr(std), _ptr(target), _ptr(weight), B, T, D,
+                                          float(step), int(iters), _ptr(out), _ptr(loss), _stream()))
+    return out, loss
+
+
 class Engine:
     """One engine per model instance (weights + workspace live on the current CUDA device)."""
 
@@ -329,6 +342,13 @@ class Engine:
         n, ms = np.ascontiguousarray(n), np.ascontiguousarray(ms.astype(np.uint8))
         check(self.lib.b200mdm_set_handshake(self.h, int(handshake_size), n.ctypes.data_as(ctypes.c_void_p),
                                              ms.ctypes.data_as(ctypes.c_void_p), _stream()))
+
+    def set_joint_guidance(self, mean, std, target, weight, step, iters):
+        """Joint-position control for the next DDPM / DDIM loops and steps (b200mdm_set_joint_guidance), after set_cond,
+        which clears it: mean / std [D], target [B, J, 3, T], weight [B, J, T], all on the engine's device."""
+        ts = [t.to(torch.float32).contiguous() for t in (mean, std, target, weight)]
+        check(self.lib.b200mdm_set_joint_guidance(self.h, *[_ptr(t) for t in ts], float(step), int(iters), _stream()))
+        self._keep["joint"] = ts
 
     # ------------------------------------------------------------------ compute
     def denoise(self, x, timesteps):

@@ -272,15 +272,27 @@ def _run_model(model, x, timesteps, y, guided, handshake=0):
 
 
 def _unwrap(model):
-    """(innermost model, HandshakeSampleModel or None) behind respace._WrappedModel and a HandshakeSampleModel."""
-    from ..utils.sampler_util import HandshakeSampleModel
+    """(innermost model, HandshakeSampleModel or None) behind respace._WrappedModel and a HandshakeSampleModel or
+    JointControlSampleModel."""
+    from ..utils.sampler_util import HandshakeSampleModel, JointControlSampleModel
     from ..diffusion.respace import _WrappedModel
     inner = model
     while isinstance(inner, _WrappedModel):
         inner = inner.model
     if isinstance(inner, HandshakeSampleModel):
         return inner.model, inner
+    if isinstance(inner, JointControlSampleModel):
+        return inner.model, None
     return inner, None
+
+
+def joint_control_of(model):
+    """The JointControlSampleModel a sampler was given (possibly behind respace._WrappedModel), or None."""
+    from ..utils.sampler_util import JointControlSampleModel
+    from ..diffusion.respace import _WrappedModel
+    while isinstance(model, _WrappedModel):
+        model = model.model
+    return model if isinstance(model, JointControlSampleModel) else None
 
 
 def handshake_of(model):
@@ -290,7 +302,8 @@ def handshake_of(model):
 
 def engine_for(model):
     """(engine, guided) for a bare MDM or a ClassifierFreeSampleModel wrapper (possibly behind respace._WrappedModel
-    and a HandshakeSampleModel, whose handshake the sampler sets with handshake_of).
+    and a HandshakeSampleModel or JointControlSampleModel, whose handshake / guidance the sampler sets with handshake_of
+    / joint_control_of).
 
     Only wrappers this package knows are looked through: an unknown object that merely has a `.model` attribute (for
     instance a guidance wrapper class from another import of this package, or the reference's own

@@ -122,6 +122,84 @@ class HandshakeSampleModel(nn.Module):
         return wrapped_getattr(self, name, default=None)
 
 
+class JointControlSampleModel(nn.Module):
+    """Joint-position control (this project's definition, DESIGN.md "Joint-position control"): at every DDPM / DDIM step
+    the model's x0 (after classifier-free guidance) takes `n_iters` gradient steps of size `step_size` on
+
+        G(x0) = 1/2 sum_{t,j} y['joint_weight'][b,j,t] * |recover_from_ric(x0 * std + mean)[t,j] - y['joint_target'][b,j,:,t]|^2,
+
+    before inpainting, the clamp of clip_denoised and the update.  y['joint_target'] [B, J, 3, T] is in sample_to_xyz's
+    layout and units; y['joint_weight'] [B, J, T] (float >= 0, or bool) is 0 where a joint is free.  `model` is a b200mdm
+    MDM or ClassifierFreeSampleModel of HumanML3D (263 features, J = 22) or KIT (251, J = 21); mean / std [D] are the
+    dataset's normalisation.  p_sample_loop, ddim_sample_loop (any eta), their _progressive forms, p_sample and
+    ddim_sample honour it; the other samplers, prefix-completion (DiP) models and AutoRegressiveSampler raise
+    NotImplementedError, HandshakeSampleModel and refine_transitions TypeError.  Calling the wrapper is the plain model:
+    the guidance belongs to the sampler, as inpainting does."""
+
+    def __init__(self, model, mean, std, step_size, n_iters):
+        super().__init__()
+        from ..model.mdm import MDM
+        inner = model.model if isinstance(model, ClassifierFreeSampleModel) else model
+        if not isinstance(inner, MDM):
+            raise TypeError("JointControlSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(model))
+        D = int(inner.njoints) * int(inner.nfeats)
+        if inner.data_rep != "hml_vec" or int(inner.nfeats) != 1 or D not in (263, 251):
+            raise ValueError("joint-position control needs the ric features of HumanML3D (263) or KIT (251); this model "
+                             "has data_rep %r with %d x %d features" % (inner.data_rep, inner.njoints, inner.nfeats))
+        if inner.is_prefix_comp or (inner.arch == "trans_dec" and not inner.emb_trans_dec):
+            raise NotImplementedError("joint-position control is not implemented for prefix-completion (DiP) models")
+        step, iters = float(step_size), n_iters
+        if not (np.isfinite(step) and step > 0):
+            raise ValueError("step_size must be finite and > 0 (got %r)" % step_size)
+        if isinstance(iters, bool) or not isinstance(iters, (int, np.integer)) or not 1 <= iters <= 10000:
+            raise ValueError("n_iters must be an integer in 1 .. 10000 (got %r)" % (n_iters,))
+        mean, std = (torch.as_tensor(np.asarray(v.detach().cpu() if torch.is_tensor(v) else v, dtype=np.float32)).reshape(-1)
+                     for v in (mean, std))
+        if mean.shape != (D,) or std.shape != (D,):
+            raise ValueError("mean and std need %d entries (got %s and %s)" % (D, tuple(mean.shape), tuple(std.shape)))
+        self.model = model
+        self.mean, self.std = mean, std
+        self.step_size, self.n_iters = step, int(iters)
+        self.n_joints = 22 if D == 263 else 21
+        self.rot2xyz = self.model.rot2xyz
+        self.translation = self.model.translation
+        self.njoints = self.model.njoints
+        self.nfeats = self.model.nfeats
+        self.data_rep = self.model.data_rep
+        self.cond_mode = self.model.cond_mode
+        self.encode_text = self.model.encode_text
+
+    def targets(self, y, shape):
+        """(target [B, J, 3, T], weight [B, J, T]) fp32 of y for a sample of `shape`; y is not modified.  ValueError for a
+        missing key, a shape other than these, a weight that is negative or not finite, or a target that is not finite
+        where its weight is not 0."""
+        B, T, J = int(shape[0]), int(shape[-1]), self.n_joints
+        if "joint_target" not in y or "joint_weight" not in y:
+            raise ValueError("JointControlSampleModel needs y['joint_target'] [B, %d, 3, T] and y['joint_weight'] [B, %d, T]"
+                             % (J, J))
+        c, w = y["joint_target"], y["joint_weight"]
+        if not torch.is_tensor(c) or not torch.is_tensor(w):
+            raise ValueError("y['joint_target'] and y['joint_weight'] must be tensors")
+        if tuple(c.shape) != (B, J, 3, T) or tuple(w.shape) != (B, J, T):
+            raise ValueError("y['joint_target'] %s / y['joint_weight'] %s must be %s / %s" % (
+                tuple(c.shape), tuple(w.shape), (B, J, 3, T), (B, J, T)))
+        if w.dtype != torch.bool and not w.is_floating_point():
+            raise ValueError("y['joint_weight'] must be a float or bool tensor")
+        w = w.to(torch.float32)
+        c = c.to(torch.float32)
+        if not bool((torch.isfinite(w) & (w >= 0)).all()):
+            raise ValueError("y['joint_weight'] must be finite and >= 0")
+        if not bool((torch.isfinite(c) | (w == 0)[:, :, None, :]).all()):
+            raise ValueError("y['joint_target'] must be finite where y['joint_weight'] is not 0")
+        return c, w
+
+    def forward(self, x, timesteps, y=None):
+        return self.model(x, timesteps, y)
+
+    def __getattr__(self, name, default=None):
+        return wrapped_getattr(self, name, default=None)
+
+
 def stitch_handshake(sample, lengths, handshake_size, motion_start=None):
     """The motions of a batch of chained windows (HandshakeSampleModel): for each motion, its first window's frames
     [:n], then each later window's [h:n].  sample [B, njoints, nfeats, T]; lengths [B] (None: all T); returns a list of
@@ -236,7 +314,9 @@ def refine_transitions(sample_fn, model, windows, model_kwargs, handshake_size, 
     returned as they are, with no engine call.  `model` is the plain (guided) model: a HandshakeSampleModel raises
     TypeError, a prefix-completion (DiP) model NotImplementedError; layout errors raise ValueError (transition_layout),
     as does skip_timesteps outside [0, num_timesteps).  Gather and paste are device indexing only."""
-    from ..model.mdm import _unwrap
+    from ..model.mdm import _unwrap, joint_control_of
+    if joint_control_of(model) is not None:
+        raise TypeError("refine_transitions is not implemented with joint-position control (JointControlSampleModel)")
     inner, hs = _unwrap(model)
     if hs is not None:
         raise TypeError("refine_transitions runs the plain model: pass the model a HandshakeSampleModel wraps, not the wrapper")
@@ -353,6 +433,9 @@ class AutoRegressiveSampler:
         self.required_frames = required_frames
 
     def sample(self, model, shape, **kargs):
+        from ..model.mdm import joint_control_of
+        if joint_control_of(model) is not None:
+            raise NotImplementedError("the autoregressive chain is not implemented with joint-position control")
         pred_len, context_len = self.args.pred_len, self.args.context_len
         n_iterations = self.required_frames // pred_len + int(self.required_frames % pred_len > 0)
         y0 = kargs["model_kwargs"]["y"]
