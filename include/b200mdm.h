@@ -244,6 +244,32 @@ int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t* lengths_h
 int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_dev, const float* std_dev, const float* target_dev,
                                const float* weight_dev, float step, int32_t iters, void* stream);
 
+/* Multi-prompt guidance (this project's definition, DESIGN.md "Multi-prompt guidance"): K prompts per motion, composed
+ * around the unconditional prediction as
+ *   x0[b, f, t] = x0_u + sum_{k=0..K-1} w[b, k, f, t] (x0_k - x0_u)
+ * in fp32 (k ascending, each operation rounded), then inpainting, the clamp of clip_denoised and the update.  The packed
+ * batch holds G = K + 1 groups of `batch` motions, the prompts' groups first and the unconditional one last; every group
+ * carries the lengths and the target (b200mdm_set_target).  1 <= K <= B200MDM_MAX_PROMPTS.
+ *   b200mdm_set_cond_multi (trans_enc): prompt_embed_dev fp32 [K, batch, cond_dim] device (text models) or
+ *     prompt_action_host int64 [batch, K] (action models); lengths as in b200mdm_set_cond.
+ *   b200mdm_set_cond_multi_dec (trans_dec with a CLIP memory): prompt_clip_dev fp32 [K, batch, 512] device, one memory row
+ *     per group; a prefix-completion (DiP) engine returns B200MDM_ENOTIMPL.
+ * Both clear what b200mdm_set_cond clears, and must be followed by b200mdm_set_prompt_weight: w[b, k, f, t] =
+ * weight_dev[b * stride_b + k * stride_k + f * stride_f + t * stride_t] (fp32, strides in elements, >= 0; a stride of 0
+ * broadcasts its dimension), K as given to the conditioning call.  The weights are the caller's and must stay valid until
+ * the work enqueued with them has completed; the descriptor is uploaded on `stream`, and a step graph captured with it
+ * reads it at every replay.  Every b200mdm_set_cond* clears it, and every forward returns B200MDM_ESTATE until it is set.
+ * The composition applies to b200mdm_denoise (without inpainting), b200mdm_sample_step, b200mdm_plms_step and the DDPM /
+ * DDIM, PLMS, DPM-Solver++ and DDIM-inversion loops; the variational bound, handshakes and joint-position control return
+ * B200MDM_ENOTIMPL while the conditioning is composed. */
+#define B200MDM_MAX_PROMPTS 8
+int b200mdm_set_cond_multi(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K, const float* prompt_embed_dev,
+                           const int64_t* lengths_host, const int64_t* prompt_action_host, void* stream);
+int b200mdm_set_cond_multi_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K, const float* prompt_clip_dev,
+                               const int64_t* lengths_host, void* stream);
+int b200mdm_set_prompt_weight(b200mdm_engine* e, int32_t K, const float* weight_dev, int64_t stride_b, int64_t stride_k,
+                              int64_t stride_f, int64_t stride_t, void* stream);
+
 /* MDM.forward / ClassifierFreeSampleModel.forward (model/mdm.py:189-283, utils/sampler_util.py:27-34):
  * out = model(x, timesteps, y), without inpainting (the sampler's, not the model's).  timesteps_host: int32 [batch] MODEL
  * timesteps (already mapped). */

@@ -11,7 +11,8 @@ Python here is host glue only; the per-step path is hand-written sm_90a CUDA in 
 from .utils.model_util import (create_model_and_diffusion, create_gaussian_diffusion, get_model_args,  # noqa: F401
                                load_saved_model, load_model_wo_clip)
 from .utils.sampler_util import (ClassifierFreeSampleModel, AutoRegressiveSampler, HandshakeSampleModel,  # noqa: F401
-                                 JointControlSampleModel, stitch_handshake, transition_layout, refine_transitions)
+                                 JointControlSampleModel, MultiPromptSampleModel, body_part_mask, stitch_handshake,
+                                 transition_layout, refine_transitions)
 from .diffusion.respace import SpacedDiffusion, space_timesteps  # noqa: F401
 from .diffusion.gaussian_diffusion import GaussianDiffusion, get_named_beta_schedule  # noqa: F401
 from .model.mdm import MDM  # noqa: F401

@@ -23,6 +23,7 @@
 #include "gemm_ln.cuh"
 #include "gemm_pingpong.cuh"
 #include "joint_guidance.cuh"
+#include "compose.cuh"
 #include "postprocess.cuh"
 #include "kernels.cuh"
 
@@ -146,10 +147,11 @@ struct GraphKey {
   const void* target_g = nullptr;   // the workspace's target embedding, or nullptr when the loop has no target
   const void* hs = nullptr;         // the workspace's handshake descriptor, or nullptr when the loop has none
   bool guided = false;              // joint-position control: the step ends in joint_guidance_step_kernel
+  int groups = 0;                   // multi-prompt guidance: the step ends in compose_step_kernel over G groups
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
            imask == o.imask && iweight == o.iweight && imotion == o.imotion && target_g == o.target_g && hs == o.hs &&
-           guided == o.guided;
+           guided == o.guided && groups == o.groups;
   }
 };
 
@@ -159,6 +161,11 @@ struct GraphKey {
 // loader: 32 <-> 32 x mm_num_repeats, comp_v6_model_dataset.py:148-256) neither re-allocate nor re-capture.
 struct Workspace {
   int B = 0, T = 0, S = 0, halves = 1, Bp = 0, M = 0, MB = 0;
+  // multi-prompt guidance (b200mdm_set_cond_multi*): G = K + 1 groups of B motions, Bp = G * B, the unconditional group
+  // last; 0 for the plain / CFG batch of `halves`.  g16 then holds the frame rows of every group, and mp_x0
+  // [G, B, JF, T] the raw x0 of every group, which compose_step_kernel composes.
+  int groups = 0;
+  float* mp_x0 = nullptr;
   __half *xin16 = nullptr, *hres = nullptr, *qkv16 = nullptr, *att16 = nullptr, *ffn16 = nullptr, *g16 = nullptr;
   float *tok0 = nullptr, *condproj = nullptr, *proj = nullptr, *scale = nullptr, *x_work = nullptr, *eps_buf = nullptr;
   int *kvlen = nullptr, *tvec = nullptr, *action = nullptr;
@@ -261,6 +268,11 @@ struct b200mdm_engine : Workspace {
   JointGuide* jg_desc = nullptr;
   JointGuide h_jg{};
   bool jg_set = false;
+  // multi-prompt guidance: the prompt-weight descriptor (read by the step graph at every replay, allocated on first
+  // use) and its host staging; pw_set is cleared by every b200mdm_set_cond* call
+  PromptWeight* pw_desc = nullptr;
+  PromptWeight h_pw{};
+  bool pw_set = false;
   // in-engine noise (B200MDM_FLAG_PHILOX_NOISE): counter-based Philox4x32-10 keyed by (seed, schedule index, global sample)
   unsigned long long noise_seed = 0;
   long long noise_sample_base = 0;
@@ -649,7 +661,7 @@ static void free_workspace(Workspace* w) {
   dfree(w->kvlen); dfree(w->tvec); dfree(w->action);
   dfree(w->encperm); dfree(w->memtok); dfree(w->memproj); dfree(w->mem16); dfree(w->qc16); dfree(w->kvc16); dfree(w->memmask);
   dfree(w->cross_mb); dfree(w->cross_u); dfree(w->cross_b); dfree(w->cross_c);
-  dfree(w->tgt_valid); dfree(w->tgt_g); dfree(w->hs_desc); dfree(w->jg_x0);
+  dfree(w->tgt_valid); dfree(w->tgt_g); dfree(w->hs_desc); dfree(w->jg_x0); dfree(w->mp_x0);
   dfree(w->plms_ring); dfree(w->plms_mid); dfree(w->plms_pred);
   dfree(w->dpm_hist);
   dfree(w->vb_xs); dfree(w->vb_part); dfree(w->vb_terms);
@@ -686,6 +698,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
   dfree(e->jg_desc);
+  dfree(e->pw_desc);
   if (e->work) cudaStreamDestroy(e->work);
   if (e->ev_in) cudaEventDestroy(e->ev_in);
   if (e->ev_out) cudaEventDestroy(e->ev_out);
@@ -1049,8 +1062,10 @@ extern "C" int b200mdm_set_schedule_vb(b200mdm_engine* e, int32_t n_steps, const
 // ------------------------------------------------------------------------------------------------ cond / workspace
 static void attach_l2_window(b200mdm_engine* e, cudaStream_t stream = nullptr);
 
-static int build_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStream_t s) {
-  const int d = e->d, S = T + e->s_off, Bp = halves * B;
+static int build_workspace(b200mdm_engine* e, int B, int T, int halves, int groups, cudaStream_t s) {
+  const int d = e->d, S = T + e->s_off, Bp = (groups ? groups : halves) * B;
+  const size_t g16_rows = static_cast<size_t>(groups ? Bp : B) * T;     // frame rows of the blend's output
+  const int cond_rows = groups ? Bp - B : B;                             // rows of proj / action: the conditional ones
   const size_t M = static_cast<size_t>(Bp) * S, MB = static_cast<size_t>(B) * S;
   TRY(dalloc(&e->xin16, MB * 3 * e->Kp_in, true));
   const int kw = e->kw;
@@ -1058,15 +1073,16 @@ static int build_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStre
   TRY(dalloc(&e->qkv16, M * 3 * d));
   TRY(dalloc(&e->att16, M * d * kw));
   TRY(dalloc(&e->ffn16, M * e->ff * kw));
-  TRY(dalloc(&e->g16, static_cast<size_t>(B) * T * 3 * d));           // frame rows only
+  TRY(dalloc(&e->g16, g16_rows * 3 * d));                              // frame rows only
   TRY(dalloc(&e->tok0, static_cast<size_t>(Bp) * d));
   TRY(dalloc(&e->condproj, static_cast<size_t>(Bp) * d, true));
-  TRY(dalloc(&e->proj, static_cast<size_t>(B) * d, true));
+  TRY(dalloc(&e->proj, static_cast<size_t>(cond_rows) * d, true));
   TRY(dalloc(&e->scale, B, true));
   TRY(dalloc(&e->x_work, static_cast<size_t>(B) * e->JF * T));
   TRY(dalloc(&e->kvlen, Bp));
   TRY(dalloc(&e->tvec, B, true));
-  TRY(dalloc(&e->action, B, true));
+  TRY(dalloc(&e->action, cond_rows, true));
+  if (groups) TRY(dalloc(&e->mp_x0, static_cast<size_t>(Bp) * e->JF * T));
   if (e->dec_clip) {
     const size_t rows = static_cast<size_t>(Bp) * d, all = static_cast<size_t>(e->L) * Bp * d;
     TRY(dalloc(&e->cross_mb, rows));
@@ -1079,7 +1095,7 @@ static int build_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStre
     e->Mt = 0;              // the text-memory buffers are sized by the packed batch: b200mdm_set_cond_dec rebuilds them
     e->prefix_set = false;  // xin16 was reallocated
   }
-  e->B = B; e->T = T; e->S = S; e->halves = halves; e->Bp = Bp;
+  e->B = B; e->T = T; e->S = S; e->halves = halves; e->groups = groups; e->Bp = Bp;
   e->M = static_cast<int>(M); e->MB = static_cast<int>(MB);
   attach_l2_window(e);
   TRY(make_map(&e->m_xin, e->xin16, MB, 3 * e->Kp_in, 3 * e->Kp_in, GEMM_BLOCK_M));
@@ -1087,12 +1103,14 @@ static int build_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStre
   TRY(make_map(&e->m_h16, e->hres, M, kw * d, 2 * d, GEMM_BLOCK_M));
   TRY(make_map(&e->m_att, e->att16, M, kw * d, kw * d, GEMM_BLOCK_M));
   TRY(make_map(&e->m_ffn, e->ffn16, M, kw * e->ff, kw * e->ff, GEMM_BLOCK_M));
-  TRY(make_map(&e->m_g16, e->g16, static_cast<size_t>(B) * T, 3 * d, 3 * d, GEMM_BLOCK_M));
+  TRY(make_map(&e->m_g16, e->g16, g16_rows, 3 * d, 3 * d, GEMM_BLOCK_M));
   TRY(make_map_t(&e->m_qkv_st, e->qkv16, 2, M, 3 * d, 3 * d, 32));
   TRY(make_attention_kv_map(&e->m_qkv_kv, e->qkv16, Bp, S, 3 * d));
   TRY(make_map_t(&e->m_ffn_st, e->ffn16, 2, M, kw * e->ff, kw * e->ff, 32));
   TRY(make_map_res(&e->m_res_c, e->hres, MB, d));
-  TRY(make_map_res(&e->m_res_u, e->hres + (halves == 2 ? MB * d * 2 : 0), MB, d));
+  // the embedding GEMM's second copy of the frame rows: the unconditional half, or the last (unconditional) group
+  const int last = groups ? groups - 1 : halves - 1;
+  TRY(make_map_res(&e->m_res_u, e->hres + static_cast<size_t>(last) * MB * d * 2, MB, d));
   TRY(make_hres_map(&e->m_hres, e->hres, M));
   TRY(dalloc(&e->pe_bias, static_cast<size_t>(S) * d));
   pe_bias_kernel<<<S, 128, 0, s>>>(e->pe_bias, e->pe, e->b_in, S, d);   // on the caller's stream: ordered before any forward
@@ -1132,19 +1150,19 @@ static void attach_l2_window(b200mdm_engine* e, cudaStream_t stream) {
   }
 }
 
-// Make the workspace for (B, T, halves) the current one: the one in use if it matches, else a parked one, else a new
-// one (the least recently used of more than `MAX_PARKED` parked workspaces is freed).
-static int select_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStream_t s) {
+// Make the workspace for (B, T, halves, groups) the current one: the one in use if it matches, else a parked one, else a
+// new one (the least recently used of more than `MAX_PARKED` parked workspaces is freed).
+static int select_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStream_t s, int groups = 0) {
   constexpr size_t MAX_PARKED = 3;
   Workspace* cur = static_cast<Workspace*>(e);
   e->last_use = ++e->use_clock;
-  if (cur->B == B && cur->T == T && cur->halves == halves) return B200MDM_OK;
+  if (cur->B == B && cur->T == T && cur->halves == halves && cur->groups == groups) return B200MDM_OK;
   if (cur->B > 0) {
     e->pool.push_back(*cur);
     *cur = Workspace();
   }
   for (size_t i = 0; i < e->pool.size(); ++i) {
-    if (e->pool[i].B == B && e->pool[i].T == T && e->pool[i].halves == halves) {
+    if (e->pool[i].B == B && e->pool[i].T == T && e->pool[i].halves == halves && e->pool[i].groups == groups) {
       *cur = e->pool[i];
       e->pool.erase(e->pool.begin() + i);
       cur->last_use = e->use_clock;
@@ -1163,7 +1181,7 @@ static int select_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStr
     free_workspace(&e->pool[lru]);
     e->pool.erase(e->pool.begin() + lru);
   }
-  int r = build_workspace(e, B, T, halves, s);
+  int r = build_workspace(e, B, T, halves, groups, s);
   if (r != B200MDM_OK) free_workspace(cur);
   cur->last_use = e->use_clock;
   return r;
@@ -1199,9 +1217,11 @@ static int upload_kvlen_scale(b200mdm_engine* e, int nframes, int seq_extra, boo
   return B200MDM_OK;
 }
 // condproj rows of the packed batch: proj = embed_text(text) [B, d] when the model is text-conditioned and a text is given
-// (model/mdm.py:218), then the conditional / unconditional rows of the model's conditioning mode (condproj_fill_kernel)
-static int fill_condproj(b200mdm_engine* e, const float* text_dev, bool uncond, cudaStream_t s) {
-  const int B = e->B, d = e->d;
+// (model/mdm.py:218), then the conditional / unconditional rows of the model's conditioning mode (condproj_fill_kernel).
+// With multi-prompt guidance, B = K * batch conditional rows (text_dev [K, batch, C], action [K * batch]) come first.
+static int fill_condproj(b200mdm_engine* e, const float* text_dev, bool uncond, cudaStream_t s, int B = 0) {
+  const int d = e->d;
+  if (B == 0) B = e->B;
   if (e->cfg.cond_mode == B200MDM_COND_TEXT && text_dev) {
     const size_t warps = static_cast<size_t>(B) * d;
     small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(text_dev, e->w_txt, e->b_txt, e->proj, B, d,
@@ -1224,6 +1244,7 @@ static void end_cond(b200mdm_engine* e) {
   e->inpaint_motion = nullptr;
   e->hs_set = false;
   e->jg_set = false;
+  e->pw_set = false;
   e->vb_live = false;
   e->chain_next = -1;
 }
@@ -1406,6 +1427,7 @@ extern "C" int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t
   if (e->dec && !e->dec_clip) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented for prefix-completion (DiP) models");
   if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
   if (e->jg_set) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented with joint-position control");
+  if (e->groups) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented with multi-prompt guidance");
   TRY(handshake_desc(h, e->B, e->T, lengths_host, motion_start_host, &e->h_hs));
   e->hs_set = false;
   if (e->h_hs.empty()) return B200MDM_OK;   // nothing to blend: the plain forward
@@ -1430,6 +1452,7 @@ extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_d
     return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented for prefix-completion (DiP) models");
   if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
   if (e->hs_set) return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented with handshakes");
+  if (e->groups) return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented with multi-prompt guidance");
   if (e->T > JG_MAX_FRAMES) return fail(B200MDM_ENOTIMPL, "joint-position control: at most %d frames", JG_MAX_FRAMES);
   if (!e->jg_desc) TRY(dalloc(&e->jg_desc, 1));
   if (!e->jg_x0) TRY(dalloc(&e->jg_x0, static_cast<size_t>(e->B) * e->JF * e->T));
@@ -1442,6 +1465,86 @@ extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_d
 // ENOTIMPL for the samplers joint-position control does not support, while it is set
 static int refuse_joint_guidance(const b200mdm_engine* e, const char* what) {
   if (e->jg_set) return fail(B200MDM_ENOTIMPL, "%s with joint-position control is not implemented", what);
+  return B200MDM_OK;
+}
+
+// ---- multi-prompt guidance (DESIGN.md, "Multi-prompt guidance")
+static int check_prompts(int32_t batch, int32_t nframes, int32_t K) {
+  if (batch <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
+  if (K < 1 || K > MP_MAX_PROMPTS) return fail(B200MDM_EINVAL, "prompt count %d outside 1 .. %d", K, MP_MAX_PROMPTS);
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_cond_multi(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K,
+                                      const float* prompt_embed_dev, const int64_t* lengths_host,
+                                      const int64_t* prompt_action_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (e->dec) return fail(B200MDM_EINVAL, "trans_dec engines take their prompts through b200mdm_set_cond_multi_dec");
+  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
+  TRY(check_prompts(batch, nframes, K));
+  TRY(check_seq_len(e, nframes + 1));
+  if (e->cfg.cond_mode == B200MDM_COND_NONE)
+    return fail(B200MDM_EINVAL, "multi-prompt guidance needs a conditioned model (sampler_util.py:29)");
+  if (e->cfg.cond_mode == B200MDM_COND_TEXT && !prompt_embed_dev)
+    return fail(B200MDM_EINVAL, "text-conditioned model needs the prompt embeddings [K, B, C]");
+  std::vector<int>& a = e->h_action;
+  if (e->cfg.cond_mode == B200MDM_COND_ACTION) {
+    if (!prompt_action_host) return fail(B200MDM_EINVAL, "action-conditioned model needs the prompt actions [B, K]");
+    a.assign(static_cast<size_t>(K) * batch, 0);
+    for (int b = 0; b < batch; ++b)
+      for (int k = 0; k < K; ++k) {
+        const int64_t v = prompt_action_host[static_cast<size_t>(b) * K + k];
+        if (v < 0 || v >= e->cfg.num_actions) return fail(B200MDM_EINVAL, "action index out of range");
+        a[static_cast<size_t>(k) * batch + b] = static_cast<int>(v);   // group-major, as the packed batch
+      }
+  }
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  TRY(select_workspace(e, batch, nframes, 1, s, K + 1));
+  TRY(upload_kvlen_scale(e, nframes, 1, nframes > 1, lengths_host, nullptr, s));
+  if (e->cfg.cond_mode == B200MDM_COND_ACTION)
+    CUDA_TRY(cudaMemcpyAsync(e->action, a.data(), a.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  TRY(fill_condproj(e, prompt_embed_dev, false, s, K * batch));
+  end_cond(e);
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_cond_multi_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K,
+                                          const float* prompt_clip_dev, const int64_t* lengths_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!e->dec) return fail(B200MDM_EINVAL, "b200mdm_set_cond_multi_dec is for trans_dec engines");
+  if (!e->dec_clip)
+    return fail(B200MDM_ENOTIMPL, "multi-prompt guidance is not implemented for prefix-completion (DiP) models");
+  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
+  TRY(check_prompts(batch, nframes, K));
+  if (!prompt_clip_dev) return fail(B200MDM_EINVAL, "the CLIP decoder needs the prompt embeddings [K, B, C]");
+  TRY(check_seq_len(e, nframes + 1));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  TRY(select_workspace(e, batch, nframes, 1, s, K + 1));
+  TRY(upload_kvlen_scale(e, nframes, 1, nframes > 1, lengths_host, nullptr, s));
+  // one memory row per group: W clip_k + b for the prompts, b for the unconditional group
+  TRY(fill_condproj(e, prompt_clip_dev, false, s, K * batch));
+  TRY(cross_rows_per_sample(e, nullptr, s));
+  end_cond(e);
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_prompt_weight(b200mdm_engine* e, int32_t K, const float* weight_dev, int64_t stride_b,
+                                         int64_t stride_k, int64_t stride_f, int64_t stride_t, void* stream) {
+  if (!e || !weight_dev) return fail(B200MDM_EINVAL, "null argument");
+  if (stride_b < 0 || stride_k < 0 || stride_f < 0 || stride_t < 0) return fail(B200MDM_EINVAL, "negative weight stride");
+  if (!e->cond_set || e->groups == 0)
+    return fail(B200MDM_ESTATE, "call b200mdm_set_cond_multi / b200mdm_set_cond_multi_dec first (they clear the weights)");
+  if (K != e->groups - 1) return fail(B200MDM_EINVAL, "%d prompt weights for %d prompts", K, e->groups - 1);
+  if (!e->pw_desc) TRY(dalloc(&e->pw_desc, 1));
+  e->h_pw = PromptWeight{weight_dev, stride_b, stride_k, stride_f, stride_t, K};
+  CUDA_TRY(cudaMemcpyAsync(e->pw_desc, &e->h_pw, sizeof(PromptWeight), cudaMemcpyHostToDevice, static_cast<cudaStream_t>(stream)));
+  e->pw_set = true;
+  return B200MDM_OK;
+}
+
+// ENOTIMPL for what multi-prompt guidance does not support, while the conditioning is composed
+static int refuse_multi_prompt(const b200mdm_engine* e, const char* what) {
+  if (e->groups) return fail(B200MDM_ENOTIMPL, "%s with multi-prompt guidance is not implemented", what);
   return B200MDM_OK;
 }
 
@@ -1526,7 +1629,8 @@ static void tap_source(const b200mdm_engine* e, int id, const void** src, size_t
     case B200MDM_TAP_L_QC: if (dip) { *src = e->qc16; *bytes = M * d * h; } break;
     case B200MDM_TAP_L_XATT: if (dip) { *src = e->att16; *bytes = M * kw * d * h; } break;
     case B200MDM_TAP_L_FFN: *src = e->ffn16; *bytes = M * kw * e->ff * h; break;
-    case B200MDM_TAP_BLEND: *src = e->g16; *bytes = static_cast<size_t>(e->B) * e->T * 3 * d * h; break;
+    case B200MDM_TAP_BLEND:
+      *src = e->g16; *bytes = static_cast<size_t>(e->groups ? e->Bp : e->B) * e->T * 3 * d * h; break;
   }
 }
 
@@ -1574,8 +1678,18 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     ++nk;
   }
   TRY(launch_pack_input(a.x_in, e->xin16, B, JF, T, S, Kp, e->s_off, s));
-  TRY(launch_embed_gemm(e->m_xin, e->m_win, e->m_res_c, e->m_res_u, e->pe_bias, e->MB, S, d, Kp, e->halves, s, e->num_sms));
+  TRY(launch_embed_gemm(e->m_xin, e->m_win, e->m_res_c, e->m_res_u, e->pe_bias, e->MB, S, d, Kp, e->halves > 1 || e->groups > 1 ? 2 : 1,
+                        s, e->num_sms));
   nk += 2;
+  // multi-prompt guidance: the first and last groups came from the launch above, the groups between them in pairs
+  for (int g = 1; g < e->groups - 1; g += 2) {
+    const int pair = g + 1 < e->groups - 1 ? 2 : 1;
+    CUtensorMap m_a, m_b;
+    TRY(make_map_res(&m_a, e->hres + static_cast<size_t>(g) * e->MB * d * 2, e->MB, d));
+    TRY(make_map_res(&m_b, e->hres + static_cast<size_t>(g + pair - 1) * e->MB * d * 2, e->MB, d));
+    TRY(launch_embed_gemm(e->m_xin, e->m_win, m_a, m_b, e->pe_bias, e->MB, S, d, Kp, pair, s, e->num_sms));
+    ++nk;
+  }
   if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_EMBED, B200MDM_TAP_EMBED, -1, s));
   const float* target_g = e->target_set ? e->tgt_g : nullptr;   // timestep embedding + target (model/mdm.py:197-199)
   if (!e->dec || e->dec_clip) {
@@ -1647,7 +1761,9 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_L_LN3, B200MDM_TAP_L_LN3, l, s));
     nk += 5;
   }
-  TRY(launch_blend_split(e->hres, e->g16, e->scale, B, S, T, e->s_off, d, e->halves, e->hs_set ? e->hs_desc : nullptr, s));
+  // multi-prompt guidance: every group's frame rows are split as they are (halves 1 over G * B motions)
+  const int G = e->groups, GB = G ? G * B : B;
+  TRY(launch_blend_split(e->hres, e->g16, e->scale, GB, S, T, e->s_off, d, G ? 1 : e->halves, e->hs_set ? e->hs_desc : nullptr, s));
   ++nk;
   if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_BLEND, B200MDM_TAP_BLEND, -1, s));
   {
@@ -1663,7 +1779,30 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     p.x_start = e->vb_xs;
     p.vb_part = e->vb_part;
     p.state = e->state;
-    if (e->jg_set && !a.model_only) {
+    if (G) {
+      // multi-prompt guidance: the output GEMM writes every group's raw x0, compose_step_kernel composes it and runs the
+      // step's tail (the bare model output too: b200mdm_denoise composes, without inpainting)
+      StepArgs ax = a;
+      ax.mode = MODE_X0;
+      ax.x_out = e->mp_x0;
+      ax.pred = nullptr;
+      ax.clip = 0;
+      EpiOutParams px = p;
+      px.inpaint_mask = nullptr;
+      px.inpaint_weight = nullptr;
+      px.inpaint_motion = nullptr;
+      TRY(launch_out_gemm(e->m_g16, e->m_wout, GB, T, JF, d, ax, px, s, e->num_sms));
+      set_step_params(&p, a, B, T, JF);
+      const dim3 grid(static_cast<unsigned>((static_cast<size_t>(JF) * T + MP_THREADS - 1) / MP_THREADS), B);
+      const PromptWeight* pw = e->pw_desc;
+      const float* x0g = e->mp_x0;
+      if (a.mode <= MODE_DDIM) CUDA_TRY(launch_k(compose_step_kernel<OutStep>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
+      else if (a.mode == MODE_DDIM_REVERSE) CUDA_TRY(launch_k(compose_step_kernel<OutReverse>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
+      else if (a.mode == MODE_DPM) CUDA_TRY(launch_k(compose_step_kernel<OutDpm>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
+      else if (a.mode == MODE_VB) return fail(B200MDM_ENOTIMPL, "the variational bound with multi-prompt guidance is not implemented");
+      else CUDA_TRY(launch_k(compose_step_kernel<OutPlms>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
+      nk += 2;
+    } else if (e->jg_set && !a.model_only) {
       // joint-position control: the output GEMM writes the raw x0, the guidance kernel runs the step's tail on it
       StepArgs ax = a;
       ax.mode = MODE_X0;
@@ -1699,6 +1838,7 @@ static int check_ready(b200mdm_engine* e, bool need_sched) {
   if (!e->cond_set) return fail(B200MDM_ESTATE, "b200mdm_set_cond has not been called");
   if (e->dec && e->ctx > 0 && !e->prefix_set) return fail(B200MDM_ESTATE, "b200mdm_set_prefix has not been called (y['prefix'])");
   if (need_sched && e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
+  if (e->groups && !e->pw_set) return fail(B200MDM_ESTATE, "b200mdm_set_prompt_weight has not been called");
   return B200MDM_OK;
 }
 
@@ -1883,6 +2023,7 @@ static int loop_enter(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32
     key.target_g = e->target_set ? e->tgt_g : nullptr;
     key.hs = e->hs_set ? e->hs_desc : nullptr;
     key.guided = e->jg_set;
+    key.groups = e->groups;
     TRY(ensure_step_graph(e, key, a));
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
     CUDA_TRY(cudaStreamWaitEvent(e->work, e->ev_in, 0));
@@ -2305,6 +2446,7 @@ extern "C" int b200mdm_vb_loop_range(b200mdm_engine* e, int32_t first_index, int
   if (!x_start_dev && !e->vb_live) return fail(B200MDM_ESTATE, "no bound loop to continue (pass x_start_dev)");
   if (e->hs_set) return fail(B200MDM_ENOTIMPL, "the variational bound with handshakes is not implemented");
   TRY(refuse_joint_guidance(e, "the variational bound"));
+  TRY(refuse_multi_prompt(e, "the variational bound"));
   TRY(ensure_vb(e));
   if (!x_start_dev && !e->vb_live)   // ensure_vb reallocated the tables for a longer schedule: nothing to continue
     return fail(B200MDM_ESTATE, "the schedule outgrew the bound loop's tables: no bound loop to continue (pass x_start_dev)");

@@ -245,15 +245,21 @@ class GaussianDiffusion:
         model_kwargs = model_kwargs if model_kwargs is not None else {}
         y = model_kwargs.get("y", {})
         soft = self._soft_inpainting(y, shape)
-        from ..model.mdm import joint_control_of
+        from ..model.mdm import joint_control_of, multi_prompt_of, set_cond_multi
         jc = joint_control_of(model)
         joint = jc.targets(y, shape) if jc is not None else None
+        mp = multi_prompt_of(model)
+        if mp is not None:
+            mp.prompts(y, shape)                     # y's prompts checked before any engine work
         eng, guided = self._engine_of(model)
-        if "text" in y.keys():                       # encode once, mutate y like the reference (:633-635)
+        if "text" in y.keys() and mp is None:        # encode once, mutate y like the reference (:633-635)
             y["text_embed"] = model.encode_text(y["text"])
         eng.set_schedule(self.schedule_rows(eta), self._timestep_map(), key=(id(self), float(eta), self.num_timesteps))
         B, T = int(shape[0]), int(shape[-1])
-        eng.set_cond(B, T, y, guided, device)
+        if mp is not None:
+            set_cond_multi(eng, mp, shape, y, device)
+        else:
+            eng.set_cond(B, T, y, guided, device)
         hs = self._handshake_of(model)
         if hs is not None and hs.handshake_size > 0:
             eng.set_handshake(hs.handshake_size, B, T, y)
@@ -808,6 +814,10 @@ class GaussianDiffusion:
         them to the engine's Philox stream (the eps a sampling loop of that seed would draw at the same index)."""
         self._reject_handshake(model, "The variational bound")
         self._reject_joint_control(model, "The variational bound")
+        from ..model.mdm import multi_prompt_of
+        if multi_prompt_of(model) is not None:
+            raise NotImplementedError("The variational bound with multi-prompt guidance (MultiPromptSampleModel) is not "
+                                      "implemented")
         if noise_tape is not None and noise_seed is not None:
             raise ValueError("noise_seed excludes noise_tape")
         self._model_log_variance()                           # NotImplementedError for learned variances

@@ -350,6 +350,29 @@ class Engine:
         check(self.lib.b200mdm_set_joint_guidance(self.h, *[_ptr(t) for t in ts], float(step), int(iters), _stream()))
         self._keep["joint"] = ts
 
+    def set_cond_multi(self, batch, nframes, y, embed, action, weight, device):
+        """Multi-prompt guidance (b200mdm_set_cond_multi / _dec, then b200mdm_set_prompt_weight): embed fp32 [K, B, C]
+        (text models) or action int64 numpy [B, K] (action models), weight fp32 [B, K, D or 1, T or 1], as
+        MultiPromptSampleModel.prompts returns them; lengths and the target from y as set_cond takes them."""
+        y = y or {}
+        K = int(weight.shape[1])
+        ln, _ = self._lengths_and_scale(batch, y, False, device)
+        ln_p = None if ln is None else ln.ctypes.data_as(ctypes.c_void_p)
+        te = None if embed is None else embed.detach().to(device=device, dtype=torch.float32).contiguous()
+        if self.dec:
+            check(self.lib.b200mdm_set_cond_multi_dec(self.h, batch, nframes, K, _ptr(te), ln_p, _stream()))
+        else:
+            ac = None if action is None else np.ascontiguousarray(action, dtype=np.int64)
+            check(self.lib.b200mdm_set_cond_multi(self.h, batch, nframes, K, _ptr(te), ln_p,
+                                                  None if ac is None else ac.ctypes.data_as(ctypes.c_void_p), _stream()))
+        self._keep["cond"] = (te,)
+        self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 1, 1
+        self._set_target(batch, y, device)
+        w = weight.detach().to(device=device, dtype=torch.float32).contiguous()
+        strides = [0 if w.shape[i] == 1 else w.stride(i) for i in range(4)]
+        check(self.lib.b200mdm_set_prompt_weight(self.h, K, _ptr(w), *strides, _stream()))
+        self._keep["prompt_weight"] = w
+
     # ------------------------------------------------------------------ compute
     def denoise(self, x, timesteps):
         x = x.to(torch.float32).contiguous()

@@ -260,28 +260,49 @@ def _identity_rot2xyz(x, mask=None, pose_rep="xyz", **kw):
     return x
 
 
-def _run_model(model, x, timesteps, y, guided, handshake=0):
+def _run_model(model, x, timesteps, y, guided, handshake=0, multi=None):
     eng = model.engine()
     B, T = x.shape[0], x.shape[-1]
     with torch.cuda.device(x.device):
-        eng.set_cond(B, T, y if y is not None else {}, guided, x.device)
+        if multi is not None:
+            set_cond_multi(eng, multi, x.shape, y if y is not None else {}, x.device)
+        else:
+            eng.set_cond(B, T, y if y is not None else {}, guided, x.device)
         if handshake:
             eng.set_handshake(handshake, B, T, y if y is not None else {})
         eng.set_inpaint(None, None)
         return eng.denoise(x, timesteps)
 
 
+def set_cond_multi(eng, multi, shape, y, device):
+    """The engine's conditioning for MultiPromptSampleModel `multi` and y (its prompts checked before any engine work);
+    y['prompt_text'] is encoded into y['prompt_embed'], as the samplers encode y['text'] into y['text_embed']."""
+    embed, action, weight = multi.prompts(y, shape)
+    if embed is None and action is None:
+        y["prompt_embed"] = embed = multi.encode_prompts(y["prompt_text"])
+    eng.set_cond_multi(int(shape[0]), int(shape[-1]), y, embed, action, weight, device)
+
+
+def multi_prompt_of(model):
+    """The MultiPromptSampleModel a sampler was given (possibly behind respace._WrappedModel), or None."""
+    from ..utils.sampler_util import MultiPromptSampleModel
+    from ..diffusion.respace import _WrappedModel
+    while isinstance(model, _WrappedModel):
+        model = model.model
+    return model if isinstance(model, MultiPromptSampleModel) else None
+
+
 def _unwrap(model):
-    """(innermost model, HandshakeSampleModel or None) behind respace._WrappedModel and a HandshakeSampleModel or
-    JointControlSampleModel."""
-    from ..utils.sampler_util import HandshakeSampleModel, JointControlSampleModel
+    """(innermost model, HandshakeSampleModel or None) behind respace._WrappedModel and a HandshakeSampleModel,
+    JointControlSampleModel or MultiPromptSampleModel."""
+    from ..utils.sampler_util import HandshakeSampleModel, JointControlSampleModel, MultiPromptSampleModel
     from ..diffusion.respace import _WrappedModel
     inner = model
     while isinstance(inner, _WrappedModel):
         inner = inner.model
     if isinstance(inner, HandshakeSampleModel):
         return inner.model, inner
-    if isinstance(inner, JointControlSampleModel):
+    if isinstance(inner, (JointControlSampleModel, MultiPromptSampleModel)):
         return inner.model, None
     return inner, None
 

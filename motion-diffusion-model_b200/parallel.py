@@ -62,7 +62,8 @@ def gather_objects(obj, group=None):
 
 
 _BATCH_KEYS = ("mask", "lengths", "scale", "action", "inpainting_mask", "inpainted_motion", "prefix", "target_cond",
-               "is_heading", "motion_start", "inpainting_weight", "joint_target", "joint_weight")
+               "is_heading", "motion_start", "inpainting_weight", "joint_target", "joint_weight", "prompt_action",
+               "prompt_weight")
 
 
 def shard_model_kwargs(model_kwargs, lo, hi):
@@ -80,12 +81,14 @@ def shard_model_kwargs(model_kwargs, lo, hi):
     for k, v in y.items():
         if k == "text_embed" and torch.is_tensor(v):
             out[k] = v[:, lo:hi].contiguous() if v.shape[1] > 1 else v      # [1, B, C]; a single prompt is shared
+        elif k == "prompt_embed" and torch.is_tensor(v):                     # [K, B, C]
+            out[k] = v[:, lo:hi].contiguous()
         elif k == "text_embed" and isinstance(v, tuple):                     # DiP: (tokens [Mt, B, C], mask [B, Mt])
             tok, msk = v
             out[k] = (tok[:, lo:hi].contiguous() if tok.shape[1] > 1 else tok, msk[lo:hi].contiguous() if msk.shape[0] > 1 else msk)
         elif k in _BATCH_KEYS and torch.is_tensor(v):
             out[k] = v[lo:hi].contiguous()
-        elif k in ("text", "tokens", "target_joint_names") and isinstance(v, (list, tuple)):
+        elif k in ("text", "tokens", "target_joint_names", "prompt_text") and isinstance(v, (list, tuple)):
             out[k] = list(v[lo:hi])
         elif k in ("target_cond", "is_heading", "target_joint_names", "motion_start") and isinstance(v, np.ndarray):
             out[k] = v[lo:hi]

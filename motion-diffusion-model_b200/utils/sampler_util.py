@@ -200,6 +200,123 @@ class JointControlSampleModel(nn.Module):
         return wrapped_getattr(self, name, default=None)
 
 
+# HumanML3D's 263 features per frame: root yaw velocity, root XZ velocity, root height (4), then for the 21 non-root
+# joints their root-relative positions (3 each) and rotations (6 each), for all 22 joints their velocities (3 each), and
+# 4 foot contacts.  The lower body is the pelvis, hips, knees, ankles and feet; the root features and foot contacts
+# belong to it.
+_HML_JOINTS = 22
+_HML_LOWER_JOINTS = (0, 1, 2, 4, 5, 7, 8, 10, 11)
+
+
+def body_part_mask(parts):
+    """bool [263] feature mask of HumanML3D's body parts: 'lower' or 'upper' (the reference's HML_LOWER_BODY_MASK /
+    HML_UPPER_BODY_MASK, which partition the features), or a list of them (their union)."""
+    names = [parts] if isinstance(parts, str) else list(parts)
+    if not names or any(p not in ("lower", "upper") for p in names):
+        raise ValueError("body parts are 'lower' and 'upper' (got %r)" % (parts,))
+    low = np.isin(np.arange(_HML_JOINTS), _HML_LOWER_JOINTS)
+    lower = np.concatenate([np.ones(4, bool), low[1:].repeat(3), low[1:].repeat(6), low.repeat(3), np.ones(4, bool)])
+    out = np.zeros(263, dtype=bool)
+    for p in names:
+        out |= lower if p == "lower" else ~lower
+    return torch.from_numpy(out)
+
+
+class MultiPromptSampleModel(nn.Module):
+    """Multi-prompt guidance (this project's definition, DESIGN.md "Multi-prompt guidance"): K prompts per motion,
+    composed around the unconditional prediction as
+
+        x0[b, f, t] = x0_u[b, f, t] + sum_k y['prompt_weight'][b, k, f, t] * (x0_k[b, f, t] - x0_u[b, f, t])
+
+    in fp32, before inpainting, the clamp of clip_denoised and the update.  A body-part prompt is a weight that is
+    nonzero on that part's features only (body_part_mask), a time-varying prompt a weight that changes with t, a negative
+    prompt a negative weight; K = 1 with the weight y['scale'][b] is ClassifierFreeSampleModel's formula.
+
+    `model` is a b200mdm MDM: trans_enc with CLIP text or action conditioning, or the CLIP decoder with a timestep token
+    (prefix-completion (DiP) models raise NotImplementedError, any wrapper TypeError).  y carries the prompts as
+    y['prompt_embed'] fp32 [K, B, C] (or y['prompt_text'], B lists of K strings, which the sampler encodes into it) or
+    y['prompt_action'] [B, K] for action models, and y['prompt_weight'] float [B, K, D, T] (either of the last two may
+    be 1: it is broadcast, never materialised).  lengths, mask, inpainting and target keys keep their meaning;
+    y['text'], y['text_embed'] and y['scale'] are not read.  Every sampler but calc_bpd_loop (NotImplementedError)
+    honours it; calling the wrapper returns the composed x0."""
+
+    def __init__(self, model):
+        super().__init__()
+        from ..model.mdm import MDM
+        if not isinstance(model, MDM):
+            raise TypeError("MultiPromptSampleModel wraps a b200mdm MDM (got %r)" % type(model))
+        assert model.cond_mask_prob > 0, \
+            "Cannot run a guided diffusion on a model that has not been trained with no conditions"
+        if model.is_prefix_comp or (model.arch == "trans_dec" and not model.emb_trans_dec):
+            raise NotImplementedError("multi-prompt guidance is not implemented for prefix-completion (DiP) models")
+        if model.cond_mode not in ("text", "action"):
+            raise ValueError("multi-prompt guidance needs a text- or action-conditioned model (cond_mode %r)"
+                             % model.cond_mode)
+        self.model = model
+        self.rot2xyz = self.model.rot2xyz
+        self.translation = self.model.translation
+        self.njoints = self.model.njoints
+        self.nfeats = self.model.nfeats
+        self.data_rep = self.model.data_rep
+        self.cond_mode = self.model.cond_mode
+        self.encode_text = self.model.encode_text
+
+    def prompts(self, y, shape):
+        """(embed [K, B, C] or None, action int64 numpy [B, K] or None, weight fp32 [B, K, D or 1, T or 1]) of y for a
+        sample of `shape`; y is not modified, and y['prompt_text'] is not encoded (embed is None for it).  ValueError
+        for a missing or mis-shaped key, K outside 1 .. MAX_PROMPTS, an action outside the model's classes, or a weight
+        that is not finite."""
+        from .. import _lib
+        B, T = int(shape[0]), int(shape[-1])
+        D = int(self.model.njoints) * int(self.model.nfeats)
+        w = y.get("prompt_weight")
+        if not torch.is_tensor(w) or not w.is_floating_point() or w.dim() != 4:
+            raise ValueError("MultiPromptSampleModel needs y['prompt_weight'], a float tensor [B, K, D, T]")
+        K = int(w.shape[1])
+        if not 1 <= K <= _lib.MAX_PROMPTS:
+            raise ValueError("the prompt count K = %d must lie in 1 .. %d" % (K, _lib.MAX_PROMPTS))
+        if w.shape[0] != B or w.shape[2] not in (1, D) or w.shape[3] not in (1, T):
+            raise ValueError("y['prompt_weight'] %s must be [%d, K, %d or 1, %d or 1]" % (tuple(w.shape), B, D, T))
+        if not bool(torch.isfinite(w).all()):
+            raise ValueError("y['prompt_weight'] must be finite")
+        w = w.to(torch.float32)
+        if self.model.cond_mode == "action":
+            a = y.get("prompt_action")
+            if a is None:
+                raise ValueError("an action model needs y['prompt_action'] [B, K]")
+            a = np.asarray(a.detach().cpu() if torch.is_tensor(a) else a)
+            if a.shape != (B, K) or not np.issubdtype(a.dtype, np.integer):
+                raise ValueError("y['prompt_action'] %s must be integer [%d, %d]" % (a.shape, B, K))
+            if ((a < 0) | (a >= int(self.model.num_actions))).any():
+                raise ValueError("y['prompt_action'] holds an action outside 0 .. %d" % (int(self.model.num_actions) - 1))
+            return None, a.astype(np.int64), w
+        e = y.get("prompt_embed")
+        if e is None:
+            texts = y.get("prompt_text")
+            if texts is None:
+                raise ValueError("a text model needs y['prompt_embed'] [K, B, C] or y['prompt_text'] (B lists of K strings)")
+            if len(texts) != B or any(isinstance(p, str) or len(p) != K for p in texts):
+                raise ValueError("y['prompt_text'] must hold B = %d lists of K = %d strings" % (B, K))
+            return None, None, w
+        C = int(self.model.clip_dim)
+        if not torch.is_tensor(e) or not e.is_floating_point() or tuple(e.shape) != (K, B, C):
+            raise ValueError("y['prompt_embed'] must be a float tensor [%d, %d, %d]" % (K, B, C))
+        return e, None, w
+
+    def encode_prompts(self, texts):
+        """[K, B, C] text features of y['prompt_text'] (B lists of K strings), the model's encode_text per prompt."""
+        K = len(texts[0])
+        return torch.cat([self.model.encode_text([p[k] for p in texts]) for k in range(K)], dim=0)
+
+    def forward(self, x, timesteps, y=None):
+        from ..model.mdm import _run_model
+        self.prompts(y if y is not None else {}, x.shape)       # y's prompts checked before any engine work
+        return _run_model(self.model, x, timesteps, y, guided=False, multi=self)
+
+    def __getattr__(self, name, default=None):
+        return wrapped_getattr(self, name, default=None)
+
+
 def stitch_handshake(sample, lengths, handshake_size, motion_start=None):
     """The motions of a batch of chained windows (HandshakeSampleModel): for each motion, its first window's frames
     [:n], then each later window's [h:n].  sample [B, njoints, nfeats, T]; lengths [B] (None: all T); returns a list of
@@ -314,9 +431,11 @@ def refine_transitions(sample_fn, model, windows, model_kwargs, handshake_size, 
     returned as they are, with no engine call.  `model` is the plain (guided) model: a HandshakeSampleModel raises
     TypeError, a prefix-completion (DiP) model NotImplementedError; layout errors raise ValueError (transition_layout),
     as does skip_timesteps outside [0, num_timesteps).  Gather and paste are device indexing only."""
-    from ..model.mdm import _unwrap, joint_control_of
+    from ..model.mdm import _unwrap, joint_control_of, multi_prompt_of
     if joint_control_of(model) is not None:
         raise TypeError("refine_transitions is not implemented with joint-position control (JointControlSampleModel)")
+    if multi_prompt_of(model) is not None:
+        raise TypeError("refine_transitions is not implemented with multi-prompt guidance (MultiPromptSampleModel)")
     inner, hs = _unwrap(model)
     if hs is not None:
         raise TypeError("refine_transitions runs the plain model: pass the model a HandshakeSampleModel wraps, not the wrapper")
