@@ -18,6 +18,8 @@ import numpy as np
 import torch
 
 from .. import _lib
+from ..model.mdm import condition, engine_for
+from ..utils.sampler_util import resolve
 
 
 class ModelMeanType(enum.Enum):
@@ -63,6 +65,14 @@ def get_named_beta_schedule(schedule_name, num_diffusion_timesteps, scale_betas=
 
 def _f32(a):
     return np.asarray(a, dtype=np.float64).astype(np.float32)
+
+
+# The feature wrappers (utils/sampler_util.resolve) each sampler family refuses; DDPM and DDIM take all three.
+_REFUSED = {"DDIM inversion": ("handshake", "joint"), "PLMS": ("joint",), "DPM-Solver++": ("joint",),
+            "The variational bound": ("handshake", "joint", "multi"), "p_mean_variance": ("joint",)}
+_REFUSAL = {"handshake": "%s with HandshakeSampleModel is not implemented",
+            "joint": "%s with joint-position control (JointControlSampleModel) is not implemented",
+            "multi": "%s with multi-prompt guidance (MultiPromptSampleModel) is not implemented"}
 
 
 class GaussianDiffusion:
@@ -200,24 +210,19 @@ class GaussianDiffusion:
 
     # ------------------------------------------------------------------ helpers
     @staticmethod
-    def _engine_of(model):
-        from ..model.mdm import engine_for
-        return engine_for(model)
+    def _refuse(model, family):
+        """NotImplementedError when sampler `family` does not take the feature wrapper of `model` (_REFUSED)."""
+        kind = resolve(model).kind
+        if kind in _REFUSED[family]:
+            raise NotImplementedError(_REFUSAL[kind] % family)
 
     @staticmethod
-    def _handshake_of(model):
-        from ..model.mdm import handshake_of
-        return handshake_of(model)
-
-    def _reject_handshake(self, model, what):
-        if self._handshake_of(model) is not None:
-            raise NotImplementedError("%s with HandshakeSampleModel is not implemented" % what)
+    def _device(model, device):
+        return device if device is not None else next(model.parameters()).device
 
     @staticmethod
-    def _reject_joint_control(model, what):
-        from ..model.mdm import joint_control_of
-        if joint_control_of(model) is not None:
-            raise NotImplementedError("%s with joint-position control (JointControlSampleModel) is not implemented" % what)
+    def _flags(clip_denoised, const_noise=False):
+        return (_lib.FLAG_CONST_NOISE if const_noise else 0) | (_lib.FLAG_CLIP_DENOISED if clip_denoised else 0)
 
     @staticmethod
     def _soft_inpainting(y, shape):
@@ -240,29 +245,22 @@ class GaussianDiffusion:
             raise ValueError("y['inpainting_weight'] must be finite and within [0, 1]")
         return w, motion
 
-    def _prepare(self, model, shape, model_kwargs, device, eta):
+    def _prepare(self, model, shape, model_kwargs, device, eta, table=None):
+        """The engine of `model` with this schedule, y's conditioning, inpainting and joint guidance set, and then the
+        sampler family's second table: "next" (DDIM inversion), "dpm" (DPM-Solver++) or "vb" (the variational bound)."""
         self._check_supported()
         model_kwargs = model_kwargs if model_kwargs is not None else {}
         y = model_kwargs.get("y", {})
         soft = self._soft_inpainting(y, shape)
-        from ..model.mdm import joint_control_of, multi_prompt_of, set_cond_multi
-        jc = joint_control_of(model)
-        joint = jc.targets(y, shape) if jc is not None else None
-        mp = multi_prompt_of(model)
-        if mp is not None:
-            mp.prompts(y, shape)                     # y's prompts checked before any engine work
-        eng, guided = self._engine_of(model)
-        if "text" in y.keys() and mp is None:        # encode once, mutate y like the reference (:633-635)
+        r = resolve(model)
+        joint = r.wrapper.targets(y, shape) if r.kind == "joint" else None
+        if r.kind == "multi":
+            r.wrapper.prompts(y, shape)              # y's prompts checked before any engine work
+        eng, guided = engine_for(model)
+        if "text" in y.keys() and r.kind != "multi":  # encode once, mutate y like the reference (:633-635)
             y["text_embed"] = model.encode_text(y["text"])
         eng.set_schedule(self.schedule_rows(eta), self._timestep_map(), key=(id(self), float(eta), self.num_timesteps))
-        B, T = int(shape[0]), int(shape[-1])
-        if mp is not None:
-            set_cond_multi(eng, mp, shape, y, device)
-        else:
-            eng.set_cond(B, T, y, guided, device)
-        hs = self._handshake_of(model)
-        if hs is not None and hs.handshake_size > 0:
-            eng.set_handshake(hs.handshake_size, B, T, y)
+        condition(eng, shape, y, device, guided, r.wrapper)
         if soft is not None:
             eng.set_inpaint_weight(soft[0].to(device), soft[1].to(device))
         elif "inpainting_mask" in y and "inpainted_motion" in y:
@@ -271,8 +269,15 @@ class GaussianDiffusion:
         else:
             eng.set_inpaint(None, None)
         if joint is not None:
+            jc = r.wrapper
             eng.set_joint_guidance(jc.mean.to(device), jc.std.to(device), joint[0].to(device), joint[1].to(device),
                                    jc.step_size, jc.n_iters)
+        if table == "next":
+            eng.set_schedule_next(self.schedule_next_rows(), key=(id(self), self.num_timesteps))
+        elif table == "dpm":
+            eng.set_schedule_dpm(self.schedule_dpm_rows(), key=(id(self), self.num_timesteps))
+        elif table == "vb":
+            eng.set_schedule_vb(self.schedule_vb_rows(), key=(id(self), self.num_timesteps, self.model_var_type))
         return eng
 
     @staticmethod
@@ -283,9 +288,11 @@ class GaussianDiffusion:
         if randomize_class:
             raise NotImplementedError("randomize_class is a guided-diffusion leftover (needs model.num_classes)")
 
-    def _initial(self, eng, shape, noise, device, skip_timesteps, init_image):
-        if device is None:
-            device = eng_device()
+    def _initial(self, eng, shape, noise, device, skip_timesteps, init_image, noise_seed=None, sample_index_base=0):
+        """x_T: `noise`, else the engine's Philox stream of noise_seed, else one torch.randn; noised to the first step's
+        level from init_image (zeros with skip_timesteps and no init_image)."""
+        if noise is None and noise_seed is not None:
+            noise = eng.philox_normal(shape, noise_seed, sample_index_base, -1, device)
         img = noise if noise is not None else torch.randn(*shape, device=device)
         img = img.to(device=device, dtype=torch.float32)
         if skip_timesteps and init_image is None:
@@ -385,15 +392,12 @@ class GaussianDiffusion:
               noise_seed=None, sample_index_base=0, noise_fn=None):
         self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
         assert isinstance(shape, (tuple, list))
-        if device is None:
-            device = next(model.parameters()).device
+        device = self._device(model, device)
         eng = self._prepare(model, shape, model_kwargs, device, eta)
-        if noise_seed is not None and noise is None:
-            noise = eng.philox_normal(shape, noise_seed, sample_index_base, -1, device)     # x_T from the engine stream
-        img = self._initial(eng, shape, noise, device, skip_timesteps, init_image)
+        img = self._initial(eng, shape, noise, device, skip_timesteps, init_image, noise_seed, sample_index_base)
         n_run = self.num_timesteps - skip_timesteps
         first = n_run - 1
-        flags = (1 if const_noise else 0) | (2 if clip_denoised else 0)
+        flags = self._flags(clip_denoised, const_noise)
         if noise_seed is not None:                   # engine-side counter-based eps: no tape at all
             assert noise_tape is None and dump_steps is None, "noise_seed excludes noise_tape / dump_steps"
             eng.set_noise_stream(noise_seed, sample_index_base)
@@ -426,11 +430,10 @@ class GaussianDiffusion:
     def _progressive(self, mode, model, shape, noise, clip_denoised, denoised_fn, cond_fn, model_kwargs, device,
                      skip_timesteps, init_image, randomize_class, cond_fn_with_grad, const_noise, eta, noise_tape):
         self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
-        if device is None:
-            device = next(model.parameters()).device
+        device = self._device(model, device)
         eng = self._prepare(model, shape, model_kwargs, device, eta)
         img = self._initial(eng, shape, noise, device, skip_timesteps, init_image)
-        flags = (1 if const_noise else 0) | (2 if clip_denoised else 0)
+        flags = self._flags(clip_denoised, const_noise)
         n_run = self.num_timesteps - skip_timesteps
         for k in range(n_run):
             eps = noise_tape[k].to(device) if noise_tape is not None else torch.randn_like(img)
@@ -448,8 +451,7 @@ class GaussianDiffusion:
         assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch (gaussian_diffusion.py:709)"
         eng = self._prepare(model, x.shape, model_kwargs, x.device, eta)
         eps = noise if noise is not None else torch.randn_like(x)
-        flags = (1 if const_noise else 0) | (2 if clip_denoised else 0)
-        out, pred = eng.sample_step(mode, idx, x, eps, flags, want_pred=True)
+        out, pred = eng.sample_step(mode, idx, x, eps, self._flags(clip_denoised, const_noise), want_pred=True)
         return {"sample": out, "pred_xstart": pred}
 
     # ------------------------------------------------------------------ DDIM
@@ -481,11 +483,6 @@ class GaussianDiffusion:
                                      noise_tape)
 
     # ------------------------------------------------------------------ DDIM inversion
-    def _prepare_reverse(self, model, shape, model_kwargs, device):
-        eng = self._prepare(model, shape, model_kwargs, device, 0.0)
-        eng.set_schedule_next(self.schedule_next_rows(), key=(id(self), self.num_timesteps))
-        return eng
-
     def _reverse_range(self, first_index, n_steps):
         """Schedule indices of an inversion loop (default: the whole schedule); ValueError before any engine work."""
         n = self.num_timesteps
@@ -504,13 +501,12 @@ class GaussianDiffusion:
         DDIM ODE.  Returns {'sample', 'pred_xstart'}."""
         if eta != 0.0:
             raise AssertionError("Reverse ODE only for deterministic path")
-        self._reject_handshake(model, "DDIM inversion")
-        self._reject_joint_control(model, "DDIM inversion")
+        self._refuse(model, "DDIM inversion")
         self._reject_hooks(denoised_fn, None, False, False)
         idx = int(t.reshape(-1)[0].item())
         assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch"
-        eng = self._prepare_reverse(model, x.shape, model_kwargs, x.device)
-        out, pred = eng.sample_step(_lib.MODE_DDIM_REVERSE, idx, x, None, 2 if clip_denoised else 0, want_pred=True)
+        eng = self._prepare(model, x.shape, model_kwargs, x.device, 0.0, table="next")
+        out, pred = eng.sample_step(_lib.MODE_DDIM_REVERSE, idx, x, None, self._flags(clip_denoised), want_pred=True)
         return {"sample": out, "pred_xstart": pred}
 
     def ddim_reverse_sample_loop(self, model, x_start, clip_denoised=True, model_kwargs=None, device=None, first_index=0,
@@ -518,15 +514,13 @@ class GaussianDiffusion:
         """DDIM inversion (no reference counterpart as a loop): exactly the reference step ddim_reverse_sample
         iterated for i = first_index ... first_index + n_steps - 1 (default: the whole schedule, 0 ... n - 1), as one
         engine call (every step a replay of one CUDA graph).  Returns the last step's sample; x_start is not modified."""
-        self._reject_handshake(model, "DDIM inversion")
-        self._reject_joint_control(model, "DDIM inversion")
+        self._refuse(model, "DDIM inversion")
         first, n_run = self._reverse_range(first_index, n_steps)
-        if device is None:
-            device = next(model.parameters()).device
-        eng = self._prepare_reverse(model, x_start.shape, model_kwargs, device)
+        device = self._device(model, device)
+        eng = self._prepare(model, x_start.shape, model_kwargs, device, 0.0, table="next")
         img = x_start.to(device=device, dtype=torch.float32).contiguous()
         out = torch.empty_like(img)
-        eng.ddim_reverse_loop_range(first, n_run, img, out, 2 if clip_denoised else 0, use_graph)
+        eng.ddim_reverse_loop_range(first, n_run, img, out, self._flags(clip_denoised), use_graph)
         eng._keep["loop"] = (img,)
         return out
 
@@ -534,16 +528,13 @@ class GaussianDiffusion:
                                              first_index=0, n_steps=None):
         """ddim_reverse_sample_loop as a generator of the reference step's {'sample', 'pred_xstart'}, one step call per
         yield, for i = first_index ... first_index + n_steps - 1."""
-        self._reject_handshake(model, "DDIM inversion")
-        self._reject_joint_control(model, "DDIM inversion")
+        self._refuse(model, "DDIM inversion")
         first, n_run = self._reverse_range(first_index, n_steps)
-        if device is None:
-            device = next(model.parameters()).device
-        eng = self._prepare_reverse(model, x_start.shape, model_kwargs, device)
+        device = self._device(model, device)
+        eng = self._prepare(model, x_start.shape, model_kwargs, device, 0.0, table="next")
         img = x_start.to(device=device, dtype=torch.float32).contiguous()
-        flags = 2 if clip_denoised else 0
         for i in range(first, first + n_run):
-            img, pred = eng.sample_step(_lib.MODE_DDIM_REVERSE, i, img, None, flags, want_pred=True)
+            img, pred = eng.sample_step(_lib.MODE_DDIM_REVERSE, i, img, None, self._flags(clip_denoised), want_pred=True)
             yield {"sample": img, "pred_xstart": pred}
 
     # ------------------------------------------------------------------ PLMS
@@ -566,13 +557,13 @@ class GaussianDiffusion:
         old_out['old_eps'], which is extended with this step's eps and trimmed in place as in the reference.  order must be an integer from 1 to 4
         (ValueError otherwise, including non-integers such as 2.5)."""
         order = self._plms_order(order, old_out)
-        self._reject_joint_control(model, "PLMS")
+        self._refuse(model, "PLMS")
         self._reject_hooks(denoised_fn, cond_fn, False, cond_fn_with_grad)
         idx = int(t.reshape(-1)[0].item())
         assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch (gaussian_diffusion.py:1166)"
         eng = self._prepare(model, x.shape, model_kwargs, x.device, 0.0)
         old_eps = old_out["old_eps"] if old_out is not None else None     # [] is a history too (:1050-1056)
-        sample, pred, eps = eng.plms_step(idx, order, x, old_eps, 2 if clip_denoised else 0)
+        sample, pred, eps = eng.plms_step(idx, order, x, old_eps, self._flags(clip_denoised))
         if old_out is None:
             old_eps = [eps]
         else:
@@ -589,20 +580,17 @@ class GaussianDiffusion:
         replays of one CUDA graph).  PLMS draws no per-step noise: the only draw is x_T, from torch's generator or, with
         `noise_seed` (+ `sample_index_base`), from the engine's Philox stream.  order: see plms_sample."""
         order = self._plms_order(order)
-        self._reject_joint_control(model, "PLMS")
+        self._refuse(model, "PLMS")
         if noise_tape is not None:
             raise ValueError("PLMS draws no per-step noise: a noise_tape has no use (sample it with noise_mode='philox')")
         self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
         assert isinstance(shape, (tuple, list))
-        if device is None:
-            device = next(model.parameters()).device
+        device = self._device(model, device)
         eng = self._prepare(model, shape, model_kwargs, device, 0.0)
-        if noise_seed is not None and noise is None:
-            noise = eng.philox_normal(shape, noise_seed, sample_index_base, -1, device)
-        img = self._initial(eng, shape, noise, device, skip_timesteps, init_image)
+        img = self._initial(eng, shape, noise, device, skip_timesteps, init_image, noise_seed, sample_index_base)
         n_run = self.num_timesteps - skip_timesteps
         out = torch.empty_like(img)
-        eng.plms_loop_range(order, n_run - 1, n_run, img, out, 2 if clip_denoised else 0, use_graph)
+        eng.plms_loop_range(order, n_run - 1, n_run, img, out, self._flags(clip_denoised), use_graph)
         eng._keep["loop"] = (img,)
         return out
 
@@ -611,14 +599,13 @@ class GaussianDiffusion:
                                      randomize_class=False, cond_fn_with_grad=False, order=2):
         """reference gaussian_diffusion.py:1118-1187: generator of {'sample', 'pred_xstart', 'old_eps'} per step."""
         order = self._plms_order(order)
-        self._reject_joint_control(model, "PLMS")
+        self._refuse(model, "PLMS")
         self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
         assert isinstance(shape, (tuple, list))
-        if device is None:
-            device = next(model.parameters()).device
+        device = self._device(model, device)
         eng = self._prepare(model, shape, model_kwargs, device, 0.0)
         img = self._initial(eng, shape, noise, device, skip_timesteps, init_image)
-        flags = 2 if clip_denoised else 0
+        flags = self._flags(clip_denoised)
         old_eps = None                               # then one list, extended and trimmed in place as in the reference
         for i in range(self.num_timesteps - skip_timesteps)[::-1]:
             img, pred, eps = eng.plms_step(i, order, img, old_eps, flags)
@@ -642,21 +629,17 @@ class GaussianDiffusion:
                    noise_seed, sample_index_base):
         """Argument checks (before any engine work), the tables, conditioning and x_T of a DPM-Solver++ loop."""
         order = self._dpm_order(order)
-        self._reject_joint_control(model, "DPM-Solver++")
+        self._refuse(model, "DPM-Solver++")
         if noise_tape is not None:
             raise ValueError("DPM-Solver++ draws no per-step noise: a noise_tape has no use")
         if dump_steps is not None or const_noise:
             raise NotImplementedError()
         self._reject_hooks(denoised_fn, cond_fn, randomize_class, cond_fn_with_grad)
         assert isinstance(shape, (tuple, list))
-        if device is None:
-            device = next(model.parameters()).device
-        eng = self._prepare(model, shape, model_kwargs, device, 0.0)
-        eng.set_schedule_dpm(self.schedule_dpm_rows(), key=(id(self), self.num_timesteps))
-        if noise_seed is not None and noise is None:
-            noise = eng.philox_normal(shape, noise_seed, sample_index_base, -1, device)
-        img = self._initial(eng, shape, noise, device, skip_timesteps, init_image)
-        return eng, img, order, 2 if clip_denoised else 0, self.num_timesteps - skip_timesteps
+        device = self._device(model, device)
+        eng = self._prepare(model, shape, model_kwargs, device, 0.0, table="dpm")
+        img = self._initial(eng, shape, noise, device, skip_timesteps, init_image, noise_seed, sample_index_base)
+        return eng, img, order, self._flags(clip_denoised), self.num_timesteps - skip_timesteps
 
     def dpm_solver_sample_loop(self, model, shape, noise=None, clip_denoised=True, denoised_fn=None, cond_fn=None,
                                model_kwargs=None, device=None, progress=False, skip_timesteps=0, init_image=None,
@@ -708,8 +691,7 @@ class GaussianDiffusion:
         runs those, and raises what it raises)."""
         n, N = len(ys), self.num_timesteps
         B, pred = int(shape[0]), int(shape[-1])
-        if device is None:
-            device = next(model.parameters()).device
+        device = self._device(model, device)
         for y in ys:
             if "text" in y:
                 y["text_embed"] = model.encode_text(y["text"])
@@ -718,14 +700,12 @@ class GaussianDiffusion:
         if any(te is not tes[0] for te in tes[1:]):
             if not all(isinstance(te, tuple) for te in tes):
                 return None                          # the host chain raises the conditioning's error at that chunk
-            eng, _ = self._engine_of(model)
+            eng, _ = engine_for(model)
             mems = [eng.dec_memory(te, B, device) for te in tes]
             if len({m[0].shape[0] for m in mems}) > 1:
                 return None
         y0 = {k: v for k, v in ys[0].items() if k != "text"}         # encoded above
-        eng = self._prepare(model, shape, {"y": y0}, device, eta)
-        if mode == _lib.MODE_DPM:
-            eng.set_schedule_dpm(self.schedule_dpm_rows(), key=(id(self), self.num_timesteps))
+        eng = self._prepare(model, shape, {"y": y0}, device, eta, table="dpm" if mode == _lib.MODE_DPM else None)
         ctx = eng.context_len
         prefix = ys[0]["prefix"]
         enc = None if mems is None else torch.stack([m[0] for m in mems])
@@ -733,7 +713,7 @@ class GaussianDiffusion:
         out = torch.empty(tuple(shape[:-1]) + (required_frames,), device=device, dtype=torch.float32)
         if include_prefix:
             out[..., :ctx] = prefix[..., :min(ctx, required_frames)]
-        flags = 2 if clip_denoised else 0
+        flags = self._flags(clip_denoised)
         if noise_seed is not None:
             eng.set_noise_stream(noise_seed, sample_index_base)
         x_T = None
@@ -793,14 +773,14 @@ class GaussianDiffusion:
         """reference gaussian_diffusion.py:270-381: {'mean', 'variance', 'log_variance', 'pred_xstart'} of p(x_{t-1} | x_t).
         One engine forward: the DDPM step at zero noise, whose sample is the model mean (bit for bit that step's mean)
         and whose pred_xstart is p_sample's.  t: LongTensor [B] of one schedule index."""
-        self._reject_joint_control(model, "p_mean_variance")
+        self._refuse(model, "p_mean_variance")
         self._reject_hooks(denoised_fn, None, False, False)
         idx = int(t.reshape(-1)[0].item())
         assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch (gaussian_diffusion.py:709)"
         log_variance = self._model_log_variance()           # NotImplementedError for learned variances
         eng = self._prepare(model, x.shape, model_kwargs, x.device, 0.0)
         x = x.to(torch.float32).contiguous()
-        mean, pred = eng.sample_step(_lib.MODE_DDPM, idx, x, torch.zeros_like(x), 2 if clip_denoised else 0, want_pred=True)
+        mean, pred = eng.sample_step(_lib.MODE_DDPM, idx, x, torch.zeros_like(x), self._flags(clip_denoised), want_pred=True)
         return {"mean": mean, "variance": _extract_into_tensor(self._model_variance(), t, x.shape),
                 "log_variance": _extract_into_tensor(log_variance, t, x.shape), "pred_xstart": pred}
 
@@ -812,23 +792,17 @@ class GaussianDiffusion:
         is th.randn_like(x_start) from torch's generator in the reference's order (drawn NOISE_CHUNK steps at a time);
         `noise_tape` [num_timesteps, *x_start.shape] replaces the draws, `noise_seed` (+ `sample_index_base`) switches
         them to the engine's Philox stream (the eps a sampling loop of that seed would draw at the same index)."""
-        self._reject_handshake(model, "The variational bound")
-        self._reject_joint_control(model, "The variational bound")
-        from ..model.mdm import multi_prompt_of
-        if multi_prompt_of(model) is not None:
-            raise NotImplementedError("The variational bound with multi-prompt guidance (MultiPromptSampleModel) is not "
-                                      "implemented")
+        self._refuse(model, "The variational bound")
         if noise_tape is not None and noise_seed is not None:
             raise ValueError("noise_seed excludes noise_tape")
         self._model_log_variance()                           # NotImplementedError for learned variances
         device = x_start.device
-        eng = self._prepare(model, x_start.shape, model_kwargs, device, 0.0)
-        eng.set_schedule_vb(self.schedule_vb_rows(), key=(id(self), self.num_timesteps, self.model_var_type))
+        eng = self._prepare(model, x_start.shape, model_kwargs, device, 0.0, table="vb")
         xs = x_start.to(device=device, dtype=torch.float32).contiguous()
         n, B = self.num_timesteps, int(xs.shape[0])
         terms = torch.empty((3, B, n), device=device, dtype=torch.float32)
         bpd = torch.empty((2, B), device=device, dtype=torch.float32)
-        flags = 2 if clip_denoised else 0
+        flags = self._flags(clip_denoised)
         if noise_seed is not None:
             eng.set_noise_stream(noise_seed, sample_index_base)
             eng.vb_loop_range(n - 1, n, xs, None, flags, terms, bpd, use_graph)
@@ -848,10 +822,6 @@ class GaussianDiffusion:
     # ------------------------------------------------------------------ out of scope
     def training_losses(self, *a, **k):
         raise NotImplementedError("training is outside the H100 sampling engine (SURVEY.md section 8)")
-
-
-def eng_device():
-    return torch.device("cuda", torch.cuda.current_device())
 
 
 def _extract_into_tensor(arr, timesteps, broadcast_shape):

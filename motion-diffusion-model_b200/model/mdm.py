@@ -248,10 +248,16 @@ class MDM(_Bag):
             self._engine_dirty = False
         return self._engine
 
+    @property
+    def is_dip(self):
+        """trans_dec with a BERT token memory: DiP, the prefix-completion decoder (the constructor admits no other
+        trans_dec without emb_trans_dec)."""
+        return self.arch == "trans_dec" and not self.emb_trans_dec
+
     def forward(self, x, timesteps, y=None):
         """x [B, njoints, nfeats, T] fp32, timesteps [B] (model timesteps), y dict -> [B, njoints, nfeats, T]
         (reference model/mdm.py:189-283)."""
-        return _run_model(self, x, timesteps, y, guided=False)
+        return _run_model(self, x, timesteps, y)
 
 
 def _identity_rot2xyz(x, mask=None, pose_rep="xyz", **kw):
@@ -260,83 +266,47 @@ def _identity_rot2xyz(x, mask=None, pose_rep="xyz", **kw):
     return x
 
 
-def _run_model(model, x, timesteps, y, guided, handshake=0, multi=None):
+def _run_model(model, x, timesteps, y, guided=False, wrapper=None):
+    """The forward of MDM `model`, classifier-free guided or not, under a HandshakeSampleModel or
+    MultiPromptSampleModel `wrapper`: one engine call."""
     eng = model.engine()
-    B, T = x.shape[0], x.shape[-1]
     with torch.cuda.device(x.device):
-        if multi is not None:
-            set_cond_multi(eng, multi, x.shape, y if y is not None else {}, x.device)
-        else:
-            eng.set_cond(B, T, y if y is not None else {}, guided, x.device)
-        if handshake:
-            eng.set_handshake(handshake, B, T, y if y is not None else {})
+        condition(eng, x.shape, y if y is not None else {}, x.device, guided, wrapper)
         eng.set_inpaint(None, None)
         return eng.denoise(x, timesteps)
 
 
-def set_cond_multi(eng, multi, shape, y, device):
-    """The engine's conditioning for MultiPromptSampleModel `multi` and y (its prompts checked before any engine work);
-    y['prompt_text'] is encoded into y['prompt_embed'], as the samplers encode y['text'] into y['text_embed']."""
-    embed, action, weight = multi.prompts(y, shape)
-    if embed is None and action is None:
-        y["prompt_embed"] = embed = multi.encode_prompts(y["prompt_text"])
-    eng.set_cond_multi(int(shape[0]), int(shape[-1]), y, embed, action, weight, device)
-
-
-def multi_prompt_of(model):
-    """The MultiPromptSampleModel a sampler was given (possibly behind respace._WrappedModel), or None."""
-    from ..utils.sampler_util import MultiPromptSampleModel
-    from ..diffusion.respace import _WrappedModel
-    while isinstance(model, _WrappedModel):
-        model = model.model
-    return model if isinstance(model, MultiPromptSampleModel) else None
-
-
-def _unwrap(model):
-    """(innermost model, HandshakeSampleModel or None) behind respace._WrappedModel and a HandshakeSampleModel,
-    JointControlSampleModel or MultiPromptSampleModel."""
-    from ..utils.sampler_util import HandshakeSampleModel, JointControlSampleModel, MultiPromptSampleModel
-    from ..diffusion.respace import _WrappedModel
-    inner = model
-    while isinstance(inner, _WrappedModel):
-        inner = inner.model
-    if isinstance(inner, HandshakeSampleModel):
-        return inner.model, inner
-    if isinstance(inner, (JointControlSampleModel, MultiPromptSampleModel)):
-        return inner.model, None
-    return inner, None
-
-
-def joint_control_of(model):
-    """The JointControlSampleModel a sampler was given (possibly behind respace._WrappedModel), or None."""
-    from ..utils.sampler_util import JointControlSampleModel
-    from ..diffusion.respace import _WrappedModel
-    while isinstance(model, _WrappedModel):
-        model = model.model
-    return model if isinstance(model, JointControlSampleModel) else None
-
-
-def handshake_of(model):
-    """The HandshakeSampleModel a sampler was given (possibly behind respace._WrappedModel), or None."""
-    return _unwrap(model)[1]
+def condition(eng, shape, y, device, guided, wrapper=None):
+    """The engine's conditioning for a sample of `shape`: y's, classifier-free guided or not, or the prompts of a
+    MultiPromptSampleModel `wrapper` (y['prompt_text'] is encoded into y['prompt_embed'], as the samplers encode y['text']
+    into y['text_embed']); then the handshakes of a HandshakeSampleModel `wrapper`."""
+    B, T = int(shape[0]), int(shape[-1])
+    kind = wrapper.kind if wrapper is not None else None
+    if kind == "multi":
+        embed, action, weight = wrapper.prompts(y, shape)
+        if embed is None and action is None:
+            y["prompt_embed"] = embed = wrapper.encode_prompts(y["prompt_text"])
+        eng.set_cond_multi(B, T, y, embed, action, weight, device)
+    else:
+        eng.set_cond(B, T, y, guided, device)
+    if kind == "handshake" and wrapper.handshake_size > 0:
+        eng.set_handshake(wrapper.handshake_size, B, T, y)
 
 
 def engine_for(model):
-    """(engine, guided) for a bare MDM or a ClassifierFreeSampleModel wrapper (possibly behind respace._WrappedModel
-    and a HandshakeSampleModel or JointControlSampleModel, whose handshake / guidance the sampler sets with handshake_of
-    / joint_control_of).
+    """(engine, guided) for a bare MDM or a ClassifierFreeSampleModel wrapper, possibly behind respace._WrappedModel
+    and one HandshakeSampleModel, JointControlSampleModel or MultiPromptSampleModel, whose handshake, guidance or
+    prompts the sampler reads from utils.sampler_util.resolve.
 
     Only wrappers this package knows are looked through: an unknown object that merely has a `.model` attribute (for
     instance a guidance wrapper class from another import of this package, or the reference's own
     ClassifierFreeSampleModel) would otherwise be unwrapped down to the bare denoiser and sampled WITHOUT guidance,
     silently."""
-    from ..utils.sampler_util import ClassifierFreeSampleModel
-    inner = _unwrap(model)[0]
-    if isinstance(inner, ClassifierFreeSampleModel):
-        if not isinstance(inner.model, MDM):
-            raise TypeError("ClassifierFreeSampleModel must wrap a b200mdm MDM (got %r)" % type(inner.model))
-        return inner.model.engine(), True
-    if isinstance(inner, MDM):
-        return inner.engine(), False
+    from ..utils.sampler_util import ClassifierFreeSampleModel, resolve
+    r = resolve(model)
+    if r.mdm is not None:
+        return r.mdm.engine(), r.guided
+    if isinstance(r.core, ClassifierFreeSampleModel):
+        raise TypeError("ClassifierFreeSampleModel must wrap a b200mdm MDM (got %r)" % type(r.core.model))
     raise TypeError("b200mdm diffusion objects drive b200mdm.MDM or b200mdm.ClassifierFreeSampleModel only (got %r); "
                     "wrap the model with the classes of this package" % type(model))

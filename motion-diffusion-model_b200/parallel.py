@@ -18,6 +18,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from .utils.sampler_util import resolve
+
 
 def shard_range(global_batch, rank, world):
     """Contiguous slice [lo, hi) of rank `rank`; the first (global_batch % world) ranks get one extra sample."""
@@ -114,8 +116,7 @@ def sample_sharded(sample_fn, model, shape, model_kwargs, *, n_steps, noise_mode
         raise ValueError("global batch %d is smaller than the number of ranks %d" % (B, world))
     lo, hi = shard_range(B, rank, world)
     y = model_kwargs["y"]
-    from .model.mdm import handshake_of
-    if world > 1 and handshake_of(model) is not None and y.get("motion_start") is None:
+    if world > 1 and resolve(model).kind == "handshake" and y.get("motion_start") is None:
         raise ValueError("chained windows without y['motion_start'] are one motion, which cannot be split over %d ranks"
                          % world)
     if torch.is_tensor(y.get("text_embed")) or isinstance(y.get("text_embed"), tuple):

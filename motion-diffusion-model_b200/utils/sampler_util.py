@@ -1,12 +1,35 @@
 """Sampling-time model wrappers (host mirror of the reference's utils/sampler_util.py)."""
+from typing import NamedTuple, Optional
+
 import numpy as np
 import torch
 import torch.nn as nn
 
+from ..model.mdm import MDM, _run_model
 from .misc import wrapped_getattr
 
 
-class ClassifierFreeSampleModel(nn.Module):
+class _SampleWrapper(nn.Module):
+    """A sampling-time wrapper of `model`, registered as the submodule `model`: the attributes the reference's callers
+    read are copied from it and every other attribute is looked up on it.  `kind` names a feature wrapper (resolve)."""
+    kind = None
+
+    def __init__(self, model):
+        super().__init__()
+        self.model = model
+        self.rot2xyz = self.model.rot2xyz
+        self.translation = self.model.translation
+        self.njoints = self.model.njoints
+        self.nfeats = self.model.nfeats
+        self.data_rep = self.model.data_rep
+        self.cond_mode = self.model.cond_mode
+        self.encode_text = self.model.encode_text
+
+    def __getattr__(self, name, default=None):
+        return wrapped_getattr(self, name, default=None)
+
+
+class ClassifierFreeSampleModel(_SampleWrapper):
     """Classifier-free guidance wrapper (reference utils/sampler_util.py:10-38).
 
     The reference deep-copies `y`, runs the denoiser twice and blends
@@ -16,25 +39,43 @@ class ClassifierFreeSampleModel(nn.Module):
     """
 
     def __init__(self, model):
-        super().__init__()
-        self.model = model
-        assert self.model.cond_mask_prob > 0, \
+        assert model.cond_mask_prob > 0, \
             "Cannot run a guided diffusion on a model that has not been trained with no conditions"
-        self.rot2xyz = self.model.rot2xyz
-        self.translation = self.model.translation
-        self.njoints = self.model.njoints
-        self.nfeats = self.model.nfeats
-        self.data_rep = self.model.data_rep
-        self.cond_mode = self.model.cond_mode
-        self.encode_text = self.model.encode_text
+        super().__init__(model)
 
     def forward(self, x, timesteps, y=None):
         assert self.model.cond_mode in ["text", "action"]
-        from ..model.mdm import _run_model
         return _run_model(self.model, x, timesteps, y, guided=True)
 
-    def __getattr__(self, name, default=None):
-        return wrapped_getattr(self, name, default=None)
+
+def _core(model):
+    """(mdm, guided) of a b200mdm MDM or of a ClassifierFreeSampleModel of one, else None."""
+    if isinstance(model, ClassifierFreeSampleModel):
+        return (model.model, True) if isinstance(model.model, MDM) else None
+    return (model, False) if isinstance(model, MDM) else None
+
+
+class Resolved(NamedTuple):
+    """The wrapper stack a sampler was given (resolve)."""
+    mdm: Optional[MDM]          # None: the stack does not end in a model of this package
+    guided: bool                # classifier-free guidance
+    wrapper: Optional[nn.Module]
+    kind: Optional[str]         # wrapper.kind: "handshake", "joint" or "multi"
+    core: object                # what the feature wrapper wraps; the model itself without one
+
+
+def resolve(model):
+    """The stack of a model given to a sampler: respace._WrappedModel layers, at most one feature wrapper
+    (HandshakeSampleModel, JointControlSampleModel or MultiPromptSampleModel), an optional ClassifierFreeSampleModel
+    and an MDM.  Only this package's classes are looked through (model.mdm.engine_for says why): any other object
+    gives mdm None."""
+    from ..diffusion.respace import _WrappedModel            # respace -> gaussian_diffusion -> this module
+    while isinstance(model, _WrappedModel):
+        model = model.model
+    wrapper = model if isinstance(model, _SampleWrapper) and model.kind is not None else None
+    core = model if wrapper is None else wrapper.model
+    mdm, guided = _core(core) or (None, False)
+    return Resolved(mdm, guided, wrapper, None if wrapper is None else wrapper.kind, core)
 
 
 def handshake_layout(batch, nframes, handshake_size, lengths=None, motion_start=None):
@@ -72,15 +113,7 @@ def handshake_layout(batch, nframes, handshake_size, lengths=None, motion_start=
     return n, ms
 
 
-def _inner_mdm(model):
-    from ..model.mdm import MDM
-    inner = model.model if isinstance(model, ClassifierFreeSampleModel) else model
-    if not isinstance(inner, MDM):
-        raise TypeError("HandshakeSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(model))
-    return inner
-
-
-class HandshakeSampleModel(nn.Module):
+class HandshakeSampleModel(_SampleWrapper):
     """Long motions from chained windows (DoubleTake's first take, Shafir et al., "Human Motion Diffusion as a
     Generative Prior"), with this project's weights (DESIGN.md): the batch is a list of windows, y['lengths'] their
     lengths and y['motion_start'] (bool [B]) marks the windows that begin a motion (absent: the whole batch is one
@@ -93,36 +126,27 @@ class HandshakeSampleModel(nn.Module):
     runs inside the engine's guidance-blend kernel, in every sampler (DDPM, DDIM, PLMS, DPM-Solver++).  Stitch the
     final windows with `stitch_handshake`.  Prefix-completion (DiP) models, DDIM inversion and the variational bound are
     not supported (NotImplementedError)."""
+    kind = "handshake"
 
     def __init__(self, model, handshake_size):
-        super().__init__()
-        inner = _inner_mdm(model)
-        if inner.is_prefix_comp or (inner.arch == "trans_dec" and not inner.emb_trans_dec):
+        core = _core(model)
+        if core is None:
+            raise TypeError("HandshakeSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(model))
+        if core[0].is_dip:
             raise NotImplementedError("handshakes are not implemented for prefix-completion (DiP) models")
         if int(handshake_size) < 0:
             raise ValueError("handshake_size must be >= 0 (got %d)" % int(handshake_size))
-        self.model = model
+        super().__init__(model)
         self.handshake_size = int(handshake_size)
-        self.rot2xyz = self.model.rot2xyz
-        self.translation = self.model.translation
-        self.njoints = self.model.njoints
-        self.nfeats = self.model.nfeats
-        self.data_rep = self.model.data_rep
-        self.cond_mode = self.model.cond_mode
-        self.encode_text = self.model.encode_text
 
     def forward(self, x, timesteps, y=None):
-        from ..model.mdm import _run_model
-        guided = isinstance(self.model, ClassifierFreeSampleModel)
+        mdm, guided = _core(self.model)
         if guided:
-            assert self.model.model.cond_mode in ["text", "action"]
-        return _run_model(_inner_mdm(self.model), x, timesteps, y, guided=guided, handshake=self.handshake_size)
-
-    def __getattr__(self, name, default=None):
-        return wrapped_getattr(self, name, default=None)
+            assert mdm.cond_mode in ["text", "action"]
+        return _run_model(mdm, x, timesteps, y, guided=guided, wrapper=self)
 
 
-class JointControlSampleModel(nn.Module):
+class JointControlSampleModel(_SampleWrapper):
     """Joint-position control (this project's definition, DESIGN.md "Joint-position control"): at every DDPM / DDIM step
     the model's x0 (after classifier-free guidance) takes `n_iters` gradient steps of size `step_size` on
 
@@ -135,18 +159,18 @@ class JointControlSampleModel(nn.Module):
     ddim_sample honour it; the other samplers, prefix-completion (DiP) models and AutoRegressiveSampler raise
     NotImplementedError, HandshakeSampleModel and refine_transitions TypeError.  Calling the wrapper is the plain model:
     the guidance belongs to the sampler, as inpainting does."""
+    kind = "joint"
 
     def __init__(self, model, mean, std, step_size, n_iters):
-        super().__init__()
-        from ..model.mdm import MDM
-        inner = model.model if isinstance(model, ClassifierFreeSampleModel) else model
-        if not isinstance(inner, MDM):
+        core = _core(model)
+        if core is None:
             raise TypeError("JointControlSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(model))
+        inner = core[0]
         D = int(inner.njoints) * int(inner.nfeats)
         if inner.data_rep != "hml_vec" or int(inner.nfeats) != 1 or D not in (263, 251):
             raise ValueError("joint-position control needs the ric features of HumanML3D (263) or KIT (251); this model "
                              "has data_rep %r with %d x %d features" % (inner.data_rep, inner.njoints, inner.nfeats))
-        if inner.is_prefix_comp or (inner.arch == "trans_dec" and not inner.emb_trans_dec):
+        if inner.is_dip:
             raise NotImplementedError("joint-position control is not implemented for prefix-completion (DiP) models")
         step, iters = float(step_size), n_iters
         if not (np.isfinite(step) and step > 0):
@@ -157,17 +181,10 @@ class JointControlSampleModel(nn.Module):
                      for v in (mean, std))
         if mean.shape != (D,) or std.shape != (D,):
             raise ValueError("mean and std need %d entries (got %s and %s)" % (D, tuple(mean.shape), tuple(std.shape)))
-        self.model = model
+        super().__init__(model)
         self.mean, self.std = mean, std
         self.step_size, self.n_iters = step, int(iters)
         self.n_joints = 22 if D == 263 else 21
-        self.rot2xyz = self.model.rot2xyz
-        self.translation = self.model.translation
-        self.njoints = self.model.njoints
-        self.nfeats = self.model.nfeats
-        self.data_rep = self.model.data_rep
-        self.cond_mode = self.model.cond_mode
-        self.encode_text = self.model.encode_text
 
     def targets(self, y, shape):
         """(target [B, J, 3, T], weight [B, J, T]) fp32 of y for a sample of `shape`; y is not modified.  ValueError for a
@@ -196,9 +213,6 @@ class JointControlSampleModel(nn.Module):
     def forward(self, x, timesteps, y=None):
         return self.model(x, timesteps, y)
 
-    def __getattr__(self, name, default=None):
-        return wrapped_getattr(self, name, default=None)
-
 
 # HumanML3D's 263 features per frame: root yaw velocity, root XZ velocity, root height (4), then for the 21 non-root
 # joints their root-relative positions (3 each) and rotations (6 each), for all 22 joints their velocities (3 each), and
@@ -222,7 +236,7 @@ def body_part_mask(parts):
     return torch.from_numpy(out)
 
 
-class MultiPromptSampleModel(nn.Module):
+class MultiPromptSampleModel(_SampleWrapper):
     """Multi-prompt guidance (this project's definition, DESIGN.md "Multi-prompt guidance"): K prompts per motion,
     composed around the unconditional prediction as
 
@@ -239,27 +253,19 @@ class MultiPromptSampleModel(nn.Module):
     be 1: it is broadcast, never materialised).  lengths, mask, inpainting and target keys keep their meaning;
     y['text'], y['text_embed'] and y['scale'] are not read.  Every sampler but calc_bpd_loop (NotImplementedError)
     honours it; calling the wrapper returns the composed x0."""
+    kind = "multi"
 
     def __init__(self, model):
-        super().__init__()
-        from ..model.mdm import MDM
         if not isinstance(model, MDM):
             raise TypeError("MultiPromptSampleModel wraps a b200mdm MDM (got %r)" % type(model))
         assert model.cond_mask_prob > 0, \
             "Cannot run a guided diffusion on a model that has not been trained with no conditions"
-        if model.is_prefix_comp or (model.arch == "trans_dec" and not model.emb_trans_dec):
+        if model.is_dip:
             raise NotImplementedError("multi-prompt guidance is not implemented for prefix-completion (DiP) models")
         if model.cond_mode not in ("text", "action"):
             raise ValueError("multi-prompt guidance needs a text- or action-conditioned model (cond_mode %r)"
                              % model.cond_mode)
-        self.model = model
-        self.rot2xyz = self.model.rot2xyz
-        self.translation = self.model.translation
-        self.njoints = self.model.njoints
-        self.nfeats = self.model.nfeats
-        self.data_rep = self.model.data_rep
-        self.cond_mode = self.model.cond_mode
-        self.encode_text = self.model.encode_text
+        super().__init__(model)
 
     def prompts(self, y, shape):
         """(embed [K, B, C] or None, action int64 numpy [B, K] or None, weight fp32 [B, K, D or 1, T or 1]) of y for a
@@ -309,12 +315,8 @@ class MultiPromptSampleModel(nn.Module):
         return torch.cat([self.model.encode_text([p[k] for p in texts]) for k in range(K)], dim=0)
 
     def forward(self, x, timesteps, y=None):
-        from ..model.mdm import _run_model
         self.prompts(y if y is not None else {}, x.shape)       # y's prompts checked before any engine work
-        return _run_model(self.model, x, timesteps, y, guided=False, multi=self)
-
-    def __getattr__(self, name, default=None):
-        return wrapped_getattr(self, name, default=None)
+        return _run_model(self.model, x, timesteps, y, wrapper=self)
 
 
 def stitch_handshake(sample, lengths, handshake_size, motion_start=None):
@@ -431,16 +433,16 @@ def refine_transitions(sample_fn, model, windows, model_kwargs, handshake_size, 
     returned as they are, with no engine call.  `model` is the plain (guided) model: a HandshakeSampleModel raises
     TypeError, a prefix-completion (DiP) model NotImplementedError; layout errors raise ValueError (transition_layout),
     as does skip_timesteps outside [0, num_timesteps).  Gather and paste are device indexing only."""
-    from ..model.mdm import _unwrap, joint_control_of, multi_prompt_of
-    if joint_control_of(model) is not None:
+    r = resolve(model)
+    if r.kind == "joint":
         raise TypeError("refine_transitions is not implemented with joint-position control (JointControlSampleModel)")
-    if multi_prompt_of(model) is not None:
+    if r.kind == "multi":
         raise TypeError("refine_transitions is not implemented with multi-prompt guidance (MultiPromptSampleModel)")
-    inner, hs = _unwrap(model)
-    if hs is not None:
+    if r.kind == "handshake":
         raise TypeError("refine_transitions runs the plain model: pass the model a HandshakeSampleModel wraps, not the wrapper")
-    mdm = _inner_mdm(inner)
-    if mdm.is_prefix_comp or (mdm.arch == "trans_dec" and not mdm.emb_trans_dec):
+    if r.mdm is None:
+        raise TypeError("HandshakeSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(r.core))
+    if r.mdm.is_dip:
         raise NotImplementedError("transitions are not implemented for prefix-completion (DiP) models")
     k = int(skip_timesteps)
     n_steps = getattr(getattr(sample_fn, "__self__", None), "num_timesteps", None)
@@ -450,7 +452,7 @@ def refine_transitions(sample_fn, model, windows, model_kwargs, handshake_size, 
     B, J, F, T = (int(s) for s in windows.shape)
     h = int(handshake_size)
     lay = transition_layout(B, T, h, blend_len, y.get("lengths"), y.get("motion_start"),
-                            min(MAX_TRANSITION_FRAMES, int(mdm.pos_embed_max_len) - 1))
+                            min(MAX_TRANSITION_FRAMES, int(r.mdm.pos_embed_max_len) - 1))
     motions = stitch_handshake(windows, y.get("lengths"), h, y.get("motion_start"))
     n = lay["pairs"].shape[0]
     if n == 0:
@@ -489,7 +491,6 @@ def _chain_plan(sample_fn, model, ar_shape, n_chunks, kargs):
     model a DiP MDM or its ClassifierFreeSampleModel; no keyword outside _CHAIN_KEYS unless at its default; a noise_tape
     only for DDPM / DDIM, without noise_seed, and every tape and x_T of the chain's shapes; a float32 y['prefix']."""
     from ..diffusion import gaussian_diffusion as gd
-    from ..model.mdm import MDM
     from .. import _lib
     diffusion, func = getattr(sample_fn, "__self__", None), getattr(sample_fn, "__func__", None)
     if not isinstance(diffusion, gd.GaussianDiffusion):
@@ -497,8 +498,8 @@ def _chain_plan(sample_fn, model, ar_shape, n_chunks, kargs):
     name = next((k for k in _CHAIN_SAMPLERS if func is getattr(gd.GaussianDiffusion, k)), None)
     if name is None:
         return None
-    inner = model.model if isinstance(model, ClassifierFreeSampleModel) else model
-    if not (isinstance(inner, MDM) and inner.is_prefix_comp and inner.arch == "trans_dec" and not inner.emb_trans_dec):
+    core = _core(model)
+    if core is None or not (core[0].is_prefix_comp and core[0].is_dip):
         return None
     def at_default(k):
         v, d = kargs[k], _CHAIN_DEFAULTS[k]
@@ -552,8 +553,7 @@ class AutoRegressiveSampler:
         self.required_frames = required_frames
 
     def sample(self, model, shape, **kargs):
-        from ..model.mdm import joint_control_of
-        if joint_control_of(model) is not None:
+        if resolve(model).kind == "joint":
             raise NotImplementedError("the autoregressive chain is not implemented with joint-position control")
         pred_len, context_len = self.args.pred_len, self.args.context_len
         n_iterations = self.required_frames // pred_len + int(self.required_frames % pred_len > 0)
