@@ -223,8 +223,8 @@ int b200mdm_set_inpaint_weight(b200mdm_engine* e, const float* weight_dev, const
  * clamp; the DDIM-inversion and variational-bound entry points return B200MDM_ENOTIMPL while it is set.  Call it after
  * b200mdm_set_cond / b200mdm_set_cond_dec, which clear it; h == 0 (or a batch of single-window motions) clears it too.
  * h < 0, a length outside [0, nframes], a chained window with n < h, a window with a predecessor and a successor and
- * n < 2h, or motion_start_host[0] == 0 return B200MDM_EINVAL before any CUDA call; a prefix-completion (DiP) engine
- * B200MDM_ENOTIMPL.  The descriptor is uploaded on `stream`; a step graph captured with it reads it at every replay. */
+ * n < 2h, or motion_start_host[0] == 0 return B200MDM_EINVAL before any CUDA call; a prefix-completion (DiP, context_len
+ * > 0) engine B200MDM_ENOTIMPL.  The descriptor is uploaded on `stream`; a step graph captured with it reads it at every replay. */
 int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t* lengths_host, const uint8_t* motion_start_host,
                           void* stream);
 
@@ -239,8 +239,8 @@ int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t* lengths_h
  * b200mdm_sample_step (modes 1 and 2), b200mdm_sample_loop and b200mdm_sample_loop_range; the PLMS, DPM-Solver++,
  * DDIM-inversion and variational-bound entry points return B200MDM_ENOTIMPL while it is set, and b200mdm_denoise
  * ignores it.  Null pointers, a step that is not finite or <= 0, iters outside 1 .. 10000, or a model other than
- * D = 263 / 251 with nfeats 1 return B200MDM_EINVAL; a prefix-completion (DiP) engine, or handshakes (set before or
- * after), B200MDM_ENOTIMPL. */
+ * D = 263 / 251 with nfeats 1 return B200MDM_EINVAL; a prefix-completion (DiP, context_len > 0) engine, or handshakes
+ * (set before or after), B200MDM_ENOTIMPL. */
 int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_dev, const float* std_dev, const float* target_dev,
                                const float* weight_dev, float step, int32_t iters, void* stream);
 
@@ -253,8 +253,13 @@ int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_dev, const f
  *   b200mdm_set_cond_multi (trans_enc): prompt_embed_dev fp32 [K, batch, cond_dim] device (text models) or
  *     prompt_action_host int64 [batch, K] (action models); lengths as in b200mdm_set_cond.
  *   b200mdm_set_cond_multi_dec (trans_dec with a CLIP memory): prompt_clip_dev fp32 [K, batch, 512] device, one memory row
- *     per group; a prefix-completion (DiP) engine returns B200MDM_ENOTIMPL.
- * Both clear what b200mdm_set_cond clears, and must be followed by b200mdm_set_prompt_weight: w[b, k, f, t] =
+ *     per group; a prefix-completion (DiP) engine returns B200MDM_ENOTIMPL, a BERT-memory engine B200MDM_EINVAL.
+ *   b200mdm_set_cond_multi_tokens (trans_dec with a BERT memory, context_len 0): tokens_dev fp32 [K, n_tokens, batch,
+ *     768] device and mask_host uint8 [K, batch, n_tokens] (1 = padding), every prompt padded to the same n_tokens
+ *     (1 .. 512); lengths as in b200mdm_set_cond_dec.  The unconditional group's memory is the projection bias, padded
+ *     where every prompt is (with K = 1, prompt 0's mask).  A prefix-completion (DiP) engine returns B200MDM_ENOTIMPL, a
+ *     CLIP-memory engine B200MDM_EINVAL.
+ * All three clear what b200mdm_set_cond clears, and must be followed by b200mdm_set_prompt_weight: w[b, k, f, t] =
  * weight_dev[b * stride_b + k * stride_k + f * stride_f + t * stride_t] (fp32, strides in elements, >= 0; a stride of 0
  * broadcasts its dimension), K as given to the conditioning call.  The weights are the caller's and must stay valid until
  * the work enqueued with them has completed; the descriptor is uploaded on `stream`, and a step graph captured with it
@@ -267,6 +272,8 @@ int b200mdm_set_cond_multi(b200mdm_engine* e, int32_t batch, int32_t nframes, in
                            const int64_t* lengths_host, const int64_t* prompt_action_host, void* stream);
 int b200mdm_set_cond_multi_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K, const float* prompt_clip_dev,
                                const int64_t* lengths_host, void* stream);
+int b200mdm_set_cond_multi_tokens(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K, const float* tokens_dev,
+                                  const uint8_t* mask_host, int32_t n_tokens, const int64_t* lengths_host, void* stream);
 int b200mdm_set_prompt_weight(b200mdm_engine* e, int32_t K, const float* weight_dev, int64_t stride_b, int64_t stride_k,
                               int64_t stride_f, int64_t stride_t, void* stream);
 

@@ -38,8 +38,10 @@ SYMBOLS = [
     "b200mdm_set_handshake", "b200mdm_test_blend_handshake", "b200mdm_set_inpaint_weight", "b200mdm_test_out_weight",
     "b200mdm_chain_setup", "b200mdm_chain_loop_range", "b200mdm_set_joint_guidance", "b200mdm_test_joint_guidance",
     "b200mdm_set_cond_multi", "b200mdm_set_cond_multi_dec", "b200mdm_set_prompt_weight",
+    "b200mdm_set_cond_multi_tokens",
 ]
 MAX_PROMPTS = 8                             # B200MDM_MAX_PROMPTS
+MAX_MEMORY_TOKENS = 512                     # a BERT text memory holds 1 .. 512 tokens (DistilBERT's position limit)
 # tap points of b200mdm_test_forward_taps (B200MDM_TAP_*)
 TAPS = ["EMBED", "TOK0", "CONDPROJ", "TEMB", "MEM16", "CROSS_C", "KVC16", "L_IN", "L_QKV", "L_ATT", "L_LN1", "L_QC",
         "L_XATT", "L_LN2", "L_FFN", "L_LN3", "BLEND"]
@@ -135,6 +137,7 @@ def load():
                        ("b200mdm_test_joint_guidance", [vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, vp, vp, vp]),
                        ("b200mdm_set_cond_multi", [vp, i32, i32, i32, vp, vp, vp, vp]),
                        ("b200mdm_set_cond_multi_dec", [vp, i32, i32, i32, vp, vp, vp]),
+                       ("b200mdm_set_cond_multi_tokens", [vp, i32, i32, i32, vp, vp, i32, vp, vp]),
                        ("b200mdm_set_prompt_weight", [vp, i32, vp, i64, i64, i64, i64, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args

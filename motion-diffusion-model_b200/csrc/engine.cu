@@ -1322,6 +1322,32 @@ static int set_cond_dec_clip(b200mdm_engine* e, int32_t batch, int32_t nframes, 
   return B200MDM_OK;
 }
 
+// trans_dec with a BERT memory and context_len > 0: DiP, the prefix-completion decoder (context_len 0 is the plain BERT
+// decoder, which takes every sampling extension)
+static bool is_prefix_engine(const b200mdm_engine* e) { return e->dec && !e->dec_clip && e->ctx > 0; }
+
+// The text-memory buffers of the current workspace for Mt tokens, rebuilt when Mt changes: the projected prompt rows
+// (B, or K * B under multi-prompt guidance) and the packed batch's Bp rows.
+static int ensure_text_memory(b200mdm_engine* e, int Mt) {
+  if (Mt == e->Mt) return B200MDM_OK;
+  const int d = e->d, Bp = e->Bp, C = e->cfg.cond_dim;
+  const size_t cond_rows = static_cast<size_t>(e->groups ? Bp - e->B : e->B);
+  CUDA_TRY(cudaDeviceSynchronize());
+  drop_graph(e);
+  dfree(e->encperm); dfree(e->memtok); dfree(e->memproj); dfree(e->mem16); dfree(e->kvc16); dfree(e->memmask);
+  e->Mt = 0;   // until every buffer below exists: a failed allocation leaves the next call to rebuild them
+  TRY(dalloc(&e->encperm, cond_rows * Mt * C));
+  TRY(dalloc(&e->memtok, cond_rows * Mt * d));
+  TRY(dalloc(&e->memproj, static_cast<size_t>(Bp) * Mt * d));
+  TRY(dalloc(&e->mem16, static_cast<size_t>(Bp) * Mt * 2 * d));   // [hi | lo]
+  TRY(dalloc(&e->kvc16, static_cast<size_t>(Bp) * Mt * 2 * d * e->L));      // [Bp*Mt, L * (k | v)]
+  TRY(dalloc(&e->memmask, static_cast<size_t>(Bp) * Mt));
+  TRY(make_map(&e->m_mem, e->mem16, static_cast<uint64_t>(Bp) * Mt, 2 * d, 2 * d, GEMM_BLOCK_M));
+  TRY(make_map_t(&e->m_kvc_st, e->kvc16, 2, static_cast<uint64_t>(Bp) * Mt, 2 * d * e->L, 2 * d * e->L, 32));
+  e->Mt = Mt;
+  return B200MDM_OK;
+}
+
 // ---- trans_dec (DiP) conditioning: BERT token features + padding mask as the cross-attention memory, prefix frames
 extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* enc_text_dev,
                                     const uint8_t* text_mask_host, int32_t n_tokens, const int64_t* lengths_host,
@@ -1341,21 +1367,7 @@ extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nf
   const int halves = scale_dev ? 2 : 1;
   TRY(select_workspace(e, batch, nframes, halves, s));
   const int d = e->d, B = batch, Bp = e->Bp, Mt = n_tokens, C = e->cfg.cond_dim;
-  if (Mt != e->Mt) {
-    CUDA_TRY(cudaDeviceSynchronize());
-    drop_graph(e);
-    dfree(e->encperm); dfree(e->memtok); dfree(e->memproj); dfree(e->mem16); dfree(e->kvc16); dfree(e->memmask);
-    e->Mt = 0;   // until every buffer below exists: a failed allocation leaves the next call to rebuild them
-    TRY(dalloc(&e->encperm, static_cast<size_t>(B) * Mt * C));
-    TRY(dalloc(&e->memtok, static_cast<size_t>(B) * Mt * d));
-    TRY(dalloc(&e->memproj, static_cast<size_t>(Bp) * Mt * d));
-    TRY(dalloc(&e->mem16, static_cast<size_t>(Bp) * Mt * 2 * d));   // [hi | lo]
-    TRY(dalloc(&e->kvc16, static_cast<size_t>(Bp) * Mt * 2 * d * e->L));      // [Bp*Mt, L * (k | v)]
-    TRY(dalloc(&e->memmask, static_cast<size_t>(Bp) * Mt));
-    TRY(make_map(&e->m_mem, e->mem16, static_cast<uint64_t>(Bp) * Mt, 2 * d, 2 * d, GEMM_BLOCK_M));
-    TRY(make_map_t(&e->m_kvc_st, e->kvc16, 2, static_cast<uint64_t>(Bp) * Mt, 2 * d * e->L, 2 * d * e->L, 32));
-    e->Mt = Mt;
-  }
+  TRY(ensure_text_memory(e, Mt));
   // key mask of the frames: the context frames are always valid (model/mdm.py:204-206), then `lengths` frames of x
   TRY(upload_kvlen_scale(e, nframes, e->ctx, e->S > 1, lengths_host, scale_dev, s));
   std::vector<unsigned char>& mk = e->h_mask;
@@ -1424,7 +1436,7 @@ extern "C" int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t
                                      const uint8_t* motion_start_host, void* stream) {
   if (!e) return fail(B200MDM_EINVAL, "null engine");
   if (h < 0) return fail(B200MDM_EINVAL, "handshake size %d < 0", h);
-  if (e->dec && !e->dec_clip) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented for prefix-completion (DiP) models");
+  if (is_prefix_engine(e)) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented for prefix-completion (DiP) models");
   if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
   if (e->jg_set) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented with joint-position control");
   if (e->groups) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented with multi-prompt guidance");
@@ -1448,7 +1460,7 @@ extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_d
   if (e->cfg.nfeats != 1 || (e->JF != 263 && e->JF != 251))
     return fail(B200MDM_EINVAL, "joint-position control needs the ric features of HumanML3D (263) or KIT (251) with nfeats 1 "
                 "(got %d x %d)", e->cfg.njoints, e->cfg.nfeats);
-  if (e->dec && !e->dec_clip)
+  if (is_prefix_engine(e))
     return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented for prefix-completion (DiP) models");
   if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
   if (e->hs_set) return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented with handshakes");
@@ -1512,8 +1524,10 @@ extern "C" int b200mdm_set_cond_multi_dec(b200mdm_engine* e, int32_t batch, int3
                                           const float* prompt_clip_dev, const int64_t* lengths_host, void* stream) {
   if (!e) return fail(B200MDM_EINVAL, "null engine");
   if (!e->dec) return fail(B200MDM_EINVAL, "b200mdm_set_cond_multi_dec is for trans_dec engines");
-  if (!e->dec_clip)
+  if (is_prefix_engine(e))
     return fail(B200MDM_ENOTIMPL, "multi-prompt guidance is not implemented for prefix-completion (DiP) models");
+  if (!e->dec_clip)
+    return fail(B200MDM_EINVAL, "BERT-memory decoders take their prompts through b200mdm_set_cond_multi_tokens");
   if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
   TRY(check_prompts(batch, nframes, K));
   if (!prompt_clip_dev) return fail(B200MDM_EINVAL, "the CLIP decoder needs the prompt embeddings [K, B, C]");
@@ -1524,6 +1538,57 @@ extern "C" int b200mdm_set_cond_multi_dec(b200mdm_engine* e, int32_t batch, int3
   // one memory row per group: W clip_k + b for the prompts, b for the unconditional group
   TRY(fill_condproj(e, prompt_clip_dev, false, s, K * batch));
   TRY(cross_rows_per_sample(e, nullptr, s));
+  end_cond(e);
+  return B200MDM_OK;
+}
+
+// The BERT decoder (context_len 0): one token memory per group, W tokens_k + b for the prompts and b for the
+// unconditional group (mask_cond zeroes the tokens, model/mdm.py:218).  The unconditional group admits every token some
+// prompt admits: with K = 1 that is prompt 0's mask, as in b200mdm_set_cond_dec's classifier-free pair, and it does not
+// depend on the prompts' order.  (Its tokens are all equal, so any mask admitting one gives the same output up to
+// rounding.)
+extern "C" int b200mdm_set_cond_multi_tokens(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K,
+                                             const float* tokens_dev, const uint8_t* mask_host, int32_t n_tokens,
+                                             const int64_t* lengths_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!e->dec) return fail(B200MDM_EINVAL, "b200mdm_set_cond_multi_tokens is for trans_dec engines");
+  if (is_prefix_engine(e))
+    return fail(B200MDM_ENOTIMPL, "multi-prompt guidance is not implemented for prefix-completion (DiP) models");
+  if (e->dec_clip) return fail(B200MDM_EINVAL, "CLIP-memory decoders take their prompts through b200mdm_set_cond_multi_dec");
+  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
+  TRY(check_prompts(batch, nframes, K));
+  if (n_tokens <= 0 || n_tokens > XAL_MAX_MT)
+    return fail(B200MDM_EINVAL, "n_tokens %d: a text memory holds 1..%d tokens (DistilBERT's position limit)", n_tokens, XAL_MAX_MT);
+  if (!tokens_dev || !mask_host) return fail(B200MDM_EINVAL, "the BERT decoder needs the prompt tokens and masks");
+  TRY(check_seq_len(e, nframes + e->ctx));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  TRY(select_workspace(e, batch, nframes, 1, s, K + 1));
+  const int d = e->d, B = batch, Bp = e->Bp, Mt = n_tokens, C = e->cfg.cond_dim, rows = K * B;
+  TRY(ensure_text_memory(e, Mt));
+  TRY(upload_kvlen_scale(e, nframes, e->ctx, e->S > 1, lengths_host, nullptr, s));
+  // [K, B, Mt] is already the prompts' groups in packed order; the unconditional group pads where every prompt pads
+  std::vector<unsigned char>& mk = e->h_mask;
+  mk.assign(static_cast<size_t>(Bp) * Mt, 1);
+  for (int bp = 0; bp < rows; ++bp)
+    for (int m = 0; m < Mt; ++m) {
+      const unsigned char pad = mask_host[static_cast<size_t>(bp) * Mt + m] ? 1 : 0;
+      mk[static_cast<size_t>(bp) * Mt + m] = pad;
+      mk[static_cast<size_t>(rows + bp % B) * Mt + m] &= pad;
+    }
+  CUDA_TRY(cudaMemcpyAsync(e->memmask, mk.data(), mk.size(), cudaMemcpyHostToDevice, s));
+  for (int k = 0; k < K; ++k) {
+    permute_mbc_kernel<<<dim3(Mt, B), 128, 0, s>>>(tokens_dev + static_cast<size_t>(k) * Mt * B * C,
+                                                    e->encperm + static_cast<size_t>(k) * B * Mt * C, Mt, B, C);
+    CUDA_TRY(cudaGetLastError());
+  }
+  const size_t warps = static_cast<size_t>(rows) * Mt * d;
+  small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(e->encperm, e->w_txt, e->b_txt, e->memtok,
+                                                                                     rows * Mt, d, C, C);
+  CUDA_TRY(cudaGetLastError());
+  memproj_group_fill_kernel<<<dim3(Mt, Bp), 128, 0, s>>>(e->memproj, e->memtok, e->b_txt, rows, Mt, d);
+  CUDA_TRY(cudaGetLastError());
+  e->mem_uncond = false;
+  e->launches += K + 2;
   end_cond(e);
   return B200MDM_OK;
 }
@@ -2257,8 +2322,6 @@ extern "C" int b200mdm_dpm_pred_xstart(b200mdm_engine* e, float* out_dev, void* 
 }
 
 // ------------------------------------------------------------------------------------------------ autoregressive chain
-static bool is_prefix_engine(const b200mdm_engine* e) { return e->dec && !e->dec_clip && e->ctx > 0; }
-
 template <class T>
 static int ensure_cap(T** p, size_t* cap, size_t n) {
   if (*cap >= n) return B200MDM_OK;

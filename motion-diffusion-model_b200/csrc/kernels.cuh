@@ -527,6 +527,16 @@ __global__ void memproj_fill_kernel(float* __restrict__ memproj, const float* __
     memproj[(static_cast<size_t>(bp) * Mt + m) * d + c] = unc ? bias[c] : proj[(static_cast<size_t>(b) * Mt + m) * d + c];
 }
 
+// memproj rows of multi-prompt guidance's packed batch (b200mdm_set_cond_multi_tokens): the cond_rows = K * B rows of
+// the prompts' groups are W tokens + b (proj [cond_rows*Mt, d], rows (k*B + b, m), group-major as the packed batch), the
+// unconditional group's rows b.  grid = (Mt, Bp)
+__global__ void memproj_group_fill_kernel(float* __restrict__ memproj, const float* __restrict__ proj,
+                                          const float* __restrict__ bias, int cond_rows, int Mt, int d) {
+  const int m = blockIdx.x, bp = blockIdx.y;
+  const size_t row = static_cast<size_t>(bp) * Mt + m;
+  for (int c = threadIdx.x; c < d; c += blockDim.x) memproj[row * d + c] = bp < cond_rows ? proj[row * d + c] : bias[c];
+}
+
 // enc_text [Mt, B, C] (reference layout, model/mdm.py:185) -> [B*Mt, C] rows (b, m) so that one small GEMM projects it
 __global__ void permute_mbc_kernel(const float* __restrict__ src, float* __restrict__ dst, int Mt, int B, int C) {
   const int m = blockIdx.x, b = blockIdx.y;

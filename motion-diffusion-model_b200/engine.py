@@ -314,6 +314,17 @@ class Engine:
         self._keep["cond"] = (enc, sc, pf)
         self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 2 if sc is not None else 1, Mt
 
+    def prompt_memories(self, pairs, batch, device):
+        """(tokens fp32 [K, Mt, batch, C] contiguous on device, padding mask uint8 numpy [K, batch, Mt]) of K BERT
+        (tokens [Mt_k, batch, C], mask [batch, Mt_k]) pairs, each padded to the longest Mt with masked zero tokens."""
+        Mt = max(int(t.shape[0]) for t, _ in pairs)
+        tok = torch.zeros(len(pairs), Mt, batch, self.cfg.cond_dim, device=device, dtype=torch.float32)
+        mask = np.ones((len(pairs), batch, Mt), dtype=np.uint8)
+        for k, (t, m) in enumerate(pairs):
+            tok[k, :t.shape[0]] = t.detach().to(device=device, dtype=torch.float32)
+            mask[k, :, :t.shape[0]] = m.detach().cpu().numpy() != 0
+        return tok, mask
+
     def set_inpaint(self, mask, motion):
         if mask is None:
             check(self.lib.b200mdm_set_inpaint(self.h, None, None))
@@ -351,22 +362,31 @@ class Engine:
         self._keep["joint"] = ts
 
     def set_cond_multi(self, batch, nframes, y, embed, action, weight, device):
-        """Multi-prompt guidance (b200mdm_set_cond_multi / _dec, then b200mdm_set_prompt_weight): embed fp32 [K, B, C]
-        (text models) or action int64 numpy [B, K] (action models), weight fp32 [B, K, D or 1, T or 1], as
-        MultiPromptSampleModel.prompts returns them; lengths and the target from y as set_cond takes them."""
+        """Multi-prompt guidance (b200mdm_set_cond_multi / _dec / _tokens, then b200mdm_set_prompt_weight): embed fp32
+        [K, B, C] (text models; for the BERT decoder a list of K (tokens [Mt_k, B, C], mask [B, Mt_k]) pairs) or action
+        int64 numpy [B, K] (action models), weight fp32 [B, K, D or 1, T or 1], as MultiPromptSampleModel.prompts returns
+        them; lengths and the target from y as set_cond takes them."""
         y = y or {}
         K = int(weight.shape[1])
         ln, _ = self._lengths_and_scale(batch, y, False, device)
         ln_p = None if ln is None else ln.ctypes.data_as(ctypes.c_void_p)
-        te = None if embed is None else embed.detach().to(device=device, dtype=torch.float32).contiguous()
-        if self.dec:
-            check(self.lib.b200mdm_set_cond_multi_dec(self.h, batch, nframes, K, _ptr(te), ln_p, _stream()))
+        n_tokens = 1
+        if self.dec and not self.dec_clip:
+            te, mask = self.prompt_memories(embed, batch, device)
+            n_tokens = int(te.shape[1])
+            check(self.lib.b200mdm_set_cond_multi_tokens(self.h, batch, nframes, K, _ptr(te),
+                                                         mask.ctypes.data_as(ctypes.c_void_p), n_tokens, ln_p, _stream()))
+            self._keep["cond_mask"] = mask
         else:
-            ac = None if action is None else np.ascontiguousarray(action, dtype=np.int64)
-            check(self.lib.b200mdm_set_cond_multi(self.h, batch, nframes, K, _ptr(te), ln_p,
-                                                  None if ac is None else ac.ctypes.data_as(ctypes.c_void_p), _stream()))
+            te = None if embed is None else embed.detach().to(device=device, dtype=torch.float32).contiguous()
+            if self.dec:
+                check(self.lib.b200mdm_set_cond_multi_dec(self.h, batch, nframes, K, _ptr(te), ln_p, _stream()))
+            else:
+                ac = None if action is None else np.ascontiguousarray(action, dtype=np.int64)
+                check(self.lib.b200mdm_set_cond_multi(self.h, batch, nframes, K, _ptr(te), ln_p,
+                                                      None if ac is None else ac.ctypes.data_as(ctypes.c_void_p), _stream()))
         self._keep["cond"] = (te,)
-        self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 1, 1
+        self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 1, n_tokens
         self._set_target(batch, y, device)
         w = weight.detach().to(device=device, dtype=torch.float32).contiguous()
         strides = [0 if w.shape[i] == 1 else w.stride(i) for i in range(4)]

@@ -10,7 +10,9 @@ text_encoder_type='bert' (DiP: BERT token memory, prefix completion, model/mdm.p
 with text_encoder_type='clip' and emb_trans_dec=True (the humanml-decoder-with-emb checkpoint: timestep token 0, the
 CLIP row + timestep embedding as a one-token memory, mdm.py:256-270; y takes the encoder's keys); hml_vec / rot6d /
 xyz data_rep; target-location conditioning (multi_target_cond, the single / multi / split encoders, model/mdm.py:64-73,
-197-199,399-480) with any of them.
+197-199,399-480) with any of them.  The sampling extensions (HandshakeSampleModel, refine_transitions,
+JointControlSampleModel, MultiPromptSampleModel) take every implemented model but prefix completion: the BERT decoder with
+context_len 0 (humanml_trans_dec_512_bert) included, DiP with context_len > 0 (is_prefix_comp) not.
 Not implemented (raise): arch 'gru', data_rep 'rot_vel', emb_policy != 'add', trans_dec with CLIP features and
 emb_trans_dec=False, trans_dec with BERT and emb_trans_dec=True, trans_dec with action / no_cond conditioning.
 """
@@ -250,8 +252,8 @@ class MDM(_Bag):
 
     @property
     def is_dip(self):
-        """trans_dec with a BERT token memory: DiP, the prefix-completion decoder (the constructor admits no other
-        trans_dec without emb_trans_dec)."""
+        """trans_dec with a BERT token memory (the constructor admits no other trans_dec without emb_trans_dec), with or
+        without prefix completion; DiP proper is is_dip and is_prefix_comp (context_len > 0)."""
         return self.arch == "trans_dec" and not self.emb_trans_dec
 
     def forward(self, x, timesteps, y=None):

@@ -85,6 +85,8 @@ def shard_model_kwargs(model_kwargs, lo, hi):
             out[k] = v[:, lo:hi].contiguous() if v.shape[1] > 1 else v      # [1, B, C]; a single prompt is shared
         elif k == "prompt_embed" and torch.is_tensor(v):                     # [K, B, C]
             out[k] = v[:, lo:hi].contiguous()
+        elif k == "prompt_embed" and isinstance(v, (list, tuple)):           # BERT: K (tokens [Mt, B, C], mask [B, Mt])
+            out[k] = [(tok[:, lo:hi].contiguous(), msk[lo:hi].contiguous()) for tok, msk in v]
         elif k == "text_embed" and isinstance(v, tuple):                     # DiP: (tokens [Mt, B, C], mask [B, Mt])
             tok, msk = v
             out[k] = (tok[:, lo:hi].contiguous() if tok.shape[1] > 1 else tok, msk[lo:hi].contiguous() if msk.shape[0] > 1 else msk)

@@ -124,15 +124,16 @@ class HandshakeSampleModel(_SampleWrapper):
 
     so every denoising step forces the two to agree.  `model` is a b200mdm MDM or ClassifierFreeSampleModel; the blend
     runs inside the engine's guidance-blend kernel, in every sampler (DDPM, DDIM, PLMS, DPM-Solver++).  Stitch the
-    final windows with `stitch_handshake`.  Prefix-completion (DiP) models, DDIM inversion and the variational bound are
-    not supported (NotImplementedError)."""
+    final windows with `stitch_handshake`.  Every model the engine runs is supported, the BERT decoder (context_len 0)
+    included; prefix-completion (DiP, context_len > 0) models, DDIM inversion and the variational bound are not
+    (NotImplementedError)."""
     kind = "handshake"
 
     def __init__(self, model, handshake_size):
         core = _core(model)
         if core is None:
             raise TypeError("HandshakeSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(model))
-        if core[0].is_dip:
+        if core[0].is_prefix_comp:
             raise NotImplementedError("handshakes are not implemented for prefix-completion (DiP) models")
         if int(handshake_size) < 0:
             raise ValueError("handshake_size must be >= 0 (got %d)" % int(handshake_size))
@@ -156,7 +157,8 @@ class JointControlSampleModel(_SampleWrapper):
     layout and units; y['joint_weight'] [B, J, T] (float >= 0, or bool) is 0 where a joint is free.  `model` is a b200mdm
     MDM or ClassifierFreeSampleModel of HumanML3D (263 features, J = 22) or KIT (251, J = 21); mean / std [D] are the
     dataset's normalisation.  p_sample_loop, ddim_sample_loop (any eta), their _progressive forms, p_sample and
-    ddim_sample honour it; the other samplers, prefix-completion (DiP) models and AutoRegressiveSampler raise
+    ddim_sample honour it, for every model the engine runs (the BERT decoder with context_len 0 included); the other
+    samplers, prefix-completion (DiP, context_len > 0) models and AutoRegressiveSampler raise
     NotImplementedError, HandshakeSampleModel and refine_transitions TypeError.  Calling the wrapper is the plain model:
     the guidance belongs to the sampler, as inpainting does."""
     kind = "joint"
@@ -170,7 +172,7 @@ class JointControlSampleModel(_SampleWrapper):
         if inner.data_rep != "hml_vec" or int(inner.nfeats) != 1 or D not in (263, 251):
             raise ValueError("joint-position control needs the ric features of HumanML3D (263) or KIT (251); this model "
                              "has data_rep %r with %d x %d features" % (inner.data_rep, inner.njoints, inner.nfeats))
-        if inner.is_dip:
+        if inner.is_prefix_comp:
             raise NotImplementedError("joint-position control is not implemented for prefix-completion (DiP) models")
         step, iters = float(step_size), n_iters
         if not (np.isfinite(step) and step > 0):
@@ -246,11 +248,14 @@ class MultiPromptSampleModel(_SampleWrapper):
     nonzero on that part's features only (body_part_mask), a time-varying prompt a weight that changes with t, a negative
     prompt a negative weight; K = 1 with the weight y['scale'][b] is ClassifierFreeSampleModel's formula.
 
-    `model` is a b200mdm MDM: trans_enc with CLIP text or action conditioning, or the CLIP decoder with a timestep token
-    (prefix-completion (DiP) models raise NotImplementedError, any wrapper TypeError).  y carries the prompts as
-    y['prompt_embed'] fp32 [K, B, C] (or y['prompt_text'], B lists of K strings, which the sampler encodes into it) or
+    `model` is a b200mdm MDM: trans_enc with CLIP text or action conditioning, the CLIP decoder with a timestep token, or
+    the BERT decoder with context_len 0 (prefix-completion (DiP, context_len > 0) models raise NotImplementedError, any
+    wrapper TypeError).  y carries the prompts as y['prompt_embed'] fp32 [K, B, C] (for the BERT decoder a list of K
+    (tokens [Mt_k, B, 768], padding mask [B, Mt_k]) pairs as encode_text returns them, padded here to the longest) or
+    y['prompt_text'] (B lists of K strings, which the sampler encodes into it, one prompt at a time), or
     y['prompt_action'] [B, K] for action models, and y['prompt_weight'] float [B, K, D, T] (either of the last two may
-    be 1: it is broadcast, never materialised).  lengths, mask, inpainting and target keys keep their meaning;
+    be 1: it is broadcast, never materialised).  The BERT decoder's unconditional prediction admits every token some
+    prompt admits (with K = 1, prompt 0's mask).  lengths, mask, inpainting and target keys keep their meaning;
     y['text'], y['text_embed'] and y['scale'] are not read.  Every sampler but calc_bpd_loop (NotImplementedError)
     honours it; calling the wrapper returns the composed x0."""
     kind = "multi"
@@ -260,7 +265,7 @@ class MultiPromptSampleModel(_SampleWrapper):
             raise TypeError("MultiPromptSampleModel wraps a b200mdm MDM (got %r)" % type(model))
         assert model.cond_mask_prob > 0, \
             "Cannot run a guided diffusion on a model that has not been trained with no conditions"
-        if model.is_dip:
+        if model.is_prefix_comp:
             raise NotImplementedError("multi-prompt guidance is not implemented for prefix-completion (DiP) models")
         if model.cond_mode not in ("text", "action"):
             raise ValueError("multi-prompt guidance needs a text- or action-conditioned model (cond_mode %r)"
@@ -268,10 +273,11 @@ class MultiPromptSampleModel(_SampleWrapper):
         super().__init__(model)
 
     def prompts(self, y, shape):
-        """(embed [K, B, C] or None, action int64 numpy [B, K] or None, weight fp32 [B, K, D or 1, T or 1]) of y for a
-        sample of `shape`; y is not modified, and y['prompt_text'] is not encoded (embed is None for it).  ValueError
-        for a missing or mis-shaped key, K outside 1 .. MAX_PROMPTS, an action outside the model's classes, or a weight
-        that is not finite."""
+        """(embed [K, B, C] (a list of K (tokens, mask) pairs for the BERT decoder) or None, action int64 numpy [B, K] or
+        None, weight fp32 [B, K, D or 1, T or 1]) of y for a sample of `shape`; y is not modified, and y['prompt_text']
+        is not encoded (embed is None for it).  ValueError for a missing or mis-shaped key, K outside 1 .. MAX_PROMPTS,
+        a memory outside 1 .. MAX_MEMORY_TOKENS tokens, an action outside the model's classes, or a weight that is not
+        finite."""
         from .. import _lib
         B, T = int(shape[0]), int(shape[-1])
         D = int(self.model.njoints) * int(self.model.nfeats)
@@ -305,18 +311,40 @@ class MultiPromptSampleModel(_SampleWrapper):
                 raise ValueError("y['prompt_text'] must hold B = %d lists of K = %d strings" % (B, K))
             return None, None, w
         C = int(self.model.clip_dim)
+        if self.model.text_encoder_type == "bert":
+            return _token_prompts(e, K, B, C), None, w
         if not torch.is_tensor(e) or not e.is_floating_point() or tuple(e.shape) != (K, B, C):
             raise ValueError("y['prompt_embed'] must be a float tensor [%d, %d, %d]" % (K, B, C))
         return e, None, w
 
     def encode_prompts(self, texts):
-        """[K, B, C] text features of y['prompt_text'] (B lists of K strings), the model's encode_text per prompt."""
+        """[K, B, C] text features of y['prompt_text'] (B lists of K strings), the model's encode_text per prompt; for the
+        BERT decoder the list of K (tokens, mask) pairs."""
         K = len(texts[0])
-        return torch.cat([self.model.encode_text([p[k] for p in texts]) for k in range(K)], dim=0)
+        enc = [self.model.encode_text([p[k] for p in texts]) for k in range(K)]
+        return enc if self.model.text_encoder_type == "bert" else torch.cat(enc, dim=0)
 
     def forward(self, x, timesteps, y=None):
         self.prompts(y if y is not None else {}, x.shape)       # y's prompts checked before any engine work
         return _run_model(self.model, x, timesteps, y, wrapper=self)
+
+
+def _token_prompts(e, K, B, C):
+    """y['prompt_embed'] of the BERT decoder, checked: a list of K (tokens float [Mt_k, B, C], padding mask bool or
+    integer [B, Mt_k]) pairs, 1 <= Mt_k <= MAX_MEMORY_TOKENS."""
+    from .. import _lib
+    if not isinstance(e, (list, tuple)) or len(e) != K or any(not isinstance(p, tuple) or len(p) != 2 for p in e):
+        raise ValueError("the BERT decoder's y['prompt_embed'] must be a list of K = %d (tokens [Mt, %d, %d], mask [%d, Mt]) "
+                         "pairs" % (K, B, C, B))
+    for k, (tok, msk) in enumerate(e):
+        if not torch.is_tensor(tok) or not tok.is_floating_point() or tok.dim() != 3 or tuple(tok.shape[1:]) != (B, C):
+            raise ValueError("prompt %d: tokens must be a float tensor [Mt, %d, %d]" % (k, B, C))
+        Mt = int(tok.shape[0])
+        if not 1 <= Mt <= _lib.MAX_MEMORY_TOKENS:
+            raise ValueError("prompt %d: %d tokens outside 1 .. %d" % (k, Mt, _lib.MAX_MEMORY_TOKENS))
+        if not torch.is_tensor(msk) or msk.is_floating_point() or msk.is_complex() or tuple(msk.shape) != (B, Mt):
+            raise ValueError("prompt %d: the padding mask must be a bool or integer tensor [%d, %d]" % (k, B, Mt))
+    return list(e)
 
 
 def stitch_handshake(sample, lengths, handshake_size, motion_start=None):
@@ -407,6 +435,10 @@ def _transition_y(y, windows, Lt, device):
         v = y[k]
         if k == "text_embed" and torch.is_tensor(v):
             out[k] = v if v.shape[1] == 1 else v[:, idx.to(v.device)]          # [1, B, C]; a single prompt is shared
+        elif k == "text_embed" and isinstance(v, tuple):                      # BERT: (tokens [Mt, B, C], mask [B, Mt])
+            tok, msk = v
+            out[k] = (tok if tok.shape[1] == 1 else tok[:, idx.to(tok.device)],
+                      msk if msk.shape[0] == 1 else msk[idx.to(msk.device)])
         elif torch.is_tensor(v):
             out[k] = v[idx.to(v.device)]
         elif isinstance(v, np.ndarray):
@@ -431,7 +463,7 @@ def refine_transitions(sample_fn, model, windows, model_kwargs, handshake_size, 
     and y['inpainted_motion'] = x_init, and by default each transition window b's conditioning (transition_kwargs replaces
     it).  The refined frames 1 .. Lt - 2 are pasted into stitch_handshake's motions; without a chained pair those are
     returned as they are, with no engine call.  `model` is the plain (guided) model: a HandshakeSampleModel raises
-    TypeError, a prefix-completion (DiP) model NotImplementedError; layout errors raise ValueError (transition_layout),
+    TypeError, a prefix-completion (DiP, context_len > 0) model NotImplementedError; layout errors raise ValueError (transition_layout),
     as does skip_timesteps outside [0, num_timesteps).  Gather and paste are device indexing only."""
     r = resolve(model)
     if r.kind == "joint":
@@ -442,7 +474,7 @@ def refine_transitions(sample_fn, model, windows, model_kwargs, handshake_size, 
         raise TypeError("refine_transitions runs the plain model: pass the model a HandshakeSampleModel wraps, not the wrapper")
     if r.mdm is None:
         raise TypeError("HandshakeSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(r.core))
-    if r.mdm.is_dip:
+    if r.mdm.is_prefix_comp:
         raise NotImplementedError("transitions are not implemented for prefix-completion (DiP) models")
     k = int(skip_timesteps)
     n_steps = getattr(getattr(sample_fn, "__self__", None), "num_timesteps", None)
