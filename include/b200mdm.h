@@ -244,6 +244,21 @@ int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t* lengths_h
 int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_dev, const float* std_dev, const float* target_dev,
                                const float* weight_dev, float step, int32_t iters, void* stream);
 
+/* Foot-contact and floor terms of joint-position control (DESIGN.md "Joint-position control", "Foot contact and floor"):
+ * the guided energy becomes
+ *   G = G_joint + 1/2 contact_weight sum_{k<4, t<T-1} kappa[b,k,t] |p[t+1, f_k] - p[t, f_k]|^2
+ *               + 1/2 floor_weight sum_{t<L_b, j} min(p[t,j].y - floor_height, 0)^2,
+ * with the same steps and iterations.  Contact channel k = D - 4 + k belongs to foot joint f_k: 7, 10, 8, 11
+ * (HumanML3D) or 19, 20, 14, 15 (KIT); channel t describes the frame pair (t, t+1).  contact_dev fp32 [B, 4, T] >= 0
+ * gives kappa (the caller's, valid until the work enqueued with it has completed); NULL derives kappa[b,k,t] = 1 where
+ * the step's de-normalised x0 has channel k > 0.5 at frame t and t + 1 < L_b, else 0.  lengths_host int64 [B] >= 0
+ * (NULL: every frame) gives L_b = min(lengths[b], T).  Both weights 0 turn the terms off.  A negative or non-finite
+ * weight, a non-finite height or a negative length return B200MDM_EINVAL; without b200mdm_set_joint_guidance for the
+ * current conditioning, B200MDM_ESTATE.  b200mdm_set_cond* and b200mdm_set_joint_guidance clear it.  The terms live in
+ * the guidance descriptor, so a step graph captured with them reads new values at every replay. */
+int b200mdm_set_foot_guidance(b200mdm_engine* e, float contact_weight, float floor_weight, float floor_height,
+                              const float* contact_dev, const int64_t* lengths_host, void* stream);
+
 /* Multi-prompt guidance (this project's definition, DESIGN.md "Multi-prompt guidance"): K prompts per motion, composed
  * around the unconditional prediction as
  *   x0[b, f, t] = x0_u + sum_{k=0..K-1} w[b, k, f, t] (x0_k - x0_u)
@@ -515,6 +530,14 @@ int b200mdm_test_blend_handshake(const void* hres16_dev, const float* scale_dev,
 int b200mdm_test_joint_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
                                 const float* weight_dev, int32_t B, int32_t T, int32_t D, float step, int32_t iters,
                                 float* x0_out_dev, float* loss_out_dev, void* stream);
+/* The guidance iterations with the foot-contact and floor terms of b200mdm_set_foot_guidance alone
+ * (joint_guidance_test_kernel<true>): as b200mdm_test_joint_guidance, with contact_dev / lengths_host (both nullable) and
+ * the weights and height as there; loss_out receives the total G.  Invalid arguments return B200MDM_EINVAL before any
+ * CUDA call. */
+int b200mdm_test_foot_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
+                               const float* weight_dev, const float* contact_dev, const int64_t* lengths_host, int32_t B,
+                               int32_t T, int32_t D, float step, int32_t iters, float contact_weight, float floor_weight,
+                               float floor_height, float* x0_out_dev, float* loss_out_dev, void* stream);
 /* Self-attention core (tensor-core kernel, S <= 256): softmax(q k^T / sqrt(128) + mask) v per (sample, head);
  * qkv16 [n*S, 3d]; kvlen int32 [n] device (valid keys per sample, a prefix).
  * impl 0: out16 fp16 [n*S, d] (the encoder); impl 1: out16 fp16 [n*S, 2d] = [hi | lo] with hi + lo = the fp32 result

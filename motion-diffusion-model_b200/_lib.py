@@ -38,7 +38,7 @@ SYMBOLS = [
     "b200mdm_set_handshake", "b200mdm_test_blend_handshake", "b200mdm_set_inpaint_weight", "b200mdm_test_out_weight",
     "b200mdm_chain_setup", "b200mdm_chain_loop_range", "b200mdm_set_joint_guidance", "b200mdm_test_joint_guidance",
     "b200mdm_set_cond_multi", "b200mdm_set_cond_multi_dec", "b200mdm_set_prompt_weight",
-    "b200mdm_set_cond_multi_tokens",
+    "b200mdm_set_cond_multi_tokens", "b200mdm_set_foot_guidance", "b200mdm_test_foot_guidance",
 ]
 MAX_PROMPTS = 8                             # B200MDM_MAX_PROMPTS
 MAX_MEMORY_TOKENS = 512                     # a BERT text memory holds 1 .. 512 tokens (DistilBERT's position limit)
@@ -135,6 +135,9 @@ def load():
                        ("b200mdm_chain_loop_range", [vp, i32, i32, i32, i32, vp, i64, vp, i64, vp, i32, i32, vp]),
                        ("b200mdm_set_joint_guidance", [vp, vp, vp, vp, vp, f32, i32, vp]),
                        ("b200mdm_test_joint_guidance", [vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, vp, vp, vp]),
+                       ("b200mdm_set_foot_guidance", [vp, f32, f32, f32, vp, vp, vp]),
+                       ("b200mdm_test_foot_guidance", [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, f32, f32, f32,
+                                                       vp, vp, vp]),
                        ("b200mdm_set_cond_multi", [vp, i32, i32, i32, vp, vp, vp, vp]),
                        ("b200mdm_set_cond_multi_dec", [vp, i32, i32, i32, vp, vp, vp]),
                        ("b200mdm_set_cond_multi_tokens", [vp, i32, i32, i32, vp, vp, i32, vp, vp]),

@@ -148,10 +148,11 @@ struct GraphKey {
   const void* hs = nullptr;         // the workspace's handshake descriptor, or nullptr when the loop has none
   bool guided = false;              // joint-position control: the step ends in joint_guidance_step_kernel
   int groups = 0;                   // multi-prompt guidance: the step ends in compose_step_kernel over G groups
+  bool foot = false;                // ... with the foot-contact and floor terms: joint_guidance_step_kernel<true>
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
            imask == o.imask && iweight == o.iweight && imotion == o.imotion && target_g == o.target_g && hs == o.hs &&
-           guided == o.guided && groups == o.groups;
+           guided == o.guided && groups == o.groups && foot == o.foot;
   }
 };
 
@@ -265,9 +266,17 @@ struct b200mdm_engine : Workspace {
   const float* inpaint_motion = nullptr;
   // joint-position control: its device descriptor (read by the step graph at every replay, allocated on first use) and
   // the host staging of the last upload; jg_set is cleared by every b200mdm_set_cond* call
-  JointGuide* jg_desc = nullptr;
+  GuideDesc* jg_desc = nullptr;
   JointGuide h_jg{};
   bool jg_set = false;
+  // its foot-contact and floor terms (b200mdm_set_foot_guidance): the descriptor's FootGuide, the lengths it points to
+  // (fg_len [fg_len_cap] int32 device, allocated on first use) and their host staging; fg_set is cleared by every
+  // b200mdm_set_cond* and b200mdm_set_joint_guidance call
+  FootGuide h_fg{};
+  int* fg_len = nullptr;
+  int fg_len_cap = 0;
+  std::vector<int> h_fg_len;
+  bool fg_set = false;
   // multi-prompt guidance: the prompt-weight descriptor (read by the step graph at every replay, allocated on first
   // use) and its host staging; pw_set is cleared by every b200mdm_set_cond* call
   PromptWeight* pw_desc = nullptr;
@@ -351,8 +360,11 @@ static int init_kernel_attrs() {
   TRY((set_attention_attr<256>()));
   CUDA_TRY(cudaFuncSetAttribute(cross_attention_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XAL_SMEM));
   const int jg_smem = static_cast<int>(jg_smem_bytes(JG_MAX_FRAMES, JG_MAX_FEATS));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
+  const int fg_smem = static_cast<int>(fg_smem_bytes(JG_MAX_FRAMES, JG_MAX_FEATS));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
   if (dev < 64) done_mask |= 1ull << dev;
   return B200MDM_OK;
 }
@@ -698,6 +710,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
   dfree(e->jg_desc);
+  dfree(e->fg_len);
   dfree(e->pw_desc);
   if (e->work) cudaStreamDestroy(e->work);
   if (e->ev_in) cudaEventDestroy(e->ev_in);
@@ -1244,6 +1257,7 @@ static void end_cond(b200mdm_engine* e) {
   e->inpaint_motion = nullptr;
   e->hs_set = false;
   e->jg_set = false;
+  e->fg_set = false;
   e->pw_set = false;
   e->vb_live = false;
   e->chain_next = -1;
@@ -1469,8 +1483,49 @@ extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_d
   if (!e->jg_desc) TRY(dalloc(&e->jg_desc, 1));
   if (!e->jg_x0) TRY(dalloc(&e->jg_x0, static_cast<size_t>(e->B) * e->JF * e->T));
   e->h_jg = JointGuide{mean_dev, std_dev, target_dev, weight_dev, step, iters};
-  CUDA_TRY(cudaMemcpyAsync(e->jg_desc, &e->h_jg, sizeof(JointGuide), cudaMemcpyHostToDevice, static_cast<cudaStream_t>(stream)));
+  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->j, &e->h_jg, sizeof(JointGuide), cudaMemcpyHostToDevice,
+                           static_cast<cudaStream_t>(stream)));
   e->jg_set = true;
+  e->fg_set = false;
+  return B200MDM_OK;
+}
+
+// the argument checks b200mdm_set_foot_guidance and b200mdm_test_foot_guidance share
+static int check_foot(float contact_weight, float floor_weight, float floor_height, const int64_t* lengths_host, int B) {
+  if (!std::isfinite(contact_weight) || contact_weight < 0.f || !std::isfinite(floor_weight) || floor_weight < 0.f)
+    return fail(B200MDM_EINVAL, "foot guidance weights %g, %g: finite values >= 0", contact_weight, floor_weight);
+  if (!std::isfinite(floor_height)) return fail(B200MDM_EINVAL, "floor height %g: a finite value", floor_height);
+  for (int b = 0; lengths_host && b < B; ++b)
+    if (lengths_host[b] < 0) return fail(B200MDM_EINVAL, "lengths[%d] = %lld < 0", b, static_cast<long long>(lengths_host[b]));
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_foot_guidance(b200mdm_engine* e, float contact_weight, float floor_weight, float floor_height,
+                                         const float* contact_dev, const int64_t* lengths_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  TRY(check_foot(contact_weight, floor_weight, floor_height, lengths_host, e->B));
+  if (!e->jg_set) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (foot guidance extends it)");
+  e->fg_set = false;
+  if (contact_weight == 0.f && floor_weight == 0.f) return B200MDM_OK;   // off: plain joint-position control
+  const int* len = nullptr;
+  if (lengths_host) {
+    if (e->fg_len_cap < e->B) {
+      dfree(e->fg_len);
+      e->fg_len_cap = 0;
+      TRY(dalloc(&e->fg_len, static_cast<size_t>(e->B)));
+      e->fg_len_cap = e->B;
+    }
+    // the host staging lives in the engine until the next call: no stream synchronisation
+    e->h_fg_len.resize(e->B);
+    for (int b = 0; b < e->B; ++b) e->h_fg_len[b] = static_cast<int>(std::min<int64_t>(lengths_host[b], e->T));
+    CUDA_TRY(cudaMemcpyAsync(e->fg_len, e->h_fg_len.data(), e->B * sizeof(int), cudaMemcpyHostToDevice,
+                             static_cast<cudaStream_t>(stream)));
+    len = e->fg_len;
+  }
+  e->h_fg = FootGuide{contact_dev, len, contact_weight, floor_weight, floor_height};
+  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->f, &e->h_fg, sizeof(FootGuide), cudaMemcpyHostToDevice,
+                           static_cast<cudaStream_t>(stream)));
+  e->fg_set = true;
   return B200MDM_OK;
 }
 
@@ -1881,8 +1936,12 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
       TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, ax, px, s, e->num_sms));
       set_step_params(&p, a, B, T, JF);
       const int R = 4 + 3 * ((JF == 263 ? 22 : 21) - 1);
-      CUDA_TRY(launch_k(joint_guidance_step_kernel, dim3(B), dim3(JG_THREADS), jg_smem_bytes(T, R), s,
-                        static_cast<const JointGuide*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
+      if (e->fg_set)
+        CUDA_TRY(launch_k(joint_guidance_step_kernel<true>, dim3(B), dim3(JG_THREADS), fg_smem_bytes(T, R), s,
+                          static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
+      else
+        CUDA_TRY(launch_k(joint_guidance_step_kernel<false>, dim3(B), dim3(JG_THREADS), jg_smem_bytes(T, R), s,
+                          static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
       nk += 2;
     } else {
       TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, a, p, s, e->num_sms));
@@ -2088,6 +2147,7 @@ static int loop_enter(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32
     key.target_g = e->target_set ? e->tgt_g : nullptr;
     key.hs = e->hs_set ? e->hs_desc : nullptr;
     key.guided = e->jg_set;
+    key.foot = e->jg_set && e->fg_set;
     key.groups = e->groups;
     TRY(ensure_step_graph(e, key, a));
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
@@ -2957,9 +3017,41 @@ extern "C" int b200mdm_test_joint_guidance(const float* x0_dev, const float* mea
   TRY(init_kernel_attrs());
   const JointGuide g{mean_dev, std_dev, target_dev, weight_dev, step, iters};
   const int R = D == 263 ? 67 : 64;
-  joint_guidance_test_kernel<<<B, JG_THREADS, jg_smem_bytes(T, R), static_cast<cudaStream_t>(stream)>>>(
-      g, x0_dev, x0_out_dev, loss_out_dev, B, T, D);
+  joint_guidance_test_kernel<false><<<B, JG_THREADS, jg_smem_bytes(T, R), static_cast<cudaStream_t>(stream)>>>(
+      g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, FootGuide{});
   CUDA_TRY(cudaGetLastError());
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_test_foot_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev,
+                                          const float* target_dev, const float* weight_dev, const float* contact_dev,
+                                          const int64_t* lengths_host, int32_t B, int32_t T, int32_t D, float step,
+                                          int32_t iters, float contact_weight, float floor_weight, float floor_height,
+                                          float* x0_out_dev, float* loss_out_dev, void* stream) {
+  if (!x0_dev || !mean_dev || !std_dev || !target_dev || !weight_dev || !x0_out_dev) return fail(B200MDM_EINVAL, "null argument");
+  if (!std::isfinite(step) || step <= 0.f) return fail(B200MDM_EINVAL, "guidance step %g: a finite value > 0", step);
+  if (iters < 1 || iters > 10000) return fail(B200MDM_EINVAL, "guidance iterations %d outside 1 .. 10000", iters);
+  if (D != 263 && D != 251) return fail(B200MDM_EINVAL, "D %d: 263 (HumanML3D) or 251 (KIT)", D);
+  if (B < 1 || T < 1 || T > JG_MAX_FRAMES) return fail(B200MDM_EINVAL, "B %d, T %d: B >= 1, 1 <= T <= %d", B, T, JG_MAX_FRAMES);
+  TRY(check_foot(contact_weight, floor_weight, floor_height, lengths_host, B));
+  TRY(init_kernel_attrs());
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int* len = nullptr;
+  std::vector<int> h_len;
+  if (lengths_host) {
+    h_len.resize(B);
+    for (int b = 0; b < B; ++b) h_len[b] = static_cast<int>(std::min<int64_t>(lengths_host[b], T));
+    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&len), B * sizeof(int), s));
+    CUDA_TRY(cudaMemcpyAsync(len, h_len.data(), B * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
+  const JointGuide g{mean_dev, std_dev, target_dev, weight_dev, step, iters};
+  const FootGuide f{contact_dev, len, contact_weight, floor_weight, floor_height};
+  const int R = D == 263 ? 67 : 64;
+  joint_guidance_test_kernel<true><<<B, JG_THREADS, fg_smem_bytes(T, R), s>>>(g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, f);
+  const cudaError_t err = cudaGetLastError();
+  if (len) cudaFreeAsync(len, s);
+  if (err != cudaSuccess) return fail(B200MDM_ECUDA, "%s", cudaGetErrorString(err));
+  CUDA_TRY(cudaStreamSynchronize(s));   // h_len is local
   return B200MDM_OK;
 }
 

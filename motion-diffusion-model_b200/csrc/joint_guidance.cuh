@@ -12,6 +12,10 @@
 // Per-frame arithmetic is fp32; the four scans and the loss accumulate in fp64 across the block (warp shuffles, then the
 // warp totals), so their error does not grow with T.  Features a thread's frame alone reads (height, joints) are updated
 // as soon as their gradient is known; the yaw and root velocities, which other frames read, after the last scan.
+// FOOT (DESIGN.md, "Foot contact and floor"): G gains 1/2 lc sum_{k,t} kappa_k[t] |Delta_k[t]|^2 over the four foot joints,
+// Delta_k[t] = p[t+1, f_k] - p[t, f_k] formed from the root velocity w[t+1] and the rotated root-relative feet (never from
+// world positions), and 1/2 lf sum_{t<L, j} min(p[t,j].y - h, 0)^2; both only add to e, the existing chain is unchanged.
+// The neighbour frame's w and feet, and kappa * Delta of the previous pair, go through shared memory.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -37,10 +41,35 @@ struct JointGuide {
   int iters;
 };
 
+// The foot-contact and floor terms (b200mdm_set_foot_guidance): contact [B, 4, T] fp32 (nullptr: kappa derived from x0's
+// contact features), lengths [B] (nullptr: every frame), the weights lc / lf and the floor height.
+struct FootGuide {
+  const float* contact;
+  const int* lengths;
+  float contact_w, floor_w, floor_h;
+};
+
+// The engine's device descriptor: the foot terms follow the joint terms, so a FOOT = false kernel reads what it always read
+struct GuideDesc {
+  JointGuide j;
+  FootGuide f;
+};
+
 // Shared memory of the guidance: xs [R, T] floats, mean / std of the R features, the velocity adjoints handed one frame
 // back [2, T], and the scans' warp totals.
 __host__ __device__ constexpr size_t jg_smem_bytes(int T, int R) {
   return static_cast<size_t>(JG_WARPS) * 3 * sizeof(double) + (static_cast<size_t>(R) * T + 2 * R + 2 * T) * sizeof(float);
+}
+// ... and with the foot terms: each frame's w and four rotated feet [14, FG_LD] and kappa * Delta of its pair [12, FG_LD]
+// (a fixed row pitch, so every access is the thread's base address plus an immediate)
+constexpr int FG_NB = 14, FG_CD = 12, FG_LD = JG_MAX_FRAMES;
+__host__ __device__ constexpr size_t fg_smem_bytes(int T, int R) {
+  return jg_smem_bytes(T, R) + static_cast<size_t>(FG_NB + FG_CD) * FG_LD * sizeof(float);
+}
+
+// The foot joints of contact channels D - 4 .. D - 1 (the reference's cat([..., feet_l, feet_r]) with fid_l, fid_r)
+__host__ __device__ constexpr int foot_joint(int J, int k) {
+  return J == 22 ? (k == 0 ? 7 : k == 1 ? 10 : k == 2 ? 8 : 11) : (k == 0 ? 19 : k == 1 ? 20 : k == 2 ? 14 : 15);
 }
 
 // Inclusive scan over the block's threads (REV: from the last thread down) of N fp64 values per thread.  Every thread of
@@ -80,11 +109,130 @@ __device__ __forceinline__ void jg_descend(float* x0, float step_sd, float g) {
   if (g != 0.f) *x0 = __fsub_rn(*x0, __fmul_rn(step_sd, g));
 }
 
+// The foot terms' per-frame constants: kappa_k[t] of this thread's pair (t, t + 1), whether the floor acts on its frame,
+// and the shared-memory exchange buffers nb [FG_NB, T] and cd [FG_CD, T] (unused when !FOOT)
+struct FootFrame {
+  float kap[4];
+  bool floor;
+  float* nb;
+  float* cd;
+};
+
+// One iteration's joint pass with the foot terms, for thread t's frame (every thread of the block calls it): the
+// neighbour exchange, kappa * Delta of pair (t, t + 1) and its loss, then per joint e = w (p - c) + the floor's and the
+// contact pairs' adjoints, into the position / yaw adjoints and the descent on height and joints, as joint_guidance_iterate.
+__device__ __forceinline__ void foot_iterate(float* xs, const float* mu, const float* sd, const JointGuide& g, const FootGuide& fg,
+                                             const FootFrame& ff, const float* tg, const float* wt, int T, int J, bool upd,
+                                             float c, float s, float wx, float wz, float px, float pz, float* gpx, float* gpz,
+                                             float* gyaw, double* lsum) {
+  const int t = threadIdx.x;
+  const bool act = t < T;
+  auto X = [&](int f) { return __fadd_rn(__fmul_rn(xs[f * T + t], sd[f]), mu[f]); };
+  float* nb = ff.nb + t;   // row r of frame t + o: nb[r * FG_LD + o]
+  float* cd = ff.cd + t;
+  // this frame's root velocity and rotated feet, for frame t - 1
+  float rfx[4], qfy[4], rfz[4];
+  if (act) {
+    nb[0] = wx;
+    nb[FG_LD] = wz;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int f = 4 + 3 * (foot_joint(J, k) - 1);
+      ric_rot(c, s, X(f), X(f + 2), &rfx[k], &rfz[k]);
+      qfy[k] = X(f + 1);
+      nb[(2 + 3 * k) * FG_LD] = rfx[k];
+      nb[(3 + 3 * k) * FG_LD] = qfy[k];
+      nb[(4 + 3 * k) * FG_LD] = rfz[k];
+    }
+  }
+  __syncthreads();
+  // Delta_k[t] = w[t+1] + rot(yaw[t+1]) q_f[t+1] - rot(yaw[t]) q_f[t] in x / z, q_f[t+1].y - q_f[t].y in y
+  if (act) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      float dx = 0.f, dy = 0.f, dz = 0.f;
+      if (ff.kap[k] != 0.f) {   // kappa is 0 on the last frame
+        dx = __fsub_rn(__fadd_rn(nb[1], nb[(2 + 3 * k) * FG_LD + 1]), rfx[k]);
+        dy = __fsub_rn(nb[(3 + 3 * k) * FG_LD + 1], qfy[k]);
+        dz = __fsub_rn(__fadd_rn(nb[FG_LD + 1], nb[(4 + 3 * k) * FG_LD + 1]), rfz[k]);
+        *lsum += 0.5 * static_cast<double>(fg.contact_w) * ff.kap[k] *
+                 (static_cast<double>(dx) * dx + static_cast<double>(dy) * dy + static_cast<double>(dz) * dz);
+        dx = __fmul_rn(ff.kap[k], dx);
+        dy = __fmul_rn(ff.kap[k], dy);
+        dz = __fmul_rn(ff.kap[k], dz);
+      }
+      cd[3 * k * FG_LD] = dx;
+      cd[(3 * k + 1) * FG_LD] = dy;
+      cd[(3 * k + 2) * FG_LD] = dz;
+    }
+  }
+  __syncthreads();
+  if (!act) return;
+  // the contact adjoint at (t, f_k): lc (kappa[t-1] Delta[t-1] - kappa[t] Delta[t])
+  auto ce = [&](int k, int a) {
+    const float prev = t > 0 ? cd[(3 * k + a) * FG_LD - 1] : 0.f;
+    return __fmul_rn(fg.contact_w, __fsub_rn(prev, cd[(3 * k + a) * FG_LD]));
+  };
+#pragma unroll 1
+  for (int j = 0; j < J; ++j) {
+    const float w = __ldcg(wt + static_cast<size_t>(j) * T);
+    const int f = j == 0 ? 3 : 4 + 3 * (j - 1);
+    float rx = 0.f, rz = 0.f, qx = 0.f, qy, qz = 0.f;
+    if (j == 0) {
+      qy = X(3);
+    } else {
+      qx = X(f); qy = X(f + 1); qz = X(f + 2);
+      ric_rot(c, s, qx, qz, &rx, &rz);
+    }
+    float ex = 0.f, ey = 0.f, ez = 0.f;
+    if (w != 0.f) {   // a free joint: its target is never read
+      const float* cj = tg + static_cast<size_t>(j) * 3 * T;
+      const float dx = __fsub_rn(__fadd_rn(rx, px), __ldcg(cj));
+      const float dy = __fsub_rn(qy, __ldcg(cj + T));
+      const float dz = __fsub_rn(__fadd_rn(rz, pz), __ldcg(cj + 2 * T));
+      *lsum += 0.5 * static_cast<double>(w) * (static_cast<double>(dx) * dx + static_cast<double>(dy) * dy +
+                                               static_cast<double>(dz) * dz);
+      ex = __fmul_rn(w, dx); ey = __fmul_rn(w, dy); ez = __fmul_rn(w, dz);
+    }
+    if (ff.floor) {   // the floor: lf min(p.y - h, 0)
+      const float m = fminf(__fsub_rn(qy, fg.floor_h), 0.f);
+      if (m < 0.f) {
+        *lsum += 0.5 * static_cast<double>(fg.floor_w) * (static_cast<double>(m) * m);
+        ey = __fadd_rn(ey, __fmul_rn(fg.floor_w, m));
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (j == foot_joint(J, k)) {
+        ex = __fadd_rn(ex, ce(k, 0));
+        ey = __fadd_rn(ey, ce(k, 1));
+        ez = __fadd_rn(ez, ce(k, 2));
+      }
+    }
+    if (ex == 0.f && ey == 0.f && ez == 0.f) continue;
+    *gpx = __fadd_rn(*gpx, ex);
+    *gpz = __fadd_rn(*gpz, ez);
+    if (j == 0) {
+      if (upd) jg_descend(&xs[3 * T + t], __fmul_rn(g.step, sd[3]), ey);
+      continue;
+    }
+    *gyaw = __fadd_rn(*gyaw, __fmul_rn(2.f, __fsub_rn(__fmul_rn(ez, rx), __fmul_rn(ex, rz))));
+    if (upd) {
+      float gx, gz;
+      ric_rot(c, -s, ex, ez, &gx, &gz);   // rot(yaw)^T = rot(-yaw)
+      jg_descend(&xs[f * T + t], __fmul_rn(g.step, sd[f]), gx);
+      jg_descend(&xs[(f + 1) * T + t], __fmul_rn(g.step, sd[f + 1]), ey);
+      jg_descend(&xs[(f + 2) * T + t], __fmul_rn(g.step, sd[f + 2]), gz);
+    }
+  }
+}
+
 // The K guidance iterations of motion b on xs (its R ric features, normalised, [R, T] in shared memory; mu / sd the
 // features' mean and std).  loss (nullable) [K + 1, B] receives G before each iteration and after the last one.
 // Every thread of the block calls it.
+template <bool FOOT>
 __device__ void joint_guidance_iterate(float* xs, const float* mu, const float* sd, float* gv, double* sh, const JointGuide& g,
-                                       int b, int B, int T, int J, float* loss) {
+                                       int b, int B, int T, int J, float* loss, const FootGuide& fg, const FootFrame& ff) {
   const int t = threadIdx.x;
   const bool act = t < T;
   const float* tg = g.target + static_cast<size_t>(b) * J * 3 * T + t;
@@ -107,7 +255,9 @@ __device__ void joint_guidance_iterate(float* xs, const float* mu, const float* 
     // joints: residuals, loss, the position / yaw adjoints of this frame, and the descent on height and joints
     float gpx = 0.f, gpz = 0.f, gyaw = 0.f;
     double lsum = 0.0;
-    if (act) {
+    if constexpr (FOOT) {
+      foot_iterate(xs, mu, sd, g, fg, ff, tg, wt, T, J, upd, c, s, wx, wz, px, pz, &gpx, &gpz, &gyaw, &lsum);
+    } else if (act) {
       for (int j = 0; j < J; ++j) {
         const float w = __ldcg(wt + static_cast<size_t>(j) * T);
         if (w == 0.f) continue;   // a free joint: its target is never read
@@ -172,7 +322,9 @@ __device__ void joint_guidance_iterate(float* xs, const float* mu, const float* 
 
 // The guidance of one motion around joint_guidance_iterate: shared memory carved, ric features of x0 [B, D, T] loaded
 // (through L2: x0 was written by the kernel before).  Returns the shared-memory view of the guided features.
-__device__ __forceinline__ float* joint_guidance_run(const JointGuide& g, const float* x0, int B, int T, int D, float* loss) {
+template <bool FOOT>
+__device__ __forceinline__ float* joint_guidance_run(const JointGuide& g, const FootGuide& fg, const float* x0, int B, int T,
+                                                     int D, float* loss) {
   extern __shared__ double jg_smem[];
   const int J = D == 263 ? 22 : 21, R = 4 + 3 * (J - 1), b = blockIdx.x;
   double* sh = jg_smem;
@@ -186,8 +338,30 @@ __device__ __forceinline__ float* joint_guidance_run(const JointGuide& g, const 
     mu[i] = __ldcg(g.mean + i);
     sd[i] = __ldcg(g.std + i);
   }
+  FootFrame ff{};
+  if constexpr (FOOT) {
+    // kappa of pair (t, t + 1), read once: the guidance never changes the contact features
+    const int t = threadIdx.x;
+    const int L = fg.lengths != nullptr ? min(max(__ldcg(fg.lengths + b), 0), T) : T;
+    for (int k = 0; k < 4; ++k) {
+      float kap = 0.f;
+      if (t + 1 < T) {
+        if (fg.contact != nullptr) {
+          kap = __ldcg(fg.contact + (static_cast<size_t>(b) * 4 + k) * T + t);
+        } else if (t + 1 < L) {
+          const int f = D - 4 + k;
+          kap = __fadd_rn(__fmul_rn(__ldcg(xb + static_cast<size_t>(f) * T + t), __ldcg(g.std + f)), __ldcg(g.mean + f)) > 0.5f
+                    ? 1.f : 0.f;
+        }
+      }
+      ff.kap[k] = kap;
+    }
+    ff.floor = fg.floor_w > 0.f && t < L;
+    ff.nb = gv + 2 * T;
+    ff.cd = ff.nb + FG_NB * FG_LD;
+  }
   __syncthreads();
-  joint_guidance_iterate(xs, mu, sd, gv, sh, g, b, B, T, J, loss);
+  joint_guidance_iterate<FOOT>(xs, mu, sd, gv, sh, g, b, B, T, J, loss, fg, ff);
   return xs;
 }
 
@@ -203,19 +377,32 @@ __device__ __forceinline__ JointGuide load_joint_guide(const JointGuide* d) {
   g.iters = __ldcg(&d->iters);
   return g;
 }
+__device__ __forceinline__ FootGuide load_foot_guide(const FootGuide* d) {
+  FootGuide f;
+  f.contact = reinterpret_cast<const float*>(__ldcg(reinterpret_cast<const unsigned long long*>(&d->contact)));
+  f.lengths = reinterpret_cast<const int*>(__ldcg(reinterpret_cast<const unsigned long long*>(&d->lengths)));
+  f.contact_w = __ldcg(&d->contact_w);
+  f.floor_w = __ldcg(&d->floor_w);
+  f.floor_h = __ldcg(&d->floor_h);
+  return f;
+}
 
 // The guided step of motion blockIdx.x: x0 (the output projection + bias after the CFG blend, [B, D, T], written by the
 // MODE_X0 output GEMM) -> guidance -> the output step's tail (inpainting, clamp, the DDPM / DDIM update of p.mode) for
 // every element of the motion, reading the step's noise as OutStep does.  grid = B, block = JG_THREADS,
-// dynamic shared memory jg_smem_bytes(T, R).
-__global__ void __launch_bounds__(JG_THREADS) joint_guidance_step_kernel(const JointGuide* guide, const float* x0,
+// dynamic shared memory jg_smem_bytes(T, R) (FOOT: fg_smem_bytes(T, R)).  FOOT asks for one CTA per SM (the B CTAs
+// never share one at B <= 132), which lifts the register cap ptxas otherwise picks and keeps the step free of spills.
+template <bool FOOT>
+__global__ void __launch_bounds__(JG_THREADS, FOOT ? 1 : 0) joint_guidance_step_kernel(const GuideDesc* guide, const float* x0,
                                                                          const EpiOutParams p) {
   pdl_launch_dependents();
   pdl_wait();
   const int T = p.T, D = p.J, b = blockIdx.x, t = threadIdx.x;
-  const JointGuide g = load_joint_guide(guide);
+  const JointGuide g = load_joint_guide(&guide->j);
+  FootGuide fg{};
+  if constexpr (FOOT) fg = load_foot_guide(&guide->f);
   const int R = D == 263 ? 67 : 64;
-  const float* xs = joint_guidance_run(g, x0, p.B, T, D, nullptr);
+  const float* xs = joint_guidance_run<FOOT>(g, fg, x0, p.B, T, D, nullptr);
   if (t >= T) return;
   const OutStep u(p, b);
   const size_t base = static_cast<size_t>(b) * D * T + t;
@@ -226,11 +413,13 @@ __global__ void __launch_bounds__(JG_THREADS) joint_guidance_step_kernel(const J
   }
 }
 
-// b200mdm_test_joint_guidance: the guidance alone, x0_out [B, D, T] = guided x0 (features past the ric features copied).
+// b200mdm_test_joint_guidance / b200mdm_test_foot_guidance (FOOT): the guidance alone, x0_out [B, D, T] = guided x0
+// (features past the ric features copied).  fg comes last, so the FOOT = false kernel's parameters keep their offsets.
+template <bool FOOT>
 __global__ void __launch_bounds__(JG_THREADS) joint_guidance_test_kernel(const JointGuide g, const float* x0, float* x0_out,
-                                                                         float* loss, int B, int T, int D) {
+                                                                         float* loss, int B, int T, int D, const FootGuide fg) {
   const int R = D == 263 ? 67 : 64, b = blockIdx.x;
-  const float* xs = joint_guidance_run(g, x0, B, T, D, loss);
+  const float* xs = joint_guidance_run<FOOT>(g, fg, x0, B, T, D, loss);
   const size_t base = static_cast<size_t>(b) * D * T;
   for (int i = threadIdx.x; i < D * T; i += blockDim.x) x0_out[base + i] = i < R * T ? xs[i] : x0[base + i];
 }

@@ -254,6 +254,7 @@ class GaussianDiffusion:
         soft = self._soft_inpainting(y, shape)
         r = resolve(model)
         joint = r.wrapper.targets(y, shape) if r.kind == "joint" else None
+        contact = r.wrapper.foot_contact(y, shape) if r.kind == "joint" else None
         if r.kind == "multi":
             r.wrapper.prompts(y, shape)              # y's prompts checked before any engine work
         eng, guided = engine_for(model)
@@ -272,6 +273,9 @@ class GaussianDiffusion:
             jc = r.wrapper
             eng.set_joint_guidance(jc.mean.to(device), jc.std.to(device), joint[0].to(device), joint[1].to(device),
                                    jc.step_size, jc.n_iters)
+            if jc.foot:
+                eng.set_foot_guidance(jc.contact_weight, jc.floor_weight, jc.floor_height,
+                                      None if contact is None else contact.to(device), y.get("lengths"))
         if table == "next":
             eng.set_schedule_next(self.schedule_next_rows(), key=(id(self), self.num_timesteps))
         elif table == "dpm":

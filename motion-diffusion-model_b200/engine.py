@@ -64,6 +64,34 @@ def joint_guidance_hook(x0, mean, std, target, weight, step, iters):
     return out, loss
 
 
+def _lengths_host(lengths, B):
+    """y['lengths'] (tensor, array or None) -> contiguous int64 numpy [B], or None"""
+    if lengths is None:
+        return None
+    n = np.ascontiguousarray(np.asarray(lengths.detach().cpu() if torch.is_tensor(lengths) else lengths, dtype=np.int64).reshape(-1))
+    assert n.shape == (B,), n.shape
+    return n
+
+
+def foot_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weight, floor_weight, floor_height=0.0,
+                       contact=None, lengths=None):
+    """The guidance iterations with the foot-contact and floor terms alone (b200mdm_test_foot_guidance), on x0's device:
+    (guided x0 [B, D, T], total G [iters + 1, B]).  contact [B, 4, T] or None (derived from x0), lengths [B] or None."""
+    lib = _lib.load()
+    x0, mean, std, target, weight = (t.to(torch.float32).contiguous() for t in (x0, mean, std, target, weight))
+    B, D, T = int(x0.shape[0]), int(x0.shape[1]), int(x0.shape[-1])
+    kappa = None if contact is None else contact.to(device=x0.device, dtype=torch.float32).contiguous()
+    n = _lengths_host(lengths, B)
+    out = torch.empty_like(x0)
+    loss = torch.empty((int(iters) + 1, B), device=x0.device, dtype=torch.float32)
+    check(lib.b200mdm_test_foot_guidance(_ptr(x0), _ptr(mean), _ptr(std), _ptr(target), _ptr(weight),
+                                         None if kappa is None else _ptr(kappa),
+                                         None if n is None else n.ctypes.data_as(ctypes.c_void_p), B, T, D, float(step),
+                                         int(iters), float(contact_weight), float(floor_weight), float(floor_height),
+                                         _ptr(out), _ptr(loss), _stream()))
+    return out, loss
+
+
 class Engine:
     """One engine per model instance (weights + workspace live on the current CUDA device)."""
 
@@ -360,6 +388,18 @@ class Engine:
         ts = [t.to(torch.float32).contiguous() for t in (mean, std, target, weight)]
         check(self.lib.b200mdm_set_joint_guidance(self.h, *[_ptr(t) for t in ts], float(step), int(iters), _stream()))
         self._keep["joint"] = ts
+        self._keep.pop("foot", None)
+
+    def set_foot_guidance(self, contact_weight, floor_weight, floor_height=0.0, contact=None, lengths=None):
+        """The foot-contact and floor terms of the joint guidance set last (b200mdm_set_foot_guidance), which
+        set_joint_guidance and set_cond clear: contact [B, 4, T] on the engine's device or None (derived from each step's
+        x0), lengths [B] or None (every frame)."""
+        kappa = None if contact is None else contact.to(torch.float32).contiguous()
+        n = _lengths_host(lengths, self.batch)
+        check(self.lib.b200mdm_set_foot_guidance(self.h, float(contact_weight), float(floor_weight), float(floor_height),
+                                                 None if kappa is None else _ptr(kappa),
+                                                 None if n is None else n.ctypes.data_as(ctypes.c_void_p), _stream()))
+        self._keep["foot"] = kappa
 
     def set_cond_multi(self, batch, nframes, y, embed, action, weight, device):
         """Multi-prompt guidance (b200mdm_set_cond_multi / _dec / _tokens, then b200mdm_set_prompt_weight): embed fp32

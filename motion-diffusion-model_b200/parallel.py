@@ -65,7 +65,7 @@ def gather_objects(obj, group=None):
 
 _BATCH_KEYS = ("mask", "lengths", "scale", "action", "inpainting_mask", "inpainted_motion", "prefix", "target_cond",
                "is_heading", "motion_start", "inpainting_weight", "joint_target", "joint_weight", "prompt_action",
-               "prompt_weight")
+               "prompt_weight", "foot_contact")
 
 
 def shard_model_kwargs(model_kwargs, lo, hi):

@@ -160,10 +160,17 @@ class JointControlSampleModel(_SampleWrapper):
     ddim_sample honour it, for every model the engine runs (the BERT decoder with context_len 0 included); the other
     samplers, prefix-completion (DiP, context_len > 0) models and AutoRegressiveSampler raise
     NotImplementedError, HandshakeSampleModel and refine_transitions TypeError.  Calling the wrapper is the plain model:
-    the guidance belongs to the sampler, as inpainting does."""
+    the guidance belongs to the sampler, as inpainting does.
+
+    Foot contact and floor (DESIGN.md "Joint-position control", "Foot contact and floor"): `contact_weight` adds
+    1/2 contact_weight sum_{k,t} kappa[b,k,t] |p[t+1, f_k] - p[t, f_k]|^2 over the four foot joints f_k of the contact
+    features (HumanML3D 7, 10, 8, 11; KIT 19, 20, 14, 15), kappa = y['foot_contact'] [B, 4, T] (float >= 0 or bool) or,
+    without it, 1 where the step's own de-normalised x0 has contact feature k > 0.5 at frame t and t + 1 < lengths[b];
+    `floor_weight` adds 1/2 floor_weight sum_{t < lengths[b], j} min(p[t,j].y - floor_height, 0)^2.  With either weight
+    > 0, y['joint_target'] / y['joint_weight'] are optional (absent: no joint term)."""
     kind = "joint"
 
-    def __init__(self, model, mean, std, step_size, n_iters):
+    def __init__(self, model, mean, std, step_size, n_iters, *, contact_weight=0.0, floor_weight=0.0, floor_height=0.0):
         core = _core(model)
         if core is None:
             raise TypeError("JointControlSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(model))
@@ -183,16 +190,29 @@ class JointControlSampleModel(_SampleWrapper):
                      for v in (mean, std))
         if mean.shape != (D,) or std.shape != (D,):
             raise ValueError("mean and std need %d entries (got %s and %s)" % (D, tuple(mean.shape), tuple(std.shape)))
+        cw, fw, fh = float(contact_weight), float(floor_weight), float(floor_height)
+        if not (np.isfinite(cw) and cw >= 0 and np.isfinite(fw) and fw >= 0):
+            raise ValueError("contact_weight and floor_weight must be finite and >= 0 (got %r, %r)" % (contact_weight, floor_weight))
+        if not np.isfinite(fh):
+            raise ValueError("floor_height must be finite (got %r)" % (floor_height,))
         super().__init__(model)
         self.mean, self.std = mean, std
         self.step_size, self.n_iters = step, int(iters)
         self.n_joints = 22 if D == 263 else 21
+        self.contact_weight, self.floor_weight, self.floor_height = cw, fw, fh
+
+    @property
+    def foot(self):
+        """True when the foot-contact or floor term is on"""
+        return self.contact_weight > 0 or self.floor_weight > 0
 
     def targets(self, y, shape):
         """(target [B, J, 3, T], weight [B, J, T]) fp32 of y for a sample of `shape`; y is not modified.  ValueError for a
         missing key, a shape other than these, a weight that is negative or not finite, or a target that is not finite
         where its weight is not 0."""
         B, T, J = int(shape[0]), int(shape[-1]), self.n_joints
+        if self.foot and "joint_target" not in y and "joint_weight" not in y:
+            return torch.zeros(B, J, 3, T), torch.zeros(B, J, T)      # no joint term: a target the kernel never reads
         if "joint_target" not in y or "joint_weight" not in y:
             raise ValueError("JointControlSampleModel needs y['joint_target'] [B, %d, 3, T] and y['joint_weight'] [B, %d, T]"
                              % (J, J))
@@ -211,6 +231,24 @@ class JointControlSampleModel(_SampleWrapper):
         if not bool((torch.isfinite(c) | (w == 0)[:, :, None, :]).all()):
             raise ValueError("y['joint_target'] must be finite where y['joint_weight'] is not 0")
         return c, w
+
+    def foot_contact(self, y, shape):
+        """kappa [B, 4, T] fp32 of y['foot_contact'], or None (absent: derived from each step's x0); y is not modified.
+        ValueError for a shape other than [B, 4, T], a dtype other than float or bool, or a value that is negative or
+        not finite."""
+        if not self.foot or y.get("foot_contact") is None:
+            return None
+        k = y["foot_contact"]
+        B, T = int(shape[0]), int(shape[-1])
+        if not torch.is_tensor(k) or tuple(k.shape) != (B, 4, T):
+            raise ValueError("y['foot_contact'] must be a tensor of shape %s (got %s)"
+                             % ((B, 4, T), tuple(k.shape) if torch.is_tensor(k) else type(k)))
+        if k.dtype != torch.bool and not k.is_floating_point():
+            raise ValueError("y['foot_contact'] must be a float or bool tensor")
+        k = k.to(torch.float32)
+        if not bool((torch.isfinite(k) & (k >= 0)).all()):
+            raise ValueError("y['foot_contact'] must be finite and >= 0")
+        return k
 
     def forward(self, x, timesteps, y=None):
         return self.model(x, timesteps, y)
