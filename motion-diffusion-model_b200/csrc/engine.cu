@@ -7,6 +7,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -1200,7 +1201,7 @@ static int select_workspace(b200mdm_engine* e, int B, int T, int halves, cudaStr
   return r;
 }
 
-// ---- what the three conditioning entry points share
+// ---- the conditioning of one loop (set_conditioning, behind every b200mdm_set_cond*)
 // a sequence of n_tokens tokens fits the positional table and the attention kernels
 static int check_seq_len(const b200mdm_engine* e, int n_tokens) {
   if (n_tokens > e->cfg.pos_embed_max_len) return fail(B200MDM_EINVAL, "sequence longer than the positional table");
@@ -1229,21 +1230,20 @@ static int upload_kvlen_scale(b200mdm_engine* e, int nframes, int seq_extra, boo
   if (scale_dev) CUDA_TRY(cudaMemcpyAsync(e->scale, scale_dev, e->B * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return B200MDM_OK;
 }
-// condproj rows of the packed batch: proj = embed_text(text) [B, d] when the model is text-conditioned and a text is given
-// (model/mdm.py:218), then the conditional / unconditional rows of the model's conditioning mode (condproj_fill_kernel).
-// With multi-prompt guidance, B = K * batch conditional rows (text_dev [K, batch, C], action [K * batch]) come first.
-static int fill_condproj(b200mdm_engine* e, const float* text_dev, bool uncond, cudaStream_t s, int B = 0) {
+// condproj rows of the packed batch: proj = embed_text(text) [rows, d] when the model is text-conditioned and a text is
+// given (model/mdm.py:218), then the conditional / unconditional rows of the model's conditioning mode
+// (condproj_fill_kernel).  The rows = K * batch conditional rows (text_dev [K, batch, C], action [K * batch]) come first.
+static int fill_condproj(b200mdm_engine* e, const float* text_dev, bool uncond, int rows, cudaStream_t s) {
   const int d = e->d;
-  if (B == 0) B = e->B;
   if (e->cfg.cond_mode == B200MDM_COND_TEXT && text_dev) {
-    const size_t warps = static_cast<size_t>(B) * d;
-    small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(text_dev, e->w_txt, e->b_txt, e->proj, B, d,
-                                                                                       e->cfg.cond_dim, e->cfg.cond_dim);
+    const size_t warps = static_cast<size_t>(rows) * d;
+    small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(text_dev, e->w_txt, e->b_txt, e->proj, rows,
+                                                                                       d, e->cfg.cond_dim, e->cfg.cond_dim);
     CUDA_TRY(cudaGetLastError());
     e->launches++;
   }
-  condproj_fill_kernel<<<e->Bp, 128, 0, s>>>(e->condproj, e->proj, e->b_txt, e->act_emb, e->action, B, d, e->Bp, uncond ? 1 : 0,
-                                             e->cfg.cond_mode);
+  condproj_fill_kernel<<<e->Bp, 128, 0, s>>>(e->condproj, e->proj, e->b_txt, e->act_emb, e->action, rows, d, e->Bp,
+                                             uncond ? 1 : 0, e->cfg.cond_mode);
   CUDA_TRY(cudaGetLastError());
   e->launches++;
   return B200MDM_OK;
@@ -1263,40 +1263,7 @@ static void end_cond(b200mdm_engine* e) {
   e->chain_next = -1;
 }
 
-extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* cond_embed_dev,
-                                const int64_t* lengths_host, const float* scale_dev, int32_t force_uncond,
-                                const int64_t* action_host, void* stream) {
-  if (!e) return fail(B200MDM_EINVAL, "null engine");
-  if (e->dec) return fail(B200MDM_EINVAL, "trans_dec engines take their conditioning through b200mdm_set_cond_dec");
-  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
-  if (batch <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
-  TRY(check_seq_len(e, nframes + 1));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int halves = scale_dev ? 2 : 1;
-  if (e->cfg.cond_mode == B200MDM_COND_TEXT && !cond_embed_dev && !(halves == 1 && force_uncond))
-    return fail(B200MDM_EINVAL, "text-conditioned model needs y['text_embed']");
-  if (e->cfg.cond_mode == B200MDM_COND_ACTION && !action_host && !(halves == 1 && force_uncond))
-    return fail(B200MDM_EINVAL, "action-conditioned model needs y['action']");
-  if (halves == 2 && e->cfg.cond_mode == B200MDM_COND_NONE)
-    return fail(B200MDM_EINVAL, "classifier-free guidance needs a conditioned model (sampler_util.py:29)");
-  TRY(select_workspace(e, batch, nframes, halves, s));
-  const int B = batch;
-  TRY(upload_kvlen_scale(e, nframes, 1, nframes > 1, lengths_host, scale_dev, s));
-  if (e->cfg.cond_mode == B200MDM_COND_ACTION && action_host) {
-    std::vector<int>& a = e->h_action;
-    a.assign(B, 0);
-    for (int b = 0; b < B; ++b) {
-      if (action_host[b] < 0 || action_host[b] >= e->cfg.num_actions) return fail(B200MDM_EINVAL, "action index out of range");
-      a[b] = static_cast<int>(action_host[b]);
-    }
-    CUDA_TRY(cudaMemcpyAsync(e->action, a.data(), B * sizeof(int), cudaMemcpyHostToDevice, s));
-  }
-  TRY(fill_condproj(e, cond_embed_dev, halves == 1 && force_uncond, s));
-  end_cond(e);
-  return B200MDM_OK;
-}
-
-// cb_l[b'] = W_o,l (W_v,l mb[b'] + b_v,l) + b_o,l with mb = condproj (+ g): the per-sample part of the cross-attention rows
+// cb_l[b']= W_o,l (W_v,l mb[b'] + b_v,l) + b_o,l with mb = condproj (+ g): the per-sample part of the cross-attention rows
 // of a CLIP-memory decoder, once per loop (kernels.cuh, cross_rows_kernel).
 static int cross_rows_per_sample(b200mdm_engine* e, const float* g, cudaStream_t s) {
   const int d = e->d, Bp = e->Bp;
@@ -1312,27 +1279,6 @@ static int cross_rows_per_sample(b200mdm_engine* e, const float* g, cudaStream_t
     CUDA_TRY(cudaGetLastError());
   }
   e->launches += 1 + 2 * e->L;
-  return B200MDM_OK;
-}
-
-// ---- trans_dec with emb_trans_dec and a CLIP memory: y['text_embed'] [1, B, C] is the one memory token of every sample
-static int set_cond_dec_clip(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* clip_dev,
-                             const uint8_t* text_mask_host, int32_t n_tokens, const int64_t* lengths_host,
-                             const float* scale_dev, int32_t force_uncond, cudaStream_t s) {
-  if (n_tokens != 1) return fail(B200MDM_EINVAL, "a CLIP-memory decoder takes one memory token per sample (n_tokens %d)", n_tokens);
-  if (batch <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
-  if (!clip_dev || !text_mask_host) return fail(B200MDM_EINVAL, "the CLIP decoder needs y['text_embed'] and an all-zero mask");
-  for (int b = 0; b < batch; ++b)
-    if (text_mask_host[b]) return fail(B200MDM_EINVAL, "the CLIP memory has no padding mask (model/mdm.py:262-263)");
-  TRY(check_seq_len(e, nframes + 1));
-  const int halves = scale_dev ? 2 : 1;
-  TRY(select_workspace(e, batch, nframes, halves, s));
-  // key mask: the timestep token, then `lengths` frames (the False column prepended, model/mdm.py:241-247)
-  TRY(upload_kvlen_scale(e, nframes, 1, nframes > 1, lengths_host, scale_dev, s));
-  // text_emb = embed_text(mask_cond(clip)) (model/mdm.py:218): conditional rows W clip + b, unconditional rows b
-  TRY(fill_condproj(e, clip_dev, halves == 1 && force_uncond, s));
-  TRY(cross_rows_per_sample(e, nullptr, s));
-  end_cond(e);
   return B200MDM_OK;
 }
 
@@ -1362,45 +1308,209 @@ static int ensure_text_memory(b200mdm_engine* e, int Mt) {
   return B200MDM_OK;
 }
 
-// ---- trans_dec (DiP) conditioning: BERT token features + padding mask as the cross-attention memory, prefix frames
+// The padding mask [Bp, Mt] of a token memory over the packed batch of B samples, into dst: the K * B prompt rows are
+// mask [K, B, Mt] as it is (group-major, the packed order); each unconditional row pads where every prompt pads for its
+// sample, so it admits every token some prompt admits.  With K = 1 that is the sample's own mask, as in a classifier-free
+// pair, and it does not depend on the prompts' order.  (The unconditional tokens are all equal, so any mask admitting
+// one gives the same output up to rounding.)
+static void pack_text_mask(unsigned char* dst, const uint8_t* mask, int K, int B, int Bp, int Mt) {
+  const int rows = K * B;
+  std::fill(dst, dst + static_cast<size_t>(Bp) * Mt, 1);
+  for (int bp = 0; bp < rows; ++bp)
+    for (int m = 0; m < Mt; ++m) {
+      const unsigned char pad = mask[static_cast<size_t>(bp) * Mt + m] ? 1 : 0;
+      dst[static_cast<size_t>(bp) * Mt + m] = pad;
+      if (Bp > rows) dst[static_cast<size_t>(rows + bp % B) * Mt + m] &= pad;
+    }
+}
+
+// The projected token memory [Bp * Mt, d] of the current workspace into dst, text_emb = embed_text(mask_cond(tokens))
+// per token (model/mdm.py:218): W tokens + b for the K * B prompt rows (tokens [K, Mt, B, C], the reference layout per
+// prompt), b for the unconditional rows, and b for every row with `uncond`.  K + 2 launches on s.
+static int build_text_memory(b200mdm_engine* e, const float* tokens, int K, bool uncond, float* dst, cudaStream_t s) {
+  const int d = e->d, B = e->B, Mt = e->Mt, C = e->cfg.cond_dim, rows = K * B;
+  for (int k = 0; k < K; ++k) {
+    permute_mbc_kernel<<<dim3(Mt, B), 128, 0, s>>>(tokens + static_cast<size_t>(k) * Mt * B * C,
+                                                    e->encperm + static_cast<size_t>(k) * B * Mt * C, Mt, B, C);
+    CUDA_TRY(cudaGetLastError());
+  }
+  const size_t warps = static_cast<size_t>(rows) * Mt * d;
+  small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(e->encperm, e->w_txt, e->b_txt, e->memtok,
+                                                                                     rows * Mt, d, C, C);
+  CUDA_TRY(cudaGetLastError());
+  memproj_group_fill_kernel<<<dim3(Mt, e->Bp), 128, 0, s>>>(dst, e->memtok, e->b_txt, uncond ? 0 : rows, Mt, d);
+  CUDA_TRY(cudaGetLastError());
+  e->launches += K + 2;
+  return B200MDM_OK;
+}
+
+// ---- features that exclude each other or a sampler family.  The engine's twin of _REFUSED in
+// diffusion/gaussian_diffusion.py, with the same sampler rows; the setter rows make handshakes, joint-position control
+// and multi-prompt guidance pairwise exclusive and keep each off prefix-completion (DiP) engines.
+enum Feature : unsigned { F_PREFIX = 1, F_HANDSHAKE = 2, F_JOINT = 4, F_MULTI = 8 };
+enum Family { FAM_REVERSE, FAM_PLMS, FAM_DPM, FAM_VB, FAM_HANDSHAKE, FAM_JOINT, FAM_MULTI };
+static const struct {
+  const char* name;
+  unsigned refuses;
+} REFUSED[] = {
+    {"DDIM inversion", F_HANDSHAKE | F_JOINT},
+    {"PLMS", F_JOINT},
+    {"DPM-Solver++", F_JOINT},
+    {"the variational bound", F_HANDSHAKE | F_JOINT | F_MULTI},
+    {"handshaking", F_PREFIX | F_JOINT | F_MULTI},
+    {"joint-position control", F_PREFIX | F_HANDSHAKE | F_MULTI},
+    {"multi-prompt guidance", F_PREFIX},
+};
+
+// ENOTIMPL when the engine holds a feature (of those in `among`) that `family` refuses
+static int refuse(const b200mdm_engine* e, Family family, unsigned among = ~0u) {
+  static const char* const feature[] = {"prefix-completion (DiP) models", "handshakes", "joint-position control",
+                                        "multi-prompt guidance"};
+  const unsigned live = (is_prefix_engine(e) ? F_PREFIX : 0u) | (e->hs_set ? F_HANDSHAKE : 0u) | (e->jg_set ? F_JOINT : 0u) |
+                        (e->groups ? F_MULTI : 0u);
+  const unsigned hit = REFUSED[family].refuses & among & live;
+  for (int i = 0; i < 4; ++i)
+    if (hit & (1u << i)) return fail(B200MDM_ENOTIMPL, "%s with %s is not implemented", REFUSED[family].name, feature[i]);
+  return B200MDM_OK;
+}
+
+// What a b200mdm_set_cond* call hands to set_conditioning.  For everything the upload writes, the classifier-free batch
+// (halves 1, or 2 with a scale) is the multi-prompt layout with K = 1; the two differ in the workspace's layout only.
+struct CondIn {
+  int batch, nframes;
+  const int64_t* lengths;         // [batch] host, nullable
+  const float* embed;             // text or CLIP rows [K, batch, C], or BERT token features [K, n_tokens, batch, C]
+  int K = 1;
+  bool multi = false;             // multi-prompt groups (G = K + 1), else classifier-free halves
+  const uint8_t* mask = nullptr;  // [K, batch, n_tokens] host, 1 = padding (the CLIP row: [batch], all zero)
+  int n_tokens = 0;
+  const int64_t* action = nullptr;   // [batch, K] host
+  const float* scale = nullptr;      // [batch] device: classifier-free guidance
+  bool force_uncond = false;
+};
+
+// The conditioning of a loop: argument checks (all before any CUDA call), the workspace of the packed batch, its key
+// counts and guidance scales, then the rows of the model family -- condproj rows (encoder; CLIP-memory decoder, with its
+// per-sample cross-attention rows) or the token memory and its mask (BERT-memory decoder).
+static int set_conditioning(b200mdm_engine* e, const CondIn& c, cudaStream_t s) {
+  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
+  if (c.batch <= 0 || c.nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
+  if (c.K < 1 || c.K > MP_MAX_PROMPTS) return fail(B200MDM_EINVAL, "prompt count %d outside 1 .. %d", c.K, MP_MAX_PROMPTS);
+  const bool bert = e->dec && !e->dec_clip;
+  const int halves = c.scale ? 2 : 1, B = c.batch, rows = c.K * B, mode = e->cfg.cond_mode;
+  const bool uncond = halves == 1 && c.force_uncond;
+  if (bert) {
+    if (c.n_tokens <= 0 || c.n_tokens > XAL_MAX_MT)
+      return fail(B200MDM_EINVAL, "n_tokens %d: a text memory holds 1..%d tokens (DistilBERT's position limit)", c.n_tokens,
+                  XAL_MAX_MT);
+    if (!c.embed || !c.mask) return fail(B200MDM_EINVAL, "the BERT decoder needs the token features and their masks");
+  } else if (e->dec_clip) {
+    // y['text_embed'] [1, B, C] is the one memory token of every sample, without a padding mask (model/mdm.py:262-263)
+    if (!c.multi && c.n_tokens != 1)
+      return fail(B200MDM_EINVAL, "a CLIP-memory decoder takes one memory token per sample (n_tokens %d)", c.n_tokens);
+    if (!c.embed || (!c.multi && !c.mask))
+      return fail(B200MDM_EINVAL, "the CLIP decoder needs y['text_embed'] and an all-zero mask");
+    for (int b = 0; !c.multi && b < B; ++b)
+      if (c.mask[b]) return fail(B200MDM_EINVAL, "the CLIP memory has no padding mask (model/mdm.py:262-263)");
+  } else {
+    if (mode == B200MDM_COND_NONE && (c.multi || halves == 2))
+      return fail(B200MDM_EINVAL, "%s needs a conditioned model (sampler_util.py:29)",
+                  c.multi ? "multi-prompt guidance" : "classifier-free guidance");
+    if (mode == B200MDM_COND_TEXT && !c.embed && !uncond)
+      return fail(B200MDM_EINVAL, "text-conditioned model needs the text embeddings");
+    if (mode == B200MDM_COND_ACTION && !c.action && !uncond)
+      return fail(B200MDM_EINVAL, "action-conditioned model needs the actions");
+  }
+  TRY(check_seq_len(e, c.nframes + (bert ? e->ctx : 1)));
+  std::vector<int>& a = e->h_action;
+  const bool actions = mode == B200MDM_COND_ACTION && c.action;
+  if (actions) {
+    a.assign(rows, 0);
+    for (int b = 0; b < B; ++b)
+      for (int k = 0; k < c.K; ++k) {
+        const int64_t v = c.action[static_cast<size_t>(b) * c.K + k];
+        if (v < 0 || v >= e->cfg.num_actions) return fail(B200MDM_EINVAL, "action index out of range");
+        a[static_cast<size_t>(k) * B + b] = static_cast<int>(v);   // group-major, as the packed batch
+      }
+  }
+  TRY(select_workspace(e, B, c.nframes, halves, s, c.multi ? c.K + 1 : 0));
+  if (bert) TRY(ensure_text_memory(e, c.n_tokens));
+  // valid keys: the timestep token (the False column prepended, model/mdm.py:241-247) or DiP's context frames
+  // (model/mdm.py:204-206), then `lengths` frames
+  TRY(upload_kvlen_scale(e, c.nframes, bert ? e->ctx : 1, bert ? e->S > 1 : c.nframes > 1, c.lengths, c.scale, s));
+  if (bert) {
+    e->h_mask.resize(static_cast<size_t>(e->Bp) * e->Mt);
+    pack_text_mask(e->h_mask.data(), c.mask, c.K, B, e->Bp, e->Mt);
+    CUDA_TRY(cudaMemcpyAsync(e->memmask, e->h_mask.data(), e->h_mask.size(), cudaMemcpyHostToDevice, s));
+    e->mem_uncond = uncond;
+    TRY(build_text_memory(e, c.embed, c.K, uncond, e->memproj, s));
+  } else {
+    if (actions) CUDA_TRY(cudaMemcpyAsync(e->action, a.data(), a.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    TRY(fill_condproj(e, c.embed, uncond, rows, s));
+    if (e->dec_clip) TRY(cross_rows_per_sample(e, nullptr, s));
+  }
+  end_cond(e);
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_cond(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* cond_embed_dev,
+                                const int64_t* lengths_host, const float* scale_dev, int32_t force_uncond,
+                                const int64_t* action_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (e->dec) return fail(B200MDM_EINVAL, "trans_dec engines take their conditioning through b200mdm_set_cond_dec");
+  CondIn c{batch, nframes, lengths_host, cond_embed_dev};
+  c.action = action_host;
+  c.scale = scale_dev;
+  c.force_uncond = force_uncond != 0;
+  return set_conditioning(e, c, static_cast<cudaStream_t>(stream));
+}
+
+// trans_dec: the BERT token features + padding mask (DiP, and the plain BERT decoder), or the CLIP row
 extern "C" int b200mdm_set_cond_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, const float* enc_text_dev,
                                     const uint8_t* text_mask_host, int32_t n_tokens, const int64_t* lengths_host,
                                     const float* scale_dev, int32_t force_uncond, void* stream) {
   if (!e) return fail(B200MDM_EINVAL, "null engine");
   if (!e->dec) return fail(B200MDM_EINVAL, "b200mdm_set_cond_dec is for trans_dec engines");
-  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
-  if (e->dec_clip)
-    return set_cond_dec_clip(e, batch, nframes, enc_text_dev, text_mask_host, n_tokens, lengths_host, scale_dev, force_uncond,
-                             static_cast<cudaStream_t>(stream));
-  if (batch <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
-  if (n_tokens <= 0 || n_tokens > XAL_MAX_MT)
-    return fail(B200MDM_EINVAL, "n_tokens %d: a text memory holds 1..%d tokens (DistilBERT's position limit)", n_tokens, XAL_MAX_MT);
-  TRY(check_seq_len(e, nframes + e->ctx));
-  if (!enc_text_dev || !text_mask_host) return fail(B200MDM_EINVAL, "DiP needs y['text_embed'] = (tokens, mask)");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int halves = scale_dev ? 2 : 1;
-  TRY(select_workspace(e, batch, nframes, halves, s));
-  const int d = e->d, B = batch, Bp = e->Bp, Mt = n_tokens, C = e->cfg.cond_dim;
-  TRY(ensure_text_memory(e, Mt));
-  // key mask of the frames: the context frames are always valid (model/mdm.py:204-206), then `lengths` frames of x
-  TRY(upload_kvlen_scale(e, nframes, e->ctx, e->S > 1, lengths_host, scale_dev, s));
-  std::vector<unsigned char>& mk = e->h_mask;
-  mk.assign(static_cast<size_t>(Bp) * Mt, 0);
-  for (int b = 0; b < Bp; ++b)
-    for (int m = 0; m < Mt; ++m) mk[static_cast<size_t>(b) * Mt + m] = text_mask_host[static_cast<size_t>(b % B) * Mt + m] ? 1 : 0;
-  CUDA_TRY(cudaMemcpyAsync(e->memmask, mk.data(), mk.size(), cudaMemcpyHostToDevice, s));
-  // text_emb = embed_text(mask_cond(enc_text)) per token (model/mdm.py:218), once per loop
-  permute_mbc_kernel<<<dim3(Mt, B), 128, 0, s>>>(enc_text_dev, e->encperm, Mt, B, C);
-  CUDA_TRY(cudaGetLastError());
-  const size_t warps = static_cast<size_t>(B) * Mt * d;
-  small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(e->encperm, e->w_txt, e->b_txt, e->memtok, B * Mt, d, C, C);
-  CUDA_TRY(cudaGetLastError());
-  e->mem_uncond = halves == 1 && force_uncond;
-  memproj_fill_kernel<<<dim3(Mt, Bp), 128, 0, s>>>(e->memproj, e->memtok, e->b_txt, B, Mt, d, Bp, e->mem_uncond ? 1 : 0);
-  CUDA_TRY(cudaGetLastError());
-  e->launches += 3;
-  end_cond(e);
-  return B200MDM_OK;
+  CondIn c{batch, nframes, lengths_host, enc_text_dev};
+  c.mask = text_mask_host;
+  c.n_tokens = n_tokens;
+  c.scale = scale_dev;
+  c.force_uncond = force_uncond != 0;
+  return set_conditioning(e, c, static_cast<cudaStream_t>(stream));
+}
+
+// ---- multi-prompt guidance (DESIGN.md, "Multi-prompt guidance")
+extern "C" int b200mdm_set_cond_multi(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K,
+                                      const float* prompt_embed_dev, const int64_t* lengths_host,
+                                      const int64_t* prompt_action_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (e->dec) return fail(B200MDM_EINVAL, "trans_dec engines take their prompts through b200mdm_set_cond_multi_dec");
+  CondIn c{batch, nframes, lengths_host, prompt_embed_dev, K, true};
+  c.action = prompt_action_host;
+  return set_conditioning(e, c, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b200mdm_set_cond_multi_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K,
+                                          const float* prompt_clip_dev, const int64_t* lengths_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!e->dec) return fail(B200MDM_EINVAL, "b200mdm_set_cond_multi_dec is for trans_dec engines");
+  TRY(refuse(e, FAM_MULTI));
+  if (!e->dec_clip)
+    return fail(B200MDM_EINVAL, "BERT-memory decoders take their prompts through b200mdm_set_cond_multi_tokens");
+  return set_conditioning(e, CondIn{batch, nframes, lengths_host, prompt_clip_dev, K, true}, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b200mdm_set_cond_multi_tokens(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K,
+                                             const float* tokens_dev, const uint8_t* mask_host, int32_t n_tokens,
+                                             const int64_t* lengths_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!e->dec) return fail(B200MDM_EINVAL, "b200mdm_set_cond_multi_tokens is for trans_dec engines");
+  TRY(refuse(e, FAM_MULTI));
+  if (e->dec_clip) return fail(B200MDM_EINVAL, "CLIP-memory decoders take their prompts through b200mdm_set_cond_multi_dec");
+  CondIn c{batch, nframes, lengths_host, tokens_dev, K, true};
+  c.mask = mask_host;
+  c.n_tokens = n_tokens;
+  return set_conditioning(e, c, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b200mdm_set_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, void* stream) {
@@ -1450,10 +1560,9 @@ extern "C" int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t
                                      const uint8_t* motion_start_host, void* stream) {
   if (!e) return fail(B200MDM_EINVAL, "null engine");
   if (h < 0) return fail(B200MDM_EINVAL, "handshake size %d < 0", h);
-  if (is_prefix_engine(e)) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented for prefix-completion (DiP) models");
+  TRY(refuse(e, FAM_HANDSHAKE, F_PREFIX));
   if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
-  if (e->jg_set) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented with joint-position control");
-  if (e->groups) return fail(B200MDM_ENOTIMPL, "handshakes are not implemented with multi-prompt guidance");
+  TRY(refuse(e, FAM_HANDSHAKE));
   TRY(handshake_desc(h, e->B, e->T, lengths_host, motion_start_host, &e->h_hs));
   e->hs_set = false;
   if (e->h_hs.empty()) return B200MDM_OK;   // nothing to blend: the plain forward
@@ -1474,11 +1583,9 @@ extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_d
   if (e->cfg.nfeats != 1 || (e->JF != 263 && e->JF != 251))
     return fail(B200MDM_EINVAL, "joint-position control needs the ric features of HumanML3D (263) or KIT (251) with nfeats 1 "
                 "(got %d x %d)", e->cfg.njoints, e->cfg.nfeats);
-  if (is_prefix_engine(e))
-    return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented for prefix-completion (DiP) models");
+  TRY(refuse(e, FAM_JOINT, F_PREFIX));
   if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
-  if (e->hs_set) return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented with handshakes");
-  if (e->groups) return fail(B200MDM_ENOTIMPL, "joint-position control is not implemented with multi-prompt guidance");
+  TRY(refuse(e, FAM_JOINT));
   if (e->T > JG_MAX_FRAMES) return fail(B200MDM_ENOTIMPL, "joint-position control: at most %d frames", JG_MAX_FRAMES);
   if (!e->jg_desc) TRY(dalloc(&e->jg_desc, 1));
   if (!e->jg_x0) TRY(dalloc(&e->jg_x0, static_cast<size_t>(e->B) * e->JF * e->T));
@@ -1529,125 +1636,6 @@ extern "C" int b200mdm_set_foot_guidance(b200mdm_engine* e, float contact_weight
   return B200MDM_OK;
 }
 
-// ENOTIMPL for the samplers joint-position control does not support, while it is set
-static int refuse_joint_guidance(const b200mdm_engine* e, const char* what) {
-  if (e->jg_set) return fail(B200MDM_ENOTIMPL, "%s with joint-position control is not implemented", what);
-  return B200MDM_OK;
-}
-
-// ---- multi-prompt guidance (DESIGN.md, "Multi-prompt guidance")
-static int check_prompts(int32_t batch, int32_t nframes, int32_t K) {
-  if (batch <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad batch / nframes");
-  if (K < 1 || K > MP_MAX_PROMPTS) return fail(B200MDM_EINVAL, "prompt count %d outside 1 .. %d", K, MP_MAX_PROMPTS);
-  return B200MDM_OK;
-}
-
-extern "C" int b200mdm_set_cond_multi(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K,
-                                      const float* prompt_embed_dev, const int64_t* lengths_host,
-                                      const int64_t* prompt_action_host, void* stream) {
-  if (!e) return fail(B200MDM_EINVAL, "null engine");
-  if (e->dec) return fail(B200MDM_EINVAL, "trans_dec engines take their prompts through b200mdm_set_cond_multi_dec");
-  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
-  TRY(check_prompts(batch, nframes, K));
-  TRY(check_seq_len(e, nframes + 1));
-  if (e->cfg.cond_mode == B200MDM_COND_NONE)
-    return fail(B200MDM_EINVAL, "multi-prompt guidance needs a conditioned model (sampler_util.py:29)");
-  if (e->cfg.cond_mode == B200MDM_COND_TEXT && !prompt_embed_dev)
-    return fail(B200MDM_EINVAL, "text-conditioned model needs the prompt embeddings [K, B, C]");
-  std::vector<int>& a = e->h_action;
-  if (e->cfg.cond_mode == B200MDM_COND_ACTION) {
-    if (!prompt_action_host) return fail(B200MDM_EINVAL, "action-conditioned model needs the prompt actions [B, K]");
-    a.assign(static_cast<size_t>(K) * batch, 0);
-    for (int b = 0; b < batch; ++b)
-      for (int k = 0; k < K; ++k) {
-        const int64_t v = prompt_action_host[static_cast<size_t>(b) * K + k];
-        if (v < 0 || v >= e->cfg.num_actions) return fail(B200MDM_EINVAL, "action index out of range");
-        a[static_cast<size_t>(k) * batch + b] = static_cast<int>(v);   // group-major, as the packed batch
-      }
-  }
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  TRY(select_workspace(e, batch, nframes, 1, s, K + 1));
-  TRY(upload_kvlen_scale(e, nframes, 1, nframes > 1, lengths_host, nullptr, s));
-  if (e->cfg.cond_mode == B200MDM_COND_ACTION)
-    CUDA_TRY(cudaMemcpyAsync(e->action, a.data(), a.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-  TRY(fill_condproj(e, prompt_embed_dev, false, s, K * batch));
-  end_cond(e);
-  return B200MDM_OK;
-}
-
-extern "C" int b200mdm_set_cond_multi_dec(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K,
-                                          const float* prompt_clip_dev, const int64_t* lengths_host, void* stream) {
-  if (!e) return fail(B200MDM_EINVAL, "null engine");
-  if (!e->dec) return fail(B200MDM_EINVAL, "b200mdm_set_cond_multi_dec is for trans_dec engines");
-  if (is_prefix_engine(e))
-    return fail(B200MDM_ENOTIMPL, "multi-prompt guidance is not implemented for prefix-completion (DiP) models");
-  if (!e->dec_clip)
-    return fail(B200MDM_EINVAL, "BERT-memory decoders take their prompts through b200mdm_set_cond_multi_tokens");
-  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
-  TRY(check_prompts(batch, nframes, K));
-  if (!prompt_clip_dev) return fail(B200MDM_EINVAL, "the CLIP decoder needs the prompt embeddings [K, B, C]");
-  TRY(check_seq_len(e, nframes + 1));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  TRY(select_workspace(e, batch, nframes, 1, s, K + 1));
-  TRY(upload_kvlen_scale(e, nframes, 1, nframes > 1, lengths_host, nullptr, s));
-  // one memory row per group: W clip_k + b for the prompts, b for the unconditional group
-  TRY(fill_condproj(e, prompt_clip_dev, false, s, K * batch));
-  TRY(cross_rows_per_sample(e, nullptr, s));
-  end_cond(e);
-  return B200MDM_OK;
-}
-
-// The BERT decoder (context_len 0): one token memory per group, W tokens_k + b for the prompts and b for the
-// unconditional group (mask_cond zeroes the tokens, model/mdm.py:218).  The unconditional group admits every token some
-// prompt admits: with K = 1 that is prompt 0's mask, as in b200mdm_set_cond_dec's classifier-free pair, and it does not
-// depend on the prompts' order.  (Its tokens are all equal, so any mask admitting one gives the same output up to
-// rounding.)
-extern "C" int b200mdm_set_cond_multi_tokens(b200mdm_engine* e, int32_t batch, int32_t nframes, int32_t K,
-                                             const float* tokens_dev, const uint8_t* mask_host, int32_t n_tokens,
-                                             const int64_t* lengths_host, void* stream) {
-  if (!e) return fail(B200MDM_EINVAL, "null engine");
-  if (!e->dec) return fail(B200MDM_EINVAL, "b200mdm_set_cond_multi_tokens is for trans_dec engines");
-  if (is_prefix_engine(e))
-    return fail(B200MDM_ENOTIMPL, "multi-prompt guidance is not implemented for prefix-completion (DiP) models");
-  if (e->dec_clip) return fail(B200MDM_EINVAL, "CLIP-memory decoders take their prompts through b200mdm_set_cond_multi_dec");
-  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
-  TRY(check_prompts(batch, nframes, K));
-  if (n_tokens <= 0 || n_tokens > XAL_MAX_MT)
-    return fail(B200MDM_EINVAL, "n_tokens %d: a text memory holds 1..%d tokens (DistilBERT's position limit)", n_tokens, XAL_MAX_MT);
-  if (!tokens_dev || !mask_host) return fail(B200MDM_EINVAL, "the BERT decoder needs the prompt tokens and masks");
-  TRY(check_seq_len(e, nframes + e->ctx));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  TRY(select_workspace(e, batch, nframes, 1, s, K + 1));
-  const int d = e->d, B = batch, Bp = e->Bp, Mt = n_tokens, C = e->cfg.cond_dim, rows = K * B;
-  TRY(ensure_text_memory(e, Mt));
-  TRY(upload_kvlen_scale(e, nframes, e->ctx, e->S > 1, lengths_host, nullptr, s));
-  // [K, B, Mt] is already the prompts' groups in packed order; the unconditional group pads where every prompt pads
-  std::vector<unsigned char>& mk = e->h_mask;
-  mk.assign(static_cast<size_t>(Bp) * Mt, 1);
-  for (int bp = 0; bp < rows; ++bp)
-    for (int m = 0; m < Mt; ++m) {
-      const unsigned char pad = mask_host[static_cast<size_t>(bp) * Mt + m] ? 1 : 0;
-      mk[static_cast<size_t>(bp) * Mt + m] = pad;
-      mk[static_cast<size_t>(rows + bp % B) * Mt + m] &= pad;
-    }
-  CUDA_TRY(cudaMemcpyAsync(e->memmask, mk.data(), mk.size(), cudaMemcpyHostToDevice, s));
-  for (int k = 0; k < K; ++k) {
-    permute_mbc_kernel<<<dim3(Mt, B), 128, 0, s>>>(tokens_dev + static_cast<size_t>(k) * Mt * B * C,
-                                                    e->encperm + static_cast<size_t>(k) * B * Mt * C, Mt, B, C);
-    CUDA_TRY(cudaGetLastError());
-  }
-  const size_t warps = static_cast<size_t>(rows) * Mt * d;
-  small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(e->encperm, e->w_txt, e->b_txt, e->memtok,
-                                                                                     rows * Mt, d, C, C);
-  CUDA_TRY(cudaGetLastError());
-  memproj_group_fill_kernel<<<dim3(Mt, Bp), 128, 0, s>>>(e->memproj, e->memtok, e->b_txt, rows, Mt, d);
-  CUDA_TRY(cudaGetLastError());
-  e->mem_uncond = false;
-  e->launches += K + 2;
-  end_cond(e);
-  return B200MDM_OK;
-}
-
 extern "C" int b200mdm_set_prompt_weight(b200mdm_engine* e, int32_t K, const float* weight_dev, int64_t stride_b,
                                          int64_t stride_k, int64_t stride_f, int64_t stride_t, void* stream) {
   if (!e || !weight_dev) return fail(B200MDM_EINVAL, "null argument");
@@ -1659,12 +1647,6 @@ extern "C" int b200mdm_set_prompt_weight(b200mdm_engine* e, int32_t K, const flo
   e->h_pw = PromptWeight{weight_dev, stride_b, stride_k, stride_f, stride_t, K};
   CUDA_TRY(cudaMemcpyAsync(e->pw_desc, &e->h_pw, sizeof(PromptWeight), cudaMemcpyHostToDevice, static_cast<cudaStream_t>(stream)));
   e->pw_set = true;
-  return B200MDM_OK;
-}
-
-// ENOTIMPL for what multi-prompt guidance does not support, while the conditioning is composed
-static int refuse_multi_prompt(const b200mdm_engine* e, const char* what) {
-  if (e->groups) return fail(B200MDM_ENOTIMPL, "%s with multi-prompt guidance is not implemented", what);
   return B200MDM_OK;
 }
 
@@ -1919,8 +1901,8 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
       if (a.mode <= MODE_DDIM) CUDA_TRY(launch_k(compose_step_kernel<OutStep>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
       else if (a.mode == MODE_DDIM_REVERSE) CUDA_TRY(launch_k(compose_step_kernel<OutReverse>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
       else if (a.mode == MODE_DPM) CUDA_TRY(launch_k(compose_step_kernel<OutDpm>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
-      else if (a.mode == MODE_VB) return fail(B200MDM_ENOTIMPL, "the variational bound with multi-prompt guidance is not implemented");
-      else CUDA_TRY(launch_k(compose_step_kernel<OutPlms>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
+      else   // PLMS: the variational bound refuses multi-prompt guidance (REFUSED)
+        CUDA_TRY(launch_k(compose_step_kernel<OutPlms>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
       nk += 2;
     } else if (e->jg_set && !a.model_only) {
       // joint-position control: the output GEMM writes the raw x0, the guidance kernel runs the step's tail on it
@@ -2040,8 +2022,7 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
   if (reverse) {
     TRY(check_flags("DDIM inversion", flags, B200MDM_FLAG_CLIP_DENOISED));
     TRY(need_table(e, TAB_NEXT));
-    if (e->hs_set) return fail(B200MDM_ENOTIMPL, "DDIM inversion with handshakes is not implemented");
-    TRY(refuse_joint_guidance(e, "DDIM inversion"));
+    TRY(refuse(e, FAM_REVERSE));
   }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   step_set_kernel<<<1, 1, 0, s>>>(e->state, 0, index, nullptr, 0, e->noise_seed, e->noise_sample_base, e->n_steps);
@@ -2265,8 +2246,7 @@ extern "C" int b200mdm_ddim_reverse_loop_range(b200mdm_engine* e, int32_t first_
   TRY(check_ready(e, true));
   if (n_run > e->n_steps - first_index) return fail(B200MDM_EINVAL, "bad step range");
   TRY(need_table(e, TAB_NEXT));
-  if (e->hs_set) return fail(B200MDM_ENOTIMPL, "DDIM inversion with handshakes is not implemented");
-  TRY(refuse_joint_guidance(e, "DDIM inversion"));
+  TRY(refuse(e, FAM_REVERSE));
   return run_loop(e, loop_args(e, B200MDM_MODE_DDIM_REVERSE, 0, flags, false), flags, first_index, n_run, x_in_dev, x_out_dev,
                   nullptr, 0, use_graph, stream);
 }
@@ -2289,7 +2269,7 @@ extern "C" int b200mdm_plms_loop_range(b200mdm_engine* e, int32_t order, int32_t
   TRY(check_range_down(e, first_index, n_run));
   if (!x_in_dev && (e->plms_done < 0 || e->plms_order != order))
     return fail(B200MDM_ESTATE, "no PLMS loop of order %d to continue (pass x_in_dev)", order);
-  TRY(refuse_joint_guidance(e, "PLMS"));
+  TRY(refuse(e, FAM_PLMS));
   TRY(ensure_plms(e));
   // every step after the improved-Euler one is an Adams-Bashforth step: the launches of a DDIM step, one graph per order
   const int done = x_in_dev ? 0 : e->plms_done;
@@ -2315,7 +2295,7 @@ extern "C" int b200mdm_plms_step(b200mdm_engine* e, int32_t index, int32_t order
     if (!old_eps_dev[n_old - h + j]) return fail(B200MDM_EINVAL, "null eps history entry %d", n_old - h + j);
   TRY(check_ready(e, true));
   if (index < 0 || index >= e->n_steps) return fail(B200MDM_EINVAL, "schedule index out of range");
-  TRY(refuse_joint_guidance(e, "PLMS"));
+  TRY(refuse(e, FAM_PLMS));
   TRY(ensure_plms(e));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t n = static_cast<size_t>(e->B) * e->JF * e->T, x_bytes = n * sizeof(float);
@@ -2365,7 +2345,7 @@ extern "C" int b200mdm_dpm_loop_range(b200mdm_engine* e, int32_t order, int32_t 
   TRY(need_table(e, TAB_DPM));
   if (!x_in_dev && (e->dpm_done < 0 || e->dpm_order != order))
     return fail(B200MDM_ESTATE, "no DPM-Solver++ loop of order %d to continue (pass x_in_dev)", order);
-  TRY(refuse_joint_guidance(e, "DPM-Solver++"));
+  TRY(refuse(e, FAM_DPM));
   TRY(ensure_dpm(e));
   const int done = x_in_dev ? 0 : e->dpm_done;
   return run_loop(e, loop_args(e, MODE_DPM, order, flags, false), flags, first_index, n_run, x_in_dev, x_out_dev, nullptr, 0,
@@ -2424,24 +2404,13 @@ extern "C" int b200mdm_chain_setup(b200mdm_engine* e, int32_t n_chunks, int32_t 
     TRY(ensure_cap(&e->chain_mem, &e->chain_mem_cap, n_chunks * mem));
     TRY(ensure_cap(&e->chain_mask, &e->chain_mask_cap, n_chunks * msk));
     std::vector<unsigned char>& mk = e->h_chain_mask;   // staged in the engine until the next call, as b200mdm_set_cond_dec's
-    mk.assign(n_chunks * msk, 0);
+    mk.resize(n_chunks * msk);
     for (int c = 0; c < n_chunks; ++c)
-      for (int b = 0; b < Bp; ++b)
-        for (int m = 0; m < Mt; ++m)
-          mk[c * msk + static_cast<size_t>(b) * Mt + m] = text_mask_chunks_host[(static_cast<size_t>(c) * B + b % B) * Mt + m] ? 1 : 0;
+      pack_text_mask(mk.data() + c * msk, text_mask_chunks_host + static_cast<size_t>(c) * B * Mt, 1, B, Bp, Mt);
     CUDA_TRY(cudaMemcpyAsync(e->chain_mask, mk.data(), mk.size(), cudaMemcpyHostToDevice, s));
-    // each chunk's text_emb, by the launches of b200mdm_set_cond_dec
-    const size_t warps = static_cast<size_t>(B) * Mt * d;
-    for (int c = 0; c < n_chunks; ++c) {
-      permute_mbc_kernel<<<dim3(Mt, B), 128, 0, s>>>(enc_chunks_dev + static_cast<size_t>(c) * Mt * B * C, e->encperm, Mt, B, C);
-      CUDA_TRY(cudaGetLastError());
-      small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(e->encperm, e->w_txt, e->b_txt, e->memtok,
-                                                                                       B * Mt, d, C, C);
-      CUDA_TRY(cudaGetLastError());
-      memproj_fill_kernel<<<dim3(Mt, Bp), 128, 0, s>>>(e->chain_mem + c * mem, e->memtok, e->b_txt, B, Mt, d, Bp, e->mem_uncond ? 1 : 0);
-      CUDA_TRY(cudaGetLastError());
-    }
-    e->launches += 3 * n_chunks;
+    // each chunk's text_emb, as b200mdm_set_cond_dec projects one
+    for (int c = 0; c < n_chunks; ++c)
+      TRY(build_text_memory(e, enc_chunks_dev + static_cast<size_t>(c) * Mt * B * C, 1, e->mem_uncond, e->chain_mem + c * mem, s));
   }
   e->chain_n = n_chunks;
   e->chain_off = include_prefix ? context_len : 0;
@@ -2567,9 +2536,7 @@ extern "C" int b200mdm_vb_loop_range(b200mdm_engine* e, int32_t first_index, int
   TRY(check_range_down(e, first_index, n_run));
   TRY(need_table(e, TAB_VB));
   if (!x_start_dev && !e->vb_live) return fail(B200MDM_ESTATE, "no bound loop to continue (pass x_start_dev)");
-  if (e->hs_set) return fail(B200MDM_ENOTIMPL, "the variational bound with handshakes is not implemented");
-  TRY(refuse_joint_guidance(e, "the variational bound"));
-  TRY(refuse_multi_prompt(e, "the variational bound"));
+  TRY(refuse(e, FAM_VB));
   TRY(ensure_vb(e));
   if (!x_start_dev && !e->vb_live)   // ensure_vb reallocated the tables for a longer schedule: nothing to continue
     return fail(B200MDM_ESTATE, "the schedule outgrew the bound loop's tables: no bound loop to continue (pass x_start_dev)");

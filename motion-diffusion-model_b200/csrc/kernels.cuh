@@ -516,20 +516,9 @@ __global__ void mem_build_kernel(__half* __restrict__ mem16, const float* __rest
   }
 }
 
-// memproj rows of the packed batch: cond half = W enc + b (already in proj [B*Mt, d], row (b, m)), uncond half = b.
-__global__ void memproj_fill_kernel(float* __restrict__ memproj, const float* __restrict__ proj,
-                                    const float* __restrict__ bias, int B, int Mt, int d, int rows_bp, int first_uncond) {
-  const int m = blockIdx.x, bp = blockIdx.y;
-  if (bp >= rows_bp) return;
-  const bool unc = first_uncond ? true : (bp >= B);
-  const int b = bp % B;
-  for (int c = threadIdx.x; c < d; c += blockDim.x)
-    memproj[(static_cast<size_t>(bp) * Mt + m) * d + c] = unc ? bias[c] : proj[(static_cast<size_t>(b) * Mt + m) * d + c];
-}
-
-// memproj rows of multi-prompt guidance's packed batch (b200mdm_set_cond_multi_tokens): the cond_rows = K * B rows of
-// the prompts' groups are W tokens + b (proj [cond_rows*Mt, d], rows (k*B + b, m), group-major as the packed batch), the
-// unconditional group's rows b.  grid = (Mt, Bp)
+// memproj rows of the packed batch (build_text_memory in engine.cu): the first cond_rows rows (K * B prompt rows, group-
+// major as the packed batch; 0 when every row is unconditional) are W tokens + b (proj [cond_rows*Mt, d], rows
+// (k*B + b, m)), the unconditional rows b.  grid = (Mt, Bp)
 __global__ void memproj_group_fill_kernel(float* __restrict__ memproj, const float* __restrict__ proj,
                                           const float* __restrict__ bias, int cond_rows, int Mt, int d) {
   const int m = blockIdx.x, bp = blockIdx.y;

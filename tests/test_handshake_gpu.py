@@ -253,6 +253,32 @@ def test_h0_and_single_window_motions_are_the_plain_model(small):
     assert torch.equal(b200mdm.HandshakeSampleModel(cfg, 0)(xT, t, y=yy), cfg(xT, t, y=yy))
 
 
+def test_enotimpl_refusals(small):
+    """DDIM inversion (a step and the loop) and the bound loop refuse handshakes at the C ABI."""
+    c, inp, shape, y, cfg, diffusion = small
+    B, T, steps = c["B"], c["T"], c["steps"]
+    eng = cfg.model.engine()
+    lib = eng.lib
+    s = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    eng.set_cond(B, T, _y(inp, y), True, torch.device("cuda"))
+    # the tables first: a missing table is ESTATE before the refusal
+    eng.set_schedule(diffusion.schedule_rows(0.0), diffusion._timestep_map(), key=None)
+    eng.set_schedule_next(diffusion.schedule_next_rows())
+    eng.set_schedule_vb(diffusion.schedule_vb_rows())
+    eng.set_handshake(c["h"], B, T, _y(inp, y))
+    x = inp["tape"][0].cuda()
+    out = torch.empty_like(x)
+    calls = {
+        "reverse_step": lambda: lib.b200mdm_sample_step(eng.h, _lib.MODE_DDIM_REVERSE, 0, _p(x), None, 0, _p(out), None, s),
+        "reverse": lambda: lib.b200mdm_ddim_reverse_loop_range(eng.h, 0, steps, _p(x), _p(out), 0, 1, s),
+        "vb": lambda: lib.b200mdm_vb_loop_range(eng.h, steps - 1, steps, _p(x), None, 0, _lib.FLAG_PHILOX_NOISE, None, None, 1,
+                                                s),
+    }
+    for name, call in calls.items():
+        assert call() == _lib.ENOTIMPL, name
+        assert b"handshakes" in lib.b200mdm_last_error(), name
+
+
 # ------------------------------------------------------------------------------------------------ engine state
 def test_engine_state_against_fresh_engines(small):
     c, inp, shape, y, cfg, diffusion = small

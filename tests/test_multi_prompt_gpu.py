@@ -301,6 +301,14 @@ def test_enotimpl_refusals():
     assert ei.value.code == _lib.ENOTIMPL
     import ctypes
     lib = _lib.load()
+    # the bound loop (its table armed first: a missing table is ESTATE before the refusal)
+    eng.set_schedule(diffusion.schedule_rows(0.0), diffusion._timestep_map(), key=None)
+    eng.set_schedule_vb(diffusion.schedule_vb_rows())
+    x = torch.zeros(B, 263, 1, T, device="cuda")
+    s = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    assert lib.b200mdm_vb_loop_range(eng.h, 3, 4, ctypes.c_void_p(x.data_ptr()), None, 0, _lib.FLAG_PHILOX_NOISE, None, None,
+                                     1, s) == _lib.ENOTIMPL
+    assert b"multi-prompt guidance" in lib.b200mdm_last_error()
     assert lib.b200mdm_set_prompt_weight(eng.h, 3, ctypes.c_void_p(w.data_ptr()), 0, 0, 0, 0, None) == _lib.EINVAL
     assert lib.b200mdm_set_prompt_weight(eng.h, 2, ctypes.c_void_p(w.data_ptr()), -1, 0, 0, 0, None) == _lib.EINVAL
     eng.set_cond(B, T, dict(text_embed=inp["text_embed"].cuda()), False, "cuda")      # clears the composition
