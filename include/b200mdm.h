@@ -252,12 +252,42 @@ int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_dev, const f
  * (HumanML3D) or 19, 20, 14, 15 (KIT); channel t describes the frame pair (t, t+1).  contact_dev fp32 [B, 4, T] >= 0
  * gives kappa (the caller's, valid until the work enqueued with it has completed); NULL derives kappa[b,k,t] = 1 where
  * the step's de-normalised x0 has channel k > 0.5 at frame t and t + 1 < L_b, else 0.  lengths_host int64 [B] >= 0
- * (NULL: every frame) gives L_b = min(lengths[b], T).  Both weights 0 turn the terms off.  A negative or non-finite
+ * (NULL: every frame) gives L_b = min(lengths[b], T).  Both weights 0 turn the terms off (L_b is kept for
+ * b200mdm_set_scene_guidance).  A negative or non-finite
  * weight, a non-finite height or a negative length return B200MDM_EINVAL; without b200mdm_set_joint_guidance for the
  * current conditioning, B200MDM_ESTATE.  b200mdm_set_cond* and b200mdm_set_joint_guidance clear it.  The terms live in
  * the guidance descriptor, so a step graph captured with them reads new values at every replay. */
 int b200mdm_set_foot_guidance(b200mdm_engine* e, float contact_weight, float floor_weight, float floor_height,
                               const float* contact_dev, const int64_t* lengths_host, void* stream);
+
+/* A 2D grid over the ground plane XZ (y is up): values fp32 device [gz, gx] or, batch_stride > 0, one grid per sample
+ * with sample b's at values + b * batch_stride (batch_stride 0: shared by the batch).  Row i lies at z = z0 + i * cell
+ * and column k at x = x0 + k * cell.  Sampling at (x, z): u = clamp((x - x0) / cell, 0, gx - 1), v likewise in z, cell
+ * (min(floor(v), gz - 2), min(floor(u), gx - 2)), the bilinear interpolant of that cell and its gradient, which is 0
+ * along a clamped axis.  The values are the caller's and must stay valid until the work enqueued with them has
+ * completed. */
+typedef struct b200mdm_grid {
+  const float* values;
+  int64_t batch_stride;
+  int32_t gz, gx;
+  float x0, z0, cell;
+} b200mdm_grid;
+
+/* Scene terms of joint-position control (DESIGN.md "Joint-position control", "Scene: obstacles and uneven ground"): the
+ * guided energy becomes
+ *   G = G_joint + G_contact + 1/2 floor_weight sum_{t<L_b, j} min(p[t,j].y - floor_height - H(p.x, p.z), 0)^2
+ *               + 1/2 obstacle_weight sum_{t<L_b, j} max(obstacle_margin - S(p[t,j].x, p[t,j].z), 0)^2,
+ * with S the obstacles' 2D signed distance `sdf` (positive outside) and H the heights `terrain` (NULL: H = 0, today's flat
+ * floor), the floor and contact terms and L_b those of the last b200mdm_set_foot_guidance (both of its weights may be 0;
+ * without that call, every frame).  A negative or non-finite weight or margin, a bad grid (null values, gz or gx < 2,
+ * a cell that is not finite or <= 0, an origin that is not finite, a batch stride that is neither 0 nor at least
+ * gz * gx or that overflows over B samples), an obstacle weight > 0 without an sdf, or a terrain while the floor weight
+ * is 0 return B200MDM_EINVAL before any CUDA call; without b200mdm_set_joint_guidance for the current conditioning,
+ * B200MDM_ESTATE.  An obstacle weight of 0 without a terrain turns the terms off.  b200mdm_set_cond*,
+ * b200mdm_set_joint_guidance and b200mdm_set_foot_guidance clear it.  The terms live in the guidance descriptor, so a
+ * step graph captured with them reads new values at every replay. */
+int b200mdm_set_scene_guidance(b200mdm_engine* e, float obstacle_weight, float obstacle_margin, const b200mdm_grid* sdf,
+                               const b200mdm_grid* terrain, void* stream);
 
 /* Multi-prompt guidance (this project's definition, DESIGN.md "Multi-prompt guidance"): K prompts per motion, composed
  * around the unconditional prediction as
@@ -531,13 +561,22 @@ int b200mdm_test_joint_guidance(const float* x0_dev, const float* mean_dev, cons
                                 const float* weight_dev, int32_t B, int32_t T, int32_t D, float step, int32_t iters,
                                 float* x0_out_dev, float* loss_out_dev, void* stream);
 /* The guidance iterations with the foot-contact and floor terms of b200mdm_set_foot_guidance alone
- * (joint_guidance_test_kernel<true>): as b200mdm_test_joint_guidance, with contact_dev / lengths_host (both nullable) and
+ * (joint_guidance_test_kernel<true, false>): as b200mdm_test_joint_guidance, with contact_dev / lengths_host (both nullable) and
  * the weights and height as there; loss_out receives the total G.  Invalid arguments return B200MDM_EINVAL before any
  * CUDA call. */
 int b200mdm_test_foot_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
                                const float* weight_dev, const float* contact_dev, const int64_t* lengths_host, int32_t B,
                                int32_t T, int32_t D, float step, int32_t iters, float contact_weight, float floor_weight,
                                float floor_height, float* x0_out_dev, float* loss_out_dev, void* stream);
+/* The guidance iterations with the foot and scene terms of b200mdm_set_foot_guidance and b200mdm_set_scene_guidance
+ * alone (joint_guidance_test_kernel<true, true>): as b200mdm_test_foot_guidance, with the obstacle weight, margin and
+ * grids as there (the terrain's check against floor_weight included); loss_out receives the total G.  Invalid arguments
+ * return B200MDM_EINVAL before any CUDA call. */
+int b200mdm_test_scene_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
+                                const float* weight_dev, const float* contact_dev, const int64_t* lengths_host, int32_t B,
+                                int32_t T, int32_t D, float step, int32_t iters, float contact_weight, float floor_weight,
+                                float floor_height, float obstacle_weight, float obstacle_margin, const b200mdm_grid* sdf,
+                                const b200mdm_grid* terrain, float* x0_out_dev, float* loss_out_dev, void* stream);
 /* Self-attention core (tensor-core kernel, S <= 256): softmax(q k^T / sqrt(128) + mask) v per (sample, head);
  * qkv16 [n*S, 3d]; kvlen int32 [n] device (valid keys per sample, a prefix).
  * impl 0: out16 fp16 [n*S, d] (the encoder); impl 1: out16 fp16 [n*S, 2d] = [hi | lo] with hi + lo = the fp32 result

@@ -13,6 +13,7 @@ from .utils.model_util import (create_model_and_diffusion, create_gaussian_diffu
 from .utils.sampler_util import (ClassifierFreeSampleModel, AutoRegressiveSampler, HandshakeSampleModel,  # noqa: F401
                                  JointControlSampleModel, MultiPromptSampleModel, body_part_mask, stitch_handshake,
                                  transition_layout, refine_transitions)
+from .utils.scene import SceneGrid, shape_sdf  # noqa: F401
 from .diffusion.respace import SpacedDiffusion, space_timesteps  # noqa: F401
 from .diffusion.gaussian_diffusion import GaussianDiffusion, get_named_beta_schedule  # noqa: F401
 from .model.mdm import MDM  # noqa: F401

@@ -39,6 +39,7 @@ SYMBOLS = [
     "b200mdm_chain_setup", "b200mdm_chain_loop_range", "b200mdm_set_joint_guidance", "b200mdm_test_joint_guidance",
     "b200mdm_set_cond_multi", "b200mdm_set_cond_multi_dec", "b200mdm_set_prompt_weight",
     "b200mdm_set_cond_multi_tokens", "b200mdm_set_foot_guidance", "b200mdm_test_foot_guidance",
+    "b200mdm_set_scene_guidance", "b200mdm_test_scene_guidance",
 ]
 MAX_PROMPTS = 8                             # B200MDM_MAX_PROMPTS
 MAX_MEMORY_TOKENS = 512                     # a BERT text memory holds 1 .. 512 tokens (DistilBERT's position limit)
@@ -53,6 +54,12 @@ class Config(ctypes.Structure):
         "arch", "latent_dim", "ff_size", "num_layers", "num_heads", "njoints", "nfeats", "cond_mode", "cond_dim",
         "num_actions", "mask_frames", "pos_embed_max_len", "temb_rows", "context_len", "target_encoder",
         "target_enc_layers", "target_joints", "emb_trans_dec", "dec_memory")] + [("reserved", ctypes.c_int32 * 1)]
+
+
+class Grid(ctypes.Structure):
+    """b200mdm_grid: a 2D grid over the ground plane (values device fp32, batch_stride 0 = shared by the batch)"""
+    _fields_ = [("values", ctypes.c_void_p), ("batch_stride", ctypes.c_int64), ("gz", ctypes.c_int32),
+                ("gx", ctypes.c_int32), ("x0", ctypes.c_float), ("z0", ctypes.c_float), ("cell", ctypes.c_float)]
 
 
 class B200MDMError(RuntimeError):
@@ -138,6 +145,9 @@ def load():
                        ("b200mdm_set_foot_guidance", [vp, f32, f32, f32, vp, vp, vp]),
                        ("b200mdm_test_foot_guidance", [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, f32, f32, f32,
                                                        vp, vp, vp]),
+                       ("b200mdm_set_scene_guidance", [vp, f32, f32, ctypes.POINTER(Grid), ctypes.POINTER(Grid), vp]),
+                       ("b200mdm_test_scene_guidance", [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, f32, f32, f32,
+                                                        f32, f32, ctypes.POINTER(Grid), ctypes.POINTER(Grid), vp, vp, vp]),
                        ("b200mdm_set_cond_multi", [vp, i32, i32, i32, vp, vp, vp, vp]),
                        ("b200mdm_set_cond_multi_dec", [vp, i32, i32, i32, vp, vp, vp]),
                        ("b200mdm_set_cond_multi_tokens", [vp, i32, i32, i32, vp, vp, i32, vp, vp]),

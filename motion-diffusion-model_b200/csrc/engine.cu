@@ -149,11 +149,12 @@ struct GraphKey {
   const void* hs = nullptr;         // the workspace's handshake descriptor, or nullptr when the loop has none
   bool guided = false;              // joint-position control: the step ends in joint_guidance_step_kernel
   int groups = 0;                   // multi-prompt guidance: the step ends in compose_step_kernel over G groups
-  bool foot = false;                // ... with the foot-contact and floor terms: joint_guidance_step_kernel<true>
+  bool foot = false;                // ... with the foot-contact and floor terms: joint_guidance_step_kernel<true, false>
+  bool scene = false;               // ... and the scene terms: joint_guidance_step_kernel<true, true>
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
            imask == o.imask && iweight == o.iweight && imotion == o.imotion && target_g == o.target_g && hs == o.hs &&
-           guided == o.guided && groups == o.groups && foot == o.foot;
+           guided == o.guided && groups == o.groups && foot == o.foot && scene == o.scene;
   }
 };
 
@@ -272,12 +273,17 @@ struct b200mdm_engine : Workspace {
   bool jg_set = false;
   // its foot-contact and floor terms (b200mdm_set_foot_guidance): the descriptor's FootGuide, the lengths it points to
   // (fg_len [fg_len_cap] int32 device, allocated on first use) and their host staging; fg_set is cleared by every
-  // b200mdm_set_cond* and b200mdm_set_joint_guidance call
+  // b200mdm_set_cond* and b200mdm_set_joint_guidance call.  h_fg also holds the lengths of a call with both weights 0,
+  // which the scene terms read.
   FootGuide h_fg{};
   int* fg_len = nullptr;
   int fg_len_cap = 0;
   std::vector<int> h_fg_len;
   bool fg_set = false;
+  // its scene terms (b200mdm_set_scene_guidance): the descriptor's SceneGuide; sg_set is cleared by every
+  // b200mdm_set_cond*, b200mdm_set_joint_guidance and b200mdm_set_foot_guidance call
+  SceneGuide h_sg{};
+  bool sg_set = false;
   // multi-prompt guidance: the prompt-weight descriptor (read by the step graph at every replay, allocated on first
   // use) and its host staging; pw_set is cleared by every b200mdm_set_cond* call
   PromptWeight* pw_desc = nullptr;
@@ -361,11 +367,13 @@ static int init_kernel_attrs() {
   TRY((set_attention_attr<256>()));
   CUDA_TRY(cudaFuncSetAttribute(cross_attention_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XAL_SMEM));
   const int jg_smem = static_cast<int>(jg_smem_bytes(JG_MAX_FRAMES, JG_MAX_FEATS));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
   const int fg_smem = static_cast<int>(fg_smem_bytes(JG_MAX_FRAMES, JG_MAX_FEATS));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
   if (dev < 64) done_mask |= 1ull << dev;
   return B200MDM_OK;
 }
@@ -1258,6 +1266,7 @@ static void end_cond(b200mdm_engine* e) {
   e->hs_set = false;
   e->jg_set = false;
   e->fg_set = false;
+  e->sg_set = false;
   e->pw_set = false;
   e->vb_live = false;
   e->chain_next = -1;
@@ -1594,6 +1603,8 @@ extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_d
                            static_cast<cudaStream_t>(stream)));
   e->jg_set = true;
   e->fg_set = false;
+  e->h_fg = FootGuide{};
+  e->sg_set = false;
   return B200MDM_OK;
 }
 
@@ -1613,7 +1624,7 @@ extern "C" int b200mdm_set_foot_guidance(b200mdm_engine* e, float contact_weight
   TRY(check_foot(contact_weight, floor_weight, floor_height, lengths_host, e->B));
   if (!e->jg_set) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (foot guidance extends it)");
   e->fg_set = false;
-  if (contact_weight == 0.f && floor_weight == 0.f) return B200MDM_OK;   // off: plain joint-position control
+  e->sg_set = false;
   const int* len = nullptr;
   if (lengths_host) {
     if (e->fg_len_cap < e->B) {
@@ -1630,9 +1641,61 @@ extern "C" int b200mdm_set_foot_guidance(b200mdm_engine* e, float contact_weight
     len = e->fg_len;
   }
   e->h_fg = FootGuide{contact_dev, len, contact_weight, floor_weight, floor_height};
+  // both weights 0: plain joint-position control, with the lengths kept for the scene terms
+  if (contact_weight == 0.f && floor_weight == 0.f) return B200MDM_OK;
   CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->f, &e->h_fg, sizeof(FootGuide), cudaMemcpyHostToDevice,
                            static_cast<cudaStream_t>(stream)));
   e->fg_set = true;
+  return B200MDM_OK;
+}
+
+// the argument checks of one grid of b200mdm_set_scene_guidance and b200mdm_test_scene_guidance (NULL: no grid)
+static int check_grid(const b200mdm_grid* g, const char* what, int B, SceneGrid* out) {
+  *out = SceneGrid{};
+  if (!g) return B200MDM_OK;
+  if (!g->values) return fail(B200MDM_EINVAL, "%s: null values", what);
+  if (g->gz < 2 || g->gx < 2 || static_cast<int64_t>(g->gz) * g->gx > (int64_t{1} << 30))
+    return fail(B200MDM_EINVAL, "%s: %d x %d cells: at least 2 x 2, at most 2^30", what, g->gz, g->gx);
+  if (!std::isfinite(g->cell) || g->cell <= 0.f) return fail(B200MDM_EINVAL, "%s: cell %g: a finite value > 0", what, g->cell);
+  if (!std::isfinite(g->x0) || !std::isfinite(g->z0)) return fail(B200MDM_EINVAL, "%s: origin (%g, %g): finite values", what, g->x0, g->z0);
+  const int64_t n = static_cast<int64_t>(g->gz) * g->gx;
+  if (g->batch_stride != 0 && (g->batch_stride < n || g->batch_stride > (INT64_MAX - n) / std::max(B - 1, 1)))
+    return fail(B200MDM_EINVAL, "%s: batch stride %lld: 0 (shared) or at least %lld, with %d samples", what,
+                static_cast<long long>(g->batch_stride), static_cast<long long>(n), B);
+  *out = SceneGrid{g->values, static_cast<long long>(g->batch_stride), g->gz, g->gx, g->x0, g->z0, g->cell};
+  return B200MDM_OK;
+}
+
+// the argument checks b200mdm_set_scene_guidance and b200mdm_test_scene_guidance share; the terrain's floor-weight check
+// is the caller's (the engine's floor weight is state)
+static int check_scene(float obstacle_weight, float obstacle_margin, const b200mdm_grid* sdf, const b200mdm_grid* terrain,
+                       int B, SceneGuide* out) {
+  if (!std::isfinite(obstacle_weight) || obstacle_weight < 0.f || !std::isfinite(obstacle_margin) || obstacle_margin < 0.f)
+    return fail(B200MDM_EINVAL, "obstacle weight %g, margin %g: finite values >= 0", obstacle_weight, obstacle_margin);
+  TRY(check_grid(sdf, "obstacle sdf", B, &out->sdf));
+  TRY(check_grid(terrain, "terrain", B, &out->terrain));
+  if (obstacle_weight > 0.f && !sdf) return fail(B200MDM_EINVAL, "obstacle weight %g without an obstacle sdf", obstacle_weight);
+  out->obstacle_w = obstacle_weight;
+  out->margin = obstacle_margin;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_scene_guidance(b200mdm_engine* e, float obstacle_weight, float obstacle_margin,
+                                          const b200mdm_grid* sdf, const b200mdm_grid* terrain, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  SceneGuide sg{};
+  TRY(check_scene(obstacle_weight, obstacle_margin, sdf, terrain, e->B, &sg));
+  if (!e->jg_set) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (scene guidance extends it)");
+  if (terrain && e->h_fg.floor_w == 0.f)
+    return fail(B200MDM_EINVAL, "a terrain needs a floor weight > 0 (b200mdm_set_foot_guidance)");
+  e->sg_set = false;
+  if (obstacle_weight == 0.f && !terrain) return B200MDM_OK;   // off: no scene
+  e->h_sg = sg;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // the foot terms as set (both weights 0 included: the lengths), then the scene
+  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->f, &e->h_fg, sizeof(FootGuide), cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->s, &e->h_sg, sizeof(SceneGuide), cudaMemcpyHostToDevice, s));
+  e->sg_set = true;
   return B200MDM_OK;
 }
 
@@ -1918,11 +1981,14 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
       TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, ax, px, s, e->num_sms));
       set_step_params(&p, a, B, T, JF);
       const int R = 4 + 3 * ((JF == 263 ? 22 : 21) - 1);
-      if (e->fg_set)
-        CUDA_TRY(launch_k(joint_guidance_step_kernel<true>, dim3(B), dim3(JG_THREADS), fg_smem_bytes(T, R), s,
+      if (e->sg_set)
+        CUDA_TRY(launch_k(joint_guidance_step_kernel<true, true>, dim3(B), dim3(JG_THREADS), fg_smem_bytes(T, R), s,
+                          static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
+      else if (e->fg_set)
+        CUDA_TRY(launch_k(joint_guidance_step_kernel<true, false>, dim3(B), dim3(JG_THREADS), fg_smem_bytes(T, R), s,
                           static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
       else
-        CUDA_TRY(launch_k(joint_guidance_step_kernel<false>, dim3(B), dim3(JG_THREADS), jg_smem_bytes(T, R), s,
+        CUDA_TRY(launch_k(joint_guidance_step_kernel<false, false>, dim3(B), dim3(JG_THREADS), jg_smem_bytes(T, R), s,
                           static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
       nk += 2;
     } else {
@@ -2129,6 +2195,7 @@ static int loop_enter(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32
     key.hs = e->hs_set ? e->hs_desc : nullptr;
     key.guided = e->jg_set;
     key.foot = e->jg_set && e->fg_set;
+    key.scene = e->jg_set && e->sg_set;
     key.groups = e->groups;
     TRY(ensure_step_graph(e, key, a));
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
@@ -2984,23 +3051,17 @@ extern "C" int b200mdm_test_joint_guidance(const float* x0_dev, const float* mea
   TRY(init_kernel_attrs());
   const JointGuide g{mean_dev, std_dev, target_dev, weight_dev, step, iters};
   const int R = D == 263 ? 67 : 64;
-  joint_guidance_test_kernel<false><<<B, JG_THREADS, jg_smem_bytes(T, R), static_cast<cudaStream_t>(stream)>>>(
-      g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, FootGuide{});
+  joint_guidance_test_kernel<false, false><<<B, JG_THREADS, jg_smem_bytes(T, R), static_cast<cudaStream_t>(stream)>>>(
+      g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, FootGuide{}, SceneGuide{});
   CUDA_TRY(cudaGetLastError());
   return B200MDM_OK;
 }
 
-extern "C" int b200mdm_test_foot_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev,
-                                          const float* target_dev, const float* weight_dev, const float* contact_dev,
-                                          const int64_t* lengths_host, int32_t B, int32_t T, int32_t D, float step,
-                                          int32_t iters, float contact_weight, float floor_weight, float floor_height,
-                                          float* x0_out_dev, float* loss_out_dev, void* stream) {
-  if (!x0_dev || !mean_dev || !std_dev || !target_dev || !weight_dev || !x0_out_dev) return fail(B200MDM_EINVAL, "null argument");
-  if (!std::isfinite(step) || step <= 0.f) return fail(B200MDM_EINVAL, "guidance step %g: a finite value > 0", step);
-  if (iters < 1 || iters > 10000) return fail(B200MDM_EINVAL, "guidance iterations %d outside 1 .. 10000", iters);
-  if (D != 263 && D != 251) return fail(B200MDM_EINVAL, "D %d: 263 (HumanML3D) or 251 (KIT)", D);
-  if (B < 1 || T < 1 || T > JG_MAX_FRAMES) return fail(B200MDM_EINVAL, "B %d, T %d: B >= 1, 1 <= T <= %d", B, T, JG_MAX_FRAMES);
-  TRY(check_foot(contact_weight, floor_weight, floor_height, lengths_host, B));
+// b200mdm_test_foot_guidance and b200mdm_test_scene_guidance (sg: nullptr without the scene terms)
+static int test_foot_scene(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
+                           const float* weight_dev, const float* contact_dev, const int64_t* lengths_host, int32_t B,
+                           int32_t T, int32_t D, float step, int32_t iters, float contact_weight, float floor_weight,
+                           float floor_height, const SceneGuide* sg, float* x0_out_dev, float* loss_out_dev, void* stream) {
   TRY(init_kernel_attrs());
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int* len = nullptr;
@@ -3014,12 +3075,56 @@ extern "C" int b200mdm_test_foot_guidance(const float* x0_dev, const float* mean
   const JointGuide g{mean_dev, std_dev, target_dev, weight_dev, step, iters};
   const FootGuide f{contact_dev, len, contact_weight, floor_weight, floor_height};
   const int R = D == 263 ? 67 : 64;
-  joint_guidance_test_kernel<true><<<B, JG_THREADS, fg_smem_bytes(T, R), s>>>(g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, f);
+  if (sg)
+    joint_guidance_test_kernel<true, true><<<B, JG_THREADS, fg_smem_bytes(T, R), s>>>(g, x0_dev, x0_out_dev, loss_out_dev, B,
+                                                                                      T, D, f, *sg);
+  else
+    joint_guidance_test_kernel<true, false><<<B, JG_THREADS, fg_smem_bytes(T, R), s>>>(g, x0_dev, x0_out_dev, loss_out_dev, B,
+                                                                                       T, D, f, SceneGuide{});
   const cudaError_t err = cudaGetLastError();
   if (len) cudaFreeAsync(len, s);
   if (err != cudaSuccess) return fail(B200MDM_ECUDA, "%s", cudaGetErrorString(err));
   CUDA_TRY(cudaStreamSynchronize(s));   // h_len is local
   return B200MDM_OK;
+}
+
+// the argument checks of the guidance test hooks (the foot terms' included)
+static int check_foot_test(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
+                           const float* weight_dev, const int64_t* lengths_host, int32_t B, int32_t T, int32_t D, float step,
+                           int32_t iters, float contact_weight, float floor_weight, float floor_height, const float* x0_out_dev) {
+  if (!x0_dev || !mean_dev || !std_dev || !target_dev || !weight_dev || !x0_out_dev) return fail(B200MDM_EINVAL, "null argument");
+  if (!std::isfinite(step) || step <= 0.f) return fail(B200MDM_EINVAL, "guidance step %g: a finite value > 0", step);
+  if (iters < 1 || iters > 10000) return fail(B200MDM_EINVAL, "guidance iterations %d outside 1 .. 10000", iters);
+  if (D != 263 && D != 251) return fail(B200MDM_EINVAL, "D %d: 263 (HumanML3D) or 251 (KIT)", D);
+  if (B < 1 || T < 1 || T > JG_MAX_FRAMES) return fail(B200MDM_EINVAL, "B %d, T %d: B >= 1, 1 <= T <= %d", B, T, JG_MAX_FRAMES);
+  return check_foot(contact_weight, floor_weight, floor_height, lengths_host, B);
+}
+
+extern "C" int b200mdm_test_foot_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev,
+                                          const float* target_dev, const float* weight_dev, const float* contact_dev,
+                                          const int64_t* lengths_host, int32_t B, int32_t T, int32_t D, float step,
+                                          int32_t iters, float contact_weight, float floor_weight, float floor_height,
+                                          float* x0_out_dev, float* loss_out_dev, void* stream) {
+  TRY(check_foot_test(x0_dev, mean_dev, std_dev, target_dev, weight_dev, lengths_host, B, T, D, step, iters, contact_weight,
+                      floor_weight, floor_height, x0_out_dev));
+  return test_foot_scene(x0_dev, mean_dev, std_dev, target_dev, weight_dev, contact_dev, lengths_host, B, T, D, step, iters,
+                         contact_weight, floor_weight, floor_height, nullptr, x0_out_dev, loss_out_dev, stream);
+}
+
+extern "C" int b200mdm_test_scene_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev,
+                                           const float* target_dev, const float* weight_dev, const float* contact_dev,
+                                           const int64_t* lengths_host, int32_t B, int32_t T, int32_t D, float step,
+                                           int32_t iters, float contact_weight, float floor_weight, float floor_height,
+                                           float obstacle_weight, float obstacle_margin, const b200mdm_grid* sdf,
+                                           const b200mdm_grid* terrain, float* x0_out_dev, float* loss_out_dev,
+                                           void* stream) {
+  TRY(check_foot_test(x0_dev, mean_dev, std_dev, target_dev, weight_dev, lengths_host, B, T, D, step, iters, contact_weight,
+                      floor_weight, floor_height, x0_out_dev));
+  SceneGuide sg{};
+  TRY(check_scene(obstacle_weight, obstacle_margin, sdf, terrain, B, &sg));
+  if (terrain && floor_weight == 0.f) return fail(B200MDM_EINVAL, "a terrain needs a floor weight > 0");
+  return test_foot_scene(x0_dev, mean_dev, std_dev, target_dev, weight_dev, contact_dev, lengths_host, B, T, D, step, iters,
+                         contact_weight, floor_weight, floor_height, &sg, x0_out_dev, loss_out_dev, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ post-processing

@@ -16,6 +16,10 @@
 // Delta_k[t] = p[t+1, f_k] - p[t, f_k] formed from the root velocity w[t+1] and the rotated root-relative feet (never from
 // world positions), and 1/2 lf sum_{t<L, j} min(p[t,j].y - h, 0)^2; both only add to e, the existing chain is unchanged.
 // The neighbour frame's w and feet, and kappa * Delta of the previous pair, go through shared memory.
+// SCENE (DESIGN.md, "Scene: obstacles and uneven ground"), on top of FOOT: two 2D grids over the XZ plane, sampled
+// bilinearly at every joint's world XZ (scene_sample; read through L2).  G gains 1/2 lo sum_{t<L, j} max(r - S, 0)^2 with
+// S the obstacles' signed distance, and the floor term's height becomes h + H(x, z) with H the terrain; both only add to e
+// (in x / z through the grids' gradients), the existing chain is unchanged.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -49,10 +53,28 @@ struct FootGuide {
   float contact_w, floor_w, floor_h;
 };
 
-// The engine's device descriptor: the foot terms follow the joint terms, so a FOOT = false kernel reads what it always read
+// A 2D grid over the XZ plane (b200mdm_grid): values [gz, gx] fp32, sample b's at v + b * stride (stride 0: shared);
+// row i at z = z0 + i * cell, column k at x = x0 + k * cell.  v == nullptr: no grid.
+struct SceneGrid {
+  const float* v;
+  long long stride;
+  int gz, gx;
+  float x0, z0, cell;
+};
+
+// The scene terms (b200mdm_set_scene_guidance): the obstacles' signed distance (nullptr values: none) with weight lo and
+// margin r, and the terrain heights H added to the floor height (nullptr values: a flat floor).
+struct SceneGuide {
+  SceneGrid sdf, terrain;
+  float obstacle_w, margin;
+};
+
+// The engine's device descriptor: the foot terms follow the joint terms and the scene terms the foot terms, so a kernel
+// without them reads what it always read
 struct GuideDesc {
   JointGuide j;
   FootGuide f;
+  SceneGuide s;
 };
 
 // Shared memory of the guidance: xs [R, T] floats, mean / std of the R features, the velocity adjoints handed one frame
@@ -104,6 +126,27 @@ __device__ __forceinline__ void jg_scan(double (&v)[N], double* sh) {
   __syncthreads();
 }
 
+// The bilinear interpolant of grid G (sample b) at (x, z) and its gradient (*dx, *dz), fp32: u = clamp((x - x0) / cell,
+// 0, gx - 1), cell column k = min(floor(u), gx - 2), alpha = u - k (and v, i, beta in z); the gradient is the cell's,
+// 0 along a clamped axis.
+__device__ __forceinline__ float scene_sample(const SceneGrid& G, int b, float x, float z, float* dx, float* dz) {
+  const float* V = G.v + static_cast<size_t>(b) * static_cast<size_t>(G.stride);
+  const float ur = __fdiv_rn(__fsub_rn(x, G.x0), G.cell), vr = __fdiv_rn(__fsub_rn(z, G.z0), G.cell);
+  const float u = fminf(fmaxf(ur, 0.f), static_cast<float>(G.gx - 1));
+  const float v = fminf(fmaxf(vr, 0.f), static_cast<float>(G.gz - 1));
+  const int k = min(static_cast<int>(u), G.gx - 2), i = min(static_cast<int>(v), G.gz - 2);
+  const float a = __fsub_rn(u, static_cast<float>(k)), c = __fsub_rn(v, static_cast<float>(i));
+  const float* r0 = V + static_cast<size_t>(i) * G.gx + k;
+  const float v00 = __ldcg(r0), v01 = __ldcg(r0 + 1), v10 = __ldcg(r0 + G.gx), v11 = __ldcg(r0 + G.gx + 1);
+  const float e0 = __fsub_rn(v01, v00), e1 = __fsub_rn(v11, v10);   // x differences of rows i, i + 1
+  const float f0 = __fsub_rn(v10, v00), f1 = __fsub_rn(v11, v01);   // z differences of columns k, k + 1
+  const bool cx = ur == u, cz = vr == v;                            // false on a clamped axis (or a NaN coordinate)
+  *dx = cx ? __fdiv_rn(__fadd_rn(__fmul_rn(__fsub_rn(1.f, c), e0), __fmul_rn(c, e1)), G.cell) : 0.f;
+  *dz = cz ? __fdiv_rn(__fadd_rn(__fmul_rn(__fsub_rn(1.f, a), f0), __fmul_rn(a, f1)), G.cell) : 0.f;
+  const float w0 = __fadd_rn(v00, __fmul_rn(a, e0)), w1 = __fadd_rn(v10, __fmul_rn(a, e1));
+  return __fadd_rn(w0, __fmul_rn(c, __fsub_rn(w1, w0)));
+}
+
 // x0[f] <- x0[f] - (step * std[f]) * g; a zero gradient leaves x0 bit for bit (a -0 gradient would turn -0 into +0)
 __device__ __forceinline__ void jg_descend(float* x0, float step_sd, float g) {
   if (g != 0.f) *x0 = __fsub_rn(*x0, __fmul_rn(step_sd, g));
@@ -121,10 +164,12 @@ struct FootFrame {
 // One iteration's joint pass with the foot terms, for thread t's frame (every thread of the block calls it): the
 // neighbour exchange, kappa * Delta of pair (t, t + 1) and its loss, then per joint e = w (p - c) + the floor's and the
 // contact pairs' adjoints, into the position / yaw adjoints and the descent on height and joints, as joint_guidance_iterate.
+// SCENE: the floor's height gains the terrain, and the obstacles' adjoint joins (sg.obstacle_w is 0 on frames >= L).
+template <bool SCENE>
 __device__ __forceinline__ void foot_iterate(float* xs, const float* mu, const float* sd, const JointGuide& g, const FootGuide& fg,
                                              const FootFrame& ff, const float* tg, const float* wt, int T, int J, bool upd,
                                              float c, float s, float wx, float wz, float px, float pz, float* gpx, float* gpz,
-                                             float* gyaw, double* lsum) {
+                                             float* gyaw, double* lsum, const SceneGuide& sg, int b) {
   const int t = threadIdx.x;
   const bool act = t < T;
   auto X = [&](int f) { return __fadd_rn(__fmul_rn(xs[f * T + t], sd[f]), mu[f]); };
@@ -194,7 +239,31 @@ __device__ __forceinline__ void foot_iterate(float* xs, const float* mu, const f
                                                static_cast<double>(dz) * dz);
       ex = __fmul_rn(w, dx); ey = __fmul_rn(w, dy); ez = __fmul_rn(w, dz);
     }
-    if (ff.floor) {   // the floor: lf min(p.y - h, 0)
+    if constexpr (SCENE) {
+      const float x = __fadd_rn(rx, px), z = __fadd_rn(rz, pz);   // the joint's world XZ (rx = rz = 0 at the root)
+      if (ff.floor) {   // the floor over the terrain: lf min(p.y - h - H, 0), and -lf m dH in x / z
+        float hx = 0.f, hz = 0.f;
+        const float H = sg.terrain.v != nullptr ? scene_sample(sg.terrain, b, x, z, &hx, &hz) : 0.f;
+        const float m = fminf(__fsub_rn(__fsub_rn(qy, fg.floor_h), H), 0.f);
+        if (m < 0.f) {
+          *lsum += 0.5 * static_cast<double>(fg.floor_w) * (static_cast<double>(m) * m);
+          const float lm = __fmul_rn(fg.floor_w, m);
+          ey = __fadd_rn(ey, lm);
+          ex = __fsub_rn(ex, __fmul_rn(lm, hx));
+          ez = __fsub_rn(ez, __fmul_rn(lm, hz));
+        }
+      }
+      if (sg.obstacle_w > 0.f) {   // the obstacles: lo max(r - S, 0), and -lo m dS in x / z
+        float sx, sz;
+        const float m = fmaxf(__fsub_rn(sg.margin, scene_sample(sg.sdf, b, x, z, &sx, &sz)), 0.f);
+        if (m > 0.f) {
+          *lsum += 0.5 * static_cast<double>(sg.obstacle_w) * (static_cast<double>(m) * m);
+          const float lm = __fmul_rn(sg.obstacle_w, m);
+          ex = __fsub_rn(ex, __fmul_rn(lm, sx));
+          ez = __fsub_rn(ez, __fmul_rn(lm, sz));
+        }
+      }
+    } else if (ff.floor) {   // the floor: lf min(p.y - h, 0)
       const float m = fminf(__fsub_rn(qy, fg.floor_h), 0.f);
       if (m < 0.f) {
         *lsum += 0.5 * static_cast<double>(fg.floor_w) * (static_cast<double>(m) * m);
@@ -230,9 +299,10 @@ __device__ __forceinline__ void foot_iterate(float* xs, const float* mu, const f
 // The K guidance iterations of motion b on xs (its R ric features, normalised, [R, T] in shared memory; mu / sd the
 // features' mean and std).  loss (nullable) [K + 1, B] receives G before each iteration and after the last one.
 // Every thread of the block calls it.
-template <bool FOOT>
+template <bool FOOT, bool SCENE>
 __device__ void joint_guidance_iterate(float* xs, const float* mu, const float* sd, float* gv, double* sh, const JointGuide& g,
-                                       int b, int B, int T, int J, float* loss, const FootGuide& fg, const FootFrame& ff) {
+                                       int b, int B, int T, int J, float* loss, const FootGuide& fg, const FootFrame& ff,
+                                       const SceneGuide& sg) {
   const int t = threadIdx.x;
   const bool act = t < T;
   const float* tg = g.target + static_cast<size_t>(b) * J * 3 * T + t;
@@ -256,7 +326,7 @@ __device__ void joint_guidance_iterate(float* xs, const float* mu, const float* 
     float gpx = 0.f, gpz = 0.f, gyaw = 0.f;
     double lsum = 0.0;
     if constexpr (FOOT) {
-      foot_iterate(xs, mu, sd, g, fg, ff, tg, wt, T, J, upd, c, s, wx, wz, px, pz, &gpx, &gpz, &gyaw, &lsum);
+      foot_iterate<SCENE>(xs, mu, sd, g, fg, ff, tg, wt, T, J, upd, c, s, wx, wz, px, pz, &gpx, &gpz, &gyaw, &lsum, sg, b);
     } else if (act) {
       for (int j = 0; j < J; ++j) {
         const float w = __ldcg(wt + static_cast<size_t>(j) * T);
@@ -322,9 +392,9 @@ __device__ void joint_guidance_iterate(float* xs, const float* mu, const float* 
 
 // The guidance of one motion around joint_guidance_iterate: shared memory carved, ric features of x0 [B, D, T] loaded
 // (through L2: x0 was written by the kernel before).  Returns the shared-memory view of the guided features.
-template <bool FOOT>
-__device__ __forceinline__ float* joint_guidance_run(const JointGuide& g, const FootGuide& fg, const float* x0, int B, int T,
-                                                     int D, float* loss) {
+template <bool FOOT, bool SCENE>
+__device__ __forceinline__ float* joint_guidance_run(const JointGuide& g, const FootGuide& fg, SceneGuide sg, const float* x0,
+                                                     int B, int T, int D, float* loss) {
   extern __shared__ double jg_smem[];
   const int J = D == 263 ? 22 : 21, R = 4 + 3 * (J - 1), b = blockIdx.x;
   double* sh = jg_smem;
@@ -357,11 +427,14 @@ __device__ __forceinline__ float* joint_guidance_run(const JointGuide& g, const 
       ff.kap[k] = kap;
     }
     ff.floor = fg.floor_w > 0.f && t < L;
+    if constexpr (SCENE) {
+      if (t >= L) sg.obstacle_w = 0.f;   // the obstacles act on frames t < L
+    }
     ff.nb = gv + 2 * T;
     ff.cd = ff.nb + FG_NB * FG_LD;
   }
   __syncthreads();
-  joint_guidance_iterate<FOOT>(xs, mu, sd, gv, sh, g, b, B, T, J, loss, fg, ff);
+  joint_guidance_iterate<FOOT, SCENE>(xs, mu, sd, gv, sh, g, b, B, T, J, loss, fg, ff, sg);
   return xs;
 }
 
@@ -386,23 +459,46 @@ __device__ __forceinline__ FootGuide load_foot_guide(const FootGuide* d) {
   f.floor_h = __ldcg(&d->floor_h);
   return f;
 }
+__device__ __forceinline__ SceneGrid load_scene_grid(const SceneGrid* d) {
+  SceneGrid G;
+  G.v = reinterpret_cast<const float*>(__ldcg(reinterpret_cast<const unsigned long long*>(&d->v)));
+  G.stride = __ldcg(&d->stride);
+  G.gz = __ldcg(&d->gz);
+  G.gx = __ldcg(&d->gx);
+  G.x0 = __ldcg(&d->x0);
+  G.z0 = __ldcg(&d->z0);
+  G.cell = __ldcg(&d->cell);
+  return G;
+}
+__device__ __forceinline__ SceneGuide load_scene_guide(const SceneGuide* d) {
+  SceneGuide s;
+  s.sdf = load_scene_grid(&d->sdf);
+  s.terrain = load_scene_grid(&d->terrain);
+  s.obstacle_w = __ldcg(&d->obstacle_w);
+  s.margin = __ldcg(&d->margin);
+  return s;
+}
 
 // The guided step of motion blockIdx.x: x0 (the output projection + bias after the CFG blend, [B, D, T], written by the
 // MODE_X0 output GEMM) -> guidance -> the output step's tail (inpainting, clamp, the DDPM / DDIM update of p.mode) for
 // every element of the motion, reading the step's noise as OutStep does.  grid = B, block = JG_THREADS,
 // dynamic shared memory jg_smem_bytes(T, R) (FOOT: fg_smem_bytes(T, R)).  FOOT asks for one CTA per SM (the B CTAs
 // never share one at B <= 132), which lifts the register cap ptxas otherwise picks and keeps the step free of spills.
-template <bool FOOT>
+// SCENE (only with FOOT) adds the scene terms.
+template <bool FOOT, bool SCENE>
 __global__ void __launch_bounds__(JG_THREADS, FOOT ? 1 : 0) joint_guidance_step_kernel(const GuideDesc* guide, const float* x0,
                                                                          const EpiOutParams p) {
+  static_assert(FOOT || !SCENE, "the scene terms extend the foot family");
   pdl_launch_dependents();
   pdl_wait();
   const int T = p.T, D = p.J, b = blockIdx.x, t = threadIdx.x;
   const JointGuide g = load_joint_guide(&guide->j);
   FootGuide fg{};
   if constexpr (FOOT) fg = load_foot_guide(&guide->f);
+  SceneGuide sg{};
+  if constexpr (SCENE) sg = load_scene_guide(&guide->s);
   const int R = D == 263 ? 67 : 64;
-  const float* xs = joint_guidance_run<FOOT>(g, fg, x0, p.B, T, D, nullptr);
+  const float* xs = joint_guidance_run<FOOT, SCENE>(g, fg, sg, x0, p.B, T, D, nullptr);
   if (t >= T) return;
   const OutStep u(p, b);
   const size_t base = static_cast<size_t>(b) * D * T + t;
@@ -413,13 +509,16 @@ __global__ void __launch_bounds__(JG_THREADS, FOOT ? 1 : 0) joint_guidance_step_
   }
 }
 
-// b200mdm_test_joint_guidance / b200mdm_test_foot_guidance (FOOT): the guidance alone, x0_out [B, D, T] = guided x0
-// (features past the ric features copied).  fg comes last, so the FOOT = false kernel's parameters keep their offsets.
-template <bool FOOT>
+// b200mdm_test_joint_guidance / b200mdm_test_foot_guidance (FOOT) / b200mdm_test_scene_guidance (SCENE): the guidance
+// alone, x0_out [B, D, T] = guided x0 (features past the ric features copied).  fg and sg come last, so the FOOT = false
+// kernel's parameters keep their offsets.
+template <bool FOOT, bool SCENE>
 __global__ void __launch_bounds__(JG_THREADS) joint_guidance_test_kernel(const JointGuide g, const float* x0, float* x0_out,
-                                                                         float* loss, int B, int T, int D, const FootGuide fg) {
+                                                                         float* loss, int B, int T, int D, const FootGuide fg,
+                                                                         const SceneGuide sg) {
+  static_assert(FOOT || !SCENE, "the scene terms extend the foot family");
   const int R = D == 263 ? 67 : 64, b = blockIdx.x;
-  const float* xs = joint_guidance_run<FOOT>(g, fg, x0, B, T, D, loss);
+  const float* xs = joint_guidance_run<FOOT, SCENE>(g, fg, sg, x0, B, T, D, loss);
   const size_t base = static_cast<size_t>(b) * D * T;
   for (int i = threadIdx.x; i < D * T; i += blockDim.x) x0_out[base + i] = i < R * T ? xs[i] : x0[base + i];
 }

@@ -255,6 +255,7 @@ class GaussianDiffusion:
         r = resolve(model)
         joint = r.wrapper.targets(y, shape) if r.kind == "joint" else None
         contact = r.wrapper.foot_contact(y, shape) if r.kind == "joint" else None
+        scene = r.wrapper.scene(y, shape) if r.kind == "joint" else None
         if r.kind == "multi":
             r.wrapper.prompts(y, shape)              # y's prompts checked before any engine work
         eng, guided = engine_for(model)
@@ -273,9 +274,11 @@ class GaussianDiffusion:
             jc = r.wrapper
             eng.set_joint_guidance(jc.mean.to(device), jc.std.to(device), joint[0].to(device), joint[1].to(device),
                                    jc.step_size, jc.n_iters)
-            if jc.foot:
+            if jc.foot or scene is not None:     # (both weights 0 with a scene: its lengths)
                 eng.set_foot_guidance(jc.contact_weight, jc.floor_weight, jc.floor_height,
                                       None if contact is None else contact.to(device), y.get("lengths"))
+            if scene is not None:
+                eng.set_scene_guidance(jc.obstacle_weight, jc.obstacle_margin, *scene)
         if table == "next":
             eng.set_schedule_next(self.schedule_next_rows(), key=(id(self), self.num_timesteps))
         elif table == "dpm":

@@ -92,6 +92,41 @@ def foot_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weigh
     return out, loss
 
 
+def _grid(grid, device):
+    """(b200mdm_grid, the fp32 values on `device` it points to) of a SceneGrid, or (None, None)"""
+    if grid is None:
+        return None, None
+    v = grid.values.to(device=device, dtype=torch.float32).contiguous()
+    gz, gx = grid.shape
+    return _lib.Grid(v.data_ptr(), gz * gx if grid.per_sample else 0, gz, gx, grid.origin[0], grid.origin[1], grid.cell), v
+
+
+def _grid_ref(g):
+    return None if g is None else ctypes.byref(g)
+
+
+def scene_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weight, floor_weight, floor_height,
+                        obstacle_weight, obstacle_margin, sdf=None, terrain=None, contact=None, lengths=None):
+    """The guidance iterations with the foot and scene terms alone (b200mdm_test_scene_guidance), on x0's device:
+    (guided x0 [B, D, T], total G [iters + 1, B]).  sdf / terrain: SceneGrid or None; contact, lengths as
+    foot_guidance_hook's."""
+    lib = _lib.load()
+    x0, mean, std, target, weight = (t.to(torch.float32).contiguous() for t in (x0, mean, std, target, weight))
+    B, D, T = int(x0.shape[0]), int(x0.shape[1]), int(x0.shape[-1])
+    kappa = None if contact is None else contact.to(device=x0.device, dtype=torch.float32).contiguous()
+    n = _lengths_host(lengths, B)
+    (gs, vs), (gt, vt) = _grid(sdf, x0.device), _grid(terrain, x0.device)
+    out = torch.empty_like(x0)
+    loss = torch.empty((int(iters) + 1, B), device=x0.device, dtype=torch.float32)
+    check(lib.b200mdm_test_scene_guidance(_ptr(x0), _ptr(mean), _ptr(std), _ptr(target), _ptr(weight),
+                                          None if kappa is None else _ptr(kappa),
+                                          None if n is None else n.ctypes.data_as(ctypes.c_void_p), B, T, D, float(step),
+                                          int(iters), float(contact_weight), float(floor_weight), float(floor_height),
+                                          float(obstacle_weight), float(obstacle_margin), _grid_ref(gs), _grid_ref(gt),
+                                          _ptr(out), _ptr(loss), _stream()))
+    return out, loss
+
+
 class Engine:
     """One engine per model instance (weights + workspace live on the current CUDA device)."""
 
@@ -389,6 +424,7 @@ class Engine:
         check(self.lib.b200mdm_set_joint_guidance(self.h, *[_ptr(t) for t in ts], float(step), int(iters), _stream()))
         self._keep["joint"] = ts
         self._keep.pop("foot", None)
+        self._keep.pop("scene", None)
 
     def set_foot_guidance(self, contact_weight, floor_weight, floor_height=0.0, contact=None, lengths=None):
         """The foot-contact and floor terms of the joint guidance set last (b200mdm_set_foot_guidance), which
@@ -400,6 +436,17 @@ class Engine:
                                                  None if kappa is None else _ptr(kappa),
                                                  None if n is None else n.ctypes.data_as(ctypes.c_void_p), _stream()))
         self._keep["foot"] = kappa
+        self._keep.pop("scene", None)
+
+    def set_scene_guidance(self, obstacle_weight, obstacle_margin, sdf=None, terrain=None):
+        """The scene terms of the joint guidance set last (b200mdm_set_scene_guidance), after set_foot_guidance (whose
+        lengths and floor they use), which set_joint_guidance, set_foot_guidance and set_cond clear: sdf / terrain
+        SceneGrid or None, copied to the engine's device."""
+        dev = torch.device("cuda", torch.cuda.current_device())
+        (gs, vs), (gt, vt) = _grid(sdf, dev), _grid(terrain, dev)
+        check(self.lib.b200mdm_set_scene_guidance(self.h, float(obstacle_weight), float(obstacle_margin), _grid_ref(gs),
+                                                  _grid_ref(gt), _stream()))
+        self._keep["scene"] = (vs, vt)
 
     def set_cond_multi(self, batch, nframes, y, embed, action, weight, device):
         """Multi-prompt guidance (b200mdm_set_cond_multi / _dec / _tokens, then b200mdm_set_prompt_weight): embed fp32

@@ -19,6 +19,7 @@ import torch
 import torch.distributed as dist
 
 from .utils.sampler_util import resolve
+from .utils.scene import SceneGrid
 
 
 def shard_range(global_batch, rank, world):
@@ -92,6 +93,8 @@ def shard_model_kwargs(model_kwargs, lo, hi):
             out[k] = (tok[:, lo:hi].contiguous() if tok.shape[1] > 1 else tok, msk[lo:hi].contiguous() if msk.shape[0] > 1 else msk)
         elif k in _BATCH_KEYS and torch.is_tensor(v):
             out[k] = v[lo:hi].contiguous()
+        elif k in ("obstacle_sdf", "terrain") and isinstance(v, SceneGrid):  # per-sample grids; a shared one as it is
+            out[k] = v.shard(lo, hi)
         elif k in ("text", "tokens", "target_joint_names", "prompt_text") and isinstance(v, (list, tuple)):
             out[k] = list(v[lo:hi])
         elif k in ("target_cond", "is_heading", "target_joint_names", "motion_start") and isinstance(v, np.ndarray):

@@ -7,6 +7,7 @@ import torch.nn as nn
 
 from ..model.mdm import MDM, _run_model
 from .misc import wrapped_getattr
+from .scene import SceneGrid
 
 
 class _SampleWrapper(nn.Module):
@@ -167,10 +168,18 @@ class JointControlSampleModel(_SampleWrapper):
     features (HumanML3D 7, 10, 8, 11; KIT 19, 20, 14, 15), kappa = y['foot_contact'] [B, 4, T] (float >= 0 or bool) or,
     without it, 1 where the step's own de-normalised x0 has contact feature k > 0.5 at frame t and t + 1 < lengths[b];
     `floor_weight` adds 1/2 floor_weight sum_{t < lengths[b], j} min(p[t,j].y - floor_height, 0)^2.  With either weight
-    > 0, y['joint_target'] / y['joint_weight'] are optional (absent: no joint term)."""
+    > 0, y['joint_target'] / y['joint_weight'] are optional (absent: no joint term).
+
+    Scene (DESIGN.md "Joint-position control", "Scene: obstacles and uneven ground"): `obstacle_weight` adds
+    1/2 obstacle_weight sum_{t < lengths[b], j} max(obstacle_margin - S(p[t,j].x, p[t,j].z), 0)^2 with S = y['obstacle_sdf'],
+    a SceneGrid of the obstacles' 2D signed distance (positive outside; SceneGrid.from_shapes builds it for discs and
+    boxes), and y['terrain'], a SceneGrid of heights, raises the floor to floor_height + H(p.x, p.z).  Either grid is
+    shared by the batch or has one grid per sample.  With obstacle_weight > 0, y['joint_target'] / y['joint_weight'] are
+    optional."""
     kind = "joint"
 
-    def __init__(self, model, mean, std, step_size, n_iters, *, contact_weight=0.0, floor_weight=0.0, floor_height=0.0):
+    def __init__(self, model, mean, std, step_size, n_iters, *, contact_weight=0.0, floor_weight=0.0, floor_height=0.0,
+                 obstacle_weight=0.0, obstacle_margin=0.0):
         core = _core(model)
         if core is None:
             raise TypeError("JointControlSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(model))
@@ -195,11 +204,16 @@ class JointControlSampleModel(_SampleWrapper):
             raise ValueError("contact_weight and floor_weight must be finite and >= 0 (got %r, %r)" % (contact_weight, floor_weight))
         if not np.isfinite(fh):
             raise ValueError("floor_height must be finite (got %r)" % (floor_height,))
+        ow, om = float(obstacle_weight), float(obstacle_margin)
+        if not (np.isfinite(ow) and ow >= 0 and np.isfinite(om) and om >= 0):
+            raise ValueError("obstacle_weight and obstacle_margin must be finite and >= 0 (got %r, %r)"
+                             % (obstacle_weight, obstacle_margin))
         super().__init__(model)
         self.mean, self.std = mean, std
         self.step_size, self.n_iters = step, int(iters)
         self.n_joints = 22 if D == 263 else 21
         self.contact_weight, self.floor_weight, self.floor_height = cw, fw, fh
+        self.obstacle_weight, self.obstacle_margin = ow, om
 
     @property
     def foot(self):
@@ -211,7 +225,7 @@ class JointControlSampleModel(_SampleWrapper):
         missing key, a shape other than these, a weight that is negative or not finite, or a target that is not finite
         where its weight is not 0."""
         B, T, J = int(shape[0]), int(shape[-1]), self.n_joints
-        if self.foot and "joint_target" not in y and "joint_weight" not in y:
+        if (self.foot or self.obstacle_weight > 0) and "joint_target" not in y and "joint_weight" not in y:
             return torch.zeros(B, J, 3, T), torch.zeros(B, J, T)      # no joint term: a target the kernel never reads
         if "joint_target" not in y or "joint_weight" not in y:
             raise ValueError("JointControlSampleModel needs y['joint_target'] [B, %d, 3, T] and y['joint_weight'] [B, %d, T]"
@@ -249,6 +263,27 @@ class JointControlSampleModel(_SampleWrapper):
         if not bool((torch.isfinite(k) & (k >= 0)).all()):
             raise ValueError("y['foot_contact'] must be finite and >= 0")
         return k
+
+    def scene(self, y, shape):
+        """(obstacle sdf, terrain) of y, each a SceneGrid or None, or None when no scene term applies; y is not
+        modified.  y['obstacle_sdf'] is read when obstacle_weight > 0, y['terrain'] when present.  ValueError for an
+        obstacle weight without y['obstacle_sdf'], a terrain with floor_weight 0, a value that is not a SceneGrid, or a
+        per-sample grid whose batch is not the sample's."""
+        B = int(shape[0])
+        sdf = y.get("obstacle_sdf") if self.obstacle_weight > 0 else None
+        terrain = y.get("terrain")
+        if self.obstacle_weight > 0 and sdf is None:
+            raise ValueError("obstacle_weight > 0 needs y['obstacle_sdf'] (a SceneGrid)")
+        if terrain is not None and self.floor_weight == 0:
+            raise ValueError("y['terrain'] needs floor_weight > 0")
+        for name, g in (("obstacle_sdf", sdf), ("terrain", terrain)):
+            if g is None:
+                continue
+            if not isinstance(g, SceneGrid):
+                raise ValueError("y[%r] must be a b200mdm.SceneGrid (got %r)" % (name, type(g)))
+            if g.per_sample and g.values.shape[0] != B:
+                raise ValueError("y[%r] has %d grids for %d samples" % (name, g.values.shape[0], B))
+        return None if sdf is None and terrain is None else (sdf, terrain)
 
     def forward(self, x, timesteps, y=None):
         return self.model(x, timesteps, y)
