@@ -435,6 +435,30 @@ int b200mdm_chain_setup(b200mdm_engine* e, int32_t n_chunks, int32_t pred_len, i
 int b200mdm_chain_loop_range(b200mdm_engine* e, int32_t mode, int32_t order, int32_t first_step, int32_t n_run,
                              const float* x_T_dev, int64_t x_T_chunk_stride, const float* noise_tape_dev,
                              int64_t noise_step_stride, float* out_dev, int32_t flags, int32_t use_graph, void* stream);
+/* Goals in the world frame for the chain set up last (DESIGN.md, "Goals in the world frame"), called after
+ * b200mdm_chain_setup and before its first b200mdm_chain_loop_range.  goal_dev [n_goals, batch, n_ext, 3] fp32 device
+ * (n_ext = target_joints, the extended joint list in target_cond's layout; n_goals 1: one goal for the whole chain, or
+ * n_chunks: chunk c aims at goal c) and valid_host uint8 [batch, n_ext] as b200mdm_set_target takes them; mean_dev /
+ * std_dev [JF] the dataset normalisation.  W is the frame of recover_from_ric on the chain's output (the prefix starts it
+ * under include_prefix, else chunk 0's first frame at yaw 0); chunk c is conditioned on its goal re-expressed in its own
+ * frame (b200mdm_chunk_frame), computed on the device after chunk c - 1's hand-off from the carry of every frame before
+ * it (two launches per chunk boundary).  Chunk 0's carry covers the b200mdm_set_prefix prefix under include_prefix (which
+ * must still be alive), else nothing, so its target is then the goal itself.  The goals, mean and std must stay alive
+ * until the chain has run.  B200MDM_EINVAL for a null argument, an engine without a target encoder or prefix, or n_goals
+ * other than 1 and n_chunks; B200MDM_ESTATE unless a chain was set up and has not run yet.  b200mdm_chain_setup and
+ * everything that ends a chain end the goals. */
+int b200mdm_chain_set_goal(b200mdm_engine* e, const float* mean_dev, const float* std_dev, const float* goal_dev,
+                           int32_t n_goals, const uint8_t* valid_host, void* stream);
+/* One chunk boundary of a goal-directed chain, without an engine: advance carry_dev [batch, 6] fp64 (yaw, root P.x, P.z,
+ * the last frame's root velocity x, z, and 1.0 once a frame was seen; zeros at the start of W) over frames_dev
+ * [batch, n_feats, n_frames] (normalised features; n_frames 0 .. 256, 0 advances nothing), then write target_dev
+ * [batch, n_ext, 3]: goal_dev [batch, n_ext, 3] in the frame of the frame after the last one seen (positions: XZ
+ * translated and rotated, y unchanged; the heading entry n_ext - 1: wrap(heading + 2 yaw) in (-pi, pi], its components
+ * 1 and 2 unchanged).  B200MDM_EINVAL before any CUDA call for a null pointer (frames may be NULL with 0 frames),
+ * batch <= 0, n_feats < 4, n_frames outside 0 .. 256 or n_ext outside 2 .. 64. */
+int b200mdm_chunk_frame(double* carry_dev, const float* frames_dev, int32_t batch, int32_t n_feats, int32_t n_frames,
+                        const float* mean_dev, const float* std_dev, const float* goal_dev, int32_t n_ext, float* target_dev,
+                        void* stream);
 
 /* The variational lower bound (calc_bpd_loop, gaussian_diffusion.py:1544-1599) at schedule indices first_index,
  * first_index-1, ... (n_run of them), each step one forward (one CUDA graph, replayed, when use_graph != 0):

@@ -39,7 +39,7 @@ SYMBOLS = [
     "b200mdm_chain_setup", "b200mdm_chain_loop_range", "b200mdm_set_joint_guidance", "b200mdm_test_joint_guidance",
     "b200mdm_set_cond_multi", "b200mdm_set_cond_multi_dec", "b200mdm_set_prompt_weight",
     "b200mdm_set_cond_multi_tokens", "b200mdm_set_foot_guidance", "b200mdm_test_foot_guidance",
-    "b200mdm_set_scene_guidance", "b200mdm_test_scene_guidance",
+    "b200mdm_set_scene_guidance", "b200mdm_test_scene_guidance", "b200mdm_chain_set_goal", "b200mdm_chunk_frame",
 ]
 MAX_PROMPTS = 8                             # B200MDM_MAX_PROMPTS
 MAX_MEMORY_TOKENS = 512                     # a BERT text memory holds 1 .. 512 tokens (DistilBERT's position limit)
@@ -151,7 +151,9 @@ def load():
                        ("b200mdm_set_cond_multi", [vp, i32, i32, i32, vp, vp, vp, vp]),
                        ("b200mdm_set_cond_multi_dec", [vp, i32, i32, i32, vp, vp, vp]),
                        ("b200mdm_set_cond_multi_tokens", [vp, i32, i32, i32, vp, vp, i32, vp, vp]),
-                       ("b200mdm_set_prompt_weight", [vp, i32, vp, i64, i64, i64, i64, vp])):
+                       ("b200mdm_set_prompt_weight", [vp, i32, vp, i64, i64, i64, i64, vp]),
+                       ("b200mdm_chain_set_goal", [vp, vp, vp, vp, i32, vp, vp]),
+                       ("b200mdm_chunk_frame", [vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

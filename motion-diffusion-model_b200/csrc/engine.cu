@@ -23,6 +23,7 @@
 #include "gemm.cuh"
 #include "gemm_ln.cuh"
 #include "gemm_pingpong.cuh"
+#include "chunk_frame.cuh"
 #include "joint_guidance.cuh"
 #include "compose.cuh"
 #include "postprocess.cuh"
@@ -308,6 +309,17 @@ struct b200mdm_engine : Workspace {
   std::vector<unsigned char> h_chain_mask;
   int chain_n = 0, chain_off = 0, chain_crop = 0, chain_next = -1;
   bool chain_mems = false;
+  // the prefix of b200mdm_set_prefix (caller-owned), which b200mdm_chain_set_goal reads under include_prefix
+  const float* prefix_src = nullptr;
+  // a goal-directed chain (b200mdm_chain_set_goal): the caller's mean / std [JF] and goals [n_goals, B, n_ext, 3], the
+  // per-sample carry [B, CF_CARRY] and the next chunk's target [B, n_ext, 3]; live while goal_set and the chain is
+  // (chain_setup clears goal_set, and everything that ends a chain sets chain_next = -1)
+  const float *goal_mean = nullptr, *goal_std = nullptr, *goal_src = nullptr;
+  double* goal_carry = nullptr;
+  float* goal_tgt = nullptr;
+  size_t goal_carry_cap = 0, goal_tgt_cap = 0;
+  int goal_n = 0;
+  bool goal_set = false;
 };
 
 template <class T>
@@ -716,6 +728,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   for (float*& t : e->tab) dfree(t);
   dfree(e->tmap);
   dfree(e->chain_mem); dfree(e->chain_mask); dfree(e->chain_prefix);
+  dfree(e->goal_carry); dfree(e->goal_tgt);
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
   dfree(e->jg_desc);
@@ -875,19 +888,24 @@ static int pack_target_weights(b200mdm_engine* e, cudaStream_t s) {
   return B200MDM_OK;
 }
 
-// g [B, d] = embed_target_cond(target [B, n, 3], valid) on stream s; valid_dev [B, n] receives the validity as fp32
-// (staged through `staging`, which must stay alive until the copy has run)
-static int encode_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, int B, float* valid_dev,
-                         float* g_dev, std::vector<float>& staging, cudaStream_t s) {
+// g [B, d] = embed_target_cond(target [B, n, 3], valid_dev [B, n] fp32) on stream s
+static int embed_target(b200mdm_engine* e, const float* target_dev, const float* valid_dev, int B, float* g_dev, cudaStream_t s) {
   const int n = e->cfg.target_joints, d = e->d;
-  staging.assign(static_cast<size_t>(B) * n, 0.f);
-  for (size_t i = 0; i < staging.size(); ++i) staging[i] = valid_host[i] ? 1.f : 0.f;
-  CUDA_TRY(cudaMemcpyAsync(valid_dev, staging.data(), staging.size() * sizeof(float), cudaMemcpyHostToDevice, s));
   const size_t smem = sizeof(float) * (4 * n + 2 * d);
   target_embed_kernel<<<B, d, smem, s>>>(target_dev, valid_dev, e->tw0, e->tb0, e->twk, e->tbk, e->twsum, g_dev, n, e->tG,
                                          e->tdj, e->tin, e->tlayers, e->cfg.target_encoder == B200MDM_TARGET_MULTI ? 1 : 0);
   CUDA_TRY(cudaGetLastError());
   return B200MDM_OK;
+}
+// ... with the validity from the host: valid_dev receives it as fp32 (staged through `staging`, which must stay alive
+// until the copy has run)
+static int encode_target(b200mdm_engine* e, const float* target_dev, const uint8_t* valid_host, int B, float* valid_dev,
+                         float* g_dev, std::vector<float>& staging, cudaStream_t s) {
+  const int n = e->cfg.target_joints;
+  staging.assign(static_cast<size_t>(B) * n, 0.f);
+  for (size_t i = 0; i < staging.size(); ++i) staging[i] = valid_host[i] ? 1.f : 0.f;
+  CUDA_TRY(cudaMemcpyAsync(valid_dev, staging.data(), staging.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+  return embed_target(e, target_dev, valid_dev, B, g_dev, s);
 }
 
 extern "C" int b200mdm_finalize_weights(b200mdm_engine* e, void* stream) {
@@ -1543,6 +1561,7 @@ extern "C" int b200mdm_set_prefix(b200mdm_engine* e, const float* prefix_dev, vo
   TRY(launch_pack_input(prefix_dev, e->xin16, e->B, e->JF, e->ctx, e->S, e->Kp_in, 0, static_cast<cudaStream_t>(stream)));
   e->launches++;
   e->prefix_set = true;
+  e->prefix_src = prefix_dev;
   e->chain_next = -1;   // a chain's prefix rows were replaced
   return B200MDM_OK;
 }
@@ -2480,9 +2499,70 @@ extern "C" int b200mdm_chain_setup(b200mdm_engine* e, int32_t n_chunks, int32_t 
       TRY(build_text_memory(e, enc_chunks_dev + static_cast<size_t>(c) * Mt * B * C, 1, e->mem_uncond, e->chain_mem + c * mem, s));
   }
   e->chain_n = n_chunks;
+  e->goal_set = false;
   e->chain_off = include_prefix ? context_len : 0;
   e->chain_crop = crop;
   e->chain_next = 0;
+  return B200MDM_OK;
+}
+
+// ---- goal-directed chains (chunk_frame.cuh)
+static int check_chunk_frame(const void* carry, const void* frames, int B, int D, int n, const void* mean, const void* std,
+                             const void* goal, int n_ext, const void* target) {
+  if (!carry || (!frames && n > 0) || !mean || !std || !goal || !target) return fail(B200MDM_EINVAL, "null argument");
+  if (B <= 0 || D < 4 || n < 0 || n > JG_MAX_FRAMES || n_ext < 2 || n_ext > 64)
+    return fail(B200MDM_EINVAL, "batch %d, %d features, %d frames, %d goal entries: batch >= 1, >= 4 features, 0 .. %d frames "
+                "and 2 .. 64 entries", B, D, n, n_ext, JG_MAX_FRAMES);
+  return B200MDM_OK;
+}
+static int launch_chunk_frame(double* carry, const float* frames, int B, int D, int n, const float* mean, const float* std,
+                              const float* goal, int n_ext, float* target, cudaStream_t s) {
+  chunk_frame_kernel<<<B, JG_THREADS, 0, s>>>(frames, D, n, mean, std, carry, goal, n_ext, target);
+  CUDA_TRY(cudaGetLastError());
+  return B200MDM_OK;
+}
+// chunk c's goal rows [B, n_ext, 3]: one goal for the whole chain, or one per chunk
+static const float* goal_row(const b200mdm_engine* e, int c) {
+  return e->goal_src + (e->goal_n == 1 ? 0 : static_cast<size_t>(c) * e->B * e->cfg.target_joints * 3);
+}
+
+extern "C" int b200mdm_chunk_frame(double* carry_dev, const float* frames_dev, int32_t batch, int32_t n_feats,
+                                   int32_t n_frames, const float* mean_dev, const float* std_dev, const float* goal_dev,
+                                   int32_t n_ext, float* target_dev, void* stream) {
+  TRY(check_chunk_frame(carry_dev, frames_dev, batch, n_feats, n_frames, mean_dev, std_dev, goal_dev, n_ext, target_dev));
+  return launch_chunk_frame(carry_dev, frames_dev, batch, n_feats, n_frames, mean_dev, std_dev, goal_dev, n_ext, target_dev,
+                            static_cast<cudaStream_t>(stream));
+}
+
+// Goals for the chain set up last: chunk 0's carry (over the prefix under include_prefix, else none) and target, then
+// its embedding into the workspace's target, which every step graph of the chain reads.
+extern "C" int b200mdm_chain_set_goal(b200mdm_engine* e, const float* mean_dev, const float* std_dev, const float* goal_dev,
+                                      int32_t n_goals, const uint8_t* valid_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!mean_dev || !std_dev || !goal_dev || !valid_host) return fail(B200MDM_EINVAL, "null argument");
+  if (e->cfg.target_encoder == B200MDM_TARGET_NONE) return fail(B200MDM_EINVAL, "this engine has no target encoder");
+  if (!is_prefix_engine(e)) return fail(B200MDM_EINVAL, "the chain is for prefix-completion (DiP) engines");
+  if (e->chain_next != 0) return fail(B200MDM_ESTATE, "b200mdm_chain_setup first (a goal is set before the chain runs)");
+  if (n_goals != 1 && n_goals != e->chain_n)
+    return fail(B200MDM_EINVAL, "%d goals: one for the whole chain or one per chunk (%d)", n_goals, e->chain_n);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int B = e->B, n_ext = e->cfg.target_joints;
+  if (e->goal_carry_cap < static_cast<size_t>(B) * CF_CARRY || e->goal_tgt_cap < static_cast<size_t>(B) * n_ext * 3) {
+    CUDA_TRY(cudaDeviceSynchronize());   // a previous chain may still read the buffers being replaced
+  }
+  TRY(ensure_cap(&e->goal_carry, &e->goal_carry_cap, static_cast<size_t>(B) * CF_CARRY));
+  TRY(ensure_cap(&e->goal_tgt, &e->goal_tgt_cap, static_cast<size_t>(B) * n_ext * 3));
+  e->goal_mean = mean_dev;
+  e->goal_std = std_dev;
+  e->goal_src = goal_dev;
+  e->goal_n = n_goals;
+  CUDA_TRY(cudaMemsetAsync(e->goal_carry, 0, static_cast<size_t>(B) * CF_CARRY * sizeof(double), s));
+  TRY(launch_chunk_frame(e->goal_carry, e->prefix_src, B, e->JF, e->chain_off, mean_dev, std_dev, goal_row(e, 0), n_ext,
+                         e->goal_tgt, s));
+  TRY(encode_target(e, e->goal_tgt, valid_host, B, e->tgt_valid, e->tgt_g, e->h_valid, s));
+  e->launches += 2;
+  e->target_set = true;
+  e->goal_set = true;
   return B200MDM_OK;
 }
 
@@ -2515,6 +2595,7 @@ extern "C" int b200mdm_chain_loop_range(b200mdm_engine* e, int32_t mode, int32_t
   if (static_cast<long long>(first_step) + n_run > static_cast<long long>(e->chain_n) * N)
     return fail(B200MDM_EINVAL, "steps %d .. %d past the chain's %d x %d", first_step, first_step + n_run - 1, e->chain_n, N);
   if (dpm) TRY(ensure_dpm(e));
+  const bool goal = e->goal_set;
   const StepArgs a = loop_args(e, mode, order, flags, philox && !dpm);
   cudaStream_t user = static_cast<cudaStream_t>(stream), s;
   TRY(loop_enter(e, a, flags, use_graph, user, &s));
@@ -2560,6 +2641,12 @@ extern "C" int b200mdm_chain_loop_range(b200mdm_engine* e, int32_t mode, int32_t
       if (!last) {
         TRY(launch_pack_input(e->chain_prefix, e->xin16, B, JF, e->ctx, e->S, e->Kp_in, 0, s));
         e->launches += 1;
+      }
+      if (!last && goal) {   // chunk c + 1's target, in its own frame, into the embedding the step graph reads
+        TRY(launch_chunk_frame(e->goal_carry, e->x_work, B, JF, T, e->goal_mean, e->goal_std, goal_row(e, c + 1),
+                               e->cfg.target_joints, e->goal_tgt, s));
+        TRY(embed_target(e, e->goal_tgt, e->tgt_valid, B, e->tgt_g, s));
+        e->launches += 2;
       }
     }
   }

@@ -685,7 +685,8 @@ class GaussianDiffusion:
 
     # ------------------------------------------------------------------ DiP's autoregressive chain
     def _ar_chain(self, mode, model, shape, ys, required_frames, include_prefix, noise=None, clip_denoised=True,
-                  device=None, eta=0.0, order=0, noise_tape=None, use_graph=True, noise_seed=None, sample_index_base=0):
+                  device=None, eta=0.0, order=0, noise_tape=None, use_graph=True, noise_seed=None, sample_index_base=0,
+                  goal=None):
         """AutoRegressiveSampler.sample's chain of len(ys) prefix completions of shape [B, J, F, pred_len] as engine loops
         (DESIGN.md, "Autoregressive chain"), for the p_sample_loop (MODE_DDPM), ddim_sample_loop (MODE_DDIM) or
         dpm_solver_sample_loop (MODE_DPM) keywords utils/sampler_util._chain_plan admits.  ys[c] is chunk c's y without
@@ -695,7 +696,8 @@ class GaussianDiffusion:
         noise / noise_seed's Philox x_T / one torch.randn) and then its steps' eps (noise_tape[c] / Philox / one normal_()
         each, drawn NOISE_CHUNK steps at a time).  Returns [B, J, F, required_frames], or None before any sampling when a later
         chunk's text_embed is not a (tokens, mask) pair or the chunks' memories differ in token count (the host chain
-        runs those, and raises what it raises)."""
+        runs those, and raises what it raises).  goal: (mean, std, goals [n_goals, B, n_ext, 3], validity) of
+        AutoRegressiveSampler's y['target_world'], re-expressed in each chunk's frame on the device."""
         n, N = len(ys), self.num_timesteps
         B, pred = int(shape[0]), int(shape[-1])
         device = self._device(model, device)
@@ -717,6 +719,9 @@ class GaussianDiffusion:
         prefix = ys[0]["prefix"]
         enc = None if mems is None else torch.stack([m[0] for m in mems])
         eng.chain_setup(n, pred, include_prefix, required_frames, enc, None if mems is None else np.stack([m[1] for m in mems]))
+        if goal is not None:
+            mean, std, g, valid = goal
+            eng.chain_set_goal(mean.to(device), std.to(device), g.to(device), valid)
         out = torch.empty(tuple(shape[:-1]) + (required_frames,), device=device, dtype=torch.float32)
         if include_prefix:
             out[..., :ctx] = prefix[..., :min(ctx, required_frames)]

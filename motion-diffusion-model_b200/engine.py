@@ -594,6 +594,29 @@ class Engine:
                                            _stream()))
         self._keep["chain"] = (enc_chunks, mask)
 
+    def chain_set_goal(self, mean, std, goal, valid):
+        """Goals in the world frame for the chain set up last (b200mdm_chain_set_goal): mean / std [D], goal
+        [n_goals, B, n_ext, 3] (n_goals 1 or n_chunks) on the engine's device, valid uint8 numpy [B, n_ext]."""
+        mean, std, goal = (t.to(torch.float32).contiguous() for t in (mean, std, goal))
+        valid = np.ascontiguousarray(valid, dtype=np.uint8)
+        check(self.lib.b200mdm_chain_set_goal(self.h, _ptr(mean), _ptr(std), _ptr(goal), int(goal.shape[0]),
+                                              valid.ctypes.data_as(ctypes.c_void_p), _stream()))
+        self._keep["goal"] = (mean, std, goal)
+
+    @staticmethod
+    def chunk_frame(carry, frames, mean, std, goal):
+        """One chunk boundary of a goal-directed chain (b200mdm_chunk_frame): advances carry [B, 6] fp64 (in place) over
+        frames [B, D, ..., n] (normalised; n may be 0) and returns goal [B, n_ext, 3] in the frame of the next frame."""
+        lib = _lib.load()
+        assert carry.dtype == torch.float64 and carry.is_contiguous()
+        B, D, n = int(frames.shape[0]), int(frames.shape[1]), int(frames.shape[-1])
+        frames = frames.to(torch.float32).reshape(B, D, n).contiguous()
+        mean, std, goal = (t.to(torch.float32).contiguous() for t in (mean, std, goal))
+        out = torch.empty_like(goal)
+        check(lib.b200mdm_chunk_frame(_ptr(carry), _ptr(frames) if n > 0 else None, B, D, n, _ptr(mean), _ptr(std),
+                                      _ptr(goal), int(goal.shape[1]), _ptr(out), _stream()))
+        return out
+
     def chain_loop_range(self, mode, order, first_step, n_run, x_T, noise, out, flags=0, use_graph=True):
         """Global steps first_step .. first_step+n_run-1 of the chain (b200mdm_chain_loop_range).  x_T [n_chunks, ...]
         one per chunk, [...] one for every chunk, or None (the Philox x_T); noise [>= n_run, ...] or None (Philox eps, or

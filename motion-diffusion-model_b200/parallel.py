@@ -91,6 +91,8 @@ def shard_model_kwargs(model_kwargs, lo, hi):
         elif k == "text_embed" and isinstance(v, tuple):                     # DiP: (tokens [Mt, B, C], mask [B, Mt])
             tok, msk = v
             out[k] = (tok[:, lo:hi].contiguous() if tok.shape[1] > 1 else tok, msk[lo:hi].contiguous() if msk.shape[0] > 1 else msk)
+        elif k == "target_world" and torch.is_tensor(v):                     # [B, n_ext, 3] or [n_chunks, B, n_ext, 3]
+            out[k] = (v[lo:hi] if v.dim() == 3 else v[:, lo:hi]).contiguous()
         elif k in _BATCH_KEYS and torch.is_tensor(v):
             out[k] = v[lo:hi].contiguous()
         elif k in ("obstacle_sdf", "terrain") and isinstance(v, SceneGrid):  # per-sample grids; a shared one as it is

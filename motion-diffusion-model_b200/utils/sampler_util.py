@@ -650,12 +650,48 @@ class AutoRegressiveSampler:
     (_chain_plan), the whole chain runs as engine loops: the conditioning is set once, and the prefix hand-off between
     chunks happens on the device, with the same result bit for bit (DESIGN.md, "Autoregressive chain").  Any other
     sample_fn runs here on the host, one `sample_fn` call per chunk.  The caller's kwargs are never mutated (the
-    reference deep-copies them per chunk; here only the dicts that change are rebuilt)."""
+    reference deep-copies them per chunk; here only the dicts that change are rebuilt).
 
-    def __init__(self, args, sample_fn, required_frames=196):
+    Goals in the world frame (DESIGN.md, "Goals in the world frame"): y['target_world'] [B, n_ext, 3] (one goal for the
+    whole chain) or [n_chunks, B, n_ext, 3] (a waypoint per chunk), in target_cond's layout and validity keys, is
+    re-expressed in each chunk's own frame on the device and given to that chunk as its target; mean / std [D] are the
+    dataset normalisation that recover_from_ric needs.  W is the frame of recover_from_ric on the returned motion."""
+
+    def __init__(self, args, sample_fn, required_frames=196, *, mean=None, std=None):
         self.sample_fn = sample_fn
         self.args = args
         self.required_frames = required_frames
+        self.mean, self.std = mean, std
+
+    def _goal(self, model, y, batch, n_chunks):
+        """(goals [n_goals, B, n_ext, 3] fp32, validity uint8 [B, n_ext]) of y['target_world'], or None without it or
+        with y['target_uncond']; ValueError for keys that clash, before any engine work."""
+        if "target_world" not in y:
+            return None
+        if "target_cond" in y:
+            raise ValueError("y['target_world'] and y['target_cond'] both give the target: pass one of them")
+        mdm = resolve(model).mdm
+        if mdm is None or not mdm.multi_target_cond:
+            raise ValueError("y['target_world'] was given, but the model has no target encoder (multi_target_cond=False)")
+        if self.mean is None or self.std is None:
+            raise ValueError("y['target_world'] needs AutoRegressiveSampler(..., mean=, std=), the dataset normalisation")
+        g = y["target_world"]
+        if not torch.is_tensor(g):
+            g = torch.as_tensor(np.asarray(g, dtype=np.float32))
+        n_ext = len(mdm.extended_goal_joint_names)
+        if g.dim() == 3:
+            g = g[None]
+        elif g.dim() != 4 or g.shape[0] != n_chunks:
+            raise ValueError("y['target_world'] must be [B, %d, 3] or [n_chunks = %d, B, %d, 3] (got %s)"
+                             % (n_ext, n_chunks, n_ext, tuple(g.shape)))
+        for v, name in ((self.mean, "mean"), (self.std, "std")):
+            if tuple(v.shape) != (mdm.njoints * mdm.nfeats,):
+                raise ValueError("%s must be [%d] (got %s)" % (name, mdm.njoints * mdm.nfeats, tuple(v.shape)))
+        from ..engine import canonical_target
+        _, valid = canonical_target(dict(y, target_cond=g[0]), batch, mdm.extended_goal_joint_names)
+        if bool(y.get("target_uncond", False)):
+            return None
+        return g.to(torch.float32), valid
 
     def sample(self, model, shape, **kargs):
         if resolve(model).kind == "joint":
@@ -663,6 +699,9 @@ class AutoRegressiveSampler:
         pred_len, context_len = self.args.pred_len, self.args.context_len
         n_iterations = self.required_frames // pred_len + int(self.required_frames % pred_len > 0)
         y0 = kargs["model_kwargs"]["y"]
+        goal = self._goal(model, y0, shape[0], n_iterations)
+        if "target_world" in y0:
+            y0 = {k: v for k, v in y0.items() if k != "target_world"}
         cur_prefix = y0["prefix"].clone()
         dynamic_text_mode = isinstance(y0["text"][0], list) if "text" in y0 else False   # a prompt per chunk
         samples_buf = [cur_prefix] if getattr(self.args, "autoregressive_include_prefix", False) else []
@@ -681,12 +720,23 @@ class AutoRegressiveSampler:
                     y["text_embed"] = (y0["text_embed"][0][:, :, i], y0["text_embed"][1][:, i])
                 ys.append(y)
             diffusion, mode, kw = plan
+            if goal is not None:
+                kw = dict(kw, goal=(self.mean, self.std) + goal)
             out = diffusion._ar_chain(mode, model, ar_shape, ys, self.required_frames, bool(samples_buf), **kw)
             if out is not None:
                 return out
+        if goal is not None:            # the carry stays on the device; each chunk's target is computed there
+            from ..engine import Engine
+            dev = next(model.parameters()).device
+            g, mean, std = (t.to(dev) for t in (goal[0], self.mean, self.std))
+            carry = torch.zeros(shape[0], 6, dtype=torch.float64, device=dev)
+            first = cur_prefix if samples_buf else cur_prefix[..., :0]
+            target = Engine.chunk_frame(carry, first.to(dev), mean, std, g[0])
         for i in range(n_iterations):
             y = dict(y0)
             y["prefix"] = cur_prefix
+            if goal is not None:
+                y["target_cond"] = target
             if dynamic_text_mode:
                 y["text"] = [s[i] for s in y0["text"]]
                 if getattr(model, "text_encoder_type", "bert") != "bert":
@@ -701,4 +751,6 @@ class AutoRegressiveSampler:
             sample = self.sample_fn(model, ar_shape, **cur)
             samples_buf.append(sample[..., -pred_len:].clone())
             cur_prefix = sample[..., -context_len:].clone()
+            if goal is not None and i + 1 < n_iterations:
+                target = Engine.chunk_frame(carry, samples_buf[-1].to(dev), mean, std, g[min(i + 1, g.shape[0] - 1)])
         return torch.cat(samples_buf, dim=-1)[..., :self.required_frames]
