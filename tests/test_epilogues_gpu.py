@@ -335,17 +335,17 @@ def test_out_step(mode, halves, JF, B, T, s_off, flags, inpaint, alias):
     check_x_out(mode, pred, xt0, noise, xout)
 
 
-def check_x_out(mode, pred, xt0, noise, xout):
-    """x_out bit for bit against the float32 update evaluated from the pred_xstart the kernel returned; an FMA-contracted
-    evaluation must differ somewhere."""
+def check_x_out(mode, pred, xt0, noise, xout, row=SCHED_ROW):
+    """x_out bit for bit against the float32 update evaluated from the pred_xstart the kernel returned, with schedule
+    row `row`; an FMA-contracted evaluation must differ somewhere."""
     x0n, xtn = pred.cpu().numpy(), xt0.cpu().numpy()
     nzn = np.broadcast_to(noise.cpu().numpy(), xtn.shape)
-    want = _step_f32(mode, x0n, xtn, nzn, SCHED_ROW)
+    want = _step_f32(mode, x0n, xtn, nzn, row)
     gotx = xout.cpu().numpy()
     diff = int((gotx.view(np.int32) != want.view(np.int32)).sum())
     line = "  x_out: %d of %d elements differ from the float32 evaluation" % (diff, want.size)
     if mode != 0:
-        fm = _step_f32(mode, x0n, xtn, nzn, SCHED_ROW, fma=True)
+        fm = _step_f32(mode, x0n, xtn, nzn, row, fma=True)
         nfm = int((fm.view(np.int32) != want.view(np.int32)).sum())
         line += "; FMA-contracted mutant differs in %d" % nfm
         assert nfm > 0, "the bit-exact check would not see an FMA-contracted update"
