@@ -289,6 +289,28 @@ typedef struct b200mdm_grid {
 int b200mdm_set_scene_guidance(b200mdm_engine* e, float obstacle_weight, float obstacle_margin, const b200mdm_grid* sdf,
                                const b200mdm_grid* terrain, void* stream);
 
+/* Interaction terms of joint-position control (DESIGN.md "Joint-position control", "Several characters in one scene"):
+ * the B motions are B / C scenes of C = `characters` characters (2 <= C <= 8, B % C == 0), motions [sC, sC + C) forming
+ * scene s.  placement_dev fp32 device [B, 3] (x, z, phi) places each motion's own frame in its scene,
+ * Q = rot(phi) p + (x, 0, z) with rot(phi) (x, z) = (x cos phi - z sin phi, x sin phi + z cos phi).  With
+ * L_ab = min(L_a, L_b) (the lengths of b200mdm_set_foot_guidance) and d = |Q_a[t,j] - Q_b[t,k]|, the guided energy adds
+ *   1/2 weight sum_scenes sum_{a<b} sum_{t<L_ab} sum_{j,k} max(margin - d, 0)^2
+ *   + 1/2 sum_n sum_{t<L_ab} w_n[t] max(|Q_{a_n}[t, j_n] - Q_{b_n}[t, k_n]| - reach[n], 0)^2,
+ * on top of the joint, foot and scene terms as set (their weights may be 0).  pairs_host int32 [n_pairs, 4] holds the
+ * scene-local rows (a, j, b, k), a != b, and reach_host fp32 [n_pairs] their distances (both copied); pair_weight_dev
+ * fp32 device [n_pairs, T] >= 0 at pair_weight_dev + s * pair_weight_stride for scene s (stride 0: shared by every
+ * scene).  The avoidance gradient at d = 0 is 0.  The guided step runs as clusters of C CTAs; a bad count, weight,
+ * margin, row, reach or stride returns B200MDM_EINVAL before any CUDA call, a cluster that cannot be resident
+ * B200MDM_ENOTIMPL, and without b200mdm_set_joint_guidance for the current conditioning, B200MDM_ESTATE.  The device
+ * arrays are the caller's, valid until the work enqueued with them has completed.  b200mdm_set_cond*,
+ * b200mdm_set_joint_guidance, b200mdm_set_foot_guidance and b200mdm_set_scene_guidance clear it.  The terms live in the
+ * guidance descriptor, so a step graph captured with them reads new values at every replay. */
+#define B200MDM_MAX_INTERACTION_PAIRS 1024
+int b200mdm_set_interaction_guidance(b200mdm_engine* e, int32_t characters, float weight, float margin,
+                                     const float* placement_dev, const int32_t* pairs_host, int32_t n_pairs,
+                                     const float* reach_host, const float* pair_weight_dev, int64_t pair_weight_stride,
+                                     void* stream);
+
 /* Multi-prompt guidance (this project's definition, DESIGN.md "Multi-prompt guidance"): K prompts per motion, composed
  * around the unconditional prediction as
  *   x0[b, f, t] = x0_u + sum_{k=0..K-1} w[b, k, f, t] (x0_k - x0_u)
@@ -601,6 +623,18 @@ int b200mdm_test_scene_guidance(const float* x0_dev, const float* mean_dev, cons
                                 int32_t T, int32_t D, float step, int32_t iters, float contact_weight, float floor_weight,
                                 float floor_height, float obstacle_weight, float obstacle_margin, const b200mdm_grid* sdf,
                                 const b200mdm_grid* terrain, float* x0_out_dev, float* loss_out_dev, void* stream);
+/* The guidance iterations with the foot, scene and interaction terms alone (joint_guidance_test_kernel<true, true, true>,
+ * in clusters of `characters` CTAs): as b200mdm_test_scene_guidance, with the interaction arguments of
+ * b200mdm_set_interaction_guidance; loss_out receives the total G per motion, each pair's energy at its lower rank.
+ * Invalid arguments return B200MDM_EINVAL before any CUDA call. */
+int b200mdm_test_interaction_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
+                                      const float* weight_dev, const float* contact_dev, const int64_t* lengths_host,
+                                      int32_t B, int32_t T, int32_t D, float step, int32_t iters, float contact_weight,
+                                      float floor_weight, float floor_height, float obstacle_weight, float obstacle_margin,
+                                      const b200mdm_grid* sdf, const b200mdm_grid* terrain, int32_t characters, float weight,
+                                      float margin, const float* placement_dev, const int32_t* pairs_host, int32_t n_pairs,
+                                      const float* reach_host, const float* pair_weight_dev, int64_t pair_weight_stride,
+                                      float* x0_out_dev, float* loss_out_dev, void* stream);
 /* Self-attention core (tensor-core kernel, S <= 256): softmax(q k^T / sqrt(128) + mask) v per (sample, head);
  * qkv16 [n*S, 3d]; kvlen int32 [n] device (valid keys per sample, a prefix).
  * impl 0: out16 fp16 [n*S, d] (the encoder); impl 1: out16 fp16 [n*S, 2d] = [hi | lo] with hi + lo = the fp32 result

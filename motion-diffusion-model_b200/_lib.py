@@ -40,8 +40,11 @@ SYMBOLS = [
     "b200mdm_set_cond_multi", "b200mdm_set_cond_multi_dec", "b200mdm_set_prompt_weight",
     "b200mdm_set_cond_multi_tokens", "b200mdm_set_foot_guidance", "b200mdm_test_foot_guidance",
     "b200mdm_set_scene_guidance", "b200mdm_test_scene_guidance", "b200mdm_chain_set_goal", "b200mdm_chunk_frame",
+    "b200mdm_set_interaction_guidance", "b200mdm_test_interaction_guidance",
 ]
 MAX_PROMPTS = 8                             # B200MDM_MAX_PROMPTS
+MAX_CHARACTERS = 8                          # characters per scene: one cluster of at most 8 CTAs
+MAX_INTERACTION_PAIRS = 1024                # B200MDM_MAX_INTERACTION_PAIRS
 MAX_MEMORY_TOKENS = 512                     # a BERT text memory holds 1 .. 512 tokens (DistilBERT's position limit)
 # tap points of b200mdm_test_forward_taps (B200MDM_TAP_*)
 TAPS = ["EMBED", "TOK0", "CONDPROJ", "TEMB", "MEM16", "CROSS_C", "KVC16", "L_IN", "L_QKV", "L_ATT", "L_LN1", "L_QC",
@@ -148,6 +151,10 @@ def load():
                        ("b200mdm_set_scene_guidance", [vp, f32, f32, ctypes.POINTER(Grid), ctypes.POINTER(Grid), vp]),
                        ("b200mdm_test_scene_guidance", [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, f32, f32, f32,
                                                         f32, f32, ctypes.POINTER(Grid), ctypes.POINTER(Grid), vp, vp, vp]),
+                       ("b200mdm_set_interaction_guidance", [vp, i32, f32, f32, vp, vp, i32, vp, vp, ctypes.c_int64, vp]),
+                       ("b200mdm_test_interaction_guidance", [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, i32, f32, f32,
+                                                              f32, f32, f32, ctypes.POINTER(Grid), ctypes.POINTER(Grid), i32,
+                                                              f32, f32, vp, vp, i32, vp, vp, ctypes.c_int64, vp, vp, vp]),
                        ("b200mdm_set_cond_multi", [vp, i32, i32, i32, vp, vp, vp, vp]),
                        ("b200mdm_set_cond_multi_dec", [vp, i32, i32, i32, vp, vp, vp]),
                        ("b200mdm_set_cond_multi_tokens", [vp, i32, i32, i32, vp, vp, i32, vp, vp]),

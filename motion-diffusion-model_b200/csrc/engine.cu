@@ -152,10 +152,13 @@ struct GraphKey {
   int groups = 0;                   // multi-prompt guidance: the step ends in compose_step_kernel over G groups
   bool foot = false;                // ... with the foot-contact and floor terms: joint_guidance_step_kernel<true, false>
   bool scene = false;               // ... and the scene terms: joint_guidance_step_kernel<true, true>
+  bool inter = false;               // ... and the interaction terms: joint_guidance_step_kernel<true, true, true>
+  int chars = 0;                    //     in clusters of `chars` CTAs
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
            imask == o.imask && iweight == o.iweight && imotion == o.imotion && target_g == o.target_g && hs == o.hs &&
-           guided == o.guided && groups == o.groups && foot == o.foot && scene == o.scene;
+           guided == o.guided && groups == o.groups && foot == o.foot && scene == o.scene && inter == o.inter &&
+           chars == o.chars;
   }
 };
 
@@ -285,6 +288,14 @@ struct b200mdm_engine : Workspace {
   // b200mdm_set_cond*, b200mdm_set_joint_guidance and b200mdm_set_foot_guidance call
   SceneGuide h_sg{};
   bool sg_set = false;
+  // its interaction terms (b200mdm_set_interaction_guidance): the descriptor's InterGuide, the reach rows it points to
+  // (ig_pairs [ig_pairs_cap] device, allocated on first use) and their host staging; ig_set is cleared by every
+  // b200mdm_set_cond*, b200mdm_set_joint_guidance, b200mdm_set_foot_guidance and b200mdm_set_scene_guidance call
+  InterGuide h_ig{};
+  InterPair* ig_pairs = nullptr;
+  int ig_pairs_cap = 0;
+  std::vector<InterPair> h_ig_pairs;
+  bool ig_set = false;
   // multi-prompt guidance: the prompt-weight descriptor (read by the step graph at every replay, allocated on first
   // use) and its host staging; pw_set is cleared by every b200mdm_set_cond* call
   PromptWeight* pw_desc = nullptr;
@@ -386,6 +397,9 @@ static int init_kernel_attrs() {
   CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
   CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
   CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
+  const int ig_smem = static_cast<int>(ig_smem_bytes(JG_MAX_FRAMES, JG_MAX_FEATS));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ig_smem));
+  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ig_smem));
   if (dev < 64) done_mask |= 1ull << dev;
   return B200MDM_OK;
 }
@@ -408,20 +422,37 @@ struct PdlScope {
   PdlScope() { g_pdl_now = pdl_enabled(); }
   ~PdlScope() { g_pdl_now = false; }
 };
+// cluster > 0: thread-block clusters of `cluster` CTAs along x
 template <class... KArgs, class... Args>
-static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
+static cudaError_t launch_kc(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, int cluster,
+                             Args&&... args) {
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute at[2];
+  int n = 0;
+  if (cluster > 0) {
+    at[n].id = cudaLaunchAttributeClusterDimension;
+    at[n].val.clusterDim.x = static_cast<unsigned>(cluster);
+    at[n].val.clusterDim.y = 1;
+    at[n].val.clusterDim.z = 1;
+    ++n;
+  }
+  if (g_pdl_now) {
+    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
   cfg.attrs = at;
-  cfg.numAttrs = g_pdl_now ? 1 : 0;
+  cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(std::forward<Args>(args))...);
+}
+template <class... KArgs, class... Args>
+static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
+  return launch_kc(kern, grid, block, smem, s, 0, std::forward<Args>(args)...);
 }
 
 template <class Epi, class = void> struct epi_unstaged : std::false_type {};
@@ -732,6 +763,7 @@ extern "C" int b200mdm_destroy(b200mdm_engine* e) {
   dfree(e->tw0); dfree(e->tb0); dfree(e->twk); dfree(e->tbk); dfree(e->twsum);
   dfree(e->state);
   dfree(e->jg_desc);
+  dfree(e->ig_pairs);
   dfree(e->fg_len);
   dfree(e->pw_desc);
   if (e->work) cudaStreamDestroy(e->work);
@@ -1285,6 +1317,7 @@ static void end_cond(b200mdm_engine* e) {
   e->jg_set = false;
   e->fg_set = false;
   e->sg_set = false;
+  e->ig_set = false;
   e->pw_set = false;
   e->vb_live = false;
   e->chain_next = -1;
@@ -1624,6 +1657,8 @@ extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_d
   e->fg_set = false;
   e->h_fg = FootGuide{};
   e->sg_set = false;
+  e->h_sg = SceneGuide{};
+  e->ig_set = false;
   return B200MDM_OK;
 }
 
@@ -1644,6 +1679,8 @@ extern "C" int b200mdm_set_foot_guidance(b200mdm_engine* e, float contact_weight
   if (!e->jg_set) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (foot guidance extends it)");
   e->fg_set = false;
   e->sg_set = false;
+  e->h_sg = SceneGuide{};
+  e->ig_set = false;
   const int* len = nullptr;
   if (lengths_host) {
     if (e->fg_len_cap < e->B) {
@@ -1708,13 +1745,102 @@ extern "C" int b200mdm_set_scene_guidance(b200mdm_engine* e, float obstacle_weig
   if (terrain && e->h_fg.floor_w == 0.f)
     return fail(B200MDM_EINVAL, "a terrain needs a floor weight > 0 (b200mdm_set_foot_guidance)");
   e->sg_set = false;
+  e->ig_set = false;
+  e->h_sg = sg;   // (kept when off: the interaction terms' scene)
   if (obstacle_weight == 0.f && !terrain) return B200MDM_OK;   // off: no scene
-  e->h_sg = sg;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   // the foot terms as set (both weights 0 included: the lengths), then the scene
   CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->f, &e->h_fg, sizeof(FootGuide), cudaMemcpyHostToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->s, &e->h_sg, sizeof(SceneGuide), cudaMemcpyHostToDevice, s));
   e->sg_set = true;
+  return B200MDM_OK;
+}
+
+// the argument checks b200mdm_set_interaction_guidance and b200mdm_test_interaction_guidance share (J joints per motion);
+// the reach rows go to `rows`
+static int check_inter(int32_t characters, float weight, float margin, const float* placement_dev, const int32_t* pairs_host,
+                       int32_t n_pairs, const float* reach_host, const float* pair_weight_dev, int64_t pair_weight_stride, int B,
+                       int T, int J, std::vector<InterPair>* rows) {
+  if (characters < 2 || characters > IG_MAX_CHARS)
+    return fail(B200MDM_EINVAL, "%d characters per scene: 2 .. %d", characters, IG_MAX_CHARS);
+  if (B % characters) return fail(B200MDM_EINVAL, "batch %d is not a whole number of %d-character scenes", B, characters);
+  if (!std::isfinite(weight) || weight < 0.f || !std::isfinite(margin) || margin < 0.f)
+    return fail(B200MDM_EINVAL, "interaction weight %g, margin %g: finite values >= 0", weight, margin);
+  if (!placement_dev) return fail(B200MDM_EINVAL, "null placement");
+  if (n_pairs < 0 || n_pairs > B200MDM_MAX_INTERACTION_PAIRS)
+    return fail(B200MDM_EINVAL, "%d reach rows: 0 .. %d", n_pairs, B200MDM_MAX_INTERACTION_PAIRS);
+  if (n_pairs > 0 && (!pairs_host || !reach_host || !pair_weight_dev)) return fail(B200MDM_EINVAL, "null reach rows");
+  if (n_pairs > 0 && pair_weight_stride != 0 && pair_weight_stride < static_cast<int64_t>(n_pairs) * T)
+    return fail(B200MDM_EINVAL, "pair weight stride %lld: 0 (shared) or at least %lld", static_cast<long long>(pair_weight_stride),
+                static_cast<long long>(n_pairs) * T);
+  rows->resize(n_pairs);
+  for (int n = 0; n < n_pairs; ++n) {
+    const int32_t* r = pairs_host + 4 * n;
+    if (r[0] < 0 || r[0] >= characters || r[2] < 0 || r[2] >= characters || r[0] == r[2] || r[1] < 0 || r[1] >= J ||
+        r[3] < 0 || r[3] >= J)
+      return fail(B200MDM_EINVAL, "reach row %d (%d, %d, %d, %d): characters in 0 .. %d and distinct, joints in 0 .. %d", n,
+                  r[0], r[1], r[2], r[3], characters - 1, J - 1);
+    if (!std::isfinite(reach_host[n]) || reach_host[n] < 0.f)
+      return fail(B200MDM_EINVAL, "reach[%d] = %g: a finite value >= 0", n, reach_host[n]);
+    (*rows)[n] = InterPair{r[0], r[1], r[2], r[3], reach_host[n]};
+  }
+  return B200MDM_OK;
+}
+
+// ENOTIMPL unless a cluster of `characters` guidance CTAs (ig_smem_bytes each) can be resident
+template <class Kern>
+static int check_inter_cluster(Kern kern, int characters, int B, int T, int R) {
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(B);
+  cfg.blockDim = dim3(JG_THREADS);
+  cfg.dynamicSmemBytes = ig_smem_bytes(T, R);
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = static_cast<unsigned>(characters);
+  at[0].val.clusterDim.y = 1;
+  at[0].val.clusterDim.z = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  int n = 0;
+  CUDA_TRY(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+  if (n < 1) return fail(B200MDM_ENOTIMPL, "a cluster of %d guidance CTAs (%zu B of shared memory each) cannot be resident",
+                         characters, ig_smem_bytes(T, R));
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_interaction_guidance(b200mdm_engine* e, int32_t characters, float weight, float margin,
+                                                const float* placement_dev, const int32_t* pairs_host, int32_t n_pairs,
+                                                const float* reach_host, const float* pair_weight_dev,
+                                                int64_t pair_weight_stride, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!e->jg_set) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (interaction guidance extends it)");
+  const int J = e->JF == 263 ? 22 : 21, R = 4 + 3 * (J - 1);
+  std::vector<InterPair> rows;
+  TRY(check_inter(characters, weight, margin, placement_dev, pairs_host, n_pairs, reach_host, pair_weight_dev,
+                  pair_weight_stride, e->B, e->T, J, &rows));
+  TRY(init_kernel_attrs());
+  TRY(check_inter_cluster(joint_guidance_step_kernel<true, true, true>, characters, e->B, e->T, R));
+  e->ig_set = false;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (n_pairs > 0) {
+    if (e->ig_pairs_cap < n_pairs) {
+      dfree(e->ig_pairs);
+      e->ig_pairs_cap = 0;
+      TRY(dalloc(&e->ig_pairs, static_cast<size_t>(n_pairs)));
+      e->ig_pairs_cap = n_pairs;
+    }
+    // the host staging lives in the engine until the next call: no stream synchronisation
+    e->h_ig_pairs = std::move(rows);
+    CUDA_TRY(cudaMemcpyAsync(e->ig_pairs, e->h_ig_pairs.data(), n_pairs * sizeof(InterPair), cudaMemcpyHostToDevice, s));
+  }
+  e->h_ig = InterGuide{placement_dev, e->ig_pairs, pair_weight_dev, static_cast<long long>(pair_weight_stride), characters,
+                       n_pairs, weight, margin};
+  // the foot and scene terms as set (their weights may be 0: the lengths), then the interaction
+  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->f, &e->h_fg, sizeof(FootGuide), cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->s, &e->h_sg, sizeof(SceneGuide), cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->i, &e->h_ig, sizeof(InterGuide), cudaMemcpyHostToDevice, s));
+  e->ig_set = true;
   return B200MDM_OK;
 }
 
@@ -2000,7 +2126,10 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
       TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, ax, px, s, e->num_sms));
       set_step_params(&p, a, B, T, JF);
       const int R = 4 + 3 * ((JF == 263 ? 22 : 21) - 1);
-      if (e->sg_set)
+      if (e->ig_set)
+        CUDA_TRY(launch_kc(joint_guidance_step_kernel<true, true, true>, dim3(B), dim3(JG_THREADS), ig_smem_bytes(T, R), s,
+                           e->h_ig.chars, static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
+      else if (e->sg_set)
         CUDA_TRY(launch_k(joint_guidance_step_kernel<true, true>, dim3(B), dim3(JG_THREADS), fg_smem_bytes(T, R), s,
                           static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
       else if (e->fg_set)
@@ -2215,6 +2344,8 @@ static int loop_enter(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32
     key.guided = e->jg_set;
     key.foot = e->jg_set && e->fg_set;
     key.scene = e->jg_set && e->sg_set;
+    key.inter = e->jg_set && e->ig_set;
+    key.chars = key.inter ? e->h_ig.chars : 0;
     key.groups = e->groups;
     TRY(ensure_step_graph(e, key, a));
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
@@ -3139,16 +3270,18 @@ extern "C" int b200mdm_test_joint_guidance(const float* x0_dev, const float* mea
   const JointGuide g{mean_dev, std_dev, target_dev, weight_dev, step, iters};
   const int R = D == 263 ? 67 : 64;
   joint_guidance_test_kernel<false, false><<<B, JG_THREADS, jg_smem_bytes(T, R), static_cast<cudaStream_t>(stream)>>>(
-      g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, FootGuide{}, SceneGuide{});
+      g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, FootGuide{}, SceneGuide{}, InterGuide{});
   CUDA_TRY(cudaGetLastError());
   return B200MDM_OK;
 }
 
-// b200mdm_test_foot_guidance and b200mdm_test_scene_guidance (sg: nullptr without the scene terms)
+// b200mdm_test_foot_guidance, b200mdm_test_scene_guidance (sg: nullptr without the scene terms) and
+// b200mdm_test_interaction_guidance (ig: nullptr without the interaction terms; its reach rows `rows`)
 static int test_foot_scene(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
                            const float* weight_dev, const float* contact_dev, const int64_t* lengths_host, int32_t B,
                            int32_t T, int32_t D, float step, int32_t iters, float contact_weight, float floor_weight,
-                           float floor_height, const SceneGuide* sg, float* x0_out_dev, float* loss_out_dev, void* stream) {
+                           float floor_height, const SceneGuide* sg, float* x0_out_dev, float* loss_out_dev, void* stream,
+                           const InterGuide* ig = nullptr, const std::vector<InterPair>* rows = nullptr) {
   TRY(init_kernel_attrs());
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int* len = nullptr;
@@ -3162,14 +3295,27 @@ static int test_foot_scene(const float* x0_dev, const float* mean_dev, const flo
   const JointGuide g{mean_dev, std_dev, target_dev, weight_dev, step, iters};
   const FootGuide f{contact_dev, len, contact_weight, floor_weight, floor_height};
   const int R = D == 263 ? 67 : 64;
-  if (sg)
+  InterPair* pairs = nullptr;
+  cudaError_t err = cudaSuccess;
+  if (ig) {
+    InterGuide i = *ig;
+    if (!rows->empty()) {
+      CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&pairs), rows->size() * sizeof(InterPair), s));
+      CUDA_TRY(cudaMemcpyAsync(pairs, rows->data(), rows->size() * sizeof(InterPair), cudaMemcpyHostToDevice, s));
+    }
+    i.pairs = pairs;
+    err = launch_kc(joint_guidance_test_kernel<true, true, true>, dim3(B), dim3(JG_THREADS), ig_smem_bytes(T, R), s, i.chars,
+                    g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, f, *sg, i);
+  } else if (sg) {
     joint_guidance_test_kernel<true, true><<<B, JG_THREADS, fg_smem_bytes(T, R), s>>>(g, x0_dev, x0_out_dev, loss_out_dev, B,
-                                                                                      T, D, f, *sg);
-  else
+                                                                                      T, D, f, *sg, InterGuide{});
+  } else {
     joint_guidance_test_kernel<true, false><<<B, JG_THREADS, fg_smem_bytes(T, R), s>>>(g, x0_dev, x0_out_dev, loss_out_dev, B,
-                                                                                       T, D, f, SceneGuide{});
-  const cudaError_t err = cudaGetLastError();
+                                                                                       T, D, f, SceneGuide{}, InterGuide{});
+  }
+  if (err == cudaSuccess) err = cudaGetLastError();
   if (len) cudaFreeAsync(len, s);
+  if (pairs) cudaFreeAsync(pairs, s);
   if (err != cudaSuccess) return fail(B200MDM_ECUDA, "%s", cudaGetErrorString(err));
   CUDA_TRY(cudaStreamSynchronize(s));   // h_len is local
   return B200MDM_OK;
@@ -3212,6 +3358,30 @@ extern "C" int b200mdm_test_scene_guidance(const float* x0_dev, const float* mea
   if (terrain && floor_weight == 0.f) return fail(B200MDM_EINVAL, "a terrain needs a floor weight > 0");
   return test_foot_scene(x0_dev, mean_dev, std_dev, target_dev, weight_dev, contact_dev, lengths_host, B, T, D, step, iters,
                          contact_weight, floor_weight, floor_height, &sg, x0_out_dev, loss_out_dev, stream);
+}
+
+extern "C" int b200mdm_test_interaction_guidance(
+    const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev, const float* weight_dev,
+    const float* contact_dev, const int64_t* lengths_host, int32_t B, int32_t T, int32_t D, float step, int32_t iters,
+    float contact_weight, float floor_weight, float floor_height, float obstacle_weight, float obstacle_margin,
+    const b200mdm_grid* sdf, const b200mdm_grid* terrain, int32_t characters, float weight, float margin,
+    const float* placement_dev, const int32_t* pairs_host, int32_t n_pairs, const float* reach_host,
+    const float* pair_weight_dev, int64_t pair_weight_stride, float* x0_out_dev, float* loss_out_dev, void* stream) {
+  TRY(check_foot_test(x0_dev, mean_dev, std_dev, target_dev, weight_dev, lengths_host, B, T, D, step, iters, contact_weight,
+                      floor_weight, floor_height, x0_out_dev));
+  SceneGuide sg{};
+  TRY(check_scene(obstacle_weight, obstacle_margin, sdf, terrain, B, &sg));
+  if (terrain && floor_weight == 0.f) return fail(B200MDM_EINVAL, "a terrain needs a floor weight > 0");
+  const int J = D == 263 ? 22 : 21, R = 4 + 3 * (J - 1);
+  std::vector<InterPair> rows;
+  TRY(check_inter(characters, weight, margin, placement_dev, pairs_host, n_pairs, reach_host, pair_weight_dev,
+                  pair_weight_stride, B, T, J, &rows));
+  TRY(init_kernel_attrs());
+  TRY(check_inter_cluster(joint_guidance_test_kernel<true, true, true>, characters, B, T, R));
+  const InterGuide ig{placement_dev, nullptr, pair_weight_dev, static_cast<long long>(pair_weight_stride), characters, n_pairs,
+                      weight, margin};
+  return test_foot_scene(x0_dev, mean_dev, std_dev, target_dev, weight_dev, contact_dev, lengths_host, B, T, D, step, iters,
+                         contact_weight, floor_weight, floor_height, &sg, x0_out_dev, loss_out_dev, stream, &ig, &rows);
 }
 
 // ------------------------------------------------------------------------------------------------ post-processing

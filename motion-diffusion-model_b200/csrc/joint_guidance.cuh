@@ -20,6 +20,13 @@
 // bilinearly at every joint's world XZ (scene_sample; read through L2).  G gains 1/2 lo sum_{t<L, j} max(r - S, 0)^2 with
 // S the obstacles' signed distance, and the floor term's height becomes h + H(x, z) with H the terrain; both only add to e
 // (in x / z through the grids' gradients), the existing chain is unchanged.
+// INTER (DESIGN.md, "Several characters in one scene"), on top of SCENE: the B motions are B / C scenes of C characters,
+// one thread-block cluster of C CTAs per scene.  Each CTA places its frame's joints in the scene frame, Q = rot(phi) p +
+// (X, 0, Z), and writes them to its shared memory; after a cluster barrier every thread reads its partners' frame-t rows
+// (mapa + ld.shared::cluster) and adds the avoidance adjoint la max(r - d, 0) and the reach rows' w max(d - delta, 0),
+// along the unit vector between the joints and rotated back by rot(phi)^T, to e.  Every character reads the positions
+// of the same iteration (Jacobi descent on the scene's energy): the next iteration's writes wait on a second cluster
+// barrier that follows the reads.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -69,12 +76,32 @@ struct SceneGuide {
   float obstacle_w, margin;
 };
 
-// The engine's device descriptor: the foot terms follow the joint terms and the scene terms the foot terms, so a kernel
-// without them reads what it always read
+// One reach row (b200mdm_set_interaction_guidance): joint j of scene-local character a toward joint k of character b,
+// within `reach` metres
+struct InterPair {
+  int a, j, b, k;
+  float reach;
+};
+
+// The interaction terms (b200mdm_set_interaction_guidance): C characters per scene, placement [B, 3] (x, z, phi) fp32,
+// n_pairs reach rows and their per-frame weights [N, T] at pair_w + s * pw_stride for scene s (pw_stride 0: shared),
+// the avoidance weight la and margin r.
+struct InterGuide {
+  const float* placement;
+  const InterPair* pairs;
+  const float* pair_w;
+  long long pw_stride;
+  int chars, n_pairs;
+  float weight, margin;
+};
+
+// The engine's device descriptor: the foot terms follow the joint terms, the scene terms the foot terms and the
+// interaction terms the scene terms, so a kernel without them reads what it always read
 struct GuideDesc {
   JointGuide j;
   FootGuide f;
   SceneGuide s;
+  InterGuide i;
 };
 
 // Shared memory of the guidance: xs [R, T] floats, mean / std of the R features, the velocity adjoints handed one frame
@@ -88,6 +115,12 @@ constexpr int FG_NB = 14, FG_CD = 12, FG_LD = JG_MAX_FRAMES;
 __host__ __device__ constexpr size_t fg_smem_bytes(int T, int R) {
   return jg_smem_bytes(T, R) + static_cast<size_t>(FG_NB + FG_CD) * FG_LD * sizeof(float);
 }
+// ... and with the interaction terms: each frame's scene-frame joints [3 J, FG_LD] (J <= 22), which the cluster reads
+constexpr int IG_ROWS = 3 * 22;
+__host__ __device__ constexpr size_t ig_smem_bytes(int T, int R) {
+  return fg_smem_bytes(T, R) + static_cast<size_t>(IG_ROWS) * FG_LD * sizeof(float);
+}
+constexpr int IG_MAX_CHARS = 8;   // the portable cluster size
 
 // The foot joints of contact channels D - 4 .. D - 1 (the reference's cat([..., feet_l, feet_r]) with fid_l, fid_r)
 __host__ __device__ constexpr int foot_joint(int J, int k) {
@@ -161,17 +194,132 @@ struct FootFrame {
   float* cd;
 };
 
+// The interaction terms' per-thread constants: this CTA's scene-frame joints q [IG_ROWS, FG_LD] (row 3 j + c), its rank
+// in the scene and the scene's first motion, its placement (cos phi, sin phi, X, Z), and bit b of `live` set when
+// frame t < L_ab for partner b (unused when !INTER)
+struct InterFrame {
+  float* q;
+  int rank, first;
+  float c, s, X, Z;
+  unsigned live;
+};
+
+// The interaction adjoint of joint j at thread t's frame (own-frame e += rot(phi)^T dG/dQ) and the pairs' loss counted
+// at the lower rank, reading the partners' rows of this iteration
+__device__ __forceinline__ void inter_joint(const InterGuide& ig, const InterFrame& xf, int j, int J, int T, float* ex,
+                                            float* ey, float* ez, double* lsum) {
+  const int t = threadIdx.x;
+  const float* qo = xf.q + t;
+  const float ax = qo[3 * j * FG_LD], ay = qo[(3 * j + 1) * FG_LD], az = qo[(3 * j + 2) * FG_LD];
+  const uint32_t q0 = smem_u32(qo);
+  float gx = 0.f, gy = 0.f, gz = 0.f;
+  // one pair term along Qa - Qb (partner p's joint k): coefficient cf of the unit vector, added to g
+  auto pair = [&](int p, int k, float* dx, float* dy, float* dz) {
+    const uint32_t r = mapa_shared(q0 + static_cast<uint32_t>(3 * k * FG_LD * sizeof(float)), static_cast<uint32_t>(p));
+    *dx = __fsub_rn(ax, ld_shared_cluster_f32(r));
+    *dy = __fsub_rn(ay, ld_shared_cluster_f32(r + FG_LD * sizeof(float)));
+    *dz = __fsub_rn(az, ld_shared_cluster_f32(r + 2 * FG_LD * sizeof(float)));
+    return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(*dx, *dx), __fmul_rn(*dy, *dy)), __fmul_rn(*dz, *dz)));
+  };
+  auto add = [&](float cf, float dx, float dy, float dz) {
+    gx = __fadd_rn(gx, __fmul_rn(cf, dx));
+    gy = __fadd_rn(gy, __fmul_rn(cf, dy));
+    gz = __fadd_rn(gz, __fmul_rn(cf, dz));
+  };
+  if (ig.weight > 0.f) {   // avoidance against every joint of every partner: -la max(r - d, 0) (Qa - Qb) / d
+#pragma unroll 1
+    for (int p = 0; p < ig.chars; ++p) {
+      if (p == xf.rank || !((xf.live >> p) & 1u)) continue;
+#pragma unroll 1
+      for (int k = 0; k < J; ++k) {
+        float dx, dy, dz;
+        const float d = pair(p, k, &dx, &dy, &dz);
+        const float m = __fsub_rn(ig.margin, d);
+        if (!(m > 0.f)) continue;
+        if (xf.rank < p) *lsum += 0.5 * static_cast<double>(ig.weight) * (static_cast<double>(m) * m);
+        if (d > 0.f) add(-__fdiv_rn(__fmul_rn(ig.weight, m), d), dx, dy, dz);   // 0 at d = 0
+      }
+    }
+  }
+  // the reach rows this joint belongs to, on either side: w max(d - delta, 0) (Qa - Qb) / d
+  const float* pw = ig.pair_w + static_cast<size_t>(xf.first / ig.chars) * static_cast<size_t>(ig.pw_stride) + t;
+#pragma unroll 1
+  for (int n = 0; n < ig.n_pairs; ++n) {
+    const InterPair* row = ig.pairs + n;
+    const int a = __ldcg(&row->a), b = __ldcg(&row->b);
+    int p, k;
+    if (a == xf.rank && __ldcg(&row->j) == j) {
+      p = b;
+      k = __ldcg(&row->k);
+    } else if (b == xf.rank && __ldcg(&row->k) == j) {
+      p = a;
+      k = __ldcg(&row->j);
+    } else {
+      continue;
+    }
+    if (!((xf.live >> p) & 1u)) continue;
+    const float w = __ldcg(pw + static_cast<size_t>(n) * T);
+    if (w == 0.f) continue;
+    float dx, dy, dz;
+    const float d = pair(p, k, &dx, &dy, &dz);
+    const float m = __fsub_rn(d, __ldcg(&row->reach));
+    if (!(m > 0.f)) continue;
+    if (xf.rank < p) *lsum += 0.5 * static_cast<double>(w) * (static_cast<double>(m) * m);
+    add(__fdiv_rn(__fmul_rn(w, m), d), dx, dy, dz);
+  }
+  if (gx == 0.f && gy == 0.f && gz == 0.f) return;
+  // rot(phi)^T back to the character's own frame
+  *ex = __fadd_rn(*ex, __fadd_rn(__fmul_rn(xf.c, gx), __fmul_rn(xf.s, gz)));
+  *ey = __fadd_rn(*ey, gy);
+  *ez = __fadd_rn(*ez, __fsub_rn(__fmul_rn(xf.c, gz), __fmul_rn(xf.s, gx)));
+}
+
+// Thread t's frame of this CTA in the scene frame: Q = rot(phi) p + (X, 0, Z) of every joint into xf.q, from the
+// forward pass's yaw (c, s) and root position (px, pz)
+__device__ __forceinline__ void inter_place(const InterFrame& xf, const float* xs, const float* mu, const float* sd, int T,
+                                            int J, float c, float s, float px, float pz) {
+  const int t = threadIdx.x;
+  auto X = [&](int f) { return __fadd_rn(__fmul_rn(xs[f * T + t], sd[f]), mu[f]); };
+  float* q = xf.q + t;
+#pragma unroll 1
+  for (int j = 0; j < J; ++j) {
+    float x = px, y, z = pz;
+    if (j == 0) {
+      y = X(3);
+    } else {
+      const int f = 4 + 3 * (j - 1);
+      float rx, rz;
+      ric_rot(c, s, X(f), X(f + 2), &rx, &rz);
+      x = __fadd_rn(rx, px);
+      y = X(f + 1);
+      z = __fadd_rn(rz, pz);
+    }
+    q[3 * j * FG_LD] = __fadd_rn(__fsub_rn(__fmul_rn(xf.c, x), __fmul_rn(xf.s, z)), xf.X);
+    q[(3 * j + 1) * FG_LD] = y;
+    q[(3 * j + 2) * FG_LD] = __fadd_rn(__fadd_rn(__fmul_rn(xf.s, x), __fmul_rn(xf.c, z)), xf.Z);
+  }
+}
+
 // One iteration's joint pass with the foot terms, for thread t's frame (every thread of the block calls it): the
 // neighbour exchange, kappa * Delta of pair (t, t + 1) and its loss, then per joint e = w (p - c) + the floor's and the
 // contact pairs' adjoints, into the position / yaw adjoints and the descent on height and joints, as joint_guidance_iterate.
 // SCENE: the floor's height gains the terrain, and the obstacles' adjoint joins (sg.obstacle_w is 0 on frames >= L).
-template <bool SCENE>
+// INTER: the frame's scene-frame joints are published to the cluster (after the partners' reads of the previous
+// iteration, `wait`), and the interaction adjoint joins.
+template <bool SCENE, bool INTER>
 __device__ __forceinline__ void foot_iterate(float* xs, const float* mu, const float* sd, const JointGuide& g, const FootGuide& fg,
                                              const FootFrame& ff, const float* tg, const float* wt, int T, int J, bool upd,
                                              float c, float s, float wx, float wz, float px, float pz, float* gpx, float* gpz,
-                                             float* gyaw, double* lsum, const SceneGuide& sg, int b) {
+                                             float* gyaw, double* lsum, const SceneGuide& sg, int b, const InterGuide& ig,
+                                             const InterFrame& xf, bool wait) {
   const int t = threadIdx.x;
   const bool act = t < T;
+  if constexpr (INTER) {
+    if (wait) cluster_wait_acquire();
+    if (act) inter_place(xf, xs, mu, sd, T, J, c, s, px, pz);
+    cluster_arrive_release();
+    cluster_wait_acquire();
+  }
   auto X = [&](int f) { return __fadd_rn(__fmul_rn(xs[f * T + t], sd[f]), mu[f]); };
   float* nb = ff.nb + t;   // row r of frame t + o: nb[r * FG_LD + o]
   float* cd = ff.cd + t;
@@ -263,6 +411,7 @@ __device__ __forceinline__ void foot_iterate(float* xs, const float* mu, const f
           ez = __fsub_rn(ez, __fmul_rn(lm, sz));
         }
       }
+      if constexpr (INTER) inter_joint(ig, xf, j, J, T, &ex, &ey, &ez, lsum);
     } else if (ff.floor) {   // the floor: lf min(p.y - h, 0)
       const float m = fminf(__fsub_rn(qy, fg.floor_h), 0.f);
       if (m < 0.f) {
@@ -299,10 +448,10 @@ __device__ __forceinline__ void foot_iterate(float* xs, const float* mu, const f
 // The K guidance iterations of motion b on xs (its R ric features, normalised, [R, T] in shared memory; mu / sd the
 // features' mean and std).  loss (nullable) [K + 1, B] receives G before each iteration and after the last one.
 // Every thread of the block calls it.
-template <bool FOOT, bool SCENE>
+template <bool FOOT, bool SCENE, bool INTER>
 __device__ void joint_guidance_iterate(float* xs, const float* mu, const float* sd, float* gv, double* sh, const JointGuide& g,
                                        int b, int B, int T, int J, float* loss, const FootGuide& fg, const FootFrame& ff,
-                                       const SceneGuide& sg) {
+                                       const SceneGuide& sg, const InterGuide& ig, const InterFrame& xf) {
   const int t = threadIdx.x;
   const bool act = t < T;
   const float* tg = g.target + static_cast<size_t>(b) * J * 3 * T + t;
@@ -326,7 +475,9 @@ __device__ void joint_guidance_iterate(float* xs, const float* mu, const float* 
     float gpx = 0.f, gpz = 0.f, gyaw = 0.f;
     double lsum = 0.0;
     if constexpr (FOOT) {
-      foot_iterate<SCENE>(xs, mu, sd, g, fg, ff, tg, wt, T, J, upd, c, s, wx, wz, px, pz, &gpx, &gpz, &gyaw, &lsum, sg, b);
+      foot_iterate<SCENE, INTER>(xs, mu, sd, g, fg, ff, tg, wt, T, J, upd, c, s, wx, wz, px, pz, &gpx, &gpz, &gyaw, &lsum, sg, b,
+                                 ig, xf, k > 0);
+      if constexpr (INTER) cluster_arrive_release();   // this iteration's reads of the partners' rows are done
     } else if (act) {
       for (int j = 0; j < J; ++j) {
         const float w = __ldcg(wt + static_cast<size_t>(j) * T);
@@ -388,13 +539,14 @@ __device__ void joint_guidance_iterate(float* xs, const float* mu, const float* 
     }
     __syncthreads();   // the next iteration reads the neighbours' velocities
   }
+  if constexpr (INTER) cluster_wait_acquire();   // no CTA leaves while a partner may still read its rows
 }
 
 // The guidance of one motion around joint_guidance_iterate: shared memory carved, ric features of x0 [B, D, T] loaded
 // (through L2: x0 was written by the kernel before).  Returns the shared-memory view of the guided features.
-template <bool FOOT, bool SCENE>
+template <bool FOOT, bool SCENE, bool INTER>
 __device__ __forceinline__ float* joint_guidance_run(const JointGuide& g, const FootGuide& fg, SceneGuide sg, const float* x0,
-                                                     int B, int T, int D, float* loss) {
+                                                     int B, int T, int D, float* loss, const InterGuide& ig) {
   extern __shared__ double jg_smem[];
   const int J = D == 263 ? 22 : 21, R = 4 + 3 * (J - 1), b = blockIdx.x;
   double* sh = jg_smem;
@@ -433,8 +585,25 @@ __device__ __forceinline__ float* joint_guidance_run(const JointGuide& g, const 
     ff.nb = gv + 2 * T;
     ff.cd = ff.nb + FG_NB * FG_LD;
   }
+  InterFrame xf{};
+  if constexpr (INTER) {
+    const int t = threadIdx.x;
+    xf.q = ff.cd + FG_CD * FG_LD;
+    xf.rank = b % ig.chars;
+    xf.first = b - xf.rank;
+    const float phi = __ldcg(ig.placement + 3 * b + 2);
+    xf.c = cosf(phi);
+    xf.s = sinf(phi);
+    xf.X = __ldcg(ig.placement + 3 * b);
+    xf.Z = __ldcg(ig.placement + 3 * b + 1);
+    // partner p acts on frame t < min(L_self, L_p)
+    auto len = [&](int m) { return fg.lengths != nullptr ? min(max(__ldcg(fg.lengths + m), 0), T) : T; };
+    const int L = len(b);
+    for (int p = 0; p < ig.chars; ++p)
+      if (t < L && t < len(xf.first + p)) xf.live |= 1u << p;
+  }
   __syncthreads();
-  joint_guidance_iterate<FOOT, SCENE>(xs, mu, sd, gv, sh, g, b, B, T, J, loss, fg, ff, sg);
+  joint_guidance_iterate<FOOT, SCENE, INTER>(xs, mu, sd, gv, sh, g, b, B, T, J, loss, fg, ff, sg, ig, xf);
   return xs;
 }
 
@@ -478,17 +647,31 @@ __device__ __forceinline__ SceneGuide load_scene_guide(const SceneGuide* d) {
   s.margin = __ldcg(&d->margin);
   return s;
 }
+__device__ __forceinline__ InterGuide load_inter_guide(const InterGuide* d) {
+  InterGuide i;
+  i.placement = reinterpret_cast<const float*>(__ldcg(reinterpret_cast<const unsigned long long*>(&d->placement)));
+  i.pairs = reinterpret_cast<const InterPair*>(__ldcg(reinterpret_cast<const unsigned long long*>(&d->pairs)));
+  i.pair_w = reinterpret_cast<const float*>(__ldcg(reinterpret_cast<const unsigned long long*>(&d->pair_w)));
+  i.pw_stride = __ldcg(&d->pw_stride);
+  i.chars = __ldcg(&d->chars);
+  i.n_pairs = __ldcg(&d->n_pairs);
+  i.weight = __ldcg(&d->weight);
+  i.margin = __ldcg(&d->margin);
+  return i;
+}
 
 // The guided step of motion blockIdx.x: x0 (the output projection + bias after the CFG blend, [B, D, T], written by the
 // MODE_X0 output GEMM) -> guidance -> the output step's tail (inpainting, clamp, the DDPM / DDIM update of p.mode) for
 // every element of the motion, reading the step's noise as OutStep does.  grid = B, block = JG_THREADS,
 // dynamic shared memory jg_smem_bytes(T, R) (FOOT: fg_smem_bytes(T, R)).  FOOT asks for one CTA per SM (the B CTAs
 // never share one at B <= 132), which lifts the register cap ptxas otherwise picks and keeps the step free of spills.
-// SCENE (only with FOOT) adds the scene terms.
-template <bool FOOT, bool SCENE>
+// SCENE (only with FOOT) adds the scene terms, INTER (only with SCENE) the interaction terms: the grid is then B / C
+// clusters of C CTAs (C = the descriptor's chars) and the dynamic shared memory ig_smem_bytes(T, R).
+template <bool FOOT, bool SCENE, bool INTER = false>
 __global__ void __launch_bounds__(JG_THREADS, FOOT ? 1 : 0) joint_guidance_step_kernel(const GuideDesc* guide, const float* x0,
                                                                          const EpiOutParams p) {
   static_assert(FOOT || !SCENE, "the scene terms extend the foot family");
+  static_assert(SCENE || !INTER, "the interaction terms extend the scene family");
   pdl_launch_dependents();
   pdl_wait();
   const int T = p.T, D = p.J, b = blockIdx.x, t = threadIdx.x;
@@ -497,8 +680,10 @@ __global__ void __launch_bounds__(JG_THREADS, FOOT ? 1 : 0) joint_guidance_step_
   if constexpr (FOOT) fg = load_foot_guide(&guide->f);
   SceneGuide sg{};
   if constexpr (SCENE) sg = load_scene_guide(&guide->s);
+  InterGuide ig{};
+  if constexpr (INTER) ig = load_inter_guide(&guide->i);
   const int R = D == 263 ? 67 : 64;
-  const float* xs = joint_guidance_run<FOOT, SCENE>(g, fg, sg, x0, p.B, T, D, nullptr);
+  const float* xs = joint_guidance_run<FOOT, SCENE, INTER>(g, fg, sg, x0, p.B, T, D, nullptr, ig);
   if (t >= T) return;
   const OutStep u(p, b);
   const size_t base = static_cast<size_t>(b) * D * T + t;
@@ -509,16 +694,18 @@ __global__ void __launch_bounds__(JG_THREADS, FOOT ? 1 : 0) joint_guidance_step_
   }
 }
 
-// b200mdm_test_joint_guidance / b200mdm_test_foot_guidance (FOOT) / b200mdm_test_scene_guidance (SCENE): the guidance
-// alone, x0_out [B, D, T] = guided x0 (features past the ric features copied).  fg and sg come last, so the FOOT = false
-// kernel's parameters keep their offsets.
-template <bool FOOT, bool SCENE>
+// b200mdm_test_joint_guidance / b200mdm_test_foot_guidance (FOOT) / b200mdm_test_scene_guidance (SCENE) /
+// b200mdm_test_interaction_guidance (INTER, clusters as the step kernel's): the guidance alone, x0_out [B, D, T] = guided
+// x0 (features past the ric features copied).  fg, sg and ig come last, so the other kernels' parameters keep their
+// offsets.
+template <bool FOOT, bool SCENE, bool INTER = false>
 __global__ void __launch_bounds__(JG_THREADS) joint_guidance_test_kernel(const JointGuide g, const float* x0, float* x0_out,
                                                                          float* loss, int B, int T, int D, const FootGuide fg,
-                                                                         const SceneGuide sg) {
+                                                                         const SceneGuide sg, const InterGuide ig) {
   static_assert(FOOT || !SCENE, "the scene terms extend the foot family");
+  static_assert(SCENE || !INTER, "the interaction terms extend the scene family");
   const int R = D == 263 ? 67 : 64, b = blockIdx.x;
-  const float* xs = joint_guidance_run<FOOT, SCENE>(g, fg, sg, x0, B, T, D, loss);
+  const float* xs = joint_guidance_run<FOOT, SCENE, INTER>(g, fg, sg, x0, B, T, D, loss, ig);
   const size_t base = static_cast<size_t>(b) * D * T;
   for (int i = threadIdx.x; i < D * T; i += blockDim.x) x0_out[base + i] = i < R * T ? xs[i] : x0[base + i];
 }

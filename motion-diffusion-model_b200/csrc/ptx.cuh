@@ -158,6 +158,15 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// the two halves of cluster_sync_all, for work in between (every thread of the cluster calls both, in turn)
+__device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+// a float of a peer CTA's shared memory (address from mapa_shared)
+__device__ __forceinline__ float ld_shared_cluster_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+  return v;
+}
 // 8 bytes into the shared memory of a peer CTA + complete_tx(8) on an mbarrier of that CTA, as ONE asynchronous message:
 // the receiver sees the data once its barrier phase completes; the sender needs no fence.
 __device__ __forceinline__ void st_async_f32x2(uint32_t remote_addr, float a, float b, uint32_t remote_bar) {

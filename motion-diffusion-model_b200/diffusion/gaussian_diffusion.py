@@ -256,6 +256,7 @@ class GaussianDiffusion:
         joint = r.wrapper.targets(y, shape) if r.kind == "joint" else None
         contact = r.wrapper.foot_contact(y, shape) if r.kind == "joint" else None
         scene = r.wrapper.scene(y, shape) if r.kind == "joint" else None
+        inter = r.wrapper.interaction(y, shape) if r.kind == "joint" else None
         if r.kind == "multi":
             r.wrapper.prompts(y, shape)              # y's prompts checked before any engine work
         eng, guided = engine_for(model)
@@ -274,11 +275,13 @@ class GaussianDiffusion:
             jc = r.wrapper
             eng.set_joint_guidance(jc.mean.to(device), jc.std.to(device), joint[0].to(device), joint[1].to(device),
                                    jc.step_size, jc.n_iters)
-            if jc.foot or scene is not None:     # (both weights 0 with a scene: its lengths)
+            if jc.foot or scene is not None or inter is not None:     # (both weights 0: the lengths)
                 eng.set_foot_guidance(jc.contact_weight, jc.floor_weight, jc.floor_height,
                                       None if contact is None else contact.to(device), y.get("lengths"))
             if scene is not None:
                 eng.set_scene_guidance(jc.obstacle_weight, jc.obstacle_margin, *scene)
+            if inter is not None:
+                eng.set_interaction_guidance(jc.characters, jc.interaction_weight, jc.interaction_margin, *inter)
         if table == "next":
             eng.set_schedule_next(self.schedule_next_rows(), key=(id(self), self.num_timesteps))
         elif table == "dpm":

@@ -127,6 +127,48 @@ def scene_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weig
     return out, loss
 
 
+def _interaction(characters, weight, margin, placement, pairs, reach, pair_weight, device):
+    """(the interaction arguments of b200mdm_set_interaction_guidance after the engine, the tensors they point to):
+    placement [B, 3], pairs int [N, 4] or None, reach [N], pair_weight [N, T] (every scene) or [B / C, N, T]"""
+    pl = placement.to(device=device, dtype=torch.float32).contiguous()
+    n = 0 if pairs is None else int(pairs.shape[0])
+    if n == 0:
+        return (int(characters), float(weight), float(margin), _ptr(pl), None, 0, None, None, 0), (pl,)
+    rows = np.ascontiguousarray(np.asarray(pairs.cpu() if torch.is_tensor(pairs) else pairs, dtype=np.int32).reshape(n, 4))
+    dist = np.ascontiguousarray(np.asarray(reach.cpu() if torch.is_tensor(reach) else reach, dtype=np.float32).reshape(n))
+    pw = pair_weight.to(device=device, dtype=torch.float32).contiguous()
+    stride = int(pw.shape[1] * pw.shape[2]) if pw.dim() == 3 else 0
+    return ((int(characters), float(weight), float(margin), _ptr(pl), rows.ctypes.data_as(ctypes.c_void_p), n,
+             dist.ctypes.data_as(ctypes.c_void_p), _ptr(pw), stride), (pl, rows, dist, pw))
+
+
+def interaction_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weight, floor_weight, floor_height,
+                              obstacle_weight, obstacle_margin, sdf, terrain, characters, interaction_weight,
+                              interaction_margin, placement, pairs=None, reach=None, pair_weight=None, contact=None,
+                              lengths=None):
+    """The guidance iterations with the foot, scene and interaction terms alone (b200mdm_test_interaction_guidance), on
+    x0's device: (guided x0 [B, D, T], total G [iters + 1, B], each pair's energy at its lower rank).  placement [B, 3],
+    pairs int [N, 4] scene-local (a, j, b, k) or None, reach [N], pair_weight [N, T] or [B / C, N, T]; the other
+    arguments as scene_guidance_hook's."""
+    lib = _lib.load()
+    x0, mean, std, target, weight = (t.to(torch.float32).contiguous() for t in (x0, mean, std, target, weight))
+    B, D, T = int(x0.shape[0]), int(x0.shape[1]), int(x0.shape[-1])
+    kappa = None if contact is None else contact.to(device=x0.device, dtype=torch.float32).contiguous()
+    n = _lengths_host(lengths, B)
+    (gs, vs), (gt, vt) = _grid(sdf, x0.device), _grid(terrain, x0.device)
+    args, keep = _interaction(characters, interaction_weight, interaction_margin, placement, pairs, reach, pair_weight,
+                              x0.device)
+    out = torch.empty_like(x0)
+    loss = torch.empty((int(iters) + 1, B), device=x0.device, dtype=torch.float32)
+    check(lib.b200mdm_test_interaction_guidance(_ptr(x0), _ptr(mean), _ptr(std), _ptr(target), _ptr(weight),
+                                                None if kappa is None else _ptr(kappa),
+                                                None if n is None else n.ctypes.data_as(ctypes.c_void_p), B, T, D,
+                                                float(step), int(iters), float(contact_weight), float(floor_weight),
+                                                float(floor_height), float(obstacle_weight), float(obstacle_margin),
+                                                _grid_ref(gs), _grid_ref(gt), *args, _ptr(out), _ptr(loss), _stream()))
+    return out, loss
+
+
 class Engine:
     """One engine per model instance (weights + workspace live on the current CUDA device)."""
 
@@ -425,6 +467,7 @@ class Engine:
         self._keep["joint"] = ts
         self._keep.pop("foot", None)
         self._keep.pop("scene", None)
+        self._keep.pop("interaction", None)
 
     def set_foot_guidance(self, contact_weight, floor_weight, floor_height=0.0, contact=None, lengths=None):
         """The foot-contact and floor terms of the joint guidance set last (b200mdm_set_foot_guidance), which
@@ -437,6 +480,7 @@ class Engine:
                                                  None if n is None else n.ctypes.data_as(ctypes.c_void_p), _stream()))
         self._keep["foot"] = kappa
         self._keep.pop("scene", None)
+        self._keep.pop("interaction", None)
 
     def set_scene_guidance(self, obstacle_weight, obstacle_margin, sdf=None, terrain=None):
         """The scene terms of the joint guidance set last (b200mdm_set_scene_guidance), after set_foot_guidance (whose
@@ -447,6 +491,17 @@ class Engine:
         check(self.lib.b200mdm_set_scene_guidance(self.h, float(obstacle_weight), float(obstacle_margin), _grid_ref(gs),
                                                   _grid_ref(gt), _stream()))
         self._keep["scene"] = (vs, vt)
+        self._keep.pop("interaction", None)
+
+    def set_interaction_guidance(self, characters, weight, margin, placement, pairs=None, reach=None, pair_weight=None):
+        """The interaction terms of the joint guidance set last (b200mdm_set_interaction_guidance), after
+        set_scene_guidance or set_foot_guidance, whose terms and lengths they extend and which clear them, as do
+        set_joint_guidance and set_cond: placement [B, 3], pairs int [N, 4] scene-local (a, j, b, k) or None, reach [N],
+        pair_weight [N, T] or [B / C, N, T], copied to the engine's device."""
+        dev = torch.device("cuda", torch.cuda.current_device())
+        args, keep = _interaction(characters, weight, margin, placement, pairs, reach, pair_weight, dev)
+        check(self.lib.b200mdm_set_interaction_guidance(self.h, *args, _stream()))
+        self._keep["interaction"] = keep
 
     def set_cond_multi(self, batch, nframes, y, embed, action, weight, device):
         """Multi-prompt guidance (b200mdm_set_cond_multi / _dec / _tokens, then b200mdm_set_prompt_weight): embed fp32

@@ -66,14 +66,17 @@ def gather_objects(obj, group=None):
 
 _BATCH_KEYS = ("mask", "lengths", "scale", "action", "inpainting_mask", "inpainted_motion", "prefix", "target_cond",
                "is_heading", "motion_start", "inpainting_weight", "joint_target", "joint_weight", "prompt_action",
-               "prompt_weight", "foot_contact")
+               "prompt_weight", "foot_contact", "scene_placement")
 
 
-def shard_model_kwargs(model_kwargs, lo, hi):
+def shard_model_kwargs(model_kwargs, lo, hi, characters=1):
     """Slice the reference's `y` dict (data_loaders/tensors.py:22-64 schema) along the batch dimension.  With
     y['motion_start'] (chained windows, HandshakeSampleModel) both ends of the slice must be motion boundaries: a motion
-    is never split across shards (ValueError)."""
+    is never split across shards (ValueError).  With `characters` C > 1 (JointControlSampleModel scenes) both ends must
+    be scene boundaries (ValueError), and a per-scene y['interaction_pair_weight'] [B / C, N, T] is sliced by scene."""
     y = model_kwargs["y"]
+    if lo % characters or hi % characters:
+        raise ValueError("shard [%d, %d) cuts a scene of %d characters" % (lo, hi, characters))
     if y.get("motion_start") is not None:
         ms = np.asarray(y["motion_start"].detach().cpu() if torch.is_tensor(y["motion_start"]) else y["motion_start"]).astype(bool)
         for edge in (lo, hi):
@@ -95,6 +98,8 @@ def shard_model_kwargs(model_kwargs, lo, hi):
             out[k] = (v[lo:hi] if v.dim() == 3 else v[:, lo:hi]).contiguous()
         elif k in _BATCH_KEYS and torch.is_tensor(v):
             out[k] = v[lo:hi].contiguous()
+        elif k == "interaction_pair_weight" and torch.is_tensor(v) and v.dim() == 3:   # per scene; [N, T] as it is
+            out[k] = v[lo // characters:hi // characters].contiguous()
         elif k in ("obstacle_sdf", "terrain") and isinstance(v, SceneGrid):  # per-sample grids; a shared one as it is
             out[k] = v.shard(lo, hi)
         elif k in ("text", "tokens", "target_joint_names", "prompt_text") and isinstance(v, (list, tuple)):
@@ -128,7 +133,8 @@ def sample_sharded(sample_fn, model, shape, model_kwargs, *, n_steps, noise_mode
                          % world)
     if torch.is_tensor(y.get("text_embed")) or isinstance(y.get("text_embed"), tuple):
         broadcast_text_embed(y["text_embed"], 0, group)
-    local_kwargs = shard_model_kwargs(model_kwargs, lo, hi)
+    r = resolve(model)
+    local_kwargs = shard_model_kwargs(model_kwargs, lo, hi, r.wrapper.characters if r.kind == "joint" else 1)
     local_shape = (hi - lo,) + tuple(shape[1:])
     if device is None:
         te = y.get("text_embed")

@@ -175,11 +175,21 @@ class JointControlSampleModel(_SampleWrapper):
     a SceneGrid of the obstacles' 2D signed distance (positive outside; SceneGrid.from_shapes builds it for discs and
     boxes), and y['terrain'], a SceneGrid of heights, raises the floor to floor_height + H(p.x, p.z).  Either grid is
     shared by the batch or has one grid per sample.  With obstacle_weight > 0, y['joint_target'] / y['joint_weight'] are
-    optional."""
+    optional.
+
+    Several characters in one scene (DESIGN.md "Joint-position control", "Several characters in one scene"): with
+    `characters` = C >= 2 the batch is B / C scenes, motions [sC, sC + C) forming scene s.  y['scene_placement'] [B, 3]
+    (x, z, phi) places each motion's own frame in its scene, Q = rot(phi) p + (x, 0, z) with rot(phi) (x, z) =
+    (x cos phi - z sin phi, x sin phi + z cos phi); the other terms keep reading the own frame.  `interaction_weight`
+    adds 1/2 interaction_weight sum_{a<b} sum_{t<L_ab} sum_{j,k} max(interaction_margin - |Q_a[t,j] - Q_b[t,k]|, 0)^2 over
+    each scene's pairs, L_ab = min(lengths[a], lengths[b]); the reach rows y['interaction_pairs'] int [N, 4] (scene-local
+    a, j, b, k with a != b), y['interaction_reach'] [N] and y['interaction_pair_weight'] [N, T] (every scene) or
+    [B / C, N, T] add 1/2 sum_n sum_{t<L_ab} w_n[t] max(|Q_a[t,j] - Q_b[t,k]| - reach_n, 0)^2.  With C >= 2,
+    y['joint_target'] / y['joint_weight'] are optional."""
     kind = "joint"
 
     def __init__(self, model, mean, std, step_size, n_iters, *, contact_weight=0.0, floor_weight=0.0, floor_height=0.0,
-                 obstacle_weight=0.0, obstacle_margin=0.0):
+                 obstacle_weight=0.0, obstacle_margin=0.0, characters=1, interaction_weight=0.0, interaction_margin=0.0):
         core = _core(model)
         if core is None:
             raise TypeError("JointControlSampleModel wraps a b200mdm MDM or ClassifierFreeSampleModel (got %r)" % type(model))
@@ -208,12 +218,21 @@ class JointControlSampleModel(_SampleWrapper):
         if not (np.isfinite(ow) and ow >= 0 and np.isfinite(om) and om >= 0):
             raise ValueError("obstacle_weight and obstacle_margin must be finite and >= 0 (got %r, %r)"
                              % (obstacle_weight, obstacle_margin))
+        if isinstance(characters, bool) or not isinstance(characters, (int, np.integer)) or not 1 <= characters <= 8:
+            raise ValueError("characters must be an integer in 1 .. 8 (got %r)" % (characters,))
+        iw, im = float(interaction_weight), float(interaction_margin)
+        if not (np.isfinite(iw) and iw >= 0 and np.isfinite(im) and im >= 0):
+            raise ValueError("interaction_weight and interaction_margin must be finite and >= 0 (got %r, %r)"
+                             % (interaction_weight, interaction_margin))
+        if characters == 1 and iw > 0:
+            raise ValueError("interaction_weight > 0 needs characters >= 2")
         super().__init__(model)
         self.mean, self.std = mean, std
         self.step_size, self.n_iters = step, int(iters)
         self.n_joints = 22 if D == 263 else 21
         self.contact_weight, self.floor_weight, self.floor_height = cw, fw, fh
         self.obstacle_weight, self.obstacle_margin = ow, om
+        self.characters, self.interaction_weight, self.interaction_margin = int(characters), iw, im
 
     @property
     def foot(self):
@@ -225,7 +244,7 @@ class JointControlSampleModel(_SampleWrapper):
         missing key, a shape other than these, a weight that is negative or not finite, or a target that is not finite
         where its weight is not 0."""
         B, T, J = int(shape[0]), int(shape[-1]), self.n_joints
-        if (self.foot or self.obstacle_weight > 0) and "joint_target" not in y and "joint_weight" not in y:
+        if (self.foot or self.obstacle_weight > 0 or self.characters > 1) and "joint_target" not in y and "joint_weight" not in y:
             return torch.zeros(B, J, 3, T), torch.zeros(B, J, T)      # no joint term: a target the kernel never reads
         if "joint_target" not in y or "joint_weight" not in y:
             raise ValueError("JointControlSampleModel needs y['joint_target'] [B, %d, 3, T] and y['joint_weight'] [B, %d, T]"
@@ -284,6 +303,49 @@ class JointControlSampleModel(_SampleWrapper):
             if g.per_sample and g.values.shape[0] != B:
                 raise ValueError("y[%r] has %d grids for %d samples" % (name, g.values.shape[0], B))
         return None if sdf is None and terrain is None else (sdf, terrain)
+
+    def interaction(self, y, shape):
+        """(placement [B, 3], pairs int64 [N, 4] or None, reach [N] or None, pair weight [N, T] / [B / C, N, T] or None)
+        fp32 of y, or None with one character per scene; y is not modified.  ValueError for a batch that is not a whole
+        number of scenes, a missing or misshaped placement, reach rows without their reach or weights, a row outside
+        the scene or its joints or with a == b, or a reach or weight that is negative or not finite."""
+        keys = ("scene_placement", "interaction_pairs", "interaction_reach", "interaction_pair_weight")
+        if self.characters == 1:
+            if any(k in y for k in keys):
+                raise ValueError("y[%r] needs characters >= 2" % next(k for k in keys if k in y))
+            return None
+        B, T, C, J = int(shape[0]), int(shape[-1]), self.characters, self.n_joints
+        if B % C:
+            raise ValueError("a batch of %d motions is not a whole number of %d-character scenes" % (B, C))
+        pl = y.get("scene_placement")
+        if not torch.is_tensor(pl) or tuple(pl.shape) != (B, 3) or not pl.is_floating_point():
+            raise ValueError("characters >= 2 needs y['scene_placement'], a float tensor [%d, 3] (x, z, phi)" % B)
+        pl = pl.to(torch.float32)
+        if not bool(torch.isfinite(pl).all()):
+            raise ValueError("y['scene_placement'] must be finite")
+        if y.get("interaction_pairs") is None:
+            return pl, None, None, None
+        pairs, reach, pw = y["interaction_pairs"], y.get("interaction_reach"), y.get("interaction_pair_weight")
+        pairs = torch.as_tensor(pairs)
+        if pairs.dim() != 2 or pairs.shape[1] != 4 or pairs.is_floating_point() or pairs.dtype == torch.bool:
+            raise ValueError("y['interaction_pairs'] must be an integer tensor [N, 4] (got %s)" % (tuple(pairs.shape),))
+        N = int(pairs.shape[0])
+        if not 1 <= N <= 1024:
+            raise ValueError("y['interaction_pairs'] holds 1 .. 1024 rows (got %d)" % N)
+        pairs = pairs.to(torch.int64).cpu()
+        a, j, b, k = pairs.unbind(1)
+        if bool(((a < 0) | (a >= C) | (b < 0) | (b >= C) | (a == b) | (j < 0) | (j >= J) | (k < 0) | (k >= J)).any()):
+            raise ValueError("y['interaction_pairs'] rows (a, j, b, k) need 0 <= a, b < %d, a != b and 0 <= j, k < %d"
+                             % (C, J))
+        if not torch.is_tensor(reach) or tuple(reach.shape) != (N,) or not reach.is_floating_point():
+            raise ValueError("y['interaction_pairs'] needs y['interaction_reach'], a float tensor [%d]" % N)
+        if not torch.is_tensor(pw) or tuple(pw.shape) not in ((N, T), (B // C, N, T)) or not pw.is_floating_point():
+            raise ValueError("y['interaction_pairs'] needs y['interaction_pair_weight'], a float tensor %s or %s"
+                             % ((N, T), (B // C, N, T)))
+        reach, pw = reach.to(torch.float32), pw.to(torch.float32)
+        if not bool((torch.isfinite(reach) & (reach >= 0)).all()) or not bool((torch.isfinite(pw) & (pw >= 0)).all()):
+            raise ValueError("y['interaction_reach'] and y['interaction_pair_weight'] must be finite and >= 0")
+        return pl, pairs, reach, pw
 
     def forward(self, x, timesteps, y=None):
         return self.model(x, timesteps, y)
