@@ -377,6 +377,43 @@ int b200mdm_sample_loop_range(b200mdm_engine* e, int32_t mode, int32_t first_ind
                               float* x_out_dev, const float* noise_tape_dev, int64_t noise_step_stride, int32_t flags,
                               int32_t use_graph, void* stream);
 
+/* ---- continuous batching (DESIGN.md, "Continuous batching")
+ * One p_sample / ddim_sample where sample b takes its own schedule index index_host[b] (b = 0 .. batch - 1), as the
+ * reference's per-sample t does: the model embeds each sample's timestep and the update reads each sample's schedule row.
+ * Each row is bitwise the row of b200mdm_sample_step at that row's index.  noise_dev [B, ...] is required; the only
+ * valid flag is B200MDM_FLAG_CLIP_DENOISED (B200MDM_FLAG_CONST_NOISE returns ENOTIMPL).  ENOTIMPL for BERT-memory
+ * decoders, target conditioning, inpainting, handshakes, joint-position control and multi-prompt guidance.  Ends a slot
+ * session (it reuses the slot state). */
+int b200mdm_sample_step_at(b200mdm_engine* e, int32_t mode, const int32_t* index_host, const float* x_t_dev,
+                           const float* noise_dev, int32_t flags, float* x_out_dev, float* pred_xstart_dev, void* stream);
+
+/* A slot session: the (slots, nframes, guided ? 2 : 1) workspace, every row a slot that runs its own request at its own
+ * schedule index of the current schedule (mode B200MDM_MODE_DDPM, or B200MDM_MODE_DDIM with the rows uploaded for the
+ * caller's eta).  Every slot starts idle and x is zeroed.  flags: B200MDM_FLAG_CLIP_DENOISED (B200MDM_FLAG_PHILOX_NOISE
+ * is implied: every eps comes from the request's own Philox stream).  ENOTIMPL for other modes, for
+ * B200MDM_FLAG_CONST_NOISE and for BERT-memory decoders.  The session ends at the next b200mdm_set_cond* call (or
+ * b200mdm_sample_step_at); the per-loop features (target, inpainting, handshakes, guidance) are cleared here, and
+ * b200mdm_slots_run refuses any set later. */
+int b200mdm_slots_begin(b200mdm_engine* e, int32_t slots, int32_t nframes, int32_t guided, int32_t mode, int32_t flags,
+                        void* stream);
+
+/* Admit one request into an idle slot (ESTATE while the slot holds a request not yet read): its condproj rows in both
+ * classifier-free halves (cond_embed_dev: its text / CLIP row [cond_dim] on the device; NULL for an unconditioned model),
+ * action (action models), its guidance scale (guided sessions), its frame count `length` (< 0: every frame valid; used
+ * under mask_frames), its x_T -- b200mdm_philox_normal of (seed, global sample index sample_index, step id -1) -- and
+ * its Philox key for every step, starting at schedule index n_steps - 1.  A request admitted into slot b gives bitwise
+ * row b of a uniform Philox loop with noise_seed = seed and sample_index_base = sample_index - b.  No synchronisation. */
+int b200mdm_slot_admit(b200mdm_engine* e, int32_t slot, const float* cond_embed_dev, int64_t action, float scale,
+                       int64_t length, uint64_t seed, int64_t sample_index, void* stream);
+
+/* n_steps steps of every slot: the slot step graph replayed n_steps times (use_graph != 0), or the same launches.  A
+ * slot finishes after n_steps (the schedule length) steps since its admission; the rest of its steps write nothing. */
+int b200mdm_slots_run(b200mdm_engine* e, int32_t n_steps, int32_t use_graph, void* stream);
+
+/* Copy a finished slot's sample [njoints * nfeats, nframes] to out_dev and free the slot.  ESTATE unless the slot has
+ * run all its steps. */
+int b200mdm_slot_read(b200mdm_engine* e, int32_t slot, float* out_dev, void* stream);
+
 /* ddim_reverse_sample (gaussian_diffusion.py:838-874) repeated without returning to the host: schedule indices
  * first_index, first_index+1, ... (n_run of them, up to n_steps - 1) on the engine's working buffer, one CUDA graph of a
  * single step replayed when use_graph != 0.  x_in_dev / x_out_dev NULL as in b200mdm_sample_loop_range.  flags:

@@ -41,6 +41,7 @@ SYMBOLS = [
     "b200mdm_set_cond_multi_tokens", "b200mdm_set_foot_guidance", "b200mdm_test_foot_guidance",
     "b200mdm_set_scene_guidance", "b200mdm_test_scene_guidance", "b200mdm_chain_set_goal", "b200mdm_chunk_frame",
     "b200mdm_set_interaction_guidance", "b200mdm_test_interaction_guidance",
+    "b200mdm_sample_step_at", "b200mdm_slots_begin", "b200mdm_slot_admit", "b200mdm_slots_run", "b200mdm_slot_read",
 ]
 MAX_PROMPTS = 8                             # B200MDM_MAX_PROMPTS
 MAX_CHARACTERS = 8                          # characters per scene: one cluster of at most 8 CTAs
@@ -101,6 +102,11 @@ def load():
     lib.b200mdm_recover_from_ric.argtypes = [vp, i64, i64, i64, vp, vp, vp, i64, i64, i64, i32, i32, i32, vp]
     lib.b200mdm_denoise.argtypes = [vp, vp, vp, vp, vp]
     lib.b200mdm_sample_step.argtypes = [vp, i32, i32, vp, vp, i32, vp, vp, vp]
+    lib.b200mdm_sample_step_at.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, vp]
+    lib.b200mdm_slots_begin.argtypes = [vp, i32, i32, i32, i32, i32, vp]
+    lib.b200mdm_slot_admit.argtypes = [vp, i32, vp, i64, f32, i64, ctypes.c_uint64, i64, vp]
+    lib.b200mdm_slots_run.argtypes = [vp, i32, i32, vp]
+    lib.b200mdm_slot_read.argtypes = [vp, i32, vp, vp]
     lib.b200mdm_sample_loop.argtypes = [vp, i32, i32, vp, vp, vp, i64, i32, i32, vp]
     lib.b200mdm_sample_loop_range.argtypes = [vp, i32, i32, i32, vp, vp, vp, i64, i32, i32, vp]
     lib.b200mdm_set_noise_stream.argtypes = [vp, ctypes.c_uint64, i64]

@@ -154,11 +154,12 @@ struct GraphKey {
   bool scene = false;               // ... and the scene terms: joint_guidance_step_kernel<true, true>
   bool inter = false;               // ... and the interaction terms: joint_guidance_step_kernel<true, true, true>
   int chars = 0;                    //     in clusters of `chars` CTAs
+  bool slots = false;               // continuous batching: a schedule index per row (b200mdm_slots_begin)
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
            imask == o.imask && iweight == o.iweight && imotion == o.imotion && target_g == o.target_g && hs == o.hs &&
            guided == o.guided && groups == o.groups && foot == o.foot && scene == o.scene && inter == o.inter &&
-           chars == o.chars;
+           chars == o.chars && slots == o.slots;
   }
 };
 
@@ -218,6 +219,9 @@ struct Workspace {
   float *vb_xs = nullptr, *vb_part = nullptr, *vb_terms = nullptr;
   int vb_cap = 0;
   bool vb_live = false;
+  // continuous batching (b200mdm_slots_begin), allocated on first use: the per-row slot state [B], read and written
+  // inside the step graph (epilogues.cuh, SlotState)
+  SlotState* slots = nullptr;
   // captured step graph of this workspace
   cudaGraphExec_t graph_exec = nullptr;
   GraphKey graph_key;
@@ -322,6 +326,14 @@ struct b200mdm_engine : Workspace {
   bool chain_mems = false;
   // the prefix of b200mdm_set_prefix (caller-owned), which b200mdm_chain_set_goal reads under include_prefix
   const float* prefix_src = nullptr;
+  // continuous batching on the workspace in use (b200mdm_slots_begin .. the next b200mdm_set_cond*): the sampler and
+  // flags of the session, and per slot whether it holds a request not yet read and how many of its steps are still to
+  // run -- the host knows when each slot finishes without asking the device
+  bool slot_mode = false;
+  int slot_sampler = 0, slot_flags = 0;
+  std::vector<unsigned char> slot_busy;
+  std::vector<int> slot_left;
+  std::vector<int> h_slot_idx;   // host staging of b200mdm_sample_step_at's indices
   // a goal-directed chain (b200mdm_chain_set_goal): the caller's mean / std [JF] and goals [n_goals, B, n_ext, 3], the
   // per-sample carry [B, CF_CARRY] and the next chunk's target [B, n_ext, 3]; live while goal_set and the chain is
   // (chain_setup clears goal_set, and everything that ends a chain sets chain_next = -1)
@@ -381,6 +393,7 @@ static int init_kernel_attrs() {
   CUDA_TRY(cudaFuncSetAttribute(gemm_resid_ln_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmLnSmem::TOTAL));
   TRY((set_gemm_attr<128, EpiEmbed>()));
   TRY((set_gemm_attr<96, EpiOut<OutStep>>()));
+  TRY((set_gemm_attr<96, EpiOut<OutStepSlots>>()));
   TRY((set_gemm_attr<96, EpiOut<OutPlms>>()));
   TRY((set_gemm_attr<96, EpiOut<OutReverse>>()));
   TRY((set_gemm_attr<96, EpiOut<OutDpm>>()));
@@ -551,12 +564,16 @@ static int launch_row_bias_ln(__half* hres, const float* c, const float* gamma, 
                     hres, c, gamma, beta, M, S, 1e-5f));
   return B200MDM_OK;
 }
+// grid of the Philox kernels over B samples of n elements (256 threads, one quad each, grid-stride beyond 1184 blocks)
+static int philox_blocks(int B, long long n) {
+  const long long quads = (n + 3) / 4 * B;
+  return static_cast<int>(quads / 256 + 1 < 1184 ? quads / 256 + 1 : 1184);
+}
 // eps [B, n] of the counter-based noise stream; state != nullptr: seed, sample base and step come from the step state
 static int launch_philox(float* out, int B, long long n, unsigned long long seed, long long sample_base, uint32_t step_id,
                          const StepState* state, cudaStream_t s) {
-  const long long quads = (n + 3) / 4 * B;
-  const int blocks = static_cast<int>(quads / 256 + 1 < 1184 ? quads / 256 + 1 : 1184);
-  CUDA_TRY(launch_k(philox_normal_kernel, dim3(blocks), dim3(256), 0, s, out, B, n, seed, sample_base, step_id, state));
+  CUDA_TRY(launch_k(philox_normal_kernel, dim3(philox_blocks(B, n)), dim3(256), 0, s, out, B, n, seed, sample_base, step_id,
+                    state));
   return B200MDM_OK;
 }
 // x [B, JF, cols] -> rows row_off .. row_off + cols of every S-row sequence of the embedding GEMM's A operand [hi | lo | hi]
@@ -722,7 +739,7 @@ static void free_workspace(Workspace* w) {
   drop_graph(w);
   dfree(w->xin16); dfree(w->hres); dfree(w->qkv16); dfree(w->att16); dfree(w->ffn16); dfree(w->g16);
   dfree(w->tok0); dfree(w->condproj); dfree(w->proj); dfree(w->scale); dfree(w->x_work); dfree(w->pe_bias); dfree(w->eps_buf);
-  dfree(w->kvlen); dfree(w->tvec); dfree(w->action);
+  dfree(w->kvlen); dfree(w->tvec); dfree(w->action); dfree(w->slots);
   dfree(w->encperm); dfree(w->memtok); dfree(w->memproj); dfree(w->mem16); dfree(w->qc16); dfree(w->kvc16); dfree(w->memmask);
   dfree(w->cross_mb); dfree(w->cross_u); dfree(w->cross_b); dfree(w->cross_c);
   dfree(w->tgt_valid); dfree(w->tgt_g); dfree(w->hs_desc); dfree(w->jg_x0); dfree(w->mp_x0);
@@ -1291,12 +1308,16 @@ static int upload_kvlen_scale(b200mdm_engine* e, int nframes, int seq_extra, boo
 // condproj rows of the packed batch: proj = embed_text(text) [rows, d] when the model is text-conditioned and a text is
 // given (model/mdm.py:218), then the conditional / unconditional rows of the model's conditioning mode
 // (condproj_fill_kernel).  The rows = K * batch conditional rows (text_dev [K, batch, C], action [K * batch]) come first.
-static int fill_condproj(b200mdm_engine* e, const float* text_dev, bool uncond, int rows, cudaStream_t s) {
+// slot >= 0 (b200mdm_slot_admit): text_dev is that one row's text, projected into proj row `slot`; every condproj row
+// is then refilled from proj as it is, which rewrites the other rows with their own bits.
+static int fill_condproj(b200mdm_engine* e, const float* text_dev, bool uncond, int rows, cudaStream_t s, int slot = -1) {
   const int d = e->d;
   if (e->cfg.cond_mode == B200MDM_COND_TEXT && text_dev) {
-    const size_t warps = static_cast<size_t>(rows) * d;
-    small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(text_dev, e->w_txt, e->b_txt, e->proj, rows,
-                                                                                       d, e->cfg.cond_dim, e->cfg.cond_dim);
+    const int n = slot >= 0 ? 1 : rows;
+    const size_t warps = static_cast<size_t>(n) * d;
+    small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(
+        text_dev, e->w_txt, e->b_txt, e->proj + static_cast<size_t>(slot >= 0 ? slot : 0) * d, n, d, e->cfg.cond_dim,
+        e->cfg.cond_dim);
     CUDA_TRY(cudaGetLastError());
     e->launches++;
   }
@@ -1321,6 +1342,7 @@ static void end_cond(b200mdm_engine* e) {
   e->pw_set = false;
   e->vb_live = false;
   e->chain_next = -1;
+  e->slot_mode = false;
 }
 
 // cb_l[b']= W_o,l (W_v,l mb[b'] + b_v,l) + b_o,l with mb = condproj (+ g): the per-sample part of the cross-attention rows
@@ -1407,8 +1429,8 @@ static int build_text_memory(b200mdm_engine* e, const float* tokens, int K, bool
 // ---- features that exclude each other or a sampler family.  The engine's twin of _REFUSED in
 // diffusion/gaussian_diffusion.py, with the same sampler rows; the setter rows make handshakes, joint-position control
 // and multi-prompt guidance pairwise exclusive and keep each off prefix-completion (DiP) engines.
-enum Feature : unsigned { F_PREFIX = 1, F_HANDSHAKE = 2, F_JOINT = 4, F_MULTI = 8 };
-enum Family { FAM_REVERSE, FAM_PLMS, FAM_DPM, FAM_VB, FAM_HANDSHAKE, FAM_JOINT, FAM_MULTI };
+enum Feature : unsigned { F_PREFIX = 1, F_HANDSHAKE = 2, F_JOINT = 4, F_MULTI = 8, F_TOKENS = 16, F_TARGET = 32, F_INPAINT = 64 };
+enum Family { FAM_REVERSE, FAM_PLMS, FAM_DPM, FAM_VB, FAM_HANDSHAKE, FAM_JOINT, FAM_MULTI, FAM_SLOTS };
 static const struct {
   const char* name;
   unsigned refuses;
@@ -1420,16 +1442,19 @@ static const struct {
     {"handshaking", F_PREFIX | F_JOINT | F_MULTI},
     {"joint-position control", F_PREFIX | F_HANDSHAKE | F_MULTI},
     {"multi-prompt guidance", F_PREFIX},
+    // a schedule index per row: every per-loop input but the conditioning rows, scale and lengths is one for the batch
+    {"continuous batching", F_PREFIX | F_HANDSHAKE | F_JOINT | F_MULTI | F_TOKENS | F_TARGET | F_INPAINT},
 };
 
 // ENOTIMPL when the engine holds a feature (of those in `among`) that `family` refuses
 static int refuse(const b200mdm_engine* e, Family family, unsigned among = ~0u) {
   static const char* const feature[] = {"prefix-completion (DiP) models", "handshakes", "joint-position control",
-                                        "multi-prompt guidance"};
+                                        "multi-prompt guidance", "BERT text memories", "target conditioning", "inpainting"};
   const unsigned live = (is_prefix_engine(e) ? F_PREFIX : 0u) | (e->hs_set ? F_HANDSHAKE : 0u) | (e->jg_set ? F_JOINT : 0u) |
-                        (e->groups ? F_MULTI : 0u);
+                        (e->groups ? F_MULTI : 0u) | (e->dec && !e->dec_clip ? F_TOKENS : 0u) |
+                        (e->target_set ? F_TARGET : 0u) | (e->inpaint_mask || e->inpaint_weight ? F_INPAINT : 0u);
   const unsigned hit = REFUSED[family].refuses & among & live;
-  for (int i = 0; i < 4; ++i)
+  for (int i = 0; i < 7; ++i)
     if (hit & (1u << i)) return fail(B200MDM_ENOTIMPL, "%s with %s is not implemented", REFUSED[family].name, feature[i]);
   return B200MDM_OK;
 }
@@ -1873,6 +1898,7 @@ struct StepArgs {
   const float* x_step = nullptr;  // MODE_PLMS_EULER2: x_t of the step
   int order = 0;                  // MODE_PLMS_AB
   bool model_only = false;        // b200mdm_denoise: the bare model output, without the engine's inpainting
+  bool slots = false;             // a schedule index per row (e->slots): OutStepSlots, philox_slots_kernel, slot_advance_kernel
 };
 
 // The per-step fields of the output step's parameters (p already holds the tables, the step state and the inpainting
@@ -1897,6 +1923,7 @@ static int launch_out_gemm(const CUtensorMap& m_g16, const CUtensorMap& m_wout, 
                            const StepArgs& a, EpiOutParams p, cudaStream_t s, int sms) {
   set_step_params(&p, a, B, T, JF);
   const int M = B * T, N = ((JF + 95) / 96) * 96, K = 3 * d;
+  if (a.slots) return launch_gemm<96, EpiOut<OutStepSlots>>(m_g16, m_wout, M, N, K, p, s, sms);
   if (a.mode <= MODE_DDIM) return launch_gemm<96, EpiOut<OutStep>>(m_g16, m_wout, M, N, K, p, s, sms);
   if (a.mode == MODE_DDIM_REVERSE) return launch_gemm<96, EpiOut<OutReverse>>(m_g16, m_wout, M, N, K, p, s, sms);
   if (a.mode == MODE_DPM) return launch_gemm<96, EpiOut<OutDpm>>(m_g16, m_wout, M, N, K, p, s, sms);
@@ -1979,7 +2006,12 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
   const int d = e->d, ff = e->ff, B = e->B, T = e->T, S = e->S, JF = e->JF, Kp = e->Kp_in;
   int nk = 0;
   PdlScope pdl_scope;
-  if (a.philox) {
+  if (a.philox && a.slots) {
+    const long long n = static_cast<long long>(JF) * T;
+    CUDA_TRY(launch_k(philox_slots_kernel, dim3(philox_blocks(B, n)), dim3(256), 0, s, e->eps_buf, B, n,
+                      static_cast<const SlotState*>(e->slots)));
+    ++nk;
+  } else if (a.philox) {
     TRY(launch_philox(e->eps_buf, B, static_cast<long long>(JF) * T, 0ull, 0ll, 0u, e->state, s));
     ++nk;
   }
@@ -2089,6 +2121,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
     p.x_start = e->vb_xs;
     p.vb_part = e->vb_part;
     p.state = e->state;
+    p.slots = e->slots;
     if (G) {
       // multi-prompt guidance: the output GEMM writes every group's raw x0, compose_step_kernel composes it and runs the
       // step's tail (the bare model output too: b200mdm_denoise composes, without inpainting)
@@ -2258,6 +2291,9 @@ extern "C" int b200mdm_sample_step(b200mdm_engine* e, int32_t mode, int32_t inde
 // Move the step state to the next step of the loop: down the schedule, or up it for the DDIM inversion.
 static cudaError_t launch_advance(b200mdm_engine* e, const StepArgs& a, cudaStream_t s) {
   PdlScope pdl_scope;
+  if (a.slots)
+    return launch_k(slot_advance_kernel, dim3((e->B + 127) / 128), dim3(128), 0, s, e->slots, e->tvec,
+                    static_cast<const int*>(e->tmap), e->B);
   return launch_k(step_advance_kernel, dim3(1), dim3(1), 0, s, e->state, a.mode == MODE_DDIM_REVERSE ? 1 : -1);
 }
 
@@ -2347,6 +2383,7 @@ static int loop_enter(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32
     key.inter = e->jg_set && e->ig_set;
     key.chars = key.inter ? e->h_ig.chars : 0;
     key.groups = e->groups;
+    key.slots = a.slots;
     TRY(ensure_step_graph(e, key, a));
     CUDA_TRY(cudaEventRecord(e->ev_in, user));
     CUDA_TRY(cudaStreamWaitEvent(e->work, e->ev_in, 0));
@@ -2451,6 +2488,146 @@ extern "C" int b200mdm_sample_loop(b200mdm_engine* e, int32_t mode, int32_t skip
   if (!x_T_dev || !x_0_dev) return fail(B200MDM_EINVAL, "null tensor");
   return b200mdm_sample_loop_range(e, mode, e->n_steps - 1 - skip_timesteps, e->n_steps - skip_timesteps, x_T_dev, x_0_dev,
                                    noise_tape_dev, noise_step_stride, flags, use_graph, stream);
+}
+
+// ------------------------------------------------------------------------------------------------ continuous batching
+// DESIGN.md, "Continuous batching".  Every row of the workspace is a slot running its own request at its own schedule
+// index; the step graph is the uniform one with three kernels swapped for their slot variants (philox_slots_kernel,
+// EpiOut<OutStepSlots>, slot_advance_kernel), and the forward reads the per-row timesteps through its explicit_t path.
+static int ensure_slots(b200mdm_engine* e) {
+  if (!e->slots) TRY(dalloc(&e->slots, e->B));
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_sample_step_at(b200mdm_engine* e, int32_t mode, const int32_t* index_host, const float* x_t_dev,
+                                      const float* noise_dev, int32_t flags, float* x_out_dev, float* pred_xstart_dev,
+                                      void* stream) {
+  TRY(check_ready(e, true));
+  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM) return fail(B200MDM_EINVAL, "bad mode");
+  if (!index_host || !x_t_dev || !noise_dev || !x_out_dev) return fail(B200MDM_EINVAL, "null argument");
+  if (flags & B200MDM_FLAG_CONST_NOISE)
+    return fail(B200MDM_ENOTIMPL, "B200MDM_FLAG_CONST_NOISE with a schedule index per sample is not implemented");
+  TRY(check_flags("b200mdm_sample_step_at", flags, B200MDM_FLAG_CLIP_DENOISED));
+  for (int b = 0; b < e->B; ++b)
+    if (index_host[b] < 0 || index_host[b] >= e->n_steps) return fail(B200MDM_EINVAL, "schedule index out of range");
+  TRY(refuse(e, FAM_SLOTS));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  TRY(ensure_slots(e));
+  e->slot_mode = false;   // the step overwrites the slot state
+  e->h_slot_idx.assign(index_host, index_host + e->B);
+  CUDA_TRY(cudaMemcpyAsync(e->tvec, e->h_slot_idx.data(), e->B * sizeof(int), cudaMemcpyHostToDevice, s));
+  slots_from_index_kernel<<<(e->B + 127) / 128, 128, 0, s>>>(e->slots, e->tvec, e->tmap, e->B);
+  CUDA_TRY(cudaGetLastError());
+  StepArgs a;
+  a.mode = mode;
+  a.x_in = x_t_dev;
+  a.noise = noise_dev;
+  a.clip = (flags & B200MDM_FLAG_CLIP_DENOISED) ? 1 : 0;
+  a.x_out = x_out_dev;
+  a.pred = pred_xstart_dev;
+  a.explicit_t = true;
+  a.slots = true;
+  int nk = 0;
+  TRY(enqueue_forward(e, a, s, &nk));
+  e->launches += nk + 1;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_slots_begin(b200mdm_engine* e, int32_t slots, int32_t nframes, int32_t guided, int32_t mode,
+                                   int32_t flags, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
+  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
+  if (slots <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad slots / nframes");
+  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM)
+    return fail(B200MDM_ENOTIMPL, "continuous batching runs DDPM and DDIM (PLMS, DPM-Solver++, DDIM inversion and the "
+                "bound carry history or tables that are not per slot)");
+  if (flags & B200MDM_FLAG_CONST_NOISE) return fail(B200MDM_ENOTIMPL, "B200MDM_FLAG_CONST_NOISE with continuous batching");
+  TRY(check_flags("continuous batching", flags, B200MDM_FLAG_CLIP_DENOISED | B200MDM_FLAG_PHILOX_NOISE));
+  if (e->dec && !e->dec_clip) return fail(B200MDM_ENOTIMPL, "continuous batching with BERT text memories is not implemented");
+  if (guided && e->cfg.cond_mode == B200MDM_COND_NONE)
+    return fail(B200MDM_EINVAL, "classifier-free guidance needs a conditioned model (sampler_util.py:29)");
+  TRY(check_seq_len(e, nframes + 1));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  TRY(select_workspace(e, slots, nframes, guided ? 2 : 1, s));
+  TRY(ensure_slots(e));
+  slots_reset_kernel<<<(e->Bp + 127) / 128, 128, 0, s>>>(e->slots, e->tvec, e->kvlen, e->scale,
+                                                         e->cfg.cond_mode == B200MDM_COND_ACTION ? e->action : nullptr,
+                                                         e->tmap, e->B, e->Bp, e->S);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemsetAsync(e->x_work, 0, static_cast<size_t>(e->B) * e->JF * e->T * sizeof(float), s));
+  e->launches += 1;
+  end_cond(e);
+  e->slot_mode = true;
+  e->slot_sampler = mode;
+  e->slot_flags = (flags & B200MDM_FLAG_CLIP_DENOISED) | B200MDM_FLAG_PHILOX_NOISE;
+  e->slot_busy.assign(e->B, 0);
+  e->slot_left.assign(e->B, 0);
+  return B200MDM_OK;
+}
+
+static int check_slot(const b200mdm_engine* e, int32_t slot) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!e->slot_mode) return fail(B200MDM_ESTATE, "no slot session (b200mdm_slots_begin)");
+  if (slot < 0 || slot >= e->B) return fail(B200MDM_EINVAL, "slot %d outside [0, %d)", slot, e->B);
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_slot_admit(b200mdm_engine* e, int32_t slot, const float* cond_embed_dev, int64_t action,
+                                  float scale, int64_t length, uint64_t seed, int64_t sample_index, void* stream) {
+  TRY(check_slot(e, slot));
+  if (e->slot_busy[slot]) return fail(B200MDM_ESTATE, "slot %d holds a request that has not been read", slot);
+  const int mode = e->cfg.cond_mode;
+  if ((mode == B200MDM_COND_TEXT || e->dec_clip) && !cond_embed_dev)
+    return fail(B200MDM_EINVAL, "a text-conditioned model needs the request's text embedding");
+  if (mode == B200MDM_COND_ACTION && (action < 0 || action >= e->cfg.num_actions))
+    return fail(B200MDM_EINVAL, "action index out of range");
+  if (!std::isfinite(scale)) return fail(B200MDM_EINVAL, "scale must be finite");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // valid keys as upload_kvlen_scale counts them: the timestep token, then `length` frames (length < 0: every frame)
+  int kv = e->S;
+  if (e->cfg.mask_frames && length >= 0 && e->T > 1) kv = static_cast<int>(std::min<int64_t>(length, e->T)) + 1;
+  const size_t n = static_cast<size_t>(e->JF) * e->T;
+  slot_admit_kernel<<<1, 1, 0, s>>>(e->slots, e->tvec, e->kvlen, e->scale, mode == B200MDM_COND_ACTION ? e->action : nullptr,
+                                     e->tmap, slot, e->B, e->halves, e->n_steps - 1, static_cast<unsigned long long>(seed),
+                                     static_cast<long long>(sample_index), scale, kv, static_cast<int>(action));
+  CUDA_TRY(cudaGetLastError());
+  // x_T as p_sample_loop(noise_seed=seed) draws it for global sample `sample_index`
+  TRY(launch_philox(e->x_work + slot * n, 1, static_cast<long long>(n), seed, sample_index, 0xffffffffu, nullptr, s));
+  e->launches += 2;
+  TRY(fill_condproj(e, cond_embed_dev, false, e->B, s, slot));
+  if (e->dec_clip) TRY(cross_rows_per_sample(e, nullptr, s));
+  e->slot_busy[slot] = 1;
+  e->slot_left[slot] = e->n_steps;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_slots_run(b200mdm_engine* e, int32_t n_steps, int32_t use_graph, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!e->slot_mode) return fail(B200MDM_ESTATE, "no slot session (b200mdm_slots_begin)");
+  if (n_steps <= 0) return fail(B200MDM_EINVAL, "n_steps %d <= 0", n_steps);
+  TRY(check_ready(e, true));
+  TRY(refuse(e, FAM_SLOTS));
+  StepArgs a = loop_args(e, e->slot_sampler, 0, e->slot_flags, true);
+  a.explicit_t = true;
+  a.slots = true;
+  cudaStream_t user = static_cast<cudaStream_t>(stream), s;
+  TRY(loop_enter(e, a, e->slot_flags, use_graph, user, &s));
+  for (int k = 0; k < n_steps; ++k) TRY(enqueue_step(e, a, s, use_graph));
+  for (int b = 0; b < e->B; ++b) e->slot_left[b] = std::max(0, e->slot_left[b] - n_steps);
+  return loop_leave(e, use_graph, user);
+}
+
+extern "C" int b200mdm_slot_read(b200mdm_engine* e, int32_t slot, float* out_dev, void* stream) {
+  TRY(check_slot(e, slot));
+  if (!out_dev) return fail(B200MDM_EINVAL, "null tensor");
+  if (!e->slot_busy[slot] || e->slot_left[slot] > 0)
+    return fail(B200MDM_ESTATE, "slot %d has no finished request (%d steps to run)", slot, e->slot_left[slot]);
+  const size_t n = static_cast<size_t>(e->JF) * e->T;
+  CUDA_TRY(cudaMemcpyAsync(out_dev, e->x_work + slot * n, n * sizeof(float), cudaMemcpyDeviceToDevice,
+                           static_cast<cudaStream_t>(stream)));
+  e->slot_busy[slot] = 0;
+  return B200MDM_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ DDIM inversion

@@ -276,6 +276,17 @@ struct StepState {
   long long sample_base;         // ... and the global index of this workspace's sample 0
 };
 
+// One slot of a continuously batched workspace (b200mdm_slots_begin): the schedule index of the step its row takes next
+// (-1: idle, or finished and waiting to be read), and the Philox key of its request -- the stream seed and the request's
+// global sample index.  Written by the slot kernels inside the step graph, so every reader loads it through L2, as
+// load_step_state below.
+struct SlotState {
+  int cur;
+  int pad;
+  unsigned long long seed;
+  long long g;
+};
+
 // The step state as of the last step_set / step_advance.  Every reader goes through L2 (ld.global.cg), never through
 // the SM's L1 / read-only cache: under programmatic dependent launch a kernel is resident on an SM before the
 // step_advance it depends on has written the state, and an L1 line of the previous step's state -- brought in by another
@@ -327,6 +338,7 @@ struct EpiOutParams {
   int clip_denoised;        // clamp x0 to [-1, 1] after the inpainting blend (gaussian_diffusion.py:348-352)
   int order;                // mode 3: 1..4; mode 7: 1..2
   int back;                 // modes 3-5: this forward evaluates schedule index eval_index(state, back)
+  const SlotState* slots;   // OutStepSlots: [B] per-row schedule index (last, so the other fields keep their offsets)
 };
 
 // The update policies of EpiOut: the constructor reads the chunk's scalars, load() the extra inputs of one element
@@ -338,11 +350,16 @@ struct OutStep {   // modes 0-2
   __device__ __forceinline__ OutStep(const EpiOutParams& p, int b) {
     if (p.mode == MODE_X0) return;
     const StepState st = load_step_state(p.state);
-    const float* row_s = p.sched + static_cast<size_t>(st.cur) * SCHED_STRIDE;
-    c1 = row_s[0]; c2 = row_s[1]; sr = row_s[3]; srm1 = row_s[4]; sq = row_s[5]; ce = row_s[6];
-    sg = (p.mode == MODE_DDPM) ? row_s[2] : row_s[7];
+    set_row(p, st.cur);
     nz = (p.noise != nullptr ? p.noise : st.noise + static_cast<long long>(st.done) * st.noise_step_stride) +
          static_cast<long long>(b) * p.noise_batch_stride;
+  }
+  __device__ __forceinline__ OutStep() {}
+  // the scalars of schedule row i
+  __device__ __forceinline__ void set_row(const EpiOutParams& p, int i) {
+    const float* row_s = p.sched + static_cast<size_t>(i) * SCHED_STRIDE;
+    c1 = row_s[0]; c2 = row_s[1]; sr = row_s[3]; srm1 = row_s[4]; sq = row_s[5]; ce = row_s[6];
+    sg = (p.mode == MODE_DDPM) ? row_s[2] : row_s[7];
   }
   __device__ __forceinline__ In load(const EpiOutParams& p, bool in, size_t idx, int col, int t) const {
     in = in && p.mode != MODE_X0;
@@ -362,6 +379,26 @@ struct OutStep {   // modes 0-2
     p.x_out[idx] = o;
   }
   __device__ __forceinline__ void end(const EpiOutParams&, int, int) const {}
+};
+
+// DDPM / DDIM with a schedule index per row (continuous batching, b200mdm_sample_step_at): row b takes the step of its
+// slot's index, with OutStep's arithmetic, and an idle slot (index -1) writes nothing -- a finished sample stays in
+// place until it is read.  The eps is always explicit (the caller's, or the slot Philox kernel's eps_buf).
+struct OutStepSlots : OutStep {   // modes 1-2
+  bool idle;
+  __device__ __forceinline__ OutStepSlots(const EpiOutParams& p, int b) {
+    const int i = __ldcg(&p.slots[b].cur);
+    idle = i < 0;
+    if (idle) return;
+    set_row(p, i);
+    nz = p.noise + static_cast<long long>(b) * p.noise_batch_stride;
+  }
+  __device__ __forceinline__ In load(const EpiOutParams& p, bool in, size_t idx, int col, int t) const {
+    return OutStep::load(p, in && !idle, idx, col, t);
+  }
+  __device__ __forceinline__ void store(const EpiOutParams& p, size_t idx, float x0, const In& v) const {
+    if (!idle) OutStep::store(p, idx, x0, v);
+  }
 };
 
 struct OutPlms {   // modes 3-5

@@ -43,7 +43,8 @@ __global__ void pack_input_kernel(const float* __restrict__ x, __half* __restric
 // Conditioning-token rows of the sequence (reference model/mdm.py:195,218-220,251-252):
 //   h[b', s=0, :] = (condproj[b', :] + temb_table[t(b'), :]) + pe[0, :]
 //   t(b') = tvec[b' % B] when tvec != nullptr (model called with explicit timesteps), else timestep_map[i] with
-//   i = eval_index(state, back): the step in flight, or the one before it (PLMS improved Euler)
+//   i = eval_index(state, back): the step in flight, or the one before it (PLMS improved Euler).  tvec is read through
+//   L2: in slot mode slot_advance_kernel writes it inside the step graph (see load_step_state).
 // With a target embedding g [B, d] (model/mdm.py:197-199, both CFG halves): (condproj + (temb + g[b' % B])) + pe[0].
 // condproj == nullptr (the timestep token of trans_dec with emb_trans_dec, mdm.py:256): (temb + g) + pe[0], no text.
 // Runs right after the embedding GEMM (which leaves placeholder values in these rows).
@@ -56,7 +57,7 @@ __global__ void tok0_rows_kernel(__half* __restrict__ hres, const float* __restr
   pdl_launch_dependents();
   pdl_wait();
   const int bp = blockIdx.x;
-  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(load_step_state(state), back)];
+  int t = (tvec != nullptr) ? __ldcg(tvec + bp % B) : tmap[eval_index(load_step_state(state), back)];
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = static_cast<size_t>(bp) * S;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
@@ -133,6 +134,31 @@ __device__ __forceinline__ void philox4x32_10(uint32_t (&c)[4], uint32_t k0, uin
     k1 += 0xBB67AE85u;
   }
 }
+// Elements 4q .. 4q + 3 of one sample's eps (out: the sample's n elements), keyed by (seed, step_id, g).
+__device__ __forceinline__ void philox_quad(float* out, long long n, long long q, unsigned long long seed,
+                                            unsigned long long g, uint32_t step_id) {
+  uint32_t c[4] = {static_cast<uint32_t>(q), step_id, static_cast<uint32_t>(g), static_cast<uint32_t>(g >> 32) ^ 0x4d444d42u};
+  philox4x32_10(c, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+  float z[4];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float u0 = (static_cast<float>(c[2 * h] >> 8) + 0.5f) * 5.9604644775390625e-08f;
+    const float u1 = (static_cast<float>(c[2 * h + 1] >> 8) + 0.5f) * 5.9604644775390625e-08f;
+    const float r = sqrtf(-2.0f * logf(u0));
+    float sn, cs;
+    sincospif(2.0f * u1, &sn, &cs);
+    z[2 * h] = r * cs;
+    z[2 * h + 1] = r * sn;
+  }
+  float* dst = out + 4 * q;
+  if (4 * q + 3 < n && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+    *reinterpret_cast<float4*>(dst) = make_float4(z[0], z[1], z[2], z[3]);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (4 * q + j < n) dst[j] = z[j];
+  }
+}
 __global__ void philox_normal_kernel(float* __restrict__ out, int B, long long n, unsigned long long seed,
                                      long long sample_base, uint32_t step_id, const StepState* __restrict__ state) {
   pdl_launch_dependents();
@@ -147,29 +173,75 @@ __global__ void philox_normal_kernel(float* __restrict__ out, int B, long long n
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const long long b = i / qn, q = i - b * qn;
-    const unsigned long long g = static_cast<unsigned long long>(sample_base + b);
-    uint32_t c[4] = {static_cast<uint32_t>(q), step_id, static_cast<uint32_t>(g), static_cast<uint32_t>(g >> 32) ^ 0x4d444d42u};
-    philox4x32_10(c, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
-    float z[4];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const float u0 = (static_cast<float>(c[2 * h] >> 8) + 0.5f) * 5.9604644775390625e-08f;
-      const float u1 = (static_cast<float>(c[2 * h + 1] >> 8) + 0.5f) * 5.9604644775390625e-08f;
-      const float r = sqrtf(-2.0f * logf(u0));
-      float sn, cs;
-      sincospif(2.0f * u1, &sn, &cs);
-      z[2 * h] = r * cs;
-      z[2 * h + 1] = r * sn;
-    }
-    float* dst = out + b * n + 4 * q;
-    if (4 * q + 3 < n && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-      *reinterpret_cast<float4*>(dst) = make_float4(z[0], z[1], z[2], z[3]);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (4 * q + j < n) dst[j] = z[j];
-    }
+    philox_quad(out + b * n, n, q, seed, static_cast<unsigned long long>(sample_base + b), step_id);
   }
+}
+
+// philox_normal_kernel with every sample keyed by its own slot (seed, schedule index cur, global sample index g): the eps
+// of each active slot's step, exactly as a uniform loop with noise_seed = seed draws it for sample g at index cur.
+// Idle slots draw nothing.
+__global__ void philox_slots_kernel(float* __restrict__ out, int B, long long n, const SlotState* slots) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long qn = (n + 3) / 4, total = qn * B;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long b = i / qn, q = i - b * qn;
+    const int cur = __ldcg(&slots[b].cur);
+    if (cur < 0) continue;
+    philox_quad(out + b * n, n, q, __ldcg(&slots[b].seed), static_cast<unsigned long long>(__ldcg(&slots[b].g)),
+                static_cast<uint32_t>(cur));
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Continuous batching (b200mdm_slots_begin): every row of the workspace is a slot with its own schedule index.
+// Every slot idle; tvec at a valid row for the idle forward, all keys valid, scale 0.
+__global__ void slots_reset_kernel(SlotState* slots, int* tvec, int* kvlen, float* scale, int* action, const int* tmap, int B,
+                                   int Bp, int S) {
+  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < Bp; b += gridDim.x * blockDim.x) {
+    kvlen[b] = S;
+    if (b >= B) continue;
+    slots[b].cur = -1;
+    slots[b].seed = 0ull;
+    slots[b].g = 0ll;
+    tvec[b] = tmap[0];
+    scale[b] = 0.f;
+    if (action != nullptr) action[b] = 0;
+  }
+}
+// Slot b's per-request scalars (b200mdm_slot_admit): its state at schedule index cur, the model timestep of its first
+// step, its guidance scale and its valid-key count in each classifier-free half.  One thread.
+__global__ void slot_admit_kernel(SlotState* slots, int* tvec, int* kvlen, float* scale, int* action, const int* tmap, int b,
+                                  int B, int halves, int cur, unsigned long long seed, long long g, float sc, int kv,
+                                  int act) {
+  slots[b].cur = cur;
+  slots[b].seed = seed;
+  slots[b].g = g;
+  tvec[b] = tmap[cur];
+  scale[b] = sc;
+  for (int h = 0; h < halves; ++h) kvlen[h * B + b] = kv;
+  if (action != nullptr) action[b] = act;
+}
+// The last kernel of a slot step: every active slot moves one index down the schedule (after index 0 it is -1: done),
+// and tvec takes the model timestep of its next step (idle slots: row 0, a valid row for the idle forward).
+__global__ void slot_advance_kernel(SlotState* slots, int* tvec, const int* __restrict__ tmap, int B) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  int cur = __ldcg(&slots[b].cur);
+  if (cur >= 0) slots[b].cur = --cur;
+  tvec[b] = tmap[cur > 0 ? cur : 0];
+}
+// b200mdm_sample_step_at: slot b at schedule index tvec[b] (the caller's indices, uploaded there), tvec[b] <- its model
+// timestep.  Noise comes from the caller, so no Philox key is set.
+__global__ void slots_from_index_kernel(SlotState* slots, int* tvec, const int* __restrict__ tmap, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int cur = tvec[b];
+  slots[b].cur = cur;
+  tvec[b] = tmap[cur];
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -503,7 +575,7 @@ __global__ void mem_build_kernel(__half* __restrict__ mem16, const float* __rest
   pdl_launch_dependents();
   pdl_wait();
   const int m = blockIdx.x, bp = blockIdx.y;
-  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(load_step_state(state), back)];
+  int t = (tvec != nullptr) ? __ldcg(tvec + bp % B) : tmap[eval_index(load_step_state(state), back)];
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = static_cast<size_t>(bp) * Mt + m;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
@@ -561,7 +633,7 @@ __global__ void cross_rows_kernel(float* __restrict__ c, const float* __restrict
   pdl_launch_dependents();
   pdl_wait();
   const int bp = blockIdx.x, l = blockIdx.y;
-  int t = (tvec != nullptr) ? tvec[bp % B] : tmap[eval_index(load_step_state(state), back)];
+  int t = (tvec != nullptr) ? __ldcg(tvec + bp % B) : tmap[eval_index(load_step_state(state), back)];
   t = min(max(t, 0), temb_rows - 1);
   const size_t row = (static_cast<size_t>(l) * Bp + bp) * d, trow = (static_cast<size_t>(l) * temb_rows + t) * d;
   for (int i = threadIdx.x; i < d / 4; i += blockDim.x) {

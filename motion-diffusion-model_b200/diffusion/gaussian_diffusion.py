@@ -69,7 +69,8 @@ def _f32(a):
 
 # The feature wrappers (utils/sampler_util.resolve) each sampler family refuses; DDPM and DDIM take all three.
 _REFUSED = {"DDIM inversion": ("handshake", "joint"), "PLMS": ("joint",), "DPM-Solver++": ("joint",),
-            "The variational bound": ("handshake", "joint", "multi"), "p_mean_variance": ("joint",)}
+            "The variational bound": ("handshake", "joint", "multi"), "p_mean_variance": ("joint",),
+            "Continuous batching": ("handshake", "joint", "multi")}
 _REFUSAL = {"handshake": "%s with HandshakeSampleModel is not implemented",
             "joint": "%s with joint-position control (JointControlSampleModel) is not implemented",
             "multi": "%s with multi-prompt guidance (MultiPromptSampleModel) is not implemented"}
@@ -452,16 +453,31 @@ class GaussianDiffusion:
 
     def p_sample(self, model, x, t, clip_denoised=True, denoised_fn=None, cond_fn=None, model_kwargs=None,
                  const_noise=False, noise=None):
-        """reference gaussian_diffusion.py:489-541 (t: LongTensor [B] of identical schedule indices)."""
+        """reference gaussian_diffusion.py:489-541 (t: LongTensor [B] of schedule indices, one per sample)."""
         return self._single(_lib.MODE_DDPM, model, x, t, clip_denoised, denoised_fn, cond_fn, model_kwargs, const_noise, 0.0, noise)
 
     def _single(self, mode, model, x, t, clip_denoised, denoised_fn, cond_fn, model_kwargs, const_noise, eta, noise):
+        """One step at t: one schedule index for the batch (b200mdm_sample_step), or, when the values of t differ, each
+        sample at its own (b200mdm_sample_step_at), as the reference's per-sample _extract_into_tensor reads them."""
         self._reject_hooks(denoised_fn, cond_fn, False, False)
-        idx = int(t.reshape(-1)[0].item())
-        assert bool((t == idx).all()), "the fused step takes one schedule index for the whole batch (gaussian_diffusion.py:709)"
+        idx = [int(v) for v in t.reshape(-1).tolist()]
+        mixed = any(v != idx[0] for v in idx)
+        if mixed:                                    # the refusals of b200mdm_sample_step_at, before any engine work
+            self._refuse(model, "Continuous batching")
+            y = (model_kwargs or {}).get("y", {})
+            mdm = resolve(model).mdm
+            target = "target_cond" in y and not bool(y.get("target_uncond", False))
+            if (const_noise or "inpainting_mask" in y or "inpainting_weight" in y or target
+                    or (mdm is not None and mdm.is_dip)):
+                raise NotImplementedError("p_sample / ddim_sample with a schedule index per sample take no const_noise, "
+                                          "inpainting, target or BERT text memory")
         eng = self._prepare(model, x.shape, model_kwargs, x.device, eta)
         eps = noise if noise is not None else torch.randn_like(x)
-        out, pred = eng.sample_step(mode, idx, x, eps, self._flags(clip_denoised, const_noise), want_pred=True)
+        flags = self._flags(clip_denoised, const_noise)
+        if mixed:
+            out, pred = eng.sample_step_at(mode, idx, x, eps, flags, want_pred=True)
+        else:
+            out, pred = eng.sample_step(mode, idx[0], x, eps, flags, want_pred=True)
         return {"sample": out, "pred_xstart": pred}
 
     # ------------------------------------------------------------------ DDIM

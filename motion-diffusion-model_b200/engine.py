@@ -589,6 +589,40 @@ class Engine:
                                            _stream()))
         return out, pred
 
+    def sample_step_at(self, mode, indices, x_t, noise, flags=0, want_pred=True):
+        """One DDPM / DDIM step where sample b takes schedule index indices[b] (b200mdm_sample_step_at)."""
+        idx = np.ascontiguousarray(np.asarray(indices).reshape(-1), dtype=np.int32)
+        x_t = x_t.to(torch.float32).contiguous()
+        noise = noise.to(torch.float32).contiguous()
+        out = torch.empty_like(x_t)
+        pred = torch.empty_like(x_t) if want_pred else None
+        check(self.lib.b200mdm_sample_step_at(self.h, mode, idx.ctypes.data_as(ctypes.c_void_p), _ptr(x_t), _ptr(noise),
+                                              flags, _ptr(out), _ptr(pred), _stream()))
+        return out, pred
+
+    # ------------------------------------------------------------------ continuous batching (serving.ContinuousSampler)
+    def slots_begin(self, slots, nframes, guided, mode, flags=0):
+        """A slot session on the (slots, nframes) workspace (b200mdm_slots_begin): every slot idle."""
+        check(self.lib.b200mdm_slots_begin(self.h, int(slots), int(nframes), int(bool(guided)), mode, flags, _stream()))
+        self.batch, self.nframes, self.halves, self.n_tokens = int(slots), int(nframes), 2 if guided else 1, 1
+        self._keep["slots"] = {}
+
+    def slot_admit(self, slot, embed, action, scale, length, seed, sample_index):
+        """One request into an idle slot (b200mdm_slot_admit): embed [cond_dim] fp32 on the device or None."""
+        embed = embed.to(torch.float32).contiguous() if embed is not None else None
+        check(self.lib.b200mdm_slot_admit(self.h, int(slot), _ptr(embed), int(action), float(scale), int(length),
+                                          ctypes.c_uint64(int(seed) & (2 ** 64 - 1)), int(sample_index), _stream()))
+        self._keep["slots"][int(slot)] = embed      # read by the admission's kernels, which run asynchronously
+
+    def slots_run(self, n_steps, use_graph=True):
+        check(self.lib.b200mdm_slots_run(self.h, int(n_steps), int(use_graph), _stream()))
+
+    def slot_read(self, slot, out):
+        """out [njoints, nfeats, nframes] fp32 <- the finished sample of `slot`, which becomes free (b200mdm_slot_read)."""
+        assert out.is_contiguous() and out.dtype == torch.float32
+        check(self.lib.b200mdm_slot_read(self.h, int(slot), _ptr(out), _stream()))
+        return out
+
     def sample_loop(self, mode, x, tape, skip_timesteps=0, flags=0, use_graph=True):
         """x: [B,J,F,T] fp32 (x_T, left untouched); tape: [n_run, B,J,F,T] fp32.  Returns x_0 (new tensor)."""
         x = x.to(torch.float32).contiguous()
