@@ -391,7 +391,8 @@ int b200mdm_sample_step_at(b200mdm_engine* e, int32_t mode, const int32_t* index
  * schedule index of the current schedule (mode B200MDM_MODE_DDPM, or B200MDM_MODE_DDIM with the rows uploaded for the
  * caller's eta).  Every slot starts idle and x is zeroed.  flags: B200MDM_FLAG_CLIP_DENOISED (B200MDM_FLAG_PHILOX_NOISE
  * is implied: every eps comes from the request's own Philox stream).  ENOTIMPL for other modes, for
- * B200MDM_FLAG_CONST_NOISE and for BERT-memory decoders.  The session ends at the next b200mdm_set_cond* call (or
+ * B200MDM_FLAG_CONST_NOISE and for BERT-memory decoders (b200mdm_chain_slots_begin).  The session ends at the next
+ * b200mdm_set_cond* call (or
  * b200mdm_sample_step_at); the per-loop features (target, inpainting, handshakes, guidance) are cleared here, and
  * b200mdm_slots_run refuses any set later. */
 int b200mdm_slots_begin(b200mdm_engine* e, int32_t slots, int32_t nframes, int32_t guided, int32_t mode, int32_t flags,
@@ -413,6 +414,41 @@ int b200mdm_slots_run(b200mdm_engine* e, int32_t n_steps, int32_t use_graph, voi
 /* Copy a finished slot's sample [njoints * nfeats, nframes] to out_dev and free the slot.  ESTATE unless the slot has
  * run all its steps. */
 int b200mdm_slot_read(b200mdm_engine* e, int32_t slot, float* out_dev, void* stream);
+
+/* ---- continuous batching with a token memory (DESIGN.md, "Continuous batching", "Token memories and chains")
+ * A slot session of a BERT-memory decoder: DiP (context_len > 0), where every slot runs its own autoregressive chain of
+ * nframes-frame (pred_len) chunks, or the plain BERT decoder (context_len 0), where a request is one chunk.  As
+ * b200mdm_slots_begin, plus a memory width of n_tokens (1 .. 512) tokens for every slot, sized here once: no admission
+ * or hand-off synchronises or drops the step graph.  Widths above 64 take the key-blocked cross-attention, as a uniform
+ * loop does.  Every slot's memory starts as the unconditional rows (W 0 + b) with no padding.  EINVAL for other engines
+ * (they take b200mdm_slots_begin), ENOTIMPL as b200mdm_slots_begin.  Ends as b200mdm_slots_begin's session ends. */
+int b200mdm_chain_slots_begin(b200mdm_engine* e, int32_t slots, int32_t nframes, int32_t guided, int32_t mode,
+                              int32_t flags, int32_t n_tokens, void* stream);
+
+/* Admit one request into an idle slot of a token-memory session (ESTATE while the slot holds a request):
+ *   tokens_dev [n_tokens, cond_dim] and mask_dev [n_tokens] (uint8, 1 = padding), both on the device: its chunk-0 prompt,
+ *   padded to the session's width with mask 1;  prefix_dev [njoints * nfeats, context_len] on the device (DiP; NULL for
+ *   the plain BERT decoder);  its guidance scale;  length: frames of its motion (DiP: ceil(length / nframes) chunks,
+ *   every chunk attending all its context_len + nframes frames; the BERT decoder: 1 .. nframes, its valid keys under
+ *   mask_frames as b200mdm_set_cond_dec counts them);  include_prefix: the motion starts with the prefix (DiP), so chunk
+ *   c lands at frame context_len + c * nframes of it;  its Philox (seed, sample_index).
+ * It projects the slot's conditional memory rows (W tokens + b), writes its mask into its row of every classifier-free
+ * half, packs its prefix into the first context_len rows of its sequence, draws its x_T (step id -1) and arms it at
+ * schedule index n_steps - 1: 5 kernel launches (4 without a prefix), no synchronisation.  A request admitted into slot
+ * b with (seed s, sample_index g) gives bitwise row b of the uniform chain (AutoRegressiveSampler with p_sample_loop /
+ * ddim_sample_loop, noise_seed = s, sample_index_base = g - b) at the same slots, nframes and width. */
+int b200mdm_chain_slot_admit(b200mdm_engine* e, int32_t slot, const float* tokens_dev, const uint8_t* mask_dev,
+                             const float* prefix_dev, float scale, int64_t length, int32_t include_prefix, uint64_t seed,
+                             int64_t sample_index, void* stream);
+
+/* The hand-off of a slot that has just finished a chunk (ESTATE otherwise): its sample goes to frames
+ * off + c * nframes .. of out_dev [njoints * nfeats, length] (off = context_len under include_prefix, else 0; frames at
+ * or past length are dropped).  If chunks remain, its last context_len frames become its prefix (packed as at
+ * admission), tokens_dev / mask_dev (both or neither; NULL: keep the prompt) replace its memory and mask with chunk
+ * c + 1's prompt, and it is armed again with a fresh x_T of the same (seed, sample_index): 4 kernel launches, 6 with a
+ * new prompt.  After its last chunk the slot is free: 1 launch.  No synchronisation. */
+int b200mdm_chain_slot_handoff(b200mdm_engine* e, int32_t slot, float* out_dev, const float* tokens_dev,
+                               const uint8_t* mask_dev, void* stream);
 
 /* ddim_reverse_sample (gaussian_diffusion.py:838-874) repeated without returning to the host: schedule indices
  * first_index, first_index+1, ... (n_run of them, up to n_steps - 1) on the engine's working buffer, one CUDA graph of a

@@ -16,7 +16,7 @@ from .utils.sampler_util import (ClassifierFreeSampleModel, AutoRegressiveSample
 from .utils.scene import SceneGrid, shape_sdf  # noqa: F401
 from .diffusion.respace import SpacedDiffusion, space_timesteps  # noqa: F401
 from .diffusion.gaussian_diffusion import GaussianDiffusion, get_named_beta_schedule  # noqa: F401
-from .serving import ContinuousSampler  # noqa: F401
+from .serving import ContinuousSampler, ContinuousChainSampler  # noqa: F401
 from .model.mdm import MDM  # noqa: F401
 from .synthetic import (synthetic_state_dict, synthetic_inputs, synthetic_dip_inputs, synthetic_norm_stats,  # noqa: F401
                         synthetic_target_inputs)

@@ -42,6 +42,7 @@ SYMBOLS = [
     "b200mdm_set_scene_guidance", "b200mdm_test_scene_guidance", "b200mdm_chain_set_goal", "b200mdm_chunk_frame",
     "b200mdm_set_interaction_guidance", "b200mdm_test_interaction_guidance",
     "b200mdm_sample_step_at", "b200mdm_slots_begin", "b200mdm_slot_admit", "b200mdm_slots_run", "b200mdm_slot_read",
+    "b200mdm_chain_slots_begin", "b200mdm_chain_slot_admit", "b200mdm_chain_slot_handoff",
 ]
 MAX_PROMPTS = 8                             # B200MDM_MAX_PROMPTS
 MAX_CHARACTERS = 8                          # characters per scene: one cluster of at most 8 CTAs
@@ -166,7 +167,10 @@ def load():
                        ("b200mdm_set_cond_multi_tokens", [vp, i32, i32, i32, vp, vp, i32, vp, vp]),
                        ("b200mdm_set_prompt_weight", [vp, i32, vp, i64, i64, i64, i64, vp]),
                        ("b200mdm_chain_set_goal", [vp, vp, vp, vp, i32, vp, vp]),
-                       ("b200mdm_chunk_frame", [vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp])):
+                       ("b200mdm_chunk_frame", [vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp]),
+                       ("b200mdm_chain_slots_begin", [vp, i32, i32, i32, i32, i32, i32, vp]),
+                       ("b200mdm_chain_slot_admit", [vp, i32, vp, vp, vp, f32, i64, i32, ctypes.c_uint64, i64, vp]),
+                       ("b200mdm_chain_slot_handoff", [vp, i32, vp, vp, vp, vp])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

@@ -334,6 +334,15 @@ struct b200mdm_engine : Workspace {
   std::vector<unsigned char> slot_busy;
   std::vector<int> slot_left;
   std::vector<int> h_slot_idx;   // host staging of b200mdm_sample_step_at's indices
+  // a token-memory session (b200mdm_chain_slots_begin; slot_mode on a BERT-memory engine): per slot, what its hand-offs
+  // need -- its Philox key, scale and valid keys to re-arm it, its motion length, first output frame and chunk position
+  struct ChainSlot {
+    unsigned long long seed = 0;
+    long long g = 0;
+    float scale = 0.f;
+    int kv = 0, length = 0, off = 0, chunk = 0, n_chunks = 0;
+  };
+  std::vector<ChainSlot> chain_slot;
   // a goal-directed chain (b200mdm_chain_set_goal): the caller's mean / std [JF] and goals [n_goals, B, n_ext, 3], the
   // per-sample carry [B, CF_CARRY] and the next chunk's target [B, n_ext, 3]; live while goal_set and the chain is
   // (chain_setup clears goal_set, and everything that ends a chain sets chain_next = -1)
@@ -1430,7 +1439,7 @@ static int build_text_memory(b200mdm_engine* e, const float* tokens, int K, bool
 // diffusion/gaussian_diffusion.py, with the same sampler rows; the setter rows make handshakes, joint-position control
 // and multi-prompt guidance pairwise exclusive and keep each off prefix-completion (DiP) engines.
 enum Feature : unsigned { F_PREFIX = 1, F_HANDSHAKE = 2, F_JOINT = 4, F_MULTI = 8, F_TOKENS = 16, F_TARGET = 32, F_INPAINT = 64 };
-enum Family { FAM_REVERSE, FAM_PLMS, FAM_DPM, FAM_VB, FAM_HANDSHAKE, FAM_JOINT, FAM_MULTI, FAM_SLOTS };
+enum Family { FAM_REVERSE, FAM_PLMS, FAM_DPM, FAM_VB, FAM_HANDSHAKE, FAM_JOINT, FAM_MULTI, FAM_SLOTS, FAM_STEP_AT };
 static const struct {
   const char* name;
   unsigned refuses;
@@ -1442,7 +1451,10 @@ static const struct {
     {"handshaking", F_PREFIX | F_JOINT | F_MULTI},
     {"joint-position control", F_PREFIX | F_HANDSHAKE | F_MULTI},
     {"multi-prompt guidance", F_PREFIX},
-    // a schedule index per row: every per-loop input but the conditioning rows, scale and lengths is one for the batch
+    // a schedule index per row: every per-loop input but the conditioning rows or token memory, prefix, scale and
+    // lengths is one for the batch (a token memory and a prefix are per slot in a b200mdm_chain_slots_begin session)
+    {"continuous batching", F_HANDSHAKE | F_JOINT | F_MULTI | F_TARGET | F_INPAINT},
+    // b200mdm_sample_step_at: the rows of the one conditioning upload, so no token memory or prefix
     {"continuous batching", F_PREFIX | F_HANDSHAKE | F_JOINT | F_MULTI | F_TOKENS | F_TARGET | F_INPAINT},
 };
 
@@ -2510,7 +2522,7 @@ extern "C" int b200mdm_sample_step_at(b200mdm_engine* e, int32_t mode, const int
   TRY(check_flags("b200mdm_sample_step_at", flags, B200MDM_FLAG_CLIP_DENOISED));
   for (int b = 0; b < e->B; ++b)
     if (index_host[b] < 0 || index_host[b] >= e->n_steps) return fail(B200MDM_EINVAL, "schedule index out of range");
-  TRY(refuse(e, FAM_SLOTS));
+  TRY(refuse(e, FAM_STEP_AT));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   TRY(ensure_slots(e));
   e->slot_mode = false;   // the step overwrites the slot state
@@ -2576,6 +2588,7 @@ static int check_slot(const b200mdm_engine* e, int32_t slot) {
 extern "C" int b200mdm_slot_admit(b200mdm_engine* e, int32_t slot, const float* cond_embed_dev, int64_t action,
                                   float scale, int64_t length, uint64_t seed, int64_t sample_index, void* stream) {
   TRY(check_slot(e, slot));
+  if (e->dec && !e->dec_clip) return fail(B200MDM_EINVAL, "a token-memory session admits through b200mdm_chain_slot_admit");
   if (e->slot_busy[slot]) return fail(B200MDM_ESTATE, "slot %d holds a request that has not been read", slot);
   const int mode = e->cfg.cond_mode;
   if ((mode == B200MDM_COND_TEXT || e->dec_clip) && !cond_embed_dev)
@@ -2620,6 +2633,7 @@ extern "C" int b200mdm_slots_run(b200mdm_engine* e, int32_t n_steps, int32_t use
 
 extern "C" int b200mdm_slot_read(b200mdm_engine* e, int32_t slot, float* out_dev, void* stream) {
   TRY(check_slot(e, slot));
+  if (e->dec && !e->dec_clip) return fail(B200MDM_EINVAL, "a token-memory session reads through b200mdm_chain_slot_handoff");
   if (!out_dev) return fail(B200MDM_EINVAL, "null tensor");
   if (!e->slot_busy[slot] || e->slot_left[slot] > 0)
     return fail(B200MDM_ESTATE, "slot %d has no finished request (%d steps to run)", slot, e->slot_left[slot]);
@@ -2961,6 +2975,159 @@ extern "C" int b200mdm_chain_loop_range(b200mdm_engine* e, int32_t mode, int32_t
   const int next = first_step + n_run;
   e->chain_next = next < e->chain_n * N ? next : -1;
   return loop_leave(e, use_graph, user);
+}
+
+// ------------------------------------------------------------------------------------------------ token-memory slots
+// DESIGN.md, "Continuous batching", "Token memories and chains": DiP's chains and the plain BERT decoder in slots.  The
+// step graph is the slot graph of b200mdm_slots_begin; what is per slot here -- the memory rows (memproj, memmask), the
+// prefix rows of the embedding GEMM's A operand and the chunk position -- is written between replays, on the stream, by
+// the host, which knows every chunk boundary without asking the device.
+extern "C" int b200mdm_chain_slots_begin(b200mdm_engine* e, int32_t slots, int32_t nframes, int32_t guided, int32_t mode,
+                                         int32_t flags, int32_t n_tokens, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (!e->finalized) return fail(B200MDM_ESTATE, "weights not finalised");
+  if (e->n_steps <= 0) return fail(B200MDM_ESTATE, "b200mdm_set_schedule has not been called");
+  if (!e->dec || e->dec_clip)
+    return fail(B200MDM_EINVAL, "b200mdm_chain_slots_begin is for BERT-memory decoders (the others: b200mdm_slots_begin)");
+  if (slots <= 0 || nframes <= 0) return fail(B200MDM_EINVAL, "bad slots / nframes");
+  if (n_tokens <= 0 || n_tokens > XAL_MAX_MT)
+    return fail(B200MDM_EINVAL, "n_tokens %d: a text memory holds 1..%d tokens (DistilBERT's position limit)", n_tokens,
+                XAL_MAX_MT);
+  if (mode != B200MDM_MODE_DDPM && mode != B200MDM_MODE_DDIM)
+    return fail(B200MDM_ENOTIMPL, "continuous batching runs DDPM and DDIM (PLMS, DPM-Solver++, DDIM inversion and the "
+                "bound carry history or tables that are not per slot)");
+  if (flags & B200MDM_FLAG_CONST_NOISE) return fail(B200MDM_ENOTIMPL, "B200MDM_FLAG_CONST_NOISE with continuous batching");
+  TRY(check_flags("continuous batching", flags, B200MDM_FLAG_CLIP_DENOISED | B200MDM_FLAG_PHILOX_NOISE));
+  TRY(check_seq_len(e, nframes + e->ctx));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  TRY(select_workspace(e, slots, nframes, guided ? 2 : 1, s));
+  TRY(ensure_slots(e));
+  TRY(ensure_text_memory(e, n_tokens));   // the one place the memory is sized: admissions never resize it
+  if (e->ctx > 0) {
+    const size_t np = static_cast<size_t>(e->B) * e->JF * e->ctx;
+    if (e->chain_prefix_cap < np) CUDA_TRY(cudaDeviceSynchronize());   // a chain may still read the buffer being replaced
+    TRY(ensure_cap(&e->chain_prefix, &e->chain_prefix_cap, np));
+  }
+  slots_reset_kernel<<<(e->Bp + 127) / 128, 128, 0, s>>>(e->slots, e->tvec, e->kvlen, e->scale, nullptr, e->tmap, e->B,
+                                                         e->Bp, e->S);
+  CUDA_TRY(cudaGetLastError());
+  // every memory row the unconditional one (W 0 + b) without padding: what an idle slot attends, and for good the rows
+  // of the unconditional half, which an admission leaves as they are
+  memproj_group_fill_kernel<<<dim3(e->Mt, e->Bp), 128, 0, s>>>(e->memproj, e->memtok, e->b_txt, 0, e->Mt, e->d);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemsetAsync(e->memmask, 0, static_cast<size_t>(e->Bp) * e->Mt, s));
+  CUDA_TRY(cudaMemsetAsync(e->x_work, 0, static_cast<size_t>(e->B) * e->JF * e->T * sizeof(float), s));
+  e->launches += 2;
+  end_cond(e);
+  e->mem_uncond = false;
+  e->prefix_set = e->ctx > 0;   // each slot packs its own prefix rows
+  e->prefix_src = nullptr;
+  e->slot_mode = true;
+  e->slot_sampler = mode;
+  e->slot_flags = (flags & B200MDM_FLAG_CLIP_DENOISED) | B200MDM_FLAG_PHILOX_NOISE;
+  e->slot_busy.assign(e->B, 0);
+  e->slot_left.assign(e->B, 0);
+  e->chain_slot.assign(e->B, b200mdm_engine::ChainSlot{});
+  return B200MDM_OK;
+}
+
+static int check_token_slot(const b200mdm_engine* e, int32_t slot) {
+  TRY(check_slot(e, slot));
+  if (!e->dec || e->dec_clip) return fail(B200MDM_EINVAL, "not a token-memory session (b200mdm_chain_slots_begin)");
+  return B200MDM_OK;
+}
+// Slot b's conditional memory rows W tokens + b (tokens [Mt, C]: memproj rows b * Mt .., as build_text_memory projects
+// sample b's) and its mask rows in every half: 2 launches.
+static int slot_memory(b200mdm_engine* e, int slot, const float* tokens, const uint8_t* mask, cudaStream_t s) {
+  const int d = e->d, Mt = e->Mt, C = e->cfg.cond_dim;
+  const size_t warps = static_cast<size_t>(Mt) * d;
+  small_linear_kernel<0><<<static_cast<int>((warps * 32 + 255) / 256), 256, 0, s>>>(
+      tokens, e->w_txt, e->b_txt, e->memproj + static_cast<size_t>(slot) * Mt * d, Mt, d, C, C);
+  CUDA_TRY(cudaGetLastError());
+  slot_mask_kernel<<<1, 128, 0, s>>>(e->memmask, mask, slot, e->B, e->halves, Mt);
+  CUDA_TRY(cudaGetLastError());
+  e->launches += 2;
+  return B200MDM_OK;
+}
+// prefix [JF, ctx] into the first ctx rows of slot b's sequence of the embedding GEMM's A operand: 1 launch
+static int slot_prefix(b200mdm_engine* e, int slot, const float* prefix, cudaStream_t s) {
+  TRY(launch_pack_input(prefix, e->xin16 + static_cast<size_t>(slot) * e->S * 3 * e->Kp_in, 1, e->JF, e->ctx, e->S, e->Kp_in, 0,
+                        s));
+  e->launches += 1;
+  return B200MDM_OK;
+}
+// Slot b at schedule index n_steps - 1 with its key, scale and key counts, and its x_T (step id -1 of its Philox
+// stream, as p_sample_loop(noise_seed=seed) draws it for that sample): 2 launches.
+static int slot_arm(b200mdm_engine* e, int slot, const b200mdm_engine::ChainSlot& r, cudaStream_t s) {
+  const size_t n = static_cast<size_t>(e->JF) * e->T;
+  slot_admit_kernel<<<1, 1, 0, s>>>(e->slots, e->tvec, e->kvlen, e->scale, nullptr, e->tmap, slot, e->B, e->halves,
+                                     e->n_steps - 1, r.seed, r.g, r.scale, r.kv, 0);
+  CUDA_TRY(cudaGetLastError());
+  TRY(launch_philox(e->x_work + slot * n, 1, static_cast<long long>(n), r.seed, r.g, 0xffffffffu, nullptr, s));
+  e->launches += 2;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_chain_slot_admit(b200mdm_engine* e, int32_t slot, const float* tokens_dev, const uint8_t* mask_dev,
+                                        const float* prefix_dev, float scale, int64_t length, int32_t include_prefix,
+                                        uint64_t seed, int64_t sample_index, void* stream) {
+  TRY(check_token_slot(e, slot));
+  if (e->slot_busy[slot]) return fail(B200MDM_ESTATE, "slot %d holds a request", slot);
+  if (!tokens_dev || !mask_dev) return fail(B200MDM_EINVAL, "the request's tokens and mask are required");
+  if ((prefix_dev != nullptr) != (e->ctx > 0))
+    return fail(B200MDM_EINVAL, "a prefix [njoints * nfeats, %d] for DiP, none for the plain BERT decoder", e->ctx);
+  if (length < 1 || length > (1 << 24) || (e->ctx == 0 && length > e->T))
+    return fail(B200MDM_EINVAL, "length %lld: 1 .. %d frames", static_cast<long long>(length), e->ctx == 0 ? e->T : 1 << 24);
+  if (!std::isfinite(scale)) return fail(B200MDM_EINVAL, "scale must be finite");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  b200mdm_engine::ChainSlot r;
+  r.seed = static_cast<unsigned long long>(seed);
+  r.g = static_cast<long long>(sample_index);
+  r.scale = scale;
+  r.length = static_cast<int>(length);
+  // valid keys: a DiP chunk attends all its ctx + pred_len frames (the length only crops the motion); the plain BERT
+  // decoder has no token ahead of the frames, so `length` frames under mask_frames, as upload_kvlen_scale counts them
+  r.kv = e->S;
+  if (e->ctx == 0 && e->cfg.mask_frames && e->S > 1) r.kv = r.length;
+  r.off = include_prefix && e->ctx > 0 ? e->ctx : 0;
+  r.n_chunks = e->ctx > 0 ? (r.length + e->T - 1) / e->T : 1;
+  TRY(slot_memory(e, slot, tokens_dev, mask_dev, s));
+  if (e->ctx > 0) TRY(slot_prefix(e, slot, prefix_dev, s));
+  TRY(slot_arm(e, slot, r, s));
+  e->chain_slot[slot] = r;
+  e->slot_busy[slot] = 1;
+  e->slot_left[slot] = e->n_steps;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_chain_slot_handoff(b200mdm_engine* e, int32_t slot, float* out_dev, const float* tokens_dev,
+                                          const uint8_t* mask_dev, void* stream) {
+  TRY(check_token_slot(e, slot));
+  if (!out_dev) return fail(B200MDM_EINVAL, "null output");
+  if ((tokens_dev == nullptr) != (mask_dev == nullptr)) return fail(B200MDM_EINVAL, "a new prompt needs its tokens and mask");
+  if (!e->slot_busy[slot] || e->slot_left[slot] > 0)
+    return fail(B200MDM_ESTATE, "slot %d has not just finished a chunk (%d steps to run)", slot,
+                e->slot_busy[slot] ? e->slot_left[slot] : 0);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  b200mdm_engine::ChainSlot& r = e->chain_slot[slot];
+  const bool last = r.chunk + 1 >= r.n_chunks;
+  const int JF = e->JF, T = e->T;
+  float* prefix = last ? nullptr : e->chain_prefix + static_cast<size_t>(slot) * JF * e->ctx;
+  const long long rows = JF;
+  chain_handoff_kernel<<<static_cast<int>((rows * T + 255) / 256 < 1184 ? (rows * T + 255) / 256 : 1184), 256, 0, s>>>(
+      e->x_work + static_cast<size_t>(slot) * JF * T, out_dev, prefix, rows, T, e->ctx, r.off + r.chunk * T, r.length);
+  CUDA_TRY(cudaGetLastError());
+  e->launches += 1;
+  if (last) {
+    e->slot_busy[slot] = 0;
+    return B200MDM_OK;
+  }
+  TRY(slot_prefix(e, slot, prefix, s));
+  if (tokens_dev) TRY(slot_memory(e, slot, tokens_dev, mask_dev, s));
+  TRY(slot_arm(e, slot, r, s));
+  r.chunk += 1;
+  e->slot_left[slot] = e->n_steps;
+  return B200MDM_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ variational bound

@@ -243,6 +243,15 @@ __global__ void slots_from_index_kernel(SlotState* slots, int* tvec, const int* 
   slots[b].cur = cur;
   tvec[b] = tmap[cur];
 }
+// A token-memory slot session (b200mdm_chain_slot_admit / _handoff): slot b's padding mask [Mt] (1 = padding) into its
+// row of every classifier-free half -- the rows pack_text_mask gives sample b with one prompt.  One block.
+__global__ void slot_mask_kernel(unsigned char* __restrict__ memmask, const uint8_t* __restrict__ mask, int b, int B,
+                                 int halves, int Mt) {
+  for (int m = threadIdx.x; m < Mt; m += blockDim.x) {
+    const unsigned char pad = mask[m] ? 1 : 0;
+    for (int h = 0; h < halves; ++h) memmask[(static_cast<size_t>(h) * B + b) * Mt + m] = pad;
+  }
+}
 
 // ---------------------------------------------------------------------------------------------------------
 // CFG blend on the hidden rows + fp16 hi/lo split for the 3-pass output GEMM.

@@ -623,6 +623,30 @@ class Engine:
         check(self.lib.b200mdm_slot_read(self.h, int(slot), _ptr(out), _stream()))
         return out
 
+    # ------------------------------------------------------------------ token-memory slots (serving.ContinuousChainSampler)
+    def chain_slots_begin(self, slots, nframes, guided, mode, n_tokens, flags=0):
+        """A slot session of a BERT-memory decoder with memories of n_tokens tokens (b200mdm_chain_slots_begin)."""
+        check(self.lib.b200mdm_chain_slots_begin(self.h, int(slots), int(nframes), int(bool(guided)), mode, flags,
+                                                 int(n_tokens), _stream()))
+        self.batch, self.nframes, self.halves, self.n_tokens = int(slots), int(nframes), 2 if guided else 1, int(n_tokens)
+        self._keep["slots"] = {}
+
+    def chain_slot_admit(self, slot, tokens, mask, prefix, scale, length, include_prefix, seed, sample_index):
+        """One request into an idle slot (b200mdm_chain_slot_admit): tokens [n_tokens, cond_dim] fp32 and mask
+        [n_tokens] uint8 (1 = padding) on the device, prefix [njoints * nfeats, context_len] fp32 on the device or None."""
+        check(self.lib.b200mdm_chain_slot_admit(self.h, int(slot), _ptr(tokens), _ptr(mask), _ptr(prefix), float(scale),
+                                                int(length), int(bool(include_prefix)),
+                                                ctypes.c_uint64(int(seed) & (2 ** 64 - 1)), int(sample_index), _stream()))
+        self._keep["slots"][int(slot)] = (tokens, mask, prefix)   # read by kernels that run asynchronously
+
+    def chain_slot_handoff(self, slot, out, tokens=None, mask=None):
+        """The hand-off of a slot that has just finished a chunk (b200mdm_chain_slot_handoff): the chunk into out
+        [njoints * nfeats, length], then the next chunk armed, with a new prompt when tokens / mask are given."""
+        assert out.is_contiguous() and out.dtype == torch.float32
+        check(self.lib.b200mdm_chain_slot_handoff(self.h, int(slot), _ptr(out), _ptr(tokens), _ptr(mask), _stream()))
+        if tokens is not None:
+            self._keep["slots"][int(slot)] = (tokens, mask)
+
     def sample_loop(self, mode, x, tape, skip_timesteps=0, flags=0, use_graph=True):
         """x: [B,J,F,T] fp32 (x_T, left untouched); tape: [n_run, B,J,F,T] fp32.  Returns x_0 (new tensor)."""
         x = x.to(torch.float32).contiguous()
