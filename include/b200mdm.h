@@ -672,10 +672,10 @@ int b200mdm_test_out_weight(const void* hres16_dev, const float* scale_dev, cons
 int b200mdm_test_blend_handshake(const void* hres16_dev, const float* scale_dev, void* g16_dev, int32_t B, int32_t T,
                                  int32_t d, int32_t s_off, int32_t halves, int32_t h, const int64_t* lengths_host,
                                  const uint8_t* motion_start_host, void* stream);
-/* The guidance iterations of b200mdm_set_joint_guidance alone (joint_guidance_test_kernel, the device function the
- * step kernel runs): x0_out fp32 [B, D, T] = x0 [B, D, T] after `iters` gradient steps; loss_out (nullable) fp32
- * [iters + 1, B] receives G before each step and after the last.  1 <= T <= 256; other arguments as there; invalid
- * arguments return B200MDM_EINVAL before any CUDA call. */
+/* The guidance iterations of b200mdm_set_joint_guidance alone (joint_guidance_test_kernel<false, false>, which runs the
+ * step kernel's device function): x0_out fp32 [B, D, T] = x0 [B, D, T] after `iters` gradient steps; loss_out
+ * (nullable) fp32 [iters + 1, B] receives G before each step and after the last.  1 <= T <= 256; other arguments as
+ * there; invalid arguments return B200MDM_EINVAL before any CUDA call. */
 int b200mdm_test_joint_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
                                 const float* weight_dev, int32_t B, int32_t T, int32_t D, float step, int32_t iters,
                                 float* x0_out_dev, float* loss_out_dev, void* stream);

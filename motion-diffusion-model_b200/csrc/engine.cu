@@ -148,18 +148,14 @@ struct GraphKey {
   const void *pred = nullptr, *imask = nullptr, *iweight = nullptr, *imotion = nullptr;
   const void* target_g = nullptr;   // the workspace's target embedding, or nullptr when the loop has no target
   const void* hs = nullptr;         // the workspace's handshake descriptor, or nullptr when the loop has none
-  bool guided = false;              // joint-position control: the step ends in joint_guidance_step_kernel
-  int groups = 0;                   // multi-prompt guidance: the step ends in compose_step_kernel over G groups
-  bool foot = false;                // ... with the foot-contact and floor terms: joint_guidance_step_kernel<true, false>
-  bool scene = false;               // ... and the scene terms: joint_guidance_step_kernel<true, true>
-  bool inter = false;               // ... and the interaction terms: joint_guidance_step_kernel<true, true, true>
+  int guide = -1;                   // joint-position control: the step ends in GUIDE_VARIANTS[guide] (-1: unguided)
   int chars = 0;                    //     in clusters of `chars` CTAs
+  int groups = 0;                   // multi-prompt guidance: the step ends in compose_step_kernel over G groups
   bool slots = false;               // continuous batching: a schedule index per row (b200mdm_slots_begin)
   bool operator==(const GraphKey& o) const {
     return mode == o.mode && B == o.B && T == o.T && flags == o.flags && order == o.order && pred == o.pred &&
            imask == o.imask && iweight == o.iweight && imotion == o.imotion && target_g == o.target_g && hs == o.hs &&
-           guided == o.guided && groups == o.groups && foot == o.foot && scene == o.scene && inter == o.inter &&
-           chars == o.chars && slots == o.slots;
+           guide == o.guide && chars == o.chars && groups == o.groups && slots == o.slots;
   }
 };
 
@@ -274,32 +270,22 @@ struct b200mdm_engine : Workspace {
   const unsigned char* inpaint_mask = nullptr;
   const float* inpaint_weight = nullptr;   // soft inpainting (b200mdm_set_inpaint_weight); never set with the mask
   const float* inpaint_motion = nullptr;
-  // joint-position control: its device descriptor (read by the step graph at every replay, allocated on first use) and
-  // the host staging of the last upload; jg_set is cleared by every b200mdm_set_cond* call
+  // joint-position control and the terms that extend it (b200mdm_set_{joint,foot,scene,interaction}_guidance): the
+  // device descriptor (read by the step graph at every replay, allocated on first use), its host staging h_guide, which
+  // every setter uploads whole, and the terms on (GuideTerm bits), which every b200mdm_set_cond* call clears and each
+  // setter clears from its own term up.  h_guide.f keeps the lengths of a foot call with both weights 0 and h_guide.s
+  // the grids of a scene call that turned its terms off: the terms above them read both.  The lengths and the reach rows
+  // the descriptor points to live in fg_len [fg_len_cap] int32 and ig_pairs [ig_pairs_cap] (device, allocated on first
+  // use), staged from h_fg_len and h_ig_pairs.
   GuideDesc* jg_desc = nullptr;
-  JointGuide h_jg{};
-  bool jg_set = false;
-  // its foot-contact and floor terms (b200mdm_set_foot_guidance): the descriptor's FootGuide, the lengths it points to
-  // (fg_len [fg_len_cap] int32 device, allocated on first use) and their host staging; fg_set is cleared by every
-  // b200mdm_set_cond* and b200mdm_set_joint_guidance call.  h_fg also holds the lengths of a call with both weights 0,
-  // which the scene terms read.
-  FootGuide h_fg{};
+  GuideDesc h_guide{};
+  unsigned guide_terms = 0;
   int* fg_len = nullptr;
   int fg_len_cap = 0;
   std::vector<int> h_fg_len;
-  bool fg_set = false;
-  // its scene terms (b200mdm_set_scene_guidance): the descriptor's SceneGuide; sg_set is cleared by every
-  // b200mdm_set_cond*, b200mdm_set_joint_guidance and b200mdm_set_foot_guidance call
-  SceneGuide h_sg{};
-  bool sg_set = false;
-  // its interaction terms (b200mdm_set_interaction_guidance): the descriptor's InterGuide, the reach rows it points to
-  // (ig_pairs [ig_pairs_cap] device, allocated on first use) and their host staging; ig_set is cleared by every
-  // b200mdm_set_cond*, b200mdm_set_joint_guidance, b200mdm_set_foot_guidance and b200mdm_set_scene_guidance call
-  InterGuide h_ig{};
   InterPair* ig_pairs = nullptr;
   int ig_pairs_cap = 0;
   std::vector<InterPair> h_ig_pairs;
-  bool ig_set = false;
   // multi-prompt guidance: the prompt-weight descriptor (read by the step graph at every replay, allocated on first
   // use) and its host staging; pw_set is cleared by every b200mdm_set_cond* call
   PromptWeight* pw_desc = nullptr;
@@ -389,6 +375,35 @@ static int set_attention_attr() {
                                 AttnTcSmem::total(KEYS)));
   return B200MDM_OK;
 }
+
+// The terms of joint-position control, as bits of b200mdm_engine::guide_terms; each extends the ones below it
+enum GuideTerm : unsigned { GT_JOINT = 1, GT_FOOT = 2, GT_SCENE = 4, GT_INTER = 8 };
+// The guidance kernels, one row per highest term on (guide_variant): the step kernel, the test kernel of the
+// b200mdm_test_*_guidance hooks, their dynamic shared memory (T, R) and whether they run in clusters of the
+// descriptor's `chars` CTAs
+struct GuideVariant {
+  void (*step)(const GuideDesc*, const float*, EpiOutParams);
+  void (*test)(GuideDesc, const float*, float*, float*, int, int, int);
+  size_t (*smem)(int, int);
+  bool clusters;
+};
+static const GuideVariant GUIDE_VARIANTS[] = {
+    {joint_guidance_step_kernel<false, false>, joint_guidance_test_kernel<false, false>, jg_smem_bytes, false},
+    {joint_guidance_step_kernel<true, false>, joint_guidance_test_kernel<true, false>, fg_smem_bytes, false},
+    {joint_guidance_step_kernel<true, true>, joint_guidance_test_kernel<true, true>, fg_smem_bytes, false},
+    {joint_guidance_step_kernel<true, true, true>, joint_guidance_test_kernel<true, true, true>, ig_smem_bytes, true},
+};
+// the row of GUIDE_VARIANTS of the terms on (-1: none)
+static int guide_variant(unsigned terms) { return terms ? 31 - __builtin_clz(terms) : -1; }
+// The joints J and ric features R = 4 + 3 (J - 1) of a model the guidance accepts: HumanML3D (D = 263) or KIT (D = 251)
+struct RicDims {
+  int J, R;
+};
+static RicDims ric_dims(int D) {
+  const int J = D == 263 ? 22 : 21;
+  return {J, 4 + 3 * (J - 1)};
+}
+
 static int init_kernel_attrs() {
   // function attributes are per device: track which ordinals have been initialised
   static unsigned long long done_mask = 0;
@@ -411,17 +426,11 @@ static int init_kernel_attrs() {
   TRY((set_attention_attr<208>()));
   TRY((set_attention_attr<256>()));
   CUDA_TRY(cudaFuncSetAttribute(cross_attention_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XAL_SMEM));
-  const int jg_smem = static_cast<int>(jg_smem_bytes(JG_MAX_FRAMES, JG_MAX_FEATS));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, jg_smem));
-  const int fg_smem = static_cast<int>(fg_smem_bytes(JG_MAX_FRAMES, JG_MAX_FEATS));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fg_smem));
-  const int ig_smem = static_cast<int>(ig_smem_bytes(JG_MAX_FRAMES, JG_MAX_FEATS));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_step_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ig_smem));
-  CUDA_TRY(cudaFuncSetAttribute(joint_guidance_test_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ig_smem));
+  for (const GuideVariant& v : GUIDE_VARIANTS) {
+    const int smem = static_cast<int>(v.smem(JG_MAX_FRAMES, JG_MAX_FEATS));
+    CUDA_TRY(cudaFuncSetAttribute(v.step, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CUDA_TRY(cudaFuncSetAttribute(v.test, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  }
   if (dev < 64) done_mask |= 1ull << dev;
   return B200MDM_OK;
 }
@@ -1344,10 +1353,7 @@ static void end_cond(b200mdm_engine* e) {
   e->inpaint_weight = nullptr;
   e->inpaint_motion = nullptr;
   e->hs_set = false;
-  e->jg_set = false;
-  e->fg_set = false;
-  e->sg_set = false;
-  e->ig_set = false;
+  e->guide_terms = 0;
   e->pw_set = false;
   e->vb_live = false;
   e->chain_next = -1;
@@ -1462,7 +1468,7 @@ static const struct {
 static int refuse(const b200mdm_engine* e, Family family, unsigned among = ~0u) {
   static const char* const feature[] = {"prefix-completion (DiP) models", "handshakes", "joint-position control",
                                         "multi-prompt guidance", "BERT text memories", "target conditioning", "inpainting"};
-  const unsigned live = (is_prefix_engine(e) ? F_PREFIX : 0u) | (e->hs_set ? F_HANDSHAKE : 0u) | (e->jg_set ? F_JOINT : 0u) |
+  const unsigned live = (is_prefix_engine(e) ? F_PREFIX : 0u) | (e->hs_set ? F_HANDSHAKE : 0u) | (e->guide_terms ? F_JOINT : 0u) |
                         (e->groups ? F_MULTI : 0u) | (e->dec && !e->dec_clip ? F_TOKENS : 0u) |
                         (e->target_set ? F_TARGET : 0u) | (e->inpaint_mask || e->inpaint_weight ? F_INPAINT : 0u);
   const unsigned hit = REFUSED[family].refuses & among & live;
@@ -1672,77 +1678,33 @@ extern "C" int b200mdm_set_handshake(b200mdm_engine* e, int32_t h, const int64_t
   return B200MDM_OK;
 }
 
-extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_dev, const float* std_dev,
-                                          const float* target_dev, const float* weight_dev, float step, int32_t iters,
-                                          void* stream) {
-  if (!e || !mean_dev || !std_dev || !target_dev || !weight_dev) return fail(B200MDM_EINVAL, "null argument");
+// The argument checks of each term of joint-position control, shared by its setter and its test hook: each fills its
+// part of a GuideDesc.  The joint terms:
+static int fill_joint(const float* mean_dev, const float* std_dev, const float* target_dev, const float* weight_dev,
+                      float step, int32_t iters, JointGuide* out) {
+  if (!mean_dev || !std_dev || !target_dev || !weight_dev) return fail(B200MDM_EINVAL, "null argument");
   if (!std::isfinite(step) || step <= 0.f) return fail(B200MDM_EINVAL, "guidance step %g: a finite value > 0", step);
   if (iters < 1 || iters > 10000) return fail(B200MDM_EINVAL, "guidance iterations %d outside 1 .. 10000", iters);
-  if (e->cfg.nfeats != 1 || (e->JF != 263 && e->JF != 251))
-    return fail(B200MDM_EINVAL, "joint-position control needs the ric features of HumanML3D (263) or KIT (251) with nfeats 1 "
-                "(got %d x %d)", e->cfg.njoints, e->cfg.nfeats);
-  TRY(refuse(e, FAM_JOINT, F_PREFIX));
-  if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
-  TRY(refuse(e, FAM_JOINT));
-  if (e->T > JG_MAX_FRAMES) return fail(B200MDM_ENOTIMPL, "joint-position control: at most %d frames", JG_MAX_FRAMES);
-  if (!e->jg_desc) TRY(dalloc(&e->jg_desc, 1));
-  if (!e->jg_x0) TRY(dalloc(&e->jg_x0, static_cast<size_t>(e->B) * e->JF * e->T));
-  e->h_jg = JointGuide{mean_dev, std_dev, target_dev, weight_dev, step, iters};
-  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->j, &e->h_jg, sizeof(JointGuide), cudaMemcpyHostToDevice,
-                           static_cast<cudaStream_t>(stream)));
-  e->jg_set = true;
-  e->fg_set = false;
-  e->h_fg = FootGuide{};
-  e->sg_set = false;
-  e->h_sg = SceneGuide{};
-  e->ig_set = false;
+  *out = JointGuide{mean_dev, std_dev, target_dev, weight_dev, step, iters};
   return B200MDM_OK;
 }
 
-// the argument checks b200mdm_set_foot_guidance and b200mdm_test_foot_guidance share
-static int check_foot(float contact_weight, float floor_weight, float floor_height, const int64_t* lengths_host, int B) {
+// the foot terms, with lengths_host clamped to T in `len` (empty without lengths; the caller points out->lengths at them)
+static int fill_foot(float contact_weight, float floor_weight, float floor_height, const float* contact_dev,
+                     const int64_t* lengths_host, int B, int T, FootGuide* out, std::vector<int>* len) {
   if (!std::isfinite(contact_weight) || contact_weight < 0.f || !std::isfinite(floor_weight) || floor_weight < 0.f)
     return fail(B200MDM_EINVAL, "foot guidance weights %g, %g: finite values >= 0", contact_weight, floor_weight);
   if (!std::isfinite(floor_height)) return fail(B200MDM_EINVAL, "floor height %g: a finite value", floor_height);
-  for (int b = 0; lengths_host && b < B; ++b)
+  len->clear();
+  for (int b = 0; lengths_host && b < B; ++b) {
     if (lengths_host[b] < 0) return fail(B200MDM_EINVAL, "lengths[%d] = %lld < 0", b, static_cast<long long>(lengths_host[b]));
-  return B200MDM_OK;
-}
-
-extern "C" int b200mdm_set_foot_guidance(b200mdm_engine* e, float contact_weight, float floor_weight, float floor_height,
-                                         const float* contact_dev, const int64_t* lengths_host, void* stream) {
-  if (!e) return fail(B200MDM_EINVAL, "null engine");
-  TRY(check_foot(contact_weight, floor_weight, floor_height, lengths_host, e->B));
-  if (!e->jg_set) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (foot guidance extends it)");
-  e->fg_set = false;
-  e->sg_set = false;
-  e->h_sg = SceneGuide{};
-  e->ig_set = false;
-  const int* len = nullptr;
-  if (lengths_host) {
-    if (e->fg_len_cap < e->B) {
-      dfree(e->fg_len);
-      e->fg_len_cap = 0;
-      TRY(dalloc(&e->fg_len, static_cast<size_t>(e->B)));
-      e->fg_len_cap = e->B;
-    }
-    // the host staging lives in the engine until the next call: no stream synchronisation
-    e->h_fg_len.resize(e->B);
-    for (int b = 0; b < e->B; ++b) e->h_fg_len[b] = static_cast<int>(std::min<int64_t>(lengths_host[b], e->T));
-    CUDA_TRY(cudaMemcpyAsync(e->fg_len, e->h_fg_len.data(), e->B * sizeof(int), cudaMemcpyHostToDevice,
-                             static_cast<cudaStream_t>(stream)));
-    len = e->fg_len;
+    len->push_back(static_cast<int>(std::min<int64_t>(lengths_host[b], T)));
   }
-  e->h_fg = FootGuide{contact_dev, len, contact_weight, floor_weight, floor_height};
-  // both weights 0: plain joint-position control, with the lengths kept for the scene terms
-  if (contact_weight == 0.f && floor_weight == 0.f) return B200MDM_OK;
-  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->f, &e->h_fg, sizeof(FootGuide), cudaMemcpyHostToDevice,
-                           static_cast<cudaStream_t>(stream)));
-  e->fg_set = true;
+  *out = FootGuide{contact_dev, nullptr, contact_weight, floor_weight, floor_height};
   return B200MDM_OK;
 }
 
-// the argument checks of one grid of b200mdm_set_scene_guidance and b200mdm_test_scene_guidance (NULL: no grid)
+// one grid of the scene terms (NULL: no grid)
 static int check_grid(const b200mdm_grid* g, const char* what, int B, SceneGrid* out) {
   *out = SceneGrid{};
   if (!g) return B200MDM_OK;
@@ -1759,45 +1721,25 @@ static int check_grid(const b200mdm_grid* g, const char* what, int B, SceneGrid*
   return B200MDM_OK;
 }
 
-// the argument checks b200mdm_set_scene_guidance and b200mdm_test_scene_guidance share; the terrain's floor-weight check
-// is the caller's (the engine's floor weight is state)
-static int check_scene(float obstacle_weight, float obstacle_margin, const b200mdm_grid* sdf, const b200mdm_grid* terrain,
-                       int B, SceneGuide* out) {
+// the scene terms over the foot terms `foot`, whose floor weight a terrain needs (nullptr: no foot terms to extend, which
+// the setter refuses after these checks); floor_hint ends that message
+static int fill_scene(float obstacle_weight, float obstacle_margin, const b200mdm_grid* sdf, const b200mdm_grid* terrain,
+                      int B, const FootGuide* foot, const char* floor_hint, SceneGuide* out) {
   if (!std::isfinite(obstacle_weight) || obstacle_weight < 0.f || !std::isfinite(obstacle_margin) || obstacle_margin < 0.f)
     return fail(B200MDM_EINVAL, "obstacle weight %g, margin %g: finite values >= 0", obstacle_weight, obstacle_margin);
   TRY(check_grid(sdf, "obstacle sdf", B, &out->sdf));
   TRY(check_grid(terrain, "terrain", B, &out->terrain));
   if (obstacle_weight > 0.f && !sdf) return fail(B200MDM_EINVAL, "obstacle weight %g without an obstacle sdf", obstacle_weight);
+  if (terrain && foot && foot->floor_w == 0.f) return fail(B200MDM_EINVAL, "a terrain needs a floor weight > 0%s", floor_hint);
   out->obstacle_w = obstacle_weight;
   out->margin = obstacle_margin;
   return B200MDM_OK;
 }
 
-extern "C" int b200mdm_set_scene_guidance(b200mdm_engine* e, float obstacle_weight, float obstacle_margin,
-                                          const b200mdm_grid* sdf, const b200mdm_grid* terrain, void* stream) {
-  if (!e) return fail(B200MDM_EINVAL, "null engine");
-  SceneGuide sg{};
-  TRY(check_scene(obstacle_weight, obstacle_margin, sdf, terrain, e->B, &sg));
-  if (!e->jg_set) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (scene guidance extends it)");
-  if (terrain && e->h_fg.floor_w == 0.f)
-    return fail(B200MDM_EINVAL, "a terrain needs a floor weight > 0 (b200mdm_set_foot_guidance)");
-  e->sg_set = false;
-  e->ig_set = false;
-  e->h_sg = sg;   // (kept when off: the interaction terms' scene)
-  if (obstacle_weight == 0.f && !terrain) return B200MDM_OK;   // off: no scene
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // the foot terms as set (both weights 0 included: the lengths), then the scene
-  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->f, &e->h_fg, sizeof(FootGuide), cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->s, &e->h_sg, sizeof(SceneGuide), cudaMemcpyHostToDevice, s));
-  e->sg_set = true;
-  return B200MDM_OK;
-}
-
-// the argument checks b200mdm_set_interaction_guidance and b200mdm_test_interaction_guidance share (J joints per motion);
-// the reach rows go to `rows`
-static int check_inter(int32_t characters, float weight, float margin, const float* placement_dev, const int32_t* pairs_host,
-                       int32_t n_pairs, const float* reach_host, const float* pair_weight_dev, int64_t pair_weight_stride, int B,
-                       int T, int J, std::vector<InterPair>* rows) {
+// the interaction terms of motions of D features, with the reach rows in `rows` (the caller points out->pairs at them)
+static int fill_inter(int32_t characters, float weight, float margin, const float* placement_dev, const int32_t* pairs_host,
+                      int32_t n_pairs, const float* reach_host, const float* pair_weight_dev, int64_t pair_weight_stride, int B,
+                      int T, int D, InterGuide* out, std::vector<InterPair>* rows) {
   if (characters < 2 || characters > IG_MAX_CHARS)
     return fail(B200MDM_EINVAL, "%d characters per scene: 2 .. %d", characters, IG_MAX_CHARS);
   if (B % characters) return fail(B200MDM_EINVAL, "batch %d is not a whole number of %d-character scenes", B, characters);
@@ -1810,6 +1752,7 @@ static int check_inter(int32_t characters, float weight, float margin, const flo
   if (n_pairs > 0 && pair_weight_stride != 0 && pair_weight_stride < static_cast<int64_t>(n_pairs) * T)
     return fail(B200MDM_EINVAL, "pair weight stride %lld: 0 (shared) or at least %lld", static_cast<long long>(pair_weight_stride),
                 static_cast<long long>(n_pairs) * T);
+  const int J = ric_dims(D).J;
   rows->resize(n_pairs);
   for (int n = 0; n < n_pairs; ++n) {
     const int32_t* r = pairs_host + 4 * n;
@@ -1821,17 +1764,20 @@ static int check_inter(int32_t characters, float weight, float margin, const flo
       return fail(B200MDM_EINVAL, "reach[%d] = %g: a finite value >= 0", n, reach_host[n]);
     (*rows)[n] = InterPair{r[0], r[1], r[2], r[3], reach_host[n]};
   }
+  *out = InterGuide{placement_dev, nullptr, pair_weight_dev, static_cast<long long>(pair_weight_stride), characters, n_pairs,
+                    weight, margin};
   return B200MDM_OK;
 }
 
-// ENOTIMPL unless a cluster of `characters` guidance CTAs (ig_smem_bytes each) can be resident
+// ENOTIMPL unless a cluster of `characters` CTAs of `kern` (a kernel of the interaction terms' row) can be resident
 template <class Kern>
-static int check_inter_cluster(Kern kern, int characters, int B, int T, int R) {
+static int check_inter_cluster(Kern kern, int characters, int B, int T, int D) {
+  const size_t smem = GUIDE_VARIANTS[guide_variant(GT_INTER)].smem(T, ric_dims(D).R);
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(B);
   cfg.blockDim = dim3(JG_THREADS);
-  cfg.dynamicSmemBytes = ig_smem_bytes(T, R);
+  cfg.dynamicSmemBytes = smem;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = static_cast<unsigned>(characters);
@@ -1842,8 +1788,80 @@ static int check_inter_cluster(Kern kern, int characters, int B, int T, int R) {
   int n = 0;
   CUDA_TRY(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
   if (n < 1) return fail(B200MDM_ENOTIMPL, "a cluster of %d guidance CTAs (%zu B of shared memory each) cannot be resident",
-                         characters, ig_smem_bytes(T, R));
+                         characters, smem);
   return B200MDM_OK;
+}
+
+// The end of every guidance setter: h_guide goes up whole (it lives in the engine until the next call: no stream
+// synchronisation), then `term` is on (0: the call turned its terms off)
+static int upload_guide(b200mdm_engine* e, unsigned term, void* stream) {
+  CUDA_TRY(cudaMemcpyAsync(e->jg_desc, &e->h_guide, sizeof(GuideDesc), cudaMemcpyHostToDevice,
+                           static_cast<cudaStream_t>(stream)));
+  e->guide_terms |= term;
+  return B200MDM_OK;
+}
+
+extern "C" int b200mdm_set_joint_guidance(b200mdm_engine* e, const float* mean_dev, const float* std_dev,
+                                          const float* target_dev, const float* weight_dev, float step, int32_t iters,
+                                          void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null argument");
+  JointGuide j;
+  TRY(fill_joint(mean_dev, std_dev, target_dev, weight_dev, step, iters, &j));
+  if (e->cfg.nfeats != 1 || (e->JF != 263 && e->JF != 251))
+    return fail(B200MDM_EINVAL, "joint-position control needs the ric features of HumanML3D (263) or KIT (251) with nfeats 1 "
+                "(got %d x %d)", e->cfg.njoints, e->cfg.nfeats);
+  TRY(refuse(e, FAM_JOINT, F_PREFIX));
+  if (!e->cond_set) return fail(B200MDM_ESTATE, "call b200mdm_set_cond / b200mdm_set_cond_dec first (they size the workspace)");
+  TRY(refuse(e, FAM_JOINT));
+  if (e->T > JG_MAX_FRAMES) return fail(B200MDM_ENOTIMPL, "joint-position control: at most %d frames", JG_MAX_FRAMES);
+  if (!e->jg_desc) TRY(dalloc(&e->jg_desc, 1));
+  if (!e->jg_x0) TRY(dalloc(&e->jg_x0, static_cast<size_t>(e->B) * e->JF * e->T));
+  e->guide_terms = 0;
+  e->h_guide = GuideDesc{};
+  e->h_guide.j = j;
+  return upload_guide(e, GT_JOINT, stream);
+}
+
+extern "C" int b200mdm_set_foot_guidance(b200mdm_engine* e, float contact_weight, float floor_weight, float floor_height,
+                                         const float* contact_dev, const int64_t* lengths_host, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  FootGuide f;
+  std::vector<int> len;
+  TRY(fill_foot(contact_weight, floor_weight, floor_height, contact_dev, lengths_host, e->B, e->T, &f, &len));
+  if (!(e->guide_terms & GT_JOINT)) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (foot guidance extends it)");
+  e->guide_terms &= GT_FOOT - 1;
+  if (lengths_host) {
+    if (e->fg_len_cap < e->B) {
+      dfree(e->fg_len);
+      e->fg_len_cap = 0;
+      TRY(dalloc(&e->fg_len, static_cast<size_t>(e->B)));
+      e->fg_len_cap = e->B;
+    }
+    // the host staging lives in the engine until the next call: no stream synchronisation
+    e->h_fg_len = std::move(len);
+    CUDA_TRY(cudaMemcpyAsync(e->fg_len, e->h_fg_len.data(), e->B * sizeof(int), cudaMemcpyHostToDevice,
+                             static_cast<cudaStream_t>(stream)));
+    f.lengths = e->fg_len;
+  }
+  e->h_guide.f = f;
+  e->h_guide.s = SceneGuide{};
+  e->h_guide.i = InterGuide{};
+  // both weights 0: plain joint-position control, with the lengths kept for the scene and interaction terms
+  return upload_guide(e, contact_weight == 0.f && floor_weight == 0.f ? 0u : GT_FOOT, stream);
+}
+
+extern "C" int b200mdm_set_scene_guidance(b200mdm_engine* e, float obstacle_weight, float obstacle_margin,
+                                          const b200mdm_grid* sdf, const b200mdm_grid* terrain, void* stream) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  const bool joint = e->guide_terms & GT_JOINT;
+  SceneGuide sg{};
+  TRY(fill_scene(obstacle_weight, obstacle_margin, sdf, terrain, e->B, joint ? &e->h_guide.f : nullptr,
+                 " (b200mdm_set_foot_guidance)", &sg));
+  if (!joint) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (scene guidance extends it)");
+  e->guide_terms &= GT_SCENE - 1;
+  e->h_guide.s = sg;   // (kept when off: the interaction terms' scene)
+  e->h_guide.i = InterGuide{};
+  return upload_guide(e, obstacle_weight == 0.f && !terrain ? 0u : GT_SCENE, stream);   // off: no scene
 }
 
 extern "C" int b200mdm_set_interaction_guidance(b200mdm_engine* e, int32_t characters, float weight, float margin,
@@ -1851,15 +1869,15 @@ extern "C" int b200mdm_set_interaction_guidance(b200mdm_engine* e, int32_t chara
                                                 const float* reach_host, const float* pair_weight_dev,
                                                 int64_t pair_weight_stride, void* stream) {
   if (!e) return fail(B200MDM_EINVAL, "null engine");
-  if (!e->jg_set) return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (interaction guidance extends it)");
-  const int J = e->JF == 263 ? 22 : 21, R = 4 + 3 * (J - 1);
+  if (!(e->guide_terms & GT_JOINT))
+    return fail(B200MDM_ESTATE, "call b200mdm_set_joint_guidance first (interaction guidance extends it)");
+  InterGuide ig;
   std::vector<InterPair> rows;
-  TRY(check_inter(characters, weight, margin, placement_dev, pairs_host, n_pairs, reach_host, pair_weight_dev,
-                  pair_weight_stride, e->B, e->T, J, &rows));
+  TRY(fill_inter(characters, weight, margin, placement_dev, pairs_host, n_pairs, reach_host, pair_weight_dev,
+                 pair_weight_stride, e->B, e->T, e->JF, &ig, &rows));
   TRY(init_kernel_attrs());
-  TRY(check_inter_cluster(joint_guidance_step_kernel<true, true, true>, characters, e->B, e->T, R));
-  e->ig_set = false;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  TRY(check_inter_cluster(GUIDE_VARIANTS[guide_variant(GT_INTER)].step, characters, e->B, e->T, e->JF));
+  e->guide_terms &= GT_INTER - 1;
   if (n_pairs > 0) {
     if (e->ig_pairs_cap < n_pairs) {
       dfree(e->ig_pairs);
@@ -1869,16 +1887,12 @@ extern "C" int b200mdm_set_interaction_guidance(b200mdm_engine* e, int32_t chara
     }
     // the host staging lives in the engine until the next call: no stream synchronisation
     e->h_ig_pairs = std::move(rows);
-    CUDA_TRY(cudaMemcpyAsync(e->ig_pairs, e->h_ig_pairs.data(), n_pairs * sizeof(InterPair), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(e->ig_pairs, e->h_ig_pairs.data(), n_pairs * sizeof(InterPair), cudaMemcpyHostToDevice,
+                             static_cast<cudaStream_t>(stream)));
   }
-  e->h_ig = InterGuide{placement_dev, e->ig_pairs, pair_weight_dev, static_cast<long long>(pair_weight_stride), characters,
-                       n_pairs, weight, margin};
-  // the foot and scene terms as set (their weights may be 0: the lengths), then the interaction
-  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->f, &e->h_fg, sizeof(FootGuide), cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->s, &e->h_sg, sizeof(SceneGuide), cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaMemcpyAsync(&e->jg_desc->i, &e->h_ig, sizeof(InterGuide), cudaMemcpyHostToDevice, s));
-  e->ig_set = true;
-  return B200MDM_OK;
+  ig.pairs = e->ig_pairs;
+  e->h_guide.i = ig;
+  return upload_guide(e, GT_INTER, stream);
 }
 
 extern "C" int b200mdm_set_prompt_weight(b200mdm_engine* e, int32_t K, const float* weight_dev, int64_t stride_b,
@@ -2157,7 +2171,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
       else   // PLMS: the variational bound refuses multi-prompt guidance (REFUSED)
         CUDA_TRY(launch_k(compose_step_kernel<OutPlms>, grid, dim3(MP_THREADS), 0, s, pw, x0g, p));
       nk += 2;
-    } else if (e->jg_set && !a.model_only) {
+    } else if (e->guide_terms && !a.model_only) {
       // joint-position control: the output GEMM writes the raw x0, the guidance kernel runs the step's tail on it
       StepArgs ax = a;
       ax.mode = MODE_X0;
@@ -2170,19 +2184,9 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
       px.inpaint_motion = nullptr;
       TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, ax, px, s, e->num_sms));
       set_step_params(&p, a, B, T, JF);
-      const int R = 4 + 3 * ((JF == 263 ? 22 : 21) - 1);
-      if (e->ig_set)
-        CUDA_TRY(launch_kc(joint_guidance_step_kernel<true, true, true>, dim3(B), dim3(JG_THREADS), ig_smem_bytes(T, R), s,
-                           e->h_ig.chars, static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
-      else if (e->sg_set)
-        CUDA_TRY(launch_k(joint_guidance_step_kernel<true, true>, dim3(B), dim3(JG_THREADS), fg_smem_bytes(T, R), s,
-                          static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
-      else if (e->fg_set)
-        CUDA_TRY(launch_k(joint_guidance_step_kernel<true, false>, dim3(B), dim3(JG_THREADS), fg_smem_bytes(T, R), s,
-                          static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
-      else
-        CUDA_TRY(launch_k(joint_guidance_step_kernel<false, false>, dim3(B), dim3(JG_THREADS), jg_smem_bytes(T, R), s,
-                          static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
+      const GuideVariant& v = GUIDE_VARIANTS[guide_variant(e->guide_terms)];
+      CUDA_TRY(launch_kc(v.step, dim3(B), dim3(JG_THREADS), v.smem(T, ric_dims(JF).R), s, v.clusters ? e->h_guide.i.chars : 0,
+                         static_cast<const GuideDesc*>(e->jg_desc), static_cast<const float*>(e->jg_x0), p));
       nk += 2;
     } else {
       TRY(launch_out_gemm(e->m_g16, e->m_wout, B, T, JF, d, a, p, s, e->num_sms));
@@ -2389,11 +2393,8 @@ static int loop_enter(b200mdm_engine* e, const StepArgs& a, int32_t flags, int32
     key.imask = e->inpaint_mask; key.iweight = e->inpaint_weight; key.imotion = e->inpaint_motion;
     key.target_g = e->target_set ? e->tgt_g : nullptr;
     key.hs = e->hs_set ? e->hs_desc : nullptr;
-    key.guided = e->jg_set;
-    key.foot = e->jg_set && e->fg_set;
-    key.scene = e->jg_set && e->sg_set;
-    key.inter = e->jg_set && e->ig_set;
-    key.chars = key.inter ? e->h_ig.chars : 0;
+    key.guide = guide_variant(e->guide_terms);
+    key.chars = key.guide >= 0 && GUIDE_VARIANTS[key.guide].clusters ? e->h_guide.i.chars : 0;
     key.groups = e->groups;
     key.slots = a.slots;
     TRY(ensure_step_graph(e, key, a));
@@ -3602,79 +3603,54 @@ extern "C" int b200mdm_debug_ln_trace(uint64_t* host_out, int32_t* dims) {
 }
 #endif
 
+// The joint terms and the motion shape of a b200mdm_test_*_guidance hook
+static int fill_test_joint(const float* x0_dev, const float* x0_out_dev, const float* mean_dev, const float* std_dev,
+                           const float* target_dev, const float* weight_dev, int32_t B, int32_t T, int32_t D, float step,
+                           int32_t iters, JointGuide* out) {
+  if (!x0_dev || !x0_out_dev) return fail(B200MDM_EINVAL, "null argument");
+  TRY(fill_joint(mean_dev, std_dev, target_dev, weight_dev, step, iters, out));
+  if (D != 263 && D != 251) return fail(B200MDM_EINVAL, "D %d: 263 (HumanML3D) or 251 (KIT)", D);
+  if (B < 1 || T < 1 || T > JG_MAX_FRAMES) return fail(B200MDM_EINVAL, "B %d, T %d: B >= 1, 1 <= T <= %d", B, T, JG_MAX_FRAMES);
+  return B200MDM_OK;
+}
+
+// The b200mdm_test_*_guidance hooks after their checks: the test kernel of the row of `top` (the hook's highest term) on
+// descriptor d, with d's lengths and reach rows staged from the host `len` and `rows`, which the hook's return ends, so
+// the stream is synchronised when there are any
+static int test_guidance(GuideDesc d, unsigned top, const std::vector<int>& len, const std::vector<InterPair>& rows,
+                         const float* x0_dev, float* x0_out_dev, float* loss_out_dev, int B, int T, int D, void* stream) {
+  const GuideVariant& v = GUIDE_VARIANTS[guide_variant(top)];
+  TRY(init_kernel_attrs());
+  if (v.clusters) TRY(check_inter_cluster(v.test, d.i.chars, B, T, D));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int* dlen = nullptr;
+  InterPair* dpairs = nullptr;
+  if (!len.empty()) {
+    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&dlen), len.size() * sizeof(int), s));
+    CUDA_TRY(cudaMemcpyAsync(dlen, len.data(), len.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    d.f.lengths = dlen;
+  }
+  if (!rows.empty()) {
+    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&dpairs), rows.size() * sizeof(InterPair), s));
+    CUDA_TRY(cudaMemcpyAsync(dpairs, rows.data(), rows.size() * sizeof(InterPair), cudaMemcpyHostToDevice, s));
+    d.i.pairs = dpairs;
+  }
+  cudaError_t err = launch_kc(v.test, dim3(B), dim3(JG_THREADS), v.smem(T, ric_dims(D).R), s, v.clusters ? d.i.chars : 0,
+                              d, x0_dev, x0_out_dev, loss_out_dev, B, T, D);
+  if (err == cudaSuccess) err = cudaGetLastError();
+  if (dlen) cudaFreeAsync(dlen, s);
+  if (dpairs) cudaFreeAsync(dpairs, s);
+  if (err != cudaSuccess) return fail(B200MDM_ECUDA, "%s", cudaGetErrorString(err));
+  if (dlen || dpairs) CUDA_TRY(cudaStreamSynchronize(s));
+  return B200MDM_OK;
+}
+
 extern "C" int b200mdm_test_joint_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev,
                                            const float* target_dev, const float* weight_dev, int32_t B, int32_t T, int32_t D,
                                            float step, int32_t iters, float* x0_out_dev, float* loss_out_dev, void* stream) {
-  if (!x0_dev || !mean_dev || !std_dev || !target_dev || !weight_dev || !x0_out_dev) return fail(B200MDM_EINVAL, "null argument");
-  if (!std::isfinite(step) || step <= 0.f) return fail(B200MDM_EINVAL, "guidance step %g: a finite value > 0", step);
-  if (iters < 1 || iters > 10000) return fail(B200MDM_EINVAL, "guidance iterations %d outside 1 .. 10000", iters);
-  if (D != 263 && D != 251) return fail(B200MDM_EINVAL, "D %d: 263 (HumanML3D) or 251 (KIT)", D);
-  if (B < 1 || T < 1 || T > JG_MAX_FRAMES) return fail(B200MDM_EINVAL, "B %d, T %d: B >= 1, 1 <= T <= %d", B, T, JG_MAX_FRAMES);
-  TRY(init_kernel_attrs());
-  const JointGuide g{mean_dev, std_dev, target_dev, weight_dev, step, iters};
-  const int R = D == 263 ? 67 : 64;
-  joint_guidance_test_kernel<false, false><<<B, JG_THREADS, jg_smem_bytes(T, R), static_cast<cudaStream_t>(stream)>>>(
-      g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, FootGuide{}, SceneGuide{}, InterGuide{});
-  CUDA_TRY(cudaGetLastError());
-  return B200MDM_OK;
-}
-
-// b200mdm_test_foot_guidance, b200mdm_test_scene_guidance (sg: nullptr without the scene terms) and
-// b200mdm_test_interaction_guidance (ig: nullptr without the interaction terms; its reach rows `rows`)
-static int test_foot_scene(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
-                           const float* weight_dev, const float* contact_dev, const int64_t* lengths_host, int32_t B,
-                           int32_t T, int32_t D, float step, int32_t iters, float contact_weight, float floor_weight,
-                           float floor_height, const SceneGuide* sg, float* x0_out_dev, float* loss_out_dev, void* stream,
-                           const InterGuide* ig = nullptr, const std::vector<InterPair>* rows = nullptr) {
-  TRY(init_kernel_attrs());
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int* len = nullptr;
-  std::vector<int> h_len;
-  if (lengths_host) {
-    h_len.resize(B);
-    for (int b = 0; b < B; ++b) h_len[b] = static_cast<int>(std::min<int64_t>(lengths_host[b], T));
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&len), B * sizeof(int), s));
-    CUDA_TRY(cudaMemcpyAsync(len, h_len.data(), B * sizeof(int), cudaMemcpyHostToDevice, s));
-  }
-  const JointGuide g{mean_dev, std_dev, target_dev, weight_dev, step, iters};
-  const FootGuide f{contact_dev, len, contact_weight, floor_weight, floor_height};
-  const int R = D == 263 ? 67 : 64;
-  InterPair* pairs = nullptr;
-  cudaError_t err = cudaSuccess;
-  if (ig) {
-    InterGuide i = *ig;
-    if (!rows->empty()) {
-      CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&pairs), rows->size() * sizeof(InterPair), s));
-      CUDA_TRY(cudaMemcpyAsync(pairs, rows->data(), rows->size() * sizeof(InterPair), cudaMemcpyHostToDevice, s));
-    }
-    i.pairs = pairs;
-    err = launch_kc(joint_guidance_test_kernel<true, true, true>, dim3(B), dim3(JG_THREADS), ig_smem_bytes(T, R), s, i.chars,
-                    g, x0_dev, x0_out_dev, loss_out_dev, B, T, D, f, *sg, i);
-  } else if (sg) {
-    joint_guidance_test_kernel<true, true><<<B, JG_THREADS, fg_smem_bytes(T, R), s>>>(g, x0_dev, x0_out_dev, loss_out_dev, B,
-                                                                                      T, D, f, *sg, InterGuide{});
-  } else {
-    joint_guidance_test_kernel<true, false><<<B, JG_THREADS, fg_smem_bytes(T, R), s>>>(g, x0_dev, x0_out_dev, loss_out_dev, B,
-                                                                                       T, D, f, SceneGuide{}, InterGuide{});
-  }
-  if (err == cudaSuccess) err = cudaGetLastError();
-  if (len) cudaFreeAsync(len, s);
-  if (pairs) cudaFreeAsync(pairs, s);
-  if (err != cudaSuccess) return fail(B200MDM_ECUDA, "%s", cudaGetErrorString(err));
-  CUDA_TRY(cudaStreamSynchronize(s));   // h_len is local
-  return B200MDM_OK;
-}
-
-// the argument checks of the guidance test hooks (the foot terms' included)
-static int check_foot_test(const float* x0_dev, const float* mean_dev, const float* std_dev, const float* target_dev,
-                           const float* weight_dev, const int64_t* lengths_host, int32_t B, int32_t T, int32_t D, float step,
-                           int32_t iters, float contact_weight, float floor_weight, float floor_height, const float* x0_out_dev) {
-  if (!x0_dev || !mean_dev || !std_dev || !target_dev || !weight_dev || !x0_out_dev) return fail(B200MDM_EINVAL, "null argument");
-  if (!std::isfinite(step) || step <= 0.f) return fail(B200MDM_EINVAL, "guidance step %g: a finite value > 0", step);
-  if (iters < 1 || iters > 10000) return fail(B200MDM_EINVAL, "guidance iterations %d outside 1 .. 10000", iters);
-  if (D != 263 && D != 251) return fail(B200MDM_EINVAL, "D %d: 263 (HumanML3D) or 251 (KIT)", D);
-  if (B < 1 || T < 1 || T > JG_MAX_FRAMES) return fail(B200MDM_EINVAL, "B %d, T %d: B >= 1, 1 <= T <= %d", B, T, JG_MAX_FRAMES);
-  return check_foot(contact_weight, floor_weight, floor_height, lengths_host, B);
+  GuideDesc d{};
+  TRY(fill_test_joint(x0_dev, x0_out_dev, mean_dev, std_dev, target_dev, weight_dev, B, T, D, step, iters, &d.j));
+  return test_guidance(d, GT_JOINT, {}, {}, x0_dev, x0_out_dev, loss_out_dev, B, T, D, stream);
 }
 
 extern "C" int b200mdm_test_foot_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev,
@@ -3682,10 +3658,11 @@ extern "C" int b200mdm_test_foot_guidance(const float* x0_dev, const float* mean
                                           const int64_t* lengths_host, int32_t B, int32_t T, int32_t D, float step,
                                           int32_t iters, float contact_weight, float floor_weight, float floor_height,
                                           float* x0_out_dev, float* loss_out_dev, void* stream) {
-  TRY(check_foot_test(x0_dev, mean_dev, std_dev, target_dev, weight_dev, lengths_host, B, T, D, step, iters, contact_weight,
-                      floor_weight, floor_height, x0_out_dev));
-  return test_foot_scene(x0_dev, mean_dev, std_dev, target_dev, weight_dev, contact_dev, lengths_host, B, T, D, step, iters,
-                         contact_weight, floor_weight, floor_height, nullptr, x0_out_dev, loss_out_dev, stream);
+  GuideDesc d{};
+  std::vector<int> len;
+  TRY(fill_test_joint(x0_dev, x0_out_dev, mean_dev, std_dev, target_dev, weight_dev, B, T, D, step, iters, &d.j));
+  TRY(fill_foot(contact_weight, floor_weight, floor_height, contact_dev, lengths_host, B, T, &d.f, &len));
+  return test_guidance(d, GT_FOOT, len, {}, x0_dev, x0_out_dev, loss_out_dev, B, T, D, stream);
 }
 
 extern "C" int b200mdm_test_scene_guidance(const float* x0_dev, const float* mean_dev, const float* std_dev,
@@ -3695,13 +3672,12 @@ extern "C" int b200mdm_test_scene_guidance(const float* x0_dev, const float* mea
                                            float obstacle_weight, float obstacle_margin, const b200mdm_grid* sdf,
                                            const b200mdm_grid* terrain, float* x0_out_dev, float* loss_out_dev,
                                            void* stream) {
-  TRY(check_foot_test(x0_dev, mean_dev, std_dev, target_dev, weight_dev, lengths_host, B, T, D, step, iters, contact_weight,
-                      floor_weight, floor_height, x0_out_dev));
-  SceneGuide sg{};
-  TRY(check_scene(obstacle_weight, obstacle_margin, sdf, terrain, B, &sg));
-  if (terrain && floor_weight == 0.f) return fail(B200MDM_EINVAL, "a terrain needs a floor weight > 0");
-  return test_foot_scene(x0_dev, mean_dev, std_dev, target_dev, weight_dev, contact_dev, lengths_host, B, T, D, step, iters,
-                         contact_weight, floor_weight, floor_height, &sg, x0_out_dev, loss_out_dev, stream);
+  GuideDesc d{};
+  std::vector<int> len;
+  TRY(fill_test_joint(x0_dev, x0_out_dev, mean_dev, std_dev, target_dev, weight_dev, B, T, D, step, iters, &d.j));
+  TRY(fill_foot(contact_weight, floor_weight, floor_height, contact_dev, lengths_host, B, T, &d.f, &len));
+  TRY(fill_scene(obstacle_weight, obstacle_margin, sdf, terrain, B, &d.f, "", &d.s));
+  return test_guidance(d, GT_SCENE, len, {}, x0_dev, x0_out_dev, loss_out_dev, B, T, D, stream);
 }
 
 extern "C" int b200mdm_test_interaction_guidance(
@@ -3711,21 +3687,15 @@ extern "C" int b200mdm_test_interaction_guidance(
     const b200mdm_grid* sdf, const b200mdm_grid* terrain, int32_t characters, float weight, float margin,
     const float* placement_dev, const int32_t* pairs_host, int32_t n_pairs, const float* reach_host,
     const float* pair_weight_dev, int64_t pair_weight_stride, float* x0_out_dev, float* loss_out_dev, void* stream) {
-  TRY(check_foot_test(x0_dev, mean_dev, std_dev, target_dev, weight_dev, lengths_host, B, T, D, step, iters, contact_weight,
-                      floor_weight, floor_height, x0_out_dev));
-  SceneGuide sg{};
-  TRY(check_scene(obstacle_weight, obstacle_margin, sdf, terrain, B, &sg));
-  if (terrain && floor_weight == 0.f) return fail(B200MDM_EINVAL, "a terrain needs a floor weight > 0");
-  const int J = D == 263 ? 22 : 21, R = 4 + 3 * (J - 1);
+  GuideDesc d{};
+  std::vector<int> len;
   std::vector<InterPair> rows;
-  TRY(check_inter(characters, weight, margin, placement_dev, pairs_host, n_pairs, reach_host, pair_weight_dev,
-                  pair_weight_stride, B, T, J, &rows));
-  TRY(init_kernel_attrs());
-  TRY(check_inter_cluster(joint_guidance_test_kernel<true, true, true>, characters, B, T, R));
-  const InterGuide ig{placement_dev, nullptr, pair_weight_dev, static_cast<long long>(pair_weight_stride), characters, n_pairs,
-                      weight, margin};
-  return test_foot_scene(x0_dev, mean_dev, std_dev, target_dev, weight_dev, contact_dev, lengths_host, B, T, D, step, iters,
-                         contact_weight, floor_weight, floor_height, &sg, x0_out_dev, loss_out_dev, stream, &ig, &rows);
+  TRY(fill_test_joint(x0_dev, x0_out_dev, mean_dev, std_dev, target_dev, weight_dev, B, T, D, step, iters, &d.j));
+  TRY(fill_foot(contact_weight, floor_weight, floor_height, contact_dev, lengths_host, B, T, &d.f, &len));
+  TRY(fill_scene(obstacle_weight, obstacle_margin, sdf, terrain, B, &d.f, "", &d.s));
+  TRY(fill_inter(characters, weight, margin, placement_dev, pairs_host, n_pairs, reach_host, pair_weight_dev,
+                 pair_weight_stride, B, T, D, &d.i, &rows));
+  return test_guidance(d, GT_INTER, len, rows, x0_dev, x0_out_dev, loss_out_dev, B, T, D, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ post-processing

@@ -95,8 +95,9 @@ struct InterGuide {
   float weight, margin;
 };
 
-// The engine's device descriptor: the foot terms follow the joint terms, the scene terms the foot terms and the
-// interaction terms the scene terms, so a kernel without them reads what it always read
+// The guidance descriptor, which the step kernels read from the engine's device copy and the test kernels take by value:
+// the foot terms follow the joint terms, the scene terms the foot terms and the interaction terms the scene terms, so a
+// kernel without them reads what it always read
 struct GuideDesc {
   JointGuide j;
   FootGuide f;
@@ -695,17 +696,15 @@ __global__ void __launch_bounds__(JG_THREADS, FOOT ? 1 : 0) joint_guidance_step_
 }
 
 // b200mdm_test_joint_guidance / b200mdm_test_foot_guidance (FOOT) / b200mdm_test_scene_guidance (SCENE) /
-// b200mdm_test_interaction_guidance (INTER, clusters as the step kernel's): the guidance alone, x0_out [B, D, T] = guided
-// x0 (features past the ric features copied).  fg, sg and ig come last, so the other kernels' parameters keep their
-// offsets.
+// b200mdm_test_interaction_guidance (INTER, clusters as the step kernel's): the guidance of descriptor d alone,
+// x0_out [B, D, T] = guided x0 (features past the ric features copied).
 template <bool FOOT, bool SCENE, bool INTER = false>
-__global__ void __launch_bounds__(JG_THREADS) joint_guidance_test_kernel(const JointGuide g, const float* x0, float* x0_out,
-                                                                         float* loss, int B, int T, int D, const FootGuide fg,
-                                                                         const SceneGuide sg, const InterGuide ig) {
+__global__ void __launch_bounds__(JG_THREADS) joint_guidance_test_kernel(const GuideDesc d, const float* x0, float* x0_out,
+                                                                         float* loss, int B, int T, int D) {
   static_assert(FOOT || !SCENE, "the scene terms extend the foot family");
   static_assert(SCENE || !INTER, "the interaction terms extend the scene family");
   const int R = D == 263 ? 67 : 64, b = blockIdx.x;
-  const float* xs = joint_guidance_run<FOOT, SCENE, INTER>(g, fg, sg, x0, B, T, D, loss, ig);
+  const float* xs = joint_guidance_run<FOOT, SCENE, INTER>(d.j, d.f, d.s, x0, B, T, D, loss, d.i);
   const size_t base = static_cast<size_t>(b) * D * T;
   for (int i = threadIdx.x; i < D * T; i += blockDim.x) x0_out[base + i] = i < R * T ? xs[i] : x0[base + i];
 }

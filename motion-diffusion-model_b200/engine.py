@@ -51,19 +51,6 @@ def canonical_target(y, batch, joint_names):
     return tc, valid
 
 
-def joint_guidance_hook(x0, mean, std, target, weight, step, iters):
-    """The guidance iterations of joint-position control alone (b200mdm_test_joint_guidance), on x0's device:
-    (guided x0 [B, D, T], loss [iters + 1, B])."""
-    lib = _lib.load()
-    x0, mean, std, target, weight = (t.to(torch.float32).contiguous() for t in (x0, mean, std, target, weight))
-    B, D, T = int(x0.shape[0]), int(x0.shape[1]), int(x0.shape[-1])
-    out = torch.empty_like(x0)
-    loss = torch.empty((int(iters) + 1, B), device=x0.device, dtype=torch.float32)
-    check(lib.b200mdm_test_joint_guidance(_ptr(x0), _ptr(mean), _ptr(std), _ptr(target), _ptr(weight), B, T, D,
-                                          float(step), int(iters), _ptr(out), _ptr(loss), _stream()))
-    return out, loss
-
-
 def _lengths_host(lengths, B):
     """y['lengths'] (tensor, array or None) -> contiguous int64 numpy [B], or None"""
     if lengths is None:
@@ -71,25 +58,6 @@ def _lengths_host(lengths, B):
     n = np.ascontiguousarray(np.asarray(lengths.detach().cpu() if torch.is_tensor(lengths) else lengths, dtype=np.int64).reshape(-1))
     assert n.shape == (B,), n.shape
     return n
-
-
-def foot_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weight, floor_weight, floor_height=0.0,
-                       contact=None, lengths=None):
-    """The guidance iterations with the foot-contact and floor terms alone (b200mdm_test_foot_guidance), on x0's device:
-    (guided x0 [B, D, T], total G [iters + 1, B]).  contact [B, 4, T] or None (derived from x0), lengths [B] or None."""
-    lib = _lib.load()
-    x0, mean, std, target, weight = (t.to(torch.float32).contiguous() for t in (x0, mean, std, target, weight))
-    B, D, T = int(x0.shape[0]), int(x0.shape[1]), int(x0.shape[-1])
-    kappa = None if contact is None else contact.to(device=x0.device, dtype=torch.float32).contiguous()
-    n = _lengths_host(lengths, B)
-    out = torch.empty_like(x0)
-    loss = torch.empty((int(iters) + 1, B), device=x0.device, dtype=torch.float32)
-    check(lib.b200mdm_test_foot_guidance(_ptr(x0), _ptr(mean), _ptr(std), _ptr(target), _ptr(weight),
-                                         None if kappa is None else _ptr(kappa),
-                                         None if n is None else n.ctypes.data_as(ctypes.c_void_p), B, T, D, float(step),
-                                         int(iters), float(contact_weight), float(floor_weight), float(floor_height),
-                                         _ptr(out), _ptr(loss), _stream()))
-    return out, loss
 
 
 def _grid(grid, device):
@@ -103,28 +71,6 @@ def _grid(grid, device):
 
 def _grid_ref(g):
     return None if g is None else ctypes.byref(g)
-
-
-def scene_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weight, floor_weight, floor_height,
-                        obstacle_weight, obstacle_margin, sdf=None, terrain=None, contact=None, lengths=None):
-    """The guidance iterations with the foot and scene terms alone (b200mdm_test_scene_guidance), on x0's device:
-    (guided x0 [B, D, T], total G [iters + 1, B]).  sdf / terrain: SceneGrid or None; contact, lengths as
-    foot_guidance_hook's."""
-    lib = _lib.load()
-    x0, mean, std, target, weight = (t.to(torch.float32).contiguous() for t in (x0, mean, std, target, weight))
-    B, D, T = int(x0.shape[0]), int(x0.shape[1]), int(x0.shape[-1])
-    kappa = None if contact is None else contact.to(device=x0.device, dtype=torch.float32).contiguous()
-    n = _lengths_host(lengths, B)
-    (gs, vs), (gt, vt) = _grid(sdf, x0.device), _grid(terrain, x0.device)
-    out = torch.empty_like(x0)
-    loss = torch.empty((int(iters) + 1, B), device=x0.device, dtype=torch.float32)
-    check(lib.b200mdm_test_scene_guidance(_ptr(x0), _ptr(mean), _ptr(std), _ptr(target), _ptr(weight),
-                                          None if kappa is None else _ptr(kappa),
-                                          None if n is None else n.ctypes.data_as(ctypes.c_void_p), B, T, D, float(step),
-                                          int(iters), float(contact_weight), float(floor_weight), float(floor_height),
-                                          float(obstacle_weight), float(obstacle_margin), _grid_ref(gs), _grid_ref(gt),
-                                          _ptr(out), _ptr(loss), _stream()))
-    return out, loss
 
 
 def _interaction(characters, weight, margin, placement, pairs, reach, pair_weight, device):
@@ -142,6 +88,58 @@ def _interaction(characters, weight, margin, placement, pairs, reach, pair_weigh
              dist.ctypes.data_as(ctypes.c_void_p), _ptr(pw), stride), (pl, rows, dist, pw))
 
 
+def _guidance_hook(fn, x0, mean, std, target, weight, step, iters, foot=(), scene=(), interaction=()):
+    """The guidance iterations of the test hook `fn` (b200mdm_test_*_guidance) on x0's device: (guided x0 [B, D, T],
+    total G [iters + 1, B]).  foot: (contact_weight, floor_weight, floor_height, contact, lengths); scene:
+    (obstacle_weight, obstacle_margin, sdf, terrain); interaction: the arguments of _interaction before the device."""
+    lib = _lib.load()
+    x0, mean, std, target, weight = (t.to(torch.float32).contiguous() for t in (x0, mean, std, target, weight))
+    B, D, T = int(x0.shape[0]), int(x0.shape[1]), int(x0.shape[-1])
+    head, tail = [], []                    # the arguments before B and after iters (locals keep what they point to)
+    if foot:
+        contact_weight, floor_weight, floor_height, contact, lengths = foot
+        kappa = None if contact is None else contact.to(device=x0.device, dtype=torch.float32).contiguous()
+        n = _lengths_host(lengths, B)
+        head = [_ptr(kappa), None if n is None else n.ctypes.data_as(ctypes.c_void_p)]
+        tail += [float(contact_weight), float(floor_weight), float(floor_height)]
+    if scene:
+        obstacle_weight, obstacle_margin, sdf, terrain = scene
+        (gs, vs), (gt, vt) = _grid(sdf, x0.device), _grid(terrain, x0.device)
+        tail += [float(obstacle_weight), float(obstacle_margin), _grid_ref(gs), _grid_ref(gt)]
+    if interaction:
+        args, keep = _interaction(*interaction, x0.device)
+        tail += list(args)
+    out = torch.empty_like(x0)
+    loss = torch.empty((int(iters) + 1, B), device=x0.device, dtype=torch.float32)
+    check(getattr(lib, fn)(_ptr(x0), _ptr(mean), _ptr(std), _ptr(target), _ptr(weight), *head, B, T, D, float(step),
+                           int(iters), *tail, _ptr(out), _ptr(loss), _stream()))
+    return out, loss
+
+
+def joint_guidance_hook(x0, mean, std, target, weight, step, iters):
+    """The guidance iterations of joint-position control alone (b200mdm_test_joint_guidance), on x0's device:
+    (guided x0 [B, D, T], loss [iters + 1, B])."""
+    return _guidance_hook("b200mdm_test_joint_guidance", x0, mean, std, target, weight, step, iters)
+
+
+def foot_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weight, floor_weight, floor_height=0.0,
+                       contact=None, lengths=None):
+    """The guidance iterations with the foot-contact and floor terms alone (b200mdm_test_foot_guidance), on x0's device:
+    (guided x0 [B, D, T], total G [iters + 1, B]).  contact [B, 4, T] or None (derived from x0), lengths [B] or None."""
+    return _guidance_hook("b200mdm_test_foot_guidance", x0, mean, std, target, weight, step, iters,
+                          (contact_weight, floor_weight, floor_height, contact, lengths))
+
+
+def scene_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weight, floor_weight, floor_height,
+                        obstacle_weight, obstacle_margin, sdf=None, terrain=None, contact=None, lengths=None):
+    """The guidance iterations with the foot and scene terms alone (b200mdm_test_scene_guidance), on x0's device:
+    (guided x0 [B, D, T], total G [iters + 1, B]).  sdf / terrain: SceneGrid or None; contact, lengths as
+    foot_guidance_hook's."""
+    return _guidance_hook("b200mdm_test_scene_guidance", x0, mean, std, target, weight, step, iters,
+                          (contact_weight, floor_weight, floor_height, contact, lengths),
+                          (obstacle_weight, obstacle_margin, sdf, terrain))
+
+
 def interaction_guidance_hook(x0, mean, std, target, weight, step, iters, contact_weight, floor_weight, floor_height,
                               obstacle_weight, obstacle_margin, sdf, terrain, characters, interaction_weight,
                               interaction_margin, placement, pairs=None, reach=None, pair_weight=None, contact=None,
@@ -150,23 +148,10 @@ def interaction_guidance_hook(x0, mean, std, target, weight, step, iters, contac
     x0's device: (guided x0 [B, D, T], total G [iters + 1, B], each pair's energy at its lower rank).  placement [B, 3],
     pairs int [N, 4] scene-local (a, j, b, k) or None, reach [N], pair_weight [N, T] or [B / C, N, T]; the other
     arguments as scene_guidance_hook's."""
-    lib = _lib.load()
-    x0, mean, std, target, weight = (t.to(torch.float32).contiguous() for t in (x0, mean, std, target, weight))
-    B, D, T = int(x0.shape[0]), int(x0.shape[1]), int(x0.shape[-1])
-    kappa = None if contact is None else contact.to(device=x0.device, dtype=torch.float32).contiguous()
-    n = _lengths_host(lengths, B)
-    (gs, vs), (gt, vt) = _grid(sdf, x0.device), _grid(terrain, x0.device)
-    args, keep = _interaction(characters, interaction_weight, interaction_margin, placement, pairs, reach, pair_weight,
-                              x0.device)
-    out = torch.empty_like(x0)
-    loss = torch.empty((int(iters) + 1, B), device=x0.device, dtype=torch.float32)
-    check(lib.b200mdm_test_interaction_guidance(_ptr(x0), _ptr(mean), _ptr(std), _ptr(target), _ptr(weight),
-                                                None if kappa is None else _ptr(kappa),
-                                                None if n is None else n.ctypes.data_as(ctypes.c_void_p), B, T, D,
-                                                float(step), int(iters), float(contact_weight), float(floor_weight),
-                                                float(floor_height), float(obstacle_weight), float(obstacle_margin),
-                                                _grid_ref(gs), _grid_ref(gt), *args, _ptr(out), _ptr(loss), _stream()))
-    return out, loss
+    return _guidance_hook("b200mdm_test_interaction_guidance", x0, mean, std, target, weight, step, iters,
+                          (contact_weight, floor_weight, floor_height, contact, lengths),
+                          (obstacle_weight, obstacle_margin, sdf, terrain),
+                          (characters, interaction_weight, interaction_margin, placement, pairs, reach, pair_weight))
 
 
 class Engine:
@@ -459,15 +444,17 @@ class Engine:
         check(self.lib.b200mdm_set_handshake(self.h, int(handshake_size), n.ctypes.data_as(ctypes.c_void_p),
                                              ms.ctypes.data_as(ctypes.c_void_p), _stream()))
 
+    def _keep_guide(self, term, tensors):
+        """keep the tensors of guidance term `term` (0 joint, 1 foot, 2 scene, 3 interaction) alive, and drop those of
+        the terms above it, which its setter cleared"""
+        self._keep["guide"] = (self._keep.get("guide", []) + [None] * term)[:term] + [tensors]
+
     def set_joint_guidance(self, mean, std, target, weight, step, iters):
         """Joint-position control for the next DDPM / DDIM loops and steps (b200mdm_set_joint_guidance), after set_cond,
         which clears it: mean / std [D], target [B, J, 3, T], weight [B, J, T], all on the engine's device."""
         ts = [t.to(torch.float32).contiguous() for t in (mean, std, target, weight)]
         check(self.lib.b200mdm_set_joint_guidance(self.h, *[_ptr(t) for t in ts], float(step), int(iters), _stream()))
-        self._keep["joint"] = ts
-        self._keep.pop("foot", None)
-        self._keep.pop("scene", None)
-        self._keep.pop("interaction", None)
+        self._keep_guide(0, ts)
 
     def set_foot_guidance(self, contact_weight, floor_weight, floor_height=0.0, contact=None, lengths=None):
         """The foot-contact and floor terms of the joint guidance set last (b200mdm_set_foot_guidance), which
@@ -478,9 +465,7 @@ class Engine:
         check(self.lib.b200mdm_set_foot_guidance(self.h, float(contact_weight), float(floor_weight), float(floor_height),
                                                  None if kappa is None else _ptr(kappa),
                                                  None if n is None else n.ctypes.data_as(ctypes.c_void_p), _stream()))
-        self._keep["foot"] = kappa
-        self._keep.pop("scene", None)
-        self._keep.pop("interaction", None)
+        self._keep_guide(1, kappa)
 
     def set_scene_guidance(self, obstacle_weight, obstacle_margin, sdf=None, terrain=None):
         """The scene terms of the joint guidance set last (b200mdm_set_scene_guidance), after set_foot_guidance (whose
@@ -490,8 +475,7 @@ class Engine:
         (gs, vs), (gt, vt) = _grid(sdf, dev), _grid(terrain, dev)
         check(self.lib.b200mdm_set_scene_guidance(self.h, float(obstacle_weight), float(obstacle_margin), _grid_ref(gs),
                                                   _grid_ref(gt), _stream()))
-        self._keep["scene"] = (vs, vt)
-        self._keep.pop("interaction", None)
+        self._keep_guide(2, (vs, vt))
 
     def set_interaction_guidance(self, characters, weight, margin, placement, pairs=None, reach=None, pair_weight=None):
         """The interaction terms of the joint guidance set last (b200mdm_set_interaction_guidance), after
@@ -501,7 +485,7 @@ class Engine:
         dev = torch.device("cuda", torch.cuda.current_device())
         args, keep = _interaction(characters, weight, margin, placement, pairs, reach, pair_weight, dev)
         check(self.lib.b200mdm_set_interaction_guidance(self.h, *args, _stream()))
-        self._keep["interaction"] = keep
+        self._keep_guide(3, keep)
 
     def set_cond_multi(self, batch, nframes, y, embed, action, weight, device):
         """Multi-prompt guidance (b200mdm_set_cond_multi / _dec / _tokens, then b200mdm_set_prompt_weight): embed fp32
