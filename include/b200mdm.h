@@ -741,7 +741,8 @@ int b200mdm_test_target(b200mdm_engine* e, const float* target_dev, const uint8_
                         float* out_dev, void* stream);
 /* The per-step cross-attention rows of a B200MDM_DEC_MEMORY_CLIP engine for its current workspace (after
  * b200mdm_set_cond_dec, and b200mdm_set_target when used), every sample at model timestep `timestep`:
- * out fp32 [num_layers, Bp, 512], Bp = 2 x batch with CFG (conditional rows, then unconditional), else batch;
+ * out fp32 [num_layers, Bp, 512], Bp = 2 x batch with CFG (conditional rows, then unconditional), G x batch under
+ * multi-prompt guidance (the prompts' groups, then the unconditional one), else batch;
  * row (l, b') = out_proj_l(W_v,l (embed_text(clip[b'] or 0) + temb[timestep] + g[b' mod batch]) + b_v,l). */
 int b200mdm_test_cross_rows(b200mdm_engine* e, int32_t timestep, float* out_dev, void* stream);
 /* The step's row-bias LayerNorm of such an engine: h[r] <- LayerNorm(h[r] + c[r / S]; gamma, beta, 1e-5) in place, for
@@ -755,8 +756,9 @@ int b200mdm_test_row_bias_ln(void* hres16_dev, const float* c_dev, const float* 
  * for layer `layer` only.  Nothing else changes: no graph, no loop state, no launch count.  A non-NULL buffer for a point
  * the model does not have, a bad layer or n_taps outside 0..B200MDM_TAP_COUNT return B200MDM_EINVAL before any CUDA call.
  * Synchronises the stream once (like b200mdm_denoise) before the forward is enqueued.
- * Sizes, with M = halves*B*S rows (S = T + 1, or context_len + T for DiP), Bp = halves*B, kw = 2 for DiP else 1, Mt the
- * text tokens, ff = ff_size, d = 512; h = fp16, f = fp32; hres rows are [hi | lo]: */
+ * Sizes, with M = Bp*S rows (S = T + 1, or context_len + T for DiP), Bp = halves*B, or G*B under multi-prompt guidance
+ * (G = K + 1), kw = 2 for DiP else 1, Mt the text tokens, ff = ff_size, JF = njoints*nfeats, d = 512; h = fp16,
+ * f = fp32; hres rows are [hi | lo]; b200mdm_test_tap_bytes gives each size in bytes: */
 #define B200MDM_TAP_EMBED 0     /* h [M, 2d]  residual stream after the embedding GEMM, before token 0 */
 #define B200MDM_TAP_TOK0 1      /* h [M, 2d]  after token 0 / the DiP memory build / the CLIP decoder's cross rows */
 #define B200MDM_TAP_CONDPROJ 2  /* f [Bp, d]  conditioning rows (not DiP) */
@@ -773,10 +775,17 @@ int b200mdm_test_row_bias_ln(void* hres16_dev, const float* c_dev, const float* 
 #define B200MDM_TAP_L_LN2 13    /* h [M, 2d]  decoders: after cross out-proj + LN2 (DiP) / the row-bias LN2 (CLIP) */
 #define B200MDM_TAP_L_FFN 14    /* h [M, kw*ff] after FFN-up (GELU) */
 #define B200MDM_TAP_L_LN3 15    /* h [M, 2d]  after FFN-down + LN (norm2, decoders norm3) */
-#define B200MDM_TAP_BLEND 16    /* h [B*T, 3d] CFG blend [hi | lo | hi], the output GEMM's A operand */
-#define B200MDM_TAP_COUNT 17
+#define B200MDM_TAP_BLEND 16    /* h [B*T, 3d] CFG blend [hi | lo | hi], the output GEMM's A operand ([G*B*T, 3d] under
+                                   multi-prompt guidance: every group's frame rows, split as they are) */
+#define B200MDM_TAP_X0G 17      /* f [G*B, JF, T] multi-prompt guidance only: every group's raw x0, the output GEMM's
+                                   result that compose_step_kernel composes */
+#define B200MDM_TAP_COUNT 18
 int b200mdm_test_forward_taps(b200mdm_engine* e, const float* x_dev, const int32_t* timesteps_host, float* out_dev,
                               int32_t layer, void* const* tap_dev, int32_t n_taps, void* stream);
+/* The size in bytes of tap point `id` (B200MDM_TAP_*) in the current workspace, as b200mdm_test_forward_taps copies it;
+ * 0 where the model or the conditioning has no such point.  A null engine or an id outside 0..B200MDM_TAP_COUNT-1
+ * return B200MDM_EINVAL, an engine without conditioning B200MDM_ESTATE (both negative). */
+int64_t b200mdm_test_tap_bytes(const b200mdm_engine* e, int32_t id);
 
 #ifdef __cplusplus
 }

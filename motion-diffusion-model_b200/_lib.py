@@ -42,7 +42,7 @@ SYMBOLS = [
     "b200mdm_set_scene_guidance", "b200mdm_test_scene_guidance", "b200mdm_chain_set_goal", "b200mdm_chunk_frame",
     "b200mdm_set_interaction_guidance", "b200mdm_test_interaction_guidance",
     "b200mdm_sample_step_at", "b200mdm_slots_begin", "b200mdm_slot_admit", "b200mdm_slots_run", "b200mdm_slot_read",
-    "b200mdm_chain_slots_begin", "b200mdm_chain_slot_admit", "b200mdm_chain_slot_handoff",
+    "b200mdm_chain_slots_begin", "b200mdm_chain_slot_admit", "b200mdm_chain_slot_handoff", "b200mdm_test_tap_bytes",
 ]
 MAX_PROMPTS = 8                             # B200MDM_MAX_PROMPTS
 MAX_CHARACTERS = 8                          # characters per scene: one cluster of at most 8 CTAs
@@ -50,7 +50,7 @@ MAX_INTERACTION_PAIRS = 1024                # B200MDM_MAX_INTERACTION_PAIRS
 MAX_MEMORY_TOKENS = 512                     # a BERT text memory holds 1 .. 512 tokens (DistilBERT's position limit)
 # tap points of b200mdm_test_forward_taps (B200MDM_TAP_*)
 TAPS = ["EMBED", "TOK0", "CONDPROJ", "TEMB", "MEM16", "CROSS_C", "KVC16", "L_IN", "L_QKV", "L_ATT", "L_LN1", "L_QC",
-        "L_XATT", "L_LN2", "L_FFN", "L_LN3", "BLEND"]
+        "L_XATT", "L_LN2", "L_FFN", "L_LN3", "BLEND", "X0G"]
 DEC_MEMORY_TOKENS, DEC_MEMORY_CLIP = 0, 1   # b200mdm_config.dec_memory (trans_dec)
 
 
@@ -115,6 +115,8 @@ def load():
     lib.b200mdm_q_sample.argtypes = [vp, f32, f32, vp, vp, vp, i64, vp]
     lib.b200mdm_launch_count.argtypes = [vp, i32]
     lib.b200mdm_launch_count.restype = i64
+    if hasattr(lib, "b200mdm_test_tap_bytes"):
+        lib.b200mdm_test_tap_bytes.restype = i64
     lib.b200mdm_test_gemm_f16.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]
     lib.b200mdm_test_attention.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp]
     if hasattr(lib, "b200mdm_test_cross_attention"):
@@ -170,7 +172,8 @@ def load():
                        ("b200mdm_chunk_frame", [vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp]),
                        ("b200mdm_chain_slots_begin", [vp, i32, i32, i32, i32, i32, i32, vp]),
                        ("b200mdm_chain_slot_admit", [vp, i32, vp, vp, vp, f32, i64, i32, ctypes.c_uint64, i64, vp]),
-                       ("b200mdm_chain_slot_handoff", [vp, i32, vp, vp, vp, vp])):
+                       ("b200mdm_chain_slot_handoff", [vp, i32, vp, vp, vp, vp]),
+                       ("b200mdm_test_tap_bytes", [vp, i32])):
         if hasattr(lib, name):                        # (an older A/B build of the same ABI may lack them)
             getattr(lib, name).argtypes = args
     for name in SYMBOLS:

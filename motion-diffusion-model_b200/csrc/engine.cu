@@ -1994,7 +1994,20 @@ static void tap_source(const b200mdm_engine* e, int id, const void** src, size_t
     case B200MDM_TAP_L_FFN: *src = e->ffn16; *bytes = M * kw * e->ff * h; break;
     case B200MDM_TAP_BLEND:
       *src = e->g16; *bytes = static_cast<size_t>(e->groups ? e->Bp : e->B) * e->T * 3 * d * h; break;
+    case B200MDM_TAP_X0G:
+      if (e->groups) { *src = e->mp_x0; *bytes = static_cast<size_t>(e->Bp) * e->JF * e->T * f; }
+      break;
   }
+}
+
+extern "C" int64_t b200mdm_test_tap_bytes(const b200mdm_engine* e, int32_t id) {
+  if (!e) return fail(B200MDM_EINVAL, "null engine");
+  if (id < 0 || id >= B200MDM_TAP_COUNT) return fail(B200MDM_EINVAL, "tap point %d outside 0..%d", id, B200MDM_TAP_COUNT - 1);
+  if (!e->cond_set) return fail(B200MDM_ESTATE, "no workspace: set the conditioning first");
+  const void* src;
+  size_t bytes;
+  tap_source(e, id, &src, &bytes);
+  return static_cast<int64_t>(bytes);
 }
 
 // Copy tap points first..last (layer l, or -1 outside the layer loop) into the caller's buffers, on stream s.
@@ -2161,6 +2174,7 @@ static int enqueue_forward(b200mdm_engine* e, const StepArgs& a, cudaStream_t s,
       px.inpaint_weight = nullptr;
       px.inpaint_motion = nullptr;
       TRY(launch_out_gemm(e->m_g16, e->m_wout, GB, T, JF, d, ax, px, s, e->num_sms));
+      if (taps) TRY(take_taps(e, *taps, B200MDM_TAP_X0G, B200MDM_TAP_X0G, -1, s));
       set_step_params(&p, a, B, T, JF);
       const dim3 grid(static_cast<unsigned>((static_cast<size_t>(JF) * T + MP_THREADS - 1) / MP_THREADS), B);
       const PromptWeight* pw = e->pw_desc;

@@ -187,6 +187,7 @@ class Engine:
         self._table_keys = {}                     # "next" / "dpm" / "vb": the key of the rows uploaded for the schedule
         self.batch = self.nframes = self.n_tokens = 0
         self.halves = 1
+        self.groups = 0                           # G = K + 1 under multi-prompt guidance, else 0
 
     def close(self):
         if getattr(self, "h", None):
@@ -284,10 +285,19 @@ class Engine:
                                            _ptr(out), _stream()))
         return out
 
-    def test_cross_rows(self, timestep, halves, device):
+    def packed_batch(self):
+        """Bp, the rows of the packed batch of the conditioning set last: G * batch under multi-prompt guidance (G = K + 1
+        groups), else halves * batch (2 with classifier-free guidance)."""
+        return (self.groups or self.halves) * self.batch
+
+    def test_cross_rows(self, timestep, halves=None, device="cuda"):
         """The CLIP decoder's per-step cross-attention rows (b200mdm_test_cross_rows) for the conditioning last set:
-        [num_layers, halves * batch, d] fp32 at model timestep `timestep`."""
-        out = torch.empty(self.cfg.num_layers, halves * self.batch, self.cfg.latent_dim, device=device, dtype=torch.float32)
+        [num_layers, Bp, d] fp32 at model timestep `timestep`, Bp = packed_batch().  `halves`, when given, must describe
+        the same rows (halves * batch = Bp; under multi-prompt guidance halves = G): ValueError otherwise."""
+        if halves is not None and int(halves) * self.batch != self.packed_batch():
+            raise ValueError("halves = %d gives %d rows, but the conditioning set last packs %d"
+                             % (int(halves), int(halves) * self.batch, self.packed_batch()))
+        out = torch.empty(self.cfg.num_layers, self.packed_batch(), self.cfg.latent_dim, device=device, dtype=torch.float32)
         check(self.lib.b200mdm_test_cross_rows(self.h, int(timestep), _ptr(out), _stream()))
         return out
 
@@ -310,6 +320,7 @@ class Engine:
                                         _stream()))
         self._keep["cond"] = (te, sc)
         self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 2 if sc is not None else 1, 1
+        self.groups = 0
 
     def _text_rows(self, te, batch, device):
         """y['text_embed'] [1, B, cond_dim] (or [1, 1, cond_dim]: one prompt for the whole batch, sample/predict.py) as
@@ -364,6 +375,7 @@ class Engine:
                                             int(uncond), _stream()))
         self._keep["cond"] = (te, sc)
         self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 2 if sc is not None else 1, 1
+        self.groups = 0
 
     def dec_memory(self, te, batch, device):
         """(tokens [Mt, batch, cond_dim] contiguous fp32 on device, padding mask uint8 numpy [batch, Mt]) of a DiP
@@ -403,6 +415,7 @@ class Engine:
             check(self.lib.b200mdm_set_prefix(self.h, _ptr(pf), _stream()))
         self._keep["cond"] = (enc, sc, pf)
         self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 2 if sc is not None else 1, Mt
+        self.groups = 0
 
     def prompt_memories(self, pairs, batch, device):
         """(tokens fp32 [K, Mt, batch, C] contiguous on device, padding mask uint8 numpy [K, batch, Mt]) of K BERT
@@ -512,7 +525,7 @@ class Engine:
                 check(self.lib.b200mdm_set_cond_multi(self.h, batch, nframes, K, _ptr(te), ln_p,
                                                       None if ac is None else ac.ctypes.data_as(ctypes.c_void_p), _stream()))
         self._keep["cond"] = (te,)
-        self.batch, self.nframes, self.halves, self.n_tokens = batch, nframes, 1, n_tokens
+        self.batch, self.nframes, self.halves, self.n_tokens, self.groups = batch, nframes, 1, n_tokens, K + 1
         self._set_target(batch, y, device)
         w = weight.detach().to(device=device, dtype=torch.float32).contiguous()
         strides = [0 if w.shape[i] == 1 else w.stride(i) for i in range(4)]
@@ -530,15 +543,16 @@ class Engine:
 
     def tap_shapes(self):
         """{tap name: (shape, dtype)} of every b200mdm_test_forward_taps point the current model and workspace have
-        (include/b200mdm.h, B200MDM_TAP_*)."""
+        (include/b200mdm.h, B200MDM_TAP_*); each size is b200mdm_test_tap_bytes's, which is asserted."""
         c = self.cfg
-        d, ff, L, B, T, Bp = c.latent_dim, c.ff_size, c.num_layers, self.batch, self.nframes, self.halves * self.batch
+        d, ff, L, B, T, Bp = c.latent_dim, c.ff_size, c.num_layers, self.batch, self.nframes, self.packed_batch()
         dip = self.dec and not self.dec_clip
         S = T + (self.context_len if dip else 1)
         M, kw, mem, h, f = Bp * S, 2 if dip else 1, Bp * self.n_tokens, torch.float16, torch.float32
+        blend = Bp if self.groups else B           # multi-prompt guidance splits every group's frame rows as they are
         out = dict(EMBED=((M, 2 * d), h), TOK0=((M, 2 * d), h), TEMB=((B, d), f), L_IN=((M, 2 * d), h),
                    L_QKV=((M, 3 * d), h), L_ATT=((M, kw * d), h), L_LN1=((M, 2 * d), h), L_FFN=((M, kw * ff), h),
-                   L_LN3=((M, 2 * d), h), BLEND=((B * T, 3 * d), h))
+                   L_LN3=((M, 2 * d), h), BLEND=((blend * T, 3 * d), h))
         if not dip:
             out["CONDPROJ"] = ((Bp, d), f)
         if self.dec:
@@ -547,6 +561,14 @@ class Engine:
             out["CROSS_C"] = ((L, Bp, d), f)
         if dip:
             out.update(MEM16=((mem, 2 * d), h), KVC16=((mem, L * 2 * d), h), L_QC=((M, d), h), L_XATT=((M, kw * d), h))
+        if self.groups:
+            out["X0G"] = ((Bp, c.njoints * c.nfeats, T), f)
+        for i, name in enumerate(_lib.TAPS):
+            n = int(self.lib.b200mdm_test_tap_bytes(self.h, i))
+            if n < 0:
+                check(n)
+            want = int(np.prod(out[name][0])) * out[name][1].itemsize if name in out else 0
+            assert n == want, "tap %s: the engine copies %d bytes, tap_shapes sizes %d" % (name, n, want)
         return out
 
     def forward_taps(self, x, timesteps, layer, names=None):
@@ -589,6 +611,7 @@ class Engine:
         """A slot session on the (slots, nframes) workspace (b200mdm_slots_begin): every slot idle."""
         check(self.lib.b200mdm_slots_begin(self.h, int(slots), int(nframes), int(bool(guided)), mode, flags, _stream()))
         self.batch, self.nframes, self.halves, self.n_tokens = int(slots), int(nframes), 2 if guided else 1, 1
+        self.groups = 0
         self._keep["slots"] = {}
 
     def slot_admit(self, slot, embed, action, scale, length, seed, sample_index):
@@ -613,6 +636,7 @@ class Engine:
         check(self.lib.b200mdm_chain_slots_begin(self.h, int(slots), int(nframes), int(bool(guided)), mode, flags,
                                                  int(n_tokens), _stream()))
         self.batch, self.nframes, self.halves, self.n_tokens = int(slots), int(nframes), 2 if guided else 1, int(n_tokens)
+        self.groups = 0
         self._keep["slots"] = {}
 
     def chain_slot_admit(self, slot, tokens, mask, prefix, scale, length, include_prefix, seed, sample_index):

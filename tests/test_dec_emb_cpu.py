@@ -163,6 +163,7 @@ def test_test_hooks_reject_bad_arguments_without_gpu():
     lib = _lib.load()
     assert lib.b200mdm_test_cross_rows(None, 0, None, None) == _lib.EINVAL
     assert lib.b200mdm_test_row_bias_ln(None, None, None, None, 8, 4, None) == _lib.EINVAL
+    assert lib.b200mdm_test_tap_bytes(None, 0) == _lib.EINVAL
 
 
 def test_forward_taps_rejects_bad_arguments_without_gpu():
